@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the BCNN VGG-16 448x448 train step (BASELINE.json metric) on N B200s, one process per GPU.
+"""Benchmark of the BCNN VGG-16 448x448 train step on N GPUs, one process per GPU.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--workload bcnn_s2|bcnn_s1|cbcnn8192|mpn] [--batch 32]
                   [--impl native|reference]
@@ -8,14 +8,14 @@ Prints ONE JSON line (rank 0).
   value         device-timed images/s, inputs resident in HBM (CUDA events, max over ranks)
   e2e           the same step through hawkeye_b200.train.Trainer.batch_training with pinned HOST inputs (H2D copy and the
                 loss / accuracy read-back inside the timed region)
-  roofline      hk_bilinear_pool_fwd (K1, the kernel BASELINE.json names) against the measured HBM peak, at the workload's
+  roofline      hk_bilinear_pool_fwd (K1) against the measured HBM peak, at the workload's
                 batch 32 and at 256 / 1024; roofline_bwd = hk_bilinear_pool_bwd (K1b); roofline_cbp = hk_cbp_fwd (K2);
                 roofline_mpncov = covariance + Newton-Schulz fwd+bwd (K3/K4) against the TF32 tensor peak
   roofline_conv whole-step TF32 TFLOP/s against measured bf16-sustained / 2
   eager_gpu     informational: the same BCNN step in stock PyTorch eager (torch.nn, cuDNN/cuBLAS with TF32 allowed) on the
-                same GPU — the practical bar (SURVEY 2a), not the reference arm
+                same GPU — the practical bar, not the reference arm
   cpu_baseline  the reference step on the host cores: the UNMODIFIED reference when its tree is importable
-                ($HAWKEYE_REF, baseline/_ref, /root/reference; kind "reference"), else the oracle port (kind "port")
+                ($HAWKEYE_REF or baseline/_ref; kind "reference"), else the oracle port (kind "port")
 `--impl reference` times that CPU path only and reports the steps it actually timed.
 """
 import argparse
@@ -32,20 +32,19 @@ sys.path.insert(0, os.path.join(ROOT, 'tests'))
 
 import torch  # noqa: E402
 
-K1_FWD_BYTES_PER_IMG = 1449984      # read X 512*196*4 + write Y 512*512*4 (SURVEY.md 8(d))
+K1_FWD_BYTES_PER_IMG = 1449984      # read X 512*196*4 + write Y 512*512*4
 K1_BWD_BYTES_PER_IMG = 1851392      # read dY + read X + write dX (z recomputed)
 VGG16_FWD_GFLOP_PER_IMG = 122.9
 RESNET50_MPN_FWD_GFLOP_PER_IMG = 32.9
-MPNCOV_GFLOP_PER_IMG = 1.77         # covariance + 5-iteration Newton-Schulz, forward + backward (SURVEY.md 8(d))
-# dram__bytes_read.sum + dram__bytes_write.sum per launch from the ncu --set full captures under profiles/ (see
-# profiles/README.md for the file each number comes from); None = not captured for this build
-K1_DRAM_TRAFFIC = {32: 12.89e6 + 0.01e6, 256: 102.83e6 + 210.72e6}   # profiles/gram_r3_metrics.txt (tests/prof_bilinear.py 32 / 256)
+MPNCOV_GFLOP_PER_IMG = 1.77         # covariance + 5-iteration Newton-Schulz, forward + backward
+# measured DRAM bytes per launch (read + write); None = not captured for this build
+K1_DRAM_TRAFFIC = {32: None, 256: None}
 WORKLOADS = {
     'bcnn_s2': dict(cfg='BCNN_S2.yaml', trainer='BCNN', model='BCNN VGG-16 stage 2', fwd_gflop=VGG16_FWD_GFLOP_PER_IMG, bwd_mult=3.0),
     'bcnn_s1': dict(cfg='BCNN_S1.yaml', trainer='BCNN', model='BCNN VGG-16 stage 1 (classifier only)', fwd_gflop=VGG16_FWD_GFLOP_PER_IMG, bwd_mult=1.0),
     'cbcnn8192': dict(cfg='CBCNN_S1.yaml', trainer='CBCNN', model='CBCNN VGG-16 d=8192 stage 1', fwd_gflop=VGG16_FWD_GFLOP_PER_IMG, bwd_mult=1.0),
     'mpn': dict(cfg='MPN.yaml', trainer='MPN', model='Fast MPN-COV ResNet-50', fwd_gflop=RESNET50_MPN_FWD_GFLOP_PER_IMG, bwd_mult=3.0),
-    # BASELINE.json config 5 (OSME half): ResNet-101 trunk (4 x 7.8 GFLOP at 448x448) + two 401408 -> 1024 attention FCs; MAMC loss
+    # OSME half of the part-attention workload: ResNet-101 trunk (4 x 7.8 GFLOP at 448x448) + two 401408 -> 1024 attention FCs; MAMC loss
     'osmenet': dict(cfg='OSMENet.yaml', trainer='OSMENet', model='OSMENet ResNet-101 + OSME (2 attentions) + MAMC loss',
                     fwd_gflop=32.9, bwd_mult=3.0),
 }
@@ -66,7 +65,7 @@ def measured_peaks():
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,'
          'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,'
          'clocks_event_reasons.sw_power_cap')
@@ -162,7 +161,7 @@ def cpu_step_port(workload, B, threads, steps):
 
 def cpu_step_reference(workload, B, threads, steps):
     """The UNMODIFIED reference (model/registry.MODEL + nn.CrossEntropyLoss(label_smoothing=0.1) + torch.optim, i.e. what
-    train.py:310-325 runs) imported from $HAWKEYE_REF / baseline/_ref / /root/reference.  Raises if the tree is absent."""
+    train.py:310-325 runs) imported from $HAWKEYE_REF / baseline/_ref.  Raises if the tree is absent."""
     from oracle import ref_harness as rh
     if not rh.available():
         raise RuntimeError('reference tree not importable')
@@ -202,7 +201,7 @@ def cpu_step_reference(workload, B, threads, steps):
 
 
 def cpu_baseline(workload, steps):
-    """-> dict(value img/s, cores, kind, sample, dt).  Batch 2 (BASELINE.json configs[0]); all host threads it can use:
+    """-> dict(value img/s, cores, kind, sample, dt).  Batch 2 (configs/BCNN_S1.yaml); all host threads it can use:
     a batch-2 step stops scaling around 32 threads, so 32 and os.cpu_count() are both probed and the faster one is kept."""
     B = 2
     ncpu = os.cpu_count() or 1
@@ -241,7 +240,7 @@ def run_reference_arm(args):
         'steps': timed, 'steps_requested': args.steps, 'warmup': 1, 'ms_per_step': dt * 1e3, 'higher_is_better': True,
         'scaling': 'weak', 'vs_baseline': None, 'dtype': 'f32', 'data': 'synthetic',
         'config': {'workload': f'{WORKLOADS[args.workload]["model"]}, 448x448, 200 classes; CPU sample batch 2 '
-                               f'(BASELINE.json configs[0])'},
+                               f'(configs/BCNN_S1.yaml)'},
         'cpu_baseline': cb,
         'e2e': {'value': cb['value'], 'unit': 'img/s', 'h2d_bytes_per_step': 0, 'd2h_bytes_per_step': 0},
     }
@@ -268,7 +267,7 @@ def _timed_calls(call, nset, reps):
 
 def time_bilinear_kernel(B, bwd=False, min_footprint=640 << 20, reps=4):
     """Average device time per call of hk_bilinear_pool_fwd (or _bwd): `reps` passes over a ring of buffer sets whose
-    total footprint is >= 5x the 126 MB L2, launched back to back and bracketed by one CUDA-event pair on the launching
+    total footprint is >= 5x the 50 MB L2, launched back to back and bracketed by one CUDA-event pair on the launching
     stream.  Every call therefore reads inputs that are not L2-resident and runs while its predecessors' outputs are
     still being written back — the steady state of the kernel, with no separate flush kernel in the timed region."""
     from hawkeye_b200 import _lib
@@ -387,6 +386,25 @@ def eager_gpu_bcnn(stage, B, steps):
                      'batch; informational practical bar, not the reference arm')
 
 
+def dump_outputs(out_dir, model, last, grad_sample=1 << 20):
+    """Logits (plus any further model outputs, as output_<i>) and loss of the last timed step, and the same seeded
+    sample of grad_sample entries (4 MB) of the concatenated parameter gradients (parameter order, frozen parameters
+    skipped), as float32 .npy files."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    out = last['logits']
+    if isinstance(out, (tuple, list)):          # OSMENet returns (logits, part features): both are the step's outputs
+        for i, t in enumerate(out[1:], 1):
+            np.save(os.path.join(out_dir, f'output_{i}.npy'), t.detach().float().cpu().numpy())
+        out = out[0]
+    np.save(os.path.join(out_dir, 'logits.npy'), out.detach().float().cpu().numpy())
+    np.save(os.path.join(out_dir, 'loss.npy'), np.asarray(last['loss'].detach().float().cpu().numpy(), dtype=np.float32))
+    grads = torch.cat([p.grad.detach().float().flatten() for p in model.parameters() if p.grad is not None])
+    idx = torch.randperm(grads.numel(), generator=torch.Generator().manual_seed(0))[:grad_sample].sort().values
+    np.save(os.path.join(out_dir, 'grad_sample.npy'), grads[idx.to(grads.device)].cpu().numpy())
+    np.save(os.path.join(out_dir, 'grad_sample_index.npy'), idx.numpy().astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--gpus', type=int, default=1)
@@ -400,6 +418,9 @@ def main():
     ap.add_argument('--no-e2e', action='store_true', help='profiling runs only')
     ap.add_argument('--no-micro', action='store_true', help='skip the kernel micro-benchmarks (roofline legs)')
     ap.add_argument('--no-eager', action='store_true', help='skip the stock-PyTorch eager GPU leg')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last timed step returned (logits, loss) and a fixed, '
+                         'seeded sample of the parameter gradients it produced as DIR/<name>.npy (float32)')
     ap.add_argument('--graph', default='auto', choices=['auto', '0', '1'],
                     help='replay forward+backward from a CUDA graph (Trainer cuda_graph mode); auto = only for the '
                          'host-launch-bound ResNet-50 workload')
@@ -430,9 +451,11 @@ def main():
     y_host = torch.randint(0, 200, (B,), generator=g).pin_memory()
     x_dev, y_dev = x_host.to(dev), y_host.to(dev)
 
+    last = {}
+
     def step_resident():
         if tr._graph_wanted():           # eager for three steps, captured on the third, replayed from then on
-            _, loss = tr._graph_step(x_dev, y_dev)
+            out, loss = tr._graph_step(x_dev, y_dev)
         else:
             out = tr.model(x_dev)
             loss = tr.criterion(out, y_dev)
@@ -440,6 +463,7 @@ def main():
             loss.backward()
             tr.allreduce.finish()
         tr.optimizer.step()
+        last['logits'], last['loss'] = out, loss
         return loss
 
     def barrier():
@@ -474,6 +498,8 @@ def main():
         launches += args.steps * tr._graph['kernels']
     clocks = sampler.stop() if rank == 0 else None
     value = B * world * args.steps / (ms * 1e-3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, tr.model, last)
 
     # end to end through the public Trainer API with host inputs
     data = {'img': x_host, 'label': y_host}
@@ -498,7 +524,7 @@ def main():
         'dtype': 'tf32 (fp32 storage, fp32 accumulate)', 'data': 'synthetic',
         'config': {'workload': f'{W["model"]}, 448x448, batch {B}/GPU, 200 classes ({W["cfg"]})',
                    'global_batch': B * world, 'parallelism': f'dp{world}', 'cuda_graph': bool(use_graph),
-                   'l2': 'per-step working set (GBs of activations) >> 126 MB L2; kernel microbenches rotate through buffer '
+                   'l2': 'per-step working set (GBs of activations) >> 50 MB L2; kernel microbenches rotate through buffer '
                          'sets totalling >= 640 MB (5x L2), so every launch reads cold inputs',
                    'final_loss': final_loss},
         'clocks': clocks,
@@ -519,12 +545,10 @@ def main():
             return {'achieved': a, 'frac': a / hbm_peak, 'us_per_launch': t * 1e6}
         r32 = bw(32, t32, K1_FWD_BYTES_PER_IMG)
         line['roofline'] = {
-            'kernel': 'hk_bilinear_pool_fwd, one launch: Gram + sqrt + L2 normalise.  B=32 (the per-GPU batch of this workload, '
-                      'C=512, HW=196) = bcnn_super_fwd_kernel<true>: one wave of 4-CTA clusters, four operand-sharing items per '
-                      'image, DSMEM norm exchange; b256 / b1024 = bcnn_gram_fwd_kernel<512>: persistent 128x128 tiles, '
-                      'bounded-wait norm exchange',
+            'kernel': 'hk_bilinear_pool_fwd: Gram on the wgmma GEMM + sqrt / L2 normalise.  B=32 (the per-GPU batch of this '
+                      'workload, C=512, HW=196); b256 / b1024 the same call at larger batches',
             'bound': 'hbm', 'achieved': r32['achieved'], 'peak': hbm_peak, 'unit': 'GB/s', 'frac': r32['frac'],
-            'traffic': K1_DRAM_TRAFFIC[32], 'traffic_note': 'ncu dram read+write per launch: the 33.5 MB output of a B=32 launch stays in the 126 MB L2 under ncu (serialised launches); in the timed back-to-back series it is written back while later launches run', 'peak_source': which, 'us_per_launch': r32['us_per_launch'],
+            'traffic': K1_DRAM_TRAFFIC[32], 'peak_source': which, 'us_per_launch': r32['us_per_launch'],
             'algorithmic_bytes_per_launch': 32 * K1_FWD_BYTES_PER_IMG,
             'b256': dict(bw(256, t256, K1_FWD_BYTES_PER_IMG), traffic=K1_DRAM_TRAFFIC[256]),
             'b1024': bw(1024, t1024, K1_FWD_BYTES_PER_IMG)}

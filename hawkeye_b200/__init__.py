@@ -1,4 +1,4 @@
-"""hawkeye_b200 — B200-native (sm_100a) high-order-pooling hot path behind Hawkeye's plugin surface.
+"""hawkeye_b200 — H100-native (sm_90a) high-order-pooling hot path behind Hawkeye's plugin surface.
 
 ``from hawkeye_b200.registry import MODEL`` mirrors ``model.registry.MODEL``; ``install_into`` overrides the
 reference's own registry entries.  All compute goes through ``libhawkeye_b200.so`` (no fallback).

@@ -3,7 +3,7 @@
 ``features`` is an ``nn.Sequential`` of real ``nn.Conv2d / nn.ReLU / nn.MaxPool2d`` modules, so
 ``state_dict()`` keys (``{0,2,5,...,28}.{weight,bias}``) and shapes are identical to the reference and
 reference checkpoints load unchanged — but ``forward`` never calls those modules: the whole stack runs as
-one fused CUDA pipeline (NHWC, tcgen05 implicit-GEMM convs) through ``ops.vgg_features``.
+one fused CUDA pipeline (NHWC, wgmma implicit-GEMM convs) through ``ops.vgg_features``.
 """
 import torch
 import torch.nn as nn

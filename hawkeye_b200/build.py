@@ -1,4 +1,4 @@
-"""Build libhawkeye_b200.so in-tree with nvcc for sm_100a (called by __graft_entry__.build())."""
+"""Build libhawkeye_b200.so in-tree with nvcc for sm_90a (called by __graft_entry__.build())."""
 import glob
 import os
 import subprocess
@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 OUT = os.path.join(HERE, 'libhawkeye_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
+FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
          '--expt-relaxed-constexpr', '-Xptxas', '-v' if os.environ.get('HK_PTXAS_V') else '-O3']
 
 
@@ -43,7 +43,7 @@ def build(force=False, verbose=False):
             sys.stderr.write(out)
         if p.returncode:
             raise RuntimeError(f'nvcc failed on {s}')
-    cmd = [NVCC, '-gencode', 'arch=compute_100a,code=sm_100a', '-shared', '-o', OUT] + objs + ['-lcudart']
+    cmd = [NVCC, '-gencode', 'arch=compute_90a,code=sm_90a', '-shared', '-o', OUT] + objs + ['-lcudart']
     subprocess.check_call(cmd)
     return OUT
 

@@ -15,7 +15,7 @@ def load_config(path):
 
 
 def setup_config(argv=None):
-    parser = argparse.ArgumentParser(description='Hawkeye (B200-native hot path)')
+    parser = argparse.ArgumentParser(description='Hawkeye (H100-native hot path)')
     parser.add_argument('--config', default='configs/Baseline.yaml', type=str, help='path to config file')
     arg, _ = parser.parse_known_args(argv)
     return load_config(arg.config)

@@ -5,20 +5,13 @@
 // and for compact bilinear pooling (model/methods/CBCNN.py:96-135) the Tensor-Sketch of the
 // un-normalised Gram, which equals the signed scatter  out[(h1[i]+h2[j]) mod d] += s1[i] s2[j] (X X^T)[i][j].
 //
-// Design (B200): the C x C Gram runs on tcgen05 (kind::tf32, fp32 accumulate in TMEM); X tiles are staged by TMA into
-// 128B-swizzled shared memory straight from the NCHW feature map (HW is the K dimension, zero-filled to a multiple of 8 by
-// TMA).  Three users of that Gram live here:
-//   * hk_bilinear_pool_fwd : C = 512 -> the cluster kernel of bilinear_fwd.cu (one launch; X multicast across 4 CTAs);
-//                            other C  -> channel-sum pre-kernel + gram_pair_kernel<MODE_BCNN_FWD> (tile pairs, closed-form norm);
-//   * hk_bilinear_pool_bwd : single-pass backward (bilinear_bwd.cu) or, for shapes it does not cover, gram_pair_kernel<MODE_BCNN_BWD_S>
-//                            (S = (dY+dY^T)/(2z), z recomputed) followed by the S.X contraction on the generic GEMM;
-//   * hk_cbp_fwd           : gram_pair_kernel<MODE_CBP_FWD>, whose epilogue scatters the raw Gram into the d sketch bins.
-// gram_pair_kernel: work item = one CTA = a *pair* of 128x128 Gram tiles sharing the same two 128-row blocks of X:
-//     off-diagonal pair (bi<bj):  acc0 = X_bi X_bj^T , acc1 = X_bj X_bi^T   (same smem, swapped descriptors)
-//     diagonal pair             :  acc0 = X_b0 X_b0^T , acc1 = X_b1 X_b1^T
-// Each accumulator (lane = row of the A block, column = row of the B block) is written to the *transposed* output block —
-// legal because G is symmetric — so the 32 lanes of a warp store 32 consecutive floats (128 B, fully coalesced).
-// The L2 norm is obtained in closed form:  ||z||^2 = sum_p (sum_c x_cp)^2 / HW + C^2 * 1e-5.
+// Design: the C x C Gram X X^T runs on the generic wgmma TF32 GEMM (gemm.cu; HW is the K dimension, X is read straight
+// from the NCHW feature map) and small kernels finish it:
+//   * hk_bilinear_pool_fwd : closed-form norm from the channel sums, then the Gram with sqrt + L2 normalise in its epilogue;
+//   * hk_bilinear_pool_bwd : Gram whose epilogue writes S = (dY+dY^T)/(2z) (z recomputed) and <dY, z>, then the S.X
+//                            contraction on the same GEMM, with the rank-1 correction in its epilogue;
+//   * hk_cbp_fwd           : Gram whose epilogue scatters into the d sketch bins.
+// The C x C Gram itself is never stored.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -28,27 +21,12 @@
 
 namespace hk {
 
-int bcnn_cluster_fwd(const CUtensorMap& tmX, float* y, float* inv_norm, int B, int HW, float inv_hw, cudaStream_t stream,
-                     bool allow_pdl);                                                                          // bilinear_fwd.cu
-int bcnn_cluster_prepare();
-int bcnn_tiles_fwd(const CUtensorMap& tmX, const float* x, float* y, float* inv_norm, int B, int C, int HW, float inv_hw,
-                   cudaStream_t stream);                                                                       // bilinear_fwd_tiles.cu
-int bcnn_super_fwd(const float* x, float* y, float* inv_norm, int B, int C, int HW, float inv_hw, cudaStream_t stream);  // bilinear_fwd_super.cu
-bool bcnn_super_one_wave(int B);      // B images fit in one wave of 4-CTA clusters
 
-__device__ __forceinline__ float fast_sqrt(float x) {
-  float r;
-  asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
-  return r;
-}
 
 // ---------------------------------------------------------------- K0: per-location channel-sum partials
 // partial[b][cs][p] = sum_{c in split cs} x[b][c][p];  also zeroes the per-image scalars used by the backward.
 __global__ void colsum_partial_kernel(const float* __restrict__ X, float* __restrict__ partial, int C, int HW, int CS,
                                       float* zero_a, float* zero_b, int zero_n, unsigned keep_mask = 0xffffe000u) {
-  // let the dependent Gram kernel (launched with programmatic stream serialization) start its TMA/MMA pipeline now;
-  // it only needs our result in its epilogue (griddepcontrol.wait there).
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   extern __shared__ float red[];  // [nrl][HW]
   const int b = blockIdx.x, cs = blockIdx.y;
   if (cs == 0 && threadIdx.x < zero_n) {
@@ -84,361 +62,7 @@ __global__ void colsum_partial_kernel(const float* __restrict__ X, float* __rest
   }
 }
 
-enum { MODE_BCNN_FWD = 0, MODE_BCNN_BWD_S = 1, MODE_CBP_FWD = 2 };
-
-struct GramArgs {
-  int B, C, HW, nblk;
-  float inv_hw, eps;
-  const float* partial;  // [B][CS][HW]
-  int CS;
-  float* Y;              // mode 0: [B][C*C]
-  float* inv_norm;       // mode 0: written [B]; mode 1: read [B]
-  const float* dY;       // mode 1
-  float* S;              // mode 1: [B][C][C]
-  double* c_raw;         // mode 1: [B] (pre-zeroed).  fp64: the 80 atomic partial sums of an image then give the same fp32
-                         // value in any order (an fp32 atomic sum made the whole backward run-to-run different at the tf32
-                         // rounding level, tests/diag/bimodal_debug.py)
-  const int* h1;         // mode 2
-  const int* h2;
-  const float* s1;
-  const float* s2;
-  float* bins;           // mode 2: [B][d] (pre-zeroed)
-  int d;
-  int store_mode;        // 0: st.global.cs (streaming)  1: plain st.global
-  int x_hint;            // 1: X loads carry an L2 evict_last policy
-};
-
-constexpr int GRAM_STAGES = 6;
-constexpr int GRAM_SLOT = 128 * 128;              // 16 KB: 128 rows x 32 fp32
-constexpr int GRAM_STAGE_BYTES = 2 * GRAM_SLOT;   // two row blocks per stage
-constexpr int GRAM_SMEM = GRAM_STAGES * GRAM_STAGE_BYTES + 1024 + 512;
-constexpr int GRAM_THREADS = 320;                 // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue
-
-// decode work item t of an image into its two 128-row blocks
-__device__ __forceinline__ void gram_item(int t, int nblk, int& blk0, int& blk1, int& diag) {
-  const int n_off = nblk * (nblk - 1) / 2;
-  if (t < n_off) {
-    diag = 0;
-    int i = 0;
-    while (t >= nblk - 1 - i) { t -= nblk - 1 - i; ++i; }
-    blk0 = i; blk1 = i + 1 + t;
-  } else {
-    diag = 1;
-    blk0 = 2 * (t - n_off);
-    blk1 = (blk0 + 1 < nblk) ? blk0 + 1 : -1;
-  }
-}
-
-// Persistent: one CTA per SM walks items it, it+grid, ...  (item = image * items_per_image + pair).  The smem ring (6 stages)
-// and the two TMEM accumulator sets (2 x 256 columns) run across item boundaries, so the epilogue of item i (8 warps)
-// overlaps the TMA/MMA of item i+1.
-template <int MODE>
-__global__ void __launch_bounds__(GRAM_THREADS, 1) gram_pair_kernel(const __grid_constant__ CUtensorMap tmX, GramArgs a) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + GRAM_STAGES * GRAM_STAGE_BYTES);
-  uint64_t* empty = full + GRAM_STAGES;
-  uint64_t* acc_full = empty + GRAM_STAGES;    // [2]
-  uint64_t* acc_empty = acc_full + 2;          // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* red = reinterpret_cast<float*>(tmem_slot + 2);  // 8 partial sums + 1 broadcast slot
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int ipi = a.nblk * (a.nblk - 1) / 2 + (a.nblk + 1) / 2;   // items per image
-  const int total_items = a.B * ipi;
-  const int nk = (a.HW + 31) / 32;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmX);
-    for (int s = 0; s < GRAM_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], 8); }
-    fence_barrier_init();
-  }
-  if (warp == 1) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      uint64_t policy;   // keep X resident in L2: every row block is re-read by several CTAs while Y streams through
-      asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(policy));
-      int kbg = 0;
-      for (int it = blockIdx.x; it < total_items; it += gridDim.x) {
-        const int b = it / ipi;
-        int blk0, blk1, diag;
-        gram_item(it - b * ipi, a.nblk, blk0, blk1, diag);
-        for (int kb = 0; kb < nk; ++kb, ++kbg) {
-          const int s = kbg % GRAM_STAGES;
-          const uint32_t ph = (kbg / GRAM_STAGES) & 1;
-          mbar_wait(&empty[s], ph ^ 1);
-          mbar_expect_tx(&full[s], (blk1 >= 0 ? 2 : 1) * GRAM_SLOT);
-          uint8_t* st = smem + s * GRAM_STAGE_BYTES;
-          if (a.x_hint) {
-            tma_load_3d_hint(st, &tmX, &full[s], kb * 32, blk0 * 128, b, policy);
-            if (blk1 >= 0) tma_load_3d_hint(st + GRAM_SLOT, &tmX, &full[s], kb * 32, blk1 * 128, b, policy);
-          } else {
-            tma_load_3d(st, &tmX, &full[s], kb * 32, blk0 * 128, b);
-            if (blk1 >= 0) tma_load_3d(st + GRAM_SLOT, &tmX, &full[s], kb * 32, blk1 * 128, b);
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    {   // warp-uniform loop; tcgen05 issue predicated on one elected lane
-      const uint32_t idesc = make_idesc_tf32(128, 128, 0, 0);
-      const uint64_t desc_tmpl = make_sdesc(0, 16, 1024);
-      int kbg = 0, itl = 0;
-      for (int it = blockIdx.x; it < total_items; it += gridDim.x, ++itl) {
-        const int b = it / ipi;
-        int blk0, blk1, diag;
-        gram_item(it - b * ipi, a.nblk, blk0, blk1, diag);
-        const int set = itl & 1;
-        mbar_wait(&acc_empty[set], ((itl >> 1) & 1) ^ 1);     // epilogue has drained this accumulator set
-        tc_fence_after();
-        const uint32_t d_base = tmem_base + set * 256;
-        for (int kb = 0; kb < nk; ++kb, ++kbg) {
-          const int s = kbg % GRAM_STAGES;
-          const uint32_t ph = (kbg / GRAM_STAGES) & 1;
-          mbar_wait(&full[s], ph);
-          tc_fence_after();
-          const uint32_t s0 = smem_u32(smem + s * GRAM_STAGE_BYTES);
-          const uint64_t d0 = desc_tmpl + (s0 >> 4), d1 = desc_tmpl + ((s0 + GRAM_SLOT) >> 4);
-          const int krem = a.HW - kb * 32;
-          const int ksteps = krem >= 32 ? 4 : (krem + 7) / 8;
-          if (elect_one()) {
-            for (int ks = 0; ks < ksteps; ++ks) {
-              const uint32_t accum = (kb | ks) ? 1u : 0u;
-              if (diag) {
-                umma_tf32_ss(d_base, d0 + ks * 2, d0 + ks * 2, idesc, accum);
-                if (blk1 >= 0) umma_tf32_ss(d_base + 128, d1 + ks * 2, d1 + ks * 2, idesc, accum);
-              } else {
-                umma_tf32_ss(d_base, d0 + ks * 2, d1 + ks * 2, idesc, accum);        // acc0 = X_blk0 X_blk1^T
-                umma_tf32_ss(d_base + 128, d1 + ks * 2, d0 + ks * 2, idesc, accum);  // acc1 = X_blk1 X_blk0^T
-              }
-            }
-            umma_commit(&empty[s]);
-          }
-          __syncwarp();
-        }
-        if (elect_one()) umma_commit(&acc_full[set]);
-        __syncwarp();
-      }
-    }
-  } else {
-    // ------------------------------------------------------------ epilogue: 8 warps; warp w reads TMEM lane quarter w%4,
-    // columns [half*64, half*64+64) of each 128-column accumulator
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int et = threadIdx.x - 64;  // 0..255
-    if (MODE == MODE_BCNN_FWD) asm volatile("griddepcontrol.wait;" ::: "memory");   // K0's channel sums
-    const size_t CC = (size_t)a.C * a.C;
-    int itl = 0, cur_b = -1;
-    float inv_norm = 1.f;
-    for (int it = blockIdx.x; it < total_items; it += gridDim.x, ++itl) {
-      const int b = it / ipi;
-      int blk0, blk1, diag;
-      gram_item(it - b * ipi, a.nblk, blk0, blk1, diag);
-      const int nacc = blk1 >= 0 ? 2 : 1;
-      if (MODE == MODE_BCNN_FWD && b != cur_b) {
-        // closed-form norm from the channel-sum partials (overlaps the TMA/MMA pipeline of this item)
-        cur_b = b;
-        float acc = 0.f;
-        const float* pb = a.partial + (size_t)b * a.CS * a.HW;
-        for (int p = et; p < a.HW; p += 256) {
-          float s = 0.f;
-          for (int cs = 0; cs < a.CS; ++cs) s += pb[cs * a.HW + p];
-          acc = fmaf(s, s, acc);
-        }
-        acc = warp_sum(acc);
-        asm volatile("bar.sync 1, 256;" ::: "memory");      // previous item's readers of red[] are done
-        if (lane == 0) red[warp - 2] = acc;
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        float tot = 0.f;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) tot += red[i];
-        const float nrm = sqrtf(tot * a.inv_hw + (float)a.C * (float)a.C * a.eps);
-        inv_norm = 1.f / fmaxf(nrm, 1e-12f);
-        if (it - b * ipi == 0 && et == 0 && a.inv_norm) a.inv_norm[b] = inv_norm;
-      }
-      const int set = itl & 1;
-      mbar_wait(&acc_full[set], (itl >> 1) & 1);
-      tc_fence_after();
-      float craw = 0.f;
-      for (int ac = 0; ac < nacc; ++ac) {
-        int ablk, bblk;
-        if (diag) { ablk = bblk = (ac == 0 ? blk0 : blk1); }
-        else      { ablk = (ac == 0 ? blk0 : blk1); bblk = (ac == 0 ? blk1 : blk0); }
-        const int ia = ablk * 128 + q * 32 + lane;  // row of the A block held by this thread
-#pragma unroll 1
-        for (int c = half * 2; c < half * 2 + 2; ++c) {
-          float v[32];
-          tmem_ld32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + set * 256 + ac * 128 + c * 32, v);
-          tmem_ld_wait();
-          const int jb0 = bblk * 128 + c * 32;
-          if (MODE == MODE_BCNN_FWD) {
-            float* y = a.Y + (size_t)b * CC + (size_t)jb0 * a.C + ia;
-            if (a.store_mode == 0) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j)   // streaming store: Y is written once and must not evict X from L2
-                __stcs(y + (size_t)j * a.C, tf32_round(fast_sqrt(fmaf(v[j], a.inv_hw, a.eps)) * inv_norm));
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j)
-                y[(size_t)j * a.C] = tf32_round(fast_sqrt(fmaf(v[j], a.inv_hw, a.eps)) * inv_norm);
-            }
-          } else if (MODE == MODE_BCNN_BWD_S) {
-            const float* dyt = a.dY + (size_t)b * CC + (size_t)jb0 * a.C + ia;   // dY[jb][ia]: coalesced over lanes
-            const float4* dyd = reinterpret_cast<const float4*>(a.dY + (size_t)b * CC + (size_t)ia * a.C + jb0);
-            float* s = a.S + (size_t)b * CC + (size_t)jb0 * a.C + ia;
-            float dd[32], dtv[32];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float4 t = __ldg(dyd + j);
-              dd[4 * j] = t.x; dd[4 * j + 1] = t.y; dd[4 * j + 2] = t.z; dd[4 * j + 3] = t.w;
-            }
-#pragma unroll
-            for (int j = 0; j < 32; ++j) dtv[j] = __ldg(dyt + (size_t)j * a.C);   // all loads in flight before any store
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const float z = fast_sqrt(fmaf(v[j], a.inv_hw, a.eps));
-              craw = fmaf(dtv[j], z, craw);
-              s[(size_t)j * a.C] = tf32_round(__fdividef(dtv[j] + dd[j], 2.f * z));
-            }
-          } else {  // MODE_CBP_FWD: signed scatter of the raw Gram into the d sketch bins
-            const int hi = a.h1[ia];
-            const float si = a.s1[ia];
-            float* bins = a.bins + (size_t)b * a.d;
-#pragma unroll 8
-            for (int j = 0; j < 32; ++j) {
-              int bin = hi + a.h2[jb0 + j];
-              if (bin >= a.d) bin -= a.d;
-              atomicAdd(&bins[bin], si * a.s2[jb0 + j] * v[j]);
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[set]);     // 8 warp arrivals free the accumulator set
-      if (MODE == MODE_BCNN_BWD_S) {
-        craw = warp_sum(craw);
-        if (lane == 0) atomicAdd(&a.c_raw[b], (double)craw);
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 512);
-}
-
-static int make_x_map(CUtensorMap* tm, const float* X, int B, int C, int HW) {
-  uint64_t dims[3] = {(uint64_t)HW, (uint64_t)C, (uint64_t)B};
-  uint64_t strides[2] = {(uint64_t)HW * 4, (uint64_t)C * HW * 4};
-  uint32_t box[3] = {32, 128, 1};
-  return make_tmap(tm, X, 3, dims, strides, box);
-}
-
-static int gram_grid(int total_items) {
-  static int sms = 0;
-  if (!sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
-  }
-  return total_items < sms ? total_items : sms;
-}
-
-template <int MODE>
-static int launch_gram(const CUtensorMap& tm, const GramArgs& a, cudaStream_t stream) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gram_pair_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, GRAM_SMEM);
-    if (e != cudaSuccess) return set_error((int)e, "cudaFuncSetAttribute(gram): %s", cudaGetErrorString(e));
-    attr_set = true;
-  }
-  const int items = a.nblk * (a.nblk - 1) / 2 + (a.nblk + 1) / 2;
-  int grid = gram_grid(items * a.B);
-  if (MODE == MODE_BCNN_FWD) {
-    // programmatic dependent launch: overlap this kernel's prologue + TMA/MMA pipeline with the channel-sum kernel
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(GRAM_THREADS);
-    cfg.dynamicSmemBytes = GRAM_SMEM;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, gram_pair_kernel<MODE>, tm, a);
-    if (e != cudaSuccess) return set_error((int)e, "cudaLaunchKernelEx(gram): %s", cudaGetErrorString(e));
-  } else {
-    gram_pair_kernel<MODE><<<grid, GRAM_THREADS, GRAM_SMEM, stream>>>(tm, a);
-  }
-  HK_LAUNCH_CHECK("gram_pair_kernel");
-  return 0;
-}
-
-// ---------------------------------------------------------------- precise mode (3xTF32 Gram from the generic GEMM)
-// y (holding the raw Gram G = X X^T) -> normalize(sqrt(G/HW + eps)); one block per image.
-__global__ void bilinear_finish_kernel(float* __restrict__ y, float* __restrict__ inv_norm_out, int CC, float inv_hw,
-                                       float eps) {
-  __shared__ float red[32];
-  float* yb = y + (size_t)blockIdx.x * CC;
-  float acc = 0.f;
-  for (int e = threadIdx.x; e < CC; e += blockDim.x) acc += fmaf(yb[e], inv_hw, eps);     // z^2
-  acc = warp_sum(acc);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  float t = 0.f;
-  for (int i = 0; i < (int)(blockDim.x >> 5); ++i) t += red[i];
-  const float inv = 1.f / fmaxf(sqrtf(t), 1e-12f);
-  for (int e = threadIdx.x; e < CC; e += blockDim.x) yb[e] = sqrtf(fmaf(yb[e], inv_hw, eps)) * inv;
-  if (threadIdx.x == 0 && inv_norm_out) inv_norm_out[blockIdx.x] = inv;
-}
-// S (holding the raw Gram) -> S[i][j] = (dY[i][j] + dY[j][i]) / (2 z_ij);  inv_norm[b] = 1/||z||, c_raw[b] = <dY, z>
-__global__ void bilinear_bwd_s_kernel(float* __restrict__ S, const float* __restrict__ dY, float* __restrict__ inv_norm,
-                                      double* __restrict__ c_raw, int C, float inv_hw, float eps) {
-  __shared__ float red[2][32];
-  const size_t CC = (size_t)C * C;
-  float* Sb = S + blockIdx.x * CC;
-  const float* dyb = dY + blockIdx.x * CC;
-  float n2 = 0.f, cr = 0.f;
-  for (size_t e = threadIdx.x; e < CC; e += blockDim.x) {
-    const int i = (int)(e / C), j = (int)(e % C);
-    const float z2 = fmaf(Sb[e], inv_hw, eps);
-    const float z = sqrtf(z2);
-    const float d = dyb[e];
-    n2 += z2;
-    cr = fmaf(d, z, cr);
-    Sb[e] = (d + dyb[(size_t)j * C + i]) / (2.f * z);
-  }
-  n2 = warp_sum(n2); cr = warp_sum(cr);
-  if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = n2; red[1][threadIdx.x >> 5] = cr; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float a = 0.f, b = 0.f;
-    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { a += red[0][i]; b += red[1][i]; }
-    inv_norm[blockIdx.x] = 1.f / fmaxf(sqrtf(a), 1e-12f);
-    c_raw[blockIdx.x] = (double)b;
-  }
-}
 // bins[b][(h1[i]+h2[j]) mod d] += s1[i] s2[j] G[b][i][j]
-__global__ void cbp_scatter_kernel(const float* __restrict__ G, const int* __restrict__ h1, const int* __restrict__ h2,
-                                   const float* __restrict__ s1, const float* __restrict__ s2, float* __restrict__ bins,
-                                   int C, int d) {
-  const int b = blockIdx.y;
-  const size_t n = (size_t)C * C;
-  for (size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x; e < n; e += (size_t)gridDim.x * blockDim.x) {
-    const int i = (int)(e / C), j = (int)(e % C);
-    int k = h1[i] + h2[j];
-    if (k >= d) k -= d;
-    atomicAdd(&bins[(size_t)b * d + k], s1[i] * s2[j] * G[(size_t)b * n + e]);
-  }
-}
-
 static int check_gram_shape(const char* op, const float* X, int B, int C, int HW) {
   HK_REQUIRE(X, HK_ERR_ARG, "%s: null input", op);
   HK_REQUIRE(B > 0 && B <= 65535 && C > 0 && HW > 0, HK_ERR_ARG, "%s: bad shape B=%d C=%d HW=%d", op, B, C, HW);
@@ -467,12 +91,12 @@ __global__ void unpad_cols_kernel(const float* __restrict__ xp, float* __restric
 }
 static inline int pad4(int v) { return (v + 3) & ~3; }
 static int launch_pad(const float* x, float* xp, size_t rows, int HW, cudaStream_t st) {
-  pad_cols_kernel<<<148 * 8, 256, 0, st>>>(x, xp, rows, HW, pad4(HW));
+  pad_cols_kernel<<<132 * 8, 256, 0, st>>>(x, xp, rows, HW, pad4(HW));
   HK_LAUNCH_CHECK("pad_cols_kernel");
   return 0;
 }
 static int launch_unpad(const float* xp, float* x, size_t rows, int HW, cudaStream_t st) {
-  unpad_cols_kernel<<<148 * 8, 256, 0, st>>>(xp, x, rows, HW, pad4(HW));
+  unpad_cols_kernel<<<132 * 8, 256, 0, st>>>(xp, x, rows, HW, pad4(HW));
   HK_LAUNCH_CHECK("unpad_cols_kernel");
   return 0;
 }
@@ -524,34 +148,6 @@ __global__ void norm_from_s_kernel(const float* s, float* inv_norm, int C, int H
   }
 }
 
-// colsum_finish + norm_from_s + bilinear_bwd_scalars in one launch (one block per image, after the S kernel):
-//   s[b][p] = sum over splits of partial;  n = sqrt(sum_p s_p^2 / HW + C^2 eps);  alpha = 1/(n HW);  beta = -(c_raw/n^2)/(n HW)
-__global__ void bilinear_bwd_finish_kernel(const float* __restrict__ partial, float* __restrict__ s, float* __restrict__ inv_norm,
-                                           const double* __restrict__ c_raw, float* __restrict__ alpha, float* __restrict__ beta,
-                                           int CS, int C, int HW, float inv_hw) {
-  __shared__ float red[32];
-  const int b = blockIdx.x;
-  float acc = 0.f;
-  for (int p = threadIdx.x; p < HW; p += blockDim.x) {
-    float t = 0.f;
-    for (int cs = 0; cs < CS; ++cs) t += partial[((size_t)b * CS + cs) * HW + p];
-    s[(size_t)b * HW + p] = t;
-    acc = fmaf(t, t, acc);
-  }
-  acc = warp_sum(acc);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float t = 0.f;
-    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) t += red[i];
-    const float nrm = sqrtf(t * inv_hw + (float)C * (float)C * 1e-5f);
-    const float in = 1.f / fmaxf(nrm, 1e-12f);
-    inv_norm[b] = in;
-    alpha[b] = in * inv_hw;
-    beta[b] = -((float)c_raw[b] * in * in) * in * inv_hw;
-  }
-}
-
 }  // namespace hk
 
 namespace hk {
@@ -565,9 +161,10 @@ using namespace hk;
 extern "C" {
 
 size_t hk_bilinear_pool_fwd_workspace_bytes(int B, int C, int HW) {
-  // channel-sum partials [B][CS][HWp] of the two-kernel path + inv_norm [B] (+ the zero-padded copy of x when H*W % 4 != 0)
+  // channel-sum partials [B][CS][HWp] + channel sums [B][HWp] + inv_norm [B] (+ the zero-padded copy of x when H*W % 4 != 0)
   const int HWp = pad4(HW);
-  return ((size_t)B * COLSUM_SPLITS * HWp + pad4(B) + (HWp != HW ? (size_t)B * C * HWp : 0)) * sizeof(float);
+  return ((size_t)B * COLSUM_SPLITS * HWp + (size_t)B * HWp + pad4(B) + (HWp != HW ? (size_t)B * C * HWp : 0)) *
+         sizeof(float);
 }
 
 int hk_bilinear_pool_fwd(const float* x, float* y, float* inv_norm_out, int B, int C, int HW, void* workspace,
@@ -581,7 +178,8 @@ int hk_bilinear_pool_fwd(const float* x, float* y, float* inv_norm_out, int B, i
   const float inv_hw = 1.f / (float)HW;              // normalisations use the true H*W ...
   const int HWp = pad4(HW);
   float* partial = static_cast<float*>(workspace);
-  float* invn_ws = partial + (size_t)B * COLSUM_SPLITS * HWp;
+  float* svec = partial + (size_t)B * COLSUM_SPLITS * HWp;
+  float* invn_ws = svec + (size_t)B * HWp;
   float* invn = inv_norm_out ? inv_norm_out : invn_ws;
   if (HWp != HW) {                                   // ... the kernels' geometry the padded one
     float* xp = invn_ws + pad4(B);                    // 16-byte aligned: TMA reads it
@@ -589,54 +187,21 @@ int hk_bilinear_pool_fwd(const float* x, float* y, float* inv_norm_out, int B, i
     x = xp;
     HW = HWp;
   }
-  if (precise()) {   // 3xTF32 Gram on the generic GEMM, then sqrt + L2 normalise in place; nothing rounded
-    GemmEpi e = {};
-    e.C = y; e.ldc = C; e.strideC = (long long)C * C; e.alpha = 1.f;
-    if ((r = gemm_tf32(x, 0, HW, (long long)C * HW, x, 0, HW, (long long)C * HW, e, C, C, HW, B, stream))) return r;
-    bilinear_finish_kernel<<<B, 1024, 0, stream>>>(y, invn, C * C, inv_hw, 1e-5f);
-    HK_LAUNCH_CHECK("bilinear_finish_kernel");
-    return 0;
-  }
-  CUtensorMap tm;
-  if ((r = make_x_map(&tm, x, B, C, HW))) return r;
-  // $HK_K1: unset = "super" while the batch is one wave of 4-CTA clusters (B <= ~33: the per-GPU batch of the train step),
-  //         "tiles" beyond (measured equal or better there);
-  //         "super" = super-tile kernel, four operand-sharing items per image, cluster / DSMEM norm exchange
-  //         (bilinear_fwd_super.cu); "tiles" = persistent 128x128-tile kernel, bounded-wait exchange (bilinear_fwd_tiles.cu);
-  //         "cluster" = 4-CTA clusters, X multicast, no exchange at all (bilinear_fwd.cu; C = 512); "two" = pre-kernel + pairs
-  static int variant = -1;
-  if (variant < 0) {
-    const char* v = getenv("HK_K1");
-    variant = (v && v[0] == 'c') ? 1 : ((v && v[0] == 't' && v[1] == 'w') ? 2 : ((v && v[0] == 't') ? 0 : ((v && v[0] == 's') ? 3 : 4)));
-  }
-  // Under CUDA-graph capture the tile kernel's per-launch tag would be frozen into the graph and every replay would
-  // accept the previous replay's tile sums: captured launches take a route without cross-CTA state.
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  if (cudaStreamIsCapturing(stream, &cap) != cudaSuccess) { (void)cudaGetLastError(); cap = cudaStreamCaptureStatusNone; }
-  const bool capturing = cap != cudaStreamCaptureStatusNone;
-  if (!capturing && C == 512 && (r = bcnn_cluster_prepare())) return r;     // host-side setup never happens inside a capture
-  if ((variant == 1 || capturing) && C == 512) {
-    r = bcnn_cluster_fwd(tm, y, invn, B, HW, inv_hw, stream, /*allow_pdl=*/!capturing);
-    if (r != HK_ERR_UNSUPPORTED) return r;
-  }
-  if (!capturing && C == 512 && (variant == 3 || (variant == 4 && bcnn_super_one_wave(B)))) {
-    r = bcnn_super_fwd(x, y, invn, B, C, HW, inv_hw, stream);
-    if (r != HK_ERR_UNSUPPORTED) return r;
-  }
-  if (variant != 2 && !capturing) {
-    r = bcnn_tiles_fwd(tm, x, y, invn, B, C, HW, inv_hw, stream);
-    if (r != HK_ERR_UNSUPPORTED) return r;        // more tiles per image than the slot table holds: two-kernel path
-  }
-  GramArgs a = {};
-  a.C = C; a.HW = HW; a.nblk = C / 128;
-  a.inv_hw = inv_hw; a.eps = 1e-5f;
-  a.store_mode = 1; a.x_hint = 1;
-  // general C: channel-sum pre-kernel + tile-pair Gram kernel, overlapped by programmatic dependent launch
-  colsum_partial_kernel<<<dim3(B, COLSUM_SPLITS), 256, colsum_smem(HW), stream>>>(x, partial, C, HW, COLSUM_SPLITS, nullptr, nullptr, 0);
+  // The norm in closed form, before the Gram exists: ||z||^2 = sum_ij (G_ij / HW + eps) = sum_p (sum_c x_cp)^2 / HW +
+  // C^2 eps, from the channel sums of what the tensor core sees (tf32 mode: truncated operands).  The Gram GEMM's epilogue
+  // then writes y = sqrt(G / HW + eps) / ||z|| directly: the C x C Gram never makes a round trip through memory.
+  colsum_partial_kernel<<<dim3(B, COLSUM_SPLITS), 256, colsum_smem(HW), stream>>>(x, partial, C, HW, COLSUM_SPLITS, nullptr,
+                                                                                nullptr, 0, precise() ? 0xffffffffu : 0xffffe000u);
   HK_LAUNCH_CHECK("colsum_partial_kernel");
-  a.B = B; a.partial = partial; a.CS = COLSUM_SPLITS;
-  a.Y = y; a.inv_norm = invn;
-  return launch_gram<MODE_BCNN_FWD>(tm, a, stream);
+  colsum_finish_kernel<<<B, 256, 0, stream>>>(partial, svec, COLSUM_SPLITS, HW);
+  HK_LAUNCH_CHECK("colsum_finish_kernel");
+  norm_from_s_kernel<<<B, 256, 0, stream>>>(svec, invn, C, HW, inv_hw);
+  HK_LAUNCH_CHECK("norm_from_s_kernel");
+  GemmEpi e = {};
+  e.C = y; e.ldc = C; e.strideC = (long long)C * C;
+  e.alpha = inv_hw; e.post_scale = invn; e.post_eps = 1e-5f;
+  e.relu = precise() ? 0 : 2;                        // tf32 mode: rounded, y is the operand of the classifier GEMM
+  return gemm_tf32(x, 0, HW, (long long)C * HW, x, 0, HW, (long long)C * HW, e, C, C, HW, B, stream);
 }
 
 size_t hk_bilinear_pool_bwd_workspace_bytes(int B, int C, int HW) {
@@ -684,39 +249,27 @@ static int bilinear_bwd_impl(const float* x, const float* dy, float* dx, int B, 
                              cudaStream_t stream) {
   void* stream_ = stream;
   int r;
-  if (precise()) {
-    colsum_partial_kernel<<<dim3(B, COLSUM_SPLITS), 256, colsum_smem(HW), stream>>>(x, partial, C, HW, COLSUM_SPLITS, nullptr,
-                                                                                  nullptr, 0, 0xffffffffu);
-    HK_LAUNCH_CHECK("colsum_partial_kernel");
-    colsum_finish_kernel<<<B, 256, 0, stream>>>(partial, svec, COLSUM_SPLITS, HW);
-    HK_LAUNCH_CHECK("colsum_finish_kernel");
-    GemmEpi e = {};
-    e.C = S; e.ldc = C; e.strideC = (long long)C * C; e.alpha = 1.f;
-    if ((r = gemm_tf32(x, 0, HW, (long long)C * HW, x, 0, HW, (long long)C * HW, e, C, C, HW, B, stream))) return r;
-    bilinear_bwd_s_kernel<<<B, 1024, 0, stream>>>(S, dy, invn, craw, C, inv_hw, 1e-5f);
-    HK_LAUNCH_CHECK("bilinear_bwd_s_kernel");
-    bilinear_bwd_scalars_kernel<<<(B + 127) / 128, 128, 0, stream>>>(invn, craw, inv_hw, alpha, beta, B);
-    HK_LAUNCH_CHECK("bilinear_bwd_scalars_kernel");
-    return hk_gemm_tf32(S, 0, C, (long long)C * C, x, 1, HW, (long long)C * HW, dx, HW, (long long)C * HW, 0, C, HW, C, B,
-                        1.f, alpha, 0.f, svec, 0, HW, 1.f, beta, 0, stream_);
-  }
-  CUtensorMap tm;
-  if ((r = make_x_map(&tm, x, B, C, HW))) return r;
+  // tf32 mode: the column sums see what the tensor core sees (truncated operands); the launch also zeroes c_raw
   colsum_partial_kernel<<<dim3(B, COLSUM_SPLITS), 256, colsum_smem(HW), stream>>>(x, partial, C, HW, COLSUM_SPLITS,
-                                                                                reinterpret_cast<float*>(craw), nullptr, 2);
+                                                                                reinterpret_cast<float*>(craw), nullptr, 2,
+                                                                                precise() ? 0xffffffffu : 0xffffe000u);
   HK_LAUNCH_CHECK("colsum_partial_kernel");
-  GramArgs a = {};
-  a.B = B; a.C = C; a.HW = HW; a.nblk = C / 128;
-  a.inv_hw = inv_hw; a.eps = 1e-5f;
-  a.dY = dy; a.S = S; a.c_raw = craw;
-  if ((r = launch_gram<MODE_BCNN_BWD_S>(tm, a, stream))) return r;
-  // s_p = sum_c x_cp (the rank-1 correction vector of the backward), the closed-form norm and the epilogue scalars: one launch
-  bilinear_bwd_finish_kernel<<<B, 256, 0, stream>>>(partial, svec, invn, craw, alpha, beta, COLSUM_SPLITS, C, HW, inv_hw);
-  HK_LAUNCH_CHECK("bilinear_bwd_finish_kernel");
-  // dX = alpha_b * (S . X) + beta_b * 1 s^T      (M=C, K=C, N=HW; X is the MN-major B operand); rounded to tf32: it is
+  colsum_finish_kernel<<<B, 256, 0, stream>>>(partial, svec, COLSUM_SPLITS, HW);
+  HK_LAUNCH_CHECK("colsum_finish_kernel");
+  norm_from_s_kernel<<<B, 256, 0, stream>>>(svec, invn, C, HW, inv_hw);      // closed-form 1/||z||, as in the forward
+  HK_LAUNCH_CHECK("norm_from_s_kernel");
+  // S = (dY + dY^T) / (2 z) and c_raw = <dY, z> straight from the Gram accumulators (z recomputed in the epilogue)
+  GemmEpi e = {};
+  e.C = S; e.ldc = C; e.strideC = (long long)C * C;
+  e.alpha = inv_hw; e.post_eps = 1e-5f;
+  e.mode = EPI_BILINEAR_S; e.dY = dy; e.c_raw = craw;
+  if ((r = gemm_tf32(x, 0, HW, (long long)C * HW, x, 0, HW, (long long)C * HW, e, C, C, HW, B, stream))) return r;
+  bilinear_bwd_scalars_kernel<<<(B + 127) / 128, 128, 0, stream>>>(invn, craw, inv_hw, alpha, beta, B);
+  HK_LAUNCH_CHECK("bilinear_bwd_scalars_kernel");
+  // dX = alpha_b * (S . X) + beta_b * 1 s^T      (M=C, K=C, N=HW; X is the MN-major B operand); in tf32 mode rounded: it is
   // the dY operand of the last conv's dgrad / wgrad MMAs
   return hk_gemm_tf32(S, 0, C, (long long)C * C, x, 1, HW, (long long)C * HW, dx, HW, (long long)C * HW, 0, C, HW, C, B,
-                      1.f, alpha, 0.f, svec, 0, HW, 1.f, beta, 2, stream_);
+                      1.f, alpha, 0.f, svec, 0, HW, 1.f, beta, precise() ? 0 : 2, stream_);
 }
 }  // namespace hk
 
@@ -724,9 +277,8 @@ static int bilinear_bwd_impl(const float* x, const float* dy, float* dx, int B, 
 // =====================================================================================================
 // Compact bilinear pooling (reference model/methods/CBCNN.py:96-135) via the Gram-scatter identity:
 //   sum_p ifft(fft(x_p S1) * fft(x_p S2)).real [k]  ==  sum_{i,j : (h1[i]+h2[j]) mod d = k} s1[i] s2[j] (X X^T)[i][j]
-// so the forward is the same tcgen05 Gram (MODE_CBP_FWD epilogue scatters into the d bins), followed by
-// signed-sqrt (eps 1e-10, CBCNN.py:132) + L2 normalise (:133); no [B*HW, d] sketch or FFT intermediates ever
-// touch HBM (algorithmic traffic: read X, write d floats per image).
+// so the forward is the same Gram, scattered into the d bins by its epilogue (never stored), followed by
+// signed-sqrt (eps 1e-10, CBCNN.py:132) + L2 normalise (:133); no [B*HW, d] sketch or FFT intermediates are formed.
 // =====================================================================================================
 namespace hk {
 
@@ -827,26 +379,12 @@ int hk_cbp_fwd(const float* x, const int* h1, const int* h2, const float* s1, co
   }
   cudaError_t e = cudaMemsetAsync(pre, 0, (size_t)B * d * sizeof(float), stream);
   if (e != cudaSuccess) return set_error((int)e, "cudaMemsetAsync(pre): %s", cudaGetErrorString(e));
-  if (precise()) {   // 3xTF32 Gram on the generic GEMM, scattered into the bins by a plain kernel
-    Scratch g((size_t)B * C * C * sizeof(float), stream);
-    HK_REQUIRE(g.p, HK_ERR_DRIVER, "hk_cbp_fwd (precise): cudaMallocAsync failed");
-    GemmEpi ge = {};
-    ge.C = g.f(); ge.ldc = C; ge.strideC = (long long)C * C; ge.alpha = 1.f;
-    if ((r = gemm_tf32(x, 0, HW, (long long)C * HW, x, 0, HW, (long long)C * HW, ge, C, C, HW, B, stream))) return r;
-    cbp_scatter_kernel<<<dim3(148, B), 256, 0, stream>>>(g.f(), h1, h2, s1, s2, pre, C, d);
-    HK_LAUNCH_CHECK("cbp_scatter_kernel");
-    cbp_finalize_fwd_kernel<<<B, 256, 0, stream>>>(pre, y, d, 0);
-    HK_LAUNCH_CHECK("cbp_finalize_fwd_kernel");
-    return 0;
-  }
-  CUtensorMap tm;
-  if ((r = make_x_map(&tm, x, B, C, HW))) return r;
-  GramArgs a = {};
-  a.B = B; a.C = C; a.HW = HW; a.nblk = C / 128;
-  a.inv_hw = 1.f; a.eps = 0.f;
-  a.h1 = h1; a.h2 = h2; a.s1 = s1; a.s2 = s2; a.bins = pre; a.d = d;
-  if ((r = launch_gram<MODE_CBP_FWD>(tm, a, stream))) return r;
-  cbp_finalize_fwd_kernel<<<B, 256, 0, stream>>>(pre, y, d, 1);
+  // the Gram GEMM's epilogue scatters s1[i] s2[j] G_ij into the d bins: the C x C Gram is never stored
+  GemmEpi ge = {};
+  ge.C = pre; ge.ldc = C; ge.strideC = 0; ge.alpha = 1.f;     // C is not written in EPI_SKETCH mode
+  ge.mode = EPI_SKETCH; ge.h1 = h1; ge.h2 = h2; ge.s1 = s1; ge.s2 = s2; ge.bins = pre; ge.d = d;
+  if ((r = gemm_tf32(x, 0, HW, (long long)C * HW, x, 0, HW, (long long)C * HW, ge, C, C, HW, B, stream))) return r;
+  cbp_finalize_fwd_kernel<<<B, 256, 0, stream>>>(pre, y, d, precise() ? 0 : 1);
   HK_LAUNCH_CHECK("cbp_finalize_fwd_kernel");
   return 0;
 }
@@ -873,7 +411,7 @@ int hk_cbp_bwd(const float* x, const float* pre, const float* dy, const int* h1,
   float* dpre = S + (size_t)B * C * C;
   cbp_finalize_bwd_kernel<<<B, 256, 0, stream>>>(pre, dy, dpre, d);
   HK_LAUNCH_CHECK("cbp_finalize_bwd_kernel");
-  cbp_build_s_kernel<<<dim3(148, B), 256, 0, stream>>>(dpre, h1, h2, s1, s2, S, C, d, precise() ? 0 : 1);
+  cbp_build_s_kernel<<<dim3(132, B), 256, 0, stream>>>(dpre, h1, h2, s1, s2, S, C, d, precise() ? 0 : 1);
   HK_LAUNCH_CHECK("cbp_build_s_kernel");
   // dX = (dG + dG^T) . X      (M = C, K = C, N = HW; X is the MN-major B operand)
   return hk_gemm_tf32(S, 0, C, (long long)C * C, x, 1, HWp, (long long)C * HWp, dx, HW, (long long)C * HW, 0, C, HW, C, B,

@@ -1,6 +1,6 @@
 // Channel-interaction kernels (reference model/methods/CIN.py:24-60, ChannelInteractionModule): the row softmax of the
 // negated channel Gram (:32), the contrastive weight |W_SCI - w * W_SCI_BA| (:51-53) and the spatial average pool of the
-// classifier (:71-82).  The Gram, the W.X products, the 3x3 convolution and the fc layer run on the tcgen05 GEMM /
+// classifier (:71-82).  The Gram, the W.X products, the 3x3 convolution and the fc layer run on the wgmma GEMM /
 // implicit-GEMM kernels through the entry points of gemm.cu / conv.cu; these are the HBM-bound pieces in between.
 #include "common.cuh"
 #include "host.h"
@@ -153,7 +153,7 @@ __global__ void relu_bwd_kernel(const float* __restrict__ y, const float* __rest
 
 static inline int cgrid(size_t n, int block) {
   size_t g = (n + block - 1) / block;
-  const size_t cap = 148 * 16;
+  const size_t cap = 132 * 16;
   return (int)(g < cap ? (g ? g : 1) : cap);
 }
 

@@ -1,6 +1,5 @@
-// Shared sm_100a device primitives for the hawkeye_b200 kernels: mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (UMMA) + TMEM wrappers, shared-memory / instruction
-// descriptors.  Everything here is inline PTX; no CUTLASS dependency.
+// Shared sm_90a device primitives for the hawkeye_b200 kernels: mbarrier, TMA (cp.async.bulk.tensor), wgmma
+// wrappers and shared-memory descriptors.  Everything here is inline PTX; no CUTLASS dependency.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -47,30 +46,18 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// non-blocking probe (try_wait may suspend the thread for a system-dependent time when the phase is not complete)
-__device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-      "selp.u32 %0, 1, 0, p;\n"
-      "}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > HK_SPIN_LIMIT) {
-      printf("hawkeye_b200: mbarrier watchdog (block %d,%d,%d thread %d)\n", blockIdx.x, blockIdx.y, blockIdx.z,
-             threadIdx.x);
-      __trap();
-    }
+    if (++spins > HK_SPIN_LIMIT) __trap();
   }
 }
+
+// warp-specialised register budget: the producer warpgroup gives registers back, the MMA warpgroups take them
+template <int N>
+__device__ __forceinline__ void regs_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void regs_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // ------------------------------------------------------------------ TMA (tiled tensor maps)
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
@@ -90,20 +77,6 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uin
       "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-// 3-D load with an L2 cache-policy hint (createpolicy result)
-__device__ __forceinline__ void tma_load_3d_hint(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
-                                                 uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4, "
-      "%5}], [%2], %6;" ::"r"(smem_u32(dst)),
-      "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "l"(policy)
-      : "memory");
-}
-// L2 prefetch of a 3-D box (no shared-memory destination, no barrier): later loads of the same box hit L2.
-__device__ __forceinline__ void tma_prefetch_l2_3d(const CUtensorMap* m, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];" ::"l"(m), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
 __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
                                             int c3) {
   asm volatile(
@@ -113,130 +86,115 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-// ------------------------------------------------------------------ tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
+// ------------------------------------------------------------------ wgmma (sm_90a warpgroup MMA)
+// A warpgroup (4 consecutive warps, the first one's index a multiple of 4) computes a 64 x N tile:
+//   D[64 x N] (+)= A[64 x 8] . B[N x 8]^T, tf32 inputs (fp32 words in smem, low mantissa bits ignored), fp32 accumulate.
+// Both operands are K-major in shared memory (tf32 wgmma has no transposed form).  Accumulator fragment of thread
+// t = 32 w + l:  d[4 i + e]  at row 16 w + l / 4 + 8 (e >> 1), column 8 i + 2 (l & 3) + (e & 1).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+template <int NACC>
+__device__ __forceinline__ void wgmma_keep(float (&d)[NACC]) {   // registers stay live across the async MMA
+#pragma unroll
+  for (int i = 0; i < NACC; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// tcgen05.commit: arrives on the mbarrier when all previously issued MMAs of this thread retire.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], TF32 inputs (fp32 words in smem, low mantissa bits ignored), fp32 accumulate.
-__device__ __forceinline__ void umma_tf32_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_tf32(float (&d)[8], uint64_t adesc, uint64_t bdesc, int scale_d) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %10, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
-// A operand taken from TMEM (128 lanes x K columns of fp32 words).
-__device__ __forceinline__ void umma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_tf32(float (&d)[16], uint64_t adesc, uint64_t bdesc, int scale_d) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_tf32(float (&d)[32], uint64_t adesc, uint64_t bdesc, int scale_d) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t adesc, uint64_t bdesc, int scale_d) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
 
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns (thread i gets lane base+i).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+// named barrier over `count` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void named_bar(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// registers -> TMEM, same shape as tmem_ld32.
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float* v) {
-  const uint32_t* r = reinterpret_cast<const uint32_t*>(v);
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%32], "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31};" ::"r"(r[0]),
-      "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]),
-      "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]),
-      "r"(r[29]), "r"(r[30]), "r"(r[31]), "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // ------------------------------------------------------------------ descriptors
-// Shared-memory matrix descriptor, SWIZZLE_128B, sm_100 "version 1" (bits 46-47 = 1).
-//   K-major operand : rows of 128 B (32 fp32 of K), 8-row groups SBO bytes apart (1024); LBO unused.
-//   MN-major operand: k-rows of 128 B (32 fp32 of M/N), 8 k-rows = one 1024 B atom; the next
-//                     32 M/N elements are LBO bytes away, the next 8 k-rows SBO bytes away.
-//                     For 32-bit (tf32) data the MN-major layout is SWIZZLE_128B_BASE32B (type 1): 32 B chunks
-//                     swizzled over 4 k-rows (512 B atom), so SBO = 512 for contiguous k-rows.
-__device__ __forceinline__ uint64_t make_sdesc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                               uint32_t layout_type = 2) {
+// sm_90 shared-memory matrix descriptor of a K-major, 128B-swizzled operand: rows of 128 B (32 fp32 of K), 8-row groups
+// 1024 B apart (SBO); LBO unused for swizzled K-major layouts (1).  The tile base is 1024-byte aligned; the k-step of 8
+// tf32 inside the swizzle row is +32 B on the start address (+2 in 16-byte units).
+__device__ __forceinline__ uint64_t make_sdesc(uint32_t saddr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFFu);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(layout_type) << 61;
+  d |= static_cast<uint64_t>(1) << 16;
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;
+  d |= static_cast<uint64_t>(1) << 62;   // SWIZZLE_128B
   return d;
 }
-// Instruction descriptor for kind::tf32, fp32 accumulate.
-// MN-major tf32 operand: `mn_block_stride` bytes between consecutive 32-element M/N blocks; k-rows contiguous.
-__device__ __forceinline__ uint64_t make_sdesc_mn(uint32_t saddr, uint32_t mn_block_stride) {
-  return make_sdesc(saddr, mn_block_stride, 512, 1);
-}
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-         (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
+
+// byte offset of fp32 element (row, k) in a K-major 128B-swizzled tile (row = M/N index, k < 32): the 16-byte chunk
+// index is XOR-ed with row & 7 — the layout TMA's SWIZZLE_128B writes for a [rows][32] box.
+__device__ __forceinline__ uint32_t sw128_off(int row, int k) {
+  return (uint32_t)(row * 128 + ((((k >> 2) ^ (row & 7)) << 4) | ((k & 3) << 2)));
 }
 
-// round-to-nearest fp32 -> tf32 (low 13 mantissa bits zero).  tcgen05 kind::tf32 *truncates* its fp32 inputs, so
+// MN-major -> K-major: `src` holds (rows / 32) SWIZZLE_128B boxes of [32 k][32 rows] (box j at src + box_stride j, as TMA
+// writes a [K][rows] operand with rows contiguous); `dst` receives the [rows][32 k] K-major swizzled tile wgmma reads.
+// Called by `nthr` threads (thread index `t`); the caller fences (fence_proxy_async) before the tensor core reads dst.
+__device__ __forceinline__ void transpose_mn_tile(const uint8_t* src, uint8_t* dst, int rows, int t, int nthr,
+                                                  int box_stride = 4096) {
+  for (int r = t; r < rows; r += nthr) {
+    const uint8_t* box = src + (r >> 5) * box_stride;
+    const int rr = r & 31;
+#pragma unroll
+    for (int k4 = 0; k4 < 8; ++k4) {
+      float4 v;
+      v.x = *reinterpret_cast<const float*>(box + sw128_off(4 * k4 + 0, rr));
+      v.y = *reinterpret_cast<const float*>(box + sw128_off(4 * k4 + 1, rr));
+      v.z = *reinterpret_cast<const float*>(box + sw128_off(4 * k4 + 2, rr));
+      v.w = *reinterpret_cast<const float*>(box + sw128_off(4 * k4 + 3, rr));
+      *reinterpret_cast<float4*>(dst + sw128_off(r, 4 * k4)) = v;
+    }
+  }
+}
+
+// round-to-nearest fp32 -> tf32 (low 13 mantissa bits zero).  The tensor core *truncates* its fp32 inputs, so
 // producers round the values they hand to the next MMA; this keeps the TF32 error unbiased.
 __device__ __forceinline__ float tf32_round(float x) {
   // round to nearest, ties away from zero (= cvt.rna.tf32.f32) on the sign-magnitude bit pattern: two integer ops instead
-  // of the NaN/Inf-checked sequence the cvt is expanded to on sm_100a; +-Inf stay Inf, the largest finite values round to Inf.
+  // of the NaN/Inf-checked sequence the cvt expands to; +-Inf stay Inf, the largest finite values round to Inf.
   return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u);
-}
-
-// one lane of a fully converged warp (the MMA warp runs its loop warp-uniformly so descriptor arithmetic stays on the
-// uniform datapath; only the tcgen05 issue itself is predicated on the elected lane)
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "elect.sync _|p, 0xffffffff;\n"
-      "selp.u32 %0, 1, 0, p;\n"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
 }
 
 __device__ __forceinline__ float warp_sum(float v) {

@@ -1,10 +1,10 @@
 // VGG-16 backbone convolutions (reference model/backbone/vgg.py:56-70: Conv2d 3x3 s1 p1 + bias, ReLU,
-// MaxPool2d 2x2) as im2col-free implicit GEMMs on tcgen05 (kind::tf32, fp32 accumulate in TMEM).
+// MaxPool2d 2x2) as im2col-free implicit GEMMs on wgmma (tf32 inputs, fp32 accumulate in registers).
 //
 // Layout: activations are NHWC fp32 inside the backbone.  For a 3x3 tap (kh,kw) the A operand of the
 // implicit GEMM is the input window shifted by (kh-1,kw-1); a 4-D TMA box {32 ch, TW, TH, TN} at the
 // shifted (possibly negative) coordinate lands as 128 rows x 128 B in 128B-swizzled shared memory —
-// exactly the K-major UMMA layout — and TMA's out-of-bounds zero fill *is* the conv padding.
+// exactly the K-major wgmma operand layout — and TMA's out-of-bounds zero fill *is* the conv padding.
 //   fwd   : Y[pix, co]  = sum_{tap,ci} X[pix+tap, ci] * Wf[tap][co][ci]        (+bias, ReLU)
 //   dgrad : dX[pix, ci] = sum_{tap,co} dY[pix+tap, co] * Wd[tap][ci][co]       (Wd = flipped/transposed W; * (act>0))
 //   wgrad : dW[tap][co][ci] = sum_pix dY[pix, co] * X[pix+tap, ci]             (both operands MN-major; split-K)
@@ -111,30 +111,121 @@ __device__ __forceinline__ void epi_pool_store(const ConvArgs& a, const float* v
   }
 }
 
+constexpr int CONV_THREADS = 384;
+
 template <int BN>
 struct ConvCfg {
-  static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128 ? 3 : 4);
-  static constexpr int MIN_CTAS = (BN == 256) ? 1 : 2;
+  static constexpr int STAGES = 4;
   static constexpr int A_BYTES = 128 * 128;
   static constexpr int B_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 + 256;
+  static constexpr int ACC_TILE = 2 * 128 * 33 * 4;   // two 32-column accumulator chunks, row-major, padded rows
+  static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 + 256 + ACC_TILE;
 };
 
+// Epilogue of one 128-pixel x BN tile, run by the 256 MMA threads (ct = thread index among them).  The accumulators go
+// through shared memory two 32-column chunks at a time, after which thread (half, q, lane) owns pixel r = 32 q + lane of
+// chunk 2 c + half — the mapping the fused pooling shuffles rely on.
 template <int BN>
-__global__ void __launch_bounds__(192, ConvCfg<BN>::MIN_CTAS)
+__device__ __forceinline__ void conv_epilogue(const ConvArgs& a, const float (&acc)[BN / 2], float* acc_tile, int w0, int h0,
+                                              int n0, int co0, int ct) {
+  constexpr int NACC = BN / 2;
+  const int lane = ct & 31, wg = ct >> 7, half = ct >> 7;
+  const int q = (ct >> 5) & 3, wl = q;
+  const int r = q * 32 + lane;
+  const int wi = r % a.TW, hi = (r / a.TW) % a.TH, ni = r / (a.TW * a.TH);
+  const int w = w0 + wi, h = h0 + hi, n = n0 + ni;
+  const bool valid = (w < a.W) && (h < a.H) && (n < a.N);
+  const size_t pix = ((size_t)n * a.H + h) * a.W + w;
+#pragma unroll
+  for (int cp = 0; cp < BN / 64; ++cp) {
+    named_bar(1, 256);
+#pragma unroll
+    for (int i = 0; i < NACC / 4; ++i) {
+      const int col = 8 * i + 2 * (lane & 3);
+      if ((col >> 6) != cp) continue;
+      float* dst = acc_tile + ((col >> 5) & 1) * (128 * 33);
+      const int r0 = wg * 64 + wl * 16 + (lane >> 2);
+      dst[r0 * 33 + (col & 31)] = acc[4 * i];
+      dst[r0 * 33 + (col & 31) + 1] = acc[4 * i + 1];
+      dst[(r0 + 8) * 33 + (col & 31)] = acc[4 * i + 2];
+      dst[(r0 + 8) * 33 + (col & 31) + 1] = acc[4 * i + 3];
+    }
+    named_bar(1, 256);
+    const int c = 2 * cp + half;
+    float v[32];
+    {
+      const float* src = acc_tile + half * (128 * 33) + r * 33;
+#pragma unroll
+      for (int j = 0; j < 32; ++j) v[j] = src[j];
+    }
+    const int co = co0 + c * 32;
+    if (valid && co < a.Cout) {
+      if (a.addend) {
+        const float4* ad = reinterpret_cast<const float4*>(a.addend + pix * a.Cout + co);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float4 t = ad[j];
+          v[4 * j] += t.x; v[4 * j + 1] += t.y; v[4 * j + 2] += t.z; v[4 * j + 3] += t.w;
+        }
+      }
+      if (a.bias) {
+#pragma unroll
+        for (int j = 0; j < 32; ++j) v[j] += __ldg(a.bias + co + j);
+      }
+      if (a.relu) {
+#pragma unroll
+        for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
+      }
+      if (a.mask) {
+        const float4* m = reinterpret_cast<const float4*>(a.mask + pix * a.Cout + co);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float4 mm = m[j];
+          v[4 * j] = mm.x > 0.f ? v[4 * j] : 0.f;
+          v[4 * j + 1] = mm.y > 0.f ? v[4 * j + 1] : 0.f;
+          v[4 * j + 2] = mm.z > 0.f ? v[4 * j + 2] : 0.f;
+          v[4 * j + 3] = mm.w > 0.f ? v[4 * j + 3] : 0.f;
+        }
+      }
+      if (a.P) {       // (never combined with the precise-mode passes: rounded like the stored map would be)
+#pragma unroll
+        for (int j = 0; j < 32; ++j) v[j] = tf32_round(v[j]);
+      } else {
+      float4* dst = reinterpret_cast<float4*>(a.Y + pix * a.Cout + co);
+      if (a.no_round) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) dst[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+      } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          dst[j] = make_float4(tf32_round(v[4 * j]), tf32_round(v[4 * j + 1]), tf32_round(v[4 * j + 2]),
+                               tf32_round(v[4 * j + 3]));
+      }
+      }
+    }
+    // the window reduction is a warp-wide shuffle: every lane takes part, whether or not its own pixel is valid
+    if (a.P && co < a.Cout) epi_pool_store(a, v, a.TW, w, h, n, co, valid);
+  }
+}
+
+// warpgroup 0: TMA producer (one thread); warpgroups 1-2: wgmma on rows 0-63 / 64-127 of the 128-pixel tile, then the
+// epilogue.  The accumulators go through shared memory two 32-column chunks at a time, after which consumer thread
+// (half, q, lane) owns pixel r = 32 q + lane of chunk 2 c + half — the mapping the fused pooling shuffles rely on.
+template <int BN>
+__global__ void __launch_bounds__(CONV_THREADS, 1)
 conv3x3_igemm_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, ConvArgs a) {
   using Cfg = ConvCfg<BN>;
+  constexpr int NACC = BN / 2;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sB = smem + Cfg::STAGES * Cfg::A_BYTES;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
   uint64_t* empty = full + Cfg::STAGES;
-  uint64_t* accf = empty + Cfg::STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accf + 1);
+  float* acc_tile = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES + 256);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
   int t = blockIdx.x;
   const int tw = t % a.tiles_w; t /= a.tiles_w;
   const int th = t % a.tiles_h; t /= a.tiles_h;
@@ -143,21 +234,17 @@ conv3x3_igemm_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
   const int nchunk = a.Cin / 32;
   const int nk = 9 * nchunk;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmW);
-    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(accf, 1);
+    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
     fence_barrier_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_slot, BN); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    regs_dealloc<56>();
+    if (threadIdx.x == 0) {
       for (int kb = 0; kb < nk; ++kb) {
         const int s = kb % Cfg::STAGES;
         const uint32_t ph = (kb / Cfg::STAGES) & 1;
@@ -169,93 +256,29 @@ conv3x3_igemm_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
         tma_load_3d(sB + s * Cfg::B_BYTES, &tmW, &full[s], ck * 32, co0, tap);
       }
     }
-  } else if (warp == 1) {
-    {   // warp-uniform loop (descriptor math on the uniform datapath); tcgen05 issue predicated on one elected lane
-      const uint32_t idesc = make_idesc_tf32(128, BN, 0, 0);
-      const uint64_t desc_tmpl = make_sdesc(0, 16, 1024);
-      for (int kb = 0; kb < nk; ++kb) {
-        const int s = kb % Cfg::STAGES;
-        const uint32_t ph = (kb / Cfg::STAGES) & 1;
-        mbar_wait(&full[s], ph);
-        tc_fence_after();
-        const uint64_t a_base = desc_tmpl + (smem_u32(sA + s * Cfg::A_BYTES) >> 4);
-        const uint64_t b_base = desc_tmpl + (smem_u32(sB + s * Cfg::B_BYTES) >> 4);
-        if (elect_one()) {
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) umma_tf32_ss(tmem_base, a_base + ks * 2, b_base + ks * 2, idesc, (kb | ks) ? 1u : 0u);
-          umma_commit(&empty[s]);
-        }
-        __syncwarp();
-      }
-      if (elect_one()) umma_commit(accf);
-      __syncwarp();
-    }
   } else {
-    const int q = warp & 3;
-    const int r = q * 32 + lane;
-    const int wi = r % a.TW, hi = (r / a.TW) % a.TH, ni = r / (a.TW * a.TH);
-    const int w = w0 + wi, h = h0 + hi, n = n0 + ni;
-    const bool valid = (w < a.W) && (h < a.H) && (n < a.N);
-    const size_t pix = ((size_t)n * a.H + h) * a.W + w;
-    mbar_wait(accf, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-      float v[32];
-      tmem_ld32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + c * 32, v);
-      tmem_ld_wait();
-      const int co = co0 + c * 32;
-      if (valid && co < a.Cout) {
-        if (a.addend) {
-          const float4* ad = reinterpret_cast<const float4*>(a.addend + pix * a.Cout + co);
+    regs_alloc<224>();
+    const int ct = threadIdx.x - 128;
+    const int wg = ct >> 7;
+    float acc[NACC];          // overwritten by the first MMA (scale-d = 0): nk >= 9
+    for (int kb = 0; kb < nk; ++kb) {
+      const int s = kb % Cfg::STAGES;
+      const uint32_t ph = (kb / Cfg::STAGES) & 1;
+      mbar_wait(&full[s], ph);
+      const uint64_t a_base = make_sdesc(smem_u32(sA + s * Cfg::A_BYTES + wg * 64 * 128));
+      const uint64_t b_base = make_sdesc(smem_u32(sB + s * Cfg::B_BYTES));
+      wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 t = ad[j];
-            v[4 * j] += t.x; v[4 * j + 1] += t.y; v[4 * j + 2] += t.z; v[4 * j + 3] += t.w;
-          }
-        }
-        if (a.bias) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += __ldg(a.bias + co + j);
-        }
-        if (a.relu) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-        }
-        if (a.mask) {
-          const float4* m = reinterpret_cast<const float4*>(a.mask + pix * a.Cout + co);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 mm = m[j];
-            v[4 * j] = mm.x > 0.f ? v[4 * j] : 0.f;
-            v[4 * j + 1] = mm.y > 0.f ? v[4 * j + 1] : 0.f;
-            v[4 * j + 2] = mm.z > 0.f ? v[4 * j + 2] : 0.f;
-            v[4 * j + 3] = mm.w > 0.f ? v[4 * j + 3] : 0.f;
-          }
-        }
-        if (a.P) {       // (never combined with the precise-mode passes: rounded like the stored map would be)
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = tf32_round(v[j]);
-        } else {
-        float4* dst = reinterpret_cast<float4*>(a.Y + pix * a.Cout + co);
-        if (a.no_round) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) dst[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            dst[j] = make_float4(tf32_round(v[4 * j]), tf32_round(v[4 * j + 1]), tf32_round(v[4 * j + 2]),
-                                 tf32_round(v[4 * j + 3]));
-        }
-        }
-      }
-      // the window reduction is a warp-wide shuffle: every lane takes part, whether or not its own pixel is valid
-      if (a.P && co < a.Cout) epi_pool_store(a, v, a.TW, w, h, n, co, valid);
+      for (int ks = 0; ks < 4; ++ks) wgmma_tf32(acc, a_base + ks * 2, b_base + ks * 2, (kb | ks) != 0);
+      wgmma_commit();
+      wgmma_wait<1>();          // k-block kb stays in flight; the stage of kb - 1 is free
+      wgmma_keep(acc);
+      if (kb > 0 && (ct & 127) == 0) mbar_arrive(&empty[(kb - 1) % Cfg::STAGES]);
     }
+    wgmma_wait<0>();
+    wgmma_keep(acc);
+    conv_epilogue<BN>(a, acc, acc_tile, w0, h0, n0, co0, ct);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, BN);
 }
 
 // pick a pixel tile TW x TH x TN with product `target` that tiles W x H (x N) with as little waste as possible
@@ -271,13 +294,13 @@ static void pick_tile(int W, int H, int N, int target, int* TW, int* TH, int* TN
 }
 
 static int make_act_map(CUtensorMap* tm, const float* X, int N, int H, int W, int C, int TW, int TH, int TN,
-                        bool mn_major = false, int stride = 1) {
+                        int stride = 1) {
   uint64_t dims[4] = {(uint64_t)C, (uint64_t)W, (uint64_t)H, (uint64_t)N};
   uint64_t strides[3] = {(uint64_t)C * 4, (uint64_t)W * C * 4, (uint64_t)H * W * C * 4};
   // strided traversal: the box spans TW*stride elements and TMA keeps every stride-th one
   uint32_t box[4] = {32, (uint32_t)(TW * stride), (uint32_t)(TH * stride), (uint32_t)TN};
   uint32_t estr[4] = {1, (uint32_t)stride, (uint32_t)stride, 1};
-  return make_tmap(tm, X, 4, dims, strides, box, mn_major, stride > 1 ? estr : nullptr);
+  return make_tmap(tm, X, 4, dims, strides, box, stride > 1 ? estr : nullptr);
 }
 
 template <int BN>
@@ -290,69 +313,63 @@ static int launch_conv(const CUtensorMap& tmX, const CUtensorMap& tmW, const Con
     attr_set = true;
   }
   dim3 grid(a.tiles_w * a.tiles_h * a.tiles_n, (a.Cout + BN - 1) / BN);
-  conv3x3_igemm_kernel<BN><<<grid, 192, Cfg::SMEM, stream>>>(tmX, tmW, a);
+  conv3x3_igemm_kernel<BN><<<grid, CONV_THREADS, Cfg::SMEM, stream>>>(tmX, tmW, a);
   HK_LAUNCH_CHECK("conv3x3_igemm_kernel");
   return 0;
 }
 
 // ------------------------------------------------------------------------------------------------
-// implicit-GEMM conv v2 (stride 1, maps with W % 16 == 0 and H % 8 == 0): persistent CTAs, halo reuse, double-buffered TMEM.
+// implicit-GEMM conv v2 (stride 1, maps with W % 16 == 0 and H % 8 == 0): persistent CTAs and halo reuse.
 //   * pixel tile 16 x 8 of one image (M = 128).  For each (cin chunk, kw) ONE TMA load brings the (8+2) x 16 halo patch
 //     (160 rows x 128 B); the three kh taps are the same patch addressed kh*16 rows (2 KB = whole swizzle atoms) further
 //     down, so the input crosses the L2->SM fabric 3x (+25 % halo) instead of 9x.
-//   * RESIDENT (Cin = 64, BN = 64: VGG conv1_2 and its dgrad): all 9x2 weight tiles (147 KB) stay in shared memory for the
-//     life of the CTA; only activations stream.
-//   * the epilogue of tile i (4 warps, TMEM set i&1) overlaps the TMA/MMA of tile i+1.
+//   * RESIDENT (Cin = 64, Cout = 64: VGG conv1_2 and its dgrad): all 9x2 weight tiles (144 KB) stay in shared memory for
+//     the life of the CTA; only activations stream.
+//   * the shared-memory ring runs across tiles, so the producer loads tile i+1 while the MMA warpgroups finish tile i.
 // ------------------------------------------------------------------------------------------------
 template <int BN, bool RESIDENT>
 struct ConvV2Cfg {
   static constexpr int A_BYTES = 160 * 128;                          // 20 KB halo patch
   static constexpr int B_TILE = BN * 128;
   static constexpr int STAGE_BYTES = A_BYTES + (RESIDENT ? 0 : 3 * B_TILE);
-  static constexpr int STAGES = RESIDENT ? 3 : (BN == 64 ? 4 : 3);
+  static constexpr int STAGES = RESIDENT ? 2 : (BN == 64 ? 3 : 2);
   static constexpr int WRES_BYTES = RESIDENT ? 18 * B_TILE : 0;      // 9 taps x 2 chunks
-  static constexpr int EPI_TILE = 4 * 32 * 36 * 4;                   // four epilogue warps x a 32 x 36-float transpose tile
-  static constexpr int SMEM = STAGES * STAGE_BYTES + WRES_BYTES + 1024 + 512 + EPI_TILE;
+  static constexpr int ACC_TILE = 2 * 128 * 33 * 4;
+  static constexpr int SMEM = STAGES * STAGE_BYTES + WRES_BYTES + 1024 + 256 + ACC_TILE;
 };
 
 template <int BN, bool RESIDENT>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(CONV_THREADS, 1)
 conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, ConvArgs a,
                         int n_ntiles, int total_tiles) {
   using Cfg = ConvV2Cfg<BN, RESIDENT>;
+  constexpr int NACC = BN / 2;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* stages = smem;
   uint8_t* wres = smem + Cfg::STAGES * Cfg::STAGE_BYTES;
   uint64_t* full = reinterpret_cast<uint64_t*>(wres + Cfg::WRES_BYTES);
   uint64_t* empty = full + Cfg::STAGES;
-  uint64_t* acc_full = empty + Cfg::STAGES;
-  uint64_t* acc_empty = acc_full + 2;
-  uint64_t* wbar = acc_empty + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wbar + 1);
-  float* epi_tiles = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full) + 512);
+  uint64_t* wbar = empty + Cfg::STAGES;
+  float* acc_tile = reinterpret_cast<float*>(wres + Cfg::WRES_BYTES + 256);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
   const int nchunk = a.Cin / 32;
   const int nkb = nchunk * 3;                       // (chunk, kw) steps per tile
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmW);
-    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], 4); }
+    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
     mbar_init(wbar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_slot, 2 * BN < 32 ? 32 : 2 * BN); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      if (RESIDENT) {   // whole filter bank of this N tile (n_ntiles == 1 by construction): 18 tiles of [BN x 32]
+  if (warp < 4) {
+    regs_dealloc<56>();
+    if (threadIdx.x == 0) {
+      if (RESIDENT) {   // whole filter bank (n_ntiles == 1 by construction): 18 tiles of [BN x 32]
         mbar_expect_tx(wbar, Cfg::WRES_BYTES);
         for (int tap = 0; tap < 9; ++tap)
           for (int ck = 0; ck < 2; ++ck) tma_load_3d(wres + (tap * 2 + ck) * Cfg::B_TILE, &tmW, wbar, ck * 32, 0, tap);
@@ -380,119 +397,46 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
         }
       }
     }
-  } else if (warp == 1) {
-    {   // warp-uniform loop; tcgen05 issue predicated on one elected lane
-      const uint32_t idesc = make_idesc_tf32(128, BN, 0, 0);
-      const uint64_t desc_tmpl = make_sdesc(0, 16, 1024);
-      if (RESIDENT) { mbar_wait(wbar, 0); tc_fence_after(); }
-      int kbg = 0, itl = 0;
-      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++itl) {
-        const int set = itl & 1;
-        mbar_wait(&acc_empty[set], ((itl >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d = tmem_base + set * BN;
-        for (int kb = 0; kb < nkb; ++kb, ++kbg) {
-          const int s = kbg % Cfg::STAGES;
-          const uint32_t ph = (kbg / Cfg::STAGES) & 1;
-          const int ck = kb / 3, kw = kb - ck * 3;
-          mbar_wait(&full[s], ph);
-          tc_fence_after();
-          // descriptors = constant template + (address >> 4); per-MMA work is one 64-bit add per operand
-          const uint32_t a_addr = smem_u32(stages + s * Cfg::STAGE_BYTES);
-          const uint64_t a_base = desc_tmpl + (a_addr >> 4);
-          uint64_t b_base[3];
-#pragma unroll
-          for (int kh = 0; kh < 3; ++kh) {
-            const uint32_t b_addr = RESIDENT ? smem_u32(wres + ((kh * 3 + kw) * 2 + ck) * Cfg::B_TILE)
-                                             : a_addr + Cfg::A_BYTES + kh * Cfg::B_TILE;
-            b_base[kh] = desc_tmpl + (b_addr >> 4);
-          }
-          if (elect_one()) {
-#pragma unroll
-            for (int kh = 0; kh < 3; ++kh)
-#pragma unroll
-              for (int ks = 0; ks < 4; ++ks)
-                umma_tf32_ss(d, a_base + (kh * 128 + ks * 2), b_base[kh] + ks * 2, idesc, (kb | kh | ks) ? 1u : 0u);
-            umma_commit(&empty[s]);
-          }
-          __syncwarp();
-        }
-        if (elect_one()) umma_commit(&acc_full[set]);
-        __syncwarp();
-      }
-    }
   } else {
-    const int q = warp & 3;
-    const int r = q * 32 + lane;
-    const int wi = r & 15, hi = r >> 4;
-    int itl = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++itl) {
-      const int nt = t % n_ntiles;
+    regs_alloc<224>();
+    const int ct = threadIdx.x - 128;
+    const int wg = ct >> 7;
+    if (RESIDENT) mbar_wait(wbar, 0);
+    // the first MMA of every tile overwrites the accumulators (scale-d = 0): no register writes inside the wgmma pipeline
+    float acc[NACC];
+#pragma unroll
+    for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+    int kbg = 0;
+    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       int pt = t / n_ntiles;
       const int tw = pt % a.tiles_w; pt /= a.tiles_w;
       const int th = pt % a.tiles_h; pt /= a.tiles_h;
-      const int w = tw * 16 + wi, h = th * 8 + hi, n = pt, co0 = nt * BN;
-      const size_t pix = ((size_t)n * a.H + h) * a.W + w;
-      const int set = itl & 1;
-      mbar_wait(&acc_full[set], (itl >> 1) & 1);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        float v[32];
-        tmem_ld32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + set * BN + c * 32, v);
-        tmem_ld_wait();
-        const int co = co0 + c * 32;
-        if (a.bias) {
+      for (int kb = 0; kb < nkb; ++kb, ++kbg) {
+        const int s = kbg % Cfg::STAGES;
+        const int ck = kb / 3, kw = kb - ck * 3;
+        mbar_wait(&full[s], (kbg / Cfg::STAGES) & 1);
+        // rows 64 wg.. of the tile in the patch of tap kh: + (64 wg + 16 kh) rows of 128 B
+        const uint32_t a_addr = smem_u32(stages + s * Cfg::STAGE_BYTES) + wg * 64 * 128;
+        wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += __ldg(a.bias + co + j);
+        for (int kh = 0; kh < 3; ++kh) {
+          const uint32_t b_addr = RESIDENT ? smem_u32(wres + ((kh * 3 + kw) * 2 + ck) * Cfg::B_TILE)
+                                           : smem_u32(stages + s * Cfg::STAGE_BYTES + Cfg::A_BYTES + kh * Cfg::B_TILE);
+          const uint64_t ad = make_sdesc(a_addr + kh * 16 * 128), bd = make_sdesc(b_addr);
+#pragma unroll
+          for (int ks = 0; ks < 4; ++ks) wgmma_tf32(acc, ad + ks * 2, bd + ks * 2, (kb | kh | ks) != 0);
         }
-        if (a.relu) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-        }
-        if (a.mask) {
-          const float4* m = reinterpret_cast<const float4*>(a.mask + pix * a.Cout + co);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 mm = __ldg(m + j);
-            v[4 * j] = mm.x > 0.f ? v[4 * j] : 0.f;
-            v[4 * j + 1] = mm.y > 0.f ? v[4 * j + 1] : 0.f;
-            v[4 * j + 2] = mm.z > 0.f ? v[4 * j + 2] : 0.f;
-            v[4 * j + 3] = mm.w > 0.f ? v[4 * j + 3] : 0.f;
-          }
-        }
-        if (a.P) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = tf32_round(v[j]);
-          epi_pool_store(a, v, 16, w, h, n, co, true);
-        } else {
-          // thread = pixel owning 32 consecutive channels: a direct float4 store instruction would touch 32 pixels x 16 B
-          // (half-written sectors).  Transposed through a warp-private tile, every store instruction writes the full 128 B
-          // of four pixels.
-          float* tile = epi_tiles + q * (32 * 36);
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            *reinterpret_cast<float4*>(tile + lane * 36 + 4 * j) =
-                make_float4(tf32_round(v[4 * j]), tf32_round(v[4 * j + 1]), tf32_round(v[4 * j + 2]), tf32_round(v[4 * j + 3]));
-          __syncwarp();
-#pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            const int rr = it * 4 + (lane >> 3);                      // pixel (lane) rr of this warp: wi = rr & 15, hi = 2 q + (rr >> 4)
-            const size_t pr = ((size_t)n * a.H + (th * 8 + q * 2 + (rr >> 4))) * a.W + tw * 16 + (rr & 15);
-            *reinterpret_cast<float4*>(a.Y + pr * a.Cout + co + (lane & 7) * 4) =
-                *reinterpret_cast<const float4*>(tile + rr * 36 + (lane & 7) * 4);
-          }
-          __syncwarp();
-        }
+        wgmma_commit();
+        wgmma_wait<1>();          // (chunk, kw) step kb stays in flight; the stage of the previous step is free
+        wgmma_keep(acc);
+        if (kb > 0 && (ct & 127) == 0) mbar_arrive(&empty[(kbg - 1) % Cfg::STAGES]);
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[set]);
+      wgmma_wait<0>();
+      wgmma_keep(acc);
+      if ((ct & 127) == 0) mbar_arrive(&empty[(kbg - 1) % Cfg::STAGES]);
+      conv_epilogue<BN>(a, acc, acc_tile, tw * 16, th * 8, pt, (t % n_ntiles) * BN, ct);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 2 * BN < 32 ? 32 : 2 * BN);
 }
 
 template <int BN, bool RESIDENT>
@@ -524,28 +468,28 @@ static int launch_conv_v2(const float* x, const float* wp, ConvArgs a, int N, in
     uint32_t box[3] = {32, (uint32_t)BN, 1};
     if ((r = make_tmap(&tmW, wp, 3, dims, strides, box))) return r;
   }
-  int sms = 148;
-  {
+  static int sms = 0;
+  if (!sms) {
     int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        sms <= 0)
+      sms = 132;
   }
   const int grid = total < sms ? (int)total : sms;
-  conv3x3_igemm_v2_kernel<BN, RESIDENT><<<grid, 192, Cfg::SMEM, stream>>>(tmX, tmW, a, n_ntiles, (int)total);
+  conv3x3_igemm_v2_kernel<BN, RESIDENT><<<grid, CONV_THREADS, Cfg::SMEM, stream>>>(tmX, tmW, a, n_ntiles, (int)total);
   HK_LAUNCH_CHECK("conv3x3_igemm_v2_kernel");
   return 0;
 }
 
 static int conv3x3_igemm_1x(const float* x, const float* wp, const float* bias, const float* mask, const float* addend,
                             float* y, int N, int H, int W, int Cin, int Cout, int relu, cudaStream_t stream, int stride,
-                            bool generic_only, int no_round, float* pooled = nullptr, unsigned char* code = nullptr,
+                            int no_round, float* pooled = nullptr, unsigned char* code = nullptr,
                             int pool_nchw = 0);
 
 // x NHWC [N,H,W,Cin], wp packed [9][Cout][Cin] -> y NHWC [N,H,W,Cout]
 int conv3x3_igemm(const float* x, const float* wp, const float* bias, const float* mask, float* y, int N, int H, int W,
                   int Cin, int Cout, int relu, cudaStream_t stream, int stride = 1) {
-  if (!precise()) return conv3x3_igemm_1x(x, wp, bias, mask, nullptr, y, N, H, W, Cin, Cout, relu, stream, stride, false, 0);
+  if (!precise()) return conv3x3_igemm_1x(x, wp, bias, mask, nullptr, y, N, H, W, Cin, Cout, relu, stream, stride, 0);
   // 3xTF32: y = epi(Xh*Wh + Xl*Wh + Xh*Wl), three passes of the same implicit-GEMM kernel chained through `addend`
   HK_REQUIRE(x && wp && y, HK_ERR_ARG, "conv3x3: null pointer");
   const size_t nx = (size_t)N * H * W * Cin, nw = (size_t)9 * Cout * Cin;
@@ -555,14 +499,14 @@ int conv3x3_igemm(const float* x, const float* wp, const float* bias, const floa
   int r;
   if ((r = tf32_split(x, xh, xl, nx, stream))) return r;
   if ((r = tf32_split(wp, wh, wl, nw, stream))) return r;
-  if ((r = conv3x3_igemm_1x(xh, wl, nullptr, nullptr, nullptr, y, N, H, W, Cin, Cout, 0, stream, stride, true, 1))) return r;
-  if ((r = conv3x3_igemm_1x(xl, wh, nullptr, nullptr, y, y, N, H, W, Cin, Cout, 0, stream, stride, true, 1))) return r;
-  return conv3x3_igemm_1x(xh, wh, bias, mask, y, y, N, H, W, Cin, Cout, relu, stream, stride, true, 1);
+  if ((r = conv3x3_igemm_1x(xh, wl, nullptr, nullptr, nullptr, y, N, H, W, Cin, Cout, 0, stream, stride, 1))) return r;
+  if ((r = conv3x3_igemm_1x(xl, wh, nullptr, nullptr, y, y, N, H, W, Cin, Cout, 0, stream, stride, 1))) return r;
+  return conv3x3_igemm_1x(xh, wh, bias, mask, y, y, N, H, W, Cin, Cout, relu, stream, stride, 1);
 }
 
 static int conv3x3_igemm_1x(const float* x, const float* wp, const float* bias, const float* mask, const float* addend,
                             float* y, int N, int H, int W, int Cin, int Cout, int relu, cudaStream_t stream, int stride,
-                            bool generic_only, int no_round, float* pooled, unsigned char* code, int pool_nchw) {
+                            int no_round, float* pooled, unsigned char* code, int pool_nchw) {
   // H, W are the INPUT dims; output is H/stride x W/stride (padding 1)
   const int Hin = H, Win = W;
   if (stride == 2) {
@@ -582,14 +526,12 @@ static int conv3x3_igemm_1x(const float* x, const float* wp, const float* bias, 
   a.Y = y; a.bias = bias; a.mask = mask; a.N = N; a.H = H; a.W = W; a.Cin = Cin; a.Cout = Cout; a.relu = relu;
   a.stride = stride;
   a.addend = addend; a.no_round = no_round;
-  if (!generic_only) {
-    static int use_v2 = -1;
-    if (use_v2 < 0) { const char* v = getenv("HK_CONV_V2"); use_v2 = v ? atoi(v) : 1; }
-    if (use_v2 && stride == 1 && W % 16 == 0 && H % 8 == 0) {
-      if (Cin == 64 && Cout == 64) return launch_conv_v2<64, true>(x, wp, a, N, H, W, stream);
-      if (Cout <= 64) return launch_conv_v2<64, false>(x, wp, a, N, H, W, stream);
-      return launch_conv_v2<128, false>(x, wp, a, N, H, W, stream);
-    }
+  // the three chained 3xTF32 passes (no_round) keep the generic kernel, whose accumulation order does not depend on the
+  // map size; the single-pass layers take the halo-reuse kernel wherever its 16 x 8 pixel tile divides the map
+  if (!no_round && stride == 1 && W % 16 == 0 && H % 8 == 0) {
+    if (Cin == 64 && Cout == 64) return launch_conv_v2<64, true>(x, wp, a, N, H, W, stream);
+    if (Cout <= 64) return launch_conv_v2<64, false>(x, wp, a, N, H, W, stream);
+    return launch_conv_v2<128, false>(x, wp, a, N, H, W, stream);
   }
   pick_tile(W, H, N, 128, &a.TW, &a.TH, &a.TN);
   HK_REQUIRE(!pooled || (a.TW >= 2 && a.TH >= 2), HK_ERR_UNSUPPORTED, "conv3x3 + pool: pixel tile %dx%d", a.TW, a.TH);
@@ -597,8 +539,8 @@ static int conv3x3_igemm_1x(const float* x, const float* wp, const float* bias, 
   HK_REQUIRE((long long)a.tiles_w * a.tiles_h * a.tiles_n < (1ll << 31), HK_ERR_UNSUPPORTED, "conv3x3: grid too large");
   CUtensorMap tmX, tmW;
   int r;
-  if ((r = make_act_map(&tmX, x, N, Hin, Win, Cin, a.TW, a.TH, a.TN, false, stride))) return r;
-  const int BN = Cout <= 64 ? 64 : (Cout <= 128 ? 128 : 256);
+  if ((r = make_act_map(&tmX, x, N, Hin, Win, Cin, a.TW, a.TH, a.TN, stride))) return r;
+  const int BN = Cout <= 64 ? 64 : 128;   // 64 accumulator registers per thread at most
   {
     uint64_t dims[3] = {(uint64_t)Cin, (uint64_t)Cout, 9};
     uint64_t strides[2] = {(uint64_t)Cin * 4, (uint64_t)Cin * Cout * 4};
@@ -606,19 +548,18 @@ static int conv3x3_igemm_1x(const float* x, const float* wp, const float* bias, 
     if ((r = make_tmap(&tmW, wp, 3, dims, strides, box))) return r;
   }
   if (BN == 64) return launch_conv<64>(tmX, tmW, a, stream);
-  if (BN == 128) return launch_conv<128>(tmX, tmW, a, stream);
-  return launch_conv<256>(tmX, tmW, a, stream);
+  return launch_conv<128>(tmX, tmW, a, stream);
 }
 
 // ------------------------------------------------------------------------------------------------
-// weight gradient: one CTA accumulates dWp[tap][co0:co0+128][ci0:ci0+32] for ALL 9 taps over its share of the
-// pixels (split-K across CTAs, fp32 atomics at the end).
-//   A = dY tile (M = 128 co, MN-major, k = 64 pixels)  — loaded once per pixel tile and reused by the 9 taps;
-//   B = X halo patch, one TMA load per kw shift: (TH+2) x TW pixels x 32 ci; the three kh taps are the SAME
-//       shared-memory patch addressed kh*TW rows further down (a whole number of 512 B swizzle atoms), so the
-//       input is fetched 3x (+halo) instead of 9x;
-//   D = 9 accumulators of 128 x 32 fp32 in TMEM (288 columns) + one 128 x 16 accumulator against an all-ones
-//       B tile, whose every column is sum_pix dY[pix,co] = the bias gradient (no separate pass over dY).
+// weight gradient: one CTA accumulates dWp[tap][co0:co0+64][ci0:ci0+32] for ALL 9 taps over its share of the pixels
+// (split-K across CTAs, fp32 atomics at the end).  Per stage (64 pixels of the tile):
+//   A = dY tile (M = 64 co, k = 64 pixels), TMA-loaded pixel-major and transposed to K-major by the producer warpgroup,
+//       which also sums it over the pixels for the bias gradient (no separate pass over dY);
+//   B = X halo patch, one TMA load per kw shift: (TH+2) x TW pixels x 32 ci, transposed to [32 ci][patch pixels].  The
+//       three kh taps read the SAME patch kh*TW pixels further along k (TW a multiple of 8: whole wgmma k-steps), so
+//       the input is fetched 3x (+halo) instead of 9x.
+//   Warpgroups 1 and 2 accumulate all nine taps for ci 0-15 and 16-31 of the tile (64 x 16 fp32 each, in registers).
 // ------------------------------------------------------------------------------------------------
 struct WgradArgs {
   float* dWp;  // [9][Cout][Cin], pre-zeroed
@@ -626,329 +567,156 @@ struct WgradArgs {
   int N, H, W, Cin, Cout;
   int TW, TH, TN, tiles_w, tiles_h, tiles_n;
   int ksplit;
-  int dbg;
 };
 
-constexpr int WG_KP = 64;                       // pixels per stage
-constexpr int WG_STAGES = 3;
-constexpr int WG_A_BYTES = 4 * WG_KP * 128;     // 4 co-blocks of [64 px x 128 B]            = 32 KB
-constexpr int WG_B_ONE = 96 * 128;              // one kw patch: (TH+2)*TW*TN = 96 rows      = 12 KB
-constexpr int WG_B_BYTES = 3 * WG_B_ONE;
-constexpr int WG_STAGE_BYTES = WG_A_BYTES + WG_B_BYTES;   // 68 KB
-constexpr int WG_ONES_BYTES = 8 * 128;          // all-ones B tile: 8 k-rows x 128 B (reused for every k-step)
-constexpr int WG_BIAS_COL = 448;                 // TMEM column of the 128 x 16 bias-gradient accumulator (taps use 0..287)
-constexpr int WG_SMEM = WG_STAGES * WG_STAGE_BYTES + WG_ONES_BYTES + 1024 + 256;
+constexpr int WG_THREADS = 384;
+constexpr int WG_STAGES = 2;
+constexpr int WG_KP = 64;                        // pixels per stage
+constexpr int WG_PATCH = 96 * 128;               // one kw patch: (TH+2)*TW*TN <= 96 pixel rows x 128 B
+constexpr int WG_RAW_A = 2 * WG_KP * 128;        // dY: 2 co-boxes of [64 px x 32 co]
+constexpr int WG_RAW_BYTES = WG_RAW_A + 3 * WG_PATCH;
+constexpr int WG_A_BYTES = 2 * 64 * 128;         // A: 2 k-chunks of [64 co x 32 px]
+constexpr int WG_B_ONE = 3 * 32 * 128;           // B of one kw: 3 k-chunks of [32 ci x 32 px]
+constexpr int WG_STAGE_BYTES = WG_A_BYTES + 3 * WG_B_ONE;
+constexpr int WG_SMEM = WG_RAW_BYTES + WG_STAGES * WG_STAGE_BYTES + 1024 + 256;
 
-__global__ void __launch_bounds__(192, 1)
+// one stage of the nine tap products for ci rows [16 wg, 16 wg + 16) of the tile: acc[tap] is 64 co x 16 ci
+__device__ __forceinline__ void wgrad_mma(float (&acc)[9][8], const uint8_t* sa, const uint8_t* sb, int wg, int TW,
+                                          int img_rows) {
+  const uint32_t a_addr = smem_u32(sa), b_addr = smem_u32(sb) + wg * 16 * 128;
+  wgmma_fence();
+#pragma unroll 1   // rolled: 72 descriptors per k-step instead of 576 live at once
+  for (int ks = 0; ks < 8; ++ks) {
+    const uint64_t ad = make_sdesc(a_addr + (ks >> 2) * (64 * 128)) + (ks & 3) * 2;
+    const int kb = ks * 8 + ((ks * 8) / img_rows) * 2 * TW;    // k of this step in the patch of image n: + 2 TW per image
+#pragma unroll
+    for (int tap = 0; tap < 9; ++tap) {
+      const int kh = tap / 3, kw = tap % 3;
+      const int kk = kb + kh * TW;
+      // rows 16 wg.. of the [32 ci] chunk: two whole 8-row swizzle groups further on
+      const uint64_t bd = make_sdesc(b_addr + kw * WG_B_ONE + (kk >> 5) * (32 * 128)) + ((kk & 31) >> 3) * 2;
+      wgmma_tf32(acc[tap], ad, bd, 1);
+    }
+  }
+  wgmma_commit();
+}
+
+__device__ __forceinline__ void wgrad_store(const float (&acc)[9][8], const WgradArgs& a, int co0, int ci0, int t) {
+  const int wl = t >> 5, lane = t & 31;
+#pragma unroll
+  for (int tap = 0; tap < 9; ++tap)
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int co = co0 + wl * 16 + (lane >> 2) + 8 * ((e >> 1) & 1);
+      const int ci = ci0 + 8 * (e >> 2) + 2 * (lane & 3) + (e & 1);
+      if (co < a.Cout) atomicAdd(a.dWp + ((size_t)tap * a.Cout + co) * a.Cin + ci, acc[tap][e]);
+    }
+}
+
+__global__ void __launch_bounds__(WG_THREADS, 1)
 conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX, WgradArgs a) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + WG_STAGES * WG_A_BYTES;
-  float* ones = reinterpret_cast<float*>(smem + WG_STAGES * WG_STAGE_BYTES);
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + WG_STAGES * WG_STAGE_BYTES + WG_ONES_BYTES);
+  uint8_t* raw = smem;
+  uint8_t* stages = smem + WG_RAW_BYTES;
+  uint64_t* full = reinterpret_cast<uint64_t*>(stages + WG_STAGES * WG_STAGE_BYTES);
   uint64_t* empty = full + WG_STAGES;
-  uint64_t* accf = empty + WG_STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accf + 1);
+  uint64_t* raw_bar = empty + WG_STAGES;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
   const int n_ci_tiles = a.Cin / 32;
   const int ci_t = blockIdx.x % n_ci_tiles, co_t = blockIdx.x / n_ci_tiles;
   const int split = blockIdx.y;
-  const int co0 = co_t * 128, ci0 = ci_t * 32;
+  const int co0 = co_t * 64, ci0 = ci_t * 32;
   const bool do_bias = (a.db != nullptr) && (ci_t == 0);
   const long long total_tiles = (long long)a.tiles_w * a.tiles_h * a.tiles_n;
   const long long per = (total_tiles + a.ksplit - 1) / a.ksplit;
   const long long t_begin = per * split;
   const long long t_end = (t_begin + per < total_tiles) ? t_begin + per : total_tiles;
   const int nk = (int)(t_end > t_begin ? t_end - t_begin : 0);
-  const int img_rows = a.TH * a.TW;                 // A rows per image in the tile
-  const int patch_rows = (a.TH + 2) * a.TW;         // B rows per image in the patch
-  const int ksteps_img = img_rows / 8;
+  const int img_rows = a.TH * a.TW;                 // A pixels per image in the tile
+  const int patch_rows = (a.TH + 2) * a.TW * a.TN;  // B pixels of one kw patch
+  const int patch_chunks = (patch_rows + 31) / 32;
 
-  for (int i = threadIdx.x; i < WG_ONES_BYTES / 4; i += blockDim.x) ones[i] = 1.f;
-  fence_proxy_async();   // generic-proxy smem writes -> visible to the tensor core (async proxy)
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmDY);
     tma_prefetch_desc(&tmX);
-    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(accf, 1);
+    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
+    mbar_init(raw_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (nk == 0) return;
 
-  if (nk > 0) {
-    if (warp == 0) {
-      if (lane == 0) {
-        for (int kb = 0; kb < nk; ++kb) {
-          const int s = kb % WG_STAGES;
-          const uint32_t ph = (kb / WG_STAGES) & 1;
-          int tt = (int)t_begin + kb;
-          const int tw = tt % a.tiles_w; tt /= a.tiles_w;
-          const int th = tt % a.tiles_h; tt /= a.tiles_h;
-          const int w0 = tw * a.TW, h0 = th * a.TH, n0 = tt * a.TN;
-          mbar_wait(&empty[s], ph ^ 1);
-          mbar_expect_tx(&full[s], WG_A_BYTES + 3 * patch_rows * a.TN * 128);
-          uint8_t* pa = sA + s * WG_A_BYTES;
-          uint8_t* pb = sB + s * WG_B_BYTES;
+  if (warp < 4) {
+    regs_dealloc<56>();
+    const int t = threadIdx.x;
+    float bsum = 0.f;                               // bias gradient of co0 + (t & 63), pixel half t >> 6
+    for (int kb = 0; kb < nk; ++kb) {
+      const int s = kb % WG_STAGES;
+      const uint32_t ph = (kb / WG_STAGES) & 1;
+      if (t == 0) {
+        int tt = (int)t_begin + kb;
+        const int tw = tt % a.tiles_w; tt /= a.tiles_w;
+        const int th = tt % a.tiles_h; tt /= a.tiles_h;
+        const int w0 = tw * a.TW, h0 = th * a.TH, n0 = tt * a.TN;
+        mbar_wait(&empty[s], ph ^ 1);
+        mbar_expect_tx(raw_bar, WG_RAW_A + 3 * patch_rows * 128);
 #pragma unroll
-          for (int j = 0; j < 4; ++j) tma_load_4d(pa + j * WG_KP * 128, &tmDY, &full[s], co0 + j * 32, w0, h0, n0);
+        for (int j = 0; j < 2; ++j) tma_load_4d(raw + j * WG_KP * 128, &tmDY, raw_bar, co0 + j * 32, w0, h0, n0);
 #pragma unroll
-          for (int kw = 0; kw < 3; ++kw) tma_load_4d(pb + kw * WG_B_ONE, &tmX, &full[s], ci0, w0 + kw - 1, h0 - 1, n0);
-        }
+        for (int kw = 0; kw < 3; ++kw) tma_load_4d(raw + WG_RAW_A + kw * WG_PATCH, &tmX, raw_bar, ci0, w0 + kw - 1, h0 - 1, n0);
       }
-    } else if (warp == 1) {
-      {
-        const uint32_t idesc = make_idesc_tf32(128, 96, 1, 1);
-        const uint32_t idesc_b = make_idesc_tf32(128, 16, 1, 1);
-        const uint64_t ones_desc = make_sdesc_mn(smem_u32(ones), 0);
-        // The issuing thread is the bottleneck of this kernel (3 N=96 MMAs of 48 cycles per k-step).  The loop runs
-        // warp-uniformly (all 32 lanes) so the descriptor arithmetic is done on the uniform datapath; per-k-step offsets
-        // (16-byte units) are computed once; only the tcgen05 issue is predicated on one elected lane.
-        uint32_t a_off[8], b_off[8];
-        {
-          int ks = 0;
-          for (int n = 0; n < a.TN; ++n)
-            for (int j = 0; j < ksteps_img; ++j, ++ks) {
-              a_off[ks] = (uint32_t)((n * img_rows + j * 8) * 128) >> 4;
-              b_off[ks] = (uint32_t)((n * patch_rows + j * 8) * 128) >> 4;
-            }
-        }
-        const uint32_t kh_step = (uint32_t)(a.TW * 128) >> 4;
-        const uint64_t a_tmpl = make_sdesc_mn(0, WG_KP * 128);
-        const uint64_t b_tmpl = make_sdesc_mn(0, WG_B_ONE);
-        for (int kb = 0; kb < nk; ++kb) {
-          const int s = kb % WG_STAGES;
-          const uint32_t ph = (kb / WG_STAGES) & 1;
-          mbar_wait(&full[s], ph);
-          tc_fence_after();
-          const uint64_t a_base = a_tmpl + (smem_u32(sA + s * WG_A_BYTES) >> 4);
-          const uint64_t b_base = b_tmpl + (smem_u32(sB + s * WG_B_BYTES) >> 4);
-          if (elect_one()) {
+      mbar_wait(raw_bar, kb & 1);
+      uint8_t* st = stages + s * WG_STAGE_BYTES;
+      // A: chunk kc = pixels 32 kc .. 32 kc + 31 of both co boxes
 #pragma unroll
-            for (int ks = 0; ks < 8; ++ks) {
-              const uint32_t accum = (kb | ks) ? 1u : 0u;
-              const uint64_t ad = a_base + a_off[ks];
-              const uint64_t bd = b_base + b_off[ks];
-              umma_tf32_ss(tmem_base, ad, bd, idesc, accum);
-              umma_tf32_ss(tmem_base + 96, ad, bd + kh_step, idesc, accum);
-              umma_tf32_ss(tmem_base + 192, ad, bd + 2 * kh_step, idesc, accum);
-              if (do_bias) umma_tf32_ss(tmem_base + WG_BIAS_COL, ad, ones_desc, idesc_b, accum);
-            }
-            umma_commit(&empty[s]);
-          }
-          __syncwarp();
-        }
-        if (elect_one()) umma_commit(accf);
-        __syncwarp();
-      }
-    } else {
-      const int q = warp & 3;
-      const int co = co0 + q * 32 + lane;
-      mbar_wait(accf, 0);
-      tc_fence_after();
-#pragma unroll 1
-      for (int tap = 0; tap < 9; ++tap) {
-        float v[32];
-        tmem_ld32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + tap * 32, v);
-        tmem_ld_wait();
-        if (co < a.Cout) {
-          float* dst = a.dWp + ((size_t)tap * a.Cout + co) * a.Cin + ci0;
-#pragma unroll
-          for (int j = 0; j < 32; ++j) atomicAdd(dst + j, v[j]);
-        }
-      }
+      for (int kc = 0; kc < 2; ++kc) transpose_mn_tile(raw + kc * 4096, st + kc * (64 * 128), 64, t, 128, WG_KP * 128);
+      for (int kw = 0; kw < 3; ++kw)
+        for (int kc = 0; kc < patch_chunks; ++kc)
+          transpose_mn_tile(raw + WG_RAW_A + kw * WG_PATCH + kc * 4096, st + WG_A_BYTES + kw * WG_B_ONE + kc * 4096, 32, t, 128);
       if (do_bias) {
-        float v[32];
-        tmem_ld32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + WG_BIAS_COL, v);
-        tmem_ld_wait();
-        if (co < a.Cout) atomicAdd(a.db + co, v[0]);
+        const int co = t & 63, p0 = (t >> 6) * 32;
+        const uint8_t* box = raw + (co >> 5) * (WG_KP * 128);
+#pragma unroll 8
+        for (int p = p0; p < p0 + 32; ++p) bsum += *reinterpret_cast<const float*>(box + sw128_off(p, co & 31));
       }
+      fence_proxy_async();
+      named_bar(1, 128);
+      if (t == 0) mbar_arrive(&full[s]);
     }
+    if (do_bias && co0 + (t & 63) < a.Cout) atomicAdd(a.db + co0 + (t & 63), bsum);
+  } else {
+    regs_alloc<224>();
+    const int ct = threadIdx.x - 128;
+    const int wg = ct >> 7, t = ct & 127;
+    float acc[9][8];
+#pragma unroll
+    for (int j = 0; j < 9; ++j)
+#pragma unroll
+      for (int e = 0; e < 8; ++e) acc[j][e] = 0.f;
+    for (int kb = 0; kb < nk; ++kb) {
+      const int s = kb % WG_STAGES;
+      mbar_wait(&full[s], (kb / WG_STAGES) & 1);
+      const uint8_t* st = stages + s * WG_STAGE_BYTES;
+      wgrad_mma(acc, st, st + WG_A_BYTES, wg, a.TW, img_rows);
+      wgmma_wait<1>();          // stage kb stays in flight; the stage of kb - 1 is free
+#pragma unroll
+      for (int j = 0; j < 9; ++j) wgmma_keep(acc[j]);
+      if (kb > 0 && t == 0) mbar_arrive(&empty[(kb - 1) % WG_STAGES]);
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int j = 0; j < 9; ++j) wgmma_keep(acc[j]);
+    wgrad_store(acc, a, co0, ci0 + 16 * wg, t);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 512);
 }
 
-// ------------------------------------------------------------------------------------------------
-// wgrad, version 2: the dY tile (A operand, 128 co x 64 pixels) is reused by all nine taps, yet in the SS form every one of
-// the 3 (+1 bias) MMAs of a k-step re-reads it from shared memory: (4 KB A + 3 KB B) per 48-cycle N=96 MMA = 146 B/clk
-// against a 128 B/clk shared-memory port — the kernel was shared-memory-bound, not tensor-bound.  Here the four otherwise
-// idle epilogue warps transpose each dY tile ONCE from shared memory into tensor memory (thread = co, 64 pixel columns,
-// tcgen05.st) and the MMAs take A from TMEM (tcgen05.mma [tmem], b-desc): shared-memory traffic per k-step drops from 21 KB
-// to 9 KB + a 4 KB one-off read.  dY is TMA-loaded with the plain 128B swizzle (it is no longer a UMMA smem operand).
-// TMEM: tap accumulators 0..287, bias 288..303, A double buffer 320..447.
-// ------------------------------------------------------------------------------------------------
-constexpr int WG2_BIAS_COL = 288;
-constexpr int WG2_A_COL = 320;
-
-__global__ void __launch_bounds__(192, 1)
-conv3x3_wgrad_v2_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX, WgradArgs a) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + WG_STAGES * WG_A_BYTES;
-  float* ones = reinterpret_cast<float*>(smem + WG_STAGES * WG_STAGE_BYTES);
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + WG_STAGES * WG_STAGE_BYTES + WG_ONES_BYTES);
-  uint64_t* empty = full + WG_STAGES;
-  uint64_t* accf = empty + WG_STAGES;
-  uint64_t* a_ready = accf + 1;     // [2] stager warps (4) -> MMA: dY tile kb is in TMEM buffer kb & 1
-  uint64_t* a_free = a_ready + 2;   // [2] MMA (tcgen05.commit) -> stagers: the MMAs reading buffer kb & 1 have retired
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(a_free + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_ci_tiles = a.Cin / 32;
-  const int ci_t = blockIdx.x % n_ci_tiles, co_t = blockIdx.x / n_ci_tiles;
-  const int split = blockIdx.y;
-  const int co0 = co_t * 128, ci0 = ci_t * 32;
-  const bool do_bias = (a.db != nullptr) && (ci_t == 0);
-  const long long total_tiles = (long long)a.tiles_w * a.tiles_h * a.tiles_n;
-  const long long per = (total_tiles + a.ksplit - 1) / a.ksplit;
-  const long long t_begin = per * split;
-  const long long t_end = (t_begin + per < total_tiles) ? t_begin + per : total_tiles;
-  const int nk = (int)(t_end > t_begin ? t_end - t_begin : 0);
-  const int img_rows = a.TH * a.TW;
-  const int patch_rows = (a.TH + 2) * a.TW;
-  const int ksteps_img = img_rows / 8;
-
-  for (int i = threadIdx.x; i < WG_ONES_BYTES / 4; i += blockDim.x) ones[i] = 1.f;
-  fence_proxy_async();
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmDY);
-    tma_prefetch_desc(&tmX);
-    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(accf, 1);
-    for (int i = 0; i < 2; ++i) { mbar_init(&a_ready[i], 4); mbar_init(&a_free[i], 1); }
-    fence_barrier_init();
-  }
-  if (warp == 1) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (nk > 0) {
-    if (warp == 0) {
-      if (lane == 0) {
-        for (int kb = 0; kb < nk; ++kb) {
-          const int s = kb % WG_STAGES;
-          const uint32_t ph = (kb / WG_STAGES) & 1;
-          int tt = (int)t_begin + kb;
-          const int tw = tt % a.tiles_w; tt /= a.tiles_w;
-          const int th = tt % a.tiles_h; tt /= a.tiles_h;
-          const int w0 = tw * a.TW, h0 = th * a.TH, n0 = tt * a.TN;
-          mbar_wait(&empty[s], ph ^ 1);
-          mbar_expect_tx(&full[s], WG_A_BYTES + 3 * patch_rows * a.TN * 128);
-          uint8_t* pa = sA + s * WG_A_BYTES;
-          uint8_t* pb = sB + s * WG_B_BYTES;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) tma_load_4d(pa + j * WG_KP * 128, &tmDY, &full[s], co0 + j * 32, w0, h0, n0);
-#pragma unroll
-          for (int kw = 0; kw < 3; ++kw) tma_load_4d(pb + kw * WG_B_ONE, &tmX, &full[s], ci0, w0 + kw - 1, h0 - 1, n0);
-        }
-      }
-    } else if (warp == 1) {
-      const uint32_t idesc = make_idesc_tf32(128, 96, 0, 1);
-      const uint32_t idesc_b = make_idesc_tf32(128, 16, 0, 1);
-      const uint64_t ones_desc = make_sdesc_mn(smem_u32(ones), 0);
-      uint32_t b_off[8];
-      {
-        int ks = 0;
-        for (int n = 0; n < a.TN; ++n)
-          for (int j = 0; j < ksteps_img; ++j, ++ks) b_off[ks] = (uint32_t)((n * patch_rows + j * 8) * 128) >> 4;
-      }
-      const uint32_t kh_step = (uint32_t)(a.TW * 128) >> 4;
-      const uint64_t b_tmpl = make_sdesc_mn(0, WG_B_ONE);
-      for (int kb = 0; kb < nk; ++kb) {
-        const int s = kb % WG_STAGES;
-        const uint32_t ph = (kb / WG_STAGES) & 1;
-        const int ab = kb & 1;
-        mbar_wait(&full[s], ph);                       // the X patches of this stage have landed
-        mbar_wait(&a_ready[ab], (kb >> 1) & 1);        // ... and its dY tile is in tensor memory
-        tc_fence_after();
-        const uint64_t b_base = b_tmpl + (smem_u32(sB + s * WG_B_BYTES) >> 4);
-        const uint32_t a_tm = tmem_base + WG2_A_COL + ab * WG_KP;
-        if (elect_one()) {
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks) {
-            const uint32_t accum = (kb | ks) ? 1u : 0u;
-            const uint32_t ad = a_tm + ks * 8;
-            const uint64_t bd = b_base + b_off[ks];
-            umma_tf32_ts(tmem_base, ad, bd, idesc, accum);
-            umma_tf32_ts(tmem_base + 96, ad, bd + kh_step, idesc, accum);
-            umma_tf32_ts(tmem_base + 192, ad, bd + 2 * kh_step, idesc, accum);
-            if (do_bias) umma_tf32_ts(tmem_base + WG2_BIAS_COL, ad, ones_desc, idesc_b, accum);
-          }
-          umma_commit(&empty[s]);
-          umma_commit(&a_free[ab]);
-        }
-        __syncwarp();
-      }
-      if (elect_one()) umma_commit(accf);
-      __syncwarp();
-    } else {
-      // ---- stagers (main loop), then epilogue.  warp -> TMEM lane quarter q = co block of 32; thread = one co
-      const int q = warp & 3;
-      for (int kb = 0; kb < nk; ++kb) {
-        const int s = kb % WG_STAGES;
-        const uint32_t ph = (kb / WG_STAGES) & 1;
-        const int ab = kb & 1;
-        mbar_wait(&full[s], ph);
-        // co block q of the tile: 64 pixel rows x 128 B, 128B-swizzled (16-byte chunk ^ (row & 7)); lane = word in the row
-        const uint8_t* tile = sA + s * WG_A_BYTES + q * (WG_KP * 128);
-        float v0[32], v1[32];
-#pragma unroll
-        for (int k = 0; k < 32; ++k)
-          v0[k] = *reinterpret_cast<const float*>(tile + k * 128 + ((((lane >> 2) ^ (k & 7)) << 4) | ((lane & 3) << 2)));
-#pragma unroll
-        for (int k = 0; k < 32; ++k)
-          v1[k] = *reinterpret_cast<const float*>(tile + (32 + k) * 128 + ((((lane >> 2) ^ (k & 7)) << 4) | ((lane & 3) << 2)));
-        if (kb >= 2) { mbar_wait(&a_free[ab], ((kb >> 1) - 1) & 1); tc_fence_after(); }
-        const uint32_t dst = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + WG2_A_COL + ab * WG_KP;
-        tmem_st32(dst, v0);
-        tmem_st32(dst + 32, v1);
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&a_ready[ab]);
-      }
-      const int co = co0 + q * 32 + lane;
-      mbar_wait(accf, 0);
-      tc_fence_after();
-#pragma unroll 1
-      for (int tap = 0; tap < 9; ++tap) {
-        float v[32];
-        tmem_ld32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + tap * 32, v);
-        tmem_ld_wait();
-        if (co < a.Cout) {
-          float* dst = a.dWp + ((size_t)tap * a.Cout + co) * a.Cin + ci0;
-#pragma unroll
-          for (int j = 0; j < 32; ++j) atomicAdd(dst + j, v[j]);
-        }
-      }
-      if (do_bias) {
-        float v[32];
-        tmem_ld32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + WG2_BIAS_COL, v);
-        tmem_ld_wait();
-        if (co < a.Cout) atomicAdd(a.db + co, v[0]);
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 512);
-}
-
-// pixel tile for wgrad: TW in {4,8,16} (kh shifts must be whole 512 B swizzle atoms), TW*TH*TN = 64, TH*TW % 8 == 0
+// pixel tile for wgrad: TW in {8,16} (kh shifts must be whole wgmma k-steps of 8 pixels), TW*TH*TN = 64, TH*TW % 8 == 0
 static bool pick_wgrad_tile(int W, int H, int* TW, int* TH, int* TN) {
   int tw = 0;
-  for (int c : {16, 8, 4}) if (W % c == 0) { tw = c; break; }
-  if (!tw) tw = W <= 4 ? 4 : (W <= 8 ? 8 : 16);   // over-wide tile: out-of-range columns are TMA zero fill
+  for (int c : {16, 8}) if (W % c == 0) { tw = c; break; }
+  if (!tw) tw = W <= 8 ? 8 : 16;   // over-wide tile: out-of-range columns are TMA zero fill
   int th = 1;
   while (th * 2 * tw <= 64 && H % (th * 2) == 0) th *= 2;
   int tn = 64 / (tw * th);
@@ -987,23 +755,20 @@ static int conv3x3_wgrad_1x(const float* x, const float* dy, float* dwp, float* 
   WgradArgs a = {};
   a.dWp = dwp; a.db = db; a.N = N; a.H = H; a.W = W; a.Cin = Cin; a.Cout = Cout;
   pick_wgrad_tile(W, H, &a.TW, &a.TH, &a.TN);
-  HK_REQUIRE((a.TH + 2) * a.TW * a.TN * 128 <= WG_B_ONE, HK_ERR_UNSUPPORTED, "conv3x3_wgrad: halo patch too large");
+  HK_REQUIRE((a.TH + 2) * a.TW * a.TN * 128 <= WG_PATCH, HK_ERR_UNSUPPORTED, "conv3x3_wgrad: halo patch too large");
   a.tiles_w = (W + a.TW - 1) / a.TW; a.tiles_h = (H + a.TH - 1) / a.TH; a.tiles_n = (N + a.TN - 1) / a.TN;
-  const long long out_tiles = (long long)((Cout + 127) / 128) * (Cin / 32);
+  const long long out_tiles = (long long)((Cout + 63) / 64) * (Cin / 32);
   const long long total_tiles = (long long)a.tiles_w * a.tiles_h * a.tiles_n;
-  // split-K factor.  The kernel runs one CTA per SM (204 KB of shared memory), so the grid executes in whole waves of
+  // split-K factor.  The kernel runs one CTA per SM (157 KB of shared memory), so the grid executes in whole waves of
   // `sms` CTAs: pick the split that fills 1..3 waves best (ties -> fewer waves: fewer partial sums to add atomically).
-  // Measured in one process on the whole BCNN step: 1178.7 -> 1235.2 img/s against the first rule ("about two CTAs of work
-  // per SM", which left e.g. 304- and 320-CTA grids with a nearly empty third wave); HK_WG_SPLIT=0 restores that rule for A/B runs.
-  static int sms = 0, rule = -1;
+  static int sms = 0;
   if (!sms) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
   }
-  if (rule < 0) { const char* v = getenv("HK_WG_SPLIT"); rule = v ? atoi(v) : 1; }
-  long long ks = (148 * 2 + out_tiles - 1) / out_tiles;
-  if (rule == 1) {
+  long long ks = 1;
+  {
     double best = -1.0;
     for (int w = 1; w <= 3; ++w) {
       long long k = (long long)sms * w / out_tiles;
@@ -1019,13 +784,10 @@ static int conv3x3_wgrad_1x(const float* x, const float* dy, float* dwp, float* 
   if (ks < 1) ks = 1;
   if (ks > 65535) ks = 65535;
   a.ksplit = (int)ks;
-  { const char* v = getenv("HK_DBG_WG"); a.dbg = v ? atoi(v) : 0; }
-  static int use_v2 = -1;
-  if (use_v2 < 0) { const char* v = getenv("HK_WGRAD_V2"); use_v2 = v ? atoi(v) : 1; }
   CUtensorMap tmDY, tmX;
   int r;
-  if ((r = make_act_map(&tmDY, dy, N, H, W, Cout, a.TW, a.TH, a.TN, /*mn_major=*/!use_v2))) return r;
-  if ((r = make_act_map(&tmX, x, N, H, W, Cin, a.TW, a.TH + 2, a.TN, true))) return r;
+  if ((r = make_act_map(&tmDY, dy, N, H, W, Cout, a.TW, a.TH, a.TN))) return r;
+  if ((r = make_act_map(&tmX, x, N, H, W, Cin, a.TW, a.TH + 2, a.TN))) return r;
   cudaError_t e = cudaSuccess;
   if (zero_dw) {
     e = cudaMemsetAsync(dwp, 0, (size_t)9 * Cout * Cin * sizeof(float), stream);
@@ -1038,23 +800,21 @@ static int conv3x3_wgrad_1x(const float* x, const float* dy, float* dwp, float* 
   static bool attr_set = false;
   if (!attr_set) {
     e = cudaFuncSetAttribute(conv3x3_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv3x3_wgrad_v2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM);
     if (e != cudaSuccess) return set_error((int)e, "cudaFuncSetAttribute(wgrad): %s", cudaGetErrorString(e));
     attr_set = true;
   }
   dim3 grid((unsigned)out_tiles, a.ksplit);
-  if (use_v2) conv3x3_wgrad_v2_kernel<<<grid, 192, WG_SMEM, stream>>>(tmDY, tmX, a);
-  else conv3x3_wgrad_kernel<<<grid, 192, WG_SMEM, stream>>>(tmDY, tmX, a);
+  conv3x3_wgrad_kernel<<<grid, WG_THREADS, WG_SMEM, stream>>>(tmDY, tmX, a);
   HK_LAUNCH_CHECK("conv3x3_wgrad_kernel");
   return 0;
 }
 
 // ------------------------------------------------------------------------------------------------
-// first layer (Cin = 3; vgg.py:61 in_channels=3): im2col to X27 + one tcgen05 GEMM (see hk_conv3x3_first_fwd)
+// first layer (Cin = 3; vgg.py:61 in_channels=3): im2col to X27 + one wgmma GEMM (see hk_conv3x3_first_fwd)
 // ------------------------------------------------------------------------------------------------
 // first-layer weight gradient on the tensor cores: materialise the 3x3x3 patches as X27 [pix][32]
 // (27 taps, column 27 = 1.0 so that the GEMM's column 27 is the bias gradient, columns 28..31 = 0) and run
-// dW^T-partials[s] = dY[pix-range s]^T . X27[pix-range s]  as a batched (split-K) MN-major tcgen05 GEMM.
+// dW^T-partials[s] = dY[pix-range s]^T . X27[pix-range s]  as a batched (split-K) MN-major wgmma GEMM.
 __global__ void im2col_first_kernel(const float* __restrict__ x, float* __restrict__ x27, int N, int H, int W, int round) {
   const long long total = (long long)N * H * W;
   for (long long pix = blockIdx.x * (long long)blockDim.x + threadIdx.x; pix < total;
@@ -1248,7 +1008,7 @@ __global__ void relu_mask_kernel(float* __restrict__ dy, const float* __restrict
 
 static inline int grid_for(size_t n, int block) {
   size_t g = (n + block - 1) / block;
-  const size_t cap = 148 * 16;
+  const size_t cap = 132 * 16;
   return (int)(g < cap ? (g ? g : 1) : cap);
 }
 
@@ -1278,7 +1038,7 @@ int hk_conv3x3_fwd_pool(const float* x, const float* w_packed, const float* bias
                         int H, int W, int Cin, int Cout, int out_nchw, void* stream) {
   HK_REQUIRE(!precise(), HK_ERR_UNSUPPORTED, "hk_conv3x3_fwd_pool: not available in 3xTF32 mode (use conv + pool)");
   HK_REQUIRE(pooled, HK_ERR_ARG, "hk_conv3x3_fwd_pool: null output");
-  return conv3x3_igemm_1x(x, w_packed, bias, nullptr, nullptr, nullptr, N, H, W, Cin, Cout, 1, (cudaStream_t)stream, 1, false,
+  return conv3x3_igemm_1x(x, w_packed, bias, nullptr, nullptr, nullptr, N, H, W, Cin, Cout, 1, (cudaStream_t)stream, 1,
                           0, pooled, code, out_nchw);
 }
 
@@ -1319,7 +1079,7 @@ size_t hk_conv3x3_first_fwd_workspace_bytes(int N, int H, int W, int Cout) {
 }
 
 /* y = relu(conv3x3(x) + bias) for the 3-channel input layer: patches are materialised once as X27 [pix][32]
- * (tf32-rounded, column 27 = 1 carries the bias) and the layer is ONE tcgen05 GEMM  y = relu(X27 . W27^T).
+ * (tf32-rounded, column 27 = 1 carries the bias) and the layer is ONE wgmma GEMM  y = relu(X27 . W27^T).
  * workspace = X27 followed by W27; X27 (the first N*H*W*32 floats) is what hk_conv3x3_first_wgrad consumes. */
 int hk_conv3x3_first_fwd(const float* x_nchw, const float* w, const float* bias, float* y_nhwc, int N, int H, int W,
                          int Cout, void* workspace, size_t workspace_bytes, void* stream_) {
@@ -1352,7 +1112,7 @@ size_t hk_conv3x3_first_wgrad_workspace_bytes(int N, int H, int W, int Cout) {
 }
 
 /* dw [Cout,3,3,3], db [Cout] of the input layer from X27 (written by hk_conv3x3_first_fwd) and dy (ReLU-masked):
- * split-K batched MN-major tcgen05 GEMM  partial[s] = dY_s^T . X27_s ; column 27 of the result is the bias grad. */
+ * split-K batched MN-major wgmma GEMM  partial[s] = dY_s^T . X27_s ; column 27 of the result is the bias grad. */
 int hk_conv3x3_first_wgrad_acc(const float* x27, const float* dy_nhwc, float* dw, float* db, int N, int H, int W, int Cout,
                                void* workspace, size_t workspace_bytes, int accumulate, void* stream_);
 int hk_conv3x3_first_wgrad(const float* x27, const float* dy_nhwc, float* dw, float* db, int N, int H, int W,

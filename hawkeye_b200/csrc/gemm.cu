@@ -1,13 +1,16 @@
-// Generic batched TF32 GEMM on tcgen05 (UMMA) with TMA-fed, 128B-swizzled shared-memory
-// operands and the fp32 accumulator in TMEM.  One 128 x BN output tile per CTA.
+// Generic batched TF32 GEMM on wgmma (sm_90a) with TMA-fed, 128B-swizzled shared-memory operands and the fp32
+// accumulator in registers.  One 128 x BN output tile per CTA iteration.
 //
 //   C[b] = alpha_b * (A[b] . B[b]) + diag * I + beta_b * D[b]           (optionally stored transposed)
 //
 // Both operands may be K-major or MN-major in global memory, so the same kernel serves
 //   * Newton-Schulz chains and covariance of Fast MPN-COV (reference model/methods/MPNCOV.py:105-202),
-//   * the (S . X) contraction of the bilinear / compact-bilinear backward (BCNN.py:13-27, CBCNN.py:96-135),
+//   * the Gram and (S . X) contractions of the bilinear / compact-bilinear pooling (BCNN.py:13-27, CBCNN.py:96-135),
 //   * 1x1 convolutions in NHWC (model/backbone/resnet.py:29-37).
-// Warp roles: warp 0 = TMA producer, warp 1 = MMA issuer (+TMEM alloc), warps 2-5 = epilogue.
+// tf32 wgmma reads K-major operands only: an MN-major operand is TMA-loaded into a staging buffer and transposed into
+// the K-major stage by the producer warpgroup.
+// Warp roles: warpgroup 0 = producer (warp 0 lane 0 issues TMA; all four warps transpose MN-major tiles),
+// warpgroups 1-2 = MMA + epilogue, rows 0-63 and 64-127 of the tile.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -17,173 +20,189 @@
 
 namespace hk {
 
+constexpr int GEMM_THREADS = 384;
+constexpr int GEMM_SMEM_MAX = 227 * 1024;   // largest dynamic shared memory a block may opt in to on sm_90
 
 template <int BN>
 struct GemmCfg {
-  static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128 ? 6 : 8);
+  static constexpr int STAGES = 4;
   static constexpr int A_BYTES = 128 * 128;
   static constexpr int B_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int EPI_TILE = 4 * 32 * 36 * 4;   // four epilogue warps x a 32 x 36-float transpose tile (coalesced row-major stores)
-  static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + EPI_TILE;
+  static constexpr int RAW_BYTES = A_BYTES + B_BYTES;    // staging of MN-major operands (one k-block, hi or lo)
+  static constexpr int ACC_TILE = 2 * 128 * 33 * 4;      // two 32-column accumulator chunks, row-major, padded rows
+  static constexpr int EPI_TILE = 4 * 32 * 36 * 4;       // four epilogue warps x a 32 x 36-float transpose tile
+  static constexpr int SMEM_FIXED = 1024 /*align slack*/ + 256 /*barriers*/ + ACC_TILE + 2 * EPI_TILE;
 };
 
 // Persistent: one CTA per SM walks output tiles t, t+grid, ... (n-tile fastest, so CTAs running at the same time share
-// the A rows through L2).  The smem ring and the two TMEM accumulator sets (2 x BN columns) run across tile
-// boundaries: the epilogue of tile i overlaps the TMA/MMA of tile i+1.
-template <int BN>
-__global__ void __launch_bounds__(192, 1)
-umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ CUtensorMap tmAl, const __grid_constant__ CUtensorMap tmBl, int triple, GemmEpi epi,
-                 int M, int N, int K, int a_mn, int b_mn, int shareA, int shareB, int mn_sbo, int mn_type, int nstages,
-                 int tiles_m, int tiles_n, int total_tiles) {
+// the A rows through L2).  The smem ring runs across tile boundaries, so the producer loads tile i+1 while the consumers
+// finish tile i.  The epilogue stages each pair of 32-column accumulator chunks through shared memory, after which
+// consumer thread (half, q, lane) owns row 32 q + lane of chunk 2 c + half.
+template <int BN, bool TRIPLE>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const __grid_constant__ CUtensorMap tmAl, const __grid_constant__ CUtensorMap tmBl, GemmEpi epi,
+                  int M, int N, int K, int a_mn, int b_mn, int shareA, int shareB, int nstages,
+                  int tiles_m, int tiles_n, int total_tiles) {
   // triple: operands are (hi, lo) tf32 pairs (tmA/tmB = hi, tmAl/tmBl = lo) and every k-step issues Ah.Bl, Al.Bh, Ah.Bh
-  // into the same accumulator — the 3xTF32 product of the Newton-Schulz chain in ONE launch, no partial sums through memory
+  // — the 3xTF32 product of the Newton-Schulz chain in ONE launch, no partial sums through memory
   using Cfg = GemmCfg<BN>;
+  constexpr int NACC = BN / 2;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  constexpr int nops = TRIPLE ? 2 : 1;
   uint8_t* sA = smem;
   uint8_t* sB = smem + nstages * Cfg::A_BYTES;
   uint8_t* sAl = smem + nstages * Cfg::STAGE_BYTES;
   uint8_t* sBl = sAl + nstages * Cfg::A_BYTES;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + nstages * Cfg::STAGE_BYTES * (triple ? 2 : 1));
+  const bool any_mn = a_mn || b_mn;
+  uint8_t* raw = smem + nstages * Cfg::STAGE_BYTES * nops;                  // [nops][A_BYTES + B_BYTES] when any_mn
+  uint8_t* after = raw + (any_mn ? nops * Cfg::RAW_BYTES : 0);
+  uint64_t* full = reinterpret_cast<uint64_t*>(after);
   uint64_t* empty = full + nstages;
-  uint64_t* acc_full = empty + nstages;
-  uint64_t* acc_empty = acc_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* epi_tiles = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full) + 256);
+  uint64_t* raw_bar = empty + nstages;
+  float* acc_tile = reinterpret_cast<float*>(after + 256);
+  float* epi_tiles = acc_tile + Cfg::ACC_TILE / 4;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nk = (K + 31) / 32;
-  // triple mode keeps TWO accumulators per tile — the leading product Ah.Bh and the sum of the two correction products —
-  // and adds them in the epilogue: the tensor core's accumulator addition truncates, so feeding terms 2^-11 the size of the
-  // running sum into it loses them with a bias (the MPN 224x224 reference-gradient test moved by 10x when they shared one)
-  const int acc_cols = triple ? 2 * BN : BN;
-  const int TCOLS = 2 * acc_cols < 32 ? 32 : 2 * acc_cols;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < nstages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 2);
     }
-    for (int s = 0; s < 2; ++s) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], 4); }
+    mbar_init(raw_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, TCOLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      int kbg = 0;
-      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-        const int nt = t % tiles_n;
-        const int mt = (t / tiles_n) % tiles_m;
-        const int bz = t / (tiles_n * tiles_m);
-        const int m0 = mt * 128, n0 = nt * BN;
-        const int bza = shareA ? 0 : bz, bzb = shareB ? 0 : bz;
-        for (int kb = 0; kb < nk; ++kb, ++kbg) {
-          const int s = kbg % nstages;
-          const uint32_t ph = (kbg / nstages) & 1;
+  if (warp < 4) {
+    // ---------------------------------------------------------------- producer warpgroup
+    regs_dealloc<56>();
+    const int t = threadIdx.x;
+    int kbg = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      const int nt = tile % tiles_n;
+      const int mt = (tile / tiles_n) % tiles_m;
+      const int bz = tile / (tiles_n * tiles_m);
+      const int m0 = mt * 128, n0 = nt * BN;
+      const int bza = shareA ? 0 : bz, bzb = shareB ? 0 : bz;
+      for (int kb = 0; kb < nk; ++kb, ++kbg) {
+        const int s = kbg % nstages;
+        const uint32_t ph = (kbg / nstages) & 1;
+        if (t == 0) {
           mbar_wait(&empty[s], ph ^ 1);
-          mbar_expect_tx(&full[s], Cfg::STAGE_BYTES * (triple ? 2 : 1));
-          uint8_t* a = sA + s * Cfg::A_BYTES;
-          uint8_t* b = sB + s * Cfg::B_BYTES;
-          if (triple) {
-            uint8_t* al = sAl + s * Cfg::A_BYTES;
-            uint8_t* bl = sBl + s * Cfg::B_BYTES;
+          // K-major operands go straight into the stage; MN-major ones into the staging buffer
+          uint32_t direct = 0, staged = 0;
+          for (int o = 0; o < nops; ++o) {
+            (a_mn ? staged : direct) += Cfg::A_BYTES;
+            (b_mn ? staged : direct) += Cfg::B_BYTES;
+          }
+          if (!any_mn) mbar_expect_tx(&full[s], direct);
+          else mbar_expect_tx(raw_bar, direct + staged);
+          uint64_t* bar = any_mn ? raw_bar : &full[s];
+          for (int o = 0; o < nops; ++o) {
+            const CUtensorMap* ma = o ? &tmAl : &tmA;
+            const CUtensorMap* mb = o ? &tmBl : &tmB;
+            uint8_t* a = (o ? sAl : sA) + s * Cfg::A_BYTES;
+            uint8_t* b = (o ? sBl : sB) + s * Cfg::B_BYTES;
+            uint8_t* ra = raw + o * Cfg::RAW_BYTES;
+            uint8_t* rb = ra + Cfg::A_BYTES;
             if (!a_mn) {
-              tma_load_3d(al, &tmAl, &full[s], kb * 32, m0, bza);
+              tma_load_3d(a, ma, bar, kb * 32, m0, bza);
             } else {
 #pragma unroll
-              for (int j = 0; j < 4; ++j) tma_load_3d(al + j * 4096, &tmAl, &full[s], m0 + j * 32, kb * 32, bza);
+              for (int j = 0; j < 4; ++j) tma_load_3d(ra + j * 4096, ma, bar, m0 + j * 32, kb * 32, bza);
             }
             if (!b_mn) {
-              tma_load_3d(bl, &tmBl, &full[s], kb * 32, n0, bzb);
+              tma_load_3d(b, mb, bar, kb * 32, n0, bzb);
             } else {
 #pragma unroll
-              for (int j = 0; j < BN / 32; ++j) tma_load_3d(bl + j * 4096, &tmBl, &full[s], n0 + j * 32, kb * 32, bzb);
+              for (int j = 0; j < BN / 32; ++j) tma_load_3d(rb + j * 4096, mb, bar, n0 + j * 32, kb * 32, bzb);
             }
           }
-          if (!a_mn) {
-            tma_load_3d(a, &tmA, &full[s], kb * 32, m0, bza);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) tma_load_3d(a + j * 4096, &tmA, &full[s], m0 + j * 32, kb * 32, bza);
-          }
-          if (!b_mn) {
-            tma_load_3d(b, &tmB, &full[s], kb * 32, n0, bzb);
-          } else {
-#pragma unroll
-            for (int j = 0; j < BN / 32; ++j) tma_load_3d(b + j * 4096, &tmB, &full[s], n0 + j * 32, kb * 32, bzb);
-          }
         }
-      }
-    }
-  } else if (warp == 1) {
-    {   // warp-uniform loop; tcgen05 issue predicated on one elected lane
-      const uint32_t idesc = make_idesc_tf32(128, BN, a_mn, b_mn);
-      const uint64_t a_tmpl = a_mn ? make_sdesc(0, 4096, mn_sbo, mn_type) : make_sdesc(0, 16, 1024);
-      const uint64_t b_tmpl = b_mn ? make_sdesc(0, 4096, mn_sbo, mn_type) : make_sdesc(0, 16, 1024);
-      const uint32_t a_step = a_mn ? (1024u >> 4) : (32u >> 4);
-      const uint32_t b_step = b_mn ? (1024u >> 4) : (32u >> 4);
-      int kbg = 0, itl = 0;
-      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++itl) {
-        const int set = itl & 1;
-        mbar_wait(&acc_empty[set], ((itl >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d = tmem_base + set * acc_cols;
-        const uint32_t d_small = d + BN;
-        for (int kb = 0; kb < nk; ++kb, ++kbg) {
-          const int s = kbg % nstages;
-          const uint32_t ph = (kbg / nstages) & 1;
-          mbar_wait(&full[s], ph);
-          tc_fence_after();
-          const uint64_t a_base = a_tmpl + (smem_u32(sA + s * Cfg::A_BYTES) >> 4);
-          const uint64_t b_base = b_tmpl + (smem_u32(sB + s * Cfg::B_BYTES) >> 4);
-          const int krem = K - kb * 32;
-          const int ksteps = krem >= 32 ? 4 : (krem + 7) / 8;
-          if (elect_one()) {
-            if (triple) {
-              const uint64_t al_base = a_tmpl + (smem_u32(sAl + s * Cfg::A_BYTES) >> 4);
-              const uint64_t bl_base = b_tmpl + (smem_u32(sBl + s * Cfg::B_BYTES) >> 4);
-              for (int ks = 0; ks < ksteps; ++ks) {
-                umma_tf32_ss(d_small, a_base + ks * a_step, bl_base + ks * b_step, idesc, (kb | ks) ? 1u : 0u);
-                umma_tf32_ss(d_small, al_base + ks * a_step, b_base + ks * b_step, idesc, 1u);
-                umma_tf32_ss(d, a_base + ks * a_step, b_base + ks * b_step, idesc, (kb | ks) ? 1u : 0u);
-              }
-            } else {
-              for (int ks = 0; ks < ksteps; ++ks)
-                umma_tf32_ss(d, a_base + ks * a_step, b_base + ks * b_step, idesc, (kb | ks) ? 1u : 0u);
-            }
-            umma_commit(&empty[s]);
+        if (any_mn) {
+          mbar_wait(raw_bar, kbg & 1);
+          for (int o = 0; o < nops; ++o) {
+            const uint8_t* ra = raw + o * Cfg::RAW_BYTES;
+            if (a_mn) transpose_mn_tile(ra, (o ? sAl : sA) + s * Cfg::A_BYTES, 128, t, 128);
+            if (b_mn) transpose_mn_tile(ra + Cfg::A_BYTES, (o ? sBl : sB) + s * Cfg::B_BYTES, BN, t, 128);
           }
-          __syncwarp();
+          fence_proxy_async();       // generic-proxy stores -> visible to wgmma (async proxy)
+          named_bar(1, 128);         // whole staging buffer consumed before the next TMA overwrites it
+          if (t == 0) mbar_arrive(&full[s]);
         }
-        if (elect_one()) umma_commit(&acc_full[set]);
-        __syncwarp();
       }
     }
   } else {
-    const int q = warp & 3;
-    int itl = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++itl) {
-      const int nt = t % tiles_n;
-      const int mt = (t / tiles_n) % tiles_m;
-      const int bz = t / (tiles_n * tiles_m);
+    // ---------------------------------------------------------------- consumers: MMA, then epilogue
+    regs_alloc<224>();
+    const int ct = threadIdx.x - 128;          // 0..255
+    const int wg = ct >> 7;                    // row half of the tile this warpgroup multiplies
+    const int half = ct >> 7;                  // accumulator chunk parity this thread stores in the epilogue
+    const int q = (ct >> 5) & 3;
+    const int wl = (ct & 127) >> 5;            // warp within the warpgroup (fragment rows 16 wl ..)
+    int kbg = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      const int nt = tile % tiles_n;
+      const int mt = (tile / tiles_n) % tiles_m;
+      const int bz = tile / (tiles_n * tiles_m);
       const int m0 = mt * 128, n0 = nt * BN;
+      float acc[NACC], acc2[TRIPLE ? NACC : 1];
+#pragma unroll
+      for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+      if constexpr (TRIPLE) {
+#pragma unroll
+        for (int i = 0; i < NACC; ++i) acc2[i] = 0.f;
+      }
+      // triple mode keeps TWO accumulators — the leading product Ah.Bh and the sum of the two correction products — added
+      // in the epilogue, so the small correction terms are not lost against the running sum
+      for (int kb = 0; kb < nk; ++kb, ++kbg) {
+        const int s = kbg % nstages;
+        const uint32_t ph = (kbg / nstages) & 1;
+        mbar_wait(&full[s], ph);
+        const uint64_t a_base = make_sdesc(smem_u32(sA + s * Cfg::A_BYTES + wg * 64 * 128));
+        const uint64_t b_base = make_sdesc(smem_u32(sB + s * Cfg::B_BYTES));
+        wgmma_fence();
+        if constexpr (TRIPLE) {
+          const uint64_t al_base = make_sdesc(smem_u32(sAl + s * Cfg::A_BYTES + wg * 64 * 128));
+          const uint64_t bl_base = make_sdesc(smem_u32(sBl + s * Cfg::B_BYTES));
+          // a partial last k-block is zero-filled by TMA past K: all four k-steps run, keeping the wgmma stream uniform
+#pragma unroll
+          for (int ks = 0; ks < 4; ++ks) {
+            wgmma_tf32(acc2, a_base + ks * 2, bl_base + ks * 2, 1);
+            wgmma_tf32(acc2, al_base + ks * 2, b_base + ks * 2, 1);
+            wgmma_tf32(acc, a_base + ks * 2, b_base + ks * 2, 1);
+          }
+        } else {
+#pragma unroll
+          for (int ks = 0; ks < 4; ++ks) wgmma_tf32(acc, a_base + ks * 2, b_base + ks * 2, 1);
+        }
+        wgmma_commit();
+        // one group stays in flight: the MMAs of k-block kb overlap the wait for kb + 1; the stage of kb - 1 is released
+        wgmma_wait<1>();
+        wgmma_keep(acc);
+        if constexpr (TRIPLE) wgmma_keep(acc2);
+        if (kb > 0 && (ct & 127) == 0) mbar_arrive(&empty[(kbg - 1) % nstages]);
+      }
+      wgmma_wait<0>();
+      wgmma_keep(acc);
+      if constexpr (TRIPLE) wgmma_keep(acc2);
+      if ((ct & 127) == 0) mbar_arrive(&empty[(kbg - 1) % nstages]);
+      if constexpr (TRIPLE) {
+#pragma unroll
+        for (int i = 0; i < NACC; ++i) acc[i] += acc2[i];
+      }
       const int row = m0 + q * 32 + lane;
-      const int set = itl & 1;
-      mbar_wait(&acc_full[set], (itl >> 1) & 1);
-      tc_fence_after();
-      const float alpha = epi.alpha * (epi.alpha_vec ? epi.alpha_vec[bz] : 1.f);
+      // post_scale: the value becomes sqrt(alpha_b * acc + post_eps) * post_scale[b] before the rest of the epilogue
+      const float alpha_b = epi.alpha * (epi.alpha_vec ? epi.alpha_vec[bz] : 1.f);
+      const float pscale = epi.post_scale ? epi.post_scale[bz] : 0.f;
+      const float alpha = epi.post_scale ? 1.f : alpha_b;
       const float beta = epi.beta * (epi.beta_vec ? epi.beta_vec[bz] : 1.f);
       float* Cb = epi.C + (long long)bz * epi.strideC;
       const float* Db = epi.D ? epi.D + (long long)bz * epi.strideD : nullptr;
@@ -191,18 +210,70 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const long long ldE = epi.ldE ? epi.ldE : epi.ldc;
       const float* Eb = epi.E ? epi.E + (long long)bz * (epi.ldE ? epi.strideE : epi.strideC) : nullptr;
       float* Clb = epi.C_lo ? epi.C_lo + (long long)bz * epi.strideC : nullptr;
-      const bool simple = !Eb && !Clb && !Dlb && epi.diag == 0.f && !epi.trans_c && (!Db || epi.ldd != 0);
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        float v[32];
-        tmem_ld32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + set * acc_cols + c * 32, v);
-        tmem_ld_wait();
-        if (triple) {
-          float sm[32];
-          tmem_ld32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + set * acc_cols + BN + c * 32, sm);
-          tmem_ld_wait();
+      const bool simple = !Eb && !Clb && !Dlb && epi.diag == 0.f && !epi.trans_c && (!Db || epi.ldd != 0) && !epi.mode;
+      float cr = 0.f;                          // EPI_BILINEAR_S: this thread's share of <dY, z>
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += sm[j];
+      for (int cp = 0; cp < BN / 64; ++cp) {
+        // fragments of chunks 2 cp, 2 cp + 1 -> acc_tile[chunk parity][row][33]
+        named_bar(2, 256);
+#pragma unroll
+        for (int i = 0; i < NACC / 4; ++i) {
+          const int col = 8 * i + 2 * (lane & 3);
+          if ((col >> 6) != cp) continue;
+          float* dst = acc_tile + ((col >> 5) & 1) * (128 * 33);
+          const int r0 = wg * 64 + wl * 16 + (lane >> 2);
+          dst[r0 * 33 + (col & 31)] = acc[4 * i];
+          dst[r0 * 33 + (col & 31) + 1] = acc[4 * i + 1];
+          dst[(r0 + 8) * 33 + (col & 31)] = acc[4 * i + 2];
+          dst[(r0 + 8) * 33 + (col & 31) + 1] = acc[4 * i + 3];
+        }
+        named_bar(2, 256);
+        const int c = 2 * cp + half;
+        float v[32];
+        {
+          const float* src = acc_tile + half * (128 * 33) + (q * 32 + lane) * 33;
+#pragma unroll
+          for (int j = 0; j < 32; ++j) v[j] = src[j];
+        }
+        if (epi.post_scale) {
+#pragma unroll
+          for (int j = 0; j < 32; ++j) v[j] = sqrtf(fmaf(v[j], alpha_b, epi.post_eps)) * pscale;
+        }
+        if (epi.mode == EPI_BILINEAR_S) {
+          const int col0 = n0 + c * 32;
+          if (row < M && col0 < N) {
+            const float* dyb = epi.dY + (long long)bz * M * N;
+            const float* drow = dyb + (long long)row * N + col0;
+            float* dst = Cb + (long long)row * epi.ldc + col0;
+#pragma unroll
+            for (int j = 0; j < 32; ++j) {
+              if (col0 + j < N) {
+                const float z = sqrtf(fmaf(v[j], alpha_b, epi.post_eps));
+                const float dv = drow[j];
+                cr = fmaf(dv, z, cr);
+                // dY[j][i]: for a fixed j the lanes of the warp hold consecutive rows i — one coalesced 128 B read
+                dst[j] = (dv + dyb[(long long)(col0 + j) * N + row]) / (2.f * z);
+              }
+            }
+          }
+          continue;
+        }
+        if (epi.mode == EPI_SKETCH) {
+          const int col0 = n0 + c * 32;
+          if (row < M && col0 < N) {
+            float* bins = epi.bins + (long long)bz * epi.d;
+            const int hi = epi.h1[row];
+            const float si = epi.s1[row] * alpha_b;
+#pragma unroll 4
+            for (int j = 0; j < 32; ++j) {
+              if (col0 + j < N) {
+                int k = hi + __ldg(epi.h2 + col0 + j);
+                if (k >= epi.d) k -= epi.d;
+                atomicAdd(bins + k, si * __ldg(epi.s2 + col0 + j) * v[j]);
+              }
+            }
+          }
+          continue;
         }
         const int col0 = n0 + c * 32;
         // fast path (plain scaled store of a full, aligned 32-column chunk): a handful of instructions per element — the
@@ -213,7 +284,7 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           // half-written 32 B sectors, twice the L2 write transactions (the 1x1-conv GEMMs of the ResNet trunk are
           // output-write-bound).  Transpose the 32 x 32 chunk through a warp-private shared-memory tile instead: every store
           // instruction then writes four full 128 B rows; the optional addend D (residual gradient) is read the same way.
-          float* tile = epi_tiles + (warp - 2) * (32 * 36);
+          float* tile = epi_tiles + (ct >> 5) * (32 * 36);
 #pragma unroll
           for (int j = 0; j < 32; j += 4)
             *reinterpret_cast<float4*>(tile + lane * 36 + j) =
@@ -333,14 +404,12 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[set]);
+      if (epi.mode == EPI_BILINEAR_S) {        // fp64 atomics: the image's sum does not depend on their order at fp32 level
+        cr = warp_sum(cr);
+        if (lane == 0) atomicAdd(epi.c_raw + bz, (double)cr);
+      }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, TCOLS);
 }
 
 static int make_operand_map(CUtensorMap* tm, const float* P, int mn_major, long long ld, long long stride, int rows,
@@ -359,12 +428,18 @@ static int make_operand_map(CUtensorMap* tm, const float* P, int mn_major, long 
   }
   strides[0] = (uint64_t)ld * 4;
   strides[1] = bs;
-  return make_tmap(tm, P, 3, dims, strides, box, mn_major != 0);
+  return make_tmap(tm, P, 3, dims, strides, box);
 }
 
-static int dbg_env(const char* name, int dflt) {
-  const char* v = getenv(name);
-  return v ? atoi(v) : dflt;
+static int num_sms() {
+  static int sms = 0;
+  if (!sms) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        sms <= 0)
+      sms = 132;
+  }
+  return sms;
 }
 
 template <int BN>
@@ -374,31 +449,40 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Gem
   using Cfg = GemmCfg<BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(umma_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
+    const int max_smem = GEMM_SMEM_MAX;
+    cudaError_t e = cudaFuncSetAttribute(wgmma_gemm_kernel<BN, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
+    if constexpr (BN == 64)
+      if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(wgmma_gemm_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
     if (e != cudaSuccess) return set_error((int)e, "cudaFuncSetAttribute(gemm<%d>): %s", BN, cudaGetErrorString(e));
     attr_set = true;
   }
   const int tiles_m = (M + 127) / 128, tiles_n = (N + BN - 1) / BN;
   const long long total = (long long)tiles_m * tiles_n * batch;
   if (total >= (1ll << 31)) return set_error(HK_ERR_UNSUPPORTED, "gemm: too many tiles");
-  static int sms = 0;
-  if (!sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
-  }
+  const int sms = num_sms();
   const int nk = (K + 31) / 32;
   const long long kblocks_per_cta = (long long)nk * ((total + sms - 1) / sms);
   const int triple = tmAl ? 1 : 0;
-  const int max_stages = triple ? Cfg::STAGES / 2 : Cfg::STAGES;
+  const int nops = triple ? 2 : 1;
+  const int raw = (a_mn || b_mn) ? nops * Cfg::RAW_BYTES : 0;
+  int max_stages = (GEMM_SMEM_MAX - Cfg::SMEM_FIXED - raw) / (Cfg::STAGE_BYTES * nops);   // what fits in 227 KB
+  if (max_stages > Cfg::STAGES) max_stages = Cfg::STAGES;
   const int nstages = kblocks_per_cta < max_stages ? (int)kblocks_per_cta : max_stages;
-  const int smem = nstages * Cfg::STAGE_BYTES * (triple ? 2 : 1) + 1024 + 256 + Cfg::EPI_TILE;
+  const int smem = nstages * Cfg::STAGE_BYTES * nops + raw + Cfg::SMEM_FIXED;
   const int grid = total < sms ? (int)total : sms;
-  umma_gemm_kernel<BN><<<grid, 192, smem, stream>>>(tmA, tmB, triple ? *tmAl : tmA, triple ? *tmBl : tmB, triple, epi, M, N, K,
-                                                    a_mn, b_mn, shareA, shareB,
-                                                    dbg_env("HK_DBG_MN_SBO", 512), dbg_env("HK_DBG_MN_TYPE", 1), nstages,
-                                                    tiles_m, tiles_n, (int)total);
-  HK_LAUNCH_CHECK("umma_gemm_kernel");
+  bool launched = false;
+  if constexpr (BN == 64) {   // the 3xTF32 pair kernel runs 64-wide tiles only (two accumulators per thread)
+    if (triple) {
+      wgmma_gemm_kernel<64, true><<<grid, GEMM_THREADS, smem, stream>>>(tmA, tmB, *tmAl, *tmBl, epi, M, N, K, a_mn, b_mn, shareA,
+                                                                        shareB, nstages, tiles_m, tiles_n, (int)total);
+      launched = true;
+    }
+  }
+  if (!launched)
+    wgmma_gemm_kernel<BN, false><<<grid, GEMM_THREADS, smem, stream>>>(tmA, tmB, tmA, tmB, epi, M, N, K, a_mn, b_mn, shareA,
+                                                                       shareB, nstages, tiles_m, tiles_n, (int)total);
+  HK_LAUNCH_CHECK("wgmma_gemm_kernel");
   return 0;
 }
 
@@ -414,7 +498,7 @@ __global__ void tf32_split_kernel(const float* __restrict__ x, float* __restrict
 int tf32_split(const float* x, float* hi, float* lo, size_t n, cudaStream_t stream) {
   if (!n) return 0;
   size_t g = (n + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > 132 * 16) g = 132 * 16;
   tf32_split_kernel<<<(unsigned)g, 256, 0, stream>>>(x, hi, lo, n);
   HK_LAUNCH_CHECK("tf32_split_kernel");
   return 0;
@@ -462,12 +546,11 @@ int gemm_tf32_1x(const float* A, int a_mn, long long lda, long long strideA, con
   HK_REQUIRE(batch <= 65535, HK_ERR_UNSUPPORTED, "gemm: batch %d > 65535", batch);
   CUtensorMap tmA, tmB;
   int shareA, shareB, r;
-  const int BN = N <= 64 ? 64 : (N <= 128 ? 128 : 256);
+  const int BN = N <= 64 ? 64 : 128;   // 64 accumulator registers per thread at most
   if ((r = make_operand_map(&tmA, A, a_mn, lda, strideA, M, K, batch, 128, &shareA))) return r;
   if ((r = make_operand_map(&tmB, B, b_mn, ldb, strideB, N, K, batch, BN, &shareB))) return r;
   if (BN == 64) return launch_gemm<64>(tmA, tmB, epi, M, N, K, batch, a_mn, b_mn, shareA, shareB, stream);
-  if (BN == 128) return launch_gemm<128>(tmA, tmB, epi, M, N, K, batch, a_mn, b_mn, shareA, shareB, stream);
-  return launch_gemm<256>(tmA, tmB, epi, M, N, K, batch, a_mn, b_mn, shareA, shareB, stream);
+  return launch_gemm<128>(tmA, tmB, epi, M, N, K, batch, a_mn, b_mn, shareA, shareB, stream);
 }
 
 // C = epilogue(Ah.Bh + Al.Bh + Ah.Bl) in ONE launch; (Ah, Al) / (Bh, Bl) are tf32 (hi, lo) pairs with identical layouts.
@@ -479,21 +562,13 @@ int gemm_tf32_pair(const float* Ah, const float* Al, int a_mn, long long lda, lo
              M, N, K, batch);
   CUtensorMap tmA, tmB, tmAl, tmBl;
   int shareA, shareB, r;
-  static int sms = 0;
-  if (!sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
-  }
-  // 128-wide tiles while 256-wide ones would leave SMs idle (Newton-Schulz: n = 256, batch 32 -> 128 tiles instead of 64)
-  // two accumulators per tile x double buffering = 4 BN TMEM columns: BN <= 128
-  const int BN = N <= 64 ? 64 : 128;
+  // two accumulators per tile in registers: BN = 64 keeps them at 64 per thread
+  const int BN = 64;
   if ((r = make_operand_map(&tmA, Ah, a_mn, lda, strideA, M, K, batch, 128, &shareA))) return r;
   if ((r = make_operand_map(&tmAl, Al, a_mn, lda, strideA, M, K, batch, 128, &shareA))) return r;
   if ((r = make_operand_map(&tmB, Bh, b_mn, ldb, strideB, N, K, batch, BN, &shareB))) return r;
   if ((r = make_operand_map(&tmBl, Bl, b_mn, ldb, strideB, N, K, batch, BN, &shareB))) return r;
-  if (BN == 64) return launch_gemm<64>(tmA, tmB, epi, M, N, K, batch, a_mn, b_mn, shareA, shareB, stream, &tmAl, &tmBl);
-  return launch_gemm<128>(tmA, tmB, epi, M, N, K, batch, a_mn, b_mn, shareA, shareB, stream, &tmAl, &tmBl);
+  return launch_gemm<64>(tmA, tmB, epi, M, N, K, batch, a_mn, b_mn, shareA, shareB, stream, &tmAl, &tmBl);
 }
 
 }  // namespace hk
@@ -511,6 +586,7 @@ extern "C" int hk_gemm_3xtf32(const float* A, int a_mn_major, long long lda, lon
   epi.alpha = alpha; epi.beta = beta; epi.diag = diag;
   epi.trans_c = trans_c; epi.relu = relu;
   epi.C_lo = nullptr; epi.D_lo = nullptr; epi.E = nullptr; epi.ldE = 0; epi.strideE = 0;
+  epi.post_scale = nullptr; epi.post_eps = 0.f; epi.mode = hk::EPI_PLAIN;
   HK_REQUIRE(A && B && C && M > 0 && N > 0 && K > 0 && batch > 0, HK_ERR_ARG, "hk_gemm_3xtf32: bad args");
   return hk::gemm_tf32_3x(A, a_mn_major, lda, strideA, B, b_mn_major, ldb, strideB, epi, M, N, K, batch,
                           static_cast<cudaStream_t>(stream));
@@ -528,6 +604,7 @@ extern "C" int hk_gemm_tf32(const float* A, int a_mn_major, long long lda, long 
   epi.alpha = alpha; epi.beta = beta; epi.diag = diag;
   epi.trans_c = trans_c; epi.relu = relu;
   epi.C_lo = nullptr; epi.D_lo = nullptr; epi.E = nullptr; epi.ldE = 0; epi.strideE = 0;
+  epi.post_scale = nullptr; epi.post_eps = 0.f; epi.mode = hk::EPI_PLAIN;
   return hk::gemm_tf32(A, a_mn_major, lda, strideA, B, b_mn_major, ldb, strideB, epi, M, N, K, batch,
                        static_cast<cudaStream_t>(stream));
 }

@@ -1,4 +1,4 @@
-// Epilogue description + host entry of the generic batched tcgen05 TF32 GEMM (gemm.cu).
+// Epilogue description + host entry of the generic batched wgmma TF32 GEMM (gemm.cu).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -18,7 +18,23 @@ struct GemmEpi {
   const float* D_lo;   // optional: D given as a (hi, lo) pair
   const float* E;      // optional: raw partial product added to the accumulator before alpha (row-major [M][N] per batch)
   long long ldE, strideE;   // layout of E; 0 = same as C (ldc / strideC)
+  const float* post_scale;  // optional [batch]: value = sqrt(alpha_b * acc + post_eps) * post_scale[b], then D / ReLU / rounding
+  float post_eps;
+  // Fused consumers of a square Gram G = alpha_b * acc (M = N = C, row-major [C][C] per batch entry):
+  //   EPI_BILINEAR_S: C[i][j] = (dY[i][j] + dY[j][i]) / (2 z_ij), z_ij = sqrt(G_ij + post_eps); c_raw[b] += sum_ij dY_ij z_ij
+  //                   (c_raw pre-zeroed) — the bilinear-pool backward's S without the Gram going through memory;
+  //   EPI_SKETCH    : bins[b][(h1[i] + h2[j]) mod d] += s1[i] s2[j] G_ij (bins pre-zeroed); C is not written.
+  int mode;
+  const float* dY;
+  double* c_raw;
+  const int* h1;
+  const int* h2;
+  const float* s1;
+  const float* s2;
+  float* bins;
+  int d;
 };
+enum { EPI_PLAIN = 0, EPI_BILINEAR_S = 1, EPI_SKETCH = 2 };
 
 // C[b] = alpha_b * (A[b].B[b] + E[b]) + diag*I + beta_b * (D[b] + D_lo[b]);  see hk_gemm_tf32 in the public header.
 // Dispatches on the precision mode (host.h): one TF32 pass, or 3xTF32 over internally split operands.

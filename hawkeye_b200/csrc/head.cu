@@ -135,7 +135,7 @@ __global__ void normalize_u8_kernel(const unsigned char* __restrict__ x, float* 
 
 static inline int grid_for(size_t n, int block) {
   size_t g = (n + block - 1) / block;
-  const size_t cap = 148 * 16;
+  const size_t cap = 132 * 16;
   return (int)(g < cap ? (g ? g : 1) : cap);
 }
 
@@ -145,7 +145,7 @@ using namespace hk;
 
 extern "C" {
 
-/* y[B,N] = x[B,F] . w[N,F]^T + bias   via split-K tcgen05 GEMM; workspace = S*B*N floats */
+/* y[B,N] = x[B,F] . w[N,F]^T + bias   via split-K wgmma GEMM; workspace = S*B*N floats */
 static int linear_splits(int F) {
   int S = F / 1024;
   if (S < 1) S = 1;

@@ -69,7 +69,7 @@ static PFN_encodeTiled get_encode() {
 }
 
 int make_tmap(CUtensorMap* out, const float* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-              const uint32_t* box, bool mn_major, const uint32_t* elem_strides) {
+              const uint32_t* box, const uint32_t* elem_strides) {
   // the driver call needs a current context; autograd worker threads may not have bound one yet
   static thread_local bool ctx_ready = false;
   if (!ctx_ready) {
@@ -99,7 +99,7 @@ int make_tmap(CUtensorMap* out, const float* base, int rank, const uint64_t* dim
   if (!aligned16(base)) return set_error(HK_ERR_ALIGN, "tensor-map base pointer is not 16-byte aligned");
   CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, static_cast<cuuint32_t>(rank), const_cast<float*>(base),
                    gdim, gstr, bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   mn_major ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
     return set_error(HK_ERR_DRIVER, "cuTensorMapEncodeTiled failed (CUresult %d; rank %d dims %llu,%llu box %u,%u)",
@@ -112,7 +112,7 @@ int make_tmap(CUtensorMap* out, const float* base, int rank, const uint64_t* dim
 
 extern "C" {
 
-const char* hk_version(void) { return "hawkeye_b200 0.1 (sm_100a; tcgen05/TMA)"; }
+const char* hk_version(void) { return "hawkeye_b200 0.1 (sm_90a; wgmma/TMA)"; }
 const char* hk_last_error(void) { return hk::last_error_buf(); }
 void hk_set_precise(int on) { hk::g_precise.store(on ? 1 : 0); }
 int hk_get_precise(void) { return hk::precise() ? 1 : 0; }

@@ -27,11 +27,8 @@ inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 
 // Encode a tiled fp32 tensor map with SWIZZLE_128B and zero OOB fill.
 // dims/box are innermost-first; strides_bytes[i] is the byte stride of dim i+1 (rank-1 entries).
-// mn_major=false: CU_TENSOR_MAP_SWIZZLE_128B (16 B chunks; K-major UMMA operands).
-// mn_major=true : CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B (32 B chunks) — the only shared-memory layout tcgen05
-//                 accepts for MN-major 32-bit (tf32) operands (UMMA layout type SWIZZLE_128B_BASE32B).
 int make_tmap(CUtensorMap* out, const float* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-              const uint32_t* box, bool mn_major = false, const uint32_t* elem_strides = nullptr);
+              const uint32_t* box, const uint32_t* elem_strides = nullptr);
 
 // ---- precise mode (parity runs; hk_set_precise / $HK_PRECISE) -------------------------------------------------------
 // 0 (default): every tensor-core product is single-pass TF32 and producers round what they hand to the next MMA.

@@ -6,7 +6,7 @@
 // different-class), (different-attention same-class, different-attention different-class), built by a Python loop over the
 // anchors with repeat()ed [n_pos, n_neg] matrices (MAMC_loss.py:62-88).  Here: sum_k exp(n_k - p_j) = exp(-p_j) * E with
 // E = sum_k exp(n_k), so one anchor costs O(n) and the whole loss is ONE launch (one block per anchor) that also emits
-// d loss / d prod; the products prod = F F^T and dF = (dprod + dprod^T) F run on the 3xTF32 tcgen05 GEMM.
+// d loss / d prod; the products prod = F F^T and dF = (dprod + dprod^T) F run on the 3xTF32 wgmma GEMM.
 #include "common.cuh"
 #include "host.h"
 #include "../../include/hawkeye_b200.h"

@@ -1,8 +1,8 @@
 // Fast MPN-COV pooling head (reference model/methods/MPNCOV.py:105-230): covariance pooling, Newton-Schulz matrix
 // square root (forward AND the reference's hand-derived backward, formula by formula), upper-triangular vectorise.
 //
-// Every matrix product runs on the tcgen05 GEMM (gemm.cu).  The coupled Newton-Schulz chain is 12 dependent 256^3
-// products forward / 38 backward and is NOT converged after 5 iterations (SURVEY 3.2), so rounding compounds; the
+// Every matrix product runs on the wgmma GEMM (gemm.cu).  The coupled Newton-Schulz chain is 12 dependent 256^3
+// products forward / 38 backward and is NOT converged after 5 iterations, so rounding compounds; the
 // chain therefore runs in 3xTF32: every matrix is kept as a (hi, lo) pair of tf32 values (hi = rn(x), lo = rn(x-hi))
 // and  A.B ~= Ah.Bh + Al.Bh + Ah.Bl  (three tensor-core GEMMs, fp32 accumulation) — fp32-class accuracy at 3x the
 // (tiny: 1.8 GFLOP/img) cost.
@@ -17,7 +17,7 @@ struct Pair { float* hi; float* lo; };
 
 static inline int grid_for(size_t n, int block) {
   size_t g = (n + block - 1) / block;
-  const size_t cap = 148 * 16;
+  const size_t cap = 132 * 16;
   return (int)(g < cap ? (g ? g : 1) : cap);
 }
 
@@ -30,7 +30,7 @@ static int mm3(Pair A, Pair B, Pair C, float* tmp, int n, int batch, float alpha
   f.C = C.hi; f.C_lo = C.lo; f.ldc = n; f.strideC = s;
   f.alpha = alpha; f.alpha_vec = alpha_vec; f.diag = diag;
   if (D) { f.D = D->hi; f.D_lo = D->lo; f.ldd = n; f.strideD = s; f.beta = beta; }
-  // one launch: every k-step issues Ah.Bl, Al.Bh, Ah.Bh into the same TMEM accumulator (gemm.cu, triple mode)
+  // one launch: every k-step issues Ah.Bl, Al.Bh, Ah.Bh into the same accumulators (gemm.cu, triple mode)
   return gemm_tf32_pair(A.hi, A.lo, 0, n, s, B.hi, B.lo, 1, n, s, f, n, n, n, batch, st);
 }
 

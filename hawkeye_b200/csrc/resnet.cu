@@ -11,7 +11,7 @@ namespace hk {
 
 static inline int rgrid(size_t n, int block) {
   size_t g = (n + block - 1) / block;
-  const size_t cap = 148 * 16;
+  const size_t cap = 132 * 16;
   return (int)(g < cap ? (g ? g : 1) : cap);
 }
 
@@ -509,7 +509,7 @@ int hk_nchw_to_nhwc(const float* x, float* y, int N, int HW, int C, void* stream
 }
 
 /* weight gradient of a matrix-form (1x1 / im2col) convolution: dw [Cout][K] = dY[P][Cout]^T . X[P][K], split-K batched
- * MN-major tcgen05 GEMM + reduction.  workspace = S * Cout * K floats. */
+ * MN-major wgmma GEMM + reduction.  workspace = S * Cout * K floats. */
 size_t hk_matconv_wgrad_workspace_bytes(long long P, int K, int Cout) {
   return (size_t)kc_splits(P, Cout, K) * Cout * K * sizeof(float);
 }

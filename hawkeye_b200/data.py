@@ -1,4 +1,4 @@
-"""Host side of the input pipeline with the reference's surface (SURVEY 8(f) N4): ``FGDataset`` (dataset/dataset.py:22-64),
+"""Host side of the input pipeline with the reference's surface: ``FGDataset`` (dataset/dataset.py:22-64),
 the train / eval transform presets (dataset/transforms.py:14-73) and the class-balanced batch sampler OSMENet trains with
 (dataset/sampler.py:5-38).  JPEG decode and the PIL augmentations stay on the host exactly as in the reference — this is
 Python plumbing, not a kernel path; the tensor part of the eval preset (``ToTensor + Normalize``) can run on the GPU instead

@@ -8,7 +8,7 @@ from ..utils import initialize_weights
 
 
 class BilinearPooling(nn.Module):
-    """Fused Gram + sqrt(.+1e-5) + L2-normalise (BCNN.py:8-27) on the tcgen05 kernel."""
+    """Fused Gram + sqrt(.+1e-5) + L2-normalise (BCNN.py:8-27) on the wgmma kernel."""
 
     def forward(self, x):
         return ops.bilinear_pool(x)

@@ -1,8 +1,8 @@
-"""Channel Interaction Network head with the reference's surface (model/methods/CIN.py:9-108) — SURVEY 8(f) row N1.
+"""Channel Interaction Network head with the reference's surface (model/methods/CIN.py:9-108).
 
 ``ChannelInteractionModule`` keeps the reference's constructor, parameters (``conv``, ``fc``) and outputs — ``Z`` in eval
 mode, ``(Z, Z_CCI)`` in training — but runs on the library's kernels: the channel Gram ``X X^T / WH`` (:31) and both
-``W . X`` products (:34, :55) on the tcgen05 GEMM, ``softmax(-G)`` (:32) and ``|W_SCI - w W_SCI_BA|`` (:53) as fused row /
+``W . X`` products (:34, :55) on the wgmma GEMM, ``softmax(-G)`` (:32) and ``|W_SCI - w W_SCI_BA|`` (:53) as fused row /
 elementwise kernels, the 3x3 convolution (:36, :57) on the implicit-GEMM conv, ``fc`` (:47-48) on the skinny GEMM.
 Any spatial size works: TMA needs a 16-byte row pitch, so the [B, C, WH] view is zero-padded to a multiple of 4 columns
 (7x7 = 49 -> 52), which changes neither the Gram (divided by the true WH) nor the products.

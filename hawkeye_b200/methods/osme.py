@@ -1,4 +1,4 @@
-"""OSMENet with the reference's surface (model/methods/OSME.py:8-64) — SURVEY 8(f) row N3, the OSME half.
+"""OSMENet with the reference's surface (model/methods/OSME.py:8-64).
 
 ``OSME_block`` = squeeze (spatial mean) -> Linear -> ReLU -> Linear -> sigmoid -> channel-wise re-scaling of the feature map;
 ``OSME`` = P such blocks, each followed by a Linear over the flattened gated map; ``OSMENet`` = ResNet-101 trunk + OSME +

@@ -1,7 +1,7 @@
 """PeerLearningNet with the reference's surface (model/methods/PeerLearningNet.py:8-20): two copies of a base model built
 through the registry (``config.base_model.name`` — BCNN in configs/PeerLearning_BCNN_S{1,2}.yaml), the second with a freshly
 initialised classifier; ``forward`` returns both logit tensors.  The base model is whatever ``MODEL`` holds under that name,
-i.e. the B200-native BCNN / CBCNN / MPN, so this caller of the hot path inherits the kernels unchanged (SURVEY §8f, N2)."""
+i.e. the native BCNN / CBCNN / MPN, so this caller of the hot path inherits the kernels unchanged."""
 import copy
 
 import torch.nn as nn

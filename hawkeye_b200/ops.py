@@ -173,7 +173,7 @@ def _vgg_plan(cfg):
 
 
 class VGGFeaturesFn(Function):
-    """x NCHW image -> NCHW feature map.  Internally NHWC; convs are tcgen05 implicit GEMMs.
+    """x NCHW image -> NCHW feature map.  Internally NHWC; convs are wgmma implicit GEMMs.
 
     params = (w0, b0, w1, b1, ...) in the reference layout [Cout,Cin,3,3] / [Cout].
     """
@@ -319,7 +319,7 @@ def vgg_features(x, cfg, params, train_backbone=True):
 # ----------------------------------------------------------------------------------------------------------
 def gemm_tf32(A, B, a_mn=False, b_mn=False, M=None, N=None, K=None, alpha=1.0, diag=0.0, D=None, beta=0.0,
               alpha_vec=None, beta_vec=None, trans_c=False, relu=False, out=None):
-    """Batched C = alpha*A.B + diag*I + beta*D on the tcgen05 GEMM.  A: [b,M,K] (or [b,K,M] if a_mn),
+    """Batched C = alpha*A.B + diag*I + beta*D on the wgmma GEMM.  A: [b,M,K] (or [b,K,M] if a_mn),
     B: [b,N,K] (K-major, i.e. C = A.B^T layout) or [b,K,N] if b_mn.  2-D operands are shared across the batch."""
     _check_cuda(A, B)
     A, B = _f32c(A), _f32c(B)

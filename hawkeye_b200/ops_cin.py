@@ -1,5 +1,5 @@
 """Autograd bindings for the channel-interaction module (reference model/methods/CIN.py:24-60): batched Gram and W.X
-products on the tcgen05 GEMM, softmax(-G), the contrastive weight |W_SCI - w W_SCI_BA|, the 3x3 convolution on the
+products on the wgmma GEMM, softmax(-G), the contrastive weight |W_SCI - w W_SCI_BA|, the 3x3 convolution on the
 implicit-GEMM kernels (NCHW in / out), and the classifier's spatial mean.  Host plumbing only; all arithmetic is in
 libhawkeye_b200.so."""
 import torch
@@ -114,7 +114,7 @@ class CCIWeightFn(Function):
 
 
 class Conv3x3NCHWFn(Function):
-    """nn.Conv2d(C, C, 3, 1, 1) on an NCHW map (CIN.py:22,36,57): NHWC inside, tcgen05 implicit GEMM."""
+    """nn.Conv2d(C, C, 3, 1, 1) on an NCHW map (CIN.py:22,36,57): NHWC inside, wgmma implicit GEMM."""
 
     @staticmethod
     def forward(ctx, x, w, b):

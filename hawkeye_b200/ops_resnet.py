@@ -1,7 +1,7 @@
 """ResNet-50 v1.5 trunk (reference model/backbone/resnet.py:89-252) and the MPN-COV dimension-reduction block
 (MPNCOV.py:64-69) as explicit forward/backward pipelines over the C-ABI kernels.  NHWC fp32 inside.
 
-conv unit = convolution (tcgen05 GEMM / implicit GEMM) -> train-mode BatchNorm (+ residual) (+ ReLU).
+conv unit = convolution (wgmma GEMM / implicit GEMM) -> train-mode BatchNorm (+ residual) (+ ReLU).
 """
 import torch
 from torch.autograd import Function

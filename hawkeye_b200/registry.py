@@ -15,7 +15,7 @@ BACKBONE = Repository()
 
 
 def install_into(model_registry, names=('BCNN', 'CBCNN', 'MPN', 'CIN', 'PeerLearningNet'), backbone_registry=None):
-    """Drop-in: overwrite the reference's own ``model.registry.MODEL`` entries with the B200-native classes,
+    """Drop-in: overwrite the reference's own ``model.registry.MODEL`` entries with the H100-native classes,
     so an unmodified Hawkeye ``Trainer`` (train.py:158-169) builds them via ``MODEL.get(name)(config)``."""
     for n in names:
         if n in MODEL:

@@ -3,7 +3,7 @@
 Same hooks (``get_model / get_criterion / get_optimizer / get_scheduler / to_device / batch_training /
 batch_validate / save_model / save_checkpoint / load_checkpoint / on_*``) and the same yaml schema, so the
 reference's ``Examples/{BCNN,CBCNN,MPN}.py`` subclasses port by changing one import.  Differences, all at the
-edges (SURVEY.md §0.7): data-parallelism is one process per GPU + NCCL gradient all-reduce instead of
+edges: data-parallelism is one process per GPU + NCCL gradient all-reduce instead of
 ``nn.DataParallel`` (train.py:220-228); the criterion / optimizer are the fused CUDA kernels; ``verbose=`` is not
 passed to ReduceLROnPlateau; a missing ``resize_size`` defaults to image_size/0.875; ``train()`` re-raises.
 The JPEG input pipeline (dataset/*) is out of scope: pass ``dataloaders=`` or run inside a Hawkeye checkout

@@ -1,7 +1,7 @@
-/* hawkeye_b200 — C ABI of the B200-native high-order-pooling hot path.
+/* hawkeye_b200 — C ABI of the H100-native high-order-pooling hot path.
  *
  * One shared library (hawkeye_b200/libhawkeye_b200.so), plain C types, no torch types.
- * Conventions (SURVEY.md §8(b)):
+ * Conventions:
  *   - return 0 = success; <0 = argument/shape/alignment error, nothing was launched;
  *     >0 = cudaError_t from a launch.  hk_last_error() gives the text (thread-local).
  *   - the caller owns every device buffer including workspaces (query *_workspace_bytes);
@@ -27,7 +27,7 @@ long long hk_launch_count(void);      /* kernels launched by this library on the
 void hk_reset_launch_count(void);
 
 /* ---- precision mode (process-wide; default 0, or $HK_PRECISE at first use) ---------------------------------------
- * 0: single-pass TF32 tensor-core products (tcgen05 kind::tf32 keeps 10 mantissa bits of each operand); every kernel
+ * 0: single-pass TF32 tensor-core products (the tf32 tensor-core MMA keeps 10 mantissa bits of each operand); every kernel
  *    that produces an operand of a later MMA rounds it to tf32 on store (round-to-nearest), so outputs of
  *    hk_conv3x3_*, hk_bn_*, hk_bilinear_pool_fwd, hk_cbp_fwd carry a 2^-11 relative quantisation.  Meets the 1e-3
  *    forward tolerance of the path; gradients below ReLU / max-pool kinks then differ from an fp32 run by branch
@@ -38,7 +38,7 @@ void hk_reset_launch_count(void);
 void hk_set_precise(int on);
 int hk_get_precise(void);
 
-/* ---- generic batched TF32 tensor-core GEMM (tcgen05 + TMA) -------------------------------------
+/* ---- generic batched TF32 tensor-core GEMM (wgmma + TMA) -------------------------------------
  * C[b] = alpha*alpha_vec[b] * A[b].B[b] + diag*I + beta*beta_vec[b] * D[b]   (ReLU optional; C optionally transposed)
  * A logical [M,K]: a_mn_major=0 -> A[m*lda+k]; 1 -> A[k*lda+m].   B logical [K,N]: b_mn_major=0 -> B[n*ldb+k]; 1 -> B[k*ldb+n].
  * Replaces torch.bmm call sites model/methods/MPNCOV.py:117,132,154-160,178-194 and 1x1 convs resnet.py:34-37. */
@@ -83,7 +83,7 @@ int hk_cbp_bwd(const float* x, const float* pre, const float* dy, const int* h1,
  * Covpool (:105-134): x [B,C,M] -> cov [B,C,C] = X I_hat X^T; xc [B,C,ceil4(M)] receives the centred features at a 16-byte row
  *   pitch (saved for bwd; equal to [B,C,M] whenever M % 4 == 0).
  * Sqrtm (:137-202): coupled Newton-Schulz, iterN >= 2, forward and the reference's hand-derived backward formulae,
- *   all products as 3xTF32 tcgen05 GEMMs.  `saved` (hk_sqrtm_saved_floats floats) carries A, Y_i, Z_i, normA.
+ *   all products as 3xTF32 wgmma GEMMs.  `saved` (hk_sqrtm_saved_floats floats) carries A, Y_i, Z_i, normA.
  * Triuvec (:205-230): row-major upper triangle [B,n,n] <-> [B,n(n+1)/2]. */
 int hk_covpool_fwd(const float* x, float* cov, float* xc, int B, int C, int M, void* stream);
 int hk_covpool_bwd(const float* xc, const float* g, float* dx, int B, int C, int M, void* stream);
@@ -101,7 +101,7 @@ int hk_triuvec_bwd(const float* g, float* dx, int B, int n, void* stream);
  * Activations are NHWC fp32 inside the backbone.  Weights keep the reference layout [Cout,Cin,3,3] in the
  * state_dict and are re-packed per step: w_fwd [9][Cout][Cin], w_dgrad [9][Cin][Cout] (taps flipped). */
 int hk_conv3x3_pack_weights(const float* w, float* w_fwd, float* w_dgrad, int Cout, int Cin, void* stream);
-/* y = relu?(conv3x3(x, w) + bias): implicit GEMM on tcgen05, TMA zero-fill = padding.  Cin%32==0, Cout%32==0. */
+/* y = relu?(conv3x3(x, w) + bias): implicit GEMM on wgmma, TMA zero-fill = padding.  Cin%32==0, Cout%32==0. */
 int hk_conv3x3_fwd(const float* x_nhwc, const float* w_fwd_packed, const float* bias, float* y_nhwc, int N, int H,
                    int W, int Cin, int Cout, int relu, void* stream);
 /* relu(conv3x3(x, w) + bias) followed by MaxPool2d(2,2) (vgg.py:59-68: every pool of VGG-16 follows a conv + ReLU) in ONE
@@ -149,7 +149,7 @@ int hk_maxpool2x2_bwd_idx(const unsigned char* code, const float* dy, float* dx_
 int hk_relu_mask_inplace(float* dy, const float* act, size_t n, void* stream);
 
 /* ---- ResNet-50 v1.5 trunk support (model/backbone/resnet.py:89-252); activations NHWC [P = N*H*W, C] -----------------
- * stem 7x7/s2/p3 (resnet.py:176): patches X147 [P][160] (+ packed weights [64][160]) feed one tcgen05 GEMM. */
+ * stem 7x7/s2/p3 (resnet.py:176): patches X147 [P][160] (+ packed weights [64][160]) feed one wgmma GEMM. */
 int hk_stem_im2col(const float* x_nchw, float* x147, int N, int H, int W, void* stream);
 int hk_pack_stem_weights(const float* w, float* w147, int Cout, void* stream);
 /* nn.BatchNorm2d in train mode (batch statistics, running stats updated with momentum, eps inside the sqrt):
@@ -187,7 +187,7 @@ size_t hk_matconv_wgrad_workspace_bytes(long long P, int K, int Cout);
 int hk_matconv_wgrad(const float* x, const float* dy, float* dw, long long P, int K, int Cout, void* workspace,
                      size_t workspace_bytes, void* stream);
 
-/* ---- channel interaction (SURVEY 8(f) N1): model/methods/CIN.py:24-60, ChannelInteractionModule ---------------------
+/* ---- channel interaction: model/methods/CIN.py:24-60, ChannelInteractionModule ---------------------
  * The Gram (:31), W.X (:34,:55), the 3x3 conv (:36,:57) and fc (:47-48) use hk_gemm_tf32 / hk_conv3x3_* / hk_linear_*; these are
  * the pieces in between: W_SCI = softmax(-G) row-wise (:32) and its backward; W_CCI = |W_SCI - weight_b * W_SCI[(b+B/2)%B]|
  * (:50-53; `per` = C*C elements per sample, B even) and its backward (d_sci, d_weight [B]); AdaptiveAvgPool1d(1) (:71) as a
@@ -200,7 +200,7 @@ int hk_cci_weight_bwd(const float* w_sci, const float* weight, const float* d_cc
 int hk_row_mean_fwd(const float* x, float* y, long long rows, int cols, int ld, void* stream);
 int hk_row_mean_bwd(const float* dy, float* dx, long long rows, int cols, int ld, void* stream);
 
-/* ---- OSME excitation (SURVEY 8(f) N3, model/methods/OSME.py:8-24): s = sigmoid(m)[n,c] * x[n,c,:] and its backward; the
+/* ---- OSME excitation: s = sigmoid(m)[n,c] * x[n,c,:] and its backward; the
  * squeeze (AdaptiveAvgPool2d) is hk_row_mean_*, the two Linear layers are hk_linear_*, ReLU on the bottleneck hk_relu_* */
 int hk_se_gate_fwd(const float* x, const float* m, float* s, long long rows, int hw, void* stream);
 int hk_se_gate_bwd(const float* x, const float* m, const float* ds, float* dx, float* dm, long long rows, int hw,
@@ -217,7 +217,7 @@ int hk_npair_loss(const float* prod, const int* cls, const int* part, double* lo
 int hk_relu_fwd(const float* x, float* y, size_t n, void* stream);
 int hk_relu_bwd(const float* y, const float* dy, float* dx, size_t n, void* stream);
 
-/* ---- classifier nn.Linear (BCNN.py:42, CBCNN.py:26, MPNCOV.py:31) as skinny tcgen05 GEMMs ------------------- */
+/* ---- classifier nn.Linear (BCNN.py:42, CBCNN.py:26, MPNCOV.py:31) as skinny wgmma GEMMs ------------------- */
 size_t hk_linear_fwd_workspace_bytes(int B, int F, int N);
 int hk_linear_fwd(const float* x, const float* w, const float* bias, float* y, int B, int F, int N, void* workspace,
                   size_t workspace_bytes, void* stream);
@@ -231,7 +231,7 @@ int hk_linear_wgrad(const float* dy, const float* x, float* dw, float* db, int B
 int hk_softmax_ce_ls(const float* logits, const long long* labels, float* loss, float* dlogits, int* correct, int B,
                      int K, float label_smoothing, float grad_scale, void* stream);
 
-/* ---- input side (SURVEY 8(f) N4): transforms.ToTensor + Normalize (dataset/transforms.py:14-19, test.py:80-85) fused on
+/* ---- input side: transforms.ToTensor + Normalize (dataset/transforms.py:14-19, test.py:80-85) fused on
  * the GPU: uint8 HWC batch [N,H,W,3] -> fp32 NCHW (x/255 - mean_c)/std_c; a quarter of the float pipeline's H2D bytes */
 int hk_normalize_u8(const unsigned char* x_nhwc, float* y_nchw, int N, int H, int W, float mean0, float mean1, float mean2,
                     float std0, float std1, float std2, void* stream);

@@ -5,9 +5,9 @@ This is the parity ORACLE, not product code.  Only ``tests/``,
 legs may import it; nothing under ``hawkeye_b200/`` does, and the product fails
 loudly when its CUDA library is missing rather than routing here.
 
-Pinning: the reference ships no tests or golden vectors (SURVEY.md §4), so the
+Pinning: the reference ships no tests or golden vectors, so the
 oracle is pinned by (a) ``tests/golden/*.npz`` — outputs of the UNMODIFIED
-reference modules imported from /root/reference by ``tests/golden/make_golden.py``
+reference modules imported through oracle/ref_harness by ``tests/golden/make_golden.py``
 — and (b) the numpy-RNG known answers for the count-sketch hashes
 (``tests/test_oracle.py``).  Every function cites the reference lines it restates.
 All arithmetic is numpy / torch-CPU; ``dtype`` selects fp32 (the reference's
@@ -163,7 +163,7 @@ def cbp_fwd(x, output_dim, hashes=None, nl=Plain):
 
 
 def cbp_presqrt_gram_scatter(x, output_dim, hashes=None):
-    """Identity cross-check (SURVEY §8c): sum_p ifft(fft(xS1)*fft(xS2)) ==
+    """Identity cross-check: sum_p ifft(fft(xS1)*fft(xS2)) ==
     signed scatter of the un-normalised Gram  X X^T  into bins (h1[i]+h2[j]) mod d."""
     B, C, H, W = x.shape
     h1, s1, h2, s2 = hashes if hashes is not None else cbp_hashes(C, output_dim)
@@ -339,7 +339,7 @@ def vgg_cfg_scaled(width_div=1):
 
 
 def vgg_state_keys(cfg=VGG16_D):
-    """Sequential indices of the conv layers: backbone.{0,2,5,...}.{weight,bias} (SURVEY §5)."""
+    """Sequential indices of the conv layers: backbone.{0,2,5,...}.{weight,bias}."""
     keys, idx = [], 0
     for v in cfg:
         if v == 'M':

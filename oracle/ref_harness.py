@@ -3,7 +3,7 @@
 Only tests/, tests/golden/make_golden.py and bench.py's cpu_baseline leg may
 import this module.  Nothing under hawkeye_b200/ imports it.
 
-Reference root resolution: $HAWKEYE_REF, then baseline/_ref, then /root/reference.
+Reference root resolution: $HAWKEYE_REF, then baseline/_ref.
 The yacs / tensorboardX stand-ins under oracle/_shims are used only when the real
 packages fail to import.  ``pretrained=True`` is hard-coded in the reference
 (model/methods/BCNN.py:38, CBCNN.py:21, MPNCOV.py:28) and would hit the network
@@ -18,7 +18,7 @@ _REPO = os.path.dirname(_HERE)
 
 
 def find_reference_root():
-    for cand in (os.environ.get("HAWKEYE_REF"), os.path.join(_REPO, "baseline", "_ref"), "/root/reference"):
+    for cand in (os.environ.get("HAWKEYE_REF"), os.path.join(_REPO, "baseline", "_ref")):
         if cand and os.path.isfile(os.path.join(cand, "model", "methods", "BCNN.py")):
             return cand
     return None

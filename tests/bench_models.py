@@ -1,4 +1,4 @@
-"""Throughput of the other BASELINE configs (parity-test cases, not the bench line): CBCNN VGG-16 d=8192 and
+"""Throughput of the other benchmark configs (parity-test cases, not the bench line): CBCNN VGG-16 d=8192 and
 Fast MPN-COV ResNet-50 at 448x448, batch 32, one GPU: fwd + CE + bwd + SGD, device-timed."""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,7 +1,7 @@
-"""Generate golden fixtures by running the UNMODIFIED reference (imported from /root/reference).
+"""Generate golden fixtures by running the UNMODIFIED reference (imported through oracle/ref_harness: $HAWKEYE_REF or baseline/_ref).
 
 Run here (authoring container) only:  python tests/golden/make_golden.py
-The GPU box has no /root/reference; tests read the committed .npz files.
+Machines without the reference tree run the tests from the committed .npz files.
 Inputs are regenerated from tests/detgen.py seeds, so fixtures carry outputs only.
 """
 import hashlib
@@ -15,6 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, REPO)
 sys.path.insert(0, os.path.join(REPO, 'tests'))
+from conftest import save_golden  # noqa: E402
 
 from oracle import ref_harness as rh  # noqa: E402
 import detgen  # noqa: E402
@@ -126,5 +127,5 @@ out['cbcnn_loss'] = np.float32(loss.item())
 out['cbcnn_g_backbone.28.bias'] = net.backbone[28].bias.grad.numpy()
 out['cbcnn_g_backbone.0.bias'] = net.backbone[0].bias.grad.numpy()
 
-np.savez_compressed(os.path.join(HERE, 'reference_outputs.npz'), **out)
-print('wrote', len(out), 'arrays;', os.path.getsize(os.path.join(HERE, 'reference_outputs.npz')) / 1e6, 'MB')
+save_golden('reference_outputs', out)                 # parts of under 1 MB: tests/golden/reference_outputs.<i>.npz
+print('wrote', len(out), 'arrays')

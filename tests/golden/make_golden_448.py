@@ -1,5 +1,5 @@
-"""Golden fixtures at the BASELINE configuration (448x448, batch 2, 200 classes; BASELINE.json configs[0..3]) from the
-UNMODIFIED reference: BCNN stage 1/2, CBCNN d=8192 and d=6000, MPN.  Run here only (needs /root/reference):
+"""Golden fixtures at the benchmark configuration (448x448, batch 2, 200 classes; the benchmark configurations) from the
+UNMODIFIED reference: BCNN stage 1/2, CBCNN d=8192 and d=6000, MPN.  Needs the reference tree ($HAWKEYE_REF or baseline/_ref):
     python tests/golden/make_golden_448.py   -> tests/golden/reference_448.npz
     HK_GOLDEN_SIZE=224 python tests/golden/make_golden_448.py   -> tests/golden/reference_224.npz
 Inputs and weights are regenerated from tests/detgen.py seeds by the tests; the fixture carries outputs only:

@@ -1,5 +1,5 @@
-"""Golden fixtures for the channel-interaction row (SURVEY 8(f) N1) from the UNMODIFIED reference (model/methods/CIN.py).
-Run here only:  python tests/golden/make_golden_cin.py  -> tests/golden/reference_cin.npz
+"""Golden fixtures for the channel-interaction row from the UNMODIFIED reference (model/methods/CIN.py).
+Run here only:  python tests/golden/make_golden_cin.py  -> tests/golden/reference_cin.<i>.npz
 Weights come from detgen.state_like(module) and inputs from detgen seeds, so the fixture carries outputs only."""
 import json
 import os
@@ -12,6 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, REPO)
 sys.path.insert(0, os.path.join(REPO, 'tests'))
+from conftest import save_golden  # noqa: E402
 from oracle import ref_harness as rh  # noqa: E402
 import detgen  # noqa: E402
 
@@ -56,10 +57,10 @@ out['full_z_sum'] = np.float64(z.double().sum().item())
 out['full_logits'] = logits.numpy()
 net = MODEL.get('CIN')(rh.cfg(name='CIN', num_classes=200))
 out['cin_state_keys_json'] = np.frombuffer(json.dumps({k: list(v.shape) for k, v in net.state_dict().items()}, sort_keys=True).encode(), dtype=np.uint8)
-np.savez_compressed(os.path.join(HERE, 'reference_cin.npz'), **out)
-print('wrote', len(out), 'arrays;', os.path.getsize(os.path.join(HERE, 'reference_cin.npz')) / 1e6, 'MB')
+save_golden('reference_cin', out)                 # parts of under 1 MB: tests/golden/reference_cin.<i>.npz
+print('wrote', len(out), 'arrays')
 
-# ---- OSME (SURVEY 8(f) N3, model/methods/OSME.py:8-64): the excitation module on its own + the OSMENet key list -----------
+# ---- OSME: the excitation module on its own + the OSMENet key list -----------
 from model.methods.OSME import OSME  # noqa: E402
 
 for tag, C, shape, B in (('osme_c256_7', 256, 7, 4), ('osme_c128_14', 128, (14, 14), 2)):
@@ -76,10 +77,10 @@ for tag, C, shape, B in (('osme_c256_7', 256, 7, 4), ('osme_c128_14', 128, (14, 
         out[f'{tag}_g_{k}'] = g if g.size <= 65536 else g.reshape(g.shape[0], -1)[:, ::29]
 net = MODEL.get('OSMENet')(rh.cfg(name='OSMENet', num_attention=2, num_classes=200))
 out['osme_state_keys_json'] = np.frombuffer(json.dumps({k: list(v.shape) for k, v in net.state_dict().items()}, sort_keys=True).encode(), dtype=np.uint8)
-np.savez_compressed(os.path.join(HERE, 'reference_cin.npz'), **out)
-print('wrote', len(out), 'arrays (with OSME);', os.path.getsize(os.path.join(HERE, 'reference_cin.npz')) / 1e6, 'MB')
+save_golden('reference_cin', out)                 # parts of under 1 MB: tests/golden/reference_cin.<i>.npz
+print('wrote', len(out), 'arrays (with OSME)')
 
-# ---- MAMC / N-pairs loss (SURVEY 8(f) N3, model/loss/MAMC_loss.py:6-90): the criterion of OSMENet ---------------------------
+# ---- MAMC / N-pairs loss: the criterion of OSMENet ---------------------------
 from model.loss.MAMC_loss import MAMCLoss, NPairsLoss  # noqa: E402
 
 for tag, b, p, D, ncls in (('npair_b8_p2', 8, 2, 64, 3), ('npair_b12_p3', 12, 3, 32, 4), ('npair_b6_p2_allsame', 6, 2, 16, 1),
@@ -98,5 +99,5 @@ loss = crit((pred, parts), lab)
 loss.backward()
 out['mamc_pred'], out['mamc_parts'], out['mamc_labels'] = pred.detach().numpy(), parts.detach().numpy(), lab.numpy()
 out['mamc_loss'], out['mamc_dpred'], out['mamc_dparts'] = np.float64(loss.item()), pred.grad.numpy(), parts.grad.numpy()
-np.savez_compressed(os.path.join(HERE, 'reference_cin.npz'), **out)
-print('wrote', len(out), 'arrays (with OSME + MAMC);', os.path.getsize(os.path.join(HERE, 'reference_cin.npz')) / 1e6, 'MB')
+save_golden('reference_cin', out)                 # parts of under 1 MB: tests/golden/reference_cin.<i>.npz
+print('wrote', len(out), 'arrays (with OSME + MAMC)')

@@ -23,8 +23,8 @@ def test_reference_arm_json_line():
     assert d['value'] > 0 and d['e2e']['value'] == d['value']
     assert d['e2e']['h2d_bytes_per_step'] == 0 and d['e2e']['d2h_bytes_per_step'] == 0
     cb = d['cpu_baseline']
-    import os as _os
-    want = 'reference' if _os.path.isdir('/root/reference') or _os.path.isdir(_os.path.join(REPO, 'baseline', '_ref')) else 'port'
+    from oracle import ref_harness as rh
+    want = 'reference' if rh.available() else 'port'
     assert cb['kind'] == want and cb['cores'] >= 1 and cb['value'] == d['value'] and 'sample' in cb
     assert d['steps'] == 1 and d['steps_requested'] == 1           # the line reports the steps it actually timed
     assert 'workload' in d['config'] and 'model' not in d['config']

@@ -14,7 +14,7 @@ def test_library_exports_every_declared_symbol():
     missing = [n for n in protos if not hasattr(lib, n)]
     assert not missing, missing
     lib.hk_version.restype = ctypes.c_char_p
-    assert b'hawkeye_b200' in lib.hk_version() and b'sm_100a' in lib.hk_version()
+    assert b'hawkeye_b200' in lib.hk_version() and b'sm_90a' in lib.hk_version()
 
 
 def test_no_fallback_when_library_missing(monkeypatch, tmp_path):

@@ -1,10 +1,12 @@
-"""CIN registry surface (SURVEY 8(f) N1) on CPU: state_dict keys / shapes identical to the reference's MODEL['CIN']."""
+"""CIN registry surface on CPU: state_dict keys / shapes identical to the reference's MODEL['CIN']."""
 import json
 import os
 
 import numpy as np
 
-G = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'reference_cin.npz'))
+from conftest import load_golden  # noqa: E402
+
+G = load_golden('reference_cin')
 
 
 class Cfg(dict):

@@ -1,5 +1,5 @@
 """The shipped yamls load through hawkeye_b200.config (yacs-compatible CfgNode) and build their models through the registry
-with the parameter counts of the reference models (SURVEY §8a: BCNN 67 143 688, MPN 30 612 232)."""
+with the parameter counts of the reference models."""
 import os
 
 import pytest

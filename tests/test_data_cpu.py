@@ -1,6 +1,6 @@
 """hawkeye_b200.data — the mirror of the reference's dataset package (dataset/dataset.py, transforms.py:14-73, sampler.py) — on a
-generated image folder: item format, the deterministic eval preset, class-balanced batches; and, when the reference tree is
-importable (here: /root/reference), item-for-item / batch-for-batch equality with the reference's own classes."""
+generated image folder: item format, the deterministic eval preset, class-balanced batches; and item-for-item / batch-for-batch
+equality with the reference's own classes (recorded outputs)."""
 import os
 import sys
 
@@ -55,40 +55,36 @@ def test_balanced_batches(folder):
         assert len(cls) == 2 and (cnt == 3).all()                               # what MAMCLoss needs
 
 
-def _reference_dataset_modules():
-    from oracle import ref_harness as rh
-    if not rh.available():
-        pytest.skip('reference tree not importable')
-    root = rh.find_reference_root()
-    if root not in sys.path:
-        sys.path.insert(0, root)
-    import importlib
-    return (importlib.import_module('dataset.dataset'), importlib.import_module('dataset.transforms'),
-            importlib.import_module('dataset.sampler'))
+REFERENCE_DATA = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'reference_data.npz')
+
+
+def reference_data_outputs(root, meta, rd, rt, rs):
+    """What the reference's dataset classes return on the generated folder: eval items 0 / 7 / 23, one train-preset draw
+    (torch / python RNG seeded 11) and the class-balanced batches (numpy RNG seeded 5).  `rd, rt, rs` are its
+    dataset.dataset, dataset.transforms and dataset.sampler modules — or ours, which must give the same."""
+    import random
+    out = {}
+    ds = rd.FGDataset(root, meta, transform=rt.ClassificationPresetEval(crop_size=32, resize_size=36))
+    out['len'] = np.array(len(ds))
+    for i in (0, 7, 23):
+        it = ds[i]
+        out[f'img_{i}'], out[f'label_{i}'] = it['img'].numpy(), np.array(int(it['label']))
+    tr = rt.ClassificationPresetTrain(32, auto_augment_policy='ta_wide', random_erase_prob=0.1)
+    img = D.default_loader(os.path.join(root, 'c1/img_5.png'))
+    torch.manual_seed(11); random.seed(11)
+    out['train_draw'] = tr(img).numpy()
+    np.random.seed(5)
+    out['batches'] = np.array([list(map(int, b)) for b in rs.BalancedBatchSampler(ds, 2, 3)])
+    return out
 
 
 def test_matches_reference_classes(folder):
-    rd, rt, rs = _reference_dataset_modules()
+    """Item-for-item / batch-for-batch equality with the reference's own classes, recorded in
+    tests/golden/reference_data.npz by running reference_data_outputs on the reference's modules."""
     root, meta = folder
-    ours = D.FGDataset(root, meta, transform=D.ClassificationPresetEval(crop_size=32, resize_size=36))
-    ref = rd.FGDataset(root, meta, transform=rt.ClassificationPresetEval(crop_size=32, resize_size=36))
-    assert len(ours) == len(ref)
-    for i in (0, 7, 23):
-        a, b = ours[i], ref[i]
-        assert int(a['label']) == int(b['label']) and torch.equal(a['img'], b['img'])
-    # train preset: same transform pipeline => same draws from the same torch / python RNG state
-    import random
-    to, tr = D.ClassificationPresetTrain(32, auto_augment_policy='ta_wide', random_erase_prob=0.1), \
-        rt.ClassificationPresetTrain(32, auto_augment_policy='ta_wide', random_erase_prob=0.1)
-    img = D.default_loader(os.path.join(root, 'c1/img_5.png'))
-    torch.manual_seed(11); random.seed(11)
-    x = to(img)
-    torch.manual_seed(11); random.seed(11)
-    y = tr(img)
-    assert torch.equal(x, y)
-    # sampler: same numpy call order => same batches
-    np.random.seed(5)
-    b1 = [list(map(int, b)) for b in D.BalancedBatchSampler(ours, 2, 3)]
-    np.random.seed(5)
-    b2 = [list(map(int, b)) for b in rs.BalancedBatchSampler(ref, 2, 3)]
-    assert b1 == b2 and len(b1) > 0
+    want = np.load(REFERENCE_DATA)
+    got = reference_data_outputs(root, meta, D, D, D)
+    assert sorted(got) == sorted(want.files)
+    for k in got:
+        assert got[k].shape == want[k].shape and np.array_equal(got[k], want[k]), k
+    assert len(got['batches']) > 0

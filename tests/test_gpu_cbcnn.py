@@ -37,7 +37,7 @@ def test_cbp_golden(golden, d):
     eb = rel_l2(dx.cpu()[..., :3], golden[f'cbp_dx_{d}'])
     print(f'cbp d={d}: fwd {e:.2e} bwd {eb:.2e} (arbitrary fp32 inputs: operands are truncated to tf32)')
     assert e < 1e-3
-    # The signed-sqrt gradient 1/(2 sqrt(|v|+1e-10)) is ill-conditioned near empty bins (SURVEY §7.3): with arbitrary
+    # The signed-sqrt gradient 1/(2 sqrt(|v|+1e-10)) is ill-conditioned near empty bins: with arbitrary
     # fp32 inputs the tf32 operand truncation perturbs near-zero bins and their gradients by O(1), so dX is only
     # compared in direction here ...
     a, b = dx.cpu()[..., :3].double().flatten(), torch.as_tensor(golden[f'cbp_dx_{d}']).double().flatten()

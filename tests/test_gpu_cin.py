@@ -1,4 +1,4 @@
-"""ChannelInteractionModule / CINClassifier (SURVEY 8(f) N1) against fixtures from the UNMODIFIED reference
+"""ChannelInteractionModule / CINClassifier against fixtures from the UNMODIFIED reference
 (tests/golden/make_golden_cin.py): outputs in train and eval mode, input and parameter gradients, the 7x7 (WH = 49, padded
 to 52 columns) case, and the full-size C = 2048, 14x14 forward."""
 import os
@@ -8,10 +8,10 @@ import pytest
 import torch
 
 import detgen
-from conftest import rel_l2
+from conftest import load_golden, rel_l2
 
 pytestmark = pytest.mark.gpu
-G = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'reference_cin.npz'))
+G = load_golden('reference_cin')
 
 
 @pytest.mark.parametrize('precise', [0, 1])
@@ -74,7 +74,7 @@ def test_cin_full_size_forward(precise):
 @pytest.mark.parametrize('precise', [0, 1])
 @pytest.mark.parametrize('tag,C,shape,B', [('osme_c256_7', 256, 7, 4), ('osme_c128_14', 128, (14, 14), 2)])
 def test_osme_module(tag, C, shape, B, precise):
-    """OSME (SURVEY 8(f) N3, OSME.py:8-46) against the reference: summed / per-attention features, input and all parameter grads."""
+    """OSME against the reference: summed / per-attention features, input and all parameter grads."""
     from hawkeye_b200 import _lib
     from hawkeye_b200.methods.osme import OSME
     m = OSME(C, 64, feature_shape=shape, num_attention=2)

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM core (descriptor / swizzle / major-ness validation) vs fp64 matmul.  GPU only."""
+"""wgmma GEMM core (descriptor / swizzle / major-ness validation) vs fp64 matmul.  GPU only."""
 import pytest
 import torch
 

@@ -6,10 +6,10 @@ import numpy as np
 import pytest
 import torch
 
-from conftest import rel_l2
+from conftest import load_golden, rel_l2
 
 pytestmark = pytest.mark.gpu
-G = np.load(os.path.join(os.path.dirname(__file__), 'golden', 'reference_cin.npz'))
+G = load_golden('reference_cin')
 
 
 @pytest.mark.parametrize('tag', ['npair_b8_p2', 'npair_b12_p3', 'npair_b6_p2_allsame', 'npair_b4_p2_alldiff'])

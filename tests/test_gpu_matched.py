@@ -1,4 +1,4 @@
-"""Gradient parity of the three models, EVERY parameter, including the BASELINE 448x448 / batch-2 configuration.
+"""Gradient parity of the three models, EVERY parameter, including the benchmark 448x448 / batch-2 configuration.
 
 Two complementary checks (tests/matched.py explains why a plain comparison cannot work for a TF32 forward):
   * matched-activation: the fp64 oracle is evaluated on the branch (ReLU masks, pool arg-maxes, signed-sqrt bins) the GPU
@@ -109,8 +109,8 @@ def test_cbcnn_all_gradients(size, d, precision):
 @pytest.mark.parametrize('precision', [1], indirect=True)
 @pytest.mark.parametrize('size,B', [(128, 4), (448, 2)])
 def test_mpn_all_gradients(size, B, precision):
-    """A random-weight train-mode ResNet-50 amplifies a perturbation of its input ~170x by the last block (measured in fp64,
-    DESIGN.md section 2), so single-pass TF32 (5e-4 per layer) cannot track ANY reference run of it; the 3xTF32 mode can.
+    """A random-weight train-mode ResNet-50 amplifies a perturbation of its input ~170x by the last block (measured in fp64),
+    so single-pass TF32 (5e-4 per layer) cannot track ANY reference run of it; the 3xTF32 mode can.
     fp32 itself is only reproducible to ~2e-4 here (fp32 vs fp64 oracle on the same branch), hence the looser bound."""
     from oracle import hop_oracle as O
     torch.set_num_threads(16)
@@ -127,7 +127,7 @@ def test_mpn_all_gradients(size, B, precision):
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# precise mode vs the UNMODIFIED reference at the BASELINE configuration (fixtures: tests/golden/make_golden_448.py)
+# precise mode vs the UNMODIFIED reference at the benchmark configuration (fixtures: tests/golden/make_golden_448.py)
 # ------------------------------------------------------------------------------------------------------------------
 def _slice_like(g, k, ref):
     """apply the fixture's slicing rule to a full gradient"""

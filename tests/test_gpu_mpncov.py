@@ -25,7 +25,7 @@ def test_mpncov_golden(golden, tag, shape, it):
 
 
 def test_sqrtm_chain_vs_oracle_fp64():
-    """Sqrtm alone on an SPD batch at BASELINE size (B=4, 256x256, iterN=5): 3xTF32 keeps the 12-GEMM chain at
+    """Sqrtm alone on an SPD batch at benchmark size (B=4, 256x256, iterN=5): 3xTF32 keeps the 12-GEMM chain at
     fp32-class accuracy; backward follows the reference formulae (incl. the transpose and diagonal term)."""
     from hawkeye_b200 import ops
     from oracle import hop_oracle as O

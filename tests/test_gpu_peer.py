@@ -1,4 +1,4 @@
-"""PeerLearningNet (SURVEY 8(f) N2) on the GPU: the two-model train step of Examples/PeerLearning.py:82-91 through
+"""PeerLearningNet on the GPU: the two-model train step of Examples/PeerLearning.py:82-91 through
 PeerLearningTrainer.batch_training against fixtures from the UNMODIFIED reference (tests/golden/make_golden_peer.py), and the
 bilinear-pool kernel under concurrent streams (no co-residency assumption, VERDICT r1 weak #11)."""
 import os

@@ -1,4 +1,4 @@
-"""Evaluation entry point (SURVEY 8(f) N4): hawkeye_b200.test.Tester over a synthetic loader, fp32 and uint8 batches."""
+"""Evaluation entry point: hawkeye_b200.test.Tester over a synthetic loader, fp32 and uint8 batches."""
 import os
 
 import pytest

@@ -8,7 +8,9 @@ import torch
 
 from oracle import hop_oracle as O
 
-G = np.load(os.path.join(os.path.dirname(__file__), 'golden', 'reference_cin.npz'))
+from conftest import load_golden  # noqa: E402
+
+G = load_golden('reference_cin')
 TAGS = ['npair_b8_p2', 'npair_b12_p3', 'npair_b6_p2_allsame', 'npair_b4_p2_alldiff']
 
 

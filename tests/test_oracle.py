@@ -1,6 +1,6 @@
 """Pin the oracle restatement (oracle/hop_oracle.py) against outputs of the UNMODIFIED reference
 (tests/golden/reference_outputs.npz, made by tests/golden/make_golden.py) and the numpy-RNG
-known answers from SURVEY.md §8(c).  CPU only."""
+known answers of the reference streams.  CPU only."""
 import hashlib
 
 import numpy as np
@@ -12,7 +12,7 @@ from oracle import hop_oracle as O
 
 
 def test_cbp_hash_known_answers(golden):
-    # SURVEY §8(c) known answers (numpy legacy RNG, seeds 1/3/5/7 — CBCNN.py:76-91): bit-exact
+    # Known answers (numpy legacy RNG, seeds 1/3/5/7 — CBCNN.py:76-91): bit-exact
     h1, s1, h2, s2 = O.cbp_hashes(512, 8192)
     assert h1[:8].tolist() == [5157, 235, 3980, 5192, 7935, 905, 2763, 7813]
     assert s1[:8].tolist() == [-1, -1, 1, 1, -1, -1, -1, 1]
@@ -48,7 +48,7 @@ def test_bilinear_pool_matches_reference(golden):
 
 
 def test_bilinear_norm_closed_form():
-    # ||z||^2 = sum_p (sum_c x_cp)^2 / HW + C^2 * 1e-5   (SURVEY §7.3) — what kernel K0 computes
+    # ||z||^2 = sum_p (sum_c x_cp)^2 / HW + C^2 * 1e-5 — what kernel K0 computes
     x = detgen.det_uniform((2, 64, 5, 5), 3).double()
     xf = x.reshape(2, 64, 25)
     z2 = (torch.bmm(xf, xf.transpose(1, 2)) / 25 + 1e-5).reshape(2, -1).sum(1)

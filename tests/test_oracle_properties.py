@@ -1,5 +1,5 @@
 """Size-independent properties of the CPU oracle (oracle/hop_oracle.py) — the same invariants the GPU tests check at the
-BASELINE sizes — plus cross-checks of its hand-written backward formulas against autograd in fp64."""
+benchmark sizes — plus cross-checks of its hand-written backward formulas against autograd in fp64."""
 import numpy as np
 import pytest
 import torch
@@ -16,7 +16,7 @@ def test_bilinear_pool_invariants_and_backward(shape):
     Y = y.view(B, C, C)
     assert torch.allclose(y.norm(dim=1), torch.ones(B, dtype=torch.float64), atol=1e-12)      # F.normalize, BCNN.py:26
     assert torch.allclose(Y, Y.transpose(1, 2), atol=1e-14) and (y > 0).all()                  # Gram symmetry, sqrt(+eps)
-    # hand-derived backward (SURVEY §7.3) == autograd of the forward
+    # hand-derived backward == autograd of the forward
     xg = x.clone().requires_grad_(True)
     dy = detgen.det(y.shape, 4).double()
     (dx_auto,) = torch.autograd.grad(O.bilinear_pool_fwd(xg), xg, dy)
@@ -33,7 +33,7 @@ def test_cbp_fft_path_equals_gram_scatter(d):
     ref = torch.sign(pre) * torch.sqrt(pre.abs() + 1e-10)
     ref = ref / ref.norm(dim=1, keepdim=True).clamp_min(1e-12)
     # empty bins: the FFT path leaves ~1e-14 of round-off where the scatter has an exact 0, and sign(v) sqrt(|v| + 1e-10)
-    # turns that into +-1e-5 before normalisation (the ill-conditioning noted in SURVEY §7.3) — hence the absolute tolerance
+    # turns that into +-1e-5 before normalisation (the ill-conditioning of the signed sqrt) — hence the absolute tolerance
     assert torch.allclose(y.double(), ref, rtol=1e-6, atol=5e-6)
     h1, s1, h2, s2 = hashes
     assert (np.abs(s1) == 1).all() and (np.abs(s2) == 1).all() and h1.min() >= 0 and h1.max() < d and h2.max() < d

@@ -1,4 +1,4 @@
-"""PeerLearningNet (SURVEY §8f N2) against fixtures generated from the unmodified reference
+"""PeerLearningNet against fixtures generated from the unmodified reference
 (tests/golden/make_golden_peer.py): registry surface / state_dict, and the co-teaching loss with its gradients."""
 import json
 import os

@@ -1,4 +1,4 @@
-"""LR schedules of the hot-path methods (SURVEY Appendix C) vs torch's own schedulers, which the reference uses:
+"""LR schedules of the hot-path methods vs torch's own schedulers, which the reference uses:
 LinearLR warm-up -> CosineAnnealingLR via SequentialLR (Examples/CBCNN.py:35-45, Examples/MPN.py:20-30),
 CosineAnnealingLR(T_max, eta_min) (train.py:217-218), ReduceLROnPlateau(mode='max', factor=0.1, patience=3, threshold=1e-4)
 (Examples/BCNN.py:42-48).  Ours drive the fused optimizers' param_groups; the LR sequences must be identical."""
