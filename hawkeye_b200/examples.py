@@ -1,5 +1,5 @@
 """Trainer subclasses of the hot-path methods with the reference's Examples/ surface:
-``python -m hawkeye_b200.examples {BCNN,CBCNN,MPN,PeerLearning,OSMENet} --config <yaml>`` replaces
+``python -m hawkeye_b200.examples {BCNN,CBCNN,MPN,PeerLearning,OSMENet,APINet} --config <yaml>`` replaces
 ``python Examples/<Method>.py --config <yaml>`` (same yaml files; one process per GPU under torchrun instead of nn.DataParallel).
 
 Only what the reference's Examples override is overridden here: which parameters train, with which learning rates, and
@@ -14,6 +14,24 @@ def _warmup_cosine(opt, config, total_epoch):
     return _Cosine(opt, config['T_max'] if 'T_max' in config else total_epoch, 0.0,
                    config['warmup_epochs'] if 'warmup_epochs' in config else 0,
                    config['lr_warmup_decay'] if 'lr_warmup_decay' in config else 0.01)
+
+
+def _balanced_loaders(trainer, config):
+    """The reference's class-balanced training loader (dataset/sampler.py BalancedBatchSampler: n_classes x n_samples images
+    per batch, Examples/OSMENet.py:17-30, Examples/APINet.py:17-29) next to the base Trainer's validation loader."""
+    import numpy as np
+    from torch.utils.data import DataLoader
+    loaders = Trainer.get_dataloader(trainer, config)            # datasets, transforms, validation loader
+    try:
+        from dataset.sampler import BalancedBatchSampler
+    except Exception:
+        from .data import BalancedBatchSampler
+    if trainer.world > 1:                                        # one process per GPU: each rank draws its own balanced batches
+        np.random.seed((trainer.config.experiment.seed if 'seed' in trainer.config.experiment else 0) + trainer.rank)
+    sampler = BalancedBatchSampler(trainer.datasets['train'], config.n_classes, config.n_samples)
+    loaders['train'] = DataLoader(trainer.datasets['train'], num_workers=config.num_workers, pin_memory=True,
+                                  batch_sampler=sampler)
+    return loaders
 
 
 class BCNNTrainer(Trainer):
@@ -62,19 +80,7 @@ class OSMENetTrainer(Trainer):
 
     def get_dataloader(self, config):
         """Examples/OSMENet.py:17-30: the training loader draws class-balanced batches (n_classes x n_samples images)."""
-        import numpy as np
-        from torch.utils.data import DataLoader
-        loaders = super().get_dataloader(config)                 # datasets, transforms, validation loader
-        try:
-            from dataset.sampler import BalancedBatchSampler
-        except Exception:
-            from .data import BalancedBatchSampler
-        if self.world > 1:                                       # one process per GPU: each rank draws its own balanced batches
-            np.random.seed((self.config.experiment.seed if 'seed' in self.config.experiment else 0) + self.rank)
-        sampler = BalancedBatchSampler(self.datasets['train'], config.n_classes, config.n_samples)
-        loaders['train'] = DataLoader(self.datasets['train'], num_workers=config.num_workers, pin_memory=True,
-                                      batch_sampler=sampler)
-        return loaders
+        return _balanced_loaders(self, config)
 
     def get_criterion(self, config):
         from .losses import MAMCLoss
@@ -100,16 +106,66 @@ class OSMENetTrainer(Trainer):
         self.average_meters['acc'].update(accuracy(pred, labels, 1), images.size(0))
 
 
+class _FrozenWarmupCosine(_Cosine):
+    """_Cosine with the first ``frozen`` parameter groups at lr 0 until the warm-up ends.  That is what the reference's
+    Examples/APINet.py gets from torch: on_start_epoch sets group 0's lr to 0 at epoch 0, LinearLR's multiplicative warm-up
+    keeps it there, and at the milestone SequentialLR restarts CosineAnnealingLR from the initial lr, where both groups meet."""
+
+    def __init__(self, opt, T_max, eta_min=0.0, warmup_epochs=0, warmup_decay=0.01, frozen=1):
+        self.frozen = frozen
+        super().__init__(opt, T_max, eta_min, warmup_epochs, warmup_decay)
+
+    def _apply(self):
+        super()._apply()
+        if self.e < self.w:
+            for g in self.opt.param_groups[:self.frozen]:
+                g['lr'] = 0.0
+
+
+class APINetTrainer(Trainer):
+    """Examples/APINet.py: class-balanced batches (n_classes x n_samples images); the model takes the labels and returns
+    (self_logits, other_logits, labels1, labels2); criterion = APINetLoss (cross-entropy + margin ranking); Adam with two
+    groups — backbone and the rest — at config.lr; linear warm-up into cosine annealing, with the backbone frozen through lr = 0
+    (not requires_grad, so Adam's moments and the BN running statistics evolve as in the reference) for the warm-up epochs.
+    The meters count 8n logit rows for the accuracy and 4n for the loss, as Examples/APINet.py:74-77 does."""
+
+    def get_dataloader(self, config):
+        return _balanced_loaders(self, config)
+
+    def get_criterion(self, config):
+        from .losses import APINetLoss
+        return APINetLoss(config)
+
+    def param_groups(self):
+        m = self.get_model_module()
+        backbone = {id(p) for p in m.backbone.parameters()}
+        return [(list(m.backbone.parameters()), 1.0), ([p for p in m.parameters() if id(p) not in backbone], 1.0)]
+
+    def get_scheduler(self, config):
+        return _FrozenWarmupCosine(self.optimizer, config['T_max'] if 'T_max' in config else self.total_epoch, 0.0,
+                                   config['warmup_epochs'] if 'warmup_epochs' in config else 0,
+                                   config['lr_warmup_decay'] if 'lr_warmup_decay' in config else 0.01)
+
+    def forward_model(self, images, labels):
+        return self.model(images, labels, flag='train')
+
+    def meter_counts(self, n):
+        return 8 * n, 4 * n
+
+
 TRAINERS = {'BCNN': BCNNTrainer, 'CBCNN': CBCNNTrainer, 'MPN': MPNTrainer, 'PeerLearning': PeerLearningTrainer,
             'OSMENet': OSMENetTrainer}
+# TRAINERS keeps the key set it has always had, so code that enumerates it sees no change; the command line dispatches
+# over every method, APINet included.
+ALL_TRAINERS = dict(TRAINERS, APINet=APINetTrainer)
 
 
 def main(argv=None):
     argv = list(sys.argv[1:] if argv is None else argv)
-    if not argv or argv[0] not in TRAINERS:
-        raise SystemExit(f'usage: python -m hawkeye_b200.examples {{{",".join(TRAINERS)}}} --config <yaml>')
+    if not argv or argv[0] not in ALL_TRAINERS:
+        raise SystemExit(f'usage: python -m hawkeye_b200.examples {{{",".join(ALL_TRAINERS)}}} --config <yaml>')
     from .config import setup_config
-    trainer = TRAINERS[argv[0]](setup_config(argv[1:]))
+    trainer = ALL_TRAINERS[argv[0]](setup_config(argv[1:]))
     trainer.train()
 
 

@@ -108,3 +108,31 @@ class MAMCLoss(nn.Module):
         if not self.use_mamc:
             return loss_ce
         return loss_ce + self.lambda_a * self.npair_loss(x_part, targets)
+
+
+class APINetLoss(nn.Module):
+    """model/loss/APINet_loss.py: CrossEntropy(label_smoothing=0.1) over cat(self_logits, other_logits) with targets
+    cat(labels1, labels2, labels1, labels2), plus MarginRankingLoss(margin=0.05) between the softmax scores of the target under
+    the self and the other features.  ``inputs`` is the 4-tuple APINet returns; ``target`` is unused, as in the reference.
+    One cross-entropy kernel over the 8n rows and one ranking kernel (hk_apinet_rank_loss) that adds its term and gradient;
+    ``last_correct`` is the top-1 count over the 8n rows, on the device."""
+
+    def __init__(self, config=None):
+        super().__init__()
+        from .ops_apinet import RANK_MARGIN
+        self.margin = RANK_MARGIN
+
+    def forward(self, inputs, target=None):
+        from .ops_apinet import APINetLossFn
+        self_logits, other_logits, labels1, labels2 = inputs
+        base = self_logits._base
+        if (base is not None and base is other_logits._base and base.is_contiguous() and base.dim() == 2
+                and self_logits.data_ptr() == base.data_ptr() and self_logits.shape[0] * 2 == base.shape[0]
+                and other_logits.data_ptr() == base.data_ptr() + self_logits.numel() * base.element_size()):
+            logits = base                    # APINet's two halves of one [8n, K] fc output: no copy
+        else:
+            logits = torch.cat([self_logits, other_logits], dim=0)
+        targets = torch.cat([labels1, labels2, labels1, labels2], dim=0)
+        loss, correct = APINetLossFn.apply(logits, targets, self.margin)
+        self.last_correct = correct
+        return loss

@@ -248,7 +248,7 @@ class Trainer:
             self._graph = None                                         # another batch shape (last batch of an epoch): eager
             self._graph_steps = -1
         if self._graph is None:
-            outputs = self.model(images)
+            outputs = self.forward_model(images, labels)
             loss = self.criterion(outputs, labels)
             self.optimizer.zero_grad()
             loss.backward()
@@ -261,7 +261,7 @@ class Trainer:
                 from . import _lib
                 n0 = _lib.launch_count()
                 with torch.cuda.graph(g['graph'], stream=gs):
-                    g['out'] = self.model(g['img'])
+                    g['out'] = self.forward_model(g['img'], g['lab'])
                     g['loss'] = self.criterion(g['out'], g['lab'])
                     g['correct'] = getattr(self.criterion, 'last_correct', None)
                     self.optimizer.zero_grad()
@@ -286,7 +286,7 @@ class Trainer:
         if self._graph_wanted():
             outputs, loss = self._graph_step(images, labels)
         else:
-            outputs = self.model(images)
+            outputs = self.forward_model(images, labels)
             loss = self.criterion(outputs, labels)
             self.optimizer.zero_grad()
             loss.backward()
@@ -301,6 +301,7 @@ class Trainer:
             self.average_meters['acc'].update(accuracy(outputs, labels, 1), n)
             self.average_meters['loss'].update(loss.item(), n)
             return loss
+        n_acc, n_loss = self.meter_counts(n)
         slot = self._readback_i % len(self._readback)
         self._readback_i += 1
         buf = self._readback[slot]
@@ -314,9 +315,18 @@ class Trainer:
         ev = torch.cuda.Event()
         ev.record()
         self._readback_ev[slot] = ev
-        self.average_meters['loss'].update_async(buf, 0, 1.0, n, ev)
-        self.average_meters['acc'].update_async(buf, 1, 100.0 / n, n, ev)
+        self.average_meters['loss'].update_async(buf, 0, 1.0, n_loss, ev)
+        self.average_meters['acc'].update_async(buf, 1, 100.0 / n_acc, n_acc, ev)
         return loss
+
+    def forward_model(self, images, labels):
+        """The model call of the training step (eager and graph-captured alike).  Methods whose forward takes the labels
+        (APINet mines its pairs from them) override this."""
+        return self.model(images)
+
+    def meter_counts(self, n):
+        """-> (samples behind the top-1 count, samples behind the loss) of a batch of n images."""
+        return n, n
 
     def batch_validate(self, data):
         images, labels = self.to_device(data['img']), self.to_device(data['label'])

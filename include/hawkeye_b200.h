@@ -217,6 +217,38 @@ int hk_npair_loss(const float* prod, const int* cls, const int* part, double* lo
 int hk_relu_fwd(const float* x, float* y, size_t n, void* stream);
 int hk_relu_bwd(const float* y, const float* dy, float* dx, size_t n, void* stream);
 
+/* ---- APINet: model/methods/APINet.py:28-119, model/loss/APINet_loss.py:33-39 -------------------------------------------
+ * hk_apinet_pairs (get_pairs + pdist, :76-119): pool [n,D], labels [n] -> intra[i] = argmin over j != i of the same label,
+ *   inter[i] = argmin over other labels of dist(i,j) = (-2<x_i,x_j> + |x_j|^2) + |x_i|^2 (fp32, fixed order); ties go to
+ *   the lowest index, a row without candidates gets 0 (np.argmin of an all-inf row).  labels1 / labels2 (optional, [2n])
+ *   receive cat(labels, labels) and cat(labels[intra], labels[inter]).  2 <= n <= 4096; no host round trip.
+ * hk_apinet_gather: mutual [2n, 2D] = [pool[r mod n] | pool[idx2[r]]] with idx2 = cat(intra, inter) (:36-43);
+ *   hk_apinet_scatter is its adjoint: dpool[i] sums its sources in ascending row order (no atomics).  D % 4 == 0.
+ * hk_dropout_*: nn.Dropout(p) in train mode, y = x * keep / (1 - p); keep is a stateless hash of (*seed, call, element index)
+ *   (splitmix64; restated in oracle/hop_oracle.py), so the backward recomputes the mask.  The seed is a device int64, so a
+ *   captured graph draws new masks on every replay.  p == 0: identity (seed may be null).
+ * hk_apinet_gate_fwd (:46-61): m = map2 output [2n, D], f1 / f2 = the halves of mutual; g1 = sigmoid(m f1), g2 = sigmoid(m f2);
+ *   out [8n, D] = [drop(g1 f1 + f1); drop(g2 f2 + f2); drop(g2 f1 + f1); drop(g1 f2 + f2)] (self_1, self_2, other_1, other_2:
+ *   one hk_linear_fwd of fc over it gives cat(self_logits, other_logits), :63-69).  Dropout call ids call0 + 0..3 in the
+ *   reference's order (f1 self, f1 other, f2 self, f2 other).  The backward writes dm and STORES df1 | df2 into dmutual
+ *   (map1's dgrad then accumulates onto it).
+ * hk_apinet_rank_loss: logits [2R, K] whose rows r and r + R are a (self, other) pair, targets [2R]; adds
+ *   mean_r max(0, p_other[r] - p_self[r] + margin) (p = softmax probability of the row's target) to the fp64 accumulator
+ *   loss_acc[0] and ADDS its gradient times grad_scale to dlogits (optional; which holds the cross-entropy gradient).  At the
+ *   hinge the gradient passes, as torch's clamp_min does.  Default precision mode: the sums are rounded to tf32 on store. */
+int hk_apinet_pairs(const float* pool, const long long* labels, long long* intra, long long* inter, long long* labels1,
+                    long long* labels2, int n, int D, void* stream);
+int hk_apinet_gather(const float* pool, const long long* idx2, float* mutual, int n, int D, void* stream);
+int hk_apinet_scatter(const float* dmutual, const long long* idx2, float* dpool, int n, int D, void* stream);
+int hk_dropout_fwd(const float* x, float* y, size_t n, float p, const long long* seed, int call, void* stream);
+int hk_dropout_bwd(const float* dy, float* dx, size_t n, float p, const long long* seed, int call, void* stream);
+int hk_apinet_gate_fwd(const float* m, const float* mutual, float* out, int rows, int D, float p, const long long* seed,
+                       int call0, void* stream);
+int hk_apinet_gate_bwd(const float* m, const float* mutual, const float* dout, float* dm, float* dmutual, int rows, int D,
+                       float p, const long long* seed, int call0, void* stream);
+int hk_apinet_rank_loss(const float* logits, const long long* targets, double* loss_acc, float* dlogits, int R, int K,
+                        float margin, float grad_scale, void* stream);
+
 /* ---- classifier nn.Linear (BCNN.py:42, CBCNN.py:26, MPNCOV.py:31) as skinny wgmma GEMMs ------------------- */
 size_t hk_linear_fwd_workspace_bytes(int B, int F, int N);
 int hk_linear_fwd(const float* x, const float* w, const float* bias, float* y, int B, int F, int N, void* workspace,
