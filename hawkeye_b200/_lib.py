@@ -94,7 +94,9 @@ def query(name, *args):
 
 
 def stream_ptr():
-    return torch.cuda.current_stream().cuda_stream
+    """Handle of the current CUDA stream.  Read directly rather than through torch.cuda.current_stream(), which builds a
+    Stream object: this runs for every launch, and the ResNet steps are bound by host launch time."""
+    return torch._C._cuda_getCurrentRawStream(torch._C._cuda_getDevice())
 
 
 def set_precise(on):

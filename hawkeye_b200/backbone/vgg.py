@@ -32,7 +32,6 @@ class VGGFeatures(nn.Sequential):
         super().__init__(*layers)
         self.cfg = tuple(cfg)
         self.out_channels = cin
-        self.train_backbone = True
         self.apply(initialize_weights)   # vgg.py:45-46
 
     def conv_params(self):
@@ -43,7 +42,7 @@ class VGGFeatures(nn.Sequential):
         return ps
 
     def forward(self, x):
-        return ops.vgg_features(x, self.cfg, self.conv_params(), self.train_backbone)
+        return ops.vgg_features(x, self.cfg, self.conv_params())
 
 
 @BACKBONE.register

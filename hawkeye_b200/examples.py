@@ -51,8 +51,6 @@ class CBCNNTrainer(Trainer):
         if config.stage == 1:
             for p in model.backbone.parameters():
                 p.requires_grad = False
-            if hasattr(model.backbone, 'train_backbone'):
-                model.backbone.train_backbone = False
         return model
 
     def get_scheduler(self, config):

@@ -42,8 +42,7 @@ class NPairsLossFn(Function):
     @staticmethod
     def forward(ctx, feats, labels):
         from . import _lib
-        from .ops import _check_cuda, _f32c
-        from .ops_cin import _gemm
+        from .ops import _check_cuda, _f32c, gemm
         _check_cuda(feats, labels)
         b, p, D = feats.shape
         n = b * p
@@ -56,7 +55,7 @@ class NPairsLossFn(Function):
         xn, inv = torch.empty_like(x), torch.empty(n, device=dev, dtype=torch.float32)
         _lib.call('hk_l2norm_rows_fwd', x, xn, inv, n, D, s)                                        # :43
         prod = torch.empty(n, n, device=dev, dtype=torch.float32)
-        _gemm(xn, 0, D, 0, xn, 0, D, 0, prod, n, 0, n, n, D, 1, exact=True)                          # :46 prod = F F^T
+        gemm(xn, 0, D, 0, xn, 0, D, 0, prod, n, 0, n, n, D, exact=True)                              # :46 prod = F F^T
         cls = labels.to(torch.int32).repeat_interleave(p).contiguous()                              # :44
         part = torch.arange(p, device=dev, dtype=torch.int32).repeat(b).contiguous()                # :45
         acc = torch.zeros(1, device=dev, dtype=torch.float64)
@@ -69,16 +68,16 @@ class NPairsLossFn(Function):
     @staticmethod
     def backward(ctx, g):
         from . import _lib
-        from .ops_cin import _gemm
+        from .ops import gemm
         xn, inv, dprod = ctx.saved_tensors
         b, p, D = ctx.shape
         n = b * p
         s = _lib.stream_ptr()
         # dF = (dprod + dprod^T) F : two products into the same buffer (the second accumulates through D / beta)
         t = torch.empty_like(xn)
-        _gemm(dprod, 0, n, 0, xn, 1, D, 0, t, D, 0, n, D, n, 1, exact=True)
+        gemm(dprod, 0, n, 0, xn, 1, D, 0, t, D, 0, n, D, n, exact=True)
         dxn = torch.empty_like(xn)
-        _gemm(dprod, 1, n, 0, xn, 1, D, 0, dxn, D, 0, n, D, n, 1, D=t, ldd=D, sD=0, beta=1.0, exact=True)
+        gemm(dprod, 1, n, 0, xn, 1, D, 0, dxn, D, 0, n, D, n, D=t, ldd=D, beta=1.0, exact=True)
         dx = torch.empty_like(xn)
         _lib.call('hk_l2norm_rows_bwd', xn, inv, dxn, dx, n, D, s)
         return (dx * g).reshape(b, p, D), None

@@ -27,7 +27,6 @@ class BCNN(nn.Module):
         if self.stage == 1:                                              # BCNN.py:45-47
             for p in self.backbone.parameters():
                 p.requires_grad = False
-        self.backbone.train_backbone = self.stage != 1
 
     def features(self, x):
         x = self.backbone(x)

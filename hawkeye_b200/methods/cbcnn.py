@@ -55,7 +55,6 @@ class CBCNN(nn.Module):
         ops.check_num_classes(config.num_classes)
         self.classifier = nn.Linear(out_channel, config.num_classes)
         self.classifier.apply(initialize_weights)
-        self.backbone.train_backbone = config.stage != 1
 
     def features(self, x):
         x = self.backbone(x)

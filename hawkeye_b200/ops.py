@@ -3,26 +3,16 @@
 Every op here calls ``libhawkeye_b200.so`` through ``_lib.call``; there is no PyTorch-eager fallback.
 PyTorch owns all device buffers (caching allocator) incl. workspaces and saved-for-backward tensors.
 """
-import os
-
 import torch
 from torch.autograd import Function
 
 from . import _lib
-
-VGG16_D = (64, 64, 'M', 128, 128, 'M', 256, 256, 256, 'M', 512, 512, 512, 'M', 512, 512, 512, 'M')
 
 # Parity tests only: when set to a list, forward passes append the decisions they took at the non-smooth points of the
 # path, in execution order — ('relu', y NHWC) after every ReLU, ('pool2', x NHWC) before every 2x2 max-pool,
 # ('pool3', argmax u8 NHWC, input shape) for the ResNet stem pool, ('ssqrt', bins) for CBCNN's signed square root —
 # so that a CPU oracle can be evaluated on the same branch of the piecewise-smooth function (oracle.hop_oracle.MaskTape).
 CAPTURE = None
-
-# Backbone weight/bias gradients are accumulated by the wgrad kernels directly into an existing ``param.grad`` (see
-# VGGFeaturesFn.backward).  Set to False to make every backward return fresh gradient tensors to autograd instead.
-ACCUMULATE_INTO_GRAD = True
-# conv3x3 + ReLU + MaxPool2d(2,2) as one kernel (hk_conv3x3_fwd_pool) wherever VGG has a pool after a conv
-FUSE_CONV_POOL = os.environ.get('HK_FUSE_CONV_POOL', '1') != '0'
 
 
 def _grad_ready(p):
@@ -45,6 +35,92 @@ def _f32c(t):
 
 def _ws(nbytes, device):
     return torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=device)
+
+
+def wants_grad(x, params, training=True, what=''):
+    """Save-for-backward decision, taken from what requires grad at call time (grad mode is always off inside
+    Function.forward, so callers decide before ``apply``; freezing / unfreezing parameters after construction just works).
+    ``training=False`` means the op runs BatchNorm on its running statistics: gradients through that are not on the
+    reference's training path and have no kernel here, so asking for them is an error, never a silent None."""
+    want = torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params))
+    if want and not training:
+        raise _lib.HawkeyeLibError(f'{what}: backward through eval-mode BatchNorm is not implemented — call .train(), '
+                                   'or run under torch.no_grad() / with all inputs and parameters frozen')
+    return want
+
+
+# ----------------------------------------------------------------------------------------------------------
+# shared host bindings: GEMM, linear forward, NCHW <-> NHWC, 3x3 convolution on NHWC maps
+# ----------------------------------------------------------------------------------------------------------
+def gemm(A, a_mn, lda, sA, B, b_mn, ldb, sB, C, ldc, sC, M, N, K, batch=1, alpha=1.0, alpha_vec=None, diag=0.0, D=None,
+         ldd=0, sD=0, beta=0.0, beta_vec=None, relu=False, trans_c=False, exact=False):
+    """C[b] = alpha*alpha_vec * A[b].B[b] + diag*I + beta*beta_vec * D[b] (then ReLU; C^T stored if trans_c) on the wgmma
+    GEMM, with raw leading dimensions and batch strides (0 = shared across the batch).  A is [M,K] (or [K,M] if a_mn),
+    B is [N,K] (or [K,N] if b_mn).  ``exact`` runs 3xTF32 whatever the library's precision mode."""
+    _lib.call('hk_gemm_3xtf32' if exact else 'hk_gemm_tf32', A, int(a_mn), lda, sA, B, int(b_mn), ldb, sB, C, ldc, sC,
+              int(trans_c), M, N, K, batch, float(alpha), alpha_vec, float(diag), D, ldd, sD, float(beta), beta_vec,
+              int(relu), _lib.stream_ptr())
+
+
+def linear_fwd(x, w, b):
+    """y = x w^T + b: x [B, F], w [N, F], b [N] or None -> [B, N]"""
+    B, F = x.shape
+    N = w.shape[0]
+    y = torch.empty(B, N, device=x.device, dtype=torch.float32)
+    ws = _ws(_lib.query('hk_linear_fwd_workspace_bytes', B, F, N), x.device)
+    _lib.call('hk_linear_fwd', x, w, b, y, B, F, N, ws, ws.numel(), _lib.stream_ptr())
+    return y
+
+
+def nchw_to_nhwc(x):
+    N, C, H, W = x.shape
+    y = torch.empty(N, H, W, C, device=x.device, dtype=torch.float32)
+    _lib.call('hk_nchw_to_nhwc', x, y, N, H * W, C, _lib.stream_ptr())
+    return y
+
+
+def nhwc_to_nchw(x):
+    N, H, W, C = x.shape
+    y = torch.empty(N, C, H, W, device=x.device, dtype=torch.float32)
+    _lib.call('hk_nhwc_to_nchw', x, y, N, H * W, C, _lib.stream_ptr())
+    return y
+
+
+def conv3x3_pack(w, dgrad):
+    """[Cout, Cin, 3, 3] weights -> (w_fwd [9, Cout, Cin], w_dgrad [9, Cin, Cout] with flipped taps, or None unless dgrad)"""
+    cout, cin = w.shape[:2]
+    wf = torch.empty(9, cout, cin, device=w.device, dtype=torch.float32)
+    wd = torch.empty(9, cin, cout, device=w.device, dtype=torch.float32) if dgrad else None
+    _lib.call('hk_conv3x3_pack_weights', w, wf, wd, cout, cin, _lib.stream_ptr())
+    return wf, wd
+
+
+def conv3x3_fwd(x, wf, b, relu, stride=1):
+    """padding-1 3x3 conv (+ bias) (+ ReLU) of an NHWC map with packed weights -> NHWC [N, H/stride, W/stride, Cout]"""
+    N, H, W, cin = x.shape
+    cout = wf.shape[1]
+    y = torch.empty(N, H // stride, W // stride, cout, device=x.device, dtype=torch.float32)
+    _lib.call('hk_conv3x3_fwd' if stride == 1 else 'hk_conv3x3_s2_fwd', x, wf, b, y, N, H, W, cin, cout, int(relu),
+              _lib.stream_ptr())
+    return y
+
+
+def conv3x3_wgrad(x, g, dw, db=None, accumulate=False):
+    """dw [Cout, Cin, 3, 3] (and db [Cout]) of a stride-1 3x3 conv from its NHWC input and the (ReLU-masked) NHWC output
+    gradient, written or, with ``accumulate``, added onto"""
+    N, H, W, cin = x.shape
+    cout = g.shape[-1]
+    ws = _ws(_lib.query('hk_conv3x3_wgrad_workspace_bytes', cin, cout), x.device)
+    _lib.call('hk_conv3x3_wgrad_acc', x, g, dw, db, N, H, W, cin, cout, ws, ws.numel(), int(accumulate), _lib.stream_ptr())
+
+
+def conv3x3_dgrad(g, wd, mask=None):
+    """input gradient of a stride-1 3x3 conv from the NHWC output gradient and the packed w_dgrad, times (mask > 0) if given"""
+    N, H, W, cout = g.shape
+    cin = wd.shape[1]
+    dx = torch.empty(N, H, W, cin, device=g.device, dtype=torch.float32)
+    _lib.call('hk_conv3x3_dgrad', g, wd, mask, dx, N, H, W, cin, cout, _lib.stream_ptr())
+    return dx
 
 
 # ----------------------------------------------------------------------------------------------------------
@@ -87,11 +163,7 @@ class LinearFn(Function):
     def forward(ctx, x, w, b):
         _check_cuda(x, w, b)
         x, w = _f32c(x), _f32c(w)
-        B, F = x.shape
-        N = w.shape[0]
-        y = torch.empty(B, N, device=x.device, dtype=torch.float32)
-        ws = _ws(_lib.query('hk_linear_fwd_workspace_bytes', B, F, N), x.device)
-        _lib.call('hk_linear_fwd', x, w, b, y, B, F, N, ws, ws.numel(), _lib.stream_ptr())
+        y = linear_fwd(x, w, b)
         ctx.save_for_backward(x, w)
         ctx.has_bias = b is not None
         return y
@@ -167,9 +239,19 @@ class CrossEntropyLS(torch.nn.Module):
 # ----------------------------------------------------------------------------------------------------------
 # VGG-style backbone (reference model/backbone/vgg.py:56-70), whole feature stack as ONE autograd node
 # ----------------------------------------------------------------------------------------------------------
-def _vgg_plan(cfg):
-    """-> list of ('conv', cout) / ('pool',) entries."""
-    return [('pool',) if v == 'M' else ('conv', int(v)) for v in cfg]
+def _vgg_layers(cfg):
+    """-> [(cout, pool_after)]: one entry per conv, 'M' folded into the conv it follows."""
+    layers = []
+    for v in cfg:
+        if v != 'M':
+            layers.append((int(v), False))
+        elif layers and not layers[-1][1]:
+            layers[-1] = (layers[-1][0], True)
+        else:
+            raise _lib.HawkeyeLibError('VGG cfg: every max-pool must follow a conv')
+    if not layers[-1][1]:
+        raise _lib.HawkeyeLibError('VGG cfg must end with a max-pool (reference BCNN keeps the last pool)')
+    return layers
 
 
 class VGGFeaturesFn(Function):
@@ -179,7 +261,7 @@ class VGGFeaturesFn(Function):
     """
 
     @staticmethod
-    def forward(ctx, x, cfg, train_backbone, *params):
+    def forward(ctx, x, cfg, save, *params):
         _check_cuda(x, *params)
         x = _f32c(x)
         s = _lib.stream_ptr()
@@ -187,75 +269,48 @@ class VGGFeaturesFn(Function):
         N, cin0, H, W = x.shape
         if cin0 != 3:
             raise _lib.HawkeyeLibError('VGG features expect a 3-channel NCHW image')
-        plan = _vgg_plan(cfg)
-        if plan[-1][0] != 'pool':
-            raise _lib.HawkeyeLibError('VGG cfg must end with a max-pool (reference BCNN keeps the last pool)')
-        save = bool(train_backbone)   # decided by the caller: grad mode is always off inside Function.forward
-        records = []   # per layer: dict for backward
-        cur, C, li = None, 3, 0
-        # conv + ReLU + max-pool in one kernel (the pre-pool map is never written) whenever a pool follows a conv; the
-        # unfused pair stays for the 3xTF32 mode (its passes chain through the full map) and for activation capture
-        fuse_pool = FUSE_CONV_POOL and not _lib.get_precise() and CAPTURE is None
-        skip_pool = False
-        for idx, ent in enumerate(plan):
-            if ent[0] == 'conv':
-                cout = ent[1]
-                w, b = _f32c(params[2 * li]), params[2 * li + 1]
-                fused = fuse_pool and li > 0 and idx + 1 < len(plan) and plan[idx + 1][0] == 'pool' and H % 2 == 0 and W % 2 == 0
-                y = None if fused else torch.empty(N, H, W, cout, device=dev, dtype=torch.float32)
-                if li == 0:
-                    ws0 = _ws(_lib.query('hk_conv3x3_first_fwd_workspace_bytes', N, H, W, cout), dev)
-                    _lib.call('hk_conv3x3_first_fwd', x, w, b, y, N, H, W, cout, ws0, ws0.numel(), s)
-                    rec = dict(kind='conv0', inp=None, out=y, H=H, W=W, cin=3, cout=cout, x27=ws0 if save else None)
-                else:
-                    wf = torch.empty(9 * cout * C, device=dev, dtype=torch.float32)
-                    wd = torch.empty(9 * cout * C, device=dev, dtype=torch.float32) if save else None
-                    _lib.call('hk_conv3x3_pack_weights', w, wf, wd, cout, C, s)
-                    rec = dict(kind='conv', inp=cur, out=y, wd=wd, H=H, W=W, cin=C, cout=cout,
-                               inp_is_relu=(records[-1]['kind'] != 'pool'))
-                    if fused:
-                        last = idx + 1 == len(plan) - 1
-                        Ho, Wo = H // 2, W // 2
-                        out = torch.empty((N, cout, Ho, Wo) if last else (N, Ho, Wo, cout), device=dev, dtype=torch.float32)
-                        code = torch.empty(N, Ho, Wo, cout, device=dev, dtype=torch.uint8) if save else None
-                        _lib.call('hk_conv3x3_fwd_pool', cur, wf, b, out, code, N, H, W, C, cout, 1 if last else 0, s)
-                        records.append(rec)
-                        records.append(dict(kind='pool', code=code, H=H, W=W, C=cout, last=last))
-                        cur, C, H, W = out, cout, Ho, Wo
-                        li += 1
-                        skip_pool = True
-                        continue
-                    _lib.call('hk_conv3x3_fwd', cur, wf, b, y, N, H, W, C, cout, 1, s)
-                records.append(rec)
-                if CAPTURE is not None:
-                    CAPTURE.append(('relu', y))
-                cur, C = y, cout
-                li += 1
+        layers = _vgg_layers(cfg)
+        records = []   # per conv layer, for backward
+        cur, C = x, 3
+        # conv + ReLU + max-pool in one kernel (the pre-pool map is never written) where a pool follows a conv; the
+        # unfused pair stays for the 3xTF32 mode (its passes chain through the full map), for activation capture and
+        # for odd map sizes
+        fuse_ok = not _lib.get_precise() and CAPTURE is None
+        for li, (cout, pool) in enumerate(layers):
+            w, b = _f32c(params[2 * li]), params[2 * li + 1]
+            rec = dict(inp=cur, H=H, W=W)
+            fused = pool and li > 0 and fuse_ok and H % 2 == 0 and W % 2 == 0
+            if li == 0:
+                y = torch.empty(N, H, W, cout, device=dev, dtype=torch.float32)
+                ws0 = _ws(_lib.query('hk_conv3x3_first_fwd_workspace_bytes', N, H, W, cout), dev)
+                _lib.call('hk_conv3x3_first_fwd', x, w, b, y, N, H, W, cout, ws0, ws0.numel(), s)
+                rec['x27'] = ws0 if save else None
             else:
-                if skip_pool:       # already done by the conv before it
-                    skip_pool = False
-                    continue
-                last = idx == len(plan) - 1
+                wf, rec['wd'] = conv3x3_pack(w, save)
+                if not fused:
+                    y = conv3x3_fwd(cur, wf, b, relu=True)
+            if not fused and CAPTURE is not None:
+                CAPTURE.append(('relu', y))
+            if pool:
+                last = li == len(layers) - 1
                 Ho, Wo = H // 2, W // 2
-                out = torch.empty((N, C, Ho, Wo) if last else (N, Ho, Wo, C), device=dev, dtype=torch.float32)
-                code = None
-                if save:     # one byte per pooled element (arg-max position + ReLU mask) is all the backward needs
-                    code = torch.empty(N, Ho, Wo, C, device=dev, dtype=torch.uint8)
-                    _lib.call('hk_maxpool2x2_fwd_idx', cur, out, code, N, H, W, C, 1 if last else 0, s)
+                out = torch.empty((N, cout, Ho, Wo) if last else (N, Ho, Wo, cout), device=dev, dtype=torch.float32)
+                # one byte per pooled element (arg-max position + ReLU mask) is all the backward needs
+                code = torch.empty(N, Ho, Wo, cout, device=dev, dtype=torch.uint8) if save else None
+                if fused:
+                    _lib.call('hk_conv3x3_fwd_pool', cur, wf, b, out, code, N, H, W, C, cout, int(last), s)
+                elif save:
+                    _lib.call('hk_maxpool2x2_fwd_idx', y, out, code, N, H, W, cout, int(last), s)
                 else:
-                    _lib.call('hk_maxpool2x2_fwd', cur, out, N, H, W, C, 1 if last else 0, s)
+                    _lib.call('hk_maxpool2x2_fwd', y, out, N, H, W, cout, int(last), s)
                 if CAPTURE is not None:
-                    CAPTURE.append(('pool2', cur))
-                records.append(dict(kind='pool', code=code, H=H, W=W, C=C, last=last))
-                cur, H, W = out, Ho, Wo
-        if save:
-            ctx.records = records
-            ctx.x = x
-            ctx.N = N
-            ctx.params = params      # the nn.Parameters themselves: backward accumulates into their .grad when it can
-        else:
-            ctx.records = None
-        ctx.nparams = len(params)
+                    CAPTURE.append(('pool2', y))
+                rec.update(code=code, last=last)
+                y, H, W = out, Ho, Wo
+            records.append(rec)
+            cur, C = y, cout
+        ctx.layers, ctx.records, ctx.nparams = layers, (records if save else None), len(params)
+        ctx.params = params if save else None    # the nn.Parameters themselves: backward accumulates into their .grad
         return cur
 
     @staticmethod
@@ -263,59 +318,43 @@ class VGGFeaturesFn(Function):
         if ctx.records is None:
             return (None, None, None) + (None,) * ctx.nparams
         s = _lib.stream_ptr()
-        N = ctx.N
-        dev = dfeat.device
         g = _f32c(dfeat)
         grads = [None] * ctx.nparams
-        li = ctx.nparams // 2
-        for rec in reversed(ctx.records):
-            if rec['kind'] == 'pool':
-                dx = torch.empty(N, rec['H'], rec['W'], rec['C'], device=dev, dtype=torch.float32)
-                _lib.call('hk_maxpool2x2_bwd_idx', rec['code'], g, dx, N, rec['H'], rec['W'], rec['C'],
-                          1 if rec['last'] else 0, s)
-                rec['code'] = None
+        for li in reversed(range(len(ctx.layers))):
+            rec, (cout, pool) = ctx.records[li], ctx.layers[li]
+            N, H, W = g.shape[0], rec['H'], rec['W']
+            if pool:
+                dx = torch.empty(N, H, W, cout, device=g.device, dtype=torch.float32)
+                _lib.call('hk_maxpool2x2_bwd_idx', rec['code'], g, dx, N, H, W, cout, int(rec['last']), s)
                 g = dx
-                continue
-            li -= 1
-            H, W, cin, cout = rec['H'], rec['W'], rec['cin'], rec['cout']
             # Accumulate straight into the parameters' .grad buffers when they exist (the Trainer keeps them as views of
             # one flat buffer): same semantics as autograd's own accumulation, without the temporaries and the 26 `add`
             # launches.  Otherwise (first backward, .grad is None) return fresh tensors and let autograd install them.
             pw, pb = ctx.params[2 * li], ctx.params[2 * li + 1]
-            direct = ACCUMULATE_INTO_GRAD and _grad_ready(pw) and _grad_ready(pb)
+            direct = _grad_ready(pw) and _grad_ready(pb)
             if direct:
-                dw, db, acc = pw.grad, pb.grad, 1
+                dw, db = pw.grad, pb.grad
             else:
-                dw = torch.empty(cout, cin, 3, 3, device=dev, dtype=torch.float32)
-                db = torch.empty(cout, device=dev, dtype=torch.float32)
-                acc = 0
-            if rec['kind'] == 'conv0':
-                ws = _ws(_lib.query('hk_conv3x3_first_wgrad_workspace_bytes', N, H, W, cout), dev)
-                _lib.call('hk_conv3x3_first_wgrad_acc', rec['x27'], g, dw, db, N, H, W, cout, ws, ws.numel(), acc, s)
-            else:
-                ws = _ws(_lib.query('hk_conv3x3_wgrad_workspace_bytes', cin, cout), dev)
-                _lib.call('hk_conv3x3_wgrad_acc', rec['inp'], g, dw, db, N, H, W, cin, cout, ws, ws.numel(), acc, s)
-                dx = torch.empty_like(rec['inp'])
-                mask = rec['inp'] if rec['inp_is_relu'] else None
-                _lib.call('hk_conv3x3_dgrad', g, rec['wd'], mask, dx, N, H, W, cin, cout, s)
-                g = dx
-            if not direct:
+                dw = torch.empty(pw.shape, device=g.device, dtype=torch.float32)
+                db = torch.empty(cout, device=g.device, dtype=torch.float32)
                 grads[2 * li], grads[2 * li + 1] = dw, db
-            rec['out'] = None
-        ctx.records = None
-        ctx.params = None
+            if li == 0:
+                ws = _ws(_lib.query('hk_conv3x3_first_wgrad_workspace_bytes', N, H, W, cout), g.device)
+                _lib.call('hk_conv3x3_first_wgrad_acc', rec['x27'], g, dw, db, N, H, W, cout, ws, ws.numel(), int(direct), s)
+            else:
+                conv3x3_wgrad(rec['inp'], g, dw, db, accumulate=direct)
+                # the input is a ReLU output unless a pool came in between (the pool's code carries that mask)
+                g = conv3x3_dgrad(g, rec['wd'], mask=None if ctx.layers[li - 1][1] else rec['inp'])
+        ctx.records = ctx.params = None
         return (None, None, None) + tuple(grads)
 
 
-def vgg_features(x, cfg, params, train_backbone=True):
-    """``train_backbone`` is kept for call compatibility; whether activations are saved for backward is decided from what
-    actually requires grad at call time (so freezing / unfreezing the backbone after construction just works)."""
-    save = torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params))
-    return VGGFeaturesFn.apply(x, tuple(cfg), save, *params)
+def vgg_features(x, cfg, params):
+    return VGGFeaturesFn.apply(x, tuple(cfg), wants_grad(x, params), *params)
 
 
 # ----------------------------------------------------------------------------------------------------------
-# raw helpers used by tests / other heads
+# GEMM with the arguments derived from the operands' shapes (tests)
 # ----------------------------------------------------------------------------------------------------------
 def gemm_tf32(A, B, a_mn=False, b_mn=False, M=None, N=None, K=None, alpha=1.0, diag=0.0, D=None, beta=0.0,
               alpha_vec=None, beta_vec=None, trans_c=False, relu=False, out=None):
@@ -339,9 +378,8 @@ def gemm_tf32(A, B, a_mn=False, b_mn=False, M=None, N=None, K=None, alpha=1.0, d
         D = _f32c(D)
         ldd = D.shape[-1] if D.shape[-2] != 1 else 0
         sD = D.shape[-2] * D.shape[-1] if D.dim() == 3 else 0
-    _lib.call('hk_gemm_tf32', A, int(a_mn), a2[1], sA, B, int(b_mn), b2[1], sB, out, ldc, out.shape[-2] * out.shape[-1],
-              int(trans_c), M, N, K, batch, float(alpha), alpha_vec, float(diag), D, ldd, sD, float(beta), beta_vec,
-              int(relu), _lib.stream_ptr())
+    gemm(A, a_mn, a2[1], sA, B, b_mn, b2[1], sB, out, ldc, out.shape[-2] * out.shape[-1], M, N, K, batch, alpha, alpha_vec,
+         diag, D, ldd, sD, beta, beta_vec, relu, trans_c)
     return out
 
 

@@ -6,8 +6,7 @@ import torch
 from torch.autograd import Function
 
 from . import _lib
-from .ops import _check_cuda, _f32c, _ws
-from .ops_cin import _gemm
+from .ops import _check_cuda, _f32c, gemm, linear_fwd
 
 # dropout call ids, in the reference's call order: drop(map1_out), then drop(f1_self), drop(f1_other), drop(f2_self),
 # drop(f2_other) (the gate kernel uses GATE_CALL + 0..3)
@@ -28,15 +27,6 @@ def mine_pairs(pool, labels):
     return idx2, lab[0], lab[1]
 
 
-def _linear_fwd(x, w, b):
-    B, F = x.shape
-    N = w.shape[0]
-    y = torch.empty(B, N, device=x.device, dtype=torch.float32)
-    ws = _ws(_lib.query('hk_linear_fwd_workspace_bytes', B, F, N), x.device)
-    _lib.call('hk_linear_fwd', x, w, b, y, B, F, N, ws, ws.numel(), _lib.stream_ptr())
-    return y
-
-
 class PairHeadFn(Function):
     """pool [n, D], idx2 [2n]  ->  [8n, D] = [f1_self; f2_self; f1_other; f2_other] after dropout (APINet.py:36-61).
 
@@ -53,13 +43,13 @@ class PairHeadFn(Function):
         dev, s = pool.device, _lib.stream_ptr()
         mutual = torch.empty(2 * n, 2 * D, device=dev, dtype=torch.float32)
         _lib.call('hk_apinet_gather', pool, idx2, mutual, n, D, s)
-        h = _linear_fwd(mutual, w1, b1)
+        h = linear_fwd(mutual, w1, b1)
         if p > 0:
             hd = torch.empty_like(h)
             _lib.call('hk_dropout_fwd', h, hd, h.numel(), float(p), seed, MAP1_CALL, s)
         else:
             hd = h
-        m = _linear_fwd(hd, w2, b2)
+        m = linear_fwd(hd, w2, b2)
         out = torch.empty(8 * n, D, device=dev, dtype=torch.float32)
         _lib.call('hk_apinet_gate_fwd', m, mutual, out, 2 * n, D, float(p), seed, GATE_CALL, s)
         ctx.save_for_backward(idx2, mutual, hd, m, w1, w2, seed)
@@ -91,7 +81,7 @@ class PairHeadFn(Function):
         db1 = torch.empty(H, device=dev, dtype=torch.float32) if ctx.has_bias[0] else None
         _lib.call('hk_linear_wgrad', dh, mutual, dw1, db1, R, F, H, s)
         # dmutual += dh . W1  (map1's dgrad, accumulated onto the gate's contribution)
-        _gemm(dh, 0, H, 0, w1, 1, F, 0, dmutual, F, 0, R, F, H, 1, D=dmutual, ldd=F, sD=0, beta=1.0)
+        gemm(dh, 0, H, 0, w1, 1, F, 0, dmutual, F, 0, R, F, H, D=dmutual, ldd=F, beta=1.0)
         dpool = torch.empty(n, D, device=dev, dtype=torch.float32)
         _lib.call('hk_apinet_scatter', dmutual, idx2, dpool, n, D, s)
         return dpool, None, dw1, db1, dw2, db2, None, None

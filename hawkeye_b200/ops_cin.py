@@ -6,13 +6,8 @@ import torch
 from torch.autograd import Function
 
 from . import _lib
-from .ops import _check_cuda, _f32c, _ws
-
-
-def _gemm(A, a_mn, lda, sA, B, b_mn, ldb, sB, C, ldc, sC, M, N, K, batch, alpha=1.0, D=None, ldd=0, sD=0, beta=0.0,
-          exact=False):
-    _lib.call('hk_gemm_3xtf32' if exact else 'hk_gemm_tf32', A, int(a_mn), lda, sA, B, int(b_mn), ldb, sB, C, ldc, sC, 0, M, N, K, batch, float(alpha), None,
-              0.0, D, ldd, sD, float(beta), None, 0, _lib.stream_ptr())
+from .ops import (_check_cuda, _f32c, conv3x3_dgrad, conv3x3_fwd, conv3x3_pack, conv3x3_wgrad, gemm, nchw_to_nhwc,
+                  nhwc_to_nchw)
 
 
 class GramFn(Function):
@@ -25,7 +20,7 @@ class GramFn(Function):
         B, C, P = x.shape
         g = torch.empty(B, C, C, device=x.device, dtype=torch.float32)
         # 3xTF32: G feeds exp(-G) with |G| in the tens — a 5e-4 relative TF32 error would be percents of the softmax
-        _gemm(x, 0, P, C * P, x, 0, P, C * P, g, C, C * C, C, C, P, B, alpha, exact=True)
+        gemm(x, 0, P, C * P, x, 0, P, C * P, g, C, C * C, C, C, P, B, alpha, exact=True)
         ctx.save_for_backward(x)
         ctx.alpha = alpha
         return g
@@ -37,8 +32,8 @@ class GramFn(Function):
         dg = _f32c(dg)
         dx = torch.empty_like(x)
         # dX = alpha (dG + dG^T) X : two products, the second accumulates onto the first
-        _gemm(dg, 0, C, C * C, x, 1, P, C * P, dx, P, C * P, C, P, C, B, ctx.alpha)
-        _gemm(dg, 1, C, C * C, x, 1, P, C * P, dx, P, C * P, C, P, C, B, ctx.alpha, D=dx, ldd=P, sD=C * P, beta=1.0)
+        gemm(dg, 0, C, C * C, x, 1, P, C * P, dx, P, C * P, C, P, C, B, ctx.alpha)
+        gemm(dg, 1, C, C * C, x, 1, P, C * P, dx, P, C * P, C, P, C, B, ctx.alpha, D=dx, ldd=P, sD=C * P, beta=1.0)
         return dx, None
 
 
@@ -51,7 +46,7 @@ class WXFn(Function):
         w, x = _f32c(w), _f32c(x)
         B, C, P = x.shape
         y = torch.empty_like(x)
-        _gemm(w, 0, C, C * C, x, 1, P, C * P, y, P, C * P, C, P, C, B)
+        gemm(w, 0, C, C * C, x, 1, P, C * P, y, P, C * P, C, P, C, B)
         ctx.save_for_backward(w, x)
         return y
 
@@ -63,10 +58,10 @@ class WXFn(Function):
         dw = dx = None
         if ctx.needs_input_grad[0]:
             dw = torch.empty_like(w)
-            _gemm(dy, 0, P, C * P, x, 0, P, C * P, dw, C, C * C, C, C, P, B)            # dW = dY X^T
+            gemm(dy, 0, P, C * P, x, 0, P, C * P, dw, C, C * C, C, C, P, B)             # dW = dY X^T
         if ctx.needs_input_grad[1]:
             dx = torch.empty_like(x)
-            _gemm(w, 1, C, C * C, dy, 1, P, C * P, dx, P, C * P, C, P, C, B)            # dX = W^T dY
+            gemm(w, 1, C, C * C, dy, 1, P, C * P, dx, P, C * P, C, P, C, B)             # dX = W^T dY
         return dw, dx
 
 
@@ -119,43 +114,22 @@ class Conv3x3NCHWFn(Function):
     @staticmethod
     def forward(ctx, x, w, b):
         _check_cuda(x, w, b)
-        x, w = _f32c(x), _f32c(w)
-        s = _lib.stream_ptr()
-        N, C, H, W = x.shape
-        cout = w.shape[0]
-        xn = torch.empty(N, H, W, C, device=x.device, dtype=torch.float32)
-        _lib.call('hk_nchw_to_nhwc', x, xn, N, H * W, C, s)
-        wf = torch.empty(9 * cout * C, device=x.device, dtype=torch.float32)
-        wd = torch.empty(9 * cout * C, device=x.device, dtype=torch.float32)
-        _lib.call('hk_conv3x3_pack_weights', w, wf, wd, cout, C, s)
-        yn = torch.empty(N, H, W, cout, device=x.device, dtype=torch.float32)
-        _lib.call('hk_conv3x3_fwd', xn, wf, b, yn, N, H, W, C, cout, 0, s)
-        y = torch.empty(N, cout, H, W, device=x.device, dtype=torch.float32)
-        _lib.call('hk_nhwc_to_nchw', yn, y, N, H * W, cout, s)
+        xn = nchw_to_nhwc(_f32c(x))
+        wf, wd = conv3x3_pack(_f32c(w), True)
+        y = nhwc_to_nchw(conv3x3_fwd(xn, wf, b, relu=False))
         ctx.save_for_backward(xn, wd)
-        ctx.shape = (N, C, H, W, cout)
         ctx.has_bias = b is not None
         return y
 
     @staticmethod
     def backward(ctx, dy):
         xn, wd = ctx.saved_tensors
-        N, C, H, W, cout = ctx.shape
-        s = _lib.stream_ptr()
-        dev = dy.device
-        dy = _f32c(dy)
-        g = torch.empty(N, H, W, cout, device=dev, dtype=torch.float32)
-        _lib.call('hk_nchw_to_nhwc', dy, g, N, H * W, cout, s)
-        dw = torch.empty(cout, C, 3, 3, device=dev, dtype=torch.float32)
-        db = torch.empty(cout, device=dev, dtype=torch.float32) if ctx.has_bias else None
-        ws = _ws(_lib.query('hk_conv3x3_wgrad_workspace_bytes', C, cout), dev)
-        _lib.call('hk_conv3x3_wgrad', xn, g, dw, db, N, H, W, C, cout, ws, ws.numel(), s)
-        dx = None
-        if ctx.needs_input_grad[0]:
-            dxn = torch.empty(N, H, W, C, device=dev, dtype=torch.float32)
-            _lib.call('hk_conv3x3_dgrad', g, wd, None, dxn, N, H, W, C, cout, s)
-            dx = torch.empty(N, C, H, W, device=dev, dtype=torch.float32)
-            _lib.call('hk_nhwc_to_nchw', dxn, dx, N, H * W, C, s)
+        g = nchw_to_nhwc(_f32c(dy))
+        cin, cout = xn.shape[-1], g.shape[-1]
+        dw = torch.empty(cout, cin, 3, 3, device=g.device, dtype=torch.float32)
+        db = torch.empty(cout, device=g.device, dtype=torch.float32) if ctx.has_bias else None
+        conv3x3_wgrad(xn, g, dw, db)
+        dx = nhwc_to_nchw(conv3x3_dgrad(g, wd)) if ctx.needs_input_grad[0] else None
         return dx, dw, db
 
 

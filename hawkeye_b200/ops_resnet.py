@@ -7,15 +7,10 @@ import torch
 from torch.autograd import Function
 
 from . import _lib, ops as _ops
-from .ops import _check_cuda, _f32c, _ws
+from .ops import (_check_cuda, _f32c, _ws, conv3x3_dgrad, conv3x3_fwd, conv3x3_pack, conv3x3_wgrad, gemm, nchw_to_nhwc,
+                  nhwc_to_nchw)
 
 BN_EPS = 1e-5
-
-
-def _gemm(A, a_mn, lda, B, b_mn, ldb, C, ldc, M, N, K, relu=0, D=None):
-    """C = A.B (+ D, same layout as C: the residual-gradient add rides in the GEMM epilogue instead of a separate pass)"""
-    _lib.call('hk_gemm_tf32', A, int(a_mn), lda, 0, B, int(b_mn), ldb, 0, C, ldc, 0, 0, M, N, K, 1, 1.0, None, 0.0, D,
-              ldc if D is not None else 0, 0, 1.0 if D is not None else 0.0, None, relu, _lib.stream_ptr())
 
 
 class Unit:
@@ -42,7 +37,7 @@ class Unit:
             _lib.call('hk_stem_im2col', x, x147, N, H, W, s)
             _lib.call('hk_pack_stem_weights', w, w147, cout, s)
             c = torch.empty(N, Ho, Wo, cout, device=dev, dtype=torch.float32)
-            _gemm(x147, 0, 160, w147, 0, 160, c, cout, P, cout, 160)
+            gemm(x147, 0, 160, 0, w147, 0, 160, 0, c, cout, 0, P, cout, 160)
             rec['xin'] = x147
         else:
             N, H, W, cin = x.shape
@@ -55,22 +50,13 @@ class Unit:
                 Ho, Wo = xin.shape[1], xin.shape[2]
                 P = N * Ho * Wo
                 c = torch.empty(N, Ho, Wo, cout, device=dev, dtype=torch.float32)
-                _gemm(xin, 0, cin, w, 0, cin, c, cout, P, cout, cin)
+                gemm(xin, 0, cin, 0, w, 0, cin, 0, c, cout, 0, P, cout, cin)
                 rec['xin'] = xin
             else:
-                wf = torch.empty(9 * cout * cin, device=dev, dtype=torch.float32)
-                wd = torch.empty(9 * cout * cin, device=dev, dtype=torch.float32) if save else None
-                _lib.call('hk_conv3x3_pack_weights', w, wf, wd, cout, cin, s)
-                if self.kind == '3x3':
-                    Ho, Wo = H, W
-                    c = torch.empty(N, Ho, Wo, cout, device=dev, dtype=torch.float32)
-                    _lib.call('hk_conv3x3_fwd', x, wf, None, c, N, H, W, cin, cout, 0, s)
-                else:
-                    Ho, Wo = H // 2, W // 2
-                    c = torch.empty(N, Ho, Wo, cout, device=dev, dtype=torch.float32)
-                    _lib.call('hk_conv3x3_s2_fwd', x, wf, None, c, N, H, W, cin, cout, 0, s)
-                    rec['full_hw'] = (H, W)
-                rec['xin'], rec['wd'] = x, wd
+                wf, rec['wd'] = conv3x3_pack(w, save)
+                c = conv3x3_fwd(x, wf, None, relu=False, stride=2 if self.kind == '3x3s2' else 1)
+                Ho, Wo = c.shape[1:3]
+                rec['xin'] = x
             P = N * Ho * Wo
         y = torch.empty_like(c)
         bn = self.bn
@@ -106,7 +92,7 @@ class Unit:
         dbeta = torch.empty(cout, device=dev, dtype=torch.float32)
         ws = _ws(_lib.query('hk_bn_workspace_bytes', P, cout), dev)
         # BN + ReLU without a residual: the mask is recomputed from x (hk_bn_bwd_ex), y is not read
-        mask_beta = rec['beta'] if (self.relu and not rec['has_res'] and rec.get('train_stats', True)) else None
+        mask_beta = rec['beta'] if (self.relu and not rec['has_res']) else None
         _lib.call('hk_bn_bwd_ex', rec['c'], rec['y'], dy, rec['gamma'], mask_beta, rec['mean'], rec['invstd'], dc, dres,
                   dgamma, dbeta, P, cout, int(self.relu), ws, ws.numel(), s)
         w, xin = rec['w'], rec['xin']
@@ -123,9 +109,11 @@ class Unit:
             _lib.call('hk_matconv_wgrad', xin, dc, dw, P, cin, cout, wsb, wsb.numel(), s)
             if need_dx:
                 dxs = torch.empty_like(xin)
-                fused = addend if (addend is not None and self.kind == '1x1') else None
-                _gemm(dc, 0, cout, w, 1, cin, dxs, cin, P, cin, cout, D=fused)   # dX = dC . W (+ addend)  (W [Cout,Cin] as the MN-major B)
-                if fused is not None:
+                # dX = dC . W (+ addend, in the epilogue)  (W [Cout,Cin] as the MN-major B)
+                fuse = addend is not None and self.kind == '1x1'
+                gemm(dc, 0, cout, 0, w, 1, cin, 0, dxs, cin, 0, P, cin, cout, D=addend if fuse else None,
+                     ldd=cin if fuse else 0, beta=1.0 if fuse else 0.0)
+                if fuse:
                     addend = None
                 if self.kind == '1x1s2':
                     H, W = rec['full_hw']
@@ -134,18 +122,15 @@ class Unit:
                 else:
                     dx = dxs
         else:
-            cin = xin.shape[-1]
-            H, W = (Ho, Wo) if self.kind == '3x3' else rec['full_hw']
+            _, H, W, cin = xin.shape
             g = dc
             if self.kind == '3x3s2':                    # adjoint of the stride: zero-insert dC to the input resolution
                 g = torch.empty(N, H, W, cout, device=dev, dtype=torch.float32)
                 _lib.call('hk_upsample2_zero', dc, g, N, H, W, cout, s)
             dw = torch.empty(cout, cin, 3, 3, device=dev, dtype=torch.float32)
-            wsb = _ws(_lib.query('hk_conv3x3_wgrad_workspace_bytes', cin, cout), dev)
-            _lib.call('hk_conv3x3_wgrad', xin, g, dw, None, N, H, W, cin, cout, wsb, wsb.numel(), s)
+            conv3x3_wgrad(xin, g, dw)
             if need_dx:
-                dx = torch.empty(N, H, W, cin, device=dev, dtype=torch.float32)
-                _lib.call('hk_conv3x3_dgrad', g, rec['wd'], None, dx, N, H, W, cin, cout, s)
+                dx = conv3x3_dgrad(g, rec['wd'])
         if addend is not None and dx is not None:
             dx = _add(dx, addend)
         return dx, dres, dw, dgamma, dbeta
@@ -219,11 +204,8 @@ class ResNetTrunkFn(Function):
             out, r3 = u3.forward(a2, w3, g3, b3, identity, save, training)
             recs.append(('block', (r1, r2, r3, rd), None))
             cur = out
-        N, H, W, C = cur.shape
-        feat = torch.empty(N, C, H, W, device=x.device, dtype=torch.float32)
-        _lib.call('hk_nhwc_to_nchw', cur, feat, N, H * W, C, s)
         ctx.plan, ctx.recs, ctx.nparams = plan, (recs if save else None), len(params)
-        return feat
+        return nhwc_to_nchw(cur)
 
     @staticmethod
     def backward(ctx, dfeat):
@@ -231,10 +213,7 @@ class ResNetTrunkFn(Function):
             return (None,) * (4 + ctx.nparams)
         plan, recs = ctx.plan, ctx.recs
         s = _lib.stream_ptr()
-        dfeat = _f32c(dfeat)
-        N, C, H, W = dfeat.shape
-        g = torch.empty(N, H, W, C, device=dfeat.device, dtype=torch.float32)
-        _lib.call('hk_nchw_to_nhwc', dfeat, g, N, H * W, C, s)
+        g = nchw_to_nhwc(_f32c(dfeat))
         grads = []   # collected in reverse unit order, each (dw, dgamma, dbeta)
         for (u1, u2, u3, ds), (_, (r1, r2, r3, rd), _) in zip(reversed(plan.blocks), reversed(recs[1:])):
             d2, dres, dw3, dg3, db3 = u3.backward(r3, g)
@@ -265,19 +244,8 @@ def resnet_trunk(x, trunk_module):
     plan = trunk_module._plan
     params = plan.params()
     training = trunk_module.training
-    save = _wants_grad(x, params, training, 'ResNet trunk')
+    save = _ops.wants_grad(x, params, training, 'ResNet trunk')
     return ResNetTrunkFn.apply(x, plan, save, training, *params)
-
-
-def _wants_grad(x, params, training, what):
-    """Save-for-backward decision, taken from what requires grad at call time.  Gradients through EVAL-mode BatchNorm
-    (running statistics) are not on the reference's training path and have no kernel here: asking for them is an error,
-    never a silent None."""
-    want = torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params))
-    if want and not training:
-        raise _lib.HawkeyeLibError(f'{what}: backward through eval-mode BatchNorm is not implemented — call .train(), '
-                                   'or run under torch.no_grad() / with all inputs and parameters frozen')
-    return want
 
 
 class DRBlockFn(Function):
@@ -286,29 +254,14 @@ class DRBlockFn(Function):
     @staticmethod
     def forward(ctx, x, unit, save, training, w, gamma, beta):
         _check_cuda(x)
-        x = _f32c(x)
-        s = _lib.stream_ptr()
-        N, C, H, W = x.shape
-        xn = torch.empty(N, H, W, C, device=x.device, dtype=torch.float32)
-        _lib.call('hk_nchw_to_nhwc', x, xn, N, H * W, C, s)
-        y, rec = unit.forward(xn, _f32c(w), gamma, beta, None, save, training)
-        out = torch.empty(N, y.shape[-1], H, W, device=x.device, dtype=torch.float32)
-        _lib.call('hk_nhwc_to_nchw', y, out, N, H * W, y.shape[-1], s)
+        y, rec = unit.forward(nchw_to_nhwc(_f32c(x)), _f32c(w), gamma, beta, None, save, training)
         ctx.unit, ctx.rec = unit, rec
-        return out
+        return nhwc_to_nchw(y)
 
     @staticmethod
     def backward(ctx, dout):
         if ctx.rec is None:
             return (None,) * 7
-        s = _lib.stream_ptr()
-        dout = _f32c(dout)
-        N, C, H, W = dout.shape
-        g = torch.empty(N, H, W, C, device=dout.device, dtype=torch.float32)
-        _lib.call('hk_nchw_to_nhwc', dout, g, N, H * W, C, s)
-        dx, _, dw, dg, db = ctx.unit.backward(ctx.rec, g)
-        cin = dx.shape[-1]
-        dxn = torch.empty(N, cin, H, W, device=dout.device, dtype=torch.float32)
-        _lib.call('hk_nhwc_to_nchw', dx, dxn, N, H * W, cin, s)
+        dx, _, dw, dg, db = ctx.unit.backward(ctx.rec, nchw_to_nhwc(_f32c(dout)))
         ctx.rec = None
-        return dxn, None, None, None, dw, dg, db
+        return nhwc_to_nchw(dx), None, None, None, dw, dg, db

@@ -1,9 +1,9 @@
 #!/bin/bash
-# usage: run_gpu_tests.sh [files...]  — each test file in its own process (a trapped kernel poisons the CUDA context)
+# usage: run_gpu_tests.sh [files...]  (default: every tests/test_gpu_*.py) — each test file in its own process (a trapped kernel poisons the CUDA context)
 mkdir -p gpurun_out
 nvidia-smi --query-gpu=name,clocks.sm,clocks.max.sm,memory.total --format=csv > gpurun_out/gpu.txt 2>&1
 FILES="$@"
-[ -z "$FILES" ] && FILES="tests/test_gpu_gemm.py tests/test_gpu_bilinear.py tests/test_gpu_conv.py tests/test_gpu_head.py tests/test_gpu_model.py tests/test_gpu_cbcnn.py tests/test_gpu_mpncov.py tests/test_gpu_resnet.py tests/test_gpu_matched.py"
+[ -z "$FILES" ] && FILES=$(ls tests/test_gpu_*.py)
 for f in $FILES; do
   n=$(basename $f .py)
   timeout 900 python -m pytest $f -q -s -m gpu -p no:cacheprovider > gpurun_out/$n.log 2>&1
