@@ -217,12 +217,6 @@ __global__ void apinet_rank_loss_kernel(const float* __restrict__ logits, const 
   }
 }
 
-static inline int agrid(size_t n, int block) {
-  size_t g = (n + block - 1) / block;
-  const size_t cap = 132 * 16;
-  return (int)(g < cap ? (g ? g : 1) : cap);
-}
-
 static int check_p(float p, const long long* seed, const char* op) {
   HK_REQUIRE(p >= 0.f && p < 1.f, HK_ERR_ARG, "%s: dropout probability %g outside [0, 1)", op, (double)p);
   HK_REQUIRE(p == 0.f || seed, HK_ERR_ARG, "%s: dropout needs a device seed", op);
@@ -248,7 +242,7 @@ int hk_apinet_pairs(const float* pool, const long long* labels, long long* intra
 int hk_apinet_gather(const float* pool, const long long* idx2, float* mutual, int n, int D, void* stream) {
   HK_REQUIRE(pool && idx2 && mutual && n > 0 && D > 0, HK_ERR_ARG, "hk_apinet_gather: bad args");
   HK_REQUIRE(D % 4 == 0 && aligned16(pool) && aligned16(mutual), HK_ERR_ALIGN, "hk_apinet_gather: D %% 4, 16-byte rows");
-  apinet_gather_kernel<<<agrid((size_t)4 * n * D / 4, 256), 256, 0, (cudaStream_t)stream>>>(
+  apinet_gather_kernel<<<grid_1d((size_t)4 * n * D / 4, 256), 256, 0, (cudaStream_t)stream>>>(
       reinterpret_cast<const float4*>(pool), idx2, reinterpret_cast<float4*>(mutual), n, D / 4);
   HK_LAUNCH_CHECK("apinet_gather_kernel");
   return 0;
@@ -257,7 +251,7 @@ int hk_apinet_gather(const float* pool, const long long* idx2, float* mutual, in
 int hk_apinet_scatter(const float* dmutual, const long long* idx2, float* dpool, int n, int D, void* stream) {
   HK_REQUIRE(dmutual && idx2 && dpool && n > 0 && n <= 4096 && D > 0, HK_ERR_ARG, "hk_apinet_scatter: bad args");
   HK_REQUIRE(D % 4 == 0 && aligned16(dpool) && aligned16(dmutual), HK_ERR_ALIGN, "hk_apinet_scatter: D %% 4, 16-byte rows");
-  apinet_scatter_kernel<<<agrid((size_t)n * D / 4, 256), 256, 2 * n * sizeof(int), (cudaStream_t)stream>>>(
+  apinet_scatter_kernel<<<grid_1d((size_t)n * D / 4, 256), 256, 2 * n * sizeof(int), (cudaStream_t)stream>>>(
       reinterpret_cast<const float4*>(dmutual), idx2, reinterpret_cast<float4*>(dpool), n, D / 4);
   HK_LAUNCH_CHECK("apinet_scatter_kernel");
   return 0;
@@ -266,7 +260,7 @@ int hk_apinet_scatter(const float* dmutual, const long long* idx2, float* dpool,
 int hk_dropout_fwd(const float* x, float* y, size_t n, float p, const long long* seed, int call, void* stream) {
   HK_REQUIRE(x && y, HK_ERR_ARG, "hk_dropout_fwd: null pointer");
   if (int r = check_p(p, seed, "hk_dropout_fwd")) return r;
-  dropout_kernel<<<agrid(n, 256), 256, 0, (cudaStream_t)stream>>>(x, y, n, p, 1.f / (1.f - p), seed, call);
+  dropout_kernel<<<grid_1d(n, 256), 256, 0, (cudaStream_t)stream>>>(x, y, n, p, 1.f / (1.f - p), seed, call);
   HK_LAUNCH_CHECK("dropout_kernel");
   return 0;
 }
@@ -274,7 +268,7 @@ int hk_dropout_fwd(const float* x, float* y, size_t n, float p, const long long*
 int hk_dropout_bwd(const float* dy, float* dx, size_t n, float p, const long long* seed, int call, void* stream) {
   HK_REQUIRE(dy && dx, HK_ERR_ARG, "hk_dropout_bwd: null pointer");
   if (int r = check_p(p, seed, "hk_dropout_bwd")) return r;
-  dropout_kernel<<<agrid(n, 256), 256, 0, (cudaStream_t)stream>>>(dy, dx, n, p, 1.f / (1.f - p), seed, call);
+  dropout_kernel<<<grid_1d(n, 256), 256, 0, (cudaStream_t)stream>>>(dy, dx, n, p, 1.f / (1.f - p), seed, call);
   HK_LAUNCH_CHECK("dropout_kernel(bwd)");
   return 0;
 }
@@ -283,8 +277,8 @@ int hk_apinet_gate_fwd(const float* m, const float* mutual, float* out, int rows
                        int call0, void* stream) {
   HK_REQUIRE(m && mutual && out && rows > 0 && D > 0, HK_ERR_ARG, "hk_apinet_gate_fwd: bad args");
   if (int r = check_p(p, seed, "hk_apinet_gate_fwd")) return r;
-  apinet_gate_fwd_kernel<<<agrid((size_t)rows * D, 256), 256, 0, (cudaStream_t)stream>>>(m, mutual, out, rows, D, p,
-                                                                                       1.f / (1.f - p), seed, call0);
+  apinet_gate_fwd_kernel<<<grid_1d((size_t)rows * D, 256), 256, 0, (cudaStream_t)stream>>>(m, mutual, out, rows, D, p,
+                                                                                           1.f / (1.f - p), seed, call0);
   HK_LAUNCH_CHECK("apinet_gate_fwd_kernel");
   return 0;
 }
@@ -293,8 +287,8 @@ int hk_apinet_gate_bwd(const float* m, const float* mutual, const float* dout, f
                        float p, const long long* seed, int call0, void* stream) {
   HK_REQUIRE(m && mutual && dout && dm && dmutual && rows > 0 && D > 0, HK_ERR_ARG, "hk_apinet_gate_bwd: bad args");
   if (int r = check_p(p, seed, "hk_apinet_gate_bwd")) return r;
-  apinet_gate_bwd_kernel<<<agrid((size_t)rows * D, 256), 256, 0, (cudaStream_t)stream>>>(m, mutual, dout, dm, dmutual, rows,
-                                                                                       D, p, 1.f / (1.f - p), seed, call0);
+  apinet_gate_bwd_kernel<<<grid_1d((size_t)rows * D, 256), 256, 0, (cudaStream_t)stream>>>(m, mutual, dout, dm, dmutual, rows,
+                                                                                           D, p, 1.f / (1.f - p), seed, call0);
   HK_LAUNCH_CHECK("apinet_gate_bwd_kernel");
   return 0;
 }

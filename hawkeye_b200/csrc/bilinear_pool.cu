@@ -91,12 +91,12 @@ __global__ void unpad_cols_kernel(const float* __restrict__ xp, float* __restric
 }
 static inline int pad4(int v) { return (v + 3) & ~3; }
 static int launch_pad(const float* x, float* xp, size_t rows, int HW, cudaStream_t st) {
-  pad_cols_kernel<<<132 * 8, 256, 0, st>>>(x, xp, rows, HW, pad4(HW));
+  pad_cols_kernel<<<H100_SMS * 8, 256, 0, st>>>(x, xp, rows, HW, pad4(HW));
   HK_LAUNCH_CHECK("pad_cols_kernel");
   return 0;
 }
 static int launch_unpad(const float* xp, float* x, size_t rows, int HW, cudaStream_t st) {
-  unpad_cols_kernel<<<132 * 8, 256, 0, st>>>(xp, x, rows, HW, pad4(HW));
+  unpad_cols_kernel<<<H100_SMS * 8, 256, 0, st>>>(xp, x, rows, HW, pad4(HW));
   HK_LAUNCH_CHECK("unpad_cols_kernel");
   return 0;
 }
@@ -411,7 +411,7 @@ int hk_cbp_bwd(const float* x, const float* pre, const float* dy, const int* h1,
   float* dpre = S + (size_t)B * C * C;
   cbp_finalize_bwd_kernel<<<B, 256, 0, stream>>>(pre, dy, dpre, d);
   HK_LAUNCH_CHECK("cbp_finalize_bwd_kernel");
-  cbp_build_s_kernel<<<dim3(132, B), 256, 0, stream>>>(dpre, h1, h2, s1, s2, S, C, d, precise() ? 0 : 1);
+  cbp_build_s_kernel<<<dim3(H100_SMS, B), 256, 0, stream>>>(dpre, h1, h2, s1, s2, S, C, d, precise() ? 0 : 1);
   HK_LAUNCH_CHECK("cbp_build_s_kernel");
   // dX = (dG + dG^T) . X      (M = C, K = C, N = HW; X is the MN-major B operand)
   return hk_gemm_tf32(S, 0, C, (long long)C * C, x, 1, HWp, (long long)C * HWp, dx, HW, (long long)C * HW, 0, C, HW, C, B,

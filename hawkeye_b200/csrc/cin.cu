@@ -151,12 +151,6 @@ __global__ void relu_bwd_kernel(const float* __restrict__ y, const float* __rest
     dx[i] = y[i] > 0.f ? dy[i] : 0.f;
 }
 
-static inline int cgrid(size_t n, int block) {
-  size_t g = (n + block - 1) / block;
-  const size_t cap = 132 * 16;
-  return (int)(g < cap ? (g ? g : 1) : cap);
-}
-
 }  // namespace hk
 
 using namespace hk;
@@ -177,7 +171,7 @@ int hk_softmax_neg_rows_bwd(const float* w, const float* dw, float* dg, long lon
 }
 int hk_cci_weight_fwd(const float* w_sci, const float* weight, float* w_cci, int B, long long per, void* stream) {
   HK_REQUIRE(w_sci && weight && w_cci && B > 0 && B % 2 == 0 && per > 0, HK_ERR_ARG, "hk_cci_weight_fwd: bad args (B must be even)");
-  cci_weight_fwd_kernel<<<cgrid((size_t)B * per, 256), 256, 0, (cudaStream_t)stream>>>(w_sci, weight, w_cci, B, (size_t)per);
+  cci_weight_fwd_kernel<<<grid_1d((size_t)B * per, 256), 256, 0, (cudaStream_t)stream>>>(w_sci, weight, w_cci, B, (size_t)per);
   HK_LAUNCH_CHECK("cci_weight_fwd_kernel");
   return 0;
 }
@@ -193,7 +187,7 @@ int hk_cci_weight_bwd(const float* w_sci, const float* weight, const float* d_cc
 }
 int hk_se_gate_fwd(const float* x, const float* m, float* s, long long rows, int hw, void* stream) {
   HK_REQUIRE(x && m && s && rows > 0 && hw > 0, HK_ERR_ARG, "hk_se_gate_fwd: bad args");
-  se_gate_fwd_kernel<<<cgrid((size_t)rows * hw, 256), 256, 0, (cudaStream_t)stream>>>(x, m, s, (size_t)rows, hw);
+  se_gate_fwd_kernel<<<grid_1d((size_t)rows * hw, 256), 256, 0, (cudaStream_t)stream>>>(x, m, s, (size_t)rows, hw);
   HK_LAUNCH_CHECK("se_gate_fwd_kernel");
   return 0;
 }
@@ -206,13 +200,13 @@ int hk_se_gate_bwd(const float* x, const float* m, const float* ds, float* dx, f
 }
 int hk_relu_fwd(const float* x, float* y, size_t n, void* stream) {
   HK_REQUIRE(x && y, HK_ERR_ARG, "hk_relu_fwd: null pointer");
-  relu_fwd_kernel<<<cgrid(n, 256), 256, 0, (cudaStream_t)stream>>>(x, y, n);
+  relu_fwd_kernel<<<grid_1d(n, 256), 256, 0, (cudaStream_t)stream>>>(x, y, n);
   HK_LAUNCH_CHECK("relu_fwd_kernel");
   return 0;
 }
 int hk_relu_bwd(const float* y, const float* dy, float* dx, size_t n, void* stream) {
   HK_REQUIRE(y && dy && dx, HK_ERR_ARG, "hk_relu_bwd: null pointer");
-  relu_bwd_kernel<<<cgrid(n, 256), 256, 0, (cudaStream_t)stream>>>(y, dy, dx, n);
+  relu_bwd_kernel<<<grid_1d(n, 256), 256, 0, (cudaStream_t)stream>>>(y, dy, dx, n);
   HK_LAUNCH_CHECK("relu_bwd_kernel");
   return 0;
 }
@@ -224,7 +218,7 @@ int hk_row_mean_fwd(const float* x, float* y, long long rows, int cols, int ld, 
 }
 int hk_row_mean_bwd(const float* dy, float* dx, long long rows, int cols, int ld, void* stream) {
   HK_REQUIRE(dy && dx && rows > 0 && cols > 0 && ld >= cols, HK_ERR_ARG, "hk_row_mean_bwd: bad args");
-  row_mean_bwd_kernel<<<cgrid((size_t)rows * ld, 256), 256, 0, (cudaStream_t)stream>>>(dy, dx, rows, cols, ld);
+  row_mean_bwd_kernel<<<grid_1d((size_t)rows * ld, 256), 256, 0, (cudaStream_t)stream>>>(dy, dx, rows, cols, ld);
   HK_LAUNCH_CHECK("row_mean_bwd_kernel");
   return 0;
 }

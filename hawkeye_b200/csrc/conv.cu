@@ -306,12 +306,7 @@ static int make_act_map(CUtensorMap* tm, const float* X, int N, int H, int W, in
 template <int BN>
 static int launch_conv(const CUtensorMap& tmX, const CUtensorMap& tmW, const ConvArgs& a, cudaStream_t stream) {
   using Cfg = ConvCfg<BN>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv3x3_igemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
-    if (e != cudaSuccess) return set_error((int)e, "cudaFuncSetAttribute(conv<%d>): %s", BN, cudaGetErrorString(e));
-    attr_set = true;
-  }
+  if (int r = allow_dynamic_smem<conv3x3_igemm_kernel<BN>>(Cfg::SMEM, BN == 64 ? "conv<64>" : "conv<128>")) return r;
   dim3 grid(a.tiles_w * a.tiles_h * a.tiles_n, (a.Cout + BN - 1) / BN);
   conv3x3_igemm_kernel<BN><<<grid, CONV_THREADS, Cfg::SMEM, stream>>>(tmX, tmW, a);
   HK_LAUNCH_CHECK("conv3x3_igemm_kernel");
@@ -442,13 +437,8 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
 template <int BN, bool RESIDENT>
 static int launch_conv_v2(const float* x, const float* wp, ConvArgs a, int N, int H, int W, cudaStream_t stream) {
   using Cfg = ConvV2Cfg<BN, RESIDENT>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv3x3_igemm_v2_kernel<BN, RESIDENT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::SMEM);
-    if (e != cudaSuccess) return set_error((int)e, "cudaFuncSetAttribute(conv_v2<%d>): %s", BN, cudaGetErrorString(e));
-    attr_set = true;
-  }
+  if (int r = allow_dynamic_smem<conv3x3_igemm_v2_kernel<BN, RESIDENT>>(Cfg::SMEM, BN == 64 ? "conv_v2<64>" : "conv_v2<128>"))
+    return r;
   a.TW = 16; a.TH = 8; a.TN = 1;
   a.tiles_w = W / 16; a.tiles_h = H / 8; a.tiles_n = N;
   const int n_ntiles = (a.Cout + BN - 1) / BN;
@@ -468,13 +458,7 @@ static int launch_conv_v2(const float* x, const float* wp, ConvArgs a, int N, in
     uint32_t box[3] = {32, (uint32_t)BN, 1};
     if ((r = make_tmap(&tmW, wp, 3, dims, strides, box))) return r;
   }
-  static int sms = 0;
-  if (!sms) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
-        sms <= 0)
-      sms = 132;
-  }
+  const int sms = num_sms();
   const int grid = total < sms ? (int)total : sms;
   conv3x3_igemm_v2_kernel<BN, RESIDENT><<<grid, CONV_THREADS, Cfg::SMEM, stream>>>(tmX, tmW, a, n_ntiles, (int)total);
   HK_LAUNCH_CHECK("conv3x3_igemm_v2_kernel");
@@ -761,12 +745,7 @@ static int conv3x3_wgrad_1x(const float* x, const float* dy, float* dwp, float* 
   const long long total_tiles = (long long)a.tiles_w * a.tiles_h * a.tiles_n;
   // split-K factor.  The kernel runs one CTA per SM (157 KB of shared memory), so the grid executes in whole waves of
   // `sms` CTAs: pick the split that fills 1..3 waves best (ties -> fewer waves: fewer partial sums to add atomically).
-  static int sms = 0;
-  if (!sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
-  }
+  const int sms = num_sms();
   long long ks = 1;
   {
     double best = -1.0;
@@ -797,12 +776,7 @@ static int conv3x3_wgrad_1x(const float* x, const float* dy, float* dwp, float* 
     e = cudaMemsetAsync(db, 0, (size_t)Cout * sizeof(float), stream);
     if (e != cudaSuccess) return set_error((int)e, "cudaMemsetAsync(db): %s", cudaGetErrorString(e));
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    e = cudaFuncSetAttribute(conv3x3_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM);
-    if (e != cudaSuccess) return set_error((int)e, "cudaFuncSetAttribute(wgrad): %s", cudaGetErrorString(e));
-    attr_set = true;
-  }
+  if ((r = allow_dynamic_smem<conv3x3_wgrad_kernel>(WG_SMEM, "wgrad"))) return r;
   dim3 grid((unsigned)out_tiles, a.ksplit);
   conv3x3_wgrad_kernel<<<grid, WG_THREADS, WG_SMEM, stream>>>(tmDY, tmX, a);
   HK_LAUNCH_CHECK("conv3x3_wgrad_kernel");
@@ -1006,12 +980,6 @@ __global__ void relu_mask_kernel(float* __restrict__ dy, const float* __restrict
   }
 }
 
-static inline int grid_for(size_t n, int block) {
-  size_t g = (n + block - 1) / block;
-  const size_t cap = 132 * 16;
-  return (int)(g < cap ? (g ? g : 1) : cap);
-}
-
 }  // namespace hk
 
 using namespace hk;
@@ -1020,8 +988,8 @@ extern "C" {
 
 int hk_conv3x3_pack_weights(const float* w, float* w_fwd, float* w_dgrad, int Cout, int Cin, void* stream) {
   HK_REQUIRE(w && (w_fwd || w_dgrad), HK_ERR_ARG, "hk_conv3x3_pack_weights: null pointer");
-  pack_weights_kernel<<<grid_for((size_t)Cout * Cin * 9, 256), 256, 0, (cudaStream_t)stream>>>(w, w_fwd, w_dgrad, Cout, Cin,
-                                                                                             precise() ? 0 : 1);
+  pack_weights_kernel<<<grid_1d((size_t)Cout * Cin * 9, 256), 256, 0, (cudaStream_t)stream>>>(w, w_fwd, w_dgrad, Cout, Cin,
+                                                                                              precise() ? 0 : 1);
   HK_LAUNCH_CHECK("pack_weights_kernel");
   return 0;
 }
@@ -1064,7 +1032,7 @@ int hk_conv3x3_wgrad_acc(const float* x, const float* dy, float* dw, float* db, 
   float* dwp = static_cast<float*>(workspace);
   int r = conv3x3_wgrad(x, dy, dwp, db, N, H, W, Cin, Cout, stream, /*zero_db=*/!accumulate);
   if (r) return r;
-  unpack_wgrad_kernel<<<grid_for((size_t)Cout * Cin * 9, 256), 256, 0, stream>>>(dwp, dw, Cout, Cin, accumulate ? 1 : 0);
+  unpack_wgrad_kernel<<<grid_1d((size_t)Cout * Cin * 9, 256), 256, 0, stream>>>(dwp, dw, Cout, Cin, accumulate ? 1 : 0);
   HK_LAUNCH_CHECK("unpack_wgrad_kernel");
   return 0;
 }
@@ -1093,7 +1061,7 @@ int hk_conv3x3_first_fwd(const float* x_nchw, const float* w, const float* bias,
   float* x27 = static_cast<float*>(workspace);
   float* w27 = x27 + (size_t)P * 32;
   const int round = precise() ? 0 : 1;
-  im2col_first_kernel<<<grid_for((size_t)P, 128), 128, 0, stream>>>(x_nchw, x27, N, H, W, round);
+  im2col_first_kernel<<<grid_1d((size_t)P, 128), 128, 0, stream>>>(x_nchw, x27, N, H, W, round);
   HK_LAUNCH_CHECK("im2col_first_kernel");
   pack_first_weights_kernel<<<(Cout * 32 + 127) / 128, 128, 0, stream>>>(w, bias, w27, Cout, round);
   HK_LAUNCH_CHECK("pack_first_weights_kernel");
@@ -1142,7 +1110,7 @@ int hk_maxpool2x2_fwd(const float* x_nhwc, float* y, int N, int H, int W, int C,
   HK_REQUIRE(x_nhwc && y, HK_ERR_ARG, "hk_maxpool2x2_fwd: null pointer");
   HK_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, HK_ERR_UNSUPPORTED, "hk_maxpool2x2_fwd: C%%4, even H/W required");
   const size_t total = (size_t)N * (H / 2) * (W / 2) * (C / 4);
-  maxpool2x2_fwd_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(x_nhwc, y, N, H, W, C, out_nchw);
+  maxpool2x2_fwd_kernel<<<grid_1d(total, 256), 256, 0, (cudaStream_t)stream>>>(x_nhwc, y, N, H, W, C, out_nchw);
   HK_LAUNCH_CHECK("maxpool2x2_fwd_kernel");
   return 0;
 }
@@ -1152,7 +1120,7 @@ int hk_maxpool2x2_bwd(const float* x_nhwc, const float* dy, float* dx_nhwc, int 
   HK_REQUIRE(x_nhwc && dy && dx_nhwc, HK_ERR_ARG, "hk_maxpool2x2_bwd: null pointer");
   HK_REQUIRE(H % 2 == 0 && W % 2 == 0, HK_ERR_UNSUPPORTED, "hk_maxpool2x2_bwd: even H/W required");
   const size_t total = (size_t)N * (H / 2) * (W / 2) * C;
-  maxpool2x2_bwd_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(x_nhwc, dy, dx_nhwc, N, H, W, C, dy_nchw);
+  maxpool2x2_bwd_kernel<<<grid_1d(total, 256), 256, 0, (cudaStream_t)stream>>>(x_nhwc, dy, dx_nhwc, N, H, W, C, dy_nchw);
   HK_LAUNCH_CHECK("maxpool2x2_bwd_kernel");
   return 0;
 }
@@ -1162,7 +1130,7 @@ int hk_maxpool2x2_fwd_idx(const float* x_nhwc, float* y, unsigned char* code, in
   HK_REQUIRE(x_nhwc && y && code, HK_ERR_ARG, "hk_maxpool2x2_fwd_idx: null pointer");
   HK_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, HK_ERR_UNSUPPORTED, "hk_maxpool2x2_fwd_idx: C%%4, even H/W required");
   const size_t total = (size_t)N * (H / 2) * (W / 2) * (C / 4);
-  maxpool2x2_fwd_idx_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(x_nhwc, y, code, N, H, W, C, out_nchw);
+  maxpool2x2_fwd_idx_kernel<<<grid_1d(total, 256), 256, 0, (cudaStream_t)stream>>>(x_nhwc, y, code, N, H, W, C, out_nchw);
   HK_LAUNCH_CHECK("maxpool2x2_fwd_idx_kernel");
   return 0;
 }
@@ -1172,14 +1140,14 @@ int hk_maxpool2x2_bwd_idx(const unsigned char* code, const float* dy, float* dx_
   HK_REQUIRE(code && dy && dx_nhwc, HK_ERR_ARG, "hk_maxpool2x2_bwd_idx: null pointer");
   HK_REQUIRE(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, HK_ERR_UNSUPPORTED, "hk_maxpool2x2_bwd_idx: C%%4, even H/W required");
   const size_t total = (size_t)N * (H / 2) * (W / 2) * (C / 4);
-  maxpool2x2_bwd_idx_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(code, dy, dx_nhwc, N, H, W, C, dy_nchw);
+  maxpool2x2_bwd_idx_kernel<<<grid_1d(total, 256), 256, 0, (cudaStream_t)stream>>>(code, dy, dx_nhwc, N, H, W, C, dy_nchw);
   HK_LAUNCH_CHECK("maxpool2x2_bwd_idx_kernel");
   return 0;
 }
 
 int hk_relu_mask_inplace(float* dy, const float* act, size_t n, void* stream) {
   HK_REQUIRE(dy && act && n % 4 == 0, HK_ERR_ARG, "hk_relu_mask_inplace: bad args");
-  relu_mask_kernel<<<grid_for(n / 4, 256), 256, 0, (cudaStream_t)stream>>>(dy, act, n / 4);
+  relu_mask_kernel<<<grid_1d(n / 4, 256), 256, 0, (cudaStream_t)stream>>>(dy, act, n / 4);
   HK_LAUNCH_CHECK("relu_mask_kernel");
   return 0;
 }

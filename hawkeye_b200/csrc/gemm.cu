@@ -431,32 +431,14 @@ static int make_operand_map(CUtensorMap* tm, const float* P, int mn_major, long 
   return make_tmap(tm, P, 3, dims, strides, box);
 }
 
-static int num_sms() {
-  static int sms = 0;
-  if (!sms) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
-        sms <= 0)
-      sms = 132;
-  }
-  return sms;
-}
-
 template <int BN>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmEpi& epi, int M, int N, int K,
                        int batch, int a_mn, int b_mn, int shareA, int shareB, cudaStream_t stream,
                        const CUtensorMap* tmAl = nullptr, const CUtensorMap* tmBl = nullptr) {
   using Cfg = GemmCfg<BN>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    const int max_smem = GEMM_SMEM_MAX;
-    cudaError_t e = cudaFuncSetAttribute(wgmma_gemm_kernel<BN, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
-    if constexpr (BN == 64)
-      if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(wgmma_gemm_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
-    if (e != cudaSuccess) return set_error((int)e, "cudaFuncSetAttribute(gemm<%d>): %s", BN, cudaGetErrorString(e));
-    attr_set = true;
-  }
+  if (int r = allow_dynamic_smem<wgmma_gemm_kernel<BN, false>>(GEMM_SMEM_MAX, BN == 64 ? "gemm<64>" : "gemm<128>")) return r;
+  if constexpr (BN == 64)
+    if (int r = allow_dynamic_smem<wgmma_gemm_kernel<64, true>>(GEMM_SMEM_MAX, "gemm<64>")) return r;
   const int tiles_m = (M + 127) / 128, tiles_n = (N + BN - 1) / BN;
   const long long total = (long long)tiles_m * tiles_n * batch;
   if (total >= (1ll << 31)) return set_error(HK_ERR_UNSUPPORTED, "gemm: too many tiles");
@@ -497,9 +479,7 @@ __global__ void tf32_split_kernel(const float* __restrict__ x, float* __restrict
 
 int tf32_split(const float* x, float* hi, float* lo, size_t n, cudaStream_t stream) {
   if (!n) return 0;
-  size_t g = (n + 255) / 256;
-  if (g > 132 * 16) g = 132 * 16;
-  tf32_split_kernel<<<(unsigned)g, 256, 0, stream>>>(x, hi, lo, n);
+  tf32_split_kernel<<<grid_1d(n, 256), 256, 0, stream>>>(x, hi, lo, n);
   HK_LAUNCH_CHECK("tf32_split_kernel");
   return 0;
 }
@@ -571,6 +551,19 @@ int gemm_tf32_pair(const float* Ah, const float* Al, int a_mn, long long lda, lo
   return launch_gemm<64>(tmA, tmB, epi, M, N, K, batch, a_mn, b_mn, shareA, shareB, stream, &tmAl, &tmBl);
 }
 
+// the epilogue of hk_gemm_tf32 / hk_gemm_3xtf32 (see the public header)
+static GemmEpi plain_epi(float* C, long long ldc, long long strideC, int trans_c, float alpha, const float* alpha_vec,
+                         float diag, const float* D, long long ldd, long long strideD, float beta, const float* beta_vec,
+                         int relu) {
+  GemmEpi epi;
+  epi.C = C; epi.ldc = ldc; epi.strideC = strideC;
+  epi.D = D; epi.ldd = ldd; epi.strideD = strideD;
+  epi.alpha_vec = alpha_vec; epi.beta_vec = beta_vec;
+  epi.alpha = alpha; epi.beta = beta; epi.diag = diag;
+  epi.trans_c = trans_c; epi.relu = relu;
+  return epi;
+}
+
 }  // namespace hk
 
 // same signature as hk_gemm_tf32, always 3xTF32 (callers whose result feeds an exponential: CIN's softmax(-Gram))
@@ -579,17 +572,10 @@ extern "C" int hk_gemm_3xtf32(const float* A, int a_mn_major, long long lda, lon
                               long long strideC, int trans_c, int M, int N, int K, int batch, float alpha,
                               const float* alpha_vec, float diag, const float* D, long long ldd, long long strideD,
                               float beta, const float* beta_vec, int relu, void* stream) {
-  hk::GemmEpi epi;
-  epi.C = C; epi.ldc = ldc; epi.strideC = strideC;
-  epi.D = D; epi.ldd = ldd; epi.strideD = strideD;
-  epi.alpha_vec = alpha_vec; epi.beta_vec = beta_vec;
-  epi.alpha = alpha; epi.beta = beta; epi.diag = diag;
-  epi.trans_c = trans_c; epi.relu = relu;
-  epi.C_lo = nullptr; epi.D_lo = nullptr; epi.E = nullptr; epi.ldE = 0; epi.strideE = 0;
-  epi.post_scale = nullptr; epi.post_eps = 0.f; epi.mode = hk::EPI_PLAIN;
   HK_REQUIRE(A && B && C && M > 0 && N > 0 && K > 0 && batch > 0, HK_ERR_ARG, "hk_gemm_3xtf32: bad args");
-  return hk::gemm_tf32_3x(A, a_mn_major, lda, strideA, B, b_mn_major, ldb, strideB, epi, M, N, K, batch,
-                          static_cast<cudaStream_t>(stream));
+  return hk::gemm_tf32_3x(A, a_mn_major, lda, strideA, B, b_mn_major, ldb, strideB,
+                          hk::plain_epi(C, ldc, strideC, trans_c, alpha, alpha_vec, diag, D, ldd, strideD, beta, beta_vec, relu),
+                          M, N, K, batch, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int hk_gemm_tf32(const float* A, int a_mn_major, long long lda, long long strideA, const float* B,
@@ -597,14 +583,7 @@ extern "C" int hk_gemm_tf32(const float* A, int a_mn_major, long long lda, long 
                             long long strideC, int trans_c, int M, int N, int K, int batch, float alpha,
                             const float* alpha_vec, float diag, const float* D, long long ldd, long long strideD,
                             float beta, const float* beta_vec, int relu, void* stream) {
-  hk::GemmEpi epi;
-  epi.C = C; epi.ldc = ldc; epi.strideC = strideC;
-  epi.D = D; epi.ldd = ldd; epi.strideD = strideD;
-  epi.alpha_vec = alpha_vec; epi.beta_vec = beta_vec;
-  epi.alpha = alpha; epi.beta = beta; epi.diag = diag;
-  epi.trans_c = trans_c; epi.relu = relu;
-  epi.C_lo = nullptr; epi.D_lo = nullptr; epi.E = nullptr; epi.ldE = 0; epi.strideE = 0;
-  epi.post_scale = nullptr; epi.post_eps = 0.f; epi.mode = hk::EPI_PLAIN;
-  return hk::gemm_tf32(A, a_mn_major, lda, strideA, B, b_mn_major, ldb, strideB, epi, M, N, K, batch,
-                       static_cast<cudaStream_t>(stream));
+  return hk::gemm_tf32(A, a_mn_major, lda, strideA, B, b_mn_major, ldb, strideB,
+                       hk::plain_epi(C, ldc, strideC, trans_c, alpha, alpha_vec, diag, D, ldd, strideD, beta, beta_vec, relu),
+                       M, N, K, batch, static_cast<cudaStream_t>(stream));
 }

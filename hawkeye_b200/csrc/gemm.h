@@ -1,40 +1,45 @@
 // Epilogue description + host entry of the generic batched wgmma TF32 GEMM (gemm.cu).
 #pragma once
 #include <cuda_runtime.h>
+#include <type_traits>
 
 namespace hk {
 
+enum { EPI_PLAIN = 0, EPI_BILINEAR_S = 1, EPI_SKETCH = 2 };
+
+// Every field defaults to null / zero / EPI_PLAIN; callers set the ones they use.
 struct GemmEpi {
-  float* C;
-  long long ldc, strideC;
-  const float* D;
-  long long ldd, strideD;
-  const float* alpha_vec;
-  const float* beta_vec;
-  float alpha, beta, diag;
-  int trans_c;
-  int relu;            // bit0: ReLU, bit1: round the stored value to tf32
-  float* C_lo;         // optional: store C as a (hi, lo) tf32 pair (3xTF32 operands for the next GEMM)
-  const float* D_lo;   // optional: D given as a (hi, lo) pair
-  const float* E;      // optional: raw partial product added to the accumulator before alpha (row-major [M][N] per batch)
-  long long ldE, strideE;   // layout of E; 0 = same as C (ldc / strideC)
-  const float* post_scale;  // optional [batch]: value = sqrt(alpha_b * acc + post_eps) * post_scale[b], then D / ReLU / rounding
-  float post_eps;
+  float* C = nullptr;
+  long long ldc = 0, strideC = 0;
+  const float* D = nullptr;
+  long long ldd = 0, strideD = 0;
+  const float* alpha_vec = nullptr;
+  const float* beta_vec = nullptr;
+  float alpha = 0.f, beta = 0.f, diag = 0.f;
+  int trans_c = 0;
+  int relu = 0;                  // bit0: ReLU, bit1: round the stored value to tf32
+  float* C_lo = nullptr;         // optional: store C as a (hi, lo) tf32 pair (3xTF32 operands for the next GEMM)
+  const float* D_lo = nullptr;   // optional: D given as a (hi, lo) pair
+  const float* E = nullptr;      // optional: raw partial product added to the accumulator before alpha (row-major [M][N] per batch)
+  long long ldE = 0, strideE = 0;   // layout of E; 0 = same as C (ldc / strideC)
+  const float* post_scale = nullptr;  // optional [batch]: value = sqrt(alpha_b * acc + post_eps) * post_scale[b], then D / ReLU / rounding
+  float post_eps = 0.f;
   // Fused consumers of a square Gram G = alpha_b * acc (M = N = C, row-major [C][C] per batch entry):
   //   EPI_BILINEAR_S: C[i][j] = (dY[i][j] + dY[j][i]) / (2 z_ij), z_ij = sqrt(G_ij + post_eps); c_raw[b] += sum_ij dY_ij z_ij
   //                   (c_raw pre-zeroed) — the bilinear-pool backward's S without the Gram going through memory;
   //   EPI_SKETCH    : bins[b][(h1[i] + h2[j]) mod d] += s1[i] s2[j] G_ij (bins pre-zeroed); C is not written.
-  int mode;
-  const float* dY;
-  double* c_raw;
-  const int* h1;
-  const int* h2;
-  const float* s1;
-  const float* s2;
-  float* bins;
-  int d;
+  int mode = EPI_PLAIN;
+  const float* dY = nullptr;
+  double* c_raw = nullptr;
+  const int* h1 = nullptr;
+  const int* h2 = nullptr;
+  const float* s1 = nullptr;
+  const float* s2 = nullptr;
+  float* bins = nullptr;
+  int d = 0;
 };
-enum { EPI_PLAIN = 0, EPI_BILINEAR_S = 1, EPI_SKETCH = 2 };
+static_assert(std::is_aggregate_v<GemmEpi> && std::is_trivially_copyable_v<GemmEpi>,
+              "GemmEpi is passed to the GEMM kernel by value");
 
 // C[b] = alpha_b * (A[b].B[b] + E[b]) + diag*I + beta_b * (D[b] + D_lo[b]);  see hk_gemm_tf32 in the public header.
 // Dispatches on the precision mode (host.h): one TF32 pass, or 3xTF32 over internally split operands.

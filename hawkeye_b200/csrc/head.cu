@@ -133,12 +133,6 @@ __global__ void normalize_u8_kernel(const unsigned char* __restrict__ x, float* 
   }
 }
 
-static inline int grid_for(size_t n, int block) {
-  size_t g = (n + block - 1) / block;
-  const size_t cap = 132 * 16;
-  return (int)(g < cap ? (g ? g : 1) : cap);
-}
-
 }  // namespace hk
 
 using namespace hk;
@@ -213,7 +207,7 @@ int hk_normalize_u8(const unsigned char* x_nhwc, float* y_nchw, int N, int H, in
   HK_REQUIRE(x_nhwc && y_nchw && N > 0 && H > 0 && W > 0, HK_ERR_ARG, "hk_normalize_u8: bad args");
   HK_REQUIRE(std0 > 0.f && std1 > 0.f && std2 > 0.f, HK_ERR_ARG, "hk_normalize_u8: std must be positive");
   const size_t hw = (size_t)H * W, npix = hw * N;
-  normalize_u8_kernel<<<grid_for(npix, 256), 256, 0, (cudaStream_t)stream>>>(x_nhwc, y_nchw, npix, hw, mean0, mean1, mean2,
+  normalize_u8_kernel<<<grid_1d(npix, 256), 256, 0, (cudaStream_t)stream>>>(x_nhwc, y_nchw, npix, hw, mean0, mean1, mean2,
                                                                             1.f / std0, 1.f / std1, 1.f / std2);
   HK_LAUNCH_CHECK("normalize_u8_kernel");
   return 0;
@@ -223,7 +217,7 @@ int hk_sgd_momentum(float* p, const float* g, float* buf, size_t n, float lr, fl
                     float grad_scale, int first_step, void* stream) {
   HK_REQUIRE(p && g && buf, HK_ERR_ARG, "hk_sgd_momentum: null pointer");
   HK_REQUIRE(aligned16(p) && aligned16(g) && aligned16(buf), HK_ERR_ALIGN, "hk_sgd_momentum: unaligned pointer");
-  sgd_momentum_kernel<<<grid_for(n / 4 + 1, 256), 256, 0, (cudaStream_t)stream>>>(p, g, buf, n, lr, momentum,
+  sgd_momentum_kernel<<<grid_1d(n / 4 + 1, 256), 256, 0, (cudaStream_t)stream>>>(p, g, buf, n, lr, momentum,
                                                                                  weight_decay, grad_scale, first_step);
   HK_LAUNCH_CHECK("sgd_momentum_kernel");
   return 0;
@@ -233,7 +227,7 @@ int hk_adam(float* p, const float* g, float* m, float* v, size_t n, float lr, fl
             float weight_decay, float grad_scale, int step, void* stream) {
   HK_REQUIRE(p && g && m && v && step >= 1, HK_ERR_ARG, "hk_adam: bad args");
   const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
-  adam_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(p, g, m, v, n, lr, beta1, beta2, eps, weight_decay,
+  adam_kernel<<<grid_1d(n, 256), 256, 0, (cudaStream_t)stream>>>(p, g, m, v, n, lr, beta1, beta2, eps, weight_decay,
                                                                  grad_scale, bc1, bc2);
   HK_LAUNCH_CHECK("adam_kernel");
   return 0;

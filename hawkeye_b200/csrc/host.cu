@@ -22,6 +22,17 @@ bool precise() {
   return v != 0;
 }
 
+int num_sms() {
+  static const int sms = [] {
+    int dev = 0, n = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        n <= 0)
+      return H100_SMS;
+    return n;
+  }();
+  return sms;
+}
+
 Scratch::Scratch(size_t bytes, cudaStream_t stream) : s(stream) {
   if (cudaMallocAsync(&p, bytes ? bytes : 16, s) != cudaSuccess) { p = nullptr; (void)cudaGetLastError(); }
 }

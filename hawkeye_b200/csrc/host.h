@@ -1,5 +1,6 @@
 // Host-side helpers shared by the C-ABI translation units: error convention
 // (0 ok / <0 argument error, no launch / >0 cudaError_t), thread-local last-error text,
+// launch sizing (grid-stride grids, SM count, dynamic shared-memory opt-in)
 // and CUtensorMap construction through the driver entry point (no libcuda link dependency).
 #pragma once
 #include <cuda.h>
@@ -24,6 +25,29 @@ int check_launch(const char* what);
 extern std::atomic<long long> g_launches;  // kernels launched by this library (all host threads)
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+constexpr int H100_SMS = 132;   // SMs of an H100 SXM
+
+// Grid of a grid-stride kernel over n items: one thread per item, at least one block. The grid is capped at 16 blocks
+// per SM: with 256-thread blocks that is two full waves (an SM holds 2048 threads), enough to keep every SM busy, and
+// each thread's stride loop covers the remaining items more cheaply than further blocks would.
+inline int grid_1d(size_t n, int block) {
+  const size_t g = (n + block - 1) / block, cap = (size_t)H100_SMS * 16;
+  return (int)(g < cap ? (g ? g : 1) : cap);
+}
+
+// SM count of the current device, looked up once per process (H100_SMS if the query fails).
+int num_sms();
+
+// Raise Kernel's dynamic shared-memory limit to `bytes` (above the 48 KB default). The attribute is set once per
+// kernel: forward launches run on the caller's thread and backward launches on autograd's, and a function-local
+// static is initialised exactly once even when both get here first at the same time. A failure is kept and returned
+// on every call.
+template <auto Kernel>
+int allow_dynamic_smem(int bytes, const char* what) {
+  static const cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  return e == cudaSuccess ? 0 : set_error((int)e, "cudaFuncSetAttribute(%s): %s", what, cudaGetErrorString(e));
+}
 
 // Encode a tiled fp32 tensor map with SWIZZLE_128B and zero OOB fill.
 // dims/box are innermost-first; strides_bytes[i] is the byte stride of dim i+1 (rank-1 entries).

@@ -15,12 +15,6 @@ namespace hk {
 
 struct Pair { float* hi; float* lo; };
 
-static inline int grid_for(size_t n, int block) {
-  size_t g = (n + block - 1) / block;
-  const size_t cap = 132 * 16;
-  return (int)(g < cap ? (g ? g : 1) : cap);
-}
-
 // C(hi,lo | full) = alpha*alpha_vec[b] * (A.B) + diag*I + beta * D(hi+lo)     A,B,D: [batch][n][n] row-major pairs
 static int mm3(Pair A, Pair B, Pair C, float* tmp, int n, int batch, float alpha, const float* alpha_vec, float diag,
                const Pair* D, float beta, cudaStream_t st) {
@@ -228,8 +222,8 @@ int hk_sqrtm_fwd(const float* x, float* y, float* saved, int B, int n, int iterN
   trace_normalize_kernel<<<B, 256, 0, st>>>(x, sv.normA, sv.A.hi, sv.A.lo, n);
   HK_LAUNCH_CHECK("trace_normalize_kernel");
   // ZY = 0.5 (3I - A) ; Z_0 = ZY ; Y_0 = A . ZY                                     (MPNCOV.py:153-155)
-  affine_diag_split_kernel<<<grid_for(S, 256), 256, 0, st>>>(sv.A.hi, sv.A.lo, sv.Z(0).hi, sv.Z(0).lo, -0.5f, nullptr, 0,
-                                                          1.5f, n, S);
+  affine_diag_split_kernel<<<grid_1d(S, 256), 256, 0, st>>>(sv.A.hi, sv.A.lo, sv.Z(0).hi, sv.Z(0).lo, -0.5f, nullptr, 0,
+                                                            1.5f, n, S);
   HK_LAUNCH_CHECK("affine_diag_split_kernel");
   if ((r = mm3(sv.A, sv.Z(0), sv.Y(0), tmp, n, B, 1.f, nullptr, 0.f, nullptr, 0.f, st))) return r;
   for (int i = 1; i < L; ++i) {                                                   // (MPNCOV.py:156-159)
@@ -240,7 +234,7 @@ int hk_sqrtm_fwd(const float* x, float* y, float* saved, int B, int n, int iterN
   // YZY = 0.5 Y (3I - Z Y) ; y = YZY sqrt(normA)                                   (MPNCOV.py:160-161)
   if ((r = mm3(sv.Z(L - 1), sv.Y(L - 1), T, tmp, n, B, -1.f, nullptr, 3.f, nullptr, 0.f, st))) return r;
   if ((r = mm3(sv.Y(L - 1), T, ZY, tmp, n, B, 0.5f, nullptr, 0.f, nullptr, 0.f, st))) return r;
-  pair_combine_scale_kernel<<<grid_for(S, 256), 256, 0, st>>>(ZY.hi, ZY.lo, y, sv.normA, 1, (size_t)n * n, S);
+  pair_combine_scale_kernel<<<grid_1d(S, 256), 256, 0, st>>>(ZY.hi, ZY.lo, y, sv.normA, 1, (size_t)n * n, S);
   HK_LAUNCH_CHECK("pair_combine_scale_kernel");
   return 0;
 }
@@ -265,7 +259,7 @@ int hk_sqrtm_bwd(const float* x, const float* y, const float* g, float* saved, f
        acc = newp(), E1 = newp();   // 11 pairs = 22 matrices + tmp = 23
   int r;
   // der_postCom = g sqrt(normA)                                                       (MPNCOV.py:174)
-  affine_diag_split_kernel<<<grid_for(S, 256), 256, 0, st>>>(g, nullptr, P.hi, P.lo, 1.f, sv.normA, 1, 0.f, n, S);
+  affine_diag_split_kernel<<<grid_1d(S, 256), 256, 0, st>>>(g, nullptr, P.hi, P.lo, 1.f, sv.normA, 1, 0.f, n, S);
   HK_LAUNCH_CHECK("affine_diag_split_kernel");
   const Pair Yl = sv.Y(L - 1), Zl = sv.Z(L - 1);
   // dldY = 0.5 (P (3I - Yl Zl) - Zl Yl P)                                            (MPNCOV.py:180-181)
@@ -294,7 +288,7 @@ int hk_sqrtm_bwd(const float* x, const float* y, const float* g, float* saved, f
     t = dZ; dZ = dZ2; dZ2 = t;
   }
   // der_NSiter = 0.5 (dldY (3I - A) - dldZ - A dldY)                                  (MPNCOV.py:194)
-  affine_diag_split_kernel<<<grid_for(S, 256), 256, 0, st>>>(sv.A.hi, sv.A.lo, E1.hi, E1.lo, -1.f, nullptr, 0, 3.f, n, S);
+  affine_diag_split_kernel<<<grid_1d(S, 256), 256, 0, st>>>(sv.A.hi, sv.A.lo, E1.hi, E1.lo, -1.f, nullptr, 0, 3.f, n, S);
   HK_LAUNCH_CHECK("affine_diag_split_kernel");
   if ((r = mm3(dY, E1, U, tmp, n, B, 1.f, nullptr, 0.f, nullptr, 0.f, st))) return r;
   if ((r = mm3(sv.A, dY, acc, tmp, n, B, -0.5f, nullptr, 0.f, &U, 0.5f, st))) return r;   // acc = 0.5 dldY(3I-A) - 0.5 A dldY

@@ -9,12 +9,6 @@
 
 namespace hk {
 
-static inline int rgrid(size_t n, int block) {
-  size_t g = (n + block - 1) / block;
-  const size_t cap = 132 * 16;
-  return (int)(g < cap ? (g ? g : 1) : cap);
-}
-
 // ------------------------------------------------------------------------------------------------ stem (resnet.py:176)
 // X147[pix][ci*49 + kh*7 + kw] = x[n][ci][2*ho+kh-3][2*wo+kw-3] (0 outside), columns 147..159 = 0; tf32-rounded
 __global__ void stem_im2col_kernel(const float* __restrict__ x, float* __restrict__ o, int N, int H, int W, int Ho,
@@ -388,7 +382,7 @@ extern "C" {
 int hk_stem_im2col(const float* x_nchw, float* x147, int N, int H, int W, void* stream) {
   HK_REQUIRE(x_nchw && x147, HK_ERR_ARG, "hk_stem_im2col: null pointer");
   const int Ho = (H + 6 - 7) / 2 + 1, Wo = (W + 6 - 7) / 2 + 1;
-  stem_im2col_kernel<<<rgrid((size_t)N * Ho * Wo * 40, 256), 256, 0, (cudaStream_t)stream>>>(x_nchw, x147, N, H, W, Ho, Wo, precise() ? 0 : 1);
+  stem_im2col_kernel<<<grid_1d((size_t)N * Ho * Wo * 40, 256), 256, 0, (cudaStream_t)stream>>>(x_nchw, x147, N, H, W, Ho, Wo, precise() ? 0 : 1);
   HK_LAUNCH_CHECK("stem_im2col_kernel");
   return 0;
 }
@@ -416,8 +410,8 @@ int hk_bn_fwd(const float* x, const float* gamma, const float* beta, const float
   bn_stats_finalize_kernel<<<(C + 31) / 32, 1024, 0, st>>>(part, nb, P, C, eps, momentum, save_mean, save_invstd,
                                                          running_mean, running_var);
   HK_LAUNCH_CHECK("bn_stats_finalize_kernel");
-  bn_apply_kernel<<<rgrid((size_t)P * C4, 256), 256, 0, st>>>(x, save_mean, save_invstd, gamma, beta, residual, y,
-                                                            (size_t)P * C4, C4, relu, precise() ? 0 : 1);
+  bn_apply_kernel<<<grid_1d((size_t)P * C4, 256), 256, 0, st>>>(x, save_mean, save_invstd, gamma, beta, residual, y,
+                                                                (size_t)P * C4, C4, relu, precise() ? 0 : 1);
   HK_LAUNCH_CHECK("bn_apply_kernel");
   return 0;
 }
@@ -426,8 +420,8 @@ int hk_bn_fwd(const float* x, const float* gamma, const float* beta, const float
 int hk_bn_apply(const float* x, const float* mean, const float* invstd, const float* gamma, const float* beta,
                 const float* residual, float* y, long long P, int C, int relu, void* stream_) {
   HK_REQUIRE(x && mean && invstd && gamma && beta && y && C % 4 == 0, HK_ERR_ARG, "hk_bn_apply: bad args");
-  bn_apply_kernel<<<rgrid((size_t)P * (C / 4), 256), 256, 0, (cudaStream_t)stream_>>>(x, mean, invstd, gamma, beta, residual, y,
-                                                                                   (size_t)P * (C / 4), C / 4, relu, precise() ? 0 : 1);
+  bn_apply_kernel<<<grid_1d((size_t)P * (C / 4), 256), 256, 0, (cudaStream_t)stream_>>>(x, mean, invstd, gamma, beta, residual, y,
+                                                                                        (size_t)P * (C / 4), C / 4, relu, precise() ? 0 : 1);
   HK_LAUNCH_CHECK("bn_apply_kernel");
   return 0;
 }
@@ -458,8 +452,8 @@ int hk_bn_bwd_ex(const float* x, const float* y, const float* dy, const float* g
   HK_LAUNCH_CHECK("bn_bwd_partial_kernel");
   bn_bwd_finalize_kernel<<<(C + 31) / 32, 1024, 0, st>>>(part, nb, C, dgamma, dbeta);
   HK_LAUNCH_CHECK("bn_bwd_finalize_kernel");
-  bn_bwd_apply_kernel<<<rgrid((size_t)P * C4, 256), 256, 0, st>>>(x, y, dy, save_mean, save_invstd, gamma, dgamma, dbeta, beta,
-                                                                dx, dres, (size_t)P * C4, C4, 1.f / (float)P, relu, precise() ? 0 : 1);
+  bn_bwd_apply_kernel<<<grid_1d((size_t)P * C4, 256), 256, 0, st>>>(x, y, dy, save_mean, save_invstd, gamma, dgamma, dbeta, beta,
+                                                                    dx, dres, (size_t)P * C4, C4, 1.f / (float)P, relu, precise() ? 0 : 1);
   HK_LAUNCH_CHECK("bn_bwd_apply_kernel");
   return 0;
 }
@@ -467,7 +461,7 @@ int hk_bn_bwd_ex(const float* x, const float* y, const float* dy, const float* g
 int hk_maxpool3x3s2_fwd(const float* x, float* y, unsigned char* argmax, int N, int H, int W, int C, void* stream) {
   HK_REQUIRE(x && y && C % 4 == 0, HK_ERR_ARG, "hk_maxpool3x3s2_fwd: bad args");
   const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
-  maxpool3x3s2_fwd_kernel<<<rgrid((size_t)N * Ho * Wo * (C / 4), 256), 256, 0, (cudaStream_t)stream>>>(x, y, argmax, N, H, W, C, Ho, Wo);
+  maxpool3x3s2_fwd_kernel<<<grid_1d((size_t)N * Ho * Wo * (C / 4), 256), 256, 0, (cudaStream_t)stream>>>(x, y, argmax, N, H, W, C, Ho, Wo);
   HK_LAUNCH_CHECK("maxpool3x3s2_fwd_kernel");
   return 0;
 }
@@ -475,35 +469,37 @@ int hk_maxpool3x3s2_bwd(const unsigned char* argmax, const float* dy, float* dx,
                         void* stream) {
   HK_REQUIRE(argmax && dy && dx && C % 4 == 0, HK_ERR_ARG, "hk_maxpool3x3s2_bwd: bad args");
   const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
-  maxpool3x3s2_bwd_kernel<<<rgrid((size_t)N * H * W * (C / 4), 256), 256, 0, (cudaStream_t)stream>>>(argmax, dy, dx, N, H, W, C, Ho, Wo);
+  maxpool3x3s2_bwd_kernel<<<grid_1d((size_t)N * H * W * (C / 4), 256), 256, 0, (cudaStream_t)stream>>>(argmax, dy, dx, N, H, W, C, Ho, Wo);
   HK_LAUNCH_CHECK("maxpool3x3s2_bwd_kernel");
   return 0;
 }
 int hk_subsample2(const float* x, float* y, int N, int H, int W, int C, void* stream) {
   HK_REQUIRE(x && y && C % 4 == 0, HK_ERR_ARG, "hk_subsample2: bad args");
-  subsample2_kernel<<<rgrid((size_t)N * ((H + 1) / 2) * ((W + 1) / 2) * (C / 4), 256), 256, 0, (cudaStream_t)stream>>>(x, y, N, H, W, C / 4);
+  subsample2_kernel<<<grid_1d((size_t)N * ((H + 1) / 2) * ((W + 1) / 2) * (C / 4), 256), 256, 0, (cudaStream_t)stream>>>(x, y, N, H, W, C / 4);
   HK_LAUNCH_CHECK("subsample2_kernel");
   return 0;
 }
 int hk_upsample2_zero(const float* y, float* x, int N, int H, int W, int C, void* stream) {
   HK_REQUIRE(x && y && C % 4 == 0, HK_ERR_ARG, "hk_upsample2_zero: bad args");
-  upsample2_zero_kernel<<<rgrid((size_t)N * H * W * (C / 4), 256), 256, 0, (cudaStream_t)stream>>>(y, x, N, H, W, C / 4);
+  upsample2_zero_kernel<<<grid_1d((size_t)N * H * W * (C / 4), 256), 256, 0, (cudaStream_t)stream>>>(y, x, N, H, W, C / 4);
   HK_LAUNCH_CHECK("upsample2_zero_kernel");
   return 0;
 }
 int hk_add_inplace(float* a, const float* b, size_t n, void* stream) {
   HK_REQUIRE(a && b && n % 4 == 0, HK_ERR_ARG, "hk_add_inplace: bad args");
-  add_inplace_kernel<<<rgrid(n / 4, 256), 256, 0, (cudaStream_t)stream>>>(a, b, n / 4);
+  add_inplace_kernel<<<grid_1d(n / 4, 256), 256, 0, (cudaStream_t)stream>>>(a, b, n / 4);
   HK_LAUNCH_CHECK("add_inplace_kernel");
   return 0;
 }
 int hk_nhwc_to_nchw(const float* x, float* y, int N, int HW, int C, void* stream) {
-  nhwc_to_nchw_kernel<<<rgrid((size_t)N * HW * C, 256), 256, 0, (cudaStream_t)stream>>>(x, y, N, HW, C);
+  HK_REQUIRE(x && y, HK_ERR_ARG, "hk_nhwc_to_nchw: null pointer");
+  nhwc_to_nchw_kernel<<<grid_1d((size_t)N * HW * C, 256), 256, 0, (cudaStream_t)stream>>>(x, y, N, HW, C);
   HK_LAUNCH_CHECK("nhwc_to_nchw_kernel");
   return 0;
 }
 int hk_nchw_to_nhwc(const float* x, float* y, int N, int HW, int C, void* stream) {
-  nchw_to_nhwc_kernel<<<rgrid((size_t)N * HW * C, 256), 256, 0, (cudaStream_t)stream>>>(x, y, N, HW, C);
+  HK_REQUIRE(x && y, HK_ERR_ARG, "hk_nchw_to_nhwc: null pointer");
+  nchw_to_nhwc_kernel<<<grid_1d((size_t)N * HW * C, 256), 256, 0, (cudaStream_t)stream>>>(x, y, N, HW, C);
   HK_LAUNCH_CHECK("nchw_to_nhwc_kernel");
   return 0;
 }
@@ -527,7 +523,7 @@ int hk_matconv_wgrad(const float* x, const float* dy, float* dw, long long P, in
   e.C = S == 1 ? dw : part; e.ldc = K; e.strideC = (long long)Cout * K; e.alpha = 1.f;
   int r = gemm_tf32(dy, 1, Cout, Kc * Cout, x, 1, K, Kc * K, e, Cout, K, (int)Kc, S, st);
   if (r || S == 1) return r;
-  reduce_partials_kernel<<<rgrid((size_t)Cout * K, 256), 256, 0, st>>>(part, dw, (size_t)Cout * K, S);
+  reduce_partials_kernel<<<grid_1d((size_t)Cout * K, 256), 256, 0, st>>>(part, dw, (size_t)Cout * K, S);
   HK_LAUNCH_CHECK("reduce_partials_kernel");
   return 0;
 }

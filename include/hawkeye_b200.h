@@ -23,7 +23,7 @@ extern "C" {
 
 const char* hk_version(void);
 const char* hk_last_error(void);
-long long hk_launch_count(void);      /* kernels launched by this library on the calling thread */
+long long hk_launch_count(void);      /* kernels launched by this library, counted over all host threads */
 void hk_reset_launch_count(void);
 
 /* ---- precision mode (process-wide; default 0, or $HK_PRECISE at first use) ---------------------------------------

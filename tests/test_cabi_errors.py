@@ -93,3 +93,37 @@ def test_round2_entry_points_argument_errors(lib):
     assert lib.hk_l2norm_rows_bwd(FAKE, FAKE, None, FAKE, 4, 64, None) == -1
     assert lib.hk_npair_loss(FAKE, FAKE, FAKE, None, FAKE, 8, None) == -1
     assert lib.hk_npair_loss(FAKE, FAKE, FAKE, FAKE, FAKE, 0, None) == -1
+
+
+# Calls every `int hk_*` entry point that takes a pointer with all pointers null and small positive scalars, and prints
+# each one that does not reject the call with a return < 0 and a last-error text.
+_NULL_POINTER_CALLS = r'''
+import ctypes
+from hawkeye_b200 import _lib
+lib = _lib.lib()
+raw_error = ctypes.CDLL(_lib.LIB_PATH).hk_last_error
+raw_error.restype = ctypes.c_void_p
+error_buf = raw_error()                  # this thread's last-error text; cleared before every call
+for name, (res, argtypes, _) in sorted(_lib.parse_header().items()):
+    if res is not ctypes.c_int or ctypes.c_void_p not in argtypes:
+        continue
+    args = [None if t is ctypes.c_void_p else t(0.5) if t is ctypes.c_float else t(8) for t in argtypes]
+    ctypes.memset(error_buf, 0, 1)
+    rc = getattr(lib, name)(*args)
+    msg = lib.hk_last_error().decode()
+    if rc >= 0 or not msg:
+        print(f'{name}: returned {rc}, last error {msg!r}')
+'''
+
+
+def test_null_pointers_are_rejected_at_every_entry_point(lib):
+    """The header promises that an argument error returns < 0 and launches nothing. The calls run in a child process
+    that sees no GPU, so an entry point that skipped its checks fails to launch instead of touching a device."""
+    import os
+    import subprocess
+    import sys
+    repo = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    p = subprocess.run([sys.executable, '-c', _NULL_POINTER_CALLS], cwd=repo, capture_output=True, text=True,
+                       env=dict(os.environ, CUDA_VISIBLE_DEVICES=''), timeout=300)
+    assert p.returncode == 0, p.stderr
+    assert p.stdout == '', p.stdout
