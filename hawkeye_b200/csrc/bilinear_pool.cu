@@ -247,7 +247,6 @@ namespace hk {
 static int bilinear_bwd_impl(const float* x, const float* dy, float* dx, int B, int C, int HW, float inv_hw, float* S,
                              float* partial, float* svec, float* invn, double* craw, float* alpha, float* beta,
                              cudaStream_t stream) {
-  void* stream_ = stream;
   int r;
   // tf32 mode: the column sums see what the tensor core sees (truncated operands); the launch also zeroes c_raw
   colsum_partial_kernel<<<dim3(B, COLSUM_SPLITS), 256, colsum_smem(HW), stream>>>(x, partial, C, HW, COLSUM_SPLITS,
@@ -268,8 +267,13 @@ static int bilinear_bwd_impl(const float* x, const float* dy, float* dx, int B, 
   HK_LAUNCH_CHECK("bilinear_bwd_scalars_kernel");
   // dX = alpha_b * (S . X) + beta_b * 1 s^T      (M=C, K=C, N=HW; X is the MN-major B operand); in tf32 mode rounded: it is
   // the dY operand of the last conv's dgrad / wgrad MMAs
-  return hk_gemm_tf32(S, 0, C, (long long)C * C, x, 1, HW, (long long)C * HW, dx, HW, (long long)C * HW, 0, C, HW, C, B,
-                      1.f, alpha, 0.f, svec, 0, HW, 1.f, beta, precise() ? 0 : 2, stream_);
+  e = {};
+  e.C = dx; e.ldc = HW; e.strideC = (long long)C * HW;
+  e.alpha = 1.f; e.alpha_vec = alpha;
+  e.D = svec; e.ldd = 0; e.strideD = HW;             // ldd 0: the row s^T is added to every row
+  e.beta = 1.f; e.beta_vec = beta;
+  e.relu = precise() ? 0 : 2;
+  return gemm_tf32(S, 0, C, (long long)C * C, x, 1, HW, (long long)C * HW, e, C, HW, C, B, stream);
 }
 }  // namespace hk
 
@@ -414,8 +418,10 @@ int hk_cbp_bwd(const float* x, const float* pre, const float* dy, const int* h1,
   cbp_build_s_kernel<<<dim3(H100_SMS, B), 256, 0, stream>>>(dpre, h1, h2, s1, s2, S, C, d, precise() ? 0 : 1);
   HK_LAUNCH_CHECK("cbp_build_s_kernel");
   // dX = (dG + dG^T) . X      (M = C, K = C, N = HW; X is the MN-major B operand)
-  return hk_gemm_tf32(S, 0, C, (long long)C * C, x, 1, HWp, (long long)C * HWp, dx, HW, (long long)C * HW, 0, C, HW, C, B,
-                      1.f, nullptr, 0.f, nullptr, 0, 0, 0.f, nullptr, 2, stream_);
+  GemmEpi e = {};
+  e.C = dx; e.ldc = HW; e.strideC = (long long)C * HW; e.alpha = 1.f;
+  e.relu = 2;
+  return gemm_tf32(S, 0, C, (long long)C * C, x, 1, HWp, (long long)C * HWp, e, C, HW, C, B, stream);
 }
 
 }  // extern "C"

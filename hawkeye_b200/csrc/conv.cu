@@ -12,6 +12,7 @@
 
 #include "common.cuh"
 #include "host.h"
+#include "gemm.h"
 #include "../../include/hawkeye_b200.h"
 
 namespace hk {
@@ -820,17 +821,6 @@ __global__ void pack_first_weights_kernel(const float* __restrict__ w, const flo
   const float t = r < 27 ? w[co * 27 + r] : (r == 27 && bias ? bias[co] : 0.f);
   w27[i] = round ? tf32_round(t) : t;
 }
-// dw[co][r] = sum_s part[s][co][r] (r<27), db[co] = sum_s part[s][co][27]
-__global__ void first_wgrad_reduce_kernel(const float* __restrict__ part, float* __restrict__ dw,
-                                          float* __restrict__ db, int Cout, int S, int accumulate) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= Cout * 28) return;
-  const int co = i / 28, r = i % 28;
-  float s = 0.f;
-  for (int k = 0; k < S; ++k) s += part[((size_t)k * Cout + co) * 32 + r];
-  if (r < 27) dw[co * 27 + r] = accumulate ? dw[co * 27 + r] + s : s;
-  else if (db) db[co] = accumulate ? db[co] + s : s;
-}
 
 // ------------------------------------------------------------------------------------------------
 // MaxPool2d(2,2) (vgg.py:59) on NHWC; optional NCHW output for the last pool (feeds the pooling head)
@@ -1065,8 +1055,10 @@ int hk_conv3x3_first_fwd(const float* x_nchw, const float* w, const float* bias,
   HK_LAUNCH_CHECK("im2col_first_kernel");
   pack_first_weights_kernel<<<(Cout * 32 + 127) / 128, 128, 0, stream>>>(w, bias, w27, Cout, round);
   HK_LAUNCH_CHECK("pack_first_weights_kernel");
-  return hk_gemm_tf32(x27, 0, 32, 0, w27, 0, 32, 0, y_nhwc, Cout, 0, 0, (int)P, Cout, 32, 1, 1.f, nullptr, 0.f, nullptr,
-                      0, 0, 0.f, nullptr, 3 /*relu + tf32 round*/, stream_);
+  GemmEpi e = {};
+  e.C = y_nhwc; e.ldc = Cout; e.alpha = 1.f;
+  e.relu = 3;                                        // ReLU + tf32 rounding
+  return gemm_tf32(x27, 0, 32, 0, w27, 0, 32, 0, e, (int)P, Cout, 32, 1, stream);
 }
 
 static int first_wgrad_splits(long long P) {
@@ -1096,14 +1088,11 @@ int hk_conv3x3_first_wgrad_acc(const float* x27, const float* dy_nhwc, float* dw
              "hk_conv3x3_first_wgrad: workspace too small");
   const long long P = (long long)N * H * W;
   const int S = first_wgrad_splits(P);
-  const long long Kc = P / S;
   float* part = static_cast<float*>(workspace);
-  int r = hk_gemm_tf32(dy_nhwc, 1, Cout, Kc * Cout, x27, 1, 32, Kc * 32, part, 32, (long long)Cout * 32, 0, Cout, 32,
-                       (int)Kc, S, 1.f, nullptr, 0.f, nullptr, 0, 0, 0.f, nullptr, 0, stream_);
-  if (r) return r;
-  first_wgrad_reduce_kernel<<<(Cout * 28 + 127) / 128, 128, 0, stream>>>(part, dw, db, Cout, S, accumulate ? 1 : 0);
-  HK_LAUNCH_CHECK("first_wgrad_reduce_kernel");
-  return 0;
+  // partial columns 0..26 are dw[co][27]; column 27 (the ones column of X27) is db
+  int r = gemm_splitk(dy_nhwc, 1, Cout, x27, 1, 32, Cout, 32, P, S, part, dw, 27, 27, nullptr, accumulate, stream);
+  if (r || !db) return r;
+  return sum_splits(part + 27, S, (long long)Cout * 32, Cout, 1, 32, db, 1, nullptr, accumulate, stream);
 }
 
 int hk_maxpool2x2_fwd(const float* x_nhwc, float* y, int N, int H, int W, int C, int out_nchw, void* stream) {

@@ -551,6 +551,41 @@ int gemm_tf32_pair(const float* Ah, const float* Al, int a_mn, long long lda, lo
   return launch_gemm<64>(tmA, tmB, epi, M, N, K, batch, a_mn, b_mn, shareA, shareB, stream, &tmAl, &tmBl);
 }
 
+__global__ void sum_splits_kernel(const float* __restrict__ part, int S, long long split_stride, long long ldp, int cols,
+                                  size_t n, float* __restrict__ out, long long ldo, const float* __restrict__ bias,
+                                  int accumulate) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t r = i / cols, c = i % cols;
+    const float* p = part + r * ldp + c;
+    float s = bias ? bias[c] : 0.f;
+    for (int k = 0; k < S; ++k) s += p[(size_t)k * split_stride];
+    float* o = out + r * ldo + c;
+    *o = accumulate ? *o + s : s;
+  }
+}
+
+int sum_splits(const float* part, int S, long long split_stride, int rows, int cols, long long ldp, float* out,
+               long long ldo, const float* bias, bool accumulate, cudaStream_t stream) {
+  const size_t n = (size_t)rows * cols;
+  sum_splits_kernel<<<grid_1d(n, 256), 256, 0, stream>>>(part, S, split_stride, ldp, cols, n, out, ldo, bias,
+                                                         accumulate ? 1 : 0);
+  HK_LAUNCH_CHECK("sum_splits_kernel");
+  return 0;
+}
+
+int gemm_splitk(const float* A, int a_mn, long long lda, const float* B, int b_mn, long long ldb, int M, int N, long long K,
+                int S, float* part, float* out, long long ldo, int cols, const float* bias, bool accumulate,
+                cudaStream_t stream) {
+  const long long Kc = K / S;
+  const bool direct = S == 1 && !bias && !accumulate && cols == N && ldo == N;
+  GemmEpi e = {};
+  e.C = direct ? out : part; e.ldc = N; e.strideC = (long long)M * N; e.alpha = 1.f;
+  // batch index = K slice: slice s of a K-major operand starts s * Kc columns in, of an MN-major one s * Kc rows in
+  int r = gemm_tf32(A, a_mn, lda, a_mn ? Kc * lda : Kc, B, b_mn, ldb, b_mn ? Kc * ldb : Kc, e, M, N, (int)Kc, S, stream);
+  if (r || direct) return r;
+  return sum_splits(part, S, (long long)M * N, M, cols, N, out, ldo, bias, accumulate, stream);
+}
+
 // the epilogue of hk_gemm_tf32 / hk_gemm_3xtf32 (see the public header)
 static GemmEpi plain_epi(float* C, long long ldc, long long strideC, int trans_c, float alpha, const float* alpha_vec,
                          float diag, const float* D, long long ldd, long long strideD, float beta, const float* beta_vec,

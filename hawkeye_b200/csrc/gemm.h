@@ -1,4 +1,4 @@
-// Epilogue description + host entry of the generic batched wgmma TF32 GEMM (gemm.cu).
+// Epilogue description + host entries of the generic batched wgmma TF32 GEMM and its split-K form (gemm.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <type_traits>
@@ -53,5 +53,17 @@ int gemm_tf32_1x(const float* A, int a_mn, long long lda, long long strideA, con
 int gemm_tf32_pair(const float* Ah, const float* Al, int a_mn, long long lda, long long strideA, const float* Bh,
                    const float* Bl, int b_mn, long long ldb, long long strideB, const GemmEpi& epi, int M, int N, int K,
                    int batch, cudaStream_t stream);
+
+// Split-K product out[M][0:cols) (+)= bias + A.B for one A [M,K] (or [K,M] if a_mn) and B [N,K] (or [K,N] if b_mn):
+// an S-way batched GEMM over the K/S-long slices (S divides K) writes part [S][M][N] (the caller's workspace), which
+// sum_splits reduces into out (leading dimension ldo).  With S == 1, no bias, no accumulation and out covering the
+// whole product, the GEMM writes out directly.
+int gemm_splitk(const float* A, int a_mn, long long lda, const float* B, int b_mn, long long ldb, int M, int N, long long K,
+                int S, float* part, float* out, long long ldo, int cols, const float* bias, bool accumulate,
+                cudaStream_t stream);
+// out[r][c] = (accumulate ? out[r][c] : 0) + s,  s = (bias ? bias[c] : 0) + part_0[r][c] + ... + part_{S-1}[r][c], summed
+// in that order; partial k starts at part + k * split_stride and its rows are ldp floats apart.
+int sum_splits(const float* part, int S, long long split_stride, int rows, int cols, long long ldp, float* out,
+               long long ldo, const float* bias, bool accumulate, cudaStream_t stream);
 
 }  // namespace hk

@@ -1,22 +1,13 @@
 // Classifier head glue, loss and optimizer kernels of the training step (reference train.py:310-320):
-//   * split-K reduction for the skinny classifier GEMM (nn.Linear(512**2, K), BCNN.py:42)
+//   * the skinny classifier GEMMs (nn.Linear(512**2, K), BCNN.py:42), split-K in the forward
 //   * CrossEntropyLoss(label_smoothing=0.1) forward+backward (train.py:211-212), mean reduction
 //   * fused SGD-momentum / Adam parameter update over flat fp32 buffers (Examples/BCNN.py:40, Examples/MPN.py:14-18)
 #include "common.cuh"
 #include "host.h"
+#include "gemm.h"
 #include "../../include/hawkeye_b200.h"
 
 namespace hk {
-
-// out[i] = bias[i % N] + sum_s partial[s][i]
-__global__ void splitk_reduce_bias_kernel(const float* __restrict__ partial, const float* __restrict__ bias,
-                                          float* __restrict__ out, int MN, int N, int S) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= MN) return;
-  float s = bias ? bias[i % N] : 0.f;
-  for (int k = 0; k < S; ++k) s += partial[(size_t)k * MN + i];
-  out[i] = s;
-}
 
 // One block; warps stride over rows.  loss = mean_b [ (1-eps) * -logp[y] + eps/K * sum_k -logp[k] ]
 // dlogits = (softmax - ((1-eps) onehot + eps/K)) * grad_scale / B
@@ -159,38 +150,29 @@ int hk_linear_fwd(const float* x, const float* w, const float* bias, float* y, i
   const int S = linear_splits(F);
   HK_REQUIRE(workspace && workspace_bytes >= (size_t)S * B * N * sizeof(float), HK_ERR_WORKSPACE,
              "hk_linear_fwd: workspace too small");
-  float* part = static_cast<float*>(workspace);
-  const int Kc = F / S;
-  // batch dimension = K split: A_s = x[:, s*Kc:(s+1)*Kc], B_s = w[:, s*Kc:(s+1)*Kc]
-  int r = hk_gemm_tf32(x, 0, F, Kc, w, 0, F, Kc, part, N, (long long)B * N, 0, B, N, Kc, S, 1.f, nullptr, 0.f, nullptr, 0,
-                       0, 0.f, nullptr, 0, stream);
-  if (r) return r;
-  splitk_reduce_bias_kernel<<<(B * N + 255) / 256, 256, 0, (cudaStream_t)stream>>>(part, bias, y, B * N, N, S);
-  HK_LAUNCH_CHECK("splitk_reduce_bias_kernel");
-  return 0;
+  return gemm_splitk(x, 0, F, w, 0, F, B, N, F, S, static_cast<float*>(workspace), y, N, N, bias, false,
+                     (cudaStream_t)stream);
 }
 
 /* dx[B,F] = dy[B,N] . w[N,F] */
 int hk_linear_dgrad(const float* dy, const float* w, float* dx, int B, int F, int N, void* stream) {
   HK_REQUIRE(dy && w && dx, HK_ERR_ARG, "hk_linear_dgrad: null pointer");
   HK_REQUIRE(N % 4 == 0 && F % 4 == 0, HK_ERR_UNSUPPORTED, "hk_linear_dgrad: N=%d, F=%d must be multiples of 4", N, F);
-  return hk_gemm_tf32(dy, 0, N, 0, w, 1, F, 0, dx, F, 0, 0, B, F, N, 1, 1.f, nullptr, 0.f, nullptr, 0, 0, 0.f, nullptr, 0,
-                      stream);
+  GemmEpi e = {};
+  e.C = dx; e.ldc = F; e.alpha = 1.f;
+  return gemm_tf32(dy, 0, N, 0, w, 1, F, 0, e, B, F, N, 1, (cudaStream_t)stream);
 }
 
 /* dw[N,F] = dy[B,N]^T . x[B,F] ; db[N] = sum_b dy[b,:] */
 int hk_linear_wgrad(const float* dy, const float* x, float* dw, float* db, int B, int F, int N, void* stream) {
   HK_REQUIRE(dy && x && dw, HK_ERR_ARG, "hk_linear_wgrad: null pointer");
   HK_REQUIRE(N % 4 == 0 && F % 4 == 0, HK_ERR_UNSUPPORTED, "hk_linear_wgrad: N=%d, F=%d must be multiples of 4", N, F);
-  int r = hk_gemm_tf32(dy, 1, N, 0, x, 1, F, 0, dw, F, 0, 0, N, F, B, 1, 1.f, nullptr, 0.f, nullptr, 0, 0, 0.f, nullptr, 0,
-                       stream);
-  if (r) return r;
-  if (db) {
-    // db = column sums of dy [B,N]: reuse the split-K reducer (S=B "partials" of length N, no bias)
-    splitk_reduce_bias_kernel<<<(N + 255) / 256, 256, 0, (cudaStream_t)stream>>>(dy, nullptr, db, N, N, B);
-    HK_LAUNCH_CHECK("splitk_reduce_bias_kernel(db)");
-  }
-  return 0;
+  GemmEpi e = {};
+  e.C = dw; e.ldc = F; e.alpha = 1.f;
+  int r = gemm_tf32(dy, 1, N, 0, x, 1, F, 0, e, N, F, B, 1, (cudaStream_t)stream);
+  if (r || !db) return r;
+  // db = column sums of dy [B,N]: the B rows are B "partials" of one row of N
+  return sum_splits(dy, B, N, 1, N, N, db, N, nullptr, false, (cudaStream_t)stream);
 }
 
 int hk_softmax_ce_ls(const float* logits, const long long* labels, float* loss, float* dlogits, int* correct, int B,

@@ -15,14 +15,13 @@ namespace hk {
 
 struct Pair { float* hi; float* lo; };
 
-// C(hi,lo | full) = alpha*alpha_vec[b] * (A.B) + diag*I + beta * D(hi+lo)     A,B,D: [batch][n][n] row-major pairs
-static int mm3(Pair A, Pair B, Pair C, float* tmp, int n, int batch, float alpha, const float* alpha_vec, float diag,
-               const Pair* D, float beta, cudaStream_t st) {
+// C(hi,lo) = alpha * (A.B) + diag*I + beta * D(hi+lo)     A,B,D: [batch][n][n] row-major pairs
+static int mm3(Pair A, Pair B, Pair C, int n, int batch, float alpha, float diag, const Pair* D, float beta,
+               cudaStream_t st) {
   const long long s = (long long)n * n;
-  (void)tmp;
   GemmEpi f = {};
   f.C = C.hi; f.C_lo = C.lo; f.ldc = n; f.strideC = s;
-  f.alpha = alpha; f.alpha_vec = alpha_vec; f.diag = diag;
+  f.alpha = alpha; f.diag = diag;
   if (D) { f.D = D->hi; f.D_lo = D->lo; f.ldd = n; f.strideD = s; f.beta = beta; }
   // one launch: every k-step issues Ah.Bl, Al.Bh, Ah.Bh into the same accumulators (gemm.cu, triple mode)
   return gemm_tf32_pair(A.hi, A.lo, 0, n, s, B.hi, B.lo, 1, n, s, f, n, n, n, batch, st);
@@ -214,8 +213,7 @@ int hk_sqrtm_fwd(const float* x, float* y, float* saved, int B, int n, int iterN
   SqrtmSaved sv = saved_view(saved, B, n, iterN);
   const size_t S = sv.S;
   const int L = sv.L;
-  float* w = static_cast<float*>(workspace);
-  float* tmp = w;
+  float* w = static_cast<float*>(workspace);       // matrix slot 0 is unused
   Pair ZY = {w + S, w + 2 * S};
   Pair T = {w + 3 * S, w + 4 * S};
   int r;
@@ -225,15 +223,15 @@ int hk_sqrtm_fwd(const float* x, float* y, float* saved, int B, int n, int iterN
   affine_diag_split_kernel<<<grid_1d(S, 256), 256, 0, st>>>(sv.A.hi, sv.A.lo, sv.Z(0).hi, sv.Z(0).lo, -0.5f, nullptr, 0,
                                                             1.5f, n, S);
   HK_LAUNCH_CHECK("affine_diag_split_kernel");
-  if ((r = mm3(sv.A, sv.Z(0), sv.Y(0), tmp, n, B, 1.f, nullptr, 0.f, nullptr, 0.f, st))) return r;
+  if ((r = mm3(sv.A, sv.Z(0), sv.Y(0), n, B, 1.f, 0.f, nullptr, 0.f, st))) return r;
   for (int i = 1; i < L; ++i) {                                                   // (MPNCOV.py:156-159)
-    if ((r = mm3(sv.Z(i - 1), sv.Y(i - 1), ZY, tmp, n, B, -0.5f, nullptr, 1.5f, nullptr, 0.f, st))) return r;
-    if ((r = mm3(sv.Y(i - 1), ZY, sv.Y(i), tmp, n, B, 1.f, nullptr, 0.f, nullptr, 0.f, st))) return r;
-    if ((r = mm3(ZY, sv.Z(i - 1), sv.Z(i), tmp, n, B, 1.f, nullptr, 0.f, nullptr, 0.f, st))) return r;
+    if ((r = mm3(sv.Z(i - 1), sv.Y(i - 1), ZY, n, B, -0.5f, 1.5f, nullptr, 0.f, st))) return r;
+    if ((r = mm3(sv.Y(i - 1), ZY, sv.Y(i), n, B, 1.f, 0.f, nullptr, 0.f, st))) return r;
+    if ((r = mm3(ZY, sv.Z(i - 1), sv.Z(i), n, B, 1.f, 0.f, nullptr, 0.f, st))) return r;
   }
   // YZY = 0.5 Y (3I - Z Y) ; y = YZY sqrt(normA)                                   (MPNCOV.py:160-161)
-  if ((r = mm3(sv.Z(L - 1), sv.Y(L - 1), T, tmp, n, B, -1.f, nullptr, 3.f, nullptr, 0.f, st))) return r;
-  if ((r = mm3(sv.Y(L - 1), T, ZY, tmp, n, B, 0.5f, nullptr, 0.f, nullptr, 0.f, st))) return r;
+  if ((r = mm3(sv.Z(L - 1), sv.Y(L - 1), T, n, B, -1.f, 3.f, nullptr, 0.f, st))) return r;
+  if ((r = mm3(sv.Y(L - 1), T, ZY, n, B, 0.5f, 0.f, nullptr, 0.f, st))) return r;
   pair_combine_scale_kernel<<<grid_1d(S, 256), 256, 0, st>>>(ZY.hi, ZY.lo, y, sv.normA, 1, (size_t)n * n, S);
   HK_LAUNCH_CHECK("pair_combine_scale_kernel");
   return 0;
@@ -252,46 +250,45 @@ int hk_sqrtm_bwd(const float* x, const float* y, const float* g, float* saved, f
   const size_t S = sv.S;
   const int L = sv.L;
   float* w = static_cast<float*>(workspace);
-  float* tmp = w;
-  int slot = 1;
+  int slot = 1;                                      // matrix slot 0 is unused
   auto newp = [&]() { Pair p{w + (size_t)slot * S, w + (size_t)(slot + 1) * S}; slot += 2; return p; };
   Pair P = newp(), T1 = newp(), U = newp(), V = newp(), dY = newp(), dZ = newp(), W2 = newp(), dY2 = newp(), dZ2 = newp(),
-       acc = newp(), E1 = newp();   // 11 pairs = 22 matrices + tmp = 23
+       acc = newp(), E1 = newp();   // 11 pairs = 22 matrices + slot 0 = 23
   int r;
   // der_postCom = g sqrt(normA)                                                       (MPNCOV.py:174)
   affine_diag_split_kernel<<<grid_1d(S, 256), 256, 0, st>>>(g, nullptr, P.hi, P.lo, 1.f, sv.normA, 1, 0.f, n, S);
   HK_LAUNCH_CHECK("affine_diag_split_kernel");
   const Pair Yl = sv.Y(L - 1), Zl = sv.Z(L - 1);
   // dldY = 0.5 (P (3I - Yl Zl) - Zl Yl P)                                            (MPNCOV.py:180-181)
-  if ((r = mm3(Yl, Zl, T1, tmp, n, B, -1.f, nullptr, 3.f, nullptr, 0.f, st))) return r;
-  if ((r = mm3(P, T1, U, tmp, n, B, 1.f, nullptr, 0.f, nullptr, 0.f, st))) return r;
-  if ((r = mm3(Zl, Yl, V, tmp, n, B, 1.f, nullptr, 0.f, nullptr, 0.f, st))) return r;
-  if ((r = mm3(V, P, dY, tmp, n, B, -0.5f, nullptr, 0.f, &U, 0.5f, st))) return r;
+  if ((r = mm3(Yl, Zl, T1, n, B, -1.f, 3.f, nullptr, 0.f, st))) return r;
+  if ((r = mm3(P, T1, U, n, B, 1.f, 0.f, nullptr, 0.f, st))) return r;
+  if ((r = mm3(Zl, Yl, V, n, B, 1.f, 0.f, nullptr, 0.f, st))) return r;
+  if ((r = mm3(V, P, dY, n, B, -0.5f, 0.f, &U, 0.5f, st))) return r;
   // dldZ = -0.5 Yl P Yl                                                              (MPNCOV.py:182)
-  if ((r = mm3(Yl, P, W2, tmp, n, B, 1.f, nullptr, 0.f, nullptr, 0.f, st))) return r;
-  if ((r = mm3(W2, Yl, dZ, tmp, n, B, -0.5f, nullptr, 0.f, nullptr, 0.f, st))) return r;
+  if ((r = mm3(Yl, P, W2, n, B, 1.f, 0.f, nullptr, 0.f, st))) return r;
+  if ((r = mm3(W2, Yl, dZ, n, B, -0.5f, 0.f, nullptr, 0.f, st))) return r;
   for (int i = L - 2; i >= 0; --i) {                                                // (MPNCOV.py:183-193)
     const Pair Yi = sv.Y(i), Zi = sv.Z(i);
-    if ((r = mm3(Yi, Zi, T1, tmp, n, B, -1.f, nullptr, 3.f, nullptr, 0.f, st))) return r;   // YZ = 3I - Y Z
-    if ((r = mm3(Zi, Yi, V, tmp, n, B, 1.f, nullptr, 0.f, nullptr, 0.f, st))) return r;     // ZY = Z Y
+    if ((r = mm3(Yi, Zi, T1, n, B, -1.f, 3.f, nullptr, 0.f, st))) return r;   // YZ = 3I - Y Z
+    if ((r = mm3(Zi, Yi, V, n, B, 1.f, 0.f, nullptr, 0.f, st))) return r;     // ZY = Z Y
     // dldY_ = 0.5 (dldY YZ - Z dldZ Z - ZY dldY)
-    if ((r = mm3(dY, T1, U, tmp, n, B, 1.f, nullptr, 0.f, nullptr, 0.f, st))) return r;
-    if ((r = mm3(Zi, dZ, W2, tmp, n, B, 1.f, nullptr, 0.f, nullptr, 0.f, st))) return r;
-    if ((r = mm3(W2, Zi, acc, tmp, n, B, -0.5f, nullptr, 0.f, &U, 0.5f, st))) return r;
-    if ((r = mm3(V, dY, dY2, tmp, n, B, -0.5f, nullptr, 0.f, &acc, 1.f, st))) return r;
+    if ((r = mm3(dY, T1, U, n, B, 1.f, 0.f, nullptr, 0.f, st))) return r;
+    if ((r = mm3(Zi, dZ, W2, n, B, 1.f, 0.f, nullptr, 0.f, st))) return r;
+    if ((r = mm3(W2, Zi, acc, n, B, -0.5f, 0.f, &U, 0.5f, st))) return r;
+    if ((r = mm3(V, dY, dY2, n, B, -0.5f, 0.f, &acc, 1.f, st))) return r;
     // dldZ_ = 0.5 (YZ dldZ - Y dldY Y - dldZ ZY)
-    if ((r = mm3(T1, dZ, U, tmp, n, B, 1.f, nullptr, 0.f, nullptr, 0.f, st))) return r;
-    if ((r = mm3(Yi, dY, W2, tmp, n, B, 1.f, nullptr, 0.f, nullptr, 0.f, st))) return r;
-    if ((r = mm3(W2, Yi, acc, tmp, n, B, -0.5f, nullptr, 0.f, &U, 0.5f, st))) return r;
-    if ((r = mm3(dZ, V, dZ2, tmp, n, B, -0.5f, nullptr, 0.f, &acc, 1.f, st))) return r;
+    if ((r = mm3(T1, dZ, U, n, B, 1.f, 0.f, nullptr, 0.f, st))) return r;
+    if ((r = mm3(Yi, dY, W2, n, B, 1.f, 0.f, nullptr, 0.f, st))) return r;
+    if ((r = mm3(W2, Yi, acc, n, B, -0.5f, 0.f, &U, 0.5f, st))) return r;
+    if ((r = mm3(dZ, V, dZ2, n, B, -0.5f, 0.f, &acc, 1.f, st))) return r;
     Pair t = dY; dY = dY2; dY2 = t;
     t = dZ; dZ = dZ2; dZ2 = t;
   }
   // der_NSiter = 0.5 (dldY (3I - A) - dldZ - A dldY)                                  (MPNCOV.py:194)
   affine_diag_split_kernel<<<grid_1d(S, 256), 256, 0, st>>>(sv.A.hi, sv.A.lo, E1.hi, E1.lo, -1.f, nullptr, 0, 3.f, n, S);
   HK_LAUNCH_CHECK("affine_diag_split_kernel");
-  if ((r = mm3(dY, E1, U, tmp, n, B, 1.f, nullptr, 0.f, nullptr, 0.f, st))) return r;
-  if ((r = mm3(sv.A, dY, acc, tmp, n, B, -0.5f, nullptr, 0.f, &U, 0.5f, st))) return r;   // acc = 0.5 dldY(3I-A) - 0.5 A dldY
+  if ((r = mm3(dY, E1, U, n, B, 1.f, 0.f, nullptr, 0.f, st))) return r;
+  if ((r = mm3(sv.A, dY, acc, n, B, -0.5f, 0.f, &U, 0.5f, st))) return r;   // acc = 0.5 dldY(3I-A) - 0.5 A dldY
   // transpose, /normA, diagonal correction                                            (MPNCOV.py:195-201)
   sqrtm_bwd_tail_kernel<<<B, 256, 0, st>>>(acc.hi, acc.lo, dZ.hi, dZ.lo, x, y, g, sv.normA, grad_x, n);
   HK_LAUNCH_CHECK("sqrtm_bwd_tail_kernel");

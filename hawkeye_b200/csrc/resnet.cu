@@ -327,14 +327,6 @@ __global__ void add_inplace_kernel(float* __restrict__ a, const float* __restric
     reinterpret_cast<float4*>(a)[i] = u;
   }
 }
-// out[i] = sum_s part[s][i]
-__global__ void reduce_partials_kernel(const float* __restrict__ part, float* __restrict__ out, size_t n, int S) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    float s = 0.f;
-    for (int k = 0; k < S; ++k) s += part[(size_t)k * n + i];
-    out[i] = s;
-  }
-}
 __global__ void nhwc_to_nchw_kernel(const float* __restrict__ x, float* __restrict__ y, int N, int HW, int C) {
   const size_t total = (size_t)N * HW * C;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
@@ -516,16 +508,8 @@ int hk_matconv_wgrad(const float* x, const float* dy, float* dw, long long P, in
   HK_REQUIRE(K % 4 == 0 && Cout % 4 == 0, HK_ERR_UNSUPPORTED, "hk_matconv_wgrad: K=%d Cout=%d must be multiples of 4", K, Cout);
   HK_REQUIRE(workspace && workspace_bytes >= hk_matconv_wgrad_workspace_bytes(P, K, Cout), HK_ERR_WORKSPACE,
              "hk_matconv_wgrad: workspace too small");
-  const int S = kc_splits(P, Cout, K);
-  const long long Kc = P / S;
-  float* part = static_cast<float*>(workspace);
-  GemmEpi e = {};
-  e.C = S == 1 ? dw : part; e.ldc = K; e.strideC = (long long)Cout * K; e.alpha = 1.f;
-  int r = gemm_tf32(dy, 1, Cout, Kc * Cout, x, 1, K, Kc * K, e, Cout, K, (int)Kc, S, st);
-  if (r || S == 1) return r;
-  reduce_partials_kernel<<<grid_1d((size_t)Cout * K, 256), 256, 0, st>>>(part, dw, (size_t)Cout * K, S);
-  HK_LAUNCH_CHECK("reduce_partials_kernel");
-  return 0;
+  return gemm_splitk(dy, 1, Cout, x, 1, K, Cout, K, P, kc_splits(P, Cout, K), static_cast<float*>(workspace), dw, K, K,
+                     nullptr, false, st);
 }
 
 }  // extern "C"

@@ -91,6 +91,10 @@ def test_first_layer_and_pool():
     _lib.call('hk_conv3x3_first_wgrad', ws0, dpre, dw, db, N, H, W, Cout, ws, nb, s)
     print('first wgrad', rel_l2(dw.cpu(), gw), rel_l2(db.cpu(), gb))
     assert rel_l2(dw.cpu(), gw) < 2e-3 and rel_l2(db.cpu(), gb) < 2e-3
+    # accumulate onto what it just wrote: the same sums added once more, s + s = 2 s exactly
+    dw1, db1 = dw.clone(), db.clone()
+    _lib.call('hk_conv3x3_first_wgrad_acc', ws0, dpre, dw, db, N, H, W, Cout, ws, nb, 1, s)
+    assert torch.equal(dw, 2 * dw1) and torch.equal(db, 2 * db1)
     # max-pool fwd (NHWC and NCHW-out) and bwd (first-max routing + ReLU mask)
     a = F.relu(detgen.det((N, 64, H, W), 7)).double().requires_grad_(True)
     p_ref = F.max_pool2d(a, 2, 2)

@@ -9,8 +9,9 @@ from conftest import rel_l2
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize('B,Fdim,N', [(2, 16384, 200), (32, 262144, 200), (5, 8192, 200)])
+@pytest.mark.parametrize('B,Fdim,N', [(2, 16384, 200), (32, 262144, 200), (5, 8192, 200), (8, 1024, 200)])
 def test_linear(B, Fdim, N):
+    """with and without bias; F < 2048 runs the forward as one K slice, which without bias the GEMM writes directly"""
     from hawkeye_b200 import ops
     x = detgen.det((B, Fdim), 1, Fdim ** -0.5)
     w = detgen.det((N, Fdim), 2, (2.0 / Fdim) ** 0.5)
@@ -25,6 +26,12 @@ def test_linear(B, Fdim, N):
     errs = [rel_l2(y.detach().cpu(), y_ref.detach()), rel_l2(dx.cpu(), rx), rel_l2(dw.cpu(), rw), rel_l2(db.cpu(), rb)]
     print(f'linear B={B} F={Fdim}: y {errs[0]:.2e} dx {errs[1]:.2e} dw {errs[2]:.2e} db {errs[3]:.2e}')
     assert max(errs[:3]) < 2e-3 and errs[3] < 1e-5
+    # bias-free: the input and weight gradients do not depend on the bias
+    y0 = ops.linear(xg, wg, None)
+    dx0, dw0 = torch.autograd.grad(y0, (xg, wg), dy.cuda())
+    errs0 = [rel_l2(y0.detach().cpu(), F.linear(xd, wd_).detach()), rel_l2(dx0.cpu(), rx), rel_l2(dw0.cpu(), rw)]
+    print(f'linear B={B} F={Fdim} no bias: y {errs0[0]:.2e} dx {errs0[1]:.2e} dw {errs0[2]:.2e}')
+    assert max(errs0) < 2e-3
 
 
 @pytest.mark.parametrize('precise', [0, 1])

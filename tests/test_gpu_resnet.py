@@ -123,6 +123,23 @@ def test_conv3x3_wgrad_14x14_and_7x7():
         assert e < 2e-3
 
 
+@pytest.mark.parametrize('P,K,Cout', [(100, 64, 128),      # one K split: the GEMM writes dw directly
+                                      (1568, 64, 128),     # 16 splits and their reduction
+                                      (2048, 160, 64)])    # the stem's im2col width
+def test_matconv_wgrad(P, K, Cout):
+    from hawkeye_b200 import _lib
+    s = _lib.stream_ptr()
+    x = detgen.det((P, K), 1)
+    dy = detgen.det((P, Cout), 2)
+    dw = torch.empty(Cout, K, device='cuda')
+    nb = _lib.query('hk_matconv_wgrad_workspace_bytes', P, K, Cout)
+    ws = torch.empty(nb, dtype=torch.uint8, device='cuda')
+    _lib.call('hk_matconv_wgrad', x.cuda(), dy.cuda(), dw, P, K, Cout, ws, nb, s)
+    e = rel_l2(dw.cpu(), dy.double().t() @ x.double())
+    print('matconv wgrad', P, K, Cout, e)
+    assert e < 2e-3
+
+
 def _mpn_and_state():
     import hawkeye_b200 as hb
 
