@@ -145,6 +145,17 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t adesc, uint6
       : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
 
+// A from registers (B still a shared-memory descriptor): thread t = 32 w + l holds rows 16 w + l / 4 (+8) and columns
+// l % 4 (+4) of the 64 x 8 A tile as a = {(r, c), (r + 8, c), (r, c + 4), (r + 8, c + 4)}.  The registers must not change
+// until the wgmma that reads them has completed (wgmma_wait).
+__device__ __forceinline__ void wgmma_tf32(float (&d)[8], const uint32_t (&a)[4], uint64_t bdesc) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, 1, 1, 1;\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc));
+}
+
 // named barrier over `count` threads (id 0 is __syncthreads)
 __device__ __forceinline__ void named_bar(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
@@ -161,6 +172,12 @@ __device__ __forceinline__ uint64_t make_sdesc(uint32_t saddr) {
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
   d |= static_cast<uint64_t>(1) << 62;   // SWIZZLE_128B
   return d;
+}
+
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t saddr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(saddr) : "memory");
+  return v;
 }
 
 // byte offset of fp32 element (row, k) in a K-major 128B-swizzled tile (row = M/N index, k < 32): the 16-byte chunk

@@ -537,14 +537,19 @@ static int conv3x3_igemm_1x(const float* x, const float* wp, const float* bias, 
 }
 
 // ------------------------------------------------------------------------------------------------
-// weight gradient: one CTA accumulates dWp[tap][co0:co0+64][ci0:ci0+32] for ALL 9 taps over its share of the pixels
-// (split-K across CTAs, fp32 atomics at the end).  Per stage (64 pixels of the tile):
-//   A = dY tile (M = 64 co, k = 64 pixels), TMA-loaded pixel-major and transposed to K-major by the producer warpgroup,
-//       which also sums it over the pixels for the bias gradient (no separate pass over dY);
-//   B = X halo patch, one TMA load per kw shift: (TH+2) x TW pixels x 32 ci, transposed to [32 ci][patch pixels].  The
-//       three kh taps read the SAME patch kh*TW pixels further along k (TW a multiple of 8: whole wgmma k-steps), so
-//       the input is fetched 3x (+halo) instead of 9x.
-//   Warpgroups 1 and 2 accumulate all nine taps for ci 0-15 and 16-31 of the tile (64 x 16 fp32 each, in registers).
+// weight gradient: one CTA accumulates dWp[tap][co0 : co0 + CO][ci0 : ci0 + CI] for ALL 9 taps over its share of the
+// pixels (split-K across CTAs, fp32 atomics at the end).  A stage covers a 64-pixel tile (TW x TH x TN):
+//   A = dY^T (M = co, k = pixel).  TMA lands dY pixel-major ([64 px][32 co] boxes, 128B-swizzled); each consumer thread
+//       reads its m64k8 register fragment straight from there and feeds it to all nine taps, so dY is neither transposed
+//       nor re-read per tap.  The same registers give the bias gradient.
+//   B = X: ONE TMA box of (TH+2) x (TW+2) x TN pixels x 32 ci (the halo patch), transposed by the producer warpgroup
+//       into three kw-shifted K-major copies [32 ci][(TH+2) TW TN px].  Tap (kh, kw) reads copy kw kh*TW pixels further
+//       along k (TW a multiple of 8: whole wgmma k-steps).  Three halo buffers keep the next boxes' TMA in flight while
+//       one is transposed.
+//   Tile: 64 co x 32 ci.  Both consumer warpgroups load the same dY fragment; warpgroup wg accumulates ci 16 wg..16 wg+15
+//   for all nine taps (m64n16k8, 72 fp32 registers per thread).  With A in registers the B bytes a wgmma reads per FLOP
+//   depend on M alone, so n16 costs no more shared-memory bandwidth than n32 would; 9 x (64 x 32) accumulators per
+//   warpgroup (144 per thread) do not fit the consumer's registers without spilling.
 // ------------------------------------------------------------------------------------------------
 struct WgradArgs {
   float* dWp;  // [9][Cout][Cin], pre-zeroed
@@ -555,145 +560,183 @@ struct WgradArgs {
 };
 
 constexpr int WG_THREADS = 384;
-constexpr int WG_STAGES = 2;
-constexpr int WG_KP = 64;                        // pixels per stage
-constexpr int WG_PATCH = 96 * 128;               // one kw patch: (TH+2)*TW*TN <= 96 pixel rows x 128 B
-constexpr int WG_RAW_A = 2 * WG_KP * 128;        // dY: 2 co-boxes of [64 px x 32 co]
-constexpr int WG_RAW_BYTES = WG_RAW_A + 3 * WG_PATCH;
-constexpr int WG_A_BYTES = 2 * 64 * 128;         // A: 2 k-chunks of [64 co x 32 px]
-constexpr int WG_B_ONE = 3 * 32 * 128;           // B of one kw: 3 k-chunks of [32 ci x 32 px]
-constexpr int WG_STAGE_BYTES = WG_A_BYTES + 3 * WG_B_ONE;
-constexpr int WG_SMEM = WG_RAW_BYTES + WG_STAGES * WG_STAGE_BYTES + 1024 + 256;
+constexpr int WG_KP = 64;                          // pixels per stage
+constexpr int WG_PATCH_PX = 96;                    // (TH+2) * TW * TN: transposed patch pixels, at most 3 k-chunks of 32
+constexpr int WG_RAW_ROWS = 120;                   // (TH+2) * (TW+2) * TN: halo box rows (TW >= 8)
+constexpr int WG_RAW_BYTES = WG_RAW_ROWS * 128;    // one ci chunk of the halo box (15 KB, whole swizzle atoms)
+constexpr int WG_RAW_BUFS = 3;                     // halo boxes in flight or being transposed
+constexpr int WG_XT_KW = 3 * 32 * 128;             // one kw copy: 3 k-chunks of [32 ci x 32 px]
+constexpr int WG_XT_CHUNK = 3 * WG_XT_KW;          // the three kw copies of one ci chunk
 
-// one stage of the nine tap products for ci rows [16 wg, 16 wg + 16) of the tile: acc[tap] is 64 co x 16 ci
-__device__ __forceinline__ void wgrad_mma(float (&acc)[9][8], const uint8_t* sa, const uint8_t* sb, int wg, int TW,
-                                          int img_rows) {
-  const uint32_t a_addr = smem_u32(sa), b_addr = smem_u32(sb) + wg * 16 * 128;
-  wgmma_fence();
-#pragma unroll 1   // rolled: 72 descriptors per k-step instead of 576 live at once
-  for (int ks = 0; ks < 8; ++ks) {
-    const uint64_t ad = make_sdesc(a_addr + (ks >> 2) * (64 * 128)) + (ks & 3) * 2;
-    const int kb = ks * 8 + ((ks * 8) / img_rows) * 2 * TW;    // k of this step in the patch of image n: + 2 TW per image
-#pragma unroll
-    for (int tap = 0; tap < 9; ++tap) {
-      const int kh = tap / 3, kw = tap % 3;
-      const int kk = kb + kh * TW;
-      // rows 16 wg.. of the [32 ci] chunk: two whole 8-row swizzle groups further on
-      const uint64_t bd = make_sdesc(b_addr + kw * WG_B_ONE + (kk >> 5) * (32 * 128)) + ((kk & 31) >> 3) * 2;
-      wgmma_tf32(acc[tap], ad, bd, 1);
-    }
-  }
-  wgmma_commit();
-}
-
-__device__ __forceinline__ void wgrad_store(const float (&acc)[9][8], const WgradArgs& a, int co0, int ci0, int t) {
-  const int wl = t >> 5, lane = t & 31;
-#pragma unroll
-  for (int tap = 0; tap < 9; ++tap)
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      const int co = co0 + wl * 16 + (lane >> 2) + 8 * ((e >> 1) & 1);
-      const int ci = ci0 + 8 * (e >> 2) + 2 * (lane & 3) + (e & 1);
-      if (co < a.Cout) atomicAdd(a.dWp + ((size_t)tap * a.Cout + co) * a.Cin + ci, acc[tap][e]);
-    }
-}
+constexpr int WG_CO = 64, WG_CI = 32;             // CTA tile
+constexpr int WG_DY_BYTES = (WG_CO / 32) * WG_KP * 128;
+constexpr int WG_STAGE_BYTES = WG_DY_BYTES + WG_XT_CHUNK;
+constexpr int WG_SMEM = 2 * WG_STAGE_BYTES + WG_RAW_BUFS * WG_RAW_BYTES + 1024 + 256;
 
 __global__ void __launch_bounds__(WG_THREADS, 1)
 conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX, WgradArgs a) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* raw = smem;
-  uint8_t* stages = smem + WG_RAW_BYTES;
-  uint64_t* full = reinterpret_cast<uint64_t*>(stages + WG_STAGES * WG_STAGE_BYTES);
-  uint64_t* empty = full + WG_STAGES;
-  uint64_t* raw_bar = empty + WG_STAGES;
+  uint8_t* stages = smem;                           // [2] x {dY boxes, three kw copies of X^T}
+  uint8_t* raw = smem + 2 * WG_STAGE_BYTES;       // [WG_RAW_BUFS] halo boxes
+  uint64_t* full = reinterpret_cast<uint64_t*>(raw + WG_RAW_BUFS * WG_RAW_BYTES);
+  uint64_t* empty = full + 2;
+  uint64_t* raw_full = empty + 2;
 
   const int warp = threadIdx.x >> 5;
-  const int n_ci_tiles = a.Cin / 32;
+  const int n_ci_tiles = (a.Cin + WG_CI - 1) / WG_CI;
   const int ci_t = blockIdx.x % n_ci_tiles, co_t = blockIdx.x / n_ci_tiles;
-  const int split = blockIdx.y;
-  const int co0 = co_t * 64, ci0 = ci_t * 32;
-  const bool do_bias = (a.db != nullptr) && (ci_t == 0);
+  const int co0 = co_t * WG_CO, ci0 = ci_t * WG_CI;
   const long long total_tiles = (long long)a.tiles_w * a.tiles_h * a.tiles_n;
   const long long per = (total_tiles + a.ksplit - 1) / a.ksplit;
-  const long long t_begin = per * split;
+  const long long t_begin = per * blockIdx.y;
   const long long t_end = (t_begin + per < total_tiles) ? t_begin + per : total_tiles;
   const int nk = (int)(t_end > t_begin ? t_end - t_begin : 0);
-  const int img_rows = a.TH * a.TW;                 // A pixels per image in the tile
-  const int patch_rows = (a.TH + 2) * a.TW * a.TN;  // B pixels of one kw patch
-  const int patch_chunks = (patch_rows + 31) / 32;
+  const int img_rows = a.TH * a.TW;                 // dY pixels per image in the tile
+  const int patch_rows = (a.TH + 2) * a.TW * a.TN;  // pixels of one kw copy
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmDY);
     tma_prefetch_desc(&tmX);
-    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
-    mbar_init(raw_bar, 1);
+    // full: the dY TMA's expect_tx arrival + the producer's arrival once the X copies are written
+    for (int s = 0; s < 2; ++s) { mbar_init(&full[s], 2); mbar_init(&empty[s], 2); }
+    for (int i = 0; i < WG_RAW_BUFS; ++i) mbar_init(&raw_full[i], 1);
     fence_barrier_init();
   }
   __syncthreads();
   if (nk == 0) return;
 
+  auto tile_origin = [&](int k, int* w0, int* h0, int* n0) {
+    long long tt = t_begin + k;
+    *w0 = (int)(tt % a.tiles_w) * a.TW; tt /= a.tiles_w;
+    *h0 = (int)(tt % a.tiles_h) * a.TH; tt /= a.tiles_h;
+    *n0 = (int)tt * a.TN;
+  };
+
   if (warp < 4) {
     regs_dealloc<56>();
-    const int t = threadIdx.x;
-    float bsum = 0.f;                               // bias gradient of co0 + (t & 63), pixel half t >> 6
-    for (int kb = 0; kb < nk; ++kb) {
-      const int s = kb % WG_STAGES;
-      const uint32_t ph = (kb / WG_STAGES) & 1;
-      if (t == 0) {
-        int tt = (int)t_begin + kb;
-        const int tw = tt % a.tiles_w; tt /= a.tiles_w;
-        const int th = tt % a.tiles_h; tt /= a.tiles_h;
-        const int w0 = tw * a.TW, h0 = th * a.TH, n0 = tt * a.TN;
-        mbar_wait(&empty[s], ph ^ 1);
-        mbar_expect_tx(raw_bar, WG_RAW_A + 3 * patch_rows * 128);
-#pragma unroll
-        for (int j = 0; j < 2; ++j) tma_load_4d(raw + j * WG_KP * 128, &tmDY, raw_bar, co0 + j * 32, w0, h0, n0);
-#pragma unroll
-        for (int kw = 0; kw < 3; ++kw) tma_load_4d(raw + WG_RAW_A + kw * WG_PATCH, &tmX, raw_bar, ci0, w0 + kw - 1, h0 - 1, n0);
-      }
-      mbar_wait(raw_bar, kb & 1);
+    const int t = threadIdx.x, lane = t & 31;
+    const uint32_t raw_tx = (uint32_t)((a.TH + 2) * (a.TW + 2) * a.TN * 128);
+    auto issue_raw = [&](int u) {
+      const int b = u % WG_RAW_BUFS;
+      int w0, h0, n0;
+      tile_origin(u, &w0, &h0, &n0);
+      mbar_expect_tx(&raw_full[b], raw_tx);
+      tma_load_4d(raw + b * WG_RAW_BYTES, &tmX, &raw_full[b], ci0, w0 - 1, h0 - 1, n0);
+    };
+    if (t == 0)
+      for (int u = 0; u < WG_RAW_BUFS && u < nk; ++u) issue_raw(u);
+    const int ngrp = patch_rows / 4, ntask = 3 * ngrp;
+    for (int k = 0; k < nk; ++k) {
+      const int s = k & 1;
       uint8_t* st = stages + s * WG_STAGE_BYTES;
-      // A: chunk kc = pixels 32 kc .. 32 kc + 31 of both co boxes
+      mbar_wait(&empty[s], ((k >> 1) & 1) ^ 1);
+      if (t == 0) {
+        int w0, h0, n0;
+        tile_origin(k, &w0, &h0, &n0);
+        mbar_expect_tx(&full[s], WG_DY_BYTES);
 #pragma unroll
-      for (int kc = 0; kc < 2; ++kc) transpose_mn_tile(raw + kc * 4096, st + kc * (64 * 128), 64, t, 128, WG_KP * 128);
-      for (int kw = 0; kw < 3; ++kw)
-        for (int kc = 0; kc < patch_chunks; ++kc)
-          transpose_mn_tile(raw + WG_RAW_A + kw * WG_PATCH + kc * 4096, st + WG_A_BYTES + kw * WG_B_ONE + kc * 4096, 32, t, 128);
-      if (do_bias) {
-        const int co = t & 63, p0 = (t >> 6) * 32;
-        const uint8_t* box = raw + (co >> 5) * (WG_KP * 128);
-#pragma unroll 8
-        for (int p = p0; p < p0 + 32; ++p) bsum += *reinterpret_cast<const float*>(box + sw128_off(p, co & 31));
+        for (int j = 0; j < WG_CO / 32; ++j) tma_load_4d(st + j * (WG_KP * 128), &tmDY, &full[s], co0 + j * 32, w0, h0, n0);
       }
-      fence_proxy_async();
-      named_bar(1, 128);
+      {
+        const int b = k % WG_RAW_BUFS;
+        mbar_wait(&raw_full[b], (k / WG_RAW_BUFS) & 1);
+        const uint8_t* rw = raw + b * WG_RAW_BYTES;
+        uint8_t* xt = st + WG_DY_BYTES;
+        // one warp per (kw, 4 pixels): lane = ci, so each read is one whole 128-byte halo row and each float4 write
+        // lands in a different row of the K-major copy (conflict-free both ways)
+        for (int task = warp; task < ntask; task += 4) {
+          const int kw = task / ngrp, p0 = (task - kw * ngrp) * 4;
+          float v[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int p = p0 + i, q = p / a.TW, j = p - q * a.TW;
+            v[i] = *reinterpret_cast<const float*>(rw + sw128_off(q * (a.TW + 2) + j + kw, lane));
+          }
+          *reinterpret_cast<float4*>(xt + kw * WG_XT_KW + (p0 >> 5) * 4096 + sw128_off(lane, p0 & 31)) =
+              make_float4(v[0], v[1], v[2], v[3]);
+        }
+        fence_proxy_async();
+        named_bar(1, 128);                          // every thread is done with halo buffer b
+        if (t == 0 && k + WG_RAW_BUFS < nk) issue_raw(k + WG_RAW_BUFS);
+      }
       if (t == 0) mbar_arrive(&full[s]);
     }
-    if (do_bias && co0 + (t & 63) < a.Cout) atomicAdd(a.db + co0 + (t & 63), bsum);
   } else {
     regs_alloc<224>();
     const int ct = threadIdx.x - 128;
-    const int wg = ct >> 7, t = ct & 127;
+    const int wg = ct >> 7, t = ct & 127, wl = t >> 5, lane = t & 31, g = lane >> 2, q = lane & 3;
+    // this thread's A rows: co 16 wl + g (+8), in dY box wl / 2 at column 16 (wl & 1) + g (+8)
+    const int box = wl >> 1, col = 16 * (wl & 1) + g;
+    const uint32_t off0 = sw128_off(q, col), off1 = sw128_off(q, col + 8), off2 = sw128_off(q + 4, col),
+                   off3 = sw128_off(q + 4, col + 8);
     float acc[9][8];
 #pragma unroll
     for (int j = 0; j < 9; ++j)
 #pragma unroll
       for (int e = 0; e < 8; ++e) acc[j][e] = 0.f;
-    for (int kb = 0; kb < nk; ++kb) {
-      const int s = kb % WG_STAGES;
-      mbar_wait(&full[s], (kb / WG_STAGES) & 1);
-      const uint8_t* st = stages + s * WG_STAGE_BYTES;
-      wgrad_mma(acc, st, st + WG_A_BYTES, wg, a.TW, img_rows);
-      wgmma_wait<1>();          // stage kb stays in flight; the stage of kb - 1 is free
+    float bsum0 = 0.f, bsum1 = 0.f;                 // bias gradient of rows g and g + 8
+    uint32_t fr[2][4];                              // two fragment sets: one may still be read by the wgmmas in flight
+    for (int k = 0; k < nk; ++k) {
+      const int s = k & 1;
+      mbar_wait(&full[s], (k >> 1) & 1);
+      const uint32_t dyb = smem_u32(stages + s * WG_STAGE_BYTES + box * (WG_KP * 128));
+      // descriptor start addresses are 16-byte units in the low bits: offsets inside the stage are added to one base
+      // ci rows 16 wg.. of the [32 ci] copies: two whole 8-row swizzle groups further on
+      const uint64_t xdesc = make_sdesc(smem_u32(stages + s * WG_STAGE_BYTES + WG_DY_BYTES) + wg * 16 * 128);
+#pragma unroll 1   // rolled by k-step pairs: the tap descriptors of one pair live at a time, not all 72
+      for (int ks2 = 0; ks2 < 8; ks2 += 2) {
 #pragma unroll
-      for (int j = 0; j < 9; ++j) wgmma_keep(acc[j]);
-      if (kb > 0 && t == 0) mbar_arrive(&empty[(kb - 1) % WG_STAGES]);
+        for (int h = 0; h < 2; ++h) {
+          const int ks = ks2 + h;
+          uint32_t (&f)[4] = fr[h];
+          // pixel rows 8 ks + q (+4): the swizzle phase (row & 7) is the same every k-step, so one offset per element
+          const uint32_t fa = dyb + ks * 1024;
+          f[0] = ld_shared_u32(fa + off0);
+          f[1] = ld_shared_u32(fa + off1);
+          f[2] = ld_shared_u32(fa + off2);
+          f[3] = ld_shared_u32(fa + off3);
+          bsum0 += __uint_as_float(f[0]) + __uint_as_float(f[2]);
+          bsum1 += __uint_as_float(f[1]) + __uint_as_float(f[3]);
+          const int kb = 8 * ks + ((8 * ks) / img_rows) * 2 * a.TW;   // k of this step in the patch: + 2 TW per image
+          wgmma_fence();
+#pragma unroll
+          for (int tap = 0; tap < 9; ++tap) {
+            const int kh = tap / 3, kw = tap % 3;
+            const int kk = kb + kh * a.TW;
+            const uint32_t off = kw * WG_XT_KW + (kk >> 5) * 4096 + (kk & 31) / 8 * 32;
+            wgmma_tf32(acc[tap], f, xdesc + (off >> 4));
+          }
+          wgmma_commit();
+          wgmma_wait<1>();      // k-step ks stays in flight; ks - 1 (and its fragment set) is done
+#pragma unroll
+          for (int j = 0; j < 9; ++j) wgmma_keep(acc[j]);
+          if (ks == 0 && k > 0 && t == 0) mbar_arrive(&empty[(k - 1) & 1]);   // the last k-step of stage k - 1 is done
+        }
+      }
     }
     wgmma_wait<0>();
 #pragma unroll
     for (int j = 0; j < 9; ++j) wgmma_keep(acc[j]);
-    wgrad_store(acc, a, co0, ci0 + 16 * wg, t);
+#pragma unroll
+    for (int tap = 0; tap < 9; ++tap)
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const int co = co0 + 16 * wl + g + 8 * ((e >> 1) & 1);
+        const int ci = ci0 + 16 * wg + 8 * (e >> 2) + 2 * q + (e & 1);
+        if (co < a.Cout && ci < a.Cin) atomicAdd(a.dWp + ((size_t)tap * a.Cout + co) * a.Cin + ci, acc[tap][e]);
+      }
+    // bias: the quad's four threads hold the same rows at different pixels; one atomic per co on the ci-tile-0 CTAs
+    // (both warpgroups read the same rows: warpgroup 0 adds them)
+    bsum0 += __shfl_xor_sync(0xffffffffu, bsum0, 1);
+    bsum0 += __shfl_xor_sync(0xffffffffu, bsum0, 2);
+    bsum1 += __shfl_xor_sync(0xffffffffu, bsum1, 1);
+    bsum1 += __shfl_xor_sync(0xffffffffu, bsum1, 2);
+    if (a.db && ci_t == 0 && wg == 0 && q == 0) {
+      const int co = co0 + 16 * wl + g;
+      if (co < a.Cout) atomicAdd(a.db + co, bsum0);
+      if (co + 8 < a.Cout) atomicAdd(a.db + co + 8, bsum1);
+    }
   }
 }
 
@@ -705,12 +748,46 @@ static bool pick_wgrad_tile(int W, int H, int* TW, int* TH, int* TN) {
   int th = 1;
   while (th * 2 * tw <= 64 && H % (th * 2) == 0) th *= 2;
   int tn = 64 / (tw * th);
-  if ((th * tw) % 8 != 0 || (th + 2) * tw * tn > 96) {   // fall back to one image per tile, partial tiles in H allowed
+  if ((th * tw) % 8 != 0 || (th + 2) * tw * tn > WG_PATCH_PX) {   // fall back to one image per tile, partial tiles in H allowed
     th = 64 / tw;
     tn = 1;
   }
   *TW = tw; *TH = th; *TN = tn;
   return true;
+}
+
+static int launch_wgrad(const float* x, const float* dy, WgradArgs a, cudaStream_t stream) {
+  const long long out_tiles = (long long)((a.Cout + WG_CO - 1) / WG_CO) * ((a.Cin + WG_CI - 1) / WG_CI);
+  const long long total_tiles = (long long)a.tiles_w * a.tiles_h * a.tiles_n;
+  // split-K factor.  The kernel runs one CTA per SM (its shared memory allows no second), so the grid executes in whole
+  // waves of `sms` CTAs: pick the split that fills 1..3 waves best (ties -> fewer waves: fewer partial sums to add).
+  const int sms = num_sms();
+  long long ks = 1;
+  {
+    double best = -1.0;
+    for (int w = 1; w <= 3; ++w) {
+      long long k = (long long)sms * w / out_tiles;
+      if (k < 1) k = 1;
+      if (k > total_tiles) k = total_tiles;
+      const long long ctas = k * out_tiles;
+      const long long waves = (ctas + sms - 1) / sms;
+      const double fill = (double)ctas / (double)(waves * sms);
+      if (fill > best + 1e-9) { best = fill; ks = k; }
+    }
+  }
+  if (ks > total_tiles) ks = total_tiles;
+  if (ks < 1) ks = 1;
+  if (ks > 65535) ks = 65535;
+  a.ksplit = (int)ks;
+  CUtensorMap tmDY, tmX;
+  int r;
+  if ((r = make_act_map(&tmDY, dy, a.N, a.H, a.W, a.Cout, a.TW, a.TH, a.TN))) return r;
+  if ((r = make_act_map(&tmX, x, a.N, a.H, a.W, a.Cin, a.TW + 2, a.TH + 2, a.TN))) return r;
+  if ((r = allow_dynamic_smem<conv3x3_wgrad_kernel>(WG_SMEM, "wgrad"))) return r;
+  dim3 grid((unsigned)out_tiles, a.ksplit);
+  conv3x3_wgrad_kernel<<<grid, WG_THREADS, WG_SMEM, stream>>>(tmDY, tmX, a);
+  HK_LAUNCH_CHECK("conv3x3_wgrad_kernel");
+  return 0;
 }
 
 static int conv3x3_wgrad_1x(const float* x, const float* dy, float* dwp, float* db, int N, int H, int W, int Cin, int Cout,
@@ -740,34 +817,9 @@ static int conv3x3_wgrad_1x(const float* x, const float* dy, float* dwp, float* 
   WgradArgs a = {};
   a.dWp = dwp; a.db = db; a.N = N; a.H = H; a.W = W; a.Cin = Cin; a.Cout = Cout;
   pick_wgrad_tile(W, H, &a.TW, &a.TH, &a.TN);
-  HK_REQUIRE((a.TH + 2) * a.TW * a.TN * 128 <= WG_PATCH, HK_ERR_UNSUPPORTED, "conv3x3_wgrad: halo patch too large");
+  HK_REQUIRE((a.TH + 2) * a.TW * a.TN <= WG_PATCH_PX && (a.TH + 2) * (a.TW + 2) * a.TN <= WG_RAW_ROWS, HK_ERR_UNSUPPORTED,
+             "conv3x3_wgrad: halo patch too large");
   a.tiles_w = (W + a.TW - 1) / a.TW; a.tiles_h = (H + a.TH - 1) / a.TH; a.tiles_n = (N + a.TN - 1) / a.TN;
-  const long long out_tiles = (long long)((Cout + 63) / 64) * (Cin / 32);
-  const long long total_tiles = (long long)a.tiles_w * a.tiles_h * a.tiles_n;
-  // split-K factor.  The kernel runs one CTA per SM (157 KB of shared memory), so the grid executes in whole waves of
-  // `sms` CTAs: pick the split that fills 1..3 waves best (ties -> fewer waves: fewer partial sums to add atomically).
-  const int sms = num_sms();
-  long long ks = 1;
-  {
-    double best = -1.0;
-    for (int w = 1; w <= 3; ++w) {
-      long long k = (long long)sms * w / out_tiles;
-      if (k < 1) k = 1;
-      if (k > total_tiles) k = total_tiles;
-      const long long ctas = k * out_tiles;
-      const long long waves = (ctas + sms - 1) / sms;
-      const double fill = (double)ctas / (double)(waves * sms);
-      if (fill > best + 1e-9) { best = fill; ks = k; }
-    }
-  }
-  if (ks > total_tiles) ks = total_tiles;
-  if (ks < 1) ks = 1;
-  if (ks > 65535) ks = 65535;
-  a.ksplit = (int)ks;
-  CUtensorMap tmDY, tmX;
-  int r;
-  if ((r = make_act_map(&tmDY, dy, N, H, W, Cout, a.TW, a.TH, a.TN))) return r;
-  if ((r = make_act_map(&tmX, x, N, H, W, Cin, a.TW, a.TH + 2, a.TN))) return r;
   cudaError_t e = cudaSuccess;
   if (zero_dw) {
     e = cudaMemsetAsync(dwp, 0, (size_t)9 * Cout * Cin * sizeof(float), stream);
@@ -777,11 +829,7 @@ static int conv3x3_wgrad_1x(const float* x, const float* dy, float* dwp, float* 
     e = cudaMemsetAsync(db, 0, (size_t)Cout * sizeof(float), stream);
     if (e != cudaSuccess) return set_error((int)e, "cudaMemsetAsync(db): %s", cudaGetErrorString(e));
   }
-  if ((r = allow_dynamic_smem<conv3x3_wgrad_kernel>(WG_SMEM, "wgrad"))) return r;
-  dim3 grid((unsigned)out_tiles, a.ksplit);
-  conv3x3_wgrad_kernel<<<grid, WG_THREADS, WG_SMEM, stream>>>(tmDY, tmX, a);
-  HK_LAUNCH_CHECK("conv3x3_wgrad_kernel");
-  return 0;
+  return launch_wgrad(x, dy, a, stream);
 }
 
 // ------------------------------------------------------------------------------------------------
