@@ -44,7 +44,10 @@ __global__ void pack_stem_weights_kernel(const float* __restrict__ w, float* __r
 }
 
 // ------------------------------------------------------------------------------------------------ BatchNorm2d (train)
-// per-block partial column sums of x and x^2 over a slab of pixels:  part[blk][0][c], part[blk][1][c]
+// per-block partial column sums of d = x - x[0] and d^2 over a slab of pixels:  part[blk][0][c], part[blk][1][c].
+// Summing x and x^2 directly would lose the variance to cancellation in E[x^2] - mean^2 when a channel's mean is large
+// against its spread (at mean = 100 sigma, up to 2e-3 of invstd); the shift by the channel's first value keeps d at the
+// spread's scale, and x - x[0] is exact for values within a factor 2 of each other.
 __global__ void bn_stats_partial_kernel(const float* __restrict__ x, float* __restrict__ part, long long P, int C) {
   extern __shared__ float sm[];   // [2][plan][C4*4]
   const int C4 = C / 4;
@@ -56,9 +59,11 @@ __global__ void bn_stats_partial_kernel(const float* __restrict__ x, float* __re
   for (int c4 = cl; c4 < C4; c4 += clanes) {
     float4 s = make_float4(0.f, 0.f, 0.f, 0.f), q = s;
     if (pl < plan) {
+      const float4 k = __ldg(reinterpret_cast<const float4*>(x) + c4);
 #pragma unroll 8
       for (long long p = p0 + pl; p < p1; p += plan) {
-        const float4 v = __ldg(reinterpret_cast<const float4*>(x + p * C) + c4);
+        float4 v = __ldg(reinterpret_cast<const float4*>(x + p * C) + c4);
+        v.x -= k.x; v.y -= k.y; v.z -= k.z; v.w -= k.w;
         s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
         q.x = fmaf(v.x, v.x, q.x); q.y = fmaf(v.y, v.y, q.y); q.z = fmaf(v.z, v.z, q.z); q.w = fmaf(v.w, v.w, q.w);
       }
@@ -74,10 +79,11 @@ __global__ void bn_stats_partial_kernel(const float* __restrict__ x, float* __re
     part[((size_t)blockIdx.x * 2 + 1) * C + c] = q;
   }
 }
-// mean / invstd (biased variance) + running-stat update with the unbiased variance (nn.BatchNorm2d, momentum 0.1)
-__global__ void bn_stats_finalize_kernel(const float* __restrict__ part, int nblk, long long P, int C, float eps,
-                                         float momentum, float* __restrict__ mean, float* __restrict__ invstd,
-                                         float* __restrict__ rmean, float* __restrict__ rvar) {
+// mean / invstd (biased variance) + running-stat update with the unbiased variance (nn.BatchNorm2d, momentum 0.1), from
+// the shifted sums of bn_stats_partial_kernel: mean = x[0] + E[d], var = E[d^2] - E[d]^2
+__global__ void bn_stats_finalize_kernel(const float* __restrict__ x, const float* __restrict__ part, int nblk, long long P,
+                                         int C, float eps, float momentum, float* __restrict__ mean,
+                                         float* __restrict__ invstd, float* __restrict__ rmean, float* __restrict__ rvar) {
   // block = 32 channels x 32 partial-row lanes: lanes run along channels (coalesced 128 B reads of the partial rows)
   __shared__ float red[2][32][32];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -92,9 +98,10 @@ __global__ void bn_stats_finalize_kernel(const float* __restrict__ part, int nbl
   if (w != 0 || c >= C) return;
   double sd = 0.0, qd = 0.0;
   for (int k = 0; k < 32; ++k) { sd += (double)red[0][k][lane]; qd += (double)red[1][k][lane]; }
-  const double m = sd / (double)P;
-  double var = qd / (double)P - m * m;
+  const double md = sd / (double)P;
+  double var = qd / (double)P - md * md;
   if (var < 0.0) var = 0.0;
+  const double m = (double)x[c] + md;
   mean[c] = (float)m;
   invstd[c] = (float)(1.0 / sqrt(var + (double)eps));
   if (rmean) {
@@ -399,7 +406,7 @@ int hk_bn_fwd(const float* x, const float* gamma, const float* beta, const float
   const int C4 = C / 4, clanes = C4 < 256 ? C4 : 256, plan = 256 / clanes;
   bn_stats_partial_kernel<<<nb, 256, (size_t)2 * plan * C * sizeof(float), st>>>(x, part, P, C);
   HK_LAUNCH_CHECK("bn_stats_partial_kernel");
-  bn_stats_finalize_kernel<<<(C + 31) / 32, 1024, 0, st>>>(part, nb, P, C, eps, momentum, save_mean, save_invstd,
+  bn_stats_finalize_kernel<<<(C + 31) / 32, 1024, 0, st>>>(x, part, nb, P, C, eps, momentum, save_mean, save_invstd,
                                                          running_mean, running_var);
   HK_LAUNCH_CHECK("bn_stats_finalize_kernel");
   bn_apply_kernel<<<grid_1d((size_t)P * C4, 256), 256, 0, st>>>(x, save_mean, save_invstd, gamma, beta, residual, y,

@@ -411,30 +411,51 @@ def sgd_momentum_step(p, g, buf, lr, momentum, weight_decay, first):
 RESNET50_LAYERS = ((64, 3, 1), (128, 4, 2), (256, 6, 2), (512, 3, 2))   # (planes, blocks, stride)
 
 
+def resnet_layers(blocks):
+    """(planes, blocks, stride) of layer1..4 for a trunk with the given block counts, e.g. (3, 4, 23, 3) for ResNet-101."""
+    return tuple(zip((64, 128, 256, 512), blocks, (1, 2, 2, 2)))
+
+
 def _bn_train(x, st, pre, eps=1e-5):
     """nn.BatchNorm2d in train mode: batch statistics (biased var), affine (resnet.py:114-140 via norm_layer)."""
     return F.batch_norm(x, None, None, st[pre + '.weight'], st[pre + '.bias'], training=True, eps=eps)
 
 
-def _bottleneck(x, st, pre, stride, has_ds, nl=Plain):
+def _bn_eval(x, st, pre, eps=1e-5):
+    """nn.BatchNorm2d in eval mode: normalises with the running statistics st[pre + '.running_mean' / '.running_var']."""
+    return F.batch_norm(x, st[pre + '.running_mean'], st[pre + '.running_var'], st[pre + '.weight'], st[pre + '.bias'],
+                        training=False, eps=eps)
+
+
+def bn_batch_stats(x):
+    """Per-channel batch statistics of an NCHW tensor as train-mode BatchNorm2d takes them: (mean, biased variance, which
+    normalises, unbiased variance, which enters the running average)."""
+    mean = x.mean(dim=(0, 2, 3))
+    var = x.var(dim=(0, 2, 3), unbiased=False)
+    n = x.numel() // x.shape[1]
+    return mean, var, var * n / max(n - 1, 1)
+
+
+def _bottleneck(x, st, pre, stride, has_ds, nl=Plain, bn=_bn_train):
     """Bottleneck.forward (resnet.py:124-144): stride on the 3x3 (v1.5, :116)."""
-    out = nl.relu(_bn_train(F.conv2d(x, st[pre + '.conv1.weight']), st, pre + '.bn1'))
-    out = nl.relu(_bn_train(F.conv2d(out, st[pre + '.conv2.weight'], stride=stride, padding=1), st, pre + '.bn2'))
-    out = _bn_train(F.conv2d(out, st[pre + '.conv3.weight']), st, pre + '.bn3')
+    out = nl.relu(bn(F.conv2d(x, st[pre + '.conv1.weight']), st, pre + '.bn1'))
+    out = nl.relu(bn(F.conv2d(out, st[pre + '.conv2.weight'], stride=stride, padding=1), st, pre + '.bn2'))
+    out = bn(F.conv2d(out, st[pre + '.conv3.weight']), st, pre + '.bn3')
     identity = x
     if has_ds:
-        identity = _bn_train(F.conv2d(x, st[pre + '.downsample.0.weight'], stride=stride), st, pre + '.downsample.1')
+        identity = bn(F.conv2d(x, st[pre + '.downsample.0.weight'], stride=stride), st, pre + '.downsample.1')
     return nl.relu(out + identity)
 
 
-def resnet50_trunk_fwd(x, st, prefix='backbone.', nl=Plain):
-    """children()[:-2] of ResNet-50 (MPNCOV.py:28-29): conv1, bn1, relu, maxpool, layer1..4 -> [B,2048,H/32,W/32]."""
+def resnet50_trunk_fwd(x, st, prefix='backbone.', nl=Plain, layers=RESNET50_LAYERS, bn=_bn_train):
+    """children()[:-2] of ResNet-50 (MPNCOV.py:28-29): conv1, bn1, relu, maxpool, layer1..4 -> [B,2048,H/32,W/32].
+    ``layers`` gives other depths (``resnet_layers((3, 4, 23, 3))`` is ResNet-101); ``bn=_bn_eval`` is the eval-mode trunk."""
     x = F.conv2d(x, st[prefix + '0.weight'], stride=2, padding=3)
-    x = nl.relu(_bn_train(x, st, prefix + '1'))
+    x = nl.relu(bn(x, st, prefix + '1'))
     x = nl.maxpool(x, 3, 2, 1)
-    for li, (planes, blocks, stride) in enumerate(RESNET50_LAYERS):
+    for li, (planes, blocks, stride) in enumerate(layers):
         for b in range(blocks):
-            x = _bottleneck(x, st, f'{prefix}{4 + li}.{b}', stride if b == 0 else 1, b == 0, nl=nl)
+            x = _bottleneck(x, st, f'{prefix}{4 + li}.{b}', stride if b == 0 else 1, b == 0, nl=nl, bn=bn)
     return x
 
 

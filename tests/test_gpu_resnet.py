@@ -20,11 +20,23 @@ def _nchw(t):
     return t.permute(0, 3, 1, 2).contiguous()
 
 
-@pytest.mark.parametrize('N,H,W,C,relu,res', [(4, 6, 6, 64, 1, 0), (2, 4, 4, 256, 1, 1), (3, 5, 7, 128, 0, 0), (2, 2, 2, 2048, 1, 1)])
-def test_batchnorm_train(N, H, W, C, relu, res):
+# (N, H, W, C, relu, residual, k): the channels' means sit at k x their spread.  P = N*H*W pixels are summed in
+# min(ceil(P / 256), 592) blocks: 1 block up to P = 256; 2 at P = 300; 32 at 8192; 98 at 25088 (the stem at 224x224, batch 2:
+# the finalize loops over more than 32 partial rows); the 592 cap at 401408 (layer1 at 448x448, batch 32).
+BN_CASES = [(4, 6, 6, 64, 1, 0, 0), (2, 4, 4, 256, 1, 1, 0), (3, 5, 7, 128, 0, 0, 0), (2, 2, 2, 2048, 1, 1, 0),
+            (3, 10, 10, 12, 1, 0, 0), (3, 10, 10, 12, 0, 1, 100),
+            (2, 64, 64, 2048, 1, 0, 10), (2, 64, 64, 2048, 0, 0, 100),
+            (2, 112, 112, 64, 1, 0, 0), (2, 112, 112, 64, 1, 1, 10), (2, 112, 112, 64, 1, 0, 100),
+            (32, 112, 112, 4, 1, 0, 100), (32, 112, 112, 64, 1, 0, 10), (32, 112, 112, 12, 0, 1, 0)]
+
+
+@pytest.mark.parametrize('N,H,W,C,relu,res,k', BN_CASES,
+                         ids=['-'.join(map(str, c[:6])) + (f'-mean{c[6]}sigma' if c[6] else '') for c in BN_CASES])
+def test_batchnorm_train(N, H, W, C, relu, res, k):
     from hawkeye_b200 import _lib
     s = _lib.stream_ptr()
-    x = detgen.det((N, C, H, W), 1)
+    sigma = 0.5 + detgen.det((C,), 6, positive=True)               # per-channel spread
+    x = (detgen.det((N, C, H, W), 1) + k) * sigma.view(1, C, 1, 1)
     gamma, beta = 1 + detgen.det((C,), 2, 0.1), detgen.det((C,), 3, 0.1)
     r = detgen.det((N, C, H, W), 4) if res else None
     dy = detgen.det((N, C, H, W), 5)
@@ -34,9 +46,6 @@ def test_batchnorm_train(N, H, W, C, relu, res):
     y_ref = F.batch_norm(xd, rm, rv, gd, bd, training=True, momentum=0.1, eps=1e-5)
     if res:
         y_ref = y_ref + rd
-    if relu:
-        y_ref = F.relu(y_ref)
-    grads = torch.autograd.grad(y_ref, [xd, gd, bd] + ([rd] if res else []), dy.double())
     P = N * H * W
     xg, y = _nhwc(x).cuda(), torch.empty(N, H, W, C, device='cuda')
     mean, invstd = torch.empty(C, device='cuda'), torch.empty(C, device='cuda')
@@ -45,8 +54,23 @@ def test_batchnorm_train(N, H, W, C, relu, res):
     ws = torch.empty(nb, dtype=torch.uint8, device='cuda')
     rg = _nhwc(r).cuda() if res else None
     _lib.call('hk_bn_fwd', xg, gamma.cuda(), beta.cuda(), rg, y, mean, invstd, rmg, rvg, 0.1, 1e-5, P, C, relu, ws, nb, s)
-    assert rel_l2(_nchw(y).cpu(), y_ref.detach()) < 5e-4          # tf32-rounded on store
-    assert rel_l2(rmg.cpu(), rm) < 1e-5 and rel_l2(rvg.cpu(), rv) < 1e-5
+    # the statistics at fp32 accuracy whatever the offset; a mean near 0 has no relative scale of its own, so its error is
+    # taken in units of the channel's spread (which is what it shifts xhat = (x - mean) * invstd by)
+    xd64 = xd.detach()
+    m_ref, v_ref = xd64.mean(dim=(0, 2, 3)), xd64.var(dim=(0, 2, 3), unbiased=False)
+    sd = v_ref.sqrt()
+    errs = {'mean': ((mean.cpu().double() - m_ref).abs() / sd).max().item(),
+            'invstd': (invstd.cpu().double() * (v_ref + 1e-5).sqrt() - 1).abs().max().item(),
+            'running_mean': ((rmg.cpu().double() - rm).abs() / sd).max().item(),
+            'running_var': ((rvg.cpu().double() - rv).abs() / rv).max().item()}
+    print(f'bn P={P} C={C} mean={k} sigma:', {n: f'{e:.1e}' for n, e in errs.items()})
+    assert max(errs.values()) < 1e-5, errs
+    assert rel_l2(_nchw(y).cpu(), (F.relu(y_ref) if relu else y_ref).detach()) < 5e-4          # tf32-rounded on store
+    # the gradients on the ReLU branch this forward took: at a mean of 100 sigma, the fp32 mean itself is off by up to
+    # 6e-6 sigma, which flips the few outputs that close to zero, each an O(1) change of one dx element
+    if relu:
+        y_ref = y_ref * (_nchw(y) > 0).cpu().double()
+    grads = torch.autograd.grad(y_ref, [xd, gd, bd] + ([rd] if res else []), dy.double())
     dx, dres = torch.empty_like(xg), (torch.empty_like(xg) if res else None)
     dg, db = torch.empty(C, device='cuda'), torch.empty(C, device='cuda')
     _lib.call('hk_bn_bwd', xg, y, _nhwc(dy).cuda(), gamma.cuda(), mean, invstd, dx, dres, dg, db, P, C, relu, ws, nb, s)
@@ -60,6 +84,57 @@ def test_batchnorm_train(N, H, W, C, relu, res):
         _lib.call('hk_bn_bwd_ex', xg, None, _nhwc(dy).cuda(), gamma.cuda(), beta.cuda(), mean, invstd, dx2, None, dg2, db2, P, C,
                   relu, ws, nb, s)
         assert torch.equal(dx2, dx) and torch.equal(dg2, dg) and torch.equal(db2, db)
+
+
+@pytest.mark.parametrize('precision', [0, 1])
+@pytest.mark.parametrize('relu,res', [(0, 0), (1, 0), (0, 1), (1, 1)])
+def test_bn_apply_eval(relu, res, precision):
+    """eval-mode BatchNorm (hk_bn_apply on running statistics, the Tester path of every ResNet model) against fp64
+    F.batch_norm(training=False): the output is tf32-rounded for the next MMA in default mode, fp32 in precise mode."""
+    from hawkeye_b200 import _lib
+    N, H, W, C = 2, 14, 14, 256
+    x = detgen.det((N, C, H, W), 11, 2.0) + 0.5
+    rmean, rvar = detgen.det((C,), 12, 0.5), 0.25 + detgen.det((C,), 13, positive=True)
+    gamma, beta = 1 + detgen.det((C,), 14, 0.1), detgen.det((C,), 15, 0.1)
+    r = detgen.det((N, C, H, W), 16) if res else None
+    y_ref = F.batch_norm(x.double(), rmean.double(), rvar.double(), gamma.double(), beta.double(), training=False, eps=1e-5)
+    if res:
+        y_ref = y_ref + r.double()
+    if relu:
+        y_ref = F.relu(y_ref)
+    invstd = torch.rsqrt(rvar.cuda() + 1e-5)
+    y = torch.empty(N, H, W, C, device='cuda')
+    _lib.set_precise(precision)
+    try:
+        _lib.call('hk_bn_apply', _nhwc(x).cuda(), rmean.cuda(), invstd, gamma.cuda(), beta.cuda(),
+                  _nhwc(r).cuda() if res else None, y, N * H * W, C, relu, _lib.stream_ptr())
+    finally:
+        _lib.set_precise(0)
+    e = rel_l2(_nchw(y).cpu(), y_ref)
+    print('bn apply', relu, res, precision, e)
+    assert e < (5e-4 if not precision else 1e-6)
+    if relu:
+        assert (y >= 0).all()
+
+
+@pytest.mark.parametrize('N,H,W,C', [(2, 7, 9, 12), (3, 9, 7, 64), (2, 112, 112, 64)])
+def test_maxpool3x3_s2_edges(N, H, W, C):
+    """odd map sizes (the last window hangs over the bottom / right edge) and the stem's 112x112x64 output; post-ReLU
+    inputs put exact-zero ties in the windows, which go to the first maximum in scan order, as in PyTorch."""
+    from hawkeye_b200 import _lib
+    s = _lib.stream_ptr()
+    a = F.relu(detgen.det((N, C, H, W), 17)).double().requires_grad_(True)
+    p_ref = F.max_pool2d(a, 3, 2, 1)
+    g = detgen.det(p_ref.shape, 18).double()
+    (ga,) = torch.autograd.grad(p_ref, a, g)
+    Ho, Wo = p_ref.shape[2], p_ref.shape[3]
+    out = torch.empty(N, Ho, Wo, C, device='cuda')
+    am = torch.empty(N, Ho, Wo, C, device='cuda', dtype=torch.uint8)
+    _lib.call('hk_maxpool3x3s2_fwd', _nhwc(a.detach().float()).cuda(), out, am, N, H, W, C, s)
+    assert torch.equal(_nchw(out).cpu().double(), p_ref.detach())
+    dx = torch.empty(N, H, W, C, device='cuda')
+    _lib.call('hk_maxpool3x3s2_bwd', am, _nhwc(g.float()).cuda(), dx, N, H, W, C, s)
+    assert rel_l2(_nchw(dx).cpu(), ga) < 1e-6
 
 
 def test_maxpool3x3_s2_and_stride_helpers():

@@ -45,3 +45,19 @@ def test_resnet_mpn_tape():
     keys = {k for k, _ in net.named_parameters()}
     x, labels = detgen.det((2, 3, 64, 64), 51), detgen.det_labels(2, 200, 52)
     _check(lambda xx, s, nl: O.mpn_forward(xx, s, 5, nl=nl), x, labels, st, keys, tol=5e-3)
+
+
+def test_resnet_shallow_trunk_tape():
+    """The trunk alone with every unit kind (stem, 1x1 downsample at stride 1, an identity block, 3x3/s2 and 1x1/s2 units),
+    with its pooled features as the logits: the replay the GPU trunk tests compare against."""
+    from hawkeye_b200.backbone.resnet import ResNetTrunk
+    torch.set_num_threads(8)
+    blocks = (2, 1, 1, 1)
+    st = detgen.state_like(ResNetTrunk(blocks))
+    keys = {k for k, v in st.items() if v.is_floating_point() and 'running' not in k}
+    x, labels = detgen.det((2, 3, 64, 64), 61), detgen.det_labels(2, 2048, 62)
+
+    def forward(xx, s, nl):
+        return O.resnet50_trunk_fwd(xx, s, prefix='', nl=nl, layers=O.resnet_layers(blocks)).mean(dim=(2, 3))
+    worst = _check(forward, x, labels, st, keys)
+    print('shallow trunk tape: worst fp32 vs fp64 gradient', worst)
