@@ -96,6 +96,153 @@ class ClassificationPresetEval:
         return self.transforms(img)
 
 
+def _grid_cells(image, cols, rows):
+    """The ``cols x rows`` grid of crops of a PIL image, row by row; cell edges at int(size / count * i)."""
+    width, height = image.size
+    xs = [int(width / cols * i) for i in range(cols + 1)]
+    ys = [int(height / rows * j) for j in range(rows + 1)]
+    return [image.crop((xs[i], ys[j], min(xs[i + 1], width), min(ys[j + 1], height)))
+            for j in range(rows) for i in range(cols)]
+
+
+def _swap_last_two(seq):
+    """Shuffle the last two entries of ``seq`` in place with ``random.shuffle`` (one draw from Python's ``random``)."""
+    import random
+    if len(seq) >= 2:
+        pair = seq[-2:]
+        random.shuffle(pair)
+        seq[-2:] = pair
+
+
+class RandomSwap:
+    """DCL's jigsaw (dataset/transforms.py RandomSwap): crop 10 px off every border, cut the rest into a ``size[0] x
+    size[1]`` grid (columns x rows), and swap neighbours within a range of 2 — after each cell is placed in its row the last
+    two cells of that row may swap, and after each cell once at least two rows are complete the last two complete rows may
+    swap — then paste every cell, resized with Lanczos, into a canvas and resize it back to the input size.  The draws from
+    Python's ``random`` come in the reference's order, so a seeded run gives the reference's images.  The reference names
+    the filter ``Image.ANTIALIAS``, which Pillow 10 removed; ``Image.LANCZOS`` is the same filter."""
+
+    def __init__(self, size):
+        import numbers
+        if isinstance(size, numbers.Number):
+            size = (int(size), int(size))
+        if len(size) != 2:
+            raise ValueError('RandomSwap: give one size or two, (columns, rows)')
+        self.size = size
+
+    def __repr__(self):
+        return f'{self.__class__.__name__}(size={self.size})'
+
+    def __call__(self, img):
+        from PIL import Image
+        cols, rows = self.size
+        full_w, full_h = img.size
+        img = img.crop((10, 10, full_w - 10, full_h - 10))
+        cells = _grid_cells(img, cols, rows)
+        done, row = [], []
+        for cell in cells:
+            row.append(cell)
+            _swap_last_two(row)
+            if len(row) == cols:
+                done.append(row)
+                row = []
+            _swap_last_two(done)
+        order = [c for r in done for c in r]
+        width, height = img.size
+        iw, ih = int(width / cols), int(height / rows)
+        canvas = Image.new('RGB', (iw * cols, ih * rows))
+        for i, cell in enumerate(order):
+            canvas.paste(cell.resize((iw, ih), Image.LANCZOS), ((i % cols) * iw, (i // cols) * ih))
+        return canvas.resize((full_w, full_h))
+
+
+def _sample_tenth_per_class(paths, labels):
+    """A random tenth of every class (rounded down) in the order classes first appear: the reference's validation subset,
+    drawn with Python's ``random.sample``."""
+    import random
+    by_class = {}
+    for p, y in zip(paths, labels):
+        by_class.setdefault(y, []).append(p)
+    out_paths, out_labels = [], []
+    for y, ps in by_class.items():
+        pick = random.sample(list(range(len(ps))), len(ps) // 10)
+        out_paths += [ps[i] for i in pick]
+        out_labels += [y] * len(pick)
+    return out_paths, out_labels
+
+
+class DCLDataset(torch.utils.data.Dataset):
+    """dataset/dataset_DCL.py: items of DCL's jigsaw training.  ``transforms`` is the dict of Examples/DCL.py:19-51
+    ('swap', 'common_aug', '<mode>_totensor').
+
+    train: (image, shuffled image, label, label_swap, swap_law1, swap_law2, path); swap_law1 is the identity law
+    (i - n // 2) / n over the n = swap_size[0] x swap_size[1] cells; swap_law2 gives, for every cell of the shuffled image,
+    the law of the unshuffled cell whose summed per-band mean is nearest (the first on ties).  label_swap is -1 under cls_2
+    (the collate turns it into 1, 0) and label + num_classes under cls_2xmul only.
+    val: (image, label, label, swap_law1, swap_law1, path) over a random tenth of every class, and ``common_aug`` is
+    applied as in training — both as in the reference.  test: (image, label, path)."""
+
+    def __init__(self, root, meta_path, transforms=None, swap_size=(7, 7), mode='train', cls_2=True, cls_2xmul=False):
+        import pandas as pd
+        self.root = root
+        meta = pd.read_csv(meta_path, sep=' ', names=['label', 'path'])
+        self.paths, self.labels = meta['path'].tolist(), meta['label'].tolist()
+        if mode == 'val':
+            self.paths, self.labels = _sample_tenth_per_class(self.paths, self.labels)
+        self.use_cls_2, self.use_cls_mul = cls_2, cls_2xmul
+        self.num_classes = len(set(self.labels))
+        self.swap_size, self.mode = list(swap_size), mode
+        self.common_aug, self.swap = transforms['common_aug'], transforms['swap']
+        self.totensor = transforms[mode + '_totensor']
+
+    def __len__(self):
+        return len(self.paths)
+
+    def __getitem__(self, item):
+        from PIL import ImageStat
+        img = webfg_loader(os.path.join(self.root, self.paths[item]))
+        label = self.labels[item]
+        if self.mode == 'test':
+            return self.totensor(img), label, self.paths[item]
+        if self.common_aug is not None:
+            img = self.common_aug(img)
+        n = self.swap_size[0] * self.swap_size[1]
+        law1 = [(i - n // 2) / n for i in range(n)]
+        if self.mode != 'train':
+            return self.totensor(img), label, label, law1, list(law1), self.paths[item]
+        swapped = self.swap(img)
+        ref = [sum(ImageStat.Stat(c).mean) for c in _grid_cells(img, *self.swap_size)]
+        law2 = []
+        for s in (sum(ImageStat.Stat(c).mean) for c in _grid_cells(swapped, *self.swap_size)):
+            dist = [abs(s - r) for r in ref]
+            law2.append((dist.index(min(dist)) - n // 2) / n)
+        label_swap = -1 if self.use_cls_2 else (label + self.num_classes if self.use_cls_mul else None)
+        return self.totensor(img), self.totensor(swapped), label, label_swap, law1, law2, self.paths[item]
+
+
+def collate_fn4train(batch):
+    """Interleaves every image with its shuffled copy: -> (images [2n, ...], labels [2n], labels_swap [2n] (1, 0 per pair
+    under cls_2, else label, label_swap), swap_law [2n, cells], paths [n])."""
+    imgs, labels, labels_swap, law, names = [], [], [], [], []
+    for s in batch:
+        imgs += [s[0], s[1]]
+        labels += [s[2], s[2]]
+        labels_swap += [1, 0] if s[3] == -1 else [s[2], s[3]]
+        law += [s[4], s[5]]
+        names.append(s[-1])
+    return (torch.stack(imgs, 0), torch.from_numpy(np.array(labels)).long(), torch.from_numpy(np.array(labels_swap)).long(),
+            torch.from_numpy(np.array(law)).float(), names)
+
+
+def collate_fn4val(batch):
+    """-> (images [n, ...], labels [n], labels_swap [n] (= labels), swap_law [n, cells], paths [n])."""
+    imgs = torch.stack([s[0] for s in batch], 0)
+    labels = torch.from_numpy(np.array([s[1] for s in batch])).long()
+    labels_swap = torch.from_numpy(np.array([1 if s[3] == -1 else s[2] for s in batch])).long()
+    law = torch.from_numpy(np.array([s[3] for s in batch])).float()
+    return imgs, labels, labels_swap, law, [s[-1] for s in batch]
+
+
 class BalancedBatchSampler(BatchSampler):
     """sampler.py:5-38: every batch holds ``n_classes`` classes drawn without replacement and ``n_samples`` images of each —
     the batches MAMCLoss needs (every anchor has same-class partners).  Uses numpy's global RNG in the reference's call order

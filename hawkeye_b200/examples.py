@@ -1,13 +1,14 @@
 """Trainer subclasses of the hot-path methods with the reference's Examples/ surface:
-``python -m hawkeye_b200.examples {BCNN,CBCNN,MPN,PeerLearning,OSMENet,APINet} --config <yaml>`` replaces
+``python -m hawkeye_b200.examples {BCNN,CBCNN,MPN,PeerLearning,OSMENet,APINet,DCL} --config <yaml>`` replaces
 ``python Examples/<Method>.py --config <yaml>`` (same yaml files; one process per GPU under torchrun instead of nn.DataParallel).
 
 Only what the reference's Examples override is overridden here: which parameters train, with which learning rates, and
 which LR schedule — the step itself is ``Trainer.batch_training``.
 """
+import os
 import sys
 
-from .train import PeerLearningTrainer, Trainer, _Cosine, _Plateau
+from .train import PeerLearningTrainer, Trainer, _Cosine, _Plateau, _Step
 
 
 def _warmup_cosine(opt, config, total_epoch):
@@ -151,11 +152,106 @@ class APINetTrainer(Trainer):
         return 8 * n, 4 * n
 
 
+class DCLTrainer(Trainer):
+    """Examples/DCL.py: every source image and its jigsaw-shuffled copy are interleaved into one batch of 2n rows; the model
+    returns [logits, swap_logits, mask]; criterion = DCLLoss(labels, labels_swap, swap_law); SGD with momentum and no weight
+    decay (Examples/DCL.py:82-87 passes none, whatever the yaml says) with the trunk at lr and classifier, classifier_swap
+    and Convmask at lr_ratio x lr; StepLR(step_size, gamma) once per epoch.  The meters count the 2n rows, as
+    Examples/DCL.py:116-117 does.
+
+    The dataset's swap law is taken on the same ``swap_num`` grid the jigsaw uses.  The reference's Examples/DCL.py passes no
+    swap_size, so its law is always 7x7; with the default swap_num [7, 7] the two are identical, and with any other grid
+    the reference's law would not describe the shuffled cells.
+
+    The data path is always the mirror in hawkeye_b200.data (RandomSwap, DCLDataset, collate_fn4train / collate_fn4val),
+    even inside a Hawkeye checkout: the reference's RandomSwap calls ``Image.ANTIALIAS``, which Pillow 10 removed, so its
+    own transform no longer runs."""
+
+    def get_transformers(self, config):
+        """Examples/DCL.py:19-51, with its defaults 512, 448 and [7, 7]."""
+        from torchvision.transforms import transforms
+        from .data import RandomSwap
+        resize = config.resize_size if 'resize_size' in config else 512
+        crop = config.image_size if 'image_size' in config else 448
+        swap = config.swap_num if 'swap_num' in config else [7, 7]
+        norm = transforms.Normalize([0.485, 0.456, 0.406], [0.229, 0.224, 0.225])
+        to_tensor = transforms.Compose([transforms.Resize((crop, crop)), transforms.ToTensor(), norm])
+        return {
+            'swap': transforms.Compose([RandomSwap((swap[0], swap[1]))]),
+            'common_aug': transforms.Compose([transforms.Resize((resize, resize)), transforms.RandomRotation(degrees=15),
+                                              transforms.RandomCrop((crop, crop)), transforms.RandomHorizontalFlip()]),
+            'train_totensor': to_tensor,
+            'val_totensor': to_tensor,
+            'test_totensor': transforms.Compose([transforms.Resize((resize, resize)), transforms.CenterCrop((crop, crop)),
+                                                 transforms.ToTensor(), norm]),
+            'None': None,
+        }
+
+    def get_dataloader(self, config):
+        from torch.utils.data import DataLoader
+        from .data import DCLDataset, collate_fn4train, collate_fn4val
+        t = config.transformer
+        tf = self.get_transformers(t)
+        swap = t.swap_num if 'swap_num' in t else [7, 7]
+        mc = self.config.model
+        self.datasets = {s: DCLDataset(config.root_dir, os.path.join(config.meta_dir, s + '.txt'), transforms=tf,
+                                       swap_size=swap, mode=s, cls_2=mc.cls_2, cls_2xmul=mc.cls_2xmul)
+                         for s in ('train', 'val')}
+        if config.batch_size % self.world != 0:
+            raise ValueError(f'dataset.batch_size={config.batch_size} must be a multiple of the {self.world} ranks')
+        loaders = {}
+        for s, collate in (('train', collate_fn4train), ('val', collate_fn4val)):
+            sampler = None
+            if self.world > 1:
+                from torch.utils.data.distributed import DistributedSampler
+                sampler = DistributedSampler(self.datasets[s], num_replicas=self.world, rank=self.rank, shuffle=s == 'train')
+            self.samplers[s] = sampler
+            loaders[s] = DataLoader(self.datasets[s], config.batch_size // self.world, num_workers=config.num_workers,
+                                    pin_memory=True, sampler=sampler, shuffle=(s == 'train' and sampler is None),
+                                    collate_fn=collate)
+        return loaders
+
+    def get_criterion(self, config):
+        from .losses import DCLLoss
+        return DCLLoss(config)
+
+    def param_groups(self):
+        m = self.get_model_module()
+        ratio = self.config.train.optimizer.lr_ratio
+        return [(list(m.backbone.parameters()), 1.0), (list(m.classifier.parameters()), ratio),
+                (list(m.classifier_swap.parameters()), ratio), (list(m.Convmask.parameters()), ratio)]
+
+    def get_optimizer(self, config):
+        from . import engine
+        lrs = [config.lr * m for g, m in self.param_groups() if any(p.requires_grad for p in g)]
+        return engine.FusedSGD(self.flat, lr=config.lr, momentum=config.momentum if 'momentum' in config else 0.0,
+                               weight_decay=0.0, group_lrs=lrs)
+
+    def get_scheduler(self, config):
+        return _Step(self.optimizer, config.step_size, config.gamma)
+
+    def batch_tensors(self, data):
+        images, labels, labels_swap, swap_law, _ = data
+        return images, (labels, labels_swap, swap_law)
+
+    def batch_validate(self, data):
+        import torch
+        from .train import accuracy
+        images, labels = self.to_device(data[0]), self.to_device(data[1].long())
+        with torch.no_grad():
+            out = self.model(images)
+        logit = out[0]
+        if self.config.model.cls_2xmul:
+            K = logit.shape[1]
+            logit = logit + out[1][:, :K] + out[1][:, K:2 * K]
+        self.average_meters['acc'].update(accuracy(logit, labels, 1), labels.size(0))
+
+
 TRAINERS = {'BCNN': BCNNTrainer, 'CBCNN': CBCNNTrainer, 'MPN': MPNTrainer, 'PeerLearning': PeerLearningTrainer,
             'OSMENet': OSMENetTrainer}
 # TRAINERS keeps the key set it has always had, so code that enumerates it sees no change; the command line dispatches
-# over every method, APINet included.
-ALL_TRAINERS = dict(TRAINERS, APINet=APINetTrainer)
+# over every method, APINet and DCL included.
+ALL_TRAINERS = dict(TRAINERS, APINet=APINetTrainer, DCL=DCLTrainer)
 
 
 def main(argv=None):

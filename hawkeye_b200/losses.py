@@ -135,3 +135,38 @@ class APINetLoss(nn.Module):
         loss, correct = APINetLossFn.apply(logits, targets, self.margin)
         self.last_correct = correct
         return loss
+
+
+def dcl_stacked_logits(logits, swap_logits):
+    """-> one [R, ld] tensor with ``logits`` in columns [0, K) and ``swap_logits`` in [K, K + K2).  When the two are DCL's
+    own column views of one contiguous [R, Kp] classifier output — all its rows, its strides, adjacent columns — that output
+    is returned as it is; anything else (a row slice of it, say) is concatenated into a new tensor."""
+    base = logits._base
+    R, K = logits.shape
+    if (base is not None and base is swap_logits._base and base.dim() == 2 and base.is_contiguous()
+            and base.shape[0] == R == swap_logits.shape[0] and base.shape[1] >= K + swap_logits.shape[1]
+            and logits.stride() == base.stride() and swap_logits.stride() == base.stride()
+            and logits.data_ptr() == base.data_ptr()
+            and swap_logits.data_ptr() == base.data_ptr() + K * base.element_size()):
+        return base
+    return torch.cat([logits, swap_logits], dim=1)
+
+
+class DCLLoss(nn.Module):
+    """model/loss/DCL_loss.py: alpha CE(logits, labels) + beta CE(swap_logits, labels_swap) + gamma L1(mask, swap_law), both
+    cross-entropies with label smoothing 0.1.  ``outputs`` is the list DCL returns; its two logit tensors are read in place
+    when they are the column views of one stacked classifier output, as DCL makes them.  One hk_dcl_loss launch;
+    ``last_correct`` is the top-1 count on the device (over the summed logits under cls_2xmul, Examples/DCL.py:104-107)."""
+
+    def __init__(self, config):
+        super().__init__()
+        self.alpha, self.beta, self.gamma = config.alpha, config.beta, config.gamma
+
+    def forward(self, outputs, labels, labels_swap, swap_law):
+        from .ops_dcl import DCLLossFn
+        logits, swap_logits, mask = outputs
+        K, K2 = logits.shape[1], swap_logits.shape[1]
+        loss, correct = DCLLossFn.apply(dcl_stacked_logits(logits, swap_logits), K, K2, labels, labels_swap, mask, swap_law,
+                                        self.alpha, self.beta, self.gamma, K2 == 2 * K)
+        self.last_correct = correct
+        return loss

@@ -5,3 +5,4 @@ from .peer_learning import PeerLearningNet  # noqa: F401
 from .cin import CIN, ChannelInteractionModule, CINClassifier  # noqa: F401
 from .osme import OSMENet, OSME, OSME_block  # noqa: F401
 from .apinet import APINet  # noqa: F401
+from .dcl import DCL  # noqa: F401

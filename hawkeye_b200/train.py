@@ -63,6 +63,11 @@ def accuracy(output, target, topk=1):
         return (correct * (100.0 / target.size(0))).item()
 
 
+def _as_tuple(labels):
+    """The criterion's target arguments: one labels tensor, or the tuple a multi-target ``batch_tensors`` gives."""
+    return labels if isinstance(labels, tuple) else (labels,)
+
+
 class Trainer:
     def __init__(self, config=None, dataloaders=None):
         self.config = config if config is not None else setup_config()
@@ -187,19 +192,28 @@ class Trainer:
         return self.model if model is None else model
 
     # ---- the hot step (train.py:310-325) ------------------------------------------------------------------------
+    def batch_tensors(self, data):
+        """-> (images, labels): the tensors of one loader batch the step uses.  ``labels`` is one tensor for the dict
+        batches of FGDataset; a method whose criterion takes several targets returns their tuple, which reaches the
+        criterion as ``criterion(outputs, *labels)``."""
+        return data['img'], data['label']
+
     def stage_inputs(self, data):
         """Host -> device copy of one batch on the copy stream (asynchronous for pinned host tensors) into a ring of three
         preallocated device buffers per batch shape — no allocator traffic in the step.  The compute stream waits for the
         copy in-stream, and the copy stream waits (device-side) until the step that last used the slot has finished, so the
-        copy of step n+1 overlaps the kernels of step n whenever the host runs ahead.  Returns (images, labels, slot)."""
-        img, lab = data['img'], data['label']
-        if img.is_cuda and lab.is_cuda:
+        copy of step n+1 overlaps the kernels of step n whenever the host runs ahead.  Returns (images, labels, slot);
+        labels is a tuple when ``batch_tensors`` gives one, each target with its own buffer in the slot."""
+        img, lab = self.batch_tensors(data)
+        labs = lab if isinstance(lab, tuple) else (lab,)
+        if img.is_cuda and all(t.is_cuda for t in labs):
             return img, lab, None
-        key = (tuple(img.shape), img.dtype, tuple(lab.shape), lab.dtype)
+        key = (tuple(img.shape), img.dtype) + tuple((tuple(t.shape), t.dtype) for t in labs)
         ring = self._in_ring.get(key)
         if ring is None:
             ring = self._in_ring[key] = dict(i=0, slots=[dict(img=torch.empty(img.shape, dtype=img.dtype, device=self.device),
-                                                               lab=torch.empty(lab.shape, dtype=lab.dtype, device=self.device),
+                                                               lab=[torch.empty(t.shape, dtype=t.dtype, device=self.device)
+                                                                    for t in labs],
                                                                free=None) for _ in range(3)])
         slot = ring['slots'][ring['i'] % 3]
         ring['i'] += 1
@@ -208,11 +222,12 @@ class Trainer:
             if slot['free'] is not None:
                 self.copy_stream.wait_event(slot['free'])
             slot['img'].copy_(img, non_blocking=True)
-            slot['lab'].copy_(lab, non_blocking=True)
+            for d, t in zip(slot['lab'], labs):
+                d.copy_(t, non_blocking=True)
             ev = torch.cuda.Event()
             ev.record()
         cur.wait_event(ev)
-        return slot['img'], slot['lab'], slot
+        return slot['img'], (tuple(slot['lab']) if isinstance(lab, tuple) else slot['lab'][0]), slot
 
     # ---- CUDA-graph replay of forward + loss + backward (+ gradient all-reduce) ----------------------------------------
     # A ResNet-50 step is ~1500 short launches issued from Python: the host, not the GPU, sets the step time.  With
@@ -243,26 +258,29 @@ class Trainer:
         return out
 
     def _graph_step_on_stream(self, images, labels, gs):
-        key = (tuple(images.shape), tuple(labels.shape))
+        targets = _as_tuple(labels)
+        key = (tuple(images.shape),) + tuple(tuple(t.shape) for t in targets)
         if self._graph is not None and self._graph['key'] != key:
             self._graph = None                                         # another batch shape (last batch of an epoch): eager
             self._graph_steps = -1
         if self._graph is None:
             outputs = self.forward_model(images, labels)
-            loss = self.criterion(outputs, labels)
+            loss = self.criterion(outputs, *targets)
             self.optimizer.zero_grad()
             loss.backward()
             self.allreduce.finish()
             if self._graph_steps >= 0:
                 self._graph_steps += 1
             if self._graph_steps == 3:
-                g = dict(key=key, img=torch.empty_like(images), lab=torch.empty_like(labels), graph=torch.cuda.CUDAGraph())
+                g = dict(key=key, img=torch.empty_like(images), lab=[torch.empty_like(t) for t in targets],
+                         graph=torch.cuda.CUDAGraph())
+                static = tuple(g['lab']) if isinstance(labels, tuple) else g['lab'][0]
                 gs.synchronize()
                 from . import _lib
                 n0 = _lib.launch_count()
                 with torch.cuda.graph(g['graph'], stream=gs):
-                    g['out'] = self.forward_model(g['img'], g['lab'])
-                    g['loss'] = self.criterion(g['out'], g['lab'])
+                    g['out'] = self.forward_model(g['img'], static)
+                    g['loss'] = self.criterion(g['out'], *g['lab'])
                     g['correct'] = getattr(self.criterion, 'last_correct', None)
                     self.optimizer.zero_grad()
                     g['loss'].backward()
@@ -272,7 +290,8 @@ class Trainer:
             return outputs, loss
         g = self._graph
         g['img'].copy_(images, non_blocking=True)
-        g['lab'].copy_(labels, non_blocking=True)
+        for d, t in zip(g['lab'], targets):
+            d.copy_(t, non_blocking=True)
         g['graph'].replay()
         if g['correct'] is not None:
             self.criterion.last_correct = g['correct']
@@ -287,7 +306,7 @@ class Trainer:
             outputs, loss = self._graph_step(images, labels)
         else:
             outputs = self.forward_model(images, labels)
-            loss = self.criterion(outputs, labels)
+            loss = self.criterion(outputs, *_as_tuple(labels))
             self.optimizer.zero_grad()
             loss.backward()
             self.allreduce.finish()
@@ -491,6 +510,30 @@ class _Plateau:
 
     def load_state_dict(self, sd):
         self.best, self.bad = sd['best'], sd['bad']
+
+
+class _Step:
+    """StepLR(step_size, gamma) over FusedSGD/FusedAdam param_groups, stepped once per epoch (Examples/DCL.py:89-90):
+    lr = initial_lr * gamma ** (epoch // step_size)."""
+
+    def __init__(self, opt, step_size, gamma=0.1):
+        self.opt, self.step_size, self.gamma, self.e = opt, step_size, gamma, 0
+        self._apply()
+
+    def _apply(self):
+        for g in self.opt.param_groups:
+            g['lr'] = g['initial_lr'] * self.gamma ** (self.e // self.step_size)
+
+    def step(self):
+        self.e += 1
+        self._apply()
+
+    def state_dict(self):
+        return dict(e=self.e)
+
+    def load_state_dict(self, sd):
+        self.e = sd['e']
+        self._apply()
 
 
 class _Cosine:

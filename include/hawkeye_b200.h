@@ -249,6 +249,30 @@ int hk_apinet_gate_bwd(const float* m, const float* mutual, const float* dout, f
 int hk_apinet_rank_loss(const float* logits, const long long* targets, double* loss_acc, float* dlogits, int R, int K,
                         float margin, float grad_scale, void* stream);
 
+/* ---- DCL: model/methods/DCL.py:31-45, model/loss/DCL_loss.py:16-21 ------------------------------------------------
+ * hk_dcl_head_fwd (DCL.py:33-39): trunk map x [N,C,H,W] (NCHW), Convmask weight w [C] and bias b [1] ->
+ *   pooled [N,C] = spatial mean of x, and mask [N,Q], Q = (H/2)(W/2), = tanh(avgpool2x2(w.x[n,:,p] + b)); an odd last row /
+ *   column is dropped, as AvgPool2d(2) drops it.  x is read once; the per-block shares of the 1x1 conv go to the workspace
+ *   (hk_dcl_head_workspace_bytes, serves both directions) and are added in a fixed order: no atomics, the same bits on every
+ *   run.  Default precision mode: pooled is rounded to tf32 on store (operand of the classifier MMA); mask is not.
+ * hk_dcl_head_bwd: dpooled [N,C], dmask [N,Q] -> dx [N,C,H,W] = dpooled/HW + w[c] dz[n,p] (dz: the tanh and 2x2-mean
+ *   adjoint, 0 on a dropped row / column), dw [C], db [1]; one read of x, one write of dx, fixed-order sums.  H*W <= 1024.
+ * hk_dcl_loss (DCLLoss): logits [R,ld] with the classifier in columns [0,K) and classifier_swap in [K,K+K2); labels /
+ *   labels_swap int64 [R]; mask / law [R,Q].  ADDS alpha CE(0:K, labels) + beta CE(K:K+K2, labels_swap) + gamma L1(mask, law)
+ *   (CE with label smoothing 0.1, means over rows / entries) to the fp64 accumulator loss_acc[0]; writes dlogits [R,ld] (pad
+ *   columns zero; rounded to tf32 in the default mode, like hk_softmax_ce_ls), dmask [R,Q] = gamma sign(mask - law)/(R Q)
+ *   (0 where equal) and correct (optional) = top-1 hits over columns [0,K), or with combine (cls_2xmul, K2 == 2K,
+ *   Examples/DCL.py:104-107) over z[k] + z[K+k] + z[2K+k].  A label outside its segment gets no one-hot term and never
+ *   counts as correct, as in hk_softmax_ce_ls.  Any R. */
+size_t hk_dcl_head_workspace_bytes(int N, int C, int H, int W);
+int hk_dcl_head_fwd(const float* x, const float* w, const float* b, float* pooled, float* mask, int N, int C, int H, int W,
+                    void* workspace, size_t workspace_bytes, void* stream);
+int hk_dcl_head_bwd(const float* x, const float* w, const float* mask, const float* dpooled, const float* dmask, float* dx,
+                    float* dw, float* db, int N, int C, int H, int W, void* workspace, size_t workspace_bytes, void* stream);
+int hk_dcl_loss(const float* logits, int ld, int K, int K2, const long long* labels, const long long* labels_swap,
+                const float* mask, const float* law, int R, int Q, float alpha, float beta, float gamma, int combine,
+                double* loss_acc, float* dlogits, float* dmask, int* correct, void* stream);
+
 /* ---- classifier nn.Linear (BCNN.py:42, CBCNN.py:26, MPNCOV.py:31) as skinny wgmma GEMMs ------------------- */
 size_t hk_linear_fwd_workspace_bytes(int B, int F, int N);
 int hk_linear_fwd(const float* x, const float* w, const float* bias, float* y, int B, int F, int N, void* workspace,
