@@ -434,9 +434,13 @@ int hk_bn_bwd(const float* x, const float* y, const float* dy, const float* gamm
   return hk_bn_bwd_ex(x, y, dy, gamma, nullptr, save_mean, save_invstd, dx, dres, dgamma, dbeta, P, C, relu, workspace,
                       workspace_bytes, stream_);
 }
-int hk_bn_bwd_ex(const float* x, const float* y, const float* dy, const float* gamma, const float* beta_for_mask,
-                 const float* save_mean, const float* save_invstd, float* dx, float* dres, float* dgamma, float* dbeta,
-                 long long P, int C, int relu, void* workspace, size_t workspace_bytes, void* stream_) {
+}  // extern "C"
+
+// The backward of both BatchNorm modes: the batch-statistics one (frozen = 0) and the one on constant statistics (frozen = 1),
+// whose dx lacks the two terms through the batch mean and variance: the apply kernel then runs with invP = 0.
+static int bn_bwd(const float* x, const float* y, const float* dy, const float* gamma, const float* beta_for_mask,
+                  const float* save_mean, const float* save_invstd, float* dx, float* dres, float* dgamma, float* dbeta,
+                  long long P, int C, int relu, void* workspace, size_t workspace_bytes, void* stream_, int frozen) {
   cudaStream_t st = (cudaStream_t)stream_;
   const float* beta = relu ? beta_for_mask : nullptr;
   HK_REQUIRE(x && dy && gamma && save_mean && save_invstd && dx && dgamma && dbeta && (!relu || y || beta), HK_ERR_ARG,
@@ -452,9 +456,25 @@ int hk_bn_bwd_ex(const float* x, const float* y, const float* dy, const float* g
   bn_bwd_finalize_kernel<<<(C + 31) / 32, 1024, 0, st>>>(part, nb, C, dgamma, dbeta);
   HK_LAUNCH_CHECK("bn_bwd_finalize_kernel");
   bn_bwd_apply_kernel<<<grid_1d((size_t)P * C4, 256), 256, 0, st>>>(x, y, dy, save_mean, save_invstd, gamma, dgamma, dbeta, beta,
-                                                                    dx, dres, (size_t)P * C4, C4, 1.f / (float)P, relu, precise() ? 0 : 1);
+                                                                    dx, dres, (size_t)P * C4, C4, frozen ? 0.f : 1.f / (float)P, relu,
+                                                                    precise() ? 0 : 1);
   HK_LAUNCH_CHECK("bn_bwd_apply_kernel");
   return 0;
+}
+
+extern "C" {
+
+int hk_bn_bwd_ex(const float* x, const float* y, const float* dy, const float* gamma, const float* beta_for_mask,
+                 const float* save_mean, const float* save_invstd, float* dx, float* dres, float* dgamma, float* dbeta,
+                 long long P, int C, int relu, void* workspace, size_t workspace_bytes, void* stream_) {
+  return bn_bwd(x, y, dy, gamma, beta_for_mask, save_mean, save_invstd, dx, dres, dgamma, dbeta, P, C, relu, workspace,
+                workspace_bytes, stream_, 0);
+}
+int hk_bn_bwd_frozen(const float* x, const float* y, const float* dy, const float* gamma, const float* beta_for_mask,
+                     const float* mean, const float* invstd, float* dx, float* dres, float* dgamma, float* dbeta, long long P,
+                     int C, int relu, void* workspace, size_t workspace_bytes, void* stream_) {
+  return bn_bwd(x, y, dy, gamma, beta_for_mask, mean, invstd, dx, dres, dgamma, dbeta, P, C, relu, workspace, workspace_bytes,
+                stream_, 1);
 }
 
 int hk_maxpool3x3s2_fwd(const float* x, float* y, unsigned char* argmax, int N, int H, int W, int C, void* stream) {

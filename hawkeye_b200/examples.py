@@ -1,5 +1,5 @@
 """Trainer subclasses of the hot-path methods with the reference's Examples/ surface:
-``python -m hawkeye_b200.examples {BCNN,CBCNN,MPN,PeerLearning,OSMENet,APINet,DCL} --config <yaml>`` replaces
+``python -m hawkeye_b200.examples {BCNN,CBCNN,MPN,PeerLearning,OSMENet,APINet,DCL,ProtoTreeNet} --config <yaml>`` replaces
 ``python Examples/<Method>.py --config <yaml>`` (same yaml files; one process per GPU under torchrun instead of nn.DataParallel).
 
 Only what the reference's Examples override is overridden here: which parameters train, with which learning rates, and
@@ -247,11 +247,114 @@ class DCLTrainer(Trainer):
         self.average_meters['acc'].update(accuracy(logit, labels, 1), labels.size(0))
 
 
+class ProtoTreeTrainer(Trainer):
+    """Examples/ProtoTreeNet.py with the schedule it actually runs:
+    - Parameter groups: the trunk except layer4.2 at 0.01 x lr, layer4.2, the neck and the prototypes at lr, and, with
+      model.disable_derivative_free_leaf_optim, the leaves at lr_pi.  Nothing is frozen: the reference's freeze() sets
+      ``param.require_grad`` (sic), so its 30-epoch freeze does nothing.
+    - Adam or AdamW with eps 1e-7 through engine.FusedAdam.  The groups' ``weight_decay_rate`` is read by no torch optimizer;
+      AdamW's global weight_decay (0.0 in the yaml) is the only decay, so a nonzero one, which needs decoupled decay, is
+      rejected, and so is SGD, whose prototype group runs without momentum.
+    - LinearLR warm-up into cosine annealing (SequentialLR), stepped once per epoch.
+    - Loss F.nll_loss(torch.log(pred), labels) (losses.ProtoTreeLoss).
+    - After every optimizer step, the derivative-free leaf update against the epoch-start snapshot of the leaves, and then
+      ``model.eval()``: only the first batch of an epoch runs the trunk's BatchNorm on batch statistics, every later one on
+      the running statistics, with gradients through them, until validate() restores train mode at the end of the epoch.
+      With gradient-trained leaves there is no update and no eval().  Under torchrun the ranks all-reduce the update sum
+      before applying it, so the update covers the global batch as under the reference's nn.DataParallel.
+    The reference's Example calls ``self.model(images, labels)``, which ProtoTreeNet.forward(x) does not accept; the model is
+    called with the images alone.  Under ``cuda_graph: true`` the eval-mode steps replay one captured graph and the
+    train-mode first batch of each epoch runs eagerly, so a graph never runs in the mode it was not captured in."""
+
+    def __init__(self, config=None, dataloaders=None):
+        super().__init__(config, dataloaders)
+        self.num_batches = len(self.dataloaders['train']) if 'train' in self.dataloaders else 1
+        self._theta0 = None
+
+    def get_criterion(self, config):
+        from .losses import ProtoTreeLoss
+        return ProtoTreeLoss()
+
+    def _dfo(self):
+        mc = self.config.model
+        return not (mc.disable_derivative_free_leaf_optim if 'disable_derivative_free_leaf_optim' in mc else False)
+
+    def param_groups(self):
+        m = self.get_model_module()
+        named = list(m.backbone.named_parameters())
+        groups = [([p for n, p in named if '7.2' not in n], 0.01), ([p for n, p in named if '7.2' in n], 1.0),
+                  (list(m.neck_conv.parameters()), 1.0), ([m.tree.prototype_layer.prototype_vectors], 1.0)]
+        if not self._dfo():
+            oc = self.config.train.optimizer
+            groups.append(([m.tree.leaf_params], oc.lr_pi / oc.lr))
+        return groups
+
+    def get_optimizer(self, config):
+        from . import engine
+        name = config.name if 'name' in config else 'Adam'
+        wd = config.weight_decay if 'weight_decay' in config else 0.0
+        if name not in ('Adam', 'AdamW'):
+            raise ValueError(f'ProtoTreeTrainer: optimizer {name!r} is not supported (Adam or AdamW)')
+        if name == 'AdamW' and wd != 0:
+            raise ValueError(f'ProtoTreeTrainer: AdamW with weight_decay={wd} needs decoupled weight decay, which FusedAdam '
+                             'does not have; use weight_decay: 0.0')
+        lrs = [config.lr * m for g, m in self.param_groups() if any(p.requires_grad for p in g)]
+        return engine.FusedAdam(self.flat, lr=config.lr, eps=1e-7, weight_decay=0.0, group_lrs=lrs)
+
+    def get_scheduler(self, config):
+        return _warmup_cosine(self.optimizer, config, self.total_epoch)
+
+    def on_start_epoch(self, config):
+        self._theta0 = self.get_model_module().tree.leaf_params.detach().clone()
+
+    def _graph_step_on_stream(self, images, labels, gs):
+        if self.model.training:
+            from .train import _as_tuple
+            outputs = self.forward_model(images, labels)
+            loss = self.criterion(outputs, *_as_tuple(labels))
+            self.optimizer.zero_grad()
+            loss.backward()
+            self.allreduce.finish()
+            return outputs, loss
+        outputs, loss = super()._graph_step_on_stream(images, labels, gs)
+        # the step's own outputs (the graph's static tensors after a replay): on the capturing step the criterion last saw
+        # the static tensors of a graph that has not run yet
+        self.criterion.last = (outputs[0].detach(), outputs[1]['pa_tensor'].dense, labels)
+        return outputs, loss
+
+    def after_optimizer_step(self):
+        """The leaf update, enqueued before the step releases its input slot (it reads the step's labels).  With several
+        ranks the update sums are all-reduced first: the update then covers the global batch, as under the reference's
+        nn.DataParallel, and every rank applies the same one, so the leaves stay identical across ranks."""
+        if not self._dfo():
+            return
+        import torch
+        from .ops_prototree import leaf_update
+        pred, pa, labels = self.criterion.last
+        if self._theta0 is None:
+            self.on_start_epoch(None)
+        reduce = None
+        if self.world > 1:
+            import torch.distributed as dist
+            reduce = dist.all_reduce
+        with torch.no_grad():
+            leaf_update(self.get_model_module().tree.leaf_params, self._theta0, pa, pred, labels, self.num_batches, reduce)
+        self.model.eval()
+
+    def batch_validate(self, data):
+        import torch
+        from .train import accuracy
+        images, labels = self.to_device(data['img']), self.to_device(data['label'])
+        with torch.no_grad():
+            pred, _ = self.model(images)
+        self.average_meters['acc'].update(accuracy(pred, labels, 1), images.size(0))
+
+
 TRAINERS = {'BCNN': BCNNTrainer, 'CBCNN': CBCNNTrainer, 'MPN': MPNTrainer, 'PeerLearning': PeerLearningTrainer,
             'OSMENet': OSMENetTrainer}
 # TRAINERS keeps the key set it has always had, so code that enumerates it sees no change; the command line dispatches
-# over every method, APINet and DCL included.
-ALL_TRAINERS = dict(TRAINERS, APINet=APINetTrainer, DCL=DCLTrainer)
+# over every method, APINet, DCL and ProtoTreeNet included.
+ALL_TRAINERS = dict(TRAINERS, APINet=APINetTrainer, DCL=DCLTrainer, ProtoTreeNet=ProtoTreeTrainer)
 
 
 def main(argv=None):

@@ -170,3 +170,18 @@ class DCLLoss(nn.Module):
                                         self.alpha, self.beta, self.gamma, K2 == 2 * K)
         self.last_correct = correct
         return loss
+
+
+class ProtoTreeLoss(nn.Module):
+    """Examples/ProtoTreeNet.py:109: F.nll_loss(torch.log(pred), labels) on the (pred, info) pair ProtoTreeNet returns, in one
+    hk_prototree_nll launch.  ``last_correct`` is the top-1 count on the device; ``last`` keeps (pred, pa, labels) of the call
+    for the derivative-free leaf update that follows the optimizer step (under CUDA-graph replay these are the graph's static
+    tensors, refreshed by every replay)."""
+
+    def forward(self, outputs, labels):
+        from .ops_prototree import NLLFn
+        pred, info = outputs
+        loss, correct = NLLFn.apply(pred, labels)
+        self.last_correct = correct
+        self.last = (pred.detach(), info['pa_tensor'].dense, labels)
+        return loss

@@ -6,3 +6,4 @@ from .cin import CIN, ChannelInteractionModule, CINClassifier  # noqa: F401
 from .osme import OSMENet, OSME, OSME_block  # noqa: F401
 from .apinet import APINet  # noqa: F401
 from .dcl import DCL  # noqa: F401
+from .prototree import ProtoTreeNet  # noqa: F401

@@ -28,7 +28,7 @@ class MPNCOV(nn.Module):
         if self.dr is not None:
             u = self._dr_unit
             ps = u.params()
-            save = ops.wants_grad(x, ps, self.training, 'MPNCOV.conv_dr_block')
+            save = ops.wants_grad(x, ps)
             x = ops_resnet.DRBlockFn.apply(x, u, save, self.training, *ps)
         x = ops.CovpoolLayer(x)
         if self.is_sqrt:

@@ -37,16 +37,10 @@ def _ws(nbytes, device):
     return torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=device)
 
 
-def wants_grad(x, params, training=True, what=''):
+def wants_grad(x, params):
     """Save-for-backward decision, taken from what requires grad at call time (grad mode is always off inside
-    Function.forward, so callers decide before ``apply``; freezing / unfreezing parameters after construction just works).
-    ``training=False`` means the op runs BatchNorm on its running statistics: gradients through that are not on the
-    reference's training path and have no kernel here, so asking for them is an error, never a silent None."""
-    want = torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params))
-    if want and not training:
-        raise _lib.HawkeyeLibError(f'{what}: backward through eval-mode BatchNorm is not implemented — call .train(), '
-                                   'or run under torch.no_grad() / with all inputs and parameters frozen')
-    return want
+    Function.forward, so callers decide before ``apply``; freezing / unfreezing parameters after construction just works)."""
+    return torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params))
 
 
 # ----------------------------------------------------------------------------------------------------------

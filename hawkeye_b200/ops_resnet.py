@@ -1,7 +1,9 @@
 """ResNet-50 v1.5 trunk (reference model/backbone/resnet.py:89-252) and the MPN-COV dimension-reduction block
 (MPNCOV.py:64-69) as explicit forward/backward pipelines over the C-ABI kernels.  NHWC fp32 inside.
 
-conv unit = convolution (wgmma GEMM / implicit GEMM) -> train-mode BatchNorm (+ residual) (+ ReLU).
+conv unit = convolution (wgmma GEMM / implicit GEMM) -> BatchNorm (+ residual) (+ ReLU).  BatchNorm runs on the batch
+statistics in train mode and on the running statistics in eval mode; both have a backward (eval mode: the statistics are
+constants, hk_bn_bwd_frozen).
 """
 import torch
 from torch.autograd import Function
@@ -75,7 +77,7 @@ class Unit:
             _ops.CAPTURE.append(('relu', y))
         if save:
             rec.update(c=c, y=y if self.relu else None, mean=mean, invstd=invstd, P=P, cout=cout, w=w, gamma=gamma, beta=beta,
-                       shape=(N, Ho, Wo), has_res=residual is not None)
+                       shape=(N, Ho, Wo), has_res=residual is not None, frozen=not training)
             return y, rec
         return y, None
 
@@ -93,8 +95,8 @@ class Unit:
         ws = _ws(_lib.query('hk_bn_workspace_bytes', P, cout), dev)
         # BN + ReLU without a residual: the mask is recomputed from x (hk_bn_bwd_ex), y is not read
         mask_beta = rec['beta'] if (self.relu and not rec['has_res']) else None
-        _lib.call('hk_bn_bwd_ex', rec['c'], rec['y'], dy, rec['gamma'], mask_beta, rec['mean'], rec['invstd'], dc, dres,
-                  dgamma, dbeta, P, cout, int(self.relu), ws, ws.numel(), s)
+        _lib.call('hk_bn_bwd_frozen' if rec['frozen'] else 'hk_bn_bwd_ex', rec['c'], rec['y'], dy, rec['gamma'], mask_beta,
+                  rec['mean'], rec['invstd'], dc, dres, dgamma, dbeta, P, cout, int(self.relu), ws, ws.numel(), s)
         w, xin = rec['w'], rec['xin']
         dx = None
         if self.kind == 'stem':
@@ -244,7 +246,7 @@ def resnet_trunk(x, trunk_module):
     plan = trunk_module._plan
     params = plan.params()
     training = trunk_module.training
-    save = _ops.wants_grad(x, params, training, 'ResNet trunk')
+    save = _ops.wants_grad(x, params)
     return ResNetTrunkFn.apply(x, plan, save, training, *params)
 
 

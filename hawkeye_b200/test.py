@@ -106,6 +106,8 @@ class Tester:
         if images.dtype == torch.uint8:                          # HWC uint8 batches: ToTensor + Normalize on the GPU
             images = normalize_u8(images)
         logits = self.model(images)
+        if isinstance(logits, tuple) and isinstance(logits[1], dict):   # ProtoTreeNet returns (pred, info)
+            logits = logits[0]
         if isinstance(logits, tuple):                            # PeerLearningNet returns both heads (PeerLearning.py:94-101)
             self.average_meters['acc'].update(max(accuracy(l, labels, 1) for l in logits), images.size(0))
         else:

@@ -311,6 +311,7 @@ class Trainer:
             loss.backward()
             self.allreduce.finish()
         self.optimizer.step()
+        self.after_optimizer_step()
         if slot is not None:                                          # the input slot may be overwritten from here on
             slot['free'] = torch.cuda.Event()
             slot['free'].record()
@@ -337,6 +338,10 @@ class Trainer:
         self.average_meters['loss'].update_async(buf, 0, 1.0, n_loss, ev)
         self.average_meters['acc'].update_async(buf, 1, 100.0 / n_acc, n_acc, ev)
         return loss
+
+    def after_optimizer_step(self):
+        """Work of the step that follows the optimizer, still before the step's input slot is released (it may read the
+        step's labels).  ProtoTree's leaf update goes here."""
 
     def forward_model(self, images, labels):
         """The model call of the training step (eager and graph-captured alike).  Methods whose forward takes the labels

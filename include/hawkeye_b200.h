@@ -171,6 +171,13 @@ int hk_bn_bwd(const float* x, const float* y, const float* dy, const float* gamm
 int hk_bn_bwd_ex(const float* x, const float* y, const float* dy, const float* gamma, const float* beta_for_mask,
                  const float* save_mean, const float* save_invstd, float* dx, float* dres, float* dgamma, float* dbeta,
                  long long P, int C, int relu, void* workspace, size_t workspace_bytes, void* stream);
+/* hk_bn_bwd_ex for BatchNorm on frozen (running) statistics, i.e. backward through an eval-mode BatchNorm: mean / invstd are
+ * the constants the forward used (running_mean, 1/sqrt(running_var + eps)); dx = dy'*gamma*invstd, dgamma = sum dy'*xhat,
+ * dbeta = sum dy' (dy' = dy under the ReLU mask), with the same fixed-order workspace reduction.  The running statistics are
+ * not arguments: nothing here touches them. */
+int hk_bn_bwd_frozen(const float* x, const float* y, const float* dy, const float* gamma, const float* beta_for_mask,
+                     const float* mean, const float* invstd, float* dx, float* dres, float* dgamma, float* dbeta, long long P,
+                     int C, int relu, void* workspace, size_t workspace_bytes, void* stream);
 /* nn.MaxPool2d(3, 2, 1) (resnet.py:180) */
 /* argmax (optional, [N,Ho,Wo,C] bytes): window position of the first maximum, consumed by the backward */
 int hk_maxpool3x3s2_fwd(const float* x, float* y, unsigned char* argmax, int N, int H, int W, int C, void* stream);
@@ -272,6 +279,51 @@ int hk_dcl_head_bwd(const float* x, const float* w, const float* mask, const flo
 int hk_dcl_loss(const float* logits, int ld, int K, int K2, const long long* labels, const long long* labels_swap,
                 const float* mask, const float* law, int R, int Q, float alpha, float beta, float gamma, int combine,
                 double* loss_acc, float* dlogits, float* dmask, int* correct, void* stream);
+
+/* ---- ProtoTree: model/methods/ProtoTree/{l2conv,prototree,branch,leaf}.py, Examples/ProtoTreeNet.py ----------------------
+ * Tree of height H (1 <= H <= 12): P = 2^H - 1 branches, L = 2^H leaves, 2^(H+1) - 1 nodes numbered in pre-order (root 0,
+ * left child i + 1, right child i + 1 + size of the left subtree, prototree.py:275-287).  Prototype row k belongs to the k-th
+ * branch in pre-order; leaf j is the j-th leaf from the left.  (The reference maps rows to branches through a set ordered by
+ * object hash, prototree.py:51, which changes from process to process; this order is the package's fixed choice.)
+ * hk_prototree_dist_fwd (l2conv.py:41-63, prototree.py:111-116): x [N,HW,D] (position-major), prototypes [P,D] ->
+ *   mind [N,P] = min over positions of sqrt(sum_d (z - p)^2 + 1e-14), argmin [N,P] int32 = the first minimising position in
+ *   row-major order (what max_pool2d of -d picks).  The squared distance is summed directly in fp32 in both precision modes:
+ *   the reference's |x|^2 + |p|^2 - 2 x.p cancels at the minimum, the one position that gets a gradient.  act = 1: x is the
+ *   neck's pre-activation, z = sigmoid(x) (ProtoTreeNet.py:24-27) is applied on load and stored to z [N,HW,D]; act = 0: z = x
+ *   and the z argument is unused.  N <= 65535.
+ * hk_prototree_dist_bwd: dmind [N,P] -> dx [N,HW,D] = sum over the prototypes j with argmin h of dmind (z - p_j) / mind, 0 at
+ *   every other position (act = 1: times z (1 - z), and rounded to tf32 in the default mode: it is the neck GEMMs' operand);
+ *   dprotos [P,D] = -sum_n dmind (z[argmin] - p) / mind.  z is the forward's z (act = 1) or x (act = 0).  Every sum has one
+ *   owner and a fixed order: the same bits on every run.  HW + P <= 51199 (the per-image grouping of the prototypes by
+ *   argmin position is kept in shared memory).
+ * hk_prototree_route_fwd (branch.py:22-57, leaf.py:30-67): mind [N,P], theta [L,K] -> sm [L,K] = softmax of each leaf,
+ *   ps [N,P] = exp(-mind) (by branch rank), pa [N, 2^(H+1) - 1] = probability of arriving at each node (pre-order; the left
+ *   child gets (1 - ps) pa, the right ps pa), pred [N,K] = sum_l pa[leaf l] sm[l].
+ * hk_prototree_route_bwd: dpred [N,K] -> dmind [N,P], bottom-up with u[leaf] = dpred . sm[leaf] and u = (1 - ps) u_l + ps u_r:
+ *   dmind = -ps pa (u_r - u_l), with no division by ps or 1 - ps; dtheta [L,K] (optional, K <= 12288) = the softmax adjoint of
+ *   sum_n pa[n, leaf] dpred[n].
+ * hk_prototree_nll (Examples/ProtoTreeNet.py:109, F.nll_loss(torch.log(pred), labels)): labels int64 [N] -> loss[0] = mean of
+ *   -log pred[n, y] over the V rows whose label is in [0, K), dpred [N,K] = -onehot(y) / (V pred[n, y]), correct (optional) =
+ *   top-1 hits on pred.  A row with a label outside [0, K) gets no term, no gradient, never counts and is not in V, as
+ *   F.nll_loss treats ignore_index rows (torch raises for other out-of-range labels; this does not).  V = 0 gives a NaN loss.
+ * hk_prototree_leaf_update_sum / hk_prototree_leaf_update_apply (Examples/ProtoTreeNet.py:116-132), the derivative-free leaf
+ *   update in two steps so that data-parallel ranks can all-reduce the sum in between:
+ *   update [L,K] = sum_b [y_b = k] pa[b, leaf] softmax(theta)[k] / pred[b, k] from the step's pa, pred and labels (ascending
+ *   b); then in place theta = relu(theta - theta0 / num_batches) + update, theta0 = the epoch-start snapshot. */
+int hk_prototree_dist_fwd(const float* x, const float* protos, float* z, float* mind, int* argmin, int N, int HW, int D,
+                          int P, int act, void* stream);
+int hk_prototree_dist_bwd(const float* z, const float* protos, const float* mind, const int* argmin, const float* dmind,
+                          float* dx, float* dprotos, int N, int HW, int D, int P, int act, void* stream);
+int hk_prototree_route_fwd(const float* mind, const float* theta, float* sm, float* ps, float* pa, float* pred, int N,
+                           int height, int K, void* stream);
+int hk_prototree_route_bwd(const float* ps, const float* pa, const float* sm, const float* dpred, float* dmind,
+                           float* dtheta, int N, int height, int K, void* stream);
+int hk_prototree_nll(const float* pred, const long long* labels, float* loss, float* dpred, int* correct, int N, int K,
+                     void* stream);
+int hk_prototree_leaf_update_sum(const float* theta, const float* pa, const float* pred, const long long* labels,
+                                 float* update, int N, int height, int K, void* stream);
+int hk_prototree_leaf_update_apply(float* theta, const float* theta0, const float* update, int height, int K,
+                                   float num_batches, void* stream);
 
 /* ---- classifier nn.Linear (BCNN.py:42, CBCNN.py:26, MPNCOV.py:31) as skinny wgmma GEMMs ------------------- */
 size_t hk_linear_fwd_workspace_bytes(int B, int F, int N);
