@@ -165,8 +165,7 @@ __device__ __forceinline__ float warp_softmax_at(const float* __restrict__ row, 
   const int lane = threadIdx.x & 31;
   float m = -INFINITY;
   for (int k = lane; k < K; k += 32) m = fmaxf(m, row[k]);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  m = warp_max(m);
   float s = 0.f;
   for (int k = lane; k < K; k += 32) s += expf(row[k] - m);
   s = warp_sum(s);
@@ -208,13 +207,8 @@ __global__ void apinet_rank_loss_kernel(const float* __restrict__ logits, const 
       }
     }
   }
-  if (lane == 0) red[warp] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double s = 0.0;
-    for (int w = 0; w < nw; ++w) s += red[w];
-    loss_acc[0] += s / (double)R;
-  }
+  const double s = block_sum(lane == 0 ? acc : 0.0, red);     // every lane of a warp holds its acc
+  if (threadIdx.x == 0) loss_acc[0] += s / (double)R;
 }
 
 static int check_p(float p, const long long* seed, const char* op) {

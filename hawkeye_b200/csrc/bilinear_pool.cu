@@ -137,12 +137,8 @@ __global__ void norm_from_s_kernel(const float* s, float* inv_norm, int C, int H
     const float v = s[(size_t)b * HW + p];
     acc = fmaf(v, v, acc);
   }
-  acc = warp_sum(acc);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
-  __syncthreads();
+  const float t = block_sum(acc, red);
   if (threadIdx.x == 0) {
-    float t = 0.f;
-    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) t += red[i];
     const float nrm = sqrtf(t * inv_hw + (float)C * (float)C * 1e-5f);
     inv_norm[b] = 1.f / fmaxf(nrm, 1e-12f);
   }
@@ -286,16 +282,6 @@ static int bilinear_bwd_impl(const float* x, const float* dy, float* dx, int B, 
 // =====================================================================================================
 namespace hk {
 
-__device__ __forceinline__ float block_sum_256(float v, float* red) {
-  v = warp_sum(v);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float t = 0.f;
-  for (int i = 0; i < (int)(blockDim.x >> 5); ++i) t += red[i];
-  __syncthreads();
-  return t;
-}
-
 // y = normalize(sign(pre) * sqrt(|pre| + 1e-10)); one block per image
 __global__ void cbp_finalize_fwd_kernel(const float* __restrict__ pre, float* __restrict__ y, int d, int round) {
   __shared__ float red[32];
@@ -305,7 +291,7 @@ __global__ void cbp_finalize_fwd_kernel(const float* __restrict__ pre, float* __
   // sign(0) = 0 in torch: those bins contribute 0, not eps
   float corr = 0.f;
   for (int k = threadIdx.x; k < d; k += blockDim.x) corr += (p[k] == 0.f) ? 1e-10f : 0.f;
-  const float n2 = block_sum_256(acc - corr, red);
+  const float n2 = block_sum(acc - corr, red);
   const float inv = 1.f / fmaxf(sqrtf(n2), 1e-12f);
   for (int k = threadIdx.x; k < d; k += blockDim.x) {
     const float v = p[k];
@@ -329,8 +315,8 @@ __global__ void cbp_finalize_bwd_kernel(const float* __restrict__ pre, const flo
       dot += (v > 0.f ? r : -r) * g[k];
     }
   }
-  n2 = block_sum_256(n2, red);
-  dot = block_sum_256(dot, red);
+  n2 = block_sum(n2, red);
+  dot = block_sum(dot, red);
   const float n = fmaxf(sqrtf(n2), 1e-12f);
   const float c = dot / n;                     // <y, dy>
   for (int k = threadIdx.x; k < d; k += blockDim.x) {

@@ -8,53 +8,27 @@
 
 namespace hk {
 
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-
 // w[r][:] = softmax(-g[r][:])   (one block per row)
 __global__ void softmax_neg_rows_fwd_kernel(const float* __restrict__ g, float* __restrict__ w, int cols) {
   __shared__ float red[32];
-  __shared__ float bc;
   const float* gr = g + (size_t)blockIdx.x * cols;
   float* wr = w + (size_t)blockIdx.x * cols;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
   float m = -INFINITY;
   for (int j = threadIdx.x; j < cols; j += blockDim.x) m = fmaxf(m, -gr[j]);
-  m = warp_max(m);
-  if (lane == 0) red[warp] = m;
-  __syncthreads();
-  if (threadIdx.x == 0) { float t = red[0]; for (int i = 1; i < nw; ++i) t = fmaxf(t, red[i]); bc = t; }
-  __syncthreads();
-  m = bc;
+  m = block_max(m, red);
   float s = 0.f;
   for (int j = threadIdx.x; j < cols; j += blockDim.x) s += expf(-gr[j] - m);
-  s = warp_sum(s);
-  __syncthreads();
-  if (lane == 0) red[warp] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) { float t = 0.f; for (int i = 0; i < nw; ++i) t += red[i]; bc = t; }
-  __syncthreads();
-  const float inv = 1.f / bc;
+  const float inv = 1.f / block_sum(s, red);
   for (int j = threadIdx.x; j < cols; j += blockDim.x) wr[j] = expf(-gr[j] - m) * inv;
 }
 // dg = -(w * (dw - sum_j w_j dw_j))
 __global__ void softmax_neg_rows_bwd_kernel(const float* __restrict__ w, const float* __restrict__ dw,
                                             float* __restrict__ dg, int cols) {
   __shared__ float red[32];
-  __shared__ float bc;
   const size_t off = (size_t)blockIdx.x * cols;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
   float s = 0.f;
   for (int j = threadIdx.x; j < cols; j += blockDim.x) s = fmaf(w[off + j], dw[off + j], s);
-  s = warp_sum(s);
-  if (lane == 0) red[warp] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) { float t = 0.f; for (int i = 0; i < nw; ++i) t += red[i]; bc = t; }
-  __syncthreads();
-  const float dot = bc;
+  const float dot = block_sum(s, red);
   for (int j = threadIdx.x; j < cols; j += blockDim.x) dg[off + j] = -w[off + j] * (dw[off + j] - dot);
 }
 
@@ -89,14 +63,8 @@ __global__ void cci_weight_bwd_kernel(const float* __restrict__ w_sci, const flo
     d_sci[(size_t)b * per + e] = sb * db_ - wpb * sp * dp;
     acc = fmaf(-sb * db_, p, acc);
   }
-  acc = warp_sum(acc);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float t = 0.f;
-    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) t += red[i];
-    atomicAdd(d_weight + b, t);
-  }
+  acc = block_sum(acc, red);
+  if (threadIdx.x == 0) atomicAdd(d_weight + b, acc);
 }
 
 // y[r] = mean over the first `cols` entries of x[r][0..ld)          (AdaptiveAvgPool1d(1), CIN.py:71)

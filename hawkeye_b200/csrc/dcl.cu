@@ -129,34 +129,6 @@ __global__ void dcl_head_bwd_finish_kernel(const float* __restrict__ dwpart, con
   }
 }
 
-// Label-smoothed cross-entropy of one row segment z[0, K) with target y (eps = smoothing), by one warp: returns the row's
-// loss term and writes (softmax - target distribution) * scale to g (rounded to tf32 when `round`).  A target outside
-// [0, K) gets no one-hot term, as in hk_softmax_ce_ls.
-__device__ float warp_ce_ls(const float* __restrict__ z, int K, long long y, float eps, float scale, float* __restrict__ g,
-                            int round) {
-  const int lane = threadIdx.x & 31;
-  float m = -INFINITY;
-  for (int k = lane; k < K; k += 32) m = fmaxf(m, z[k]);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-  float se = 0.f, sl = 0.f;
-  for (int k = lane; k < K; k += 32) {
-    se += expf(z[k] - m);
-    sl += z[k];
-  }
-  se = warp_sum(se);
-  sl = warp_sum(sl);
-  const float lse = m + logf(se);
-  const bool valid = y >= 0 && y < K;
-  const float zy = valid ? z[y] : lse;
-  for (int k = lane; k < K; k += 32) {
-    const float t = (k == y ? (1.f - eps) : 0.f) + eps / (float)K;
-    const float v = (expf(z[k] - lse) - t) * scale;
-    g[k] = round ? tf32_round(v) : v;
-  }
-  return (1.f - eps) * (lse - zy) + eps * (lse - sl / (float)K);
-}
-
 // One block; warp w takes rows w, w + 32, ...  Per row: CE_ls(z[0, K), y), CE_ls(z[K, K + K2), y_swap), the gradient of
 // both (pad columns [K + K2, ld) zeroed), the L1 term over the Q mask entries with d|m - l| = sign(m - l) (0 at equality),
 // and the top-1 hit over z[0, K) or, with `combine` (cls_2xmul), over z[k] + z[K + k] + z[2K + k].  The per-warp fp64 sums
@@ -166,7 +138,7 @@ __global__ void dcl_loss_kernel(const float* __restrict__ logits, int ld, int K,
                                 const float* __restrict__ law, int R, int Q, float alpha, float beta, float gamma, int combine,
                                 double* __restrict__ loss_acc, float* __restrict__ dlogits, float* __restrict__ dmask,
                                 int* __restrict__ correct, int round) {
-  __shared__ double s_ce[32], s_sw[32], s_l1[32];
+  __shared__ double red[32];
   __shared__ int s_corr[32];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
   const float eps = 0.1f;
@@ -186,12 +158,7 @@ __global__ void dcl_loss_kernel(const float* __restrict__ logits, int ld, int K,
       const float v = combine ? (z[k] + z[K + k]) + z[2 * K + k] : z[k];
       if (v > best) { best = v; am = k; }
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-      const int oa = __shfl_xor_sync(0xffffffffu, am, o);
-      if (ob > best || (ob == best && oa < am)) { best = ob; am = oa; }
-    }
+    warp_argmax(best, am);
     const float* mr = mask + (size_t)r * Q;
     const float* lr = law + (size_t)r * Q;
     float a = 0.f;
@@ -208,12 +175,10 @@ __global__ void dcl_loss_kernel(const float* __restrict__ logits, int ld, int K,
       hits += (am == y);
     }
   }
-  if (lane == 0) { s_ce[warp] = ce; s_sw[warp] = sw; s_l1[warp] = l1; s_corr[warp] = hits; }
-  __syncthreads();
+  // ce, sw, l1, hits are 0 outside lane 0
+  const double a = block_sum(ce, red), b = block_sum(sw, red), c = block_sum(l1, red);
+  const int h = block_sum(hits, s_corr);
   if (threadIdx.x == 0) {
-    double a = 0.0, b = 0.0, c = 0.0;
-    int h = 0;
-    for (int i = 0; i < nw; ++i) { a += s_ce[i]; b += s_sw[i]; c += s_l1[i]; h += s_corr[i]; }
     loss_acc[0] += (double)alpha * (a / R) + (double)beta * (b / R) + (double)gamma * (c / ((double)R * Q));
     if (correct) correct[0] = h;
   }

@@ -10,7 +10,8 @@
 namespace hk {
 
 // One block; warps stride over rows.  loss = mean_b [ (1-eps) * -logp[y] + eps/K * sum_k -logp[k] ]
-// dlogits = (softmax - ((1-eps) onehot + eps/K)) * grad_scale / B
+// dlogits = (softmax - ((1-eps) onehot + eps/K)) * grad_scale / B, rounded in tf32 mode: the operand of the classifier
+// dgrad / wgrad MMAs.
 __global__ void softmax_ce_ls_kernel(const float* __restrict__ logits, const long long* __restrict__ labels,
                                      float* __restrict__ loss, float* __restrict__ dlogits, int* __restrict__ correct,
                                      int B, int K, float eps, float grad_scale, int round) {
@@ -21,48 +22,24 @@ __global__ void softmax_ce_ls_kernel(const float* __restrict__ logits, const lon
   int csum = 0;
   for (int b = warp; b < B; b += nw) {
     const float* row = logits + (size_t)b * K;
-    float m = -INFINITY;
+    const long long y = labels[b];
+    const float l = warp_ce_ls(row, K, y, eps, grad_scale / (float)B, dlogits ? dlogits + (size_t)b * K : nullptr, round);
+    // top-1: the first maximum of the row
+    float best = -INFINITY;
     int am = 0;
     for (int k = lane; k < K; k += 32) {
       const float v = row[k];
-      if (v > m) { m = v; am = k; }
+      if (v > best) { best = v; am = k; }
     }
-    for (int o = 16; o > 0; o >>= 1) {
-      const float om = __shfl_xor_sync(0xffffffffu, m, o);
-      const int oa = __shfl_xor_sync(0xffffffffu, am, o);
-      if (om > m || (om == m && oa < am)) { m = om; am = oa; }
-    }
-    float se = 0.f, sl = 0.f;
-    for (int k = lane; k < K; k += 32) {
-      se += expf(row[k] - m);
-      sl += row[k];
-    }
-    se = warp_sum(se);
-    sl = warp_sum(sl);
-    const float lse = m + logf(se);
-    const int y = (int)labels[b];
-    const float nll_y = lse - row[y];
-    const float nll_mean = lse - sl / (float)K;
+    warp_argmax(best, am);
     if (lane == 0) {
-      lsum += (1.f - eps) * nll_y + eps * nll_mean;
+      lsum += l;
       csum += (am == y);
     }
-    if (dlogits) {
-      const float sc = grad_scale / (float)B;
-      for (int k = lane; k < K; k += 32) {
-        const float p = expf(row[k] - lse);
-        const float t = (k == y ? (1.f - eps) : 0.f) + eps / (float)K;
-        const float g = (p - t) * sc;
-        dlogits[(size_t)b * K + k] = round ? tf32_round(g) : g;     // operand of the classifier dgrad / wgrad MMAs
-      }
-    }
   }
-  if (lane == 0) { s_loss[warp] = lsum; s_corr[warp] = csum; }
-  __syncthreads();
+  const float t = block_sum(lsum, s_loss);     // lsum, csum are 0 outside lane 0
+  const int c = block_sum(csum, s_corr);
   if (threadIdx.x == 0) {
-    float t = 0.f;
-    int c = 0;
-    for (int i = 0; i < nw; ++i) { t += s_loss[i]; c += s_corr[i]; }
     loss[0] = t / (float)B;
     if (correct) correct[0] = c;
   }

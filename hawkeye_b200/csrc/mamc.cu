@@ -13,23 +13,13 @@
 
 namespace hk {
 
-__device__ __forceinline__ float block_sum_f(float v, float* red) {
-  v = warp_sum(v);
-  __syncthreads();                                   // red[] free again
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float t = 0.f;
-  for (int i = 0; i < (int)(blockDim.x >> 5); ++i) t += red[i];
-  return t;
-}
-
 // y = x / max(||x||_2, 1e-12) per row (F.normalize); inv[r] = 1 / max(||x_r||, 1e-12)
 __global__ void l2norm_rows_fwd_kernel(const float* __restrict__ x, float* __restrict__ y, float* __restrict__ inv, int D) {
   __shared__ float red[32];
   const float* xr = x + (size_t)blockIdx.x * D;
   float s = 0.f;
   for (int i = threadIdx.x; i < D; i += blockDim.x) s = fmaf(xr[i], xr[i], s);
-  s = block_sum_f(s, red);
+  s = block_sum(s, red);
   const float iv = 1.f / fmaxf(sqrtf(s), 1e-12f);
   for (int i = threadIdx.x; i < D; i += blockDim.x) y[(size_t)blockIdx.x * D + i] = xr[i] * iv;
   if (threadIdx.x == 0) inv[blockIdx.x] = iv;
@@ -41,7 +31,7 @@ __global__ void l2norm_rows_bwd_kernel(const float* __restrict__ y, const float*
   const size_t o = (size_t)blockIdx.x * D;
   float s = 0.f;
   for (int i = threadIdx.x; i < D; i += blockDim.x) s = fmaf(y[o + i], dy[o + i], s);
-  s = block_sum_f(s, red);
+  s = block_sum(s, red);
   const float iv = inv[blockIdx.x];
   for (int i = threadIdx.x; i < D; i += blockDim.x) dx[o + i] = iv * (dy[o + i] - y[o + i] * s);
 }
@@ -65,8 +55,8 @@ __global__ void npair_fwd_bwd_kernel(const float* __restrict__ prod, const int* 
       if (t == 3) e3 += e;
     }
   }
-  const float EA = block_sum_f(e123, red);
-  const float EB = block_sum_f(e3, red);      // NEG of terms B and C is the same set
+  const float EA = block_sum(e123, red);
+  const float EB = block_sum(e3, red);      // NEG of terms B and C is the same set
   // second pass: loss and the POS-side weights  w = E e^{-p} / (1 + E e^{-p}),  W = sum_POS e^{-p} / (1 + E e^{-p})
   float loss = 0.f, WA = 0.f, WB = 0.f, WC = 0.f;
   for (int j = threadIdx.x; j < n; j += blockDim.x) {
@@ -79,10 +69,10 @@ __global__ void npair_fwd_bwd_kernel(const float* __restrict__ prod, const int* 
     const float r = em / den;
     if (t == 0) WA += r; else if (t == 1) WB += r; else WC += r;
   }
-  loss = block_sum_f(loss, red);
-  WA = block_sum_f(WA, red);
-  WB = block_sum_f(WB, red);
-  WC = block_sum_f(WC, red);
+  loss = block_sum(loss, red);
+  WA = block_sum(WA, red);
+  WB = block_sum(WB, red);
+  WC = block_sum(WC, red);
   const float invn = 1.f / (float)n;
   for (int j = threadIdx.x; j < n; j += blockDim.x) {
     const int t = (part[j] == pi ? 0 : 2) + (cls[j] == ci ? 0 : 1);

@@ -43,20 +43,11 @@ __global__ void center_rows_kernel(const float* __restrict__ x, float* __restric
 __global__ void trace_normalize_kernel(const float* __restrict__ x, float* __restrict__ normA, float* __restrict__ Ahi,
                                        float* __restrict__ Alo, int n) {
   __shared__ float red[32];
-  __shared__ float tr;
   const float* xb = x + (size_t)blockIdx.x * n * n;
   float s = 0.f;
   for (int i = threadIdx.x; i < n; i += blockDim.x) s += xb[(size_t)i * n + i];
-  s = warp_sum(s);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float t = 0.f;
-    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) t += red[i];
-    tr = t;
-    normA[blockIdx.x] = t;
-  }
-  __syncthreads();
+  const float tr = block_sum(s, red);
+  if (threadIdx.x == 0) normA[blockIdx.x] = tr;
   const float inv = 1.f / tr;
   for (int i = threadIdx.x; i < n * n; i += blockDim.x) {
     const float v = xb[i] * inv;
@@ -100,13 +91,7 @@ __global__ void sqrtm_bwd_tail_kernel(const float* __restrict__ tD_hi, const flo
     gaux = fmaf(d, x[off + i], gaux);
     gy = fmaf(g[off + i], y[off + i], gy);
   }
-  gaux = warp_sum(gaux);
-  gy = warp_sum(gy);
-  __shared__ float red2[32];
-  if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5] = gaux; red2[threadIdx.x >> 5] = gy; }
-  __syncthreads();
-  float ga = 0.f, gyy = 0.f;
-  for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { ga += red[i]; gyy += red2[i]; }
+  const float ga = block_sum(gaux, red), gyy = block_sum(gy, red);
   const float na = normA[blockIdx.x];
   const float coef = gyy / (2.f * na) - ga / (na * na);
   for (int i = threadIdx.x; i < n * n; i += blockDim.x) {

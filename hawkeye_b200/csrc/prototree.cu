@@ -33,31 +33,14 @@ __device__ __forceinline__ int pt_branch(int d, int q, int H) {
   return r;
 }
 
-// Block reduction in a fixed order (warp xor tree, then the warp partials in warp order): the same bits on every run.
-template <bool MAX>
-__device__ float block_reduce(float v, float* red) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float u = __shfl_xor_sync(0xffffffffu, v, o);
-    v = MAX ? fmaxf(v, u) : v + u;
-  }
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  float t = red[0];
-  for (int i = 1; i < nw; ++i) t = MAX ? fmaxf(t, red[i]) : t + red[i];
-  return t;
-}
-
 // (max, sum of exp(theta - max)) of one leaf's parameters: softmax(theta - max(theta)) as leaf.py:67 computes it
 __device__ void leaf_softmax_stats(const float* __restrict__ th, int K, float* red, float& m, float& s) {
   float v = -INFINITY;
   for (int k = threadIdx.x; k < K; k += blockDim.x) v = fmaxf(v, th[k]);
-  m = block_reduce<true>(v, red);
+  m = block_max(v, red);
   float e = 0.f;
   for (int k = threadIdx.x; k < K; k += blockDim.x) e += expf(th[k] - m);
-  s = block_reduce<false>(e, red);
+  s = block_sum(e, red);
 }
 
 // Block (prototype tile, image n).  For each tile of PT_TH positions, thread (tx, ty) of a 16 x 16 grid accumulates the
@@ -272,7 +255,7 @@ __global__ void pt_dtheta_kernel(const float* __restrict__ pa, const float* __re
     G[k] = acc;
     dot = fmaf(acc, s[k], dot);
   }
-  dot = block_reduce<false>(dot, red);
+  dot = block_sum(dot, red);
   for (int k = threadIdx.x; k < K; k += blockDim.x) dtheta[(size_t)l * K + k] = s[k] * (G[k] - dot);
 }
 
@@ -282,16 +265,11 @@ __global__ void pt_dtheta_kernel(const float* __restrict__ pa, const float* __re
 __global__ void pt_nll_kernel(const float* __restrict__ pred, const long long* __restrict__ labels, int R, int K,
                               float* __restrict__ loss, float* __restrict__ dpred, int* __restrict__ correct) {
   __shared__ double s_loss[32];
-  __shared__ int s_hits[32], s_valid[32];
+  __shared__ int s_int[32];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
   int v = 0;
   for (int r = threadIdx.x; r < R; r += blockDim.x) v += labels[r] >= 0 && labels[r] < K;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  if (lane == 0) s_valid[warp] = v;
-  __syncthreads();
-  int V = 0;
-  for (int i = 0; i < nw; ++i) V += s_valid[i];
+  const int V = block_sum(v, s_int);
   double acc = 0.0;
   int hits = 0;
   for (int r = warp; r < R; r += nw) {
@@ -306,23 +284,15 @@ __global__ void pt_nll_kernel(const float* __restrict__ pred, const long long* _
       if (v > best) { best = v; am = k; }
       dpred[(size_t)r * K + k] = (valid && k == y) ? -1.f / ((float)V * py) : 0.f;
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-      const int oa = __shfl_xor_sync(0xffffffffu, am, o);
-      if (ob > best || (ob == best && oa < am)) { best = ob; am = oa; }
-    }
+    warp_argmax(best, am);
     if (lane == 0 && valid) {
       acc -= (double)logf(py);
       hits += (am == y);
     }
   }
-  if (lane == 0) { s_loss[warp] = acc; s_hits[warp] = hits; }
-  __syncthreads();
+  const double t = block_sum(acc, s_loss);     // acc, hits are 0 outside lane 0
+  const int h = block_sum(hits, s_int);
   if (threadIdx.x == 0) {
-    double t = 0.0;
-    int h = 0;
-    for (int i = 0; i < nw; ++i) { t += s_loss[i]; h += s_hits[i]; }
     loss[0] = (float)(t / V);                   // no valid row: 0 / 0, NaN, as F.nll_loss gives
     if (correct) correct[0] = h;
   }

@@ -334,6 +334,7 @@ int hk_linear_wgrad(const float* dy, const float* x, float* dw, float* db, int B
 
 /* ---- nn.CrossEntropyLoss(label_smoothing) fwd+bwd (train.py:211-212, :315-319); labels int64 ----------------
  * loss[0] = mean loss; dlogits (optional) = dloss/dlogits * grad_scale; correct (optional) = #argmax==label.
+ * A label outside [0, K) gets no one-hot term (its row adds eps (lse - mean(z)) and gets softmax - eps/K) and never counts.
  * In the default precision mode dlogits is rounded to tf32 on store (it is the operand of the classifier's dgrad / wgrad
  * MMAs, which would otherwise truncate it); hk_set_precise(1) stores it unrounded. */
 int hk_softmax_ce_ls(const float* logits, const long long* labels, float* loss, float* dlogits, int* correct, int B,

@@ -36,21 +36,37 @@ def test_linear(B, Fdim, N):
 
 @pytest.mark.parametrize('precise', [0, 1])
 def test_cross_entropy_ls(precise):
-    """default mode: dlogits are rounded to tf32 on store (operand of the classifier MMAs) -> 2^-12 rms; precise: fp32"""
+    """default mode: dlogits are rounded to tf32 on store (operand of the classifier MMAs) -> 2^-12 rms; precise: fp32.
+    The top-1 count is checked against the fp64 arg-max.  A second batch labels row 0 with K and row 5 with -1: such a row
+    adds eps (lse - mean(z)) to the loss, gets softmax - eps/K and never counts (the rule of include/hawkeye_b200.h)."""
     from hawkeye_b200 import ops, _lib
-    logits = detgen.det((32, 200), 1)
-    labels = detgen.det_labels(32, 200, 2)
-    lg = logits.cuda().requires_grad_(True)
-    _lib.set_precise(precise)
-    try:
-        loss = ops.CrossEntropyLS(0.1)(lg, labels.cuda())
-        (g,) = torch.autograd.grad(loss, lg)
-    finally:
-        _lib.set_precise(0)
-    ld = logits.double().requires_grad_(True)
-    ref = F.cross_entropy(ld, labels, label_smoothing=0.1)
-    (rg,) = torch.autograd.grad(ref, ld)
-    assert abs(loss.item() - ref.item()) < 1e-5 and rel_l2(g.cpu(), rg) < (1e-5 if precise else 3e-4)
+    B, K, eps = 32, 200, 0.1
+    logits = detgen.det((B, K), 1)
+    labels = detgen.det_labels(B, K, 2)
+    out_of_range = labels.clone()
+    out_of_range[0], out_of_range[5] = K, -1     # z[y] of these rows would still lie inside the logits tensor
+    for y in (labels, out_of_range):
+        lg = logits.cuda().requires_grad_(True)
+        ce = ops.CrossEntropyLS(eps)
+        _lib.set_precise(precise)
+        try:
+            loss = ce(lg, y.cuda())
+            (g,) = torch.autograd.grad(loss, lg)
+        finally:
+            _lib.set_precise(0)
+        ld = logits.double().requires_grad_(True)
+        valid = (y >= 0) & (y < K)
+        if valid.all():
+            ref = F.cross_entropy(ld, y, label_smoothing=eps)
+            (rg,) = torch.autograd.grad(ref, ld)
+        else:
+            z, yc = ld.detach(), y.clamp(0, K - 1)
+            lse = torch.logsumexp(z, 1)
+            nll_y = torch.where(valid, lse - z.gather(1, yc[:, None])[:, 0], 0.0)
+            ref = ((1 - eps) * nll_y + eps * (lse - z.mean(1))).mean()
+            rg = (torch.softmax(z, 1) - (1 - eps) * F.one_hot(yc, K) * valid[:, None] - eps / K) / B
+        assert abs(loss.item() - ref.item()) < 1e-5 and rel_l2(g.cpu(), rg) < (1e-5 if precise else 3e-4)
+        assert ce.last_correct.item() == ((logits.double().argmax(1) == y) & valid).sum().item()
 
 
 def test_sgd_and_adam():
