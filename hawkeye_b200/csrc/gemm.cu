@@ -489,10 +489,35 @@ static size_t operand_extent(long long rows, long long cols, long long ld, long 
   return (size_t)((long long)(batch - 1) * (stride > 0 ? stride : 0) + (rows - 1) * ld + cols);
 }
 
-// 3xTF32: A.B ~= Ah.Bh + Al.Bh + Ah.Bl with (hi, lo) = tf32 halves of the operands, chained through the epilogue's raw
-// addend E so the caller's epilogue (alpha, diag, D, ReLU, transposed store ...) is applied once, to the full sum.
+// What the TMA-fed kernel needs of an operand, checked before any scratch allocation, driver call or launch so that a
+// rejected call launches nothing in either precision mode: a 16-byte aligned base, and a row pitch and (used) batch
+// stride that are whole 16-byte units.
+static int check_operand(const char* what, char name, const float* P, long long ld, long long stride, int batch) {
+  HK_REQUIRE(P, HK_ERR_ARG, "%s: null operand %c", what, name);
+  HK_REQUIRE(aligned16(P), HK_ERR_ALIGN, "%s: operand %c is not 16-byte aligned", what, name);
+  HK_REQUIRE(ld > 0 && ld % 4 == 0, HK_ERR_ALIGN, "%s: ld%c=%lld is not a positive multiple of 4 floats (16-byte stride)",
+             what, name, ld);
+  HK_REQUIRE(batch == 1 || stride % 4 == 0, HK_ERR_ALIGN,
+             "%s: batch stride of %c (%lld) is not a multiple of 4 floats (16-byte stride)", what, name, stride);
+  return 0;
+}
+
+static int check_gemm_args(const char* what, const float* A, long long lda, long long strideA, const float* B,
+                           long long ldb, long long strideB, const GemmEpi& epi, int M, int N, int K, int batch) {
+  HK_REQUIRE(epi.C, HK_ERR_ARG, "%s: null output", what);
+  HK_REQUIRE(M > 0 && N > 0 && K > 0 && batch > 0, HK_ERR_ARG, "%s: bad shape M=%d N=%d K=%d batch=%d", what, M, N, K,
+             batch);
+  HK_REQUIRE(batch <= 65535, HK_ERR_UNSUPPORTED, "%s: batch %d > 65535", what, batch);
+  if (int r = check_operand(what, 'a', A, lda, strideA, batch)) return r;
+  return check_operand(what, 'b', B, ldb, strideB, batch);
+}
+
+// 3xTF32: A.B ~= Ah.Bh + Al.Bh + Ah.Bl with (hi, lo) = tf32 halves of the operands, split into scratch and multiplied
+// by ONE launch of the pair kernel, so the caller's epilogue (alpha, diag, D, ReLU, transposed store ...) is applied
+// once, to the full sum.
 int gemm_tf32_3x(const float* A, int a_mn, long long lda, long long strideA, const float* B, int b_mn, long long ldb,
                         long long strideB, const GemmEpi& epi, int M, int N, int K, int batch, cudaStream_t st) {
+  if (int r = check_gemm_args("gemm (3xTF32)", A, lda, strideA, B, ldb, strideB, epi, M, N, K, batch)) return r;
   const size_t nA = operand_extent(a_mn ? K : M, a_mn ? M : K, lda, strideA, batch);
   const bool same = (A == B && a_mn == b_mn && lda == ldb && strideA == strideB && M == N);
   const size_t nB = same ? 0 : operand_extent(b_mn ? K : N, b_mn ? N : K, ldb, strideB, batch);
@@ -511,19 +536,13 @@ int gemm_tf32_3x(const float* A, int a_mn, long long lda, long long strideA, con
 
 int gemm_tf32(const float* A, int a_mn, long long lda, long long strideA, const float* B, int b_mn, long long ldb,
               long long strideB, const GemmEpi& epi, int M, int N, int K, int batch, cudaStream_t stream) {
-  if (precise()) {
-    HK_REQUIRE(A && B && epi.C, HK_ERR_ARG, "gemm: null pointer");
-    HK_REQUIRE(M > 0 && N > 0 && K > 0 && batch > 0, HK_ERR_ARG, "gemm: bad shape M=%d N=%d K=%d batch=%d", M, N, K, batch);
-    return gemm_tf32_3x(A, a_mn, lda, strideA, B, b_mn, ldb, strideB, epi, M, N, K, batch, stream);
-  }
+  if (precise()) return gemm_tf32_3x(A, a_mn, lda, strideA, B, b_mn, ldb, strideB, epi, M, N, K, batch, stream);
   return gemm_tf32_1x(A, a_mn, lda, strideA, B, b_mn, ldb, strideB, epi, M, N, K, batch, stream);
 }
 
 int gemm_tf32_1x(const float* A, int a_mn, long long lda, long long strideA, const float* B, int b_mn, long long ldb,
                  long long strideB, const GemmEpi& epi, int M, int N, int K, int batch, cudaStream_t stream) {
-  HK_REQUIRE(A && B && epi.C, HK_ERR_ARG, "gemm: null pointer");
-  HK_REQUIRE(M > 0 && N > 0 && K > 0 && batch > 0, HK_ERR_ARG, "gemm: bad shape M=%d N=%d K=%d batch=%d", M, N, K, batch);
-  HK_REQUIRE(batch <= 65535, HK_ERR_UNSUPPORTED, "gemm: batch %d > 65535", batch);
+  if (int r = check_gemm_args("gemm", A, lda, strideA, B, ldb, strideB, epi, M, N, K, batch)) return r;
   CUtensorMap tmA, tmB;
   int shareA, shareB, r;
   const int BN = N <= 64 ? 64 : 128;   // 64 accumulator registers per thread at most
@@ -537,9 +556,9 @@ int gemm_tf32_1x(const float* A, int a_mn, long long lda, long long strideA, con
 int gemm_tf32_pair(const float* Ah, const float* Al, int a_mn, long long lda, long long strideA, const float* Bh,
                    const float* Bl, int b_mn, long long ldb, long long strideB, const GemmEpi& epi, int M, int N, int K,
                    int batch, cudaStream_t stream) {
-  HK_REQUIRE(Ah && Al && Bh && Bl && epi.C, HK_ERR_ARG, "gemm_pair: null pointer");
-  HK_REQUIRE(M > 0 && N > 0 && K > 0 && batch > 0 && batch <= 65535, HK_ERR_ARG, "gemm_pair: bad shape M=%d N=%d K=%d batch=%d",
-             M, N, K, batch);
+  if (int r = check_gemm_args("gemm_pair", Ah, lda, strideA, Bh, ldb, strideB, epi, M, N, K, batch)) return r;
+  if (int r = check_operand("gemm_pair", 'a', Al, lda, strideA, batch)) return r;
+  if (int r = check_operand("gemm_pair", 'b', Bl, ldb, strideB, batch)) return r;
   CUtensorMap tmA, tmB, tmAl, tmBl;
   int shareA, shareB, r;
   // two accumulators per tile in registers: BN = 64 keeps them at 64 per thread
@@ -607,7 +626,6 @@ extern "C" int hk_gemm_3xtf32(const float* A, int a_mn_major, long long lda, lon
                               long long strideC, int trans_c, int M, int N, int K, int batch, float alpha,
                               const float* alpha_vec, float diag, const float* D, long long ldd, long long strideD,
                               float beta, const float* beta_vec, int relu, void* stream) {
-  HK_REQUIRE(A && B && C && M > 0 && N > 0 && K > 0 && batch > 0, HK_ERR_ARG, "hk_gemm_3xtf32: bad args");
   return hk::gemm_tf32_3x(A, a_mn_major, lda, strideA, B, b_mn_major, ldb, strideB,
                           hk::plain_epi(C, ldc, strideC, trans_c, alpha, alpha_vec, diag, D, ldd, strideD, beta, beta_vec, relu),
                           M, N, K, batch, static_cast<cudaStream_t>(stream));

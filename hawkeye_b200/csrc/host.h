@@ -57,7 +57,8 @@ int make_tmap(CUtensorMap* out, const float* base, int rank, const uint64_t* dim
 // ---- precise mode (parity runs; hk_set_precise / $HK_PRECISE) -------------------------------------------------------
 // 0 (default): every tensor-core product is single-pass TF32 and producers round what they hand to the next MMA.
 // 1          : 3xTF32 — every MMA operand is split into (hi, lo) tf32 halves and A.B ~= Ah.Bh + Al.Bh + Ah.Bl is accumulated
-//              by the SAME kernels (three passes chained through their epilogue addend); nothing is rounded on store.
+//              by the same GEMM in one launch (its pair kernel issues all three products per k-step); nothing is rounded
+//              on store.
 //              fp32-class accuracy at >3x the cost: a test mode, which is why it may allocate stream-ordered scratch.
 bool precise();
 // stream-ordered scratch buffer (cudaMallocAsync / cudaFreeAsync on `s`); used by the precise mode only

@@ -33,7 +33,7 @@ void hk_reset_launch_count(void);
  *    forward tolerance of the path; gradients below ReLU / max-pool kinks then differ from an fp32 run by branch
  *    flips (see tests/matched.py).
  * 1: 3xTF32 — every MMA operand is split into (hi, lo) tf32 halves and  A.B ~= Ah.Bh + Al.Bh + Ah.Bl  is accumulated
- *    by the same kernels in three passes; nothing is rounded on store.  fp32-class results (for parity runs against
+ *    by the same GEMM in one launch (all three products per k-step); nothing is rounded on store.  fp32-class results (for parity runs against
  *    the fp32 reference) at more than 3x the cost; this mode allocates stream-ordered scratch (cudaMallocAsync). */
 void hk_set_precise(int on);
 int hk_get_precise(void);

@@ -63,6 +63,34 @@ def test_head_and_mpncov_argument_errors(lib):
     assert lib.hk_sqrtm_fwd(FAKE, FAKE, FAKE, 2, 256, 1, FAKE, 1 << 40, None) == -3 and 'iterN' in err(lib)
 
 
+@pytest.mark.parametrize('precise', [0, 1], ids=['tf32', 'precise'])
+@pytest.mark.parametrize('entry', ['hk_gemm_tf32', 'hk_gemm_3xtf32'])
+def test_gemm_operand_errors_before_any_allocation_or_launch(lib, entry, precise):
+    """The GEMM's TMA preconditions (16-byte aligned operand base, row pitch and batch stride in 16-byte units,
+    batch <= 65535) are checked before the 3xTF32 path allocates its operand halves or anything is launched, so an
+    unaligned operand is rejected in both precision modes."""
+    f = getattr(lib, entry)
+
+    def call(A=FAKE, lda=64, strideA=64 * 64, B=FAKE, ldb=64, batch=2):
+        return f(A, 0, lda, strideA, B, 0, ldb, 64 * 64, FAKE, 64, 64 * 64, 0, 64, 64, 64, batch, 1.0, None, 0.0, None,
+                 0, 0, 0.0, None, 0, None)
+
+    lib.hk_set_precise(precise)
+    lib.hk_reset_launch_count()
+    try:
+        assert call(lda=5) == -2 and 'lda=5' in err(lib) and '16-byte' in err(lib)
+        assert call(ldb=66) == -2 and 'ldb=66' in err(lib)
+        assert call(A=FAKE + 4) == -2 and 'not 16-byte aligned' in err(lib)
+        assert call(B=FAKE + 8) == -2 and 'not 16-byte aligned' in err(lib)
+        assert call(strideA=64 * 64 + 2) == -2 and 'batch stride of a' in err(lib)
+        assert call(batch=65536) == -3 and '65535' in err(lib)
+        assert call(batch=0) == -1 and 'bad shape' in err(lib)
+        assert call(A=None) == -1 and 'null' in err(lib)
+        assert lib.hk_launch_count() == 0
+    finally:
+        lib.hk_set_precise(0)
+
+
 def test_errors_are_thread_local_text(lib):
     lib.hk_bilinear_pool_fwd(FAKE, FAKE, None, 2, 100, 196, FAKE, 1 << 30, None)
     msg = err(lib)
