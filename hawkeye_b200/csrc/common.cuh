@@ -155,6 +155,13 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[8], const uint32_t (&a)[4]
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc));
 }
+__device__ __forceinline__ void wgmma_tf32(float (&d)[16], const uint32_t (&a)[4], uint64_t bdesc) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, 1, 1, 1;\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc));
+}
 
 // named barrier over `count` threads (id 0 is __syncthreads)
 __device__ __forceinline__ void named_bar(int id, int count) {
@@ -178,6 +185,9 @@ __device__ __forceinline__ uint32_t ld_shared_u32(uint32_t saddr) {
   uint32_t v;
   asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(saddr) : "memory");
   return v;
+}
+__device__ __forceinline__ void st_shared_v4(uint32_t saddr, uint32_t x, uint32_t y, uint32_t z, uint32_t w) {
+  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
 }
 
 // byte offset of fp32 element (row, k) in a K-major 128B-swizzled tile (row = M/N index, k < 32): the 16-byte chunk

@@ -538,201 +538,237 @@ static int conv3x3_igemm_1x(const float* x, const float* wp, const float* bias, 
 
 // ------------------------------------------------------------------------------------------------
 // weight gradient: one CTA accumulates dWp[tap][co0 : co0 + CO][ci0 : ci0 + CI] for ALL 9 taps over its share of the
-// pixels (split-K across CTAs, fp32 atomics at the end).  A stage covers a 64-pixel tile (TW x TH x TN):
+// pixels (split-K across CTAs, fp32 atomics at the end).  A stage covers a 64-pixel tile (TW x TH x TN, a template
+// parameter: the producer's transposition map and the consumers' tap offsets are compile-time):
 //   A = dY^T (M = co, k = pixel).  TMA lands dY pixel-major ([64 px][32 co] boxes, 128B-swizzled); each consumer thread
-//       reads its m64k8 register fragment straight from there and feeds it to all nine taps, so dY is neither transposed
-//       nor re-read per tap.  The same registers give the bias gradient.
+//       reads its m64k8 register fragment straight from there and feeds it to all of its taps, so dY is neither
+//       transposed nor re-read per tap.  The same registers give the bias gradient.
 //   B = X: ONE TMA box of (TH+2) x (TW+2) x TN pixels x 32 ci (the halo patch), transposed by the producer warpgroup
 //       into three kw-shifted K-major copies [32 ci][(TH+2) TW TN px].  Tap (kh, kw) reads copy kw kh*TW pixels further
-//       along k (TW a multiple of 8: whole wgmma k-steps).  Three halo buffers keep the next boxes' TMA in flight while
-//       one is transposed.
-//   Tile: 64 co x 32 ci.  Both consumer warpgroups load the same dY fragment; warpgroup wg accumulates ci 16 wg..16 wg+15
-//   for all nine taps (m64n16k8, 72 fp32 registers per thread).  With A in registers the B bytes a wgmma reads per FLOP
-//   depend on M alone, so n16 costs no more shared-memory bandwidth than n32 would; 9 x (64 x 32) accumulators per
-//   warpgroup (144 per thread) do not fit the consumer's registers without spilling.
+//       along k (TW a multiple of 8: whole wgmma k-steps).  A producer task is 4 pixels of one halo row: lane = ci reads
+//       the 6 halo pixels the three kw shifts need (one 128-byte row each) and writes one 16-byte chunk per copy.
+//   Tile: 64 co x 32 ci.  Three consumer warpgroups, one per kernel row kh, load the same dY fragment; warpgroup kh
+//       accumulates taps (kh, 0..2) over all 32 ci with m64n32k8 (48 fp32 registers per thread): 24 wgmmas per stage
+//       and warpgroup.  With A in registers the B bytes a wgmma reads per FLOP depend on M alone, so n32 costs the
+//       shared memory no more than n16, and it runs at the full tensor rate where register-A m64n16k8 reaches about
+//       60 % of it (290 vs 490 TFLOP/s in a throughput loop, H100 SXM at 700 W).
+//   Pipeline: three stage slots {dY boxes, kw copies} and three halo buffers.  The halo box of stage k + 3 is requested
+//   as soon as stage k's has been transposed; dY goes out as soon as its slot is released, up to three stages before
+//   the consumers need it.  The tile origin advances incrementally (no division inside the loop).
 // ------------------------------------------------------------------------------------------------
 struct WgradArgs {
   float* dWp;  // [9][Cout][Cin], pre-zeroed
   float* db;   // [Cout], pre-zeroed, or null
   int N, H, W, Cin, Cout;
   int TW, TH, TN, tiles_w, tiles_h, tiles_n;
-  int ksplit;
+  int total_tiles, per;   // pixel tiles, and tiles per split-K CTA (blockIdx.y)
 };
 
-constexpr int WG_THREADS = 384;
+constexpr int WG_THREADS = 512;                    // producer warpgroup + one consumer warpgroup per kernel row
+constexpr int WG_STAGES = 3;                       // stage slots = halo buffers
 constexpr int WG_KP = 64;                          // pixels per stage
 constexpr int WG_PATCH_PX = 96;                    // (TH+2) * TW * TN: transposed patch pixels, at most 3 k-chunks of 32
 constexpr int WG_RAW_ROWS = 120;                   // (TH+2) * (TW+2) * TN: halo box rows (TW >= 8)
 constexpr int WG_RAW_BYTES = WG_RAW_ROWS * 128;    // one ci chunk of the halo box (15 KB, whole swizzle atoms)
-constexpr int WG_RAW_BUFS = 3;                     // halo boxes in flight or being transposed
 constexpr int WG_XT_KW = 3 * 32 * 128;             // one kw copy: 3 k-chunks of [32 ci x 32 px]
 constexpr int WG_XT_CHUNK = 3 * WG_XT_KW;          // the three kw copies of one ci chunk
 
 constexpr int WG_CO = 64, WG_CI = 32;             // CTA tile
 constexpr int WG_DY_BYTES = (WG_CO / 32) * WG_KP * 128;
 constexpr int WG_STAGE_BYTES = WG_DY_BYTES + WG_XT_CHUNK;
-constexpr int WG_SMEM = 2 * WG_STAGE_BYTES + WG_RAW_BUFS * WG_RAW_BYTES + 1024 + 256;
+constexpr int WG_SMEM = WG_STAGES * (WG_STAGE_BYTES + WG_RAW_BYTES) + 1024 + 256;   // 202 KB + alignment + barriers
+static_assert(WG_SMEM <= 227 * 1024, "wgrad shared memory");
 
+// producer warp WARP's share of one halo-box transposition (tasks WARP, WARP + 4, ...).  rw / xt: shared addresses of
+// the halo box and of the stage's kw copies.  xr[m]: this lane's (ci's) swizzled byte offset in a halo row r with
+// r & 7 == m; xw[c]: this lane's offset of 16-byte chunk c in its row of a kw copy.  Everything else is an immediate.
+template <int TW, int TH, int TN, int WARP>
+__device__ __forceinline__ void wgrad_transpose(uint32_t rw, uint32_t xt, const uint32_t (&xr)[8],
+                                                const uint32_t (&xw)[8]) {
+  constexpr int NTASK = (TH + 2) * TW * TN / 4;
+  static_assert(NTASK % 4 == 0, "tasks split evenly over the producer warps");
+#pragma unroll
+  for (int task = WARP; task < NTASK; task += 4) {
+    const int p0 = 4 * task, q = p0 / TW, j0 = p0 % TW;   // patch pixels p0..p0+3: halo row q, columns j0..j0+3
+    const int r0 = q * (TW + 2) + j0;                   // halo rows r0..r0+5 cover the three kw shifts
+    uint32_t v[6];
+#pragma unroll
+    for (int c = 0; c < 6; ++c) v[c] = ld_shared_u32(rw + xr[(r0 + c) & 7] + (r0 + c) * 128);
+#pragma unroll
+    for (int kw = 0; kw < 3; ++kw)
+      st_shared_v4(xt + xw[(p0 & 31) >> 2] + kw * WG_XT_KW + (p0 >> 5) * 4096, v[kw], v[kw + 1], v[kw + 2], v[kw + 3]);
+  }
+}
+
+// tile origin (w0, h0, n0) of pixel tile t, advanced one tile at a time
+template <int TW, int TH, int TN>
+struct WgradTile {
+  int w0, h0, n0;
+  __device__ __forceinline__ WgradTile(int t, const WgradArgs& a) {
+    w0 = t % a.tiles_w * TW; t /= a.tiles_w;
+    h0 = t % a.tiles_h * TH;
+    n0 = t / a.tiles_h * TN;
+  }
+  __device__ __forceinline__ void next(const WgradArgs& a) {
+    if ((w0 += TW) < a.W) return;
+    w0 = 0;
+    if ((h0 += TH) < a.H) return;
+    h0 = 0;
+    n0 += TN;
+  }
+};
+
+template <int TW, int TH, int TN>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX, WgradArgs a) {
+  static_assert(TW * TH * TN == WG_KP && TW % 8 == 0, "64-pixel tile of whole 8-pixel rows");
+  static_assert((TH + 2) * TW * TN <= WG_PATCH_PX && (TH + 2) * (TW + 2) * TN <= WG_RAW_ROWS, "halo patch too large");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* stages = smem;                           // [2] x {dY boxes, three kw copies of X^T}
-  uint8_t* raw = smem + 2 * WG_STAGE_BYTES;       // [WG_RAW_BUFS] halo boxes
-  uint64_t* full = reinterpret_cast<uint64_t*>(raw + WG_RAW_BUFS * WG_RAW_BYTES);
-  uint64_t* empty = full + 2;
-  uint64_t* raw_full = empty + 2;
+  uint8_t* stages = smem;                                   // [WG_STAGES] x {dY boxes, three kw copies of X^T}
+  uint8_t* raw = smem + WG_STAGES * WG_STAGE_BYTES;         // [WG_STAGES] halo boxes
+  uint64_t* full = reinterpret_cast<uint64_t*>(raw + WG_STAGES * WG_RAW_BYTES);
+  uint64_t* empty = full + WG_STAGES;
+  uint64_t* raw_full = empty + WG_STAGES;
 
   const int warp = threadIdx.x >> 5;
   const int n_ci_tiles = (a.Cin + WG_CI - 1) / WG_CI;
   const int ci_t = blockIdx.x % n_ci_tiles, co_t = blockIdx.x / n_ci_tiles;
   const int co0 = co_t * WG_CO, ci0 = ci_t * WG_CI;
-  const long long total_tiles = (long long)a.tiles_w * a.tiles_h * a.tiles_n;
-  const long long per = (total_tiles + a.ksplit - 1) / a.ksplit;
-  const long long t_begin = per * blockIdx.y;
-  const long long t_end = (t_begin + per < total_tiles) ? t_begin + per : total_tiles;
-  const int nk = (int)(t_end > t_begin ? t_end - t_begin : 0);
-  const int img_rows = a.TH * a.TW;                 // dY pixels per image in the tile
-  const int patch_rows = (a.TH + 2) * a.TW * a.TN;  // pixels of one kw copy
+  const long long t_begin = (long long)a.per * blockIdx.y;   // < total_tiles < 2^31 for every launched CTA
+  const int nk = (int)min((long long)a.per, (long long)a.total_tiles - t_begin);
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmDY);
     tma_prefetch_desc(&tmX);
-    // full: the dY TMA's expect_tx arrival + the producer's arrival once the X copies are written
-    for (int s = 0; s < 2; ++s) { mbar_init(&full[s], 2); mbar_init(&empty[s], 2); }
-    for (int i = 0; i < WG_RAW_BUFS; ++i) mbar_init(&raw_full[i], 1);
+    for (int s = 0; s < WG_STAGES; ++s) {
+      mbar_init(&full[s], 2);       // the dY TMA's expect_tx arrival + the producer's once the X copies are written
+      mbar_init(&empty[s], 3);      // one arrival per consumer warpgroup
+      mbar_init(&raw_full[s], 1);
+    }
     fence_barrier_init();
   }
   __syncthreads();
-  if (nk == 0) return;
-
-  auto tile_origin = [&](int k, int* w0, int* h0, int* n0) {
-    long long tt = t_begin + k;
-    *w0 = (int)(tt % a.tiles_w) * a.TW; tt /= a.tiles_w;
-    *h0 = (int)(tt % a.tiles_h) * a.TH; tt /= a.tiles_h;
-    *n0 = (int)tt * a.TN;
-  };
+  if (nk <= 0) return;
 
   if (warp < 4) {
     regs_dealloc<56>();
     const int t = threadIdx.x, lane = t & 31;
-    const uint32_t raw_tx = (uint32_t)((a.TH + 2) * (a.TW + 2) * a.TN * 128);
-    auto issue_raw = [&](int u) {
-      const int b = u % WG_RAW_BUFS;
-      int w0, h0, n0;
-      tile_origin(u, &w0, &h0, &n0);
-      mbar_expect_tx(&raw_full[b], raw_tx);
-      tma_load_4d(raw + b * WG_RAW_BYTES, &tmX, &raw_full[b], ci0, w0 - 1, h0 - 1, n0);
-    };
+    constexpr uint32_t raw_tx = (TH + 2) * (TW + 2) * TN * 128;
+    uint32_t xr[8], xw[8];
+#pragma unroll
+    for (int m = 0; m < 8; ++m) {
+      xr[m] = (uint32_t)((((lane >> 2) ^ m) << 4) | ((lane & 3) << 2));
+      xw[m] = sw128_off(lane, 4 * m);
+    }
+    const uint32_t stage0 = smem_u32(stages), raw0 = smem_u32(raw);
+    WgradTile<TW, TH, TN> dy_tile((int)t_begin, a), raw_tile = dy_tile;   // only thread 0 issues TMAs
     if (t == 0)
-      for (int u = 0; u < WG_RAW_BUFS && u < nk; ++u) issue_raw(u);
-    const int ngrp = patch_rows / 4, ntask = 3 * ngrp;
+      for (int u = 0; u < WG_STAGES && u < nk; ++u) {
+        mbar_expect_tx(&raw_full[u], raw_tx);
+        tma_load_4d(raw + u * WG_RAW_BYTES, &tmX, &raw_full[u], ci0, raw_tile.w0 - 1, raw_tile.h0 - 1, raw_tile.n0);
+        raw_tile.next(a);
+      }
+    int s = 0;
+    uint32_t ph = 0;
     for (int k = 0; k < nk; ++k) {
-      const int s = k & 1;
       uint8_t* st = stages + s * WG_STAGE_BYTES;
-      mbar_wait(&empty[s], ((k >> 1) & 1) ^ 1);
+      mbar_wait(&empty[s], ph ^ 1);
       if (t == 0) {
-        int w0, h0, n0;
-        tile_origin(k, &w0, &h0, &n0);
         mbar_expect_tx(&full[s], WG_DY_BYTES);
 #pragma unroll
-        for (int j = 0; j < WG_CO / 32; ++j) tma_load_4d(st + j * (WG_KP * 128), &tmDY, &full[s], co0 + j * 32, w0, h0, n0);
+        for (int j = 0; j < WG_CO / 32; ++j)
+          tma_load_4d(st + j * (WG_KP * 128), &tmDY, &full[s], co0 + j * 32, dy_tile.w0, dy_tile.h0, dy_tile.n0);
+        dy_tile.next(a);
       }
-      {
-        const int b = k % WG_RAW_BUFS;
-        mbar_wait(&raw_full[b], (k / WG_RAW_BUFS) & 1);
-        const uint8_t* rw = raw + b * WG_RAW_BYTES;
-        uint8_t* xt = st + WG_DY_BYTES;
-        // one warp per (kw, 4 pixels): lane = ci, so each read is one whole 128-byte halo row and each float4 write
-        // lands in a different row of the K-major copy (conflict-free both ways)
-        for (int task = warp; task < ntask; task += 4) {
-          const int kw = task / ngrp, p0 = (task - kw * ngrp) * 4;
-          float v[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int p = p0 + i, q = p / a.TW, j = p - q * a.TW;
-            v[i] = *reinterpret_cast<const float*>(rw + sw128_off(q * (a.TW + 2) + j + kw, lane));
-          }
-          *reinterpret_cast<float4*>(xt + kw * WG_XT_KW + (p0 >> 5) * 4096 + sw128_off(lane, p0 & 31)) =
-              make_float4(v[0], v[1], v[2], v[3]);
+      mbar_wait(&raw_full[s], ph);
+      const uint32_t rw = raw0 + s * WG_RAW_BYTES, xt = stage0 + s * WG_STAGE_BYTES + WG_DY_BYTES;
+      switch (warp) {
+        case 0: wgrad_transpose<TW, TH, TN, 0>(rw, xt, xr, xw); break;
+        case 1: wgrad_transpose<TW, TH, TN, 1>(rw, xt, xr, xw); break;
+        case 2: wgrad_transpose<TW, TH, TN, 2>(rw, xt, xr, xw); break;
+        default: wgrad_transpose<TW, TH, TN, 3>(rw, xt, xr, xw); break;
+      }
+      fence_proxy_async();
+      named_bar(1, 128);                            // every thread is done with halo buffer s
+      if (t == 0) {
+        if (k + WG_STAGES < nk) {
+          mbar_expect_tx(&raw_full[s], raw_tx);
+          tma_load_4d(raw + s * WG_RAW_BYTES, &tmX, &raw_full[s], ci0, raw_tile.w0 - 1, raw_tile.h0 - 1, raw_tile.n0);
+          raw_tile.next(a);
         }
-        fence_proxy_async();
-        named_bar(1, 128);                          // every thread is done with halo buffer b
-        if (t == 0 && k + WG_RAW_BUFS < nk) issue_raw(k + WG_RAW_BUFS);
+        mbar_arrive(&full[s]);
       }
-      if (t == 0) mbar_arrive(&full[s]);
+      if (++s == WG_STAGES) { s = 0; ph ^= 1; }
     }
   } else {
-    regs_alloc<224>();
+    regs_alloc<152>();
     const int ct = threadIdx.x - 128;
-    const int wg = ct >> 7, t = ct & 127, wl = t >> 5, lane = t & 31, g = lane >> 2, q = lane & 3;
+    const int kh = ct >> 7, t = ct & 127, wl = t >> 5, lane = t & 31, g = lane >> 2, q = lane & 3;
     // this thread's A rows: co 16 wl + g (+8), in dY box wl / 2 at column 16 (wl & 1) + g (+8)
     const int box = wl >> 1, col = 16 * (wl & 1) + g;
     const uint32_t off0 = sw128_off(q, col), off1 = sw128_off(q, col + 8), off2 = sw128_off(q + 4, col),
                    off3 = sw128_off(q + 4, col + 8);
-    float acc[9][8];
+    // B start of k-step ks in copy 0, in 16-byte descriptor units: patch pixel 8 ks + 2 TW per earlier image + kh TW
+    uint32_t boff[8];
 #pragma unroll
-    for (int j = 0; j < 9; ++j)
+    for (int ks = 0; ks < 8; ++ks) {
+      const int kk = 8 * ks + (8 * ks) / (TH * TW) * 2 * TW + kh * TW;
+      boff[ks] = (uint32_t)((kk >> 5) * 4096 + (kk & 31) / 8 * 32) >> 4;
+    }
+    float acc[3][16];
 #pragma unroll
-      for (int e = 0; e < 8; ++e) acc[j][e] = 0.f;
+    for (int j = 0; j < 3; ++j)
+#pragma unroll
+      for (int e = 0; e < 16; ++e) acc[j][e] = 0.f;
     float bsum0 = 0.f, bsum1 = 0.f;                 // bias gradient of rows g and g + 8
     uint32_t fr[2][4];                              // two fragment sets: one may still be read by the wgmmas in flight
+    int s = 0;
+    uint32_t ph = 0;
     for (int k = 0; k < nk; ++k) {
-      const int s = k & 1;
-      mbar_wait(&full[s], (k >> 1) & 1);
+      mbar_wait(&full[s], ph);
       const uint32_t dyb = smem_u32(stages + s * WG_STAGE_BYTES + box * (WG_KP * 128));
-      // descriptor start addresses are 16-byte units in the low bits: offsets inside the stage are added to one base
-      // ci rows 16 wg.. of the [32 ci] copies: two whole 8-row swizzle groups further on
-      const uint64_t xdesc = make_sdesc(smem_u32(stages + s * WG_STAGE_BYTES + WG_DY_BYTES) + wg * 16 * 128);
-#pragma unroll 1   // rolled by k-step pairs: the tap descriptors of one pair live at a time, not all 72
-      for (int ks2 = 0; ks2 < 8; ks2 += 2) {
+      const uint64_t xdesc = make_sdesc(smem_u32(stages + s * WG_STAGE_BYTES + WG_DY_BYTES));
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int ks = ks2 + h;
-          uint32_t (&f)[4] = fr[h];
-          // pixel rows 8 ks + q (+4): the swizzle phase (row & 7) is the same every k-step, so one offset per element
-          const uint32_t fa = dyb + ks * 1024;
-          f[0] = ld_shared_u32(fa + off0);
-          f[1] = ld_shared_u32(fa + off1);
-          f[2] = ld_shared_u32(fa + off2);
-          f[3] = ld_shared_u32(fa + off3);
-          bsum0 += __uint_as_float(f[0]) + __uint_as_float(f[2]);
-          bsum1 += __uint_as_float(f[1]) + __uint_as_float(f[3]);
-          const int kb = 8 * ks + ((8 * ks) / img_rows) * 2 * a.TW;   // k of this step in the patch: + 2 TW per image
-          wgmma_fence();
+      for (int ks = 0; ks < 8; ++ks) {
+        uint32_t (&f)[4] = fr[ks & 1];
+        // pixel rows 8 ks + q (+4): the swizzle phase (row & 7) is the same every k-step, so one offset per element
+        const uint32_t fa = dyb + ks * 1024;
+        f[0] = ld_shared_u32(fa + off0);
+        f[1] = ld_shared_u32(fa + off1);
+        f[2] = ld_shared_u32(fa + off2);
+        f[3] = ld_shared_u32(fa + off3);
+        bsum0 += __uint_as_float(f[0]) + __uint_as_float(f[2]);
+        bsum1 += __uint_as_float(f[1]) + __uint_as_float(f[3]);
+        wgmma_fence();
 #pragma unroll
-          for (int tap = 0; tap < 9; ++tap) {
-            const int kh = tap / 3, kw = tap % 3;
-            const int kk = kb + kh * a.TW;
-            const uint32_t off = kw * WG_XT_KW + (kk >> 5) * 4096 + (kk & 31) / 8 * 32;
-            wgmma_tf32(acc[tap], f, xdesc + (off >> 4));
-          }
-          wgmma_commit();
-          wgmma_wait<1>();      // k-step ks stays in flight; ks - 1 (and its fragment set) is done
+        for (int kw = 0; kw < 3; ++kw) wgmma_tf32(acc[kw], f, xdesc + boff[ks] + kw * (WG_XT_KW >> 4));
+        wgmma_commit();
+        wgmma_wait<1>();      // k-step ks stays in flight; ks - 1 (and its fragment set) is done
 #pragma unroll
-          for (int j = 0; j < 9; ++j) wgmma_keep(acc[j]);
-          if (ks == 0 && k > 0 && t == 0) mbar_arrive(&empty[(k - 1) & 1]);   // the last k-step of stage k - 1 is done
-        }
+        for (int j = 0; j < 3; ++j) wgmma_keep(acc[j]);
+        if (ks == 0 && k > 0 && t == 0) mbar_arrive(&empty[s == 0 ? WG_STAGES - 1 : s - 1]);   // stage k - 1 is done
       }
+      if (++s == WG_STAGES) { s = 0; ph ^= 1; }
     }
     wgmma_wait<0>();
 #pragma unroll
-    for (int j = 0; j < 9; ++j) wgmma_keep(acc[j]);
+    for (int j = 0; j < 3; ++j) wgmma_keep(acc[j]);
 #pragma unroll
-    for (int tap = 0; tap < 9; ++tap)
+    for (int kw = 0; kw < 3; ++kw)
 #pragma unroll
-      for (int e = 0; e < 8; ++e) {
+      for (int e = 0; e < 16; ++e) {
         const int co = co0 + 16 * wl + g + 8 * ((e >> 1) & 1);
-        const int ci = ci0 + 16 * wg + 8 * (e >> 2) + 2 * q + (e & 1);
-        if (co < a.Cout && ci < a.Cin) atomicAdd(a.dWp + ((size_t)tap * a.Cout + co) * a.Cin + ci, acc[tap][e]);
+        const int ci = ci0 + 8 * (e >> 2) + 2 * q + (e & 1);
+        if (co < a.Cout) atomicAdd(a.dWp + ((size_t)(3 * kh + kw) * a.Cout + co) * a.Cin + ci, acc[kw][e]);
       }
     // bias: the quad's four threads hold the same rows at different pixels; one atomic per co on the ci-tile-0 CTAs
-    // (both warpgroups read the same rows: warpgroup 0 adds them)
+    // (all three warpgroups read the same rows: warpgroup 0 adds them)
     bsum0 += __shfl_xor_sync(0xffffffffu, bsum0, 1);
     bsum0 += __shfl_xor_sync(0xffffffffu, bsum0, 2);
     bsum1 += __shfl_xor_sync(0xffffffffu, bsum1, 1);
     bsum1 += __shfl_xor_sync(0xffffffffu, bsum1, 2);
-    if (a.db && ci_t == 0 && wg == 0 && q == 0) {
+    if (a.db && ci_t == 0 && kh == 0 && q == 0) {
       const int co = co0 + 16 * wl + g;
       if (co < a.Cout) atomicAdd(a.db + co, bsum0);
       if (co + 8 < a.Cout) atomicAdd(a.db + co + 8, bsum1);
@@ -740,7 +776,8 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_cons
   }
 }
 
-// pixel tile for wgrad: TW in {8,16} (kh shifts must be whole wgmma k-steps of 8 pixels), TW*TH*TN = 64, TH*TW % 8 == 0
+// pixel tile for wgrad: TW in {8,16} (kh shifts must be whole wgmma k-steps of 8 pixels), TW*TH*TN = 64, TH*TW % 8 == 0.
+// Returns one of the three tiles launch_wgrad instantiates: (16, 4, 1), (8, 8, 1), (8, 4, 2).
 static bool pick_wgrad_tile(int W, int H, int* TW, int* TH, int* TN) {
   int tw = 0;
   for (int c : {16, 8}) if (W % c == 0) { tw = c; break; }
@@ -756,11 +793,23 @@ static bool pick_wgrad_tile(int W, int H, int* TW, int* TH, int* TN) {
   return true;
 }
 
+template <int TW, int TH, int TN>
+static int launch_wgrad_tile(const CUtensorMap& tmDY, const CUtensorMap& tmX, const WgradArgs& a, dim3 grid,
+                             cudaStream_t stream) {
+  int r;
+  if ((r = allow_dynamic_smem<conv3x3_wgrad_kernel<TW, TH, TN>>(WG_SMEM, "wgrad"))) return r;
+  conv3x3_wgrad_kernel<TW, TH, TN><<<grid, WG_THREADS, WG_SMEM, stream>>>(tmDY, tmX, a);
+  HK_LAUNCH_CHECK("conv3x3_wgrad_kernel");
+  return 0;
+}
+
 static int launch_wgrad(const float* x, const float* dy, WgradArgs a, cudaStream_t stream) {
   const long long out_tiles = (long long)((a.Cout + WG_CO - 1) / WG_CO) * ((a.Cin + WG_CI - 1) / WG_CI);
   const long long total_tiles = (long long)a.tiles_w * a.tiles_h * a.tiles_n;
-  // split-K factor.  The kernel runs one CTA per SM (its shared memory allows no second), so the grid executes in whole
-  // waves of `sms` CTAs: pick the split that fills 1..3 waves best (ties -> fewer waves: fewer partial sums to add).
+  HK_REQUIRE(total_tiles < (1ll << 31), HK_ERR_UNSUPPORTED, "conv3x3_wgrad: too many pixel tiles");
+  // split-K factor.  The kernel runs one CTA per SM (its 202 KB of shared memory allow no second, and its 512 threads
+  // hold the whole register file), so the grid executes in whole waves of `sms` CTAs: pick the split that fills
+  // 1..3 waves best (ties -> fewer waves: fewer partial sums to add).
   const int sms = num_sms();
   long long ks = 1;
   {
@@ -778,16 +827,17 @@ static int launch_wgrad(const float* x, const float* dy, WgradArgs a, cudaStream
   if (ks > total_tiles) ks = total_tiles;
   if (ks < 1) ks = 1;
   if (ks > 65535) ks = 65535;
-  a.ksplit = (int)ks;
+  a.total_tiles = (int)total_tiles;
+  a.per = (int)((total_tiles + ks - 1) / ks);
+  const dim3 grid((unsigned)out_tiles, (unsigned)((total_tiles + a.per - 1) / a.per));   // every CTA has tiles
   CUtensorMap tmDY, tmX;
   int r;
   if ((r = make_act_map(&tmDY, dy, a.N, a.H, a.W, a.Cout, a.TW, a.TH, a.TN))) return r;
   if ((r = make_act_map(&tmX, x, a.N, a.H, a.W, a.Cin, a.TW + 2, a.TH + 2, a.TN))) return r;
-  if ((r = allow_dynamic_smem<conv3x3_wgrad_kernel>(WG_SMEM, "wgrad"))) return r;
-  dim3 grid((unsigned)out_tiles, a.ksplit);
-  conv3x3_wgrad_kernel<<<grid, WG_THREADS, WG_SMEM, stream>>>(tmDY, tmX, a);
-  HK_LAUNCH_CHECK("conv3x3_wgrad_kernel");
-  return 0;
+  if (a.TW == 16 && a.TH == 4 && a.TN == 1) return launch_wgrad_tile<16, 4, 1>(tmDY, tmX, a, grid, stream);
+  if (a.TW == 8 && a.TH == 8 && a.TN == 1) return launch_wgrad_tile<8, 8, 1>(tmDY, tmX, a, grid, stream);
+  if (a.TW == 8 && a.TH == 4 && a.TN == 2) return launch_wgrad_tile<8, 4, 2>(tmDY, tmX, a, grid, stream);
+  return set_error(HK_ERR_UNSUPPORTED, "conv3x3_wgrad: pixel tile %dx%dx%d has no kernel", a.TW, a.TH, a.TN);
 }
 
 static int conv3x3_wgrad_1x(const float* x, const float* dy, float* dwp, float* db, int N, int H, int W, int Cin, int Cout,
