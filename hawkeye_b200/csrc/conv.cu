@@ -59,9 +59,9 @@ struct ConvArgs {
   const float* addend; // [N,H,W,Cout] or null: raw partial sum added to the accumulator first (3xTF32 passes; may alias Y)
   int no_round;        // 1: store fp32 as is (precise mode); 0: round to tf32 (the output feeds another MMA)
   // fused MaxPool2d(2,2) epilogue (vgg.py:59): when P != null the full-resolution map Y is NOT written; the epilogue
-  // reduces each 2x2 window across lanes (the pixel tile is a power-of-two patch, so the window partners are lane^1,
-  // lane^TW, lane^(TW+1)) and writes the pooled value plus, if code != null, the byte maxpool2x2_bwd_idx reads
-  // (bits 0-1 = first maximum in scan order, bit 2 = max > 0).
+  // reduces each 2x2 window (the generic kernel across lanes: the pixel tile is a power-of-two patch, so the window
+  // partners are lane^1, lane^TW, lane^(TW+1); the v2 kernel in its staging tile) and writes the pooled value plus, if
+  // code != null, the byte maxpool2x2_bwd_idx reads (bits 0-1 = first maximum in scan order, bit 2 = max > 0).
   float* P;            // [N,H/2,W/2,Cout] (or [N,Cout,H/2,W/2] when pool_nchw)
   unsigned char* code; // [N,H/2,W/2,Cout] or null
   int pool_nchw;
@@ -124,6 +124,59 @@ struct ConvCfg {
   static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 + 256 + ACC_TILE;
 };
 
+// Output of one 32-column chunk v (channels co .. co + 31) of pixel (w, h, n): addend, bias, ReLU, mask, then the stored
+// map or the fused pooling.  Every lane of the warp calls it (the pooling shuffles are warp-wide), valid or not; lane
+// 32 q + l must hold pixel r = 32 q + l of the tile.
+__device__ __forceinline__ void epi_chunk(const ConvArgs& a, float (&v)[32], int w, int h, int n, size_t pix, int co,
+                                          bool valid) {
+  if (valid && co < a.Cout) {
+    if (a.addend) {
+      const float4* ad = reinterpret_cast<const float4*>(a.addend + pix * a.Cout + co);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float4 t = ad[j];
+        v[4 * j] += t.x; v[4 * j + 1] += t.y; v[4 * j + 2] += t.z; v[4 * j + 3] += t.w;
+      }
+    }
+    if (a.bias) {
+#pragma unroll
+      for (int j = 0; j < 32; ++j) v[j] += __ldg(a.bias + co + j);
+    }
+    if (a.relu) {
+#pragma unroll
+      for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
+    }
+    if (a.mask) {
+      const float4* m = reinterpret_cast<const float4*>(a.mask + pix * a.Cout + co);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float4 mm = m[j];
+        v[4 * j] = mm.x > 0.f ? v[4 * j] : 0.f;
+        v[4 * j + 1] = mm.y > 0.f ? v[4 * j + 1] : 0.f;
+        v[4 * j + 2] = mm.z > 0.f ? v[4 * j + 2] : 0.f;
+        v[4 * j + 3] = mm.w > 0.f ? v[4 * j + 3] : 0.f;
+      }
+    }
+    if (a.P) {       // (never combined with the precise-mode passes: rounded like the stored map would be)
+#pragma unroll
+      for (int j = 0; j < 32; ++j) v[j] = tf32_round(v[j]);
+    } else {
+    float4* dst = reinterpret_cast<float4*>(a.Y + pix * a.Cout + co);
+    if (a.no_round) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) dst[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        dst[j] = make_float4(tf32_round(v[4 * j]), tf32_round(v[4 * j + 1]), tf32_round(v[4 * j + 2]),
+                             tf32_round(v[4 * j + 3]));
+    }
+    }
+  }
+  // the window reduction is a warp-wide shuffle: every lane takes part, whether or not its own pixel is valid
+  if (a.P && co < a.Cout) epi_pool_store(a, v, a.TW, w, h, n, co, valid);
+}
+
 // Epilogue of one 128-pixel x BN tile, run by the 256 MMA threads (ct = thread index among them).  The accumulators go
 // through shared memory two 32-column chunks at a time, after which thread (half, q, lane) owns pixel r = 32 q + lane of
 // chunk 2 c + half — the mapping the fused pooling shuffles rely on.
@@ -160,53 +213,7 @@ __device__ __forceinline__ void conv_epilogue(const ConvArgs& a, const float (&a
 #pragma unroll
       for (int j = 0; j < 32; ++j) v[j] = src[j];
     }
-    const int co = co0 + c * 32;
-    if (valid && co < a.Cout) {
-      if (a.addend) {
-        const float4* ad = reinterpret_cast<const float4*>(a.addend + pix * a.Cout + co);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float4 t = ad[j];
-          v[4 * j] += t.x; v[4 * j + 1] += t.y; v[4 * j + 2] += t.z; v[4 * j + 3] += t.w;
-        }
-      }
-      if (a.bias) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] += __ldg(a.bias + co + j);
-      }
-      if (a.relu) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-      }
-      if (a.mask) {
-        const float4* m = reinterpret_cast<const float4*>(a.mask + pix * a.Cout + co);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float4 mm = m[j];
-          v[4 * j] = mm.x > 0.f ? v[4 * j] : 0.f;
-          v[4 * j + 1] = mm.y > 0.f ? v[4 * j + 1] : 0.f;
-          v[4 * j + 2] = mm.z > 0.f ? v[4 * j + 2] : 0.f;
-          v[4 * j + 3] = mm.w > 0.f ? v[4 * j + 3] : 0.f;
-        }
-      }
-      if (a.P) {       // (never combined with the precise-mode passes: rounded like the stored map would be)
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = tf32_round(v[j]);
-      } else {
-      float4* dst = reinterpret_cast<float4*>(a.Y + pix * a.Cout + co);
-      if (a.no_round) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) dst[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-      } else {
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          dst[j] = make_float4(tf32_round(v[4 * j]), tf32_round(v[4 * j + 1]), tf32_round(v[4 * j + 2]),
-                               tf32_round(v[4 * j + 3]));
-      }
-      }
-    }
-    // the window reduction is a warp-wide shuffle: every lane takes part, whether or not its own pixel is valid
-    if (a.P && co < a.Cout) epi_pool_store(a, v, a.TW, w, h, n, co, valid);
+    epi_chunk(a, v, w, h, n, pix, co0 + c * 32, valid);
   }
 }
 
@@ -322,7 +329,11 @@ static int launch_conv(const CUtensorMap& tmX, const CUtensorMap& tmW, const Con
 //   * RESIDENT (Cin = 64, Cout = 64: VGG conv1_2 and its dgrad): all 9x2 weight tiles (144 KB) stay in shared memory for
 //     the life of the CTA; only activations stream.
 //   * the shared-memory ring runs across tiles, so the producer loads tile i+1 while the MMA warpgroups finish tile i.
+//   * the MMA warpgroups hand each finished tile to a fourth, epilogue warpgroup through a shared-memory staging tile and
+//     go straight on to the next tile: the output stores and the mask loads of tile i overlap the MMAs of tile i+1.
 // ------------------------------------------------------------------------------------------------
+constexpr int CONV_V2_THREADS = 512;
+
 template <int BN, bool RESIDENT>
 struct ConvV2Cfg {
   static constexpr int A_BYTES = 160 * 128;                          // 20 KB halo patch
@@ -330,12 +341,16 @@ struct ConvV2Cfg {
   static constexpr int STAGE_BYTES = A_BYTES + (RESIDENT ? 0 : 3 * B_TILE);
   static constexpr int STAGES = RESIDENT ? 2 : (BN == 64 ? 3 : 2);
   static constexpr int WRES_BYTES = RESIDENT ? 18 * B_TILE : 0;      // 9 taps x 2 chunks
-  static constexpr int ACC_TILE = 2 * 128 * 33 * 4;
-  static constexpr int SMEM = STAGES * STAGE_BYTES + WRES_BYTES + 1024 + 256 + ACC_TILE;
+  // staging tile [128 pixels][BN + 8] fp32: the padding makes the MMA threads' 8-byte fragment stores conflict-free
+  static constexpr int STG_LD = BN + 8;
+  static constexpr int STG_BYTES = 128 * STG_LD * 4;
+  static constexpr int SMEM = STAGES * STAGE_BYTES + WRES_BYTES + 1024 + 256 + STG_BYTES;
 };
 
+// warpgroup 0: TMA producer (one thread); warpgroups 1-2: wgmma on rows 0-63 / 64-127 of the 128-pixel tile; warpgroup 3:
+// the epilogue.
 template <int BN, bool RESIDENT>
-__global__ void __launch_bounds__(CONV_THREADS, 1)
+__global__ void __launch_bounds__(CONV_V2_THREADS, 1)
 conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, ConvArgs a,
                         int n_ntiles, int total_tiles) {
   using Cfg = ConvV2Cfg<BN, RESIDENT>;
@@ -347,7 +362,9 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
   uint64_t* full = reinterpret_cast<uint64_t*>(wres + Cfg::WRES_BYTES);
   uint64_t* empty = full + Cfg::STAGES;
   uint64_t* wbar = empty + Cfg::STAGES;
-  float* acc_tile = reinterpret_cast<float*>(wres + Cfg::WRES_BYTES + 256);
+  uint64_t* stg_full = wbar + 1;                    // the MMA threads wrote the staging tile (256 arrivals)
+  uint64_t* stg_empty = wbar + 2;                   // the epilogue threads read it (128 arrivals)
+  float* stg = reinterpret_cast<float*>(wres + Cfg::WRES_BYTES + 256);
 
   const int warp = threadIdx.x >> 5;
   const int nchunk = a.Cin / 32;
@@ -358,12 +375,38 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
     tma_prefetch_desc(&tmW);
     for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
     mbar_init(wbar, 1);
+    mbar_init(stg_full, 256);
+    mbar_init(stg_empty, 128);
     fence_barrier_init();
   }
   __syncthreads();
 
-  if (warp < 4) {
-    regs_dealloc<56>();
+  if (warp >= 12) {
+    int j = 0;
+    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++j) {
+      int pt = t / n_ntiles;
+      const int tw = pt % a.tiles_w; pt /= a.tiles_w;
+      const int th = pt % a.tiles_h; pt /= a.tiles_h;
+      mbar_wait(stg_full, j & 1);
+      // thread r owns pixel r of the tile, the mapping epi_chunk's pooling shuffles rely on; the 16 x 8 tile divides the
+      // map, so every pixel is valid.  The staging tile is released as soon as its last chunk has been read.
+      const int r = threadIdx.x - 384;
+      const int w = tw * 16 + (r & 15), h = th * 8 + (r >> 4);
+      const size_t pix = ((size_t)pt * a.H + h) * a.W + w;
+#pragma unroll 1
+      for (int c = 0; c < BN / 32; ++c) {
+        float v[32];
+        const float4* src = reinterpret_cast<const float4*>(stg + r * Cfg::STG_LD + c * 32);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+          const float4 q = src[k];
+          v[4 * k] = q.x; v[4 * k + 1] = q.y; v[4 * k + 2] = q.z; v[4 * k + 3] = q.w;
+        }
+        if (c == BN / 32 - 1) mbar_arrive(stg_empty);
+        epi_chunk(a, v, w, h, pt, pix, (t % n_ntiles) * BN + c * 32, true);
+      }
+    }
+  } else if (warp < 4) {
     if (threadIdx.x == 0) {
       if (RESIDENT) {   // whole filter bank (n_ntiles == 1 by construction): 18 tiles of [BN x 32]
         mbar_expect_tx(wbar, Cfg::WRES_BYTES);
@@ -394,7 +437,6 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
       }
     }
   } else {
-    regs_alloc<224>();
     const int ct = threadIdx.x - 128;
     const int wg = ct >> 7;
     if (RESIDENT) mbar_wait(wbar, 0);
@@ -402,11 +444,10 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
     float acc[NACC];
 #pragma unroll
     for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
-    int kbg = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-      int pt = t / n_ntiles;
-      const int tw = pt % a.tiles_w; pt /= a.tiles_w;
-      const int th = pt % a.tiles_h; pt /= a.tiles_h;
+    // this thread's accumulator fragment in the staging tile: rows r0 and r0 + 8, columns 8 i + 2 (lane & 3) + {0, 1}
+    float* frag = stg + (wg * 64 + ((ct >> 5) & 3) * 16 + ((ct & 31) >> 2)) * Cfg::STG_LD + 2 * (ct & 3);
+    int kbg = 0, j = 0;
+    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++j) {
       for (int kb = 0; kb < nkb; ++kb, ++kbg) {
         const int s = kbg % Cfg::STAGES;
         const int ck = kb / 3, kw = kb - ck * 3;
@@ -430,7 +471,13 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
       wgmma_wait<0>();
       wgmma_keep(acc);
       if ((ct & 127) == 0) mbar_arrive(&empty[(kbg - 1) % Cfg::STAGES]);
-      conv_epilogue<BN>(a, acc, acc_tile, tw * 16, th * 8, pt, (t % n_ntiles) * BN, ct);
+      mbar_wait(stg_empty, (j & 1) ^ 1);    // the epilogue warpgroup has read the previous tile
+#pragma unroll
+      for (int i = 0; i < NACC / 4; ++i) {
+        *reinterpret_cast<float2*>(frag + 8 * i) = make_float2(acc[4 * i], acc[4 * i + 1]);
+        *reinterpret_cast<float2*>(frag + 8 * Cfg::STG_LD + 8 * i) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+      }
+      mbar_arrive(stg_full);
     }
   }
 }
@@ -461,7 +508,7 @@ static int launch_conv_v2(const float* x, const float* wp, ConvArgs a, int N, in
   }
   const int sms = num_sms();
   const int grid = total < sms ? (int)total : sms;
-  conv3x3_igemm_v2_kernel<BN, RESIDENT><<<grid, CONV_THREADS, Cfg::SMEM, stream>>>(tmX, tmW, a, n_ntiles, (int)total);
+  conv3x3_igemm_v2_kernel<BN, RESIDENT><<<grid, CONV_V2_THREADS, Cfg::SMEM, stream>>>(tmX, tmW, a, n_ntiles, (int)total);
   HK_LAUNCH_CHECK("conv3x3_igemm_v2_kernel");
   return 0;
 }
