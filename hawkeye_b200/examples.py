@@ -1,5 +1,6 @@
 """Trainer subclasses of the hot-path methods with the reference's Examples/ surface:
-``python -m hawkeye_b200.examples {BCNN,CBCNN,MPN,PeerLearning,OSMENet,APINet,DCL,ProtoTreeNet} --config <yaml>`` replaces
+``python -m hawkeye_b200.examples {BCNN,CBCNN,MPN,PeerLearning,OSMENet,APINet,DCL,ProtoTreeNet,InterpPartsNet} --config
+<yaml>`` replaces
 ``python Examples/<Method>.py --config <yaml>`` (same yaml files; one process per GPU under torchrun instead of nn.DataParallel).
 
 Only what the reference's Examples override is overridden here: which parameters train, with which learning rates, and
@@ -350,11 +351,91 @@ class ProtoTreeTrainer(Trainer):
         self.average_meters['acc'].update(accuracy(pred, labels, 1), images.size(0))
 
 
+class InterpPartsNetTrainer(Trainer):
+    """Examples/InterpPartsNet.py: the reference's train / validation transforms; criterion = InterpPartsLoss (cross-entropy
+    + coeff x shaping loss on the assignment maps); SGD with momentum 0.9 and weight_decay in two groups, conv1, bn1 and
+    layer1-3 at lr and everything else at 20 x lr; CosineAnnealingLR over iterations_per_epoch x epochs, stepped after every
+    batch (the per-epoch scheduler step does nothing).  The optimizer and the schedule run outside the captured graph, so
+    under ``cuda_graph: true`` the learning rate changes from replay to replay as it does eagerly."""
+
+    FINETUNE = ('conv1', 'bn1', 'layer1', 'layer2', 'layer3')
+
+    def get_transformers(self, config):
+        """Examples/InterpPartsNet.py:17-34."""
+        from torchvision import transforms
+        norm = transforms.Normalize(mean=(0.485, 0.456, 0.406), std=(0.229, 0.224, 0.225))
+        return {
+            'train': transforms.Compose([transforms.Resize(size=config.resize_size), transforms.RandomHorizontalFlip(),
+                                         transforms.ColorJitter(0.1), transforms.RandomCrop(size=config.image_size),
+                                         transforms.ToTensor(), norm, transforms.RandomErasing(config.p_erasing)]),
+            'val': transforms.Compose([transforms.Resize(size=config.resize_size), transforms.CenterCrop(size=config.image_size),
+                                       transforms.ToTensor(), norm]),
+        }
+
+    def get_dataloader(self, config):
+        """The base Trainer's datasets, rank sharding and loaders, with the transforms above."""
+        try:
+            from dataset.dataset import FGDataset
+        except Exception:
+            from .data import FGDataset
+        from torch.utils.data import DataLoader
+        tf = self.get_transformers(config.transformer)
+        self.datasets = {s: FGDataset(config.root_dir, os.path.join(config.meta_dir, s + '.txt'), transform=tf[s])
+                         for s in ('train', 'val')}
+        if config.batch_size % self.world != 0:
+            raise ValueError(f'dataset.batch_size={config.batch_size} must be a multiple of the {self.world} ranks')
+        loaders = {}
+        for s in ('train', 'val'):
+            sampler = None
+            if self.world > 1:
+                from torch.utils.data.distributed import DistributedSampler
+                sampler = DistributedSampler(self.datasets[s], num_replicas=self.world, rank=self.rank, shuffle=s == 'train',
+                                             drop_last=False)
+            self.samplers[s] = sampler
+            loaders[s] = DataLoader(self.datasets[s], config.batch_size // self.world, num_workers=config.num_workers,
+                                    pin_memory=True, sampler=sampler, shuffle=(s == 'train' and sampler is None))
+        return loaders
+
+    def get_criterion(self, config):
+        from .losses import InterpPartsLoss
+        return InterpPartsLoss(config)
+
+    def param_groups(self):
+        named = list(self.get_model_module().named_parameters())
+        return [([p for n, p in named if n.split('.')[0] in self.FINETUNE], 1.0),
+                ([p for n, p in named if n.split('.')[0] not in self.FINETUNE], 20.0)]
+
+    def get_optimizer(self, config):
+        from . import engine
+        lrs = [config.lr * m for g, m in self.param_groups() if any(p.requires_grad for p in g)]
+        return engine.FusedSGD(self.flat, lr=config.lr, momentum=0.9,
+                               weight_decay=config.weight_decay if 'weight_decay' in config else 0.0, group_lrs=lrs)
+
+    def get_scheduler(self, config):
+        iters = len(self.dataloaders['train']) if 'train' in self.dataloaders else 1
+        return _Cosine(self.optimizer, iters * self.total_epoch)
+
+    def after_optimizer_step(self):
+        self.scheduler.step()
+
+    def do_scheduler_step(self):
+        pass
+
+    def batch_validate(self, data):
+        import torch
+        from .train import accuracy
+        images, labels = self.to_device(data['img']), self.to_device(data['label'])
+        with torch.no_grad():
+            pred, _, _ = self.model(images)
+        self.average_meters['acc'].update(accuracy(pred, labels, 1), images.size(0))
+
+
 TRAINERS = {'BCNN': BCNNTrainer, 'CBCNN': CBCNNTrainer, 'MPN': MPNTrainer, 'PeerLearning': PeerLearningTrainer,
             'OSMENet': OSMENetTrainer}
 # TRAINERS keeps the key set it has always had, so code that enumerates it sees no change; the command line dispatches
-# over every method, APINet, DCL and ProtoTreeNet included.
-ALL_TRAINERS = dict(TRAINERS, APINet=APINetTrainer, DCL=DCLTrainer, ProtoTreeNet=ProtoTreeTrainer)
+# over every method, APINet, DCL, ProtoTreeNet and InterpPartsNet included.
+ALL_TRAINERS = dict(TRAINERS, APINet=APINetTrainer, DCL=DCLTrainer, ProtoTreeNet=ProtoTreeTrainer,
+                   InterpPartsNet=InterpPartsNetTrainer)
 
 
 def main(argv=None):

@@ -185,3 +185,67 @@ class ProtoTreeLoss(nn.Module):
         self.last_correct = correct
         self.last = (pred.detach(), info['pa_tensor'].dense, labels)
         return loss
+
+
+class InterpPartsLoss(nn.Module):
+    """model/loss/InterpParts_loss.py: CrossEntropy(logits) + coeff x ShapingLoss(assign) on the (logits, att, assign)
+    triple Interp-Parts returns, with the reference's config keys and defaults (radius 2, std 0.4, num_parts 5, alpha 1,
+    beta 0.001, coeff 0.5).  ``last_correct`` is the top-1 count on the device.
+
+    The Beta prior depends only on (N, alpha, beta): it is computed once per batch size with scipy and kept on the device,
+    so after the first call with a batch size the loss makes no host round trip (the reference recomputes it on the host at
+    every call, because its ``prev_bs`` is never updated).  Under torchrun every rank all-gathers the [N_local, K]
+    occupancies, so that the ranking and the prior cover the global batch, as under the reference's nn.DataParallel, which
+    gathers assign onto one device; the local rows' gradient is then scaled by the world size, which undoes the 1 / world
+    averaging of the gradient all-reduce."""
+
+    def __init__(self, config):
+        super().__init__()
+        from . import ops, ops_interp_parts
+        self.radius = int(config.radius if 'radius' in config else 2)
+        self.std = config.std if 'std' in config else 0.4
+        self.num_parts = config.num_parts if 'num_parts' in config else 5
+        self.alpha = config.alpha if 'alpha' in config else 1
+        self.beta = config.beta if 'beta' in config else 0.001
+        self.coeff = config.coeff if 'coeff' in config else 0.5
+        if self.radius < 0:
+            raise ValueError(f'InterpPartsLoss: radius={self.radius} must be >= 0')
+        ops_interp_parts.check_parts(self.num_parts)
+        self.ce_loss = ops.CrossEntropyLS(0.0)
+        self._taps = ops_interp_parts.gaussian_taps(self.radius, self.std)
+        self._device_taps = {}
+        self._priors = {}
+
+    def prior(self, n, device):
+        """[n] fp32 Beta prior quantiles on ``device``, computed on the host the first time only."""
+        key = (n, self.alpha, self.beta, str(device))
+        if key not in self._priors:
+            from .ops_interp_parts import beta_prior
+            self._priors[key] = beta_prior(n, self.alpha, self.beta).to(device)
+        return self._priors[key]
+
+    def taps(self, device):
+        key = str(device)
+        if key not in self._device_taps:
+            self._device_taps[key] = self._taps.to(device)
+        return self._device_taps[key]
+
+    def shaping_loss(self, assign):
+        from .ops_interp_parts import SHAPING_EPS, ShapingLossFn, occupancy
+        if assign.shape[1] != self.num_parts:
+            raise ValueError(f'InterpPartsLoss: assign has {assign.shape[1]} parts, the criterion num_parts={self.num_parts}')
+        occ, _ = occupancy(assign, self.taps(assign.device), self.radius)
+        occ_all, row0, world = occ.detach(), 0, 1
+        import torch.distributed as dist
+        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+            world = dist.get_world_size()
+            occ_all = torch.empty(world * occ.shape[0], occ.shape[1], device=occ.device, dtype=occ.dtype)
+            dist.all_gather_into_tensor(occ_all, occ.detach().contiguous())
+            row0 = dist.get_rank() * occ.shape[0]
+        return ShapingLossFn.apply(occ, occ_all, self.prior(occ_all.shape[0], occ.device), row0, world, SHAPING_EPS)
+
+    def forward(self, output, target):
+        logits, att, assign = output
+        loss_ce = self.ce_loss(logits, target)
+        self.last_correct = self.ce_loss.last_correct
+        return loss_ce + self.coeff * self.shaping_loss(assign)

@@ -7,3 +7,4 @@ from .osme import OSMENet, OSME, OSME_block  # noqa: F401
 from .apinet import APINet  # noqa: F401
 from .dcl import DCL  # noqa: F401
 from .prototree import ProtoTreeNet  # noqa: F401
+from .interp_parts import IP_ResNet50, IP_ResNet101  # noqa: F401

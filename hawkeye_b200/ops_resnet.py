@@ -143,22 +143,70 @@ def _add(a, b):
     return a
 
 
+def block_units(blk):
+    """(u1, u2, u3, ds) units of one bottleneck block: ResNet's Bottleneck (3x3 middle conv, v1.5 stride on it) or a
+    Bottleneck1x1 (Interp_Parts.py:212-248, every conv 1x1); the middle unit's kind follows ``conv2.kernel_size``."""
+    s2 = blk.stride == 2
+    mid = ('3x3s2' if s2 else '3x3') if tuple(blk.conv2.kernel_size) == (3, 3) else ('1x1s2' if s2 else '1x1')
+    ds = None
+    if blk.downsample is not None:
+        ds = Unit('1x1s2' if s2 else '1x1', blk.downsample[0], blk.downsample[1], False)
+    return (Unit('1x1', blk.conv1, blk.bn1, True), Unit(mid, blk.conv2, blk.bn2, True), Unit('1x1', blk.conv3, blk.bn3, True),
+            ds)
+
+
+def block_params(blocks):
+    return [p for b in blocks for u in b if u is not None for p in u.params()]
+
+
+def blocks_forward(cur, blocks, pget, save, training):
+    """NHWC [N, H, W, C] through the bottleneck blocks -> (NHWC output, per-block records for blocks_backward).
+    ``pget()`` yields each unit's (weight, gamma, beta) in the order of ``block_params``."""
+    recs = []
+    for (u1, u2, u3, ds) in blocks:
+        w, g, b = pget()
+        a1, r1 = u1.forward(cur, w, g, b, None, save, training)
+        w, g, b = pget()
+        a2, r2 = u2.forward(a1, w, g, b, None, save, training)
+        w3, g3, b3 = pget()
+        rd = None
+        identity = cur
+        if ds is not None:
+            w, g, b = pget()
+            identity, rd = ds.forward(cur, w, g, b, None, save, training)
+        out, r3 = u3.forward(a2, w3, g3, b3, identity, save, training)
+        recs.append((r1, r2, r3, rd))
+        cur = out
+    return cur, recs
+
+
+def blocks_backward(g, blocks, recs):
+    """NHWC output gradient -> (NHWC input gradient, [(dw, dgamma, dbeta)] in the order of ``block_params``)."""
+    grads = []   # collected in reverse unit order, each (dw, dgamma, dbeta)
+    for (u1, u2, u3, ds), (r1, r2, r3, rd) in zip(reversed(blocks), reversed(recs)):
+        d2, dres, dw3, dg3, db3 = u3.backward(r3, g)
+        d1, _, dw2, dg2, db2 = u2.backward(r2, d2)
+        # the identity branch's gradient (dres, or the downsample unit's dx) is added inside u1's dgrad GEMM epilogue
+        extra = None
+        if ds is not None:
+            dxd, _, dwd, dgd, dbd = ds.backward(rd, dres)
+            extra = (dwd, dgd, dbd)
+        dx, _, dw1, dg1, db1 = u1.backward(r1, d1, addend=dxd if ds is not None else dres)
+        blk = [(dw1, dg1, db1), (dw2, dg2, db2), (dw3, dg3, db3)]
+        if extra is not None:
+            blk.append(extra)
+        grads = blk + grads
+        g = dx
+    return g, grads
+
+
 class TrunkPlan:
-    """Flattened description of a ResNet trunk module: stem unit, max-pool, list of bottleneck blocks."""
+    """Flattened description of a ResNet trunk: stem unit, max-pool, list of bottleneck blocks.  ``trunk`` is indexable as
+    conv1, bn1, relu, maxpool, then the layers (a ResNetTrunk, or the same modules in a list)."""
 
     def __init__(self, trunk):
         self.stem = Unit('stem', trunk[0], trunk[1], True)
-        self.blocks = []
-        for layer in list(trunk)[4:]:
-            for blk in layer:
-                s2 = blk.stride == 2
-                u1 = Unit('1x1', blk.conv1, blk.bn1, True)
-                u2 = Unit('3x3s2' if s2 else '3x3', blk.conv2, blk.bn2, True)
-                u3 = Unit('1x1', blk.conv3, blk.bn3, True)
-                ds = None
-                if blk.downsample is not None:
-                    ds = Unit('1x1s2' if s2 else '1x1', blk.downsample[0], blk.downsample[1], False)
-                self.blocks.append((u1, u2, u3, ds))
+        self.blocks = [block_units(blk) for layer in list(trunk)[4:] for blk in layer]
 
     def units(self):
         us = [self.stem]
@@ -170,17 +218,21 @@ class TrunkPlan:
         return [p for u in self.units() for p in u.params()]
 
 
+def _param_iter(params):
+    it = iter(range(0, len(params), 3))
+    return lambda: (lambda i: (_f32c(params[i]), params[i + 1], params[i + 2]))(next(it))
+
+
 class ResNetTrunkFn(Function):
-    """NCHW image -> NCHW feature map [N, 2048, H/32, W/32]."""
+    """NCHW image -> NCHW feature map [N, 2048, H/32, W/32]; with ``nhwc`` the NHWC map [N, H/32, W/32, 2048] as the last
+    block writes it (and its gradient arrives in NHWC)."""
 
     @staticmethod
-    def forward(ctx, x, plan, save, training, *params):
+    def forward(ctx, x, plan, save, training, nhwc, *params):
         _check_cuda(x)
         x = _f32c(x)
         s = _lib.stream_ptr()
-        it = iter(range(0, len(params), 3))
-        pget = lambda: (lambda i: (_f32c(params[i]), params[i + 1], params[i + 2]))(next(it))
-        recs = []
+        pget = _param_iter(params)
         w, g, b = pget()
         y, r = plan.stem.forward(x, w, g, b, None, save, training)
         N, H, W, C = y.shape
@@ -190,48 +242,19 @@ class ResNetTrunkFn(Function):
         _lib.call('hk_maxpool3x3s2_fwd', y, p, am, N, H, W, C, s)
         if _ops.CAPTURE is not None:
             _ops.CAPTURE.append(('pool3', am, (N, H, W, C)))
-        recs.append(('stem', r, (tuple(y.shape), am) if save else None))
-        cur = p
-        for (u1, u2, u3, ds) in plan.blocks:
-            w, g, b = pget()
-            a1, r1 = u1.forward(cur, w, g, b, None, save, training)
-            w, g, b = pget()
-            a2, r2 = u2.forward(a1, w, g, b, None, save, training)
-            w3, g3, b3 = pget()
-            rd = None
-            identity = cur
-            if ds is not None:
-                w, g, b = pget()
-                identity, rd = ds.forward(cur, w, g, b, None, save, training)
-            out, r3 = u3.forward(a2, w3, g3, b3, identity, save, training)
-            recs.append(('block', (r1, r2, r3, rd), None))
-            cur = out
-        ctx.plan, ctx.recs, ctx.nparams = plan, (recs if save else None), len(params)
-        return nhwc_to_nchw(cur)
+        cur, brecs = blocks_forward(p, plan.blocks, pget, save, training)
+        ctx.plan, ctx.nparams, ctx.nhwc = plan, len(params), nhwc
+        ctx.recs = ((r, tuple(y.shape), am), brecs) if save else None
+        return cur if nhwc else nhwc_to_nchw(cur)
 
     @staticmethod
     def backward(ctx, dfeat):
         if ctx.recs is None:
-            return (None,) * (4 + ctx.nparams)
-        plan, recs = ctx.plan, ctx.recs
+            return (None,) * (5 + ctx.nparams)
+        plan, ((r0, yshape, am), brecs) = ctx.plan, ctx.recs
         s = _lib.stream_ptr()
-        g = nchw_to_nhwc(_f32c(dfeat))
-        grads = []   # collected in reverse unit order, each (dw, dgamma, dbeta)
-        for (u1, u2, u3, ds), (_, (r1, r2, r3, rd), _) in zip(reversed(plan.blocks), reversed(recs[1:])):
-            d2, dres, dw3, dg3, db3 = u3.backward(r3, g)
-            d1, _, dw2, dg2, db2 = u2.backward(r2, d2)
-            # the identity branch's gradient (dres, or the downsample unit's dx) is added inside u1's dgrad GEMM epilogue
-            extra = None
-            if ds is not None:
-                dxd, _, dwd, dgd, dbd = ds.backward(rd, dres)
-                extra = (dwd, dgd, dbd)
-            dx, _, dw1, dg1, db1 = u1.backward(r1, d1, addend=dxd if ds is not None else dres)
-            blk = [(dw1, dg1, db1), (dw2, dg2, db2), (dw3, dg3, db3)]
-            if extra is not None:
-                blk.append(extra)
-            grads = blk + grads
-            g = dx
-        _, r0, (yshape, am) = recs[0]
+        g = _f32c(dfeat) if ctx.nhwc else nchw_to_nhwc(_f32c(dfeat))
+        g, grads = blocks_backward(g, plan.blocks, brecs)
         N, H, W, C = yshape
         dy0 = torch.empty(N, H, W, C, device=dfeat.device, dtype=torch.float32)
         _lib.call('hk_maxpool3x3s2_bwd', am, g, dy0, N, H, W, C, s)
@@ -239,7 +262,33 @@ class ResNetTrunkFn(Function):
         grads = [(dw0, dg0, db0)] + grads
         ctx.recs = None
         flat = [t for trip in grads for t in trip]
-        return (None, None, None, None) + tuple(flat)
+        return (None, None, None, None, None) + tuple(flat)
+
+
+class BlockStackFn(Function):
+    """NHWC map [N, H, W, C] through a stack of bottleneck blocks (Interp-Parts' post_block and the Bottleneck1x1 pair of
+    attconv, on P = N*K rows of 1x1 maps) -> NHWC output."""
+
+    @staticmethod
+    def forward(ctx, x, blocks, save, training, *params):
+        _check_cuda(x)
+        out, recs = blocks_forward(_f32c(x), blocks, _param_iter(params), save, training)
+        ctx.blocks, ctx.nparams, ctx.recs = blocks, len(params), (recs if save else None)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        if ctx.recs is None:
+            return (None,) * (4 + ctx.nparams)
+        dx, grads = blocks_backward(_f32c(dout), ctx.blocks, ctx.recs)
+        ctx.recs = None
+        return (dx, None, None, None) + tuple(t for trip in grads for t in trip)
+
+
+def block_stack(x, blocks, training):
+    """x NHWC through ``blocks`` (a list of block_units) with the units' own parameters."""
+    params = block_params(blocks)
+    return BlockStackFn.apply(x, blocks, _ops.wants_grad(x, params), training, *params)
 
 
 def resnet_trunk(x, trunk_module):
@@ -247,7 +296,13 @@ def resnet_trunk(x, trunk_module):
     params = plan.params()
     training = trunk_module.training
     save = _ops.wants_grad(x, params)
-    return ResNetTrunkFn.apply(x, plan, save, training, *params)
+    return ResNetTrunkFn.apply(x, plan, save, training, False, *params)
+
+
+def resnet_trunk_nhwc(x, plan, training):
+    """The trunk of ``plan`` on an NCHW image -> its NHWC output map, without the NCHW transpose."""
+    params = plan.params()
+    return ResNetTrunkFn.apply(x, plan, _ops.wants_grad(x, params), training, True, *params)
 
 
 class DRBlockFn(Function):

@@ -108,6 +108,8 @@ class Tester:
         logits = self.model(images)
         if isinstance(logits, tuple) and isinstance(logits[1], dict):   # ProtoTreeNet returns (pred, info)
             logits = logits[0]
+        if isinstance(logits, tuple) and len(logits) == 3 and logits[1].dim() == 4:   # Interp-Parts: (logits, att, assign)
+            logits = logits[0]
         if isinstance(logits, tuple):                            # PeerLearningNet returns both heads (PeerLearning.py:94-101)
             self.average_meters['acc'].update(max(accuracy(l, labels, 1) for l in logits), images.size(0))
         else:

@@ -325,6 +325,58 @@ int hk_prototree_leaf_update_sum(const float* theta, const float* pa, const floa
 int hk_prototree_leaf_update_apply(float* theta, const float* theta0, const float* update, int height, int K,
                                    float num_batches, void* stream);
 
+/* ---- Interp-Parts: model/methods/Interp_Parts.py, model/loss/InterpParts_loss.py --------------------------------------
+ * hk_ip_group_fwd (GroupingUnit.forward, Interp_Parts.py:56-122): trunk map x [N,HW,C] (NHWC, as the trunk produces it),
+ *   centres [K,C] (the grouping weight [K,C,1,1]), smooth [K] -> with beta = sigmoid(smooth):
+ *   dist [N,K,HW] = sum_c (x - c_k)^2, summed directly in fp32 in both precision modes (the reference's 2 c.x - |x|^2 - |c|^2
+ *   cancels; a direct sum is never positive after the negation, so the reference's clamp(max=0) is the identity here);
+ *   assign [N,K,HW] = softmax over k of -dist / beta; qx [N,K,C] = sum_p assign x; ssum [N,K] = sum_p assign;
+ *   u = (qx / max(ssum, 1e-5) - c_k) / sqrt(beta / 2); nrm [N,K] = |u|; out [N,K,C] = u / max(|u|, 1e-12) (F.normalize over
+ *   C; the NHWC [N,K,1,C] input of the 1x1 stacks; rounded to tf32 in the default mode, it is the next GEMM's operand).  One
+ *   read of the map: partials per 32-pixel tile go to the workspace (hk_ip_group_workspace_bytes, serves both directions)
+ *   and a second launch folds them in tile order.  1 <= K <= 32; C % 4 == 0 and C <= 1536; x 16-byte aligned.
+ *   Replaces :67-122 (the bmm's, x_sq, the expanded c_sq and beta, the permuted x).
+ * hk_ip_group_bwd: dout [N,K,C] -> dx [N,HW,C], dcentres [K,C], dsmooth [K] (through 1/beta in the softmax and through
+ *   sqrt(beta / 2)).  The clamps' zero-gradient regions are honoured: no gradient through ssum where ssum < 1e-5, and
+ *   dout / 1e-12 where |u| < 1e-12.  dassign (optional, [N,K,HW]) is a dense gradient of assign.  The shaping loss's gradient
+ *   arrives as argmax [N,K] (hk_ip_occupancy) and coef [N,K] (optional): coef times the Gaussian taps gauss [(2r+1)^2] is added
+ *   to d assign on the window under each blurred maximum, inside the same pass (no dense d assign).  One read of the map, one
+ *   write of dx; every sum in a fixed order.
+ * hk_ip_att_fwd (attconv[2:5] + softmax + pooling, :289-291,:349-361): f [P,C] (P = N K rows of the attconv stack output),
+ *   1-channel conv w [C], b [1]; BatchNorm(1) gamma, beta [1] over the P values (training: batch statistics, running_mean /
+ *   running_var updated with momentum and the unbiased variance, as hk_bn_fwd does; else the running statistics); ReLU;
+ *   att [N,K] = softmax over the K parts; pooled [N,D] = sum_k att post[n,k,:] with post [P,D] the post_block output
+ *   (avg_pool1d(K) * K).  conv [P] and stats [2] = (mean, invstd) are saved for the backward.  Training needs P > 1.
+ * hk_ip_att_bwd: dpooled [N,D] and datt (optional, [N,K]) -> df [P,C], dw [C], db [1], dgamma [1], dbeta [1], dpost [P,D];
+ *   scratch [P] floats.
+ * hk_ip_occupancy (ShapingLoss steps 1-2, InterpParts_loss.py:114-124): assign [N,K,H,W], gauss [(2r+1)^2] (the normalised
+ *   Gaussian; [1.0] for radius 0) -> occ [N,K] = max of the "valid" depthwise blur, argmax [N,K] int32 = its position in the
+ *   (H - 2r) x (W - 2r) blurred map, the first maximum in row-major order on ties.  2r < H and 2r < W.
+ * hk_ip_shaping_loss (:125-138): occ [R,K] (R = the global batch), prior [R] (the Beta prior's quantiles, on the device) ->
+ *   loss[0] = mean over (i, k) of |log(occ + eps) - log(prior[rank] + eps)|, rank = the place of occ[i,k] in the ascending
+ *   sort of its column (ties by row index); docc [R,K] = its gradient (sign(0) = 0, as torch's abs). */
+size_t hk_ip_group_workspace_bytes(int N, int HW, int K, int C);
+int hk_ip_group_fwd(const float* x, const float* centres, const float* smooth, float* assign, float* dist, float* out,
+                    float* qx, float* ssum, float* nrm, int N, int HW, int K, int C, void* workspace,
+                    size_t workspace_bytes, void* stream);
+int hk_ip_group_bwd(const float* x, const float* centres, const float* smooth, const float* assign, const float* dist,
+                    const float* qx, const float* ssum, const float* nrm, const float* dout, const float* dassign,
+                    const int* argmax, const float* coef, const float* gauss, int radius, float* dx, float* dcentres,
+                    float* dsmooth, int N, int H, int W, int K, int C, void* workspace, size_t workspace_bytes,
+                    void* stream);
+int hk_ip_att_fwd(const float* f, const float* w, const float* b, const float* gamma, const float* beta,
+                  float* running_mean, float* running_var, float momentum, float eps, int training, const float* post,
+                  float* conv, float* att, float* stats, float* pooled, int N, int K, int C, int D, void* stream);
+int hk_ip_att_bwd(const float* f, const float* w, const float* gamma, const float* beta, const float* conv,
+                  const float* att, const float* stats, const float* post, const float* dpooled, const float* datt,
+                  int training, float* df,
+                  float* dw, float* db, float* dgamma, float* dbeta, float* dpost, float* scratch, int N, int K, int C,
+                  int D, void* stream);
+int hk_ip_occupancy(const float* assign, const float* gauss, float* occ, int* argmax, int N, int K, int H, int W,
+                    int radius, void* stream);
+int hk_ip_shaping_loss(const float* occ, const float* prior, float* loss, float* docc, int R, int K, float eps,
+                       void* stream);
+
 /* ---- classifier nn.Linear (BCNN.py:42, CBCNN.py:26, MPNCOV.py:31) as skinny wgmma GEMMs ------------------- */
 size_t hk_linear_fwd_workspace_bytes(int B, int F, int N);
 int hk_linear_fwd(const float* x, const float* w, const float* bias, float* y, int B, int F, int N, void* workspace,
