@@ -1,6 +1,6 @@
 """Trainer subclasses of the hot-path methods with the reference's Examples/ surface:
-``python -m hawkeye_b200.examples {BCNN,CBCNN,MPN,PeerLearning,OSMENet,APINet,DCL,ProtoTreeNet,InterpPartsNet} --config
-<yaml>`` replaces
+``python -m hawkeye_b200.examples {BCNN,CBCNN,MPN,PeerLearning,OSMENet,APINet,DCL,ProtoTreeNet,InterpPartsNet,NTSNet}
+--config <yaml>`` replaces
 ``python Examples/<Method>.py --config <yaml>`` (same yaml files; one process per GPU under torchrun instead of nn.DataParallel).
 
 Only what the reference's Examples override is overridden here: which parameters train, with which learning rates, and
@@ -430,12 +430,34 @@ class InterpPartsNetTrainer(Trainer):
         self.average_meters['acc'].update(accuracy(pred, labels, 1), images.size(0))
 
 
+class NTSNetTrainer(Trainer):
+    """Examples/NTSNet.py: criterion = NTSLoss on the model's five outputs; Adam over all parameters with lr and
+    weight_decay (the base Trainer's); LinearLR(lr_warmup_decay, warmup_epochs) into CosineAnnealingLR(T_max -
+    warmup_epochs) through SequentialLR, stepped once per epoch.  Training and validation accuracy are top-1 on
+    concat_logits; the training step has no host synchronisation, so ``cuda_graph: true`` captures and replays it."""
+
+    def get_criterion(self, config):
+        from .losses import NTSLoss
+        return NTSLoss(config)
+
+    def get_scheduler(self, config):
+        return _warmup_cosine(self.optimizer, config, self.total_epoch)
+
+    def batch_validate(self, data):
+        import torch
+        from .train import accuracy
+        images, labels = self.to_device(data['img']), self.to_device(data['label'])
+        with torch.no_grad():
+            concat_logits = self.model(images)[1]
+        self.average_meters['acc'].update(accuracy(concat_logits, labels, 1), images.size(0))
+
+
 TRAINERS = {'BCNN': BCNNTrainer, 'CBCNN': CBCNNTrainer, 'MPN': MPNTrainer, 'PeerLearning': PeerLearningTrainer,
             'OSMENet': OSMENetTrainer}
 # TRAINERS keeps the key set it has always had, so code that enumerates it sees no change; the command line dispatches
-# over every method, APINet, DCL, ProtoTreeNet and InterpPartsNet included.
+# over every method, APINet, DCL, ProtoTreeNet, InterpPartsNet and NTSNet included.
 ALL_TRAINERS = dict(TRAINERS, APINet=APINetTrainer, DCL=DCLTrainer, ProtoTreeNet=ProtoTreeTrainer,
-                   InterpPartsNet=InterpPartsNetTrainer)
+                   InterpPartsNet=InterpPartsNetTrainer, NTSNet=NTSNetTrainer)
 
 
 def main(argv=None):

@@ -187,6 +187,36 @@ class ProtoTreeLoss(nn.Module):
         return loss
 
 
+class NTSLoss(nn.Module):
+    """model/loss/NTS_loss.py: CE(raw_logits) + CE(concat_logits) + CE over the B*T part rows (each with label smoothing 0.1
+    and its own mean) + ranking_loss(top_n_prob, list_loss(part_logits)) on the list NTSNet returns.  The cross-entropies
+    run on hk_softmax_ce_ls, the list and ranking losses in one hk_nts_rank_loss launch with no per-row read-back (the
+    reference reads every label to the host in list_loss).  ``last_correct`` is the top-1 count on concat_logits, the
+    accuracy Examples/NTSNet.py reports.
+
+    Under torchrun each rank runs on its own B_local images: with equal shards, the per-rank means and the ranking sum over
+    B_local, averaged by the gradient all-reduce, are the objective the reference optimises under nn.DataParallel."""
+
+    def __init__(self, config):
+        super().__init__()
+        from . import ops
+        self.PROPOSAL_NUM = int(config.proposal_num)
+        self.raw_ce, self.concat_ce, self.part_ce = (ops.CrossEntropyLS(0.1) for _ in range(3))
+
+    def forward(self, outputs, targets):
+        from .ops_nts import RankLossFn
+        raw_logits, concat_logits, part_logits, _, top_n_prob = outputs
+        B, T = targets.shape[0], self.PROPOSAL_NUM
+        if top_n_prob.shape != (B, T):
+            raise ValueError(f'NTSLoss: top_n_prob {tuple(top_n_prob.shape)}, expected ({B}, {T}) (criterion proposal_num)')
+        part_rows = part_logits.reshape(B * T, -1)
+        part_targets = targets.repeat_interleave(T)
+        loss = self.raw_ce(raw_logits, targets) + RankLossFn.apply(part_rows, targets, top_n_prob)
+        loss = loss + self.concat_ce(concat_logits, targets) + self.part_ce(part_rows, part_targets)
+        self.last_correct = self.concat_ce.last_correct
+        return loss
+
+
 class InterpPartsLoss(nn.Module):
     """model/loss/InterpParts_loss.py: CrossEntropy(logits) + coeff x ShapingLoss(assign) on the (logits, att, assign)
     triple Interp-Parts returns, with the reference's config keys and defaults (radius 2, std 0.4, num_parts 5, alpha 1,

@@ -8,3 +8,4 @@ from .apinet import APINet  # noqa: F401
 from .dcl import DCL  # noqa: F401
 from .prototree import ProtoTreeNet  # noqa: F401
 from .interp_parts import IP_ResNet50, IP_ResNet101  # noqa: F401
+from .nts import NTSNet  # noqa: F401

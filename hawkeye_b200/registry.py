@@ -16,7 +16,8 @@ BACKBONE = Repository()
 
 def install_into(model_registry, names=('BCNN', 'CBCNN', 'MPN', 'CIN', 'PeerLearningNet'), backbone_registry=None):
     """Drop-in: overwrite the reference's own ``model.registry.MODEL`` entries with the H100-native classes,
-    so an unmodified Hawkeye ``Trainer`` (train.py:158-169) builds them via ``MODEL.get(name)(config)``."""
+    so an unmodified Hawkeye ``Trainer`` (train.py:158-169) builds them via ``MODEL.get(name)(config)``.  Any registered
+    name may be listed (``'APINet'``, ``'DCL'``, ``'NTSNet'``, ...)."""
     for n in names:
         if n in MODEL:
             dict.__setitem__(model_registry, n, MODEL[n])

@@ -377,6 +377,43 @@ int hk_ip_occupancy(const float* assign, const float* gauss, float* occ, int* ar
 int hk_ip_shaping_loss(const float* occ, const float* prior, float* loss, float* docc, int R, int K, float eps,
                        void* stream);
 
+/* ---- NTS-Net: model/methods/NTS_Net/NTSNet.py, anchors.py, model/loss/NTS_loss.py --------------------------------------
+ * The proposal net's maps d1 [B,H1,W1,C], d2 [B,H2,W2,C], d3 [B,H3,W3,C] (NHWC ReLU outputs of down1..3, H2 = ceil(H1 / 2),
+ * H3 = ceil(H2 / 2), likewise W) feed three 1x1 tidy convs with 6, 6 and 9 outputs.  Score a of an image is tidy_k channel ch
+ * at position p with a = off_k + ch H_k W_k + p, off = (0, 6 H1 W1, 6 H1 W1 + 6 H2 W2): the reference's channel-major
+ * flatten and concatenation (NTSNet.py:79-82), A = hk_nts_num_anchors(H1, W1) scores, which is also the anchor order.
+ * hk_nts_score_fwd (ProposalNet tidy1..3, :79-82): w_k [A_k,C] (the tidy weight [A_k,C,1,1]), b_k [A_k] -> score [B,A] in one
+ *   launch; one warp per score, fixed-order sums.
+ * hk_nts_score_bwd: the sparse gradient of top_n_prob = gather(score, idx) (:42), dprob [B,T] at idx int64 [B,T] ->
+ *   g_k [B,H_k,W_k,C] = (d_k > 0) (d score / d d_k): the gradient at down_k's pre-activation from the tidy path; dw_k [A_k,C],
+ *   db_k [A_k].  Only the T kept scores of an image are read; an index outside [0, A) is skipped.  Fixed-order sums.
+ * hk_nts_nms (hard_nms, anchors.py:63-90, per image, :35-42): scores [B,A], anchors int32 [A,4] = (y0, x0, y1, x1) ->
+ *   idx int64 [B,T], prob [B,T] = scores at idx, boxes int32 [B,T,4] = anchors at idx.  Greedy: the highest-scoring alive
+ *   candidate is kept, then every alive candidate whose IoU with it is >= 0.25 is dropped, the IoU tested exactly on the
+ *   integer boxes as 4 inter >= union (inter = 0 when either overlap extent is negative).  Equal scores go to the lower
+ *   index (the reference's np.argsort leaves that order undefined).  A row with fewer than T survivors gets idx -1, prob 0
+ *   and box (0, 0, 1, 1) past its last survivor.  One block per image; A <= 2048; anchors and boxes 16-byte aligned.
+ * hk_nts_crop (:43-49): img NCHW [B,C,H,W], boxes int32 [B*T,4] in the coordinates of the image zero-padded by pad on every
+ *   side -> out NCHW [B*T,C,S,S] = F.interpolate(padded[n, :, y0:y1, x0:x1], (S, S), bilinear, align_corners=True) with
+ *   ATen's upsample_bilinear2d arithmetic.  Pixels outside the image read as zero; no padded copy is made.  B T <= 65535.
+ * hk_nts_rank_loss (list_loss + ranking_loss, NTS_loss.py:32-47): part_logits [B*T,K] (row n T + t), labels int64 [B],
+ *   prob [B,T] -> L[n,t] = logsumexp - z[y_n] in fp32; ADDS sum_n sum_i sum_j relu(1 - prob[n,i] + prob[n,j]) [L[n,j] > L[n,i]]
+ *   / B to the fp64 accumulator loss_acc[0] and writes dprob [B,T] (no gradient through L; none at the hinge).  B T <= 8192. */
+int hk_nts_num_anchors(int H1, int W1);
+int hk_nts_score_fwd(const float* d1, const float* d2, const float* d3, const float* w1, const float* b1, const float* w2,
+                     const float* b2, const float* w3, const float* b3, float* score, int B, int H1, int W1, int H2, int W2,
+                     int H3, int W3, int C, void* stream);
+int hk_nts_score_bwd(const float* d1, const float* d2, const float* d3, const float* w1, const float* w2, const float* w3,
+                     const long long* idx, const float* dprob, float* g1, float* g2, float* g3, float* dw1, float* db1,
+                     float* dw2, float* db2, float* dw3, float* db3, int B, int T, int H1, int W1, int H2, int W2, int H3,
+                     int W3, int C, void* stream);
+int hk_nts_nms(const float* scores, const int* anchors, long long* idx, float* prob, int* boxes, int B, int A, int T,
+               void* stream);
+int hk_nts_crop(const float* img, const int* boxes, float* out, int B, int T, int C, int H, int W, int pad, int S,
+                void* stream);
+int hk_nts_rank_loss(const float* part_logits, const long long* labels, const float* prob, double* loss_acc, float* dprob,
+                     int B, int T, int K, void* stream);
+
 /* ---- classifier nn.Linear (BCNN.py:42, CBCNN.py:26, MPNCOV.py:31) as skinny wgmma GEMMs ------------------- */
 size_t hk_linear_fwd_workspace_bytes(int B, int F, int N);
 int hk_linear_fwd(const float* x, const float* w, const float* bias, float* y, int B, int F, int N, void* workspace,
