@@ -1,5 +1,5 @@
 """Trainer subclasses of the hot-path methods with the reference's Examples/ surface:
-``python -m hawkeye_b200.examples {BCNN,CBCNN,MPN,PeerLearning,OSMENet,APINet,DCL,ProtoTreeNet,InterpPartsNet,NTSNet}
+``python -m hawkeye_b200.examples {BCNN,CBCNN,MPN,PeerLearning,OSMENet,APINet,DCL,ProtoTreeNet,InterpPartsNet,NTSNet,APCNN}
 --config <yaml>`` replaces
 ``python Examples/<Method>.py --config <yaml>`` (same yaml files; one process per GPU under torchrun instead of nn.DataParallel).
 
@@ -452,12 +452,92 @@ class NTSNetTrainer(Trainer):
         self.average_meters['acc'].update(accuracy(concat_logits, labels, 1), images.size(0))
 
 
+class _EpochCosine:
+    """Examples/APCNN.py:69-81: lr(epoch) = lr / 2 (cos(pi (epoch % E) / E) + 1) on every group's initial lr, set at the start
+    of each epoch; there is no other scheduler."""
+
+    def __init__(self, opt, epochs):
+        self.opt, self.E = opt, epochs
+
+    def set_epoch(self, epoch):
+        import math
+        for g in self.opt.param_groups:
+            g['lr'] = float(g['initial_lr'] / 2 * (math.cos(math.pi * (epoch % self.E) / self.E) + 1))
+
+    def state_dict(self):
+        return {}
+
+    def load_state_dict(self, sd):
+        pass
+
+
+class APCNNTrainer(Trainer):
+    """Examples/APCNN.py: the reference's transforms (TrivialAugmentWide in training); criterion = APCNNLoss (the sum of the
+    eight cross-entropies); SGD with momentum 0.9 and weight_decay in two groups, conv1..layer3 at lr / 10 and layer4 with
+    everything after it at lr (the reference's children()[:7] / [7:]); the cosine of the epoch set in on_start_epoch.
+    Training and validation accuracy are top-1 on out_mean; validation runs both stages in eval mode (no drop block).  The
+    step has no host synchronisation, so ``cuda_graph: true`` captures and replays it."""
+
+    EARLY = ('conv1', 'bn1', 'layer1', 'layer2', 'layer3')
+
+    def get_transformers(self, config):
+        """Examples/APCNN.py:18-34."""
+        from torchvision.transforms import autoaugment, transforms
+        from torchvision.transforms.functional import InterpolationMode
+        norm = transforms.Normalize([0.485, 0.456, 0.406], [0.229, 0.224, 0.225])
+        return {
+            'train': transforms.Compose([transforms.Resize((config.resize_size, config.resize_size)),
+                                         transforms.RandomCrop(config.image_size), transforms.RandomHorizontalFlip(),
+                                         autoaugment.TrivialAugmentWide(interpolation=InterpolationMode.BILINEAR),
+                                         transforms.ToTensor(), norm]),
+            'val': transforms.Compose([transforms.Resize((config.resize_size, config.resize_size)),
+                                       transforms.CenterCrop(config.image_size), transforms.ToTensor(), norm]),
+        }
+
+    get_dataloader = InterpPartsNetTrainer.get_dataloader        # the base datasets and rank sharding with the transforms above
+
+    def get_criterion(self, config):
+        from .losses import APCNNLoss
+        return APCNNLoss(config)
+
+    def param_groups(self):
+        named = list(self.get_model_module().named_parameters())
+        return [([p for n, p in named if n.split('.')[0] in self.EARLY], 0.1),
+                ([p for n, p in named if n.split('.')[0] not in self.EARLY], 1.0)]
+
+    def get_optimizer(self, config):
+        from . import engine
+        lrs = [config.lr * m for g, m in self.param_groups() if any(p.requires_grad for p in g)]
+        return engine.FusedSGD(self.flat, lr=config.lr, momentum=0.9,
+                               weight_decay=config.weight_decay if 'weight_decay' in config else 0.0, group_lrs=lrs)
+
+    def get_scheduler(self, config):
+        return _EpochCosine(self.optimizer, self.total_epoch)
+
+    def on_start_epoch(self, config):
+        self.scheduler.set_epoch(self.epoch)
+
+    def do_scheduler_step(self):
+        pass
+
+    def forward_model(self, images, labels):
+        return self.model(images, labels)
+
+    def batch_validate(self, data):
+        import torch
+        from .train import accuracy
+        images, labels = self.to_device(data['img']), self.to_device(data['label'])
+        with torch.no_grad():
+            out_mean = self.model(images, labels)[0]
+        self.average_meters['acc'].update(accuracy(out_mean, labels, 1), images.size(0))
+
+
 TRAINERS = {'BCNN': BCNNTrainer, 'CBCNN': CBCNNTrainer, 'MPN': MPNTrainer, 'PeerLearning': PeerLearningTrainer,
             'OSMENet': OSMENetTrainer}
 # TRAINERS keeps the key set it has always had, so code that enumerates it sees no change; the command line dispatches
-# over every method, APINet, DCL, ProtoTreeNet, InterpPartsNet and NTSNet included.
+# over every method, APINet, DCL, ProtoTreeNet, InterpPartsNet, NTSNet and APCNN included.
 ALL_TRAINERS = dict(TRAINERS, APINet=APINetTrainer, DCL=DCLTrainer, ProtoTreeNet=ProtoTreeTrainer,
-                   InterpPartsNet=InterpPartsNetTrainer, NTSNet=NTSNetTrainer)
+                   InterpPartsNet=InterpPartsNetTrainer, NTSNet=NTSNetTrainer, APCNN=APCNNTrainer)
 
 
 def main(argv=None):

@@ -217,6 +217,25 @@ class NTSLoss(nn.Module):
         return loss
 
 
+class APCNNLoss(nn.Module):
+    """Examples/APCNN.py:49: the sum of the base criterion (cross-entropy with label smoothing 0.1, train.py:211-212) over the
+    eight logit tensors of the 4-tuple APCNN returns, as one hk_softmax_ce_ls launch over the stacked [8N, K] rows: its mean
+    over 8N rows times 8 is the sum of the eight means.  ``last_correct`` is the top-1 count on ``out_mean``, the accuracy
+    Examples/APCNN.py reports, from the same kernel without a gradient."""
+
+    def __init__(self, config=None):
+        super().__init__()
+        self.label_smoothing = 0.1
+
+    def forward(self, outputs, targets):
+        from .ops import CrossEntropyLSFn
+        out_mean, out_list = outputs[0], outputs[1]
+        loss, _ = CrossEntropyLSFn.apply(torch.cat(out_list, dim=0), targets.repeat(len(out_list)), self.label_smoothing)
+        with torch.no_grad():
+            _, self.last_correct = CrossEntropyLSFn.apply(out_mean.detach(), targets, self.label_smoothing)
+        return loss * float(len(out_list))
+
+
 class InterpPartsLoss(nn.Module):
     """model/loss/InterpParts_loss.py: CrossEntropy(logits) + coeff x ShapingLoss(assign) on the (logits, att, assign)
     triple Interp-Parts returns, with the reference's config keys and defaults (radius 2, std 0.4, num_parts 5, alpha 1,

@@ -112,6 +112,8 @@ class Tester:
             logits = logits[0]
         if isinstance(logits, list) and len(logits) == 5:        # NTSNet's five outputs: accuracy on concat_logits
             logits = logits[1]
+        if isinstance(logits, tuple) and len(logits) == 4 and isinstance(logits[1], list):   # APCNN: accuracy on out_mean
+            logits = logits[0]
         if isinstance(logits, tuple):                            # PeerLearningNet returns both heads (PeerLearning.py:94-101)
             self.average_meters['acc'].update(max(accuracy(l, labels, 1) for l in logits), images.size(0))
         else:

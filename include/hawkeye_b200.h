@@ -414,6 +414,59 @@ int hk_nts_crop(const float* img, const int* boxes, float* out, int B, int T, in
 int hk_nts_rank_loss(const float* part_logits, const long long* labels, const float* prob, double* loss_acc, float* dprob,
                      int B, int T, int K, void* stream);
 
+/* ---- AP-CNN (model/methods/APCNN.py): feature pyramid, pyramid attention, ROI selection, ROI-guided refinement ------------
+ * All maps NHWC fp32, 16-byte aligned; every sum in a fixed order (no atomics), so results are bitwise repeatable.
+ * hk_apcnn_lateral_fwd (PyramidFeatures.forward, :221-230): out [N,2h,2w,C] = nearest-2x(top [N,h,w,C]) + lat; _bwd: dtop =
+ *   the 2x2 sums of dout (dlat is dout itself).  C % 4 == 0.
+ * hk_apcnn_bcast (SimpleFPA's x_master + x_gpb, :197): y [N,HW,C] = a (optional, else 0) + scale b [N,C].
+ * hk_apcnn_pool (AvgPool2d over the map, :194, and the adjoint of the broadcast): y [N,C] = scale sum_p x [N,HW,C].  C % 256.
+ * hk_apcnn_att_fwd (SpatialGate :271-280 and the pools behind cls3/4/5 and Concate, :533-563): F [N,H,W,256], w [256,1,3,3]
+ *   and bias [1] of the ConvTranspose2d(256, 1, 3, 1, 1) -> gate [N,H,W] = sigmoid(convT(F)), pool_f [N,256] = mean_hw F,
+ *   pool_sf [N,256] = mean_hw(gate F).  With the channel gate ch [N,256], mean_hw((gate + ch) F) = pool_sf + ch pool_f, so the
+ *   attended maps (:256-266) are never written.  F is read twice (tap products, then gate and pools).
+ * hk_apcnn_att_bwd: dpool_f (optional) and dpool_sf [N,256] -> dF = dpool_f / HW + gate dpool_sf / HW + the gate's path,
+ *   dw [256,1,3,3], db [1].  F is read twice and dF written once.  The gate itself carries no gradient (the reference uses it
+ *   under no_grad for the ROIs and for visualisation).
+ * hk_apcnn_roi (get_att_roi, :444-476, for the three levels in one launch): gates g3 [N,H3,W3], g4 [N,H3/2,W3/2], g5
+ *   [N,H3/4,W3/4]; windows int32 [3,4] = (y0, y1, x0, x1) of each level's central window (host memory); keep uint8 [3,15,15] =
+ *   1 where a cell at offset (dy + 7, dx + 7) from a pick survives it (device memory).  Cells outside the window count as 0;
+ *   a cell is a candidate iff its value is strictly above the mean over all h w cells; greedy NMS up to 5 / 3 / 1 picks,
+ *   equal scores to the highest flat index.  boxes fp32 [N,9,4] = (x1, y1, x2, y2) clamped to [0, img - 1], levels at rows
+ *   0-4, 5-7, 8, zeros past the count; counts int32 [N,3].  H3, W3 % 4 == 0; H3 W3 <= 9830.
+ * hk_apcnn_refine_fwd (get_roi_crop_feat, :478-531): x [N,H,W,C], boxes / counts as above, draws fp32 [N,2] in [0, 1) or null
+ *   (eval mode: no drop, no rescale) -> y [N,H,W,C]: the union of the image's ROIs / 8, truncated, bilinearly resized
+ *   (align_corners=False, ATen's arithmetic) to H x W.  draws[n,0] < 0.3 drops level-3 ROI floor(draws[n,1] count), < 0.6 a
+ *   level-4 ROI; the crop is multiplied by the untruncated window area over its kept cells.  meta int32 [N,12] is written for
+ *   the backward.  An image without any ROI keeps its whole map.  _bwd: dy -> dx (zero outside the window and in the dropped
+ *   block), gather form.  C % 4 == 0.
+ * hk_apcnn_act_fwd / _bwd: ReLU (elu = 0) or ELU with alpha 1 (elu = 1, the heads' nn.ELU, :383); the backward reads y.
+ * hk_apcnn_mix_fwd / _bwd (PyramidAttentions.forward, :251-268, on vectors): z, pm, psf, v, ch [3,N,C] (levels 3, 4, 5);
+ *   ch_3 = sig(z_3), ch_4 = (sig(z_4) + ch_3) / 2, ch_5 = (sig(z_5) + ch_4) / 2, v_l = psf_l + ch_l pm_l; the backward gives
+ *   dz and dpm from dv (dpsf is dv).
+ * hk_apcnn_mask_cat (:590-592): out [N,3,H3,W3] = (g3, nearest-2x g4, nearest-4x g5). */
+int hk_apcnn_lateral_fwd(const float* top, const float* lat, float* out, int N, int h, int w, int C, void* stream);
+int hk_apcnn_lateral_bwd(const float* dout, float* dtop, int N, int h, int w, int C, void* stream);
+int hk_apcnn_bcast(const float* a, const float* b, float* y, int N, int HW, int C, float scale, void* stream);
+size_t hk_apcnn_pool_workspace_bytes(int N, int HW, int C);
+int hk_apcnn_pool(const float* x, float* y, int N, int HW, int C, float scale, void* workspace, size_t workspace_bytes,
+                  void* stream);
+size_t hk_apcnn_att_workspace_bytes(int N, int H, int W);
+int hk_apcnn_att_fwd(const float* F, const float* w, const float* bias, float* gate, float* pool_f, float* pool_sf, int N,
+                     int H, int W, int C, void* workspace, size_t workspace_bytes, void* stream);
+int hk_apcnn_att_bwd(const float* F, const float* w, const float* gate, const float* dpool_f, const float* dpool_sf, float* dF,
+                     float* dw, float* db, int N, int H, int W, int C, void* workspace, size_t workspace_bytes, void* stream);
+int hk_apcnn_roi(const float* g3, const float* g4, const float* g5, const int* windows, const unsigned char* keep, float* boxes,
+                 int* counts, int N, int H3, int W3, int img_h, int img_w, void* stream);
+int hk_apcnn_refine_fwd(const float* x, const float* boxes, const int* counts, const float* draws, float* y, int* meta, int N,
+                        int H, int W, int C, void* stream);
+int hk_apcnn_refine_bwd(const float* dy, const int* meta, float* dx, int N, int H, int W, int C, void* stream);
+int hk_apcnn_act_fwd(const float* x, float* y, size_t n, int elu, void* stream);
+int hk_apcnn_act_bwd(const float* y, const float* dy, float* dx, size_t n, int elu, void* stream);
+int hk_apcnn_mix_fwd(const float* z, const float* pm, const float* psf, float* v, float* ch, int N, int C, void* stream);
+int hk_apcnn_mix_bwd(const float* z, const float* pm, const float* ch, const float* dv, float* dz, float* dpm, int N, int C,
+                     void* stream);
+int hk_apcnn_mask_cat(const float* g3, const float* g4, const float* g5, float* out, int N, int H3, int W3, void* stream);
+
 /* ---- classifier nn.Linear (BCNN.py:42, CBCNN.py:26, MPNCOV.py:31) as skinny wgmma GEMMs ------------------- */
 size_t hk_linear_fwd_workspace_bytes(int B, int F, int N);
 int hk_linear_fwd(const float* x, const float* w, const float* bias, float* y, int B, int F, int N, void* workspace,
