@@ -1,5 +1,5 @@
 """Trainer subclasses of the hot-path methods with the reference's Examples/ surface:
-``python -m hawkeye_b200.examples {BCNN,CBCNN,MPN,PeerLearning,OSMENet,APINet,DCL,ProtoTreeNet,InterpPartsNet,NTSNet,APCNN}
+``python -m hawkeye_b200.examples {BCNN,CBCNN,MPN,PeerLearning,OSMENet,APINet,DCL,ProtoTreeNet,InterpPartsNet,NTSNet,APCNN,MGE_CNN}
 --config <yaml>`` replaces
 ``python Examples/<Method>.py --config <yaml>`` (same yaml files; one process per GPU under torchrun instead of nn.DataParallel).
 
@@ -532,12 +532,45 @@ class APCNNTrainer(Trainer):
         self.average_meters['acc'].update(accuracy(out_mean, labels, 1), images.size(0))
 
 
+class MGE_CNNTrainer(Trainer):
+    """Examples/MGE_CNN.py: criterion = MGECNNLoss (the mean of the ten label-smoothed cross-entropies); Adam with weight_decay
+    in two groups, get_params('classifier') at lr and get_params('extractor') (the four trunks) at lr x lr_rate (default
+    0.1); LinearLR(lr_warmup_decay, warmup_epochs) into CosineAnnealingLR(T_max - warmup_epochs), stepped once per epoch.
+    Training and validation accuracy are top-1 on logits_gate.  The step has no host synchronisation, so
+    ``cuda_graph: true`` captures and replays it.
+
+    cls_cat_a, which forward never uses, stays out of the flat buffers: it never has a gradient, so torch's Adam skips it,
+    weight decay included, and a zero gradient in the fused Adam would decay it."""
+
+    def get_criterion(self, config):
+        from .losses import MGECNNLoss
+        return MGECNNLoss(config)
+
+    def param_groups(self):
+        m = self.get_model_module()
+        oc = self.config.train.optimizer
+        unused = {id(p) for p in m.cls_cat_a.parameters()}
+        return [([p for p in m.get_params('classifier') if id(p) not in unused], 1.0),
+                (list(m.get_params('extractor')), oc.lr_rate if 'lr_rate' in oc else 0.1)]
+
+    def get_scheduler(self, config):
+        return _warmup_cosine(self.optimizer, config, self.total_epoch)
+
+    def batch_validate(self, data):
+        import torch
+        from .train import accuracy
+        images, labels = self.to_device(data['img']), self.to_device(data['label'])
+        with torch.no_grad():
+            logits_gate = self.model(images)['logits'][-1]
+        self.average_meters['acc'].update(accuracy(logits_gate, labels, 1), images.size(0))
+
+
 TRAINERS = {'BCNN': BCNNTrainer, 'CBCNN': CBCNNTrainer, 'MPN': MPNTrainer, 'PeerLearning': PeerLearningTrainer,
             'OSMENet': OSMENetTrainer}
 # TRAINERS keeps the key set it has always had, so code that enumerates it sees no change; the command line dispatches
-# over every method, APINet, DCL, ProtoTreeNet, InterpPartsNet, NTSNet and APCNN included.
+# over every method, APINet, DCL, ProtoTreeNet, InterpPartsNet, NTSNet, APCNN and MGE_CNN included.
 ALL_TRAINERS = dict(TRAINERS, APINet=APINetTrainer, DCL=DCLTrainer, ProtoTreeNet=ProtoTreeTrainer,
-                   InterpPartsNet=InterpPartsNetTrainer, NTSNet=NTSNetTrainer, APCNN=APCNNTrainer)
+                   InterpPartsNet=InterpPartsNetTrainer, NTSNet=NTSNetTrainer, APCNN=APCNNTrainer, MGE_CNN=MGE_CNNTrainer)
 
 
 def main(argv=None):

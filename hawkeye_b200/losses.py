@@ -236,6 +236,25 @@ class APCNNLoss(nn.Module):
         return loss * float(len(out_list))
 
 
+class MGECNNLoss(nn.Module):
+    """Examples/MGE_CNN.py:43-45: the mean of the base criterion (cross-entropy with label smoothing 0.1) over the ten logit
+    tensors MGE_CNN returns, as one hk_softmax_ce_ls launch over the stacked [10N, K] rows: with equal row counts, the mean
+    over 10N rows is the mean of the ten means.  ``last_correct`` is the top-1 count on logits_gate, the accuracy
+    Examples/MGE_CNN.py reports, from the same kernel without a gradient."""
+
+    def __init__(self, config=None):
+        super().__init__()
+        self.label_smoothing = 0.1
+
+    def forward(self, outputs, targets):
+        from .ops import CrossEntropyLSFn
+        logits = outputs['logits']
+        loss, _ = CrossEntropyLSFn.apply(torch.cat(logits, dim=0), targets.repeat(len(logits)), self.label_smoothing)
+        with torch.no_grad():
+            _, self.last_correct = CrossEntropyLSFn.apply(logits[-1].detach(), targets, self.label_smoothing)
+        return loss
+
+
 class InterpPartsLoss(nn.Module):
     """model/loss/InterpParts_loss.py: CrossEntropy(logits) + coeff x ShapingLoss(assign) on the (logits, att, assign)
     triple Interp-Parts returns, with the reference's config keys and defaults (radius 2, std 0.4, num_parts 5, alpha 1,

@@ -108,6 +108,8 @@ class Tester:
         logits = self.model(images)
         if isinstance(logits, tuple) and isinstance(logits[1], dict):   # ProtoTreeNet returns (pred, info)
             logits = logits[0]
+        if isinstance(logits, dict) and 'pr_gate' in logits:     # MGE_CNN: accuracy on logits_gate, the last of the ten
+            logits = logits['logits'][-1]
         if isinstance(logits, tuple) and len(logits) == 3 and logits[1].dim() == 4:   # Interp-Parts: (logits, att, assign)
             logits = logits[0]
         if isinstance(logits, list) and len(logits) == 5:        # NTSNet's five outputs: accuracy on concat_logits

@@ -467,6 +467,44 @@ int hk_apcnn_mix_bwd(const float* z, const float* pm, const float* ch, const flo
                      void* stream);
 int hk_apcnn_mask_cat(const float* g3, const float* g4, const float* g5, float* out, int N, int H3, int W3, void* stream);
 
+/* ---- MGE-CNN (model/methods/MGE_CNN/MGE.py, grad_cam.py): part head, Grad-CAM boxes, detached concatenation, gate -------
+ * All maps NHWC fp32; every sum in a fixed order (no atomics), so results are bitwise repeatable.
+ * hk_mge_part_fwd (conv6* + F.relu + pool_max, MGE.py:135, :166, :197): x [N,H,W,C] (layer3's map), w [O,C] (the weight
+ *   [O,C,1,1] of Conv2d(C, O, 1, 1, padding 1)), bias [O] -> pooled [N,O] = max(relu(b_o), max_p relu(w_o . x_p + b_o)) (the
+ *   padded border of the conv's output is its bias) and pos int32 [N,O], the winning pixel (first in row-major order) or -1
+ *   when the border wins, ties included.  The product runs on the wgmma GEMM (bias in its epilogue) into the workspace
+ *   (hk_mge_part_workspace_bytes); pooled is rounded to tf32 on store outside the precise mode.  C, O % 4 == 0.
+ * hk_mge_part_bwd: dpooled [N,O] -> dw [O,C] = sum_n dpooled [pooled > 0] x[n, pos] (nothing for the border), db [O] =
+ *   sum_n dpooled [pooled > 0], n ascending.  No dx: the head reads conv4.detach().
+ * hk_mge_cam_box (GradCam, grad_cam.py:51-90, and get_bbox, MGE.py:48-72, for all images in one launch, one block each):
+ *   the target is targets[n] (int64, may be null) or else the first maximum of logits [N,K]; the layer weights are
+ *   relu(w_main[idx]) / (h w) (the closed form of the reference's backward: the hooked tensor is pooled and fed to the main
+ *   classifier w_main [K,C]); a target outside [0, K) gives zero weights.  CAM = sum_c feat[n] [h,w,C] * weights, upsampled
+ *   to S x S (bilinear, align_corners=True, ATen's fp32 arithmetic), min-max normalised and kept where !(m < rate) (a
+ *   constant CAM gives 0 / 0 = NaN and keeps every pixel).  boxes int32 [N,4] = (y0, x0, y1, x1), the extents of the kept
+ *   pixels with the end exclusive (x[:, y0:y1, x0:x1]), or (0, 0, S, S) when y0 == y1 or x0 == x1: what hk_nts_crop reads
+ *   with pad 0.  C + h w <= 12288; boxes 16-byte aligned.
+ * hk_mge_cat_l2n (pool_cat*, MGE.py:136, :167, :198): out [N, Da + Db] = (scale a / ||a||, scale b / ||b||) per row, without
+ *   an epsilon (l2_norm_v2); rounded to tf32 on store outside the precise mode.
+ * hk_mge_gate_fwd (cls_gate[1], softmax and the weighted sum, MGE.py:207-213): h [N,F] (cls_gate[0]'s output), w2 [3,F],
+ *   b2 [3], the three cat logits c0, c1, c2 [N,K] -> pr [N,3] = softmax(h w2^T + b2), out [N,K] = c0 pr0 + c1 pr1 + c2 pr2.
+ *   The 3-output linear lives here because the GEMM's operands need a 16-byte row pitch.
+ * hk_mge_gate_bwd: dout [N,K] (and dpr [N,3], may be null) -> dz [N,3], the gradient of the gate logits; dh [N,F] (may be
+ *   null); dw2 [3,F] and db2 [3] (both or neither), n ascending.  No gradient reaches c0..c2 (detached in the reference). */
+size_t hk_mge_part_workspace_bytes(int N, int H, int W, int O);
+int hk_mge_part_fwd(const float* x, const float* w, const float* bias, float* pooled, int* pos, int N, int H, int W, int C,
+                    int O, void* workspace, size_t workspace_bytes, void* stream);
+int hk_mge_part_bwd(const float* x, const int* pos, const float* pooled, const float* dpooled, float* dw, float* db, int N,
+                    int H, int W, int C, int O, void* stream);
+int hk_mge_cam_box(const float* logits, const long long* targets, const float* w_main, const float* feat, int* boxes, int N,
+                   int K, int C, int h, int w, int S, float rate, void* stream);
+int hk_mge_cat_l2n(const float* a, const float* b, float* out, int N, int Da, int Db, float scale, void* stream);
+int hk_mge_gate_fwd(const float* h, const float* w2, const float* b2, const float* c0, const float* c1, const float* c2,
+                    float* pr, float* out, int N, int F, int K, void* stream);
+int hk_mge_gate_bwd(const float* h, const float* w2, const float* pr, const float* c0, const float* c1, const float* c2,
+                    const float* dout, const float* dpr, float* dz, float* dh, float* dw2, float* db2, int N, int F, int K,
+                    void* stream);
+
 /* ---- classifier nn.Linear (BCNN.py:42, CBCNN.py:26, MPNCOV.py:31) as skinny wgmma GEMMs ------------------- */
 size_t hk_linear_fwd_workspace_bytes(int B, int F, int N);
 int hk_linear_fwd(const float* x, const float* w, const float* bias, float* y, int B, int F, int N, void* workspace,
