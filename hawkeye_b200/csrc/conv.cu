@@ -126,11 +126,13 @@ struct ConvCfg {
 
 // Output of one 32-column chunk v (channels co .. co + 31) of pixel (w, h, n): addend, bias, ReLU, mask, then the stored
 // map or the fused pooling.  Every lane of the warp calls it (the pooling shuffles are warp-wide), valid or not; lane
-// 32 q + l must hold pixel r = 32 q + l of the tile.
+// 32 q + l must hold pixel r = 32 q + l of the tile.  POOLED: the caller knows that a.P is set, and
+// with it neither addend nor mask (the fused pooling belongs to the single-pass forward).
+template <bool POOLED = false>
 __device__ __forceinline__ void epi_chunk(const ConvArgs& a, float (&v)[32], int w, int h, int n, size_t pix, int co,
                                           bool valid) {
   if (valid && co < a.Cout) {
-    if (a.addend) {
+    if (!POOLED && a.addend) {
       const float4* ad = reinterpret_cast<const float4*>(a.addend + pix * a.Cout + co);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
@@ -146,18 +148,18 @@ __device__ __forceinline__ void epi_chunk(const ConvArgs& a, float (&v)[32], int
 #pragma unroll
       for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
     }
-    if (a.mask) {
+    if (!POOLED && a.mask) {
       const float4* m = reinterpret_cast<const float4*>(a.mask + pix * a.Cout + co);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
-        const float4 mm = m[j];
+        const float4 mm = __ldcs(m + j);   // read once: must not displace the operands the main loop re-reads from L2
         v[4 * j] = mm.x > 0.f ? v[4 * j] : 0.f;
         v[4 * j + 1] = mm.y > 0.f ? v[4 * j + 1] : 0.f;
         v[4 * j + 2] = mm.z > 0.f ? v[4 * j + 2] : 0.f;
         v[4 * j + 3] = mm.w > 0.f ? v[4 * j + 3] : 0.f;
       }
     }
-    if (a.P) {       // (never combined with the precise-mode passes: rounded like the stored map would be)
+    if (POOLED || a.P) {       // (never combined with the precise-mode passes: rounded like the stored map would be)
 #pragma unroll
       for (int j = 0; j < 32; ++j) v[j] = tf32_round(v[j]);
     } else {
@@ -174,7 +176,7 @@ __device__ __forceinline__ void epi_chunk(const ConvArgs& a, float (&v)[32], int
     }
   }
   // the window reduction is a warp-wide shuffle: every lane takes part, whether or not its own pixel is valid
-  if (a.P && co < a.Cout) epi_pool_store(a, v, a.TW, w, h, n, co, valid);
+  if ((POOLED || a.P) && co < a.Cout) epi_pool_store(a, v, a.TW, w, h, n, co, valid);
 }
 
 // Epilogue of one 128-pixel x BN tile, run by the 256 MMA threads (ct = thread index among them).  The accumulators go
@@ -322,15 +324,26 @@ static int launch_conv(const CUtensorMap& tmX, const CUtensorMap& tmW, const Con
 }
 
 // ------------------------------------------------------------------------------------------------
-// implicit-GEMM conv v2 (stride 1, maps with W % 16 == 0 and H % 8 == 0): persistent CTAs and halo reuse.
-//   * pixel tile 16 x 8 of one image (M = 128).  For each (cin chunk, kw) ONE TMA load brings the (8+2) x 16 halo patch
-//     (160 rows x 128 B); the three kh taps are the same patch addressed kh*16 rows (2 KB = whole swizzle atoms) further
-//     down, so the input crosses the L2->SM fabric 3x (+25 % halo) instead of 9x.
+// implicit-GEMM conv v2 (stride 1, maps with W % 8 == 0 and H % 8 == 0): persistent CTAs and halo reuse.
+//   * pixel tile (M = 128): 16 wide x 8 high of one image where 16 divides W, else 8 x 8 of two consecutive images (the
+//     56 x 56 maps; an odd batch leaves the last tile's second image empty: TMA zero-fills it, the epilogue skips it).
+//     For each (cin chunk, kw) ONE TMA load brings the (8+2)-row halo patch of every image of the tile (160 rows x
+//     128 B); the three kh taps are the same patch addressed kh*TW rows (2 KB / 1 KB = whole swizzle atoms) further down,
+//     so the input crosses the L2->SM fabric 3x (+25 % halo) instead of 9x.  MMA warpgroup wg takes rows 64 wg.. of the
+//     tile: the lower half of the 16 x 8 patch, or image wg of the pair (its patch starts 80 rows = 10 atoms down).
 //   * RESIDENT (Cin = 64, Cout = 64: VGG conv1_2 and its dgrad): all 9x2 weight tiles (144 KB) stay in shared memory for
 //     the life of the CTA; only activations stream.
 //   * the shared-memory ring runs across tiles, so the producer loads tile i+1 while the MMA warpgroups finish tile i.
 //   * the MMA warpgroups hand each finished tile to a fourth, epilogue warpgroup through a shared-memory staging tile and
 //     go straight on to the next tile: the output stores and the mask loads of tile i overlap the MMAs of tile i+1.
+//   * the epilogue of the stored map has 8 lanes per pixel (one float4 of the 32-channel chunk each), so a warp's load
+//     or store instruction covers 4 whole 128-byte lines (with thread = pixel it touched 32 lines, 16 bytes of each).
+//     Mask loads and output stores are streaming (ld.global.cs / st.global.cs): each byte is touched once, and as
+//     ordinary accesses the mask pushed the halo rows and weight tiles that neighbouring CTAs re-read out of L2, which
+//     cost the data gradient of the 128-channel-and-deeper layers 8-20 %.  With no epilogue at all the main loop runs at
+//     295-305 TFLOP/s on every layer from conv2_1 on (H100 SXM, 700 W), so that is what is left to hide behind.  Asking
+//     for the mask a chunk ahead of its use measured no different and is not done.  The fused pooling keeps thread =
+//     pixel, which its shuffles need.
 // ------------------------------------------------------------------------------------------------
 constexpr int CONV_V2_THREADS = 512;
 
@@ -342,19 +355,23 @@ struct ConvV2Cfg {
   static constexpr int STAGES = RESIDENT ? 2 : (BN == 64 ? 3 : 2);
   static constexpr int WRES_BYTES = RESIDENT ? 18 * B_TILE : 0;      // 9 taps x 2 chunks
   // staging tile [128 pixels][BN + 8] fp32: the padding makes the MMA threads' 8-byte fragment stores conflict-free
+  // (rows 8 words apart in bank space, 4 lanes x 8 B per row); the epilogue of the stored map reads a pixel's 128-byte
+  // chunk with 8 consecutive lanes, one float4 each: all 32 banks once per quarter-warp, whatever the pitch.
   static constexpr int STG_LD = BN + 8;
   static constexpr int STG_BYTES = 128 * STG_LD * 4;
   static constexpr int SMEM = STAGES * STAGE_BYTES + WRES_BYTES + 1024 + 256 + STG_BYTES;
 };
 
 // warpgroup 0: TMA producer (one thread); warpgroups 1-2: wgmma on rows 0-63 / 64-127 of the 128-pixel tile; warpgroup 3:
-// the epilogue.
-template <int BN, bool RESIDENT>
+// the epilogue.  TW = 16: tile 16 x 8 x 1 image, TW = 8: tile 8 x 8 x 2 images.
+template <int BN, bool RESIDENT, int TW>
 __global__ void __launch_bounds__(CONV_V2_THREADS, 1)
 conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, ConvArgs a,
                         int n_ntiles, int total_tiles) {
   using Cfg = ConvV2Cfg<BN, RESIDENT>;
   constexpr int NACC = BN / 2;
+  constexpr int TN = 16 / TW;                       // images per tile
+  constexpr int WG_ROWS = TW == 16 ? 64 : 80;       // patch rows between the two MMA warpgroups' A operands
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* stages = smem;
@@ -381,18 +398,20 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
   }
   __syncthreads();
 
-  if (warp >= 12) {
+  if (warp >= 12 && a.P) {
+    // fused pooling: thread r owns pixel r of the tile, the mapping epi_chunk's pooling shuffles rely on.  The staging
+    // tile is released as soon as its last chunk has been read.
+    const int r = threadIdx.x - 384;
     int j = 0;
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++j) {
       int pt = t / n_ntiles;
+      const int co0 = (t - pt * n_ntiles) * BN;
       const int tw = pt % a.tiles_w; pt /= a.tiles_w;
       const int th = pt % a.tiles_h; pt /= a.tiles_h;
       mbar_wait(stg_full, j & 1);
-      // thread r owns pixel r of the tile, the mapping epi_chunk's pooling shuffles rely on; the 16 x 8 tile divides the
-      // map, so every pixel is valid.  The staging tile is released as soon as its last chunk has been read.
-      const int r = threadIdx.x - 384;
-      const int w = tw * 16 + (r & 15), h = th * 8 + (r >> 4);
-      const size_t pix = ((size_t)pt * a.H + h) * a.W + w;
+      const int w = tw * TW + (r & (TW - 1)), h = th * 8 + ((r / TW) & 7), n = pt * TN + r / (TW * 8);
+      const bool valid = TN == 1 || n < a.N;
+      const size_t pix = ((size_t)n * a.H + h) * a.W + w;
 #pragma unroll 1
       for (int c = 0; c < BN / 32; ++c) {
         float v[32];
@@ -403,7 +422,71 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
           v[4 * k] = q.x; v[4 * k + 1] = q.y; v[4 * k + 2] = q.z; v[4 * k + 3] = q.w;
         }
         if (c == BN / 32 - 1) mbar_arrive(stg_empty);
-        epi_chunk(a, v, w, h, pt, pix, (t % n_ntiles) * BN + c * 32, true);
+        epi_chunk<true>(a, v, w, h, n, pix, co0 + c * 32, valid);
+      }
+    }
+  } else if (warp >= 12) {
+    // stored map (never the precise-mode passes: no addend, always rounded).  Lane (sub, u) = (lane / 8, lane % 8) of warp
+    // ew owns channels 4 u .. 4 u + 3 of pixels 32 ew + 4 k + sub, k = 0..7, in every 32-channel chunk.
+    const int e = threadIdx.x - 384;
+    const int ew = e >> 5, sub = (e >> 3) & 3, u4 = (e & 7) * 4;
+    // element offset of pixel k = 0 from the tile origin's first channel; pixel k is k % (TW / 4) steps of 4 pixels and
+    // k / (TW / 4) map rows further on
+    const int p0 = ew * 32 + sub;
+    const int eoff0 = (TW == 16 ? (p0 >> 4) * a.W + (p0 & 15) : ((p0 >> 6) * a.H + ((p0 >> 3) & 7)) * a.W + (p0 & 7)) * a.Cout + u4;
+    const int erow = a.W * a.Cout, e4 = 4 * a.Cout;
+    auto eoff = [&](int k) { return eoff0 + (k / (TW / 4)) * erow + (k % (TW / 4)) * e4; };
+    const float* srow = stg + (ew * 32 + sub) * Cfg::STG_LD + u4;
+    // origin element and first channel of tile t; false if this warp's image lies beyond the batch
+    auto tile_org = [&](int t, size_t& org, int& co0) {
+      co0 = (t % n_ntiles) * BN;
+      int pt = t / n_ntiles;
+      const int tw = pt % a.tiles_w; pt /= a.tiles_w;
+      const int th = pt % a.tiles_h; pt /= a.tiles_h;
+      org = (((size_t)pt * TN * a.H + th * 8) * a.W + tw * TW) * a.Cout;
+      return pt * TN + (TW == 16 ? 0 : ew >> 1) < a.N;
+    };
+    int co0 = 0, j = 0;
+    size_t org = 0;
+    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++j) {
+      const bool valid = tile_org(t, org, co0);
+      mbar_wait(stg_full, j & 1);
+#pragma unroll
+      for (int c = 0; c < BN / 32; ++c) {
+        float4 v[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) v[k] = *reinterpret_cast<const float4*>(srow + 4 * k * Cfg::STG_LD + c * 32);
+        if (c == BN / 32 - 1) mbar_arrive(stg_empty);
+        const int co = co0 + c * 32;
+        const bool live = valid && co < a.Cout;
+        if (live) {
+          if (a.bias) {
+            const float4 b = __ldg(reinterpret_cast<const float4*>(a.bias + co + u4));
+#pragma unroll
+            for (int k = 0; k < 8; ++k) { v[k].x += b.x; v[k].y += b.y; v[k].z += b.z; v[k].w += b.w; }
+          }
+          if (a.relu) {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+              v[k].x = fmaxf(v[k].x, 0.f); v[k].y = fmaxf(v[k].y, 0.f);
+              v[k].z = fmaxf(v[k].z, 0.f); v[k].w = fmaxf(v[k].w, 0.f);
+            }
+          }
+          if (a.mask) {
+            float4 mk[8];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) mk[k] = __ldcs(reinterpret_cast<const float4*>(a.mask + org + co + eoff(k)));
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+              v[k].x = mk[k].x > 0.f ? v[k].x : 0.f; v[k].y = mk[k].y > 0.f ? v[k].y : 0.f;
+              v[k].z = mk[k].z > 0.f ? v[k].z : 0.f; v[k].w = mk[k].w > 0.f ? v[k].w : 0.f;
+            }
+          }
+#pragma unroll
+          for (int k = 0; k < 8; ++k)
+            __stcs(reinterpret_cast<float4*>(a.Y + org + co + eoff(k)),
+                   make_float4(tf32_round(v[k].x), tf32_round(v[k].y), tf32_round(v[k].z), tf32_round(v[k].w)));
+        }
       }
     }
   } else if (warp < 4) {
@@ -419,7 +502,7 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
         int pt = t / n_ntiles;
         const int tw = pt % a.tiles_w; pt /= a.tiles_w;
         const int th = pt % a.tiles_h; pt /= a.tiles_h;
-        const int w0 = tw * 16, h0 = th * 8, n0 = pt, co0 = nt * BN;
+        const int w0 = tw * TW, h0 = th * 8, n0 = pt * TN, co0 = nt * BN;
         for (int kb = 0; kb < nkb; ++kb, ++kbg) {
           const int s = kbg % Cfg::STAGES;
           const uint32_t ph = (kbg / Cfg::STAGES) & 1;
@@ -452,14 +535,14 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
         const int s = kbg % Cfg::STAGES;
         const int ck = kb / 3, kw = kb - ck * 3;
         mbar_wait(&full[s], (kbg / Cfg::STAGES) & 1);
-        // rows 64 wg.. of the tile in the patch of tap kh: + (64 wg + 16 kh) rows of 128 B
-        const uint32_t a_addr = smem_u32(stages + s * Cfg::STAGE_BYTES) + wg * 64 * 128;
+        // rows 64 wg.. of the tile in the patch of tap kh: + (WG_ROWS wg + TW kh) rows of 128 B
+        const uint32_t a_addr = smem_u32(stages + s * Cfg::STAGE_BYTES) + wg * WG_ROWS * 128;
         wgmma_fence();
 #pragma unroll
         for (int kh = 0; kh < 3; ++kh) {
           const uint32_t b_addr = RESIDENT ? smem_u32(wres + ((kh * 3 + kw) * 2 + ck) * Cfg::B_TILE)
                                            : smem_u32(stages + s * Cfg::STAGE_BYTES + Cfg::A_BYTES + kh * Cfg::B_TILE);
-          const uint64_t ad = make_sdesc(a_addr + kh * 16 * 128), bd = make_sdesc(b_addr);
+          const uint64_t ad = make_sdesc(a_addr + kh * TW * 128), bd = make_sdesc(b_addr);
 #pragma unroll
           for (int ks = 0; ks < 4; ++ks) wgmma_tf32(acc, ad + ks * 2, bd + ks * 2, (kb | kh | ks) != 0);
         }
@@ -482,22 +565,24 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
   }
 }
 
-template <int BN, bool RESIDENT>
+template <int BN, bool RESIDENT, int TW>
 static int launch_conv_v2(const float* x, const float* wp, ConvArgs a, int N, int H, int W, cudaStream_t stream) {
   using Cfg = ConvV2Cfg<BN, RESIDENT>;
-  if (int r = allow_dynamic_smem<conv3x3_igemm_v2_kernel<BN, RESIDENT>>(Cfg::SMEM, BN == 64 ? "conv_v2<64>" : "conv_v2<128>"))
+  if (int r = allow_dynamic_smem<conv3x3_igemm_v2_kernel<BN, RESIDENT, TW>>(Cfg::SMEM, BN == 64 ? "conv_v2<64>" : "conv_v2<128>"))
     return r;
-  a.TW = 16; a.TH = 8; a.TN = 1;
-  a.tiles_w = W / 16; a.tiles_h = H / 8; a.tiles_n = N;
+  a.TW = TW; a.TH = 8; a.TN = 16 / TW;
+  a.tiles_w = W / TW; a.tiles_h = H / 8; a.tiles_n = (N + a.TN - 1) / a.TN;
   const int n_ntiles = (a.Cout + BN - 1) / BN;
   const long long total = (long long)a.tiles_w * a.tiles_h * a.tiles_n * n_ntiles;
   HK_REQUIRE(total < (1ll << 31), HK_ERR_UNSUPPORTED, "conv3x3: too many tiles");
+  // the epilogue keeps element offsets inside a tile (up to one image apart) as int
+  HK_REQUIRE((long long)H * W * a.Cout < (1ll << 30), HK_ERR_UNSUPPORTED, "conv3x3: map too large");
   CUtensorMap tmX, tmW;
   int r;
   {
     uint64_t dims[4] = {(uint64_t)a.Cin, (uint64_t)W, (uint64_t)H, (uint64_t)N};
     uint64_t strides[3] = {(uint64_t)a.Cin * 4, (uint64_t)W * a.Cin * 4, (uint64_t)H * W * a.Cin * 4};
-    uint32_t box[4] = {32, 16, 10, 1};
+    uint32_t box[4] = {32, (uint32_t)TW, 10, (uint32_t)a.TN};
     if ((r = make_tmap(&tmX, x, 4, dims, strides, box))) return r;
   }
   {
@@ -508,9 +593,16 @@ static int launch_conv_v2(const float* x, const float* wp, ConvArgs a, int N, in
   }
   const int sms = num_sms();
   const int grid = total < sms ? (int)total : sms;
-  conv3x3_igemm_v2_kernel<BN, RESIDENT><<<grid, CONV_V2_THREADS, Cfg::SMEM, stream>>>(tmX, tmW, a, n_ntiles, (int)total);
+  conv3x3_igemm_v2_kernel<BN, RESIDENT, TW><<<grid, CONV_V2_THREADS, Cfg::SMEM, stream>>>(tmX, tmW, a, n_ntiles, (int)total);
   HK_LAUNCH_CHECK("conv3x3_igemm_v2_kernel");
   return 0;
+}
+
+template <int TW>
+static int launch_conv_v2(const float* x, const float* wp, const ConvArgs& a, int N, int H, int W, cudaStream_t stream) {
+  if (a.Cin == 64 && a.Cout == 64) return launch_conv_v2<64, true, TW>(x, wp, a, N, H, W, stream);
+  if (a.Cout <= 64) return launch_conv_v2<64, false, TW>(x, wp, a, N, H, W, stream);
+  return launch_conv_v2<128, false, TW>(x, wp, a, N, H, W, stream);
 }
 
 static int conv3x3_igemm_1x(const float* x, const float* wp, const float* bias, const float* mask, const float* addend,
@@ -559,11 +651,11 @@ static int conv3x3_igemm_1x(const float* x, const float* wp, const float* bias, 
   a.stride = stride;
   a.addend = addend; a.no_round = no_round;
   // the three chained 3xTF32 passes (no_round) keep the generic kernel, whose accumulation order does not depend on the
-  // map size; the single-pass layers take the halo-reuse kernel wherever its 16 x 8 pixel tile divides the map
-  if (!no_round && stride == 1 && W % 16 == 0 && H % 8 == 0) {
-    if (Cin == 64 && Cout == 64) return launch_conv_v2<64, true>(x, wp, a, N, H, W, stream);
-    if (Cout <= 64) return launch_conv_v2<64, false>(x, wp, a, N, H, W, stream);
-    return launch_conv_v2<128, false>(x, wp, a, N, H, W, stream);
+  // map size; the single-pass layers take the halo-reuse kernel wherever one of its pixel tiles (16 x 8 x 1 image, else
+  // 8 x 8 x 2 images) divides the map
+  if (!no_round && stride == 1 && W % 8 == 0 && H % 8 == 0) {
+    if (W % 16 == 0) return launch_conv_v2<16>(x, wp, a, N, H, W, stream);
+    return launch_conv_v2<8>(x, wp, a, N, H, W, stream);
   }
   pick_tile(W, H, N, 128, &a.TW, &a.TH, &a.TN);
   HK_REQUIRE(!pooled || (a.TW >= 2 && a.TH >= 2), HK_ERR_UNSUPPORTED, "conv3x3 + pool: pixel tile %dx%d", a.TW, a.TH);
