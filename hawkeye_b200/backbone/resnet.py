@@ -7,6 +7,9 @@ import torch.nn as nn
 
 from .. import ops_resnet
 from ..registry import BACKBONE
+from ..utils import load_pretrained
+
+RESNET_NAMES = ('conv1', 'bn1', 'relu', 'maxpool', 'layer1', 'layer2', 'layer3', 'layer4')
 
 
 class Bottleneck(nn.Module):
@@ -35,18 +38,39 @@ def _make_layer(inplanes, planes, blocks, stride):
     return nn.Sequential(*layers)
 
 
+def _resnet_modules(layers):
+    """conv1, bn1, relu, maxpool and one stage of ``layers[i]`` blocks per entry, created in torchvision's order."""
+    mods = [nn.Conv2d(3, 64, kernel_size=7, stride=2, padding=3, bias=False), nn.BatchNorm2d(64), nn.ReLU(inplace=True),
+            nn.MaxPool2d(kernel_size=3, stride=2, padding=1)]
+    inplanes = 64
+    for planes, n, stride in zip((64, 128, 256, 512), layers, (1, 2, 2, 2)):
+        mods.append(_make_layer(inplanes, planes, n, stride))
+        inplanes = planes * 4
+    return mods
+
+
+class ResNetBody(nn.Module):
+    """conv1, bn1, relu, maxpool, layer1..layer{len(layers)} under torchvision's attribute names: the base of the methods'
+    ResNets, which register their own modules after these."""
+
+    def __init__(self, layers):
+        super().__init__()
+        for name, m in zip(RESNET_NAMES, _resnet_modules(layers)):
+            self.add_module(name, m)
+        self.num_layers = len(layers)
+
+    def trunk_modules(self, cut=None):
+        """[conv1, bn1, relu, maxpool, layer1..layer{cut}] (every layer without ``cut``), as ops_resnet.TrunkPlan takes it."""
+        return [getattr(self, n) for n in RESNET_NAMES[:4 + (cut or self.num_layers)]]
+
+
 class ResNetTrunk(nn.Sequential):
     """children()[:-2] of the reference ResNet: conv1, bn1, relu, maxpool, layer1..layer4 (indices 0..7)."""
 
     def __init__(self, layers=(3, 4, 6, 3)):
-        mods = [nn.Conv2d(3, 64, kernel_size=7, stride=2, padding=3, bias=False), nn.BatchNorm2d(64), nn.ReLU(inplace=True),
-                nn.MaxPool2d(kernel_size=3, stride=2, padding=1)]
-        inplanes = 64
-        for planes, n, stride in zip((64, 128, 256, 512), layers, (1, 2, 2, 2)):
-            mods.append(_make_layer(inplanes, planes, n, stride))
-            inplanes = planes * 4
+        mods = _resnet_modules(layers)
         super().__init__(*mods)
-        self.out_channels = inplanes
+        self.out_channels = mods[-1][-1].conv3.out_channels
         for m in self.modules():                                   # resnet.py:191-196
             if isinstance(m, nn.Conv2d):
                 nn.init.kaiming_normal_(m.weight, mode='fan_out', nonlinearity='relu')
@@ -59,46 +83,20 @@ class ResNetTrunk(nn.Sequential):
         return ops_resnet.resnet_trunk(x, self)
 
 
+TRUNK_KEYS = {n: str(i) for i, n in enumerate(RESNET_NAMES)}      # torchvision's top-level name -> ResNetTrunk index
+BODY_KEYS = {n: n for n in RESNET_NAMES}                           # -> ResNetBody attribute (layers past the body: skipped)
+
+
 @BACKBONE.register
 def resnet101(pretrained=False, progress=True, **kwargs):
     """Reference signature (resnet.py:309-319); the trunk of OSMENet (OSME.py:55-56).  Offline => reference initialisers
     unless $HAWKEYE_RESNET101_PTH points at torchvision's checkpoint."""
-    import os
-    import torch
     trunk = ResNetTrunk((3, 4, 23, 3))
-    path = os.environ.get('HAWKEYE_RESNET101_PTH')
-    if pretrained and path and os.path.exists(path):
-        sd = torch.load(path, map_location='cpu')
-        names = ['conv1', 'bn1', 'relu', 'maxpool', 'layer1', 'layer2', 'layer3', 'layer4']
-        trunk.load_state_dict({str(names.index(k.split('.')[0])) + k[len(k.split('.')[0]):]: v for k, v in sd.items()
-                               if k.split('.')[0] in names})
-    elif pretrained and os.environ.get('HAWKEYE_ALLOW_RANDOM_INIT', '0') != '1':
-        import logging
-        logging.getLogger('hawkeye_b200').warning('resnet101(pretrained=True): no checkpoint at $HAWKEYE_RESNET101_PTH (%r) — the '
-                                                  'trunk keeps the reference\'s RANDOM initialisation', path)
-    return trunk
+    return load_pretrained(trunk, 'HAWKEYE_RESNET101_PTH', 'resnet101', TRUNK_KEYS) if pretrained else trunk
 
 
 @BACKBONE.register
 def resnet50(pretrained=False, progress=True, **kwargs):
     """Reference signature (resnet.py:296-306); offline => reference initialisers unless $HAWKEYE_RESNET50_PTH is set."""
-    import os
-    import torch
     trunk = ResNetTrunk((3, 4, 6, 3))
-    path = os.environ.get('HAWKEYE_RESNET50_PTH')
-    if pretrained and path and os.path.exists(path):
-        sd = torch.load(path, map_location='cpu')
-        names = ['conv1', 'bn1', 'relu', 'maxpool', 'layer1', 'layer2', 'layer3', 'layer4']
-        remap = {}
-        for k, v in sd.items():
-            head = k.split('.')[0]
-            if head in names:
-                remap[str(names.index(head)) + k[len(head):]] = v
-        trunk.load_state_dict(remap)           # strict: every trunk tensor must be present (fc.* is not part of the trunk)
-    elif pretrained and os.environ.get('HAWKEYE_ALLOW_RANDOM_INIT', '0') != '1':
-        import logging
-        logging.getLogger('hawkeye_b200').warning(
-            'resnet50(pretrained=True): no checkpoint at $HAWKEYE_RESNET50_PTH (%r) — the trunk keeps the reference\'s '
-            'RANDOM initialisation.  Point HAWKEYE_RESNET50_PTH at torchvision\'s resnet50 .pth, or set '
-            'HAWKEYE_ALLOW_RANDOM_INIT=1 (benchmarks / parity tests) to silence this.', path)
-    return trunk
+    return load_pretrained(trunk, 'HAWKEYE_RESNET50_PTH', 'resnet50', TRUNK_KEYS) if pretrained else trunk

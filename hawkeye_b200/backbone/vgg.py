@@ -5,12 +5,11 @@
 reference checkpoints load unchanged — but ``forward`` never calls those modules: the whole stack runs as
 one fused CUDA pipeline (NHWC, wgmma implicit-GEMM convs) through ``ops.vgg_features``.
 """
-import torch
 import torch.nn as nn
 
 from .. import ops
 from ..registry import BACKBONE
-from ..utils import initialize_weights
+from ..utils import initialize_weights, load_pretrained
 
 cfgs = {
     'D': [64, 64, 'M', 128, 128, 'M', 256, 256, 256, 'M', 512, 512, 512, 'M', 512, 512, 512, 'M'],
@@ -49,17 +48,5 @@ class VGGFeatures(nn.Sequential):
 def vgg16(pretrained=False, progress=True, **kwargs):
     """Reference signature (vgg.py:141-151).  ``pretrained=True`` needs the torchvision checkpoint on disk
     (``$HAWKEYE_VGG16_PTH``); there is no network here, so otherwise the reference initialisers are used."""
-    import os
     feats = VGGFeatures(cfgs['D'])
-    path = os.environ.get('HAWKEYE_VGG16_PTH')
-    if pretrained and path and os.path.exists(path):
-        sd = torch.load(path, map_location='cpu')
-        feats.load_state_dict({k[len('features.'):]: v for k, v in sd.items() if k.startswith('features.')})
-    elif pretrained and os.environ.get('HAWKEYE_ALLOW_RANDOM_INIT', '0') != '1':
-        # the reference downloads ImageNet weights here (vgg.py:83-85); silently training on a random VGG would be wrong
-        import logging
-        logging.getLogger('hawkeye_b200').warning(
-            'vgg16(pretrained=True): no checkpoint at $HAWKEYE_VGG16_PTH (%r) — the backbone keeps the reference\'s RANDOM '
-            'initialisation.  Point HAWKEYE_VGG16_PTH at torchvision\'s vgg16 .pth, or set HAWKEYE_ALLOW_RANDOM_INIT=1 '
-            '(benchmarks / parity tests) to silence this.', path)
-    return feats
+    return load_pretrained(feats, 'HAWKEYE_VGG16_PTH', 'vgg16', {'features': ''}) if pretrained else feats

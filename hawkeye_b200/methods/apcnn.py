@@ -23,15 +23,15 @@ ascending sort gives; torch's argsort leaves it undefined).  The drop block of t
 level-4 ROI), column 1 the index as a fraction of the image's count.
 """
 import math
-import os
 
 import torch
 import torch.nn as nn
 
-from .. import _lib, ops, ops_apcnn, ops_resnet
-from ..backbone.resnet import _make_layer
-from ..ops_interp_parts import RowBatchNormFn
+from .. import ops, ops_apcnn, ops_resnet
+from ..backbone.resnet import BODY_KEYS, ResNetBody
+from ..ops_resnet import RowBatchNormFn
 from ..registry import MODEL
+from ..utils import load_pretrained
 
 
 class BasicConv(nn.Module):
@@ -147,21 +147,13 @@ def _run_head(seq, v, training):
     return ops.linear(ops_apcnn.ActFn.apply(v, True), fc2.weight, fc2.bias)
 
 
-class ResNet(nn.Module):
+class ResNet(ResNetBody):
     """APCNN.py:344-599 with ``block`` = Bottleneck."""
 
     def __init__(self, num_classes, layers=(3, 4, 6, 3)):
-        super().__init__()
         ops.check_num_classes(num_classes)
+        super().__init__(layers)
         self.num_classes = num_classes
-        self.conv1 = nn.Conv2d(3, 64, kernel_size=7, stride=2, padding=3, bias=False)
-        self.bn1 = nn.BatchNorm2d(64)
-        self.relu = nn.ReLU(inplace=True)
-        self.maxpool = nn.MaxPool2d(kernel_size=3, stride=2, padding=1)
-        self.layer1 = _make_layer(64, 64, layers[0], 1)
-        self.layer2 = _make_layer(256, 128, layers[1], 2)
-        self.layer3 = _make_layer(512, 256, layers[2], 2)
-        self.layer4 = _make_layer(1024, 512, layers[3], 2)
         hidden = 512 if num_classes == 200 else 256
         self.fpn = PyramidFeatures(512, 1024, 2048)
         self.apn = PyramidAttentions(channel_size=256)
@@ -175,7 +167,7 @@ class ResNet(nn.Module):
             elif isinstance(m, nn.BatchNorm2d):
                 m.weight.data.fill_(1)
                 m.bias.data.zero_()
-        self.__dict__['_plan'] = ops_resnet.TrunkPlan([self.conv1, self.bn1, self.relu, self.maxpool, self.layer1, self.layer2])
+        self.__dict__['_plan'] = ops_resnet.TrunkPlan(self.trunk_modules(2))
         self.__dict__['_blocks3'] = [ops_resnet.block_units(b) for b in self.layer3]
         self.__dict__['_blocks4'] = [ops_resnet.block_units(b) for b in self.layer4]
         self.register_buffer('nms_keep', torch.from_numpy(ops_apcnn.suppression_table()), persistent=False)
@@ -221,26 +213,8 @@ def resnet50(num_classes):
     return ResNet(num_classes, (3, 4, 6, 3))
 
 
-def _load_pretrained(net):
-    """torchvision's ResNet-50 at $HAWKEYE_RESNET50_PTH into conv1..layer4 (the reference's load_state_dict skips fc, which
-    the model does not have), or the reference's random initialisation with the backbone's warning."""
-    path = os.environ.get('HAWKEYE_RESNET50_PTH')
-    if path and os.path.exists(path):
-        sd = torch.load(path, map_location='cpu')
-        trunk = {k: v for k, v in sd.items() if not k.startswith('fc.')}
-        missing, _ = net.load_state_dict(trunk, strict=False)
-        lacking = [k for k in missing if k.split('.')[0] in ('conv1', 'bn1', 'layer1', 'layer2', 'layer3', 'layer4')]
-        if lacking:
-            raise _lib.HawkeyeLibError(f'APCNN: {path} lacks trunk tensors {lacking[:4]}...')
-    elif os.environ.get('HAWKEYE_ALLOW_RANDOM_INIT', '0') != '1':
-        import logging
-        logging.getLogger('hawkeye_b200').warning(
-            'APCNN(pretrained): no checkpoint at $HAWKEYE_RESNET50_PTH (%r) — the trunk keeps the reference\'s RANDOM '
-            'initialisation.  Point HAWKEYE_RESNET50_PTH at torchvision\'s resnet50 .pth, or set HAWKEYE_ALLOW_RANDOM_INIT=1 '
-            '(benchmarks / parity tests) to silence this.', path)
-    return net
-
-
 @MODEL.register
 def APCNN(config):
-    return _load_pretrained(resnet50(int(config.num_classes)))
+    """torchvision's ResNet-50 at $HAWKEYE_RESNET50_PTH goes into conv1..layer4; the reference's load skips its fc, which the
+    model does not have."""
+    return load_pretrained(resnet50(int(config.num_classes)), 'HAWKEYE_RESNET50_PTH', 'resnet50', BODY_KEYS)

@@ -12,7 +12,7 @@ each replica runs ``get_pairs`` on its own shard.  Like the reference, the head 
 import torch
 import torch.nn as nn
 
-from .. import _lib, ops, ops_apinet, ops_cin
+from .. import _lib, ops, ops_apinet
 from ..backbone.resnet import resnet101
 from ..registry import MODEL
 
@@ -38,7 +38,7 @@ class APINet(nn.Module):
         if (H, W) != (7, 7):
             raise _lib.HawkeyeLibError(f'APINet: the trunk map is {H}x{W}, expected 7x7 (224x224 inputs; the reference '
                                        'pools with AvgPool2d(7, stride=1))')
-        return ops_cin.RowMeanFn.apply(conv_out.reshape(n, C, H * W))
+        return ops.RowMeanFn.apply(conv_out.reshape(n, C, H * W))
 
     def forward(self, images, targets=None, flag='train'):
         self.device = images.device

@@ -70,7 +70,7 @@ class CINClassifier(nn.Module):
         self.classifier = nn.Linear(in_channel, num_classes)
 
     def _logits(self, z):
-        return ops.linear(ops_cin.RowMeanFn.apply(z), self.classifier.weight, self.classifier.bias)
+        return ops.linear(ops.RowMeanFn.apply(z), self.classifier.weight, self.classifier.bias)
 
     def forward(self, x):
         if isinstance(x, tuple):

@@ -10,14 +10,13 @@ The trunk (ResNet v1.5 cut after layer3) runs on ops_resnet and hands its NHWC m
 grouping unit, the attention head with the part sum and the shaping loss's occupancy run on hk_ip_*; the Bottleneck1x1
 stacks run on ops_resnet's block helpers over P = N*K rows; groupingbn on hk_bn_*; mylinear on hk_linear_*.
 """
-import os
-
 import torch
 import torch.nn as nn
 
 from .. import ops, ops_interp_parts, ops_resnet
-from ..backbone.resnet import Bottleneck, _make_layer
+from ..backbone.resnet import BODY_KEYS, Bottleneck, ResNetBody
 from ..registry import MODEL
+from ..utils import load_pretrained
 
 
 class Bottleneck1x1(nn.Module):
@@ -61,21 +60,14 @@ class GroupingUnit(nn.Module):
         return f'{self.__class__.__name__} ({self.in_channels} -> {self.num_parts})'
 
 
-class ResNet(nn.Module):
-    """Interp_Parts.py:251-371 with ``block`` = Bottleneck."""
+class ResNet(ResNetBody):
+    """Interp_Parts.py:251-371 with ``block`` = Bottleneck, cut after layer3 (``layers[3]`` is not used)."""
 
     def __init__(self, layers, num_classes=1000, num_parts=32):
-        super().__init__()
         ops_interp_parts.check_parts(num_parts)
         ops.check_num_classes(num_classes)
+        super().__init__(layers[:3])
         self.n_parts, self.num_classes = num_parts, num_classes
-        self.conv1 = nn.Conv2d(3, 64, kernel_size=7, stride=2, padding=3, bias=False)
-        self.bn1 = nn.BatchNorm2d(64)
-        self.relu = nn.ReLU(inplace=True)
-        self.maxpool = nn.MaxPool2d(kernel_size=3, stride=2, padding=1)
-        self.layer1 = _make_layer(64, 64, layers[0], 1)
-        self.layer2 = _make_layer(256, 128, layers[1], 2)
-        self.layer3 = _make_layer(512, 256, layers[2], 2)
         self.grouping = GroupingUnit(256 * Bottleneck.expansion, num_parts)
         self.grouping.reset_parameters()
         self.post_block = nn.Sequential(
@@ -103,8 +95,7 @@ class ResNet(nn.Module):
         for m in self.modules():
             if isinstance(m, (Bottleneck, Bottleneck1x1)):
                 nn.init.constant_(m.bn3.weight, 0)
-        self.__dict__['_trunk_plan'] = ops_resnet.TrunkPlan([self.conv1, self.bn1, self.relu, self.maxpool, self.layer1,
-                                                             self.layer2, self.layer3])
+        self.__dict__['_trunk_plan'] = ops_resnet.TrunkPlan(self.trunk_modules())
         self.__dict__['_post_blocks'] = [ops_resnet.block_units(b) for b in self.post_block]
         self.__dict__['_att_blocks'] = [ops_resnet.block_units(b) for b in list(self.attconv)[:2]]
 
@@ -119,36 +110,19 @@ class ResNet(nn.Module):
         conv, bn = self.attconv[2], self.attconv[3]
         pooled, att = ops_interp_parts.AttentionPoolFn.apply(a.view(N * K, -1), p.view(N * K, -1), conv.weight, conv.bias,
                                                              bn.weight, bn.bias, bn, self.training, N, K)
-        out = ops_interp_parts.RowBatchNormFn.apply(pooled, self.groupingbn.weight, self.groupingbn.bias, self.groupingbn,
+        out = ops_resnet.RowBatchNormFn.apply(pooled, self.groupingbn.weight, self.groupingbn.bias, self.groupingbn,
                                                     self.training)
         logits = ops.linear(out, self.mylinear.weight, self.mylinear.bias)
         return logits, att.view(N, 1, K, 1), assign
 
 
-_TRUNK_NAMES = ('conv1', 'bn1', 'layer1', 'layer2', 'layer3')
-
-
-def _pretrained(net, env, arch):
-    """torchvision's checkpoint at $<env>, loaded as the reference loads it (strict=False: only conv1, bn1 and layer1-3
-    match), or the reference's random initialisation with the backbone's warning."""
-    path = os.environ.get(env)
-    if path and os.path.exists(path):
-        sd = torch.load(path, map_location='cpu')
-        net.load_state_dict({k: v for k, v in sd.items() if k.split('.')[0] in _TRUNK_NAMES}, strict=False)
-    elif os.environ.get('HAWKEYE_ALLOW_RANDOM_INIT', '0') != '1':
-        import logging
-        logging.getLogger('hawkeye_b200').warning(
-            '%s(pretrained): no checkpoint at $%s (%r) — the trunk keeps the reference\'s RANDOM initialisation.  Point %s at '
-            'torchvision\'s %s .pth, or set HAWKEYE_ALLOW_RANDOM_INIT=1 (benchmarks / parity tests) to silence this.',
-            'IP_ResNet' + arch[6:], env, path, env, arch)
-    return net
-
-
 @MODEL.register
 def IP_ResNet50(config):
-    return _pretrained(ResNet([3, 4, 6, 3], config.num_classes, config.num_parts), 'HAWKEYE_RESNET50_PTH', 'resnet50')
+    return load_pretrained(ResNet([3, 4, 6, 3], config.num_classes, config.num_parts), 'HAWKEYE_RESNET50_PTH', 'resnet50',
+                           BODY_KEYS)
 
 
 @MODEL.register
 def IP_ResNet101(config):
-    return _pretrained(ResNet([3, 4, 23, 3], config.num_classes, config.num_parts), 'HAWKEYE_RESNET101_PTH', 'resnet101')
+    return load_pretrained(ResNet([3, 4, 23, 3], config.num_classes, config.num_parts), 'HAWKEYE_RESNET101_PTH', 'resnet101',
+                           BODY_KEYS)

@@ -27,7 +27,6 @@ import torch.nn as nn
 
 from .. import ops, ops_mge, ops_resnet
 from ..backbone.resnet import ResNetTrunk, resnet50
-from ..ops_apcnn import PoolFn
 from ..registry import MODEL
 
 BRANCHES = ('', '_box', '_box_2', '_gate')
@@ -92,7 +91,7 @@ class LocalCamNet(nn.Module):
         plan, blocks = self._plans[branch]
         c4 = ops_resnet.resnet_trunk_nhwc(x, plan, self.training)
         c5 = ops_resnet.block_stack(c4, blocks, self.training)
-        return c4, c5, PoolFn.apply(c5)
+        return c4, c5, ops.NHWCMeanFn.apply(c5)
 
     def experts(self, c4, pool, suffix):
         """The part head and the two classifiers after it -> (logits_max, logits_cat)."""
@@ -108,7 +107,7 @@ class LocalCamNet(nn.Module):
             return logits, None
         with torch.no_grad():
             if self.training:                              # layer4 rerun on the running statistics, updating none
-                pool = PoolFn.apply(ops_resnet.block_stack(c4.detach(), self._plans[branch][1], False))
+                pool = ops.NHWCMeanFn.apply(ops_resnet.block_stack(c4.detach(), self._plans[branch][1], False))
             return self.classifier(pool), None
 
     def forward(self, x, y=None, is_vis=False, vis_idx=None, gt_top=None):

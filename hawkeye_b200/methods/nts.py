@@ -22,16 +22,16 @@ multiple of 32 works; part crops are always 224 x 224.  ``proposal_num`` may not
 pass is sure to keep (8 at 224, 26 at 448), computed from the anchors at construction, so the NMS always fills its T rows.
 """
 import math
-import os
 
 import numpy as np
 import torch
 import torch.nn as nn
 
-from .. import _lib, ops, ops_cin, ops_nts, ops_resnet
-from ..backbone.resnet import _make_layer
+from .. import ops, ops_nts, ops_resnet
+from ..backbone.resnet import BODY_KEYS, ResNetBody
 from ..ops import nchw_to_nhwc
 from ..registry import MODEL
+from ..utils import load_pretrained
 
 NUM_CLASSES = 200
 # (stride, size, scales, aspect ratios) of the three anchor levels (anchors.py:3-7)
@@ -69,19 +69,11 @@ def survivor_bound(anchors):
     return math.ceil(len(a) / int(covered.sum(1).max()))
 
 
-class ResNet(nn.Module):
+class ResNet(ResNetBody):
     """NTS_Net/resnet.py:94-152 with Bottleneck: forward(x, seed, call) -> (logits, layer4 map NCHW, dropped pooled feature)."""
 
     def __init__(self, num_classes=NUM_CLASSES):
-        super().__init__()
-        self.conv1 = nn.Conv2d(3, 64, kernel_size=7, stride=2, padding=3, bias=False)
-        self.bn1 = nn.BatchNorm2d(64)
-        self.relu = nn.ReLU(inplace=True)
-        self.maxpool = nn.MaxPool2d(kernel_size=3, stride=2, padding=1)
-        self.layer1 = _make_layer(64, 64, 3, 1)
-        self.layer2 = _make_layer(256, 128, 4, 2)
-        self.layer3 = _make_layer(512, 256, 6, 2)
-        self.layer4 = _make_layer(1024, 512, 3, 2)
+        super().__init__((3, 4, 6, 3))
         self.avgpool = nn.AdaptiveAvgPool2d(1)
         self.fc = nn.Linear(2048, num_classes)
         self.drop = nn.Dropout(p=0.5)
@@ -91,14 +83,13 @@ class ResNet(nn.Module):
             elif isinstance(m, nn.BatchNorm2d):
                 nn.init.constant_(m.weight, 1)
                 nn.init.constant_(m.bias, 0)
-        self.__dict__['_plan'] = ops_resnet.TrunkPlan([self.conv1, self.bn1, self.relu, self.maxpool, self.layer1,
-                                                       self.layer2, self.layer3, self.layer4])
+        self.__dict__['_plan'] = ops_resnet.TrunkPlan(self.trunk_modules())
 
     def forward(self, x, seed, call):
         params = self._plan.params()
         fmap = ops_resnet.ResNetTrunkFn.apply(x, self._plan, ops.wants_grad(x, params), self.training, False, *params)
         n, C, H, W = fmap.shape
-        feature = ops_nts.dropout(ops_cin.RowMeanFn.apply(fmap.reshape(n, C, H * W)), float(self.drop.p), seed, call)
+        feature = ops_nts.dropout(ops.RowMeanFn.apply(fmap.reshape(n, C, H * W)), float(self.drop.p), seed, call)
         return ops.linear(feature, self.fc.weight, self.fc.bias), fmap, feature
 
 
@@ -117,23 +108,6 @@ class ProposalNet(nn.Module):
 
     def forward(self, x_nhwc, anchors, topn):
         return ops_nts.proposal(x_nhwc, self, anchors, topn)
-
-
-def _load_pretrained(trunk):
-    """torchvision's ResNet-50 at $HAWKEYE_RESNET50_PTH into ``pretrained_model`` (its 1000-way fc skipped: the reference
-    replaces fc after loading, NTSNet.py:19-21), or the reference's random initialisation with the backbone's warning."""
-    path = os.environ.get('HAWKEYE_RESNET50_PTH')
-    if path and os.path.exists(path):
-        sd = torch.load(path, map_location='cpu')
-        missing, _ = trunk.load_state_dict({k: v for k, v in sd.items() if not k.startswith('fc.')}, strict=False)
-        if any(not k.startswith('fc.') for k in missing):
-            raise _lib.HawkeyeLibError(f'NTSNet: {path} lacks trunk tensors {missing[:4]}...')
-    elif os.environ.get('HAWKEYE_ALLOW_RANDOM_INIT', '0') != '1':
-        import logging
-        logging.getLogger('hawkeye_b200').warning(
-            'NTSNet(pretrained): no checkpoint at $HAWKEYE_RESNET50_PTH (%r) — the trunk keeps the reference\'s RANDOM '
-            'initialisation.  Point HAWKEYE_RESNET50_PTH at torchvision\'s resnet50 .pth, or set HAWKEYE_ALLOW_RANDOM_INIT=1 '
-            '(benchmarks / parity tests) to silence this.', path)
 
 
 @MODEL.register
@@ -161,7 +135,8 @@ class NTSNet(nn.Module):
         self.partcls_net = nn.Linear(2048, NUM_CLASSES)
         self.pad_side = ops_nts.PAD
         self.register_buffer('edge_anchors', torch.from_numpy(anchors), persistent=False)
-        _load_pretrained(self.pretrained_model)
+        # torchvision's ResNet-50 without its 1000-way fc: the reference replaces fc after loading (NTSNet.py:19-21)
+        load_pretrained(self.pretrained_model, 'HAWKEYE_RESNET50_PTH', 'resnet50', BODY_KEYS)
 
     def forward(self, x):
         B, T, K = x.shape[0], self.topN, self.CAT_NUM

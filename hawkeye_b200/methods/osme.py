@@ -23,8 +23,8 @@ class OSME_block(nn.Module):
 
     def forward(self, x):
         N, C, H, W = x.size()
-        z = ops_cin.RowMeanFn.apply(x.reshape(N, C, H * W))                              # OSME.py:21
-        h = ops_cin.ReluFn.apply(ops.linear(z, self.block[0].weight, self.block[0].bias))
+        z = ops.RowMeanFn.apply(x.reshape(N, C, H * W))                                  # OSME.py:21
+        h = ops.ReluFn.apply(ops.linear(z, self.block[0].weight, self.block[0].bias))
         m = ops.linear(h, self.block[2].weight, self.block[2].bias)                      # pre-sigmoid excitation
         return ops_cin.SEGateFn.apply(x, m)                                              # sigmoid(m) * x, OSME.py:22-23
 

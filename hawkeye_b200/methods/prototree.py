@@ -23,8 +23,9 @@ import torch
 import torch.nn as nn
 
 from .. import _lib, ops, ops_prototree
-from ..backbone.resnet import resnet50
+from ..backbone.resnet import TRUNK_KEYS, resnet50
 from ..registry import MODEL
+from ..utils import rename_state
 
 
 def _opt(cfg, key, default):
@@ -161,9 +162,6 @@ def inat_resnet50_state(path):
     return out
 
 
-_TRUNK_NAMES = ['conv1', 'bn1', 'relu', 'maxpool', 'layer1', 'layer2', 'layer3', 'layer4']
-
-
 @MODEL.register
 class ProtoTreeNet(nn.Module):
     def __init__(self, config):
@@ -177,14 +175,8 @@ class ProtoTreeNet(nn.Module):
             if not os.path.isfile(pretrain):
                 raise _lib.HawkeyeLibError(f'ProtoTreeNet: model.backbone.pretrain={pretrain!r} is not a file (the iNat '
                                            'ResNet-50 checkpoint); set model.backbone.pretrain to its path, or to \'\'')
-            sd = inat_resnet50_state(pretrain)
             # resnet.load_state_dict(state_dict, strict=False) on the full ResNet: keys outside the trunk are ignored
-            trunk = {}
-            for k, v in sd.items():
-                head = k.split('.')[0]
-                if head in _TRUNK_NAMES:
-                    trunk[str(_TRUNK_NAMES.index(head)) + k[len(head):]] = v
-            self.backbone.load_state_dict(trunk, strict=False)
+            self.backbone.load_state_dict(rename_state(inat_resnet50_state(pretrain), TRUNK_KEYS), strict=False)
         self.neck_conv = nn.Sequential(nn.Conv2d(self.backbone.out_channels, config.num_features, kernel_size=1, bias=False),
                                        nn.Sigmoid())
         self.tree = ProtoTree(config)

@@ -118,6 +118,87 @@ def conv3x3_dgrad(g, wd, mask=None):
 
 
 # ----------------------------------------------------------------------------------------------------------
+# layers the methods share: in-place add, image crops, means, ReLU
+# ----------------------------------------------------------------------------------------------------------
+def add_(a, b):
+    """a += b (contiguous fp32 tensors of one size) -> a"""
+    _lib.call('hk_add_inplace', a, b, a.numel(), _lib.stream_ptr())
+    return a
+
+
+def crop(images, boxes, size, pad):
+    """Bilinear (align_corners=True) crops without a gradient: images NCHW [B, C, H, W], boxes int32 [B, T, 4] as (y0, x0,
+    y1, x1), end exclusive, in the image zero-padded by ``pad`` on every side -> NCHW [B*T, C, size, size]."""
+    _check_cuda(images, boxes)
+    images = _f32c(images.detach())
+    B, C, H, W = images.shape
+    T = boxes.shape[1]
+    out = torch.empty(B * T, C, size, size, device=images.device, dtype=torch.float32)
+    _lib.call('hk_nts_crop', images, boxes.contiguous(), out, B, T, C, H, W, pad, size, _lib.stream_ptr())
+    return out
+
+
+class RowMeanFn(Function):
+    """AdaptiveAvgPool1d(1) over the last dimension (CIN.py:71): [..., P] -> [...]"""
+
+    @staticmethod
+    def forward(ctx, x):
+        _check_cuda(x)
+        x = _f32c(x)
+        P = x.shape[-1]
+        y = torch.empty(x.shape[:-1], device=x.device, dtype=torch.float32)
+        _lib.call('hk_row_mean_fwd', x, y, x.numel() // P, P, P, _lib.stream_ptr())
+        ctx.P = P
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        dy = _f32c(dy)
+        dx = torch.empty(*dy.shape, ctx.P, device=dy.device, dtype=torch.float32)
+        _lib.call('hk_row_mean_bwd', dy, dx, dy.numel(), ctx.P, ctx.P, _lib.stream_ptr())
+        return dx
+
+
+class NHWCMeanFn(Function):
+    """NHWC [N, H, W, C] -> [N, C] spatial mean (AP-CNN's global-pooling branch, MGE-CNN's pooled layer4)."""
+
+    @staticmethod
+    def forward(ctx, x):
+        _check_cuda(x)
+        x = _f32c(x)
+        N, H, W, C = x.shape
+        y = torch.empty(N, C, device=x.device, dtype=torch.float32)
+        ws = _ws(_lib.query('hk_apcnn_pool_workspace_bytes', N, H * W, C), x.device)
+        _lib.call('hk_apcnn_pool', x, y, N, H * W, C, 1.0 / (H * W), ws, ws.numel(), _lib.stream_ptr())
+        ctx.shape = x.shape
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        N, H, W, C = ctx.shape
+        dx = torch.empty(N, H, W, C, device=dy.device, dtype=torch.float32)
+        _lib.call('hk_apcnn_bcast', None, _f32c(dy), dx, N, H * W, C, 1.0 / (H * W), _lib.stream_ptr())
+        return dx
+
+
+class ReluFn(Function):
+    @staticmethod
+    def forward(ctx, x):
+        x = _f32c(x)
+        y = torch.empty_like(x)
+        _lib.call('hk_relu_fwd', x, y, x.numel(), _lib.stream_ptr())
+        ctx.save_for_backward(y)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        (y,) = ctx.saved_tensors
+        dx = torch.empty_like(y)
+        _lib.call('hk_relu_bwd', y, _f32c(dy), dx, y.numel(), _lib.stream_ptr())
+        return dx
+
+
+# ----------------------------------------------------------------------------------------------------------
 # BCNN bilinear pooling (reference model/methods/BCNN.py:8-27)
 # ----------------------------------------------------------------------------------------------------------
 class BilinearPoolFn(Function):

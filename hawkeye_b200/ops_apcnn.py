@@ -10,7 +10,8 @@ import torch
 from torch.autograd import Function
 
 from . import _lib
-from .ops import _check_cuda, _f32c, _ws, conv3x3_dgrad, conv3x3_fwd, conv3x3_pack, conv3x3_wgrad, gemm
+from .ops import (NHWCMeanFn, _check_cuda, _f32c, _ws, conv3x3_dgrad, conv3x3_fwd, conv3x3_pack, conv3x3_wgrad, gemm,
+                  wants_grad)
 
 STRIDES = (8, 16, 32)            # get_att_roi calls, :567-569
 ANCHOR_SIZES = (64, 128, 256)
@@ -80,30 +81,10 @@ class UnitFn(Function):
 
 def unit(x, u, training):
     params = u.params()
-    save = torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params))
-    return UnitFn.apply(x, u, save, training, *params)
+    return UnitFn.apply(x, u, wants_grad(x, params), training, *params)
 
 
-class PoolFn(Function):
-    """NHWC [N, H, W, C] -> [N, C] spatial mean (the AvgPool2d of SimpleFPA's global branch, :194)."""
-
-    @staticmethod
-    def forward(ctx, x):
-        _check_cuda(x)
-        x = _f32c(x)
-        N, H, W, C = x.shape
-        y = torch.empty(N, C, device=x.device, dtype=torch.float32)
-        ws = _ws(_lib.query('hk_apcnn_pool_workspace_bytes', N, H * W, C), x.device)
-        _lib.call('hk_apcnn_pool', x, y, N, H * W, C, 1.0 / (H * W), ws, ws.numel(), _lib.stream_ptr())
-        ctx.shape = x.shape
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        N, H, W, C = ctx.shape
-        dx = torch.empty(N, H, W, C, device=dy.device, dtype=torch.float32)
-        _lib.call('hk_apcnn_bcast', None, _f32c(dy), dx, N, H * W, C, 1.0 / (H * W), _lib.stream_ptr())
-        return dx
+PoolFn = NHWCMeanFn          # the AvgPool2d of SimpleFPA's global branch (:194): NHWC [N, H, W, C] -> [N, C]
 
 
 class BcastAddFn(Function):

@@ -1,12 +1,12 @@
 """Autograd bindings for the channel-interaction module (reference model/methods/CIN.py:24-60): batched Gram and W.X
 products on the wgmma GEMM, softmax(-G), the contrastive weight |W_SCI - w W_SCI_BA|, the 3x3 convolution on the
-implicit-GEMM kernels (NCHW in / out), and the classifier's spatial mean.  Host plumbing only; all arithmetic is in
+implicit-GEMM kernels (NCHW in / out), the residual add and OSME's excitation gate.  Host plumbing only; all arithmetic is in
 libhawkeye_b200.so."""
 import torch
 from torch.autograd import Function
 
 from . import _lib
-from .ops import (_check_cuda, _f32c, conv3x3_dgrad, conv3x3_fwd, conv3x3_pack, conv3x3_wgrad, gemm, nchw_to_nhwc,
+from .ops import (_check_cuda, _f32c, add_, conv3x3_dgrad, conv3x3_fwd, conv3x3_pack, conv3x3_wgrad, gemm, nchw_to_nhwc,
                   nhwc_to_nchw)
 
 
@@ -133,35 +133,12 @@ class Conv3x3NCHWFn(Function):
         return dx, dw, db
 
 
-class RowMeanFn(Function):
-    """AdaptiveAvgPool1d(1) over the last dimension (CIN.py:71): [..., P] -> [...]"""
-
-    @staticmethod
-    def forward(ctx, x):
-        _check_cuda(x)
-        x = _f32c(x)
-        P = x.shape[-1]
-        y = torch.empty(x.shape[:-1], device=x.device, dtype=torch.float32)
-        _lib.call('hk_row_mean_fwd', x, y, x.numel() // P, P, P, _lib.stream_ptr())
-        ctx.P = P
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        dy = _f32c(dy)
-        dx = torch.empty(*dy.shape, ctx.P, device=dy.device, dtype=torch.float32)
-        _lib.call('hk_row_mean_bwd', dy, dx, dy.numel(), ctx.P, ctx.P, _lib.stream_ptr())
-        return dx
-
-
 class AddFn(Function):
     """a + b (residual, CIN.py:38,59) on hk_add_inplace"""
 
     @staticmethod
     def forward(ctx, a, b):
-        out = _f32c(a).clone()
-        _lib.call('hk_add_inplace', out, _f32c(b), out.numel(), _lib.stream_ptr())
-        return out
+        return add_(_f32c(a).clone(), _f32c(b))
 
     @staticmethod
     def backward(ctx, g):
@@ -190,20 +167,3 @@ class SEGateFn(Function):
         dx, dm = torch.empty_like(x), torch.empty_like(m)
         _lib.call('hk_se_gate_bwd', x, m, _f32c(ds), dx, dm, N * C, hw, _lib.stream_ptr())
         return dx, dm
-
-
-class ReluFn(Function):
-    @staticmethod
-    def forward(ctx, x):
-        x = _f32c(x)
-        y = torch.empty_like(x)
-        _lib.call('hk_relu_fwd', x, y, x.numel(), _lib.stream_ptr())
-        ctx.save_for_backward(y)
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        (y,) = ctx.saved_tensors
-        dx = torch.empty_like(y)
-        _lib.call('hk_relu_bwd', y, _f32c(dy), dx, y.numel(), _lib.stream_ptr())
-        return dx

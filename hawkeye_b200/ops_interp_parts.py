@@ -1,7 +1,6 @@
 """Autograd bindings for Interp-Parts (reference model/methods/Interp_Parts.py, model/loss/InterpParts_loss.py): the grouping
-unit, the part attention with the attention-weighted part sum, BatchNorm over [N, C] rows (groupingbn), the blurred part
-occupancy and the shaping loss.  Host plumbing only: shapes are checked here before any launch, all arithmetic is in
-libhawkeye_b200.so.
+unit, the part attention with the attention-weighted part sum, the blurred part occupancy and the shaping loss.  Host
+plumbing only: shapes are checked here before any launch, all arithmetic is in libhawkeye_b200.so.
 
 The shaping loss's gradient reaches the grouping unit without a dense d assign: the grouping node has a third output, a
 zero [N, K] ``sink`` that the occupancy node takes as an input, and the gradient that arrives on the sink is the per-(n, k)
@@ -229,43 +228,3 @@ class AttentionPoolFn(Function):
                   C, D, _lib.stream_ptr())
         return df, dpost, dw, db, dgamma, dbeta, None, None, None, None
 
-
-class RowBatchNormFn(Function):
-    """nn.BatchNorm2d over [P, C] rows (groupingbn on the pooled [N, 2048, 1, 1] features, Interp_Parts.py:365) on
-    hk_bn_fwd / hk_bn_apply and hk_bn_bwd_ex / hk_bn_bwd_frozen."""
-
-    @staticmethod
-    def forward(ctx, x, gamma, beta, bn, training):
-        _check_cuda(x, gamma, beta)
-        x = _f32c(x)
-        P, C = x.shape
-        if training and P < 2:
-            raise _lib.HawkeyeLibError(f'groupingbn: BatchNorm in train mode needs more than one row (got {P})')
-        s = _lib.stream_ptr()
-        y = torch.empty_like(x)
-        if training:
-            mean = torch.empty(C, device=x.device, dtype=torch.float32)
-            invstd = torch.empty(C, device=x.device, dtype=torch.float32)
-            ws = _ws(_lib.query('hk_bn_workspace_bytes', P, C), x.device)
-            _lib.call('hk_bn_fwd', x, gamma, beta, None, y, mean, invstd, bn.running_mean, bn.running_var, float(bn.momentum),
-                      float(bn.eps), P, C, 0, ws, ws.numel(), s)
-            bn.num_batches_tracked += 1
-        else:
-            mean = bn.running_mean
-            invstd = torch.rsqrt(bn.running_var + bn.eps)
-            _lib.call('hk_bn_apply', x, mean, invstd, gamma, beta, None, y, P, C, 0, s)
-        ctx.save_for_backward(x, gamma, mean, invstd)
-        ctx.frozen = not training
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        x, gamma, mean, invstd = ctx.saved_tensors
-        P, C = x.shape
-        dx = torch.empty_like(x)
-        dgamma = torch.empty(C, device=x.device, dtype=torch.float32)
-        dbeta = torch.empty(C, device=x.device, dtype=torch.float32)
-        ws = _ws(_lib.query('hk_bn_workspace_bytes', P, C), x.device)
-        _lib.call('hk_bn_bwd_frozen' if ctx.frozen else 'hk_bn_bwd_ex', x, None, _f32c(dy), gamma, None, mean, invstd, dx,
-                  None, dgamma, dbeta, P, C, 0, ws, ws.numel(), _lib.stream_ptr())
-        return dx, dgamma, dbeta, None, None

@@ -10,7 +10,7 @@ import torch
 from torch.autograd import Function
 
 from . import _lib
-from .ops import _check_cuda, _f32c, _ws
+from .ops import _check_cuda, _f32c, _ws, crop as _crop
 
 CAT_SCALE = 10.0            # pool_cat* = cat(10 l2n(pool), 10 l2n(pool_conv6)), MGE.py:136
 
@@ -73,13 +73,8 @@ def cam_box(feat_nhwc, w_main, image_size, rate, logits=None, targets=None):
 
 def crop(images, boxes, image_size):
     """input_box of get_bbox: images NCHW [N, 3, S, S], boxes int32 [N, 4] -> NCHW [N, 3, S, S], each box resized to S x S
-    (bilinear, align_corners=True) without a gradient, on hk_nts_crop with no padding."""
-    _check_cuda(images, boxes)
-    images = _f32c(images.detach())
-    N, C, H, W = images.shape
-    out = torch.empty(N, C, image_size, image_size, device=images.device, dtype=torch.float32)
-    _lib.call('hk_nts_crop', images, boxes.contiguous(), out, N, 1, C, H, W, 0, int(image_size), _lib.stream_ptr())
-    return out
+    (bilinear, align_corners=True) without a gradient: one box per image, no padding."""
+    return _crop(images, boxes.reshape(-1, 1, 4), int(image_size), 0)
 
 
 def cat_l2n(a, b, scale=CAT_SCALE):

@@ -8,7 +8,7 @@ import torch
 from torch.autograd import Function
 
 from . import _lib
-from .ops import _check_cuda, _f32c, conv3x3_dgrad, conv3x3_fwd, conv3x3_pack, conv3x3_wgrad
+from .ops import _check_cuda, _f32c, add_, conv3x3_dgrad, conv3x3_fwd, conv3x3_pack, conv3x3_wgrad, crop as _crop
 
 PAD = 224                   # NTSNet.pad_side: the anchors live in the image zero-padded by 224 on every side (:26-27, :31)
 PART_SIZE = 224             # every part image is resized to 224 x 224 (:43-48)
@@ -41,11 +41,6 @@ def _down_bwd(x, g, wd, stride2, need_dx):
     db = torch.empty(cout, device=g.device, dtype=torch.float32)
     conv3x3_wgrad(x, g, dw, db)
     return dw, db, (conv3x3_dgrad(g, wd, mask=x) if need_dx else None)
-
-
-def _add_(a, b):
-    _lib.call('hk_add_inplace', a, b, a.numel(), _lib.stream_ptr())
-    return a
 
 
 def nms(scores, anchors, topn):
@@ -111,9 +106,9 @@ class ProposalFn(Function):
                   dt[1][0], dt[1][1], dt[2][0], dt[2][1], B, T, d1.shape[1], d1.shape[2], d2.shape[1], d2.shape[2],
                   d3.shape[1], d3.shape[2], d1.shape[-1], s)
         dw3, db3, dx = _down_bwd(d2, g[2], wd3, True, True)
-        _add_(g[1], dx)
+        add_(g[1], dx)
         dw2, db2, dx = _down_bwd(d1, g[1], wd2, True, True)
-        _add_(g[0], dx)
+        add_(g[0], dx)
         dw1, db1, _ = _down_bwd(x, g[0], None, False, False)
         return (None, None, None, None, dw1, db1, dw2, db2, dw3, db3, dt[0][0], dt[0][1], dt[1][0], dt[1][1], dt[2][0],
                 dt[2][1])
@@ -129,13 +124,7 @@ def proposal(x_nhwc, net, anchors, topn):
 def crop(images, boxes, size=PART_SIZE, pad=PAD):
     """The part images of NTSNet.py:40-49 without a gradient (the reference detaches them, :50): images NCHW [B, C, H, W],
     boxes int32 [B, T, 4] in the padded image -> NCHW [B*T, C, size, size]."""
-    _check_cuda(images, boxes)
-    images = _f32c(images.detach())
-    B, C, H, W = images.shape
-    T = boxes.shape[1]
-    out = torch.empty(B * T, C, size, size, device=images.device, dtype=torch.float32)
-    _lib.call('hk_nts_crop', images, boxes.contiguous(), out, B, T, C, H, W, pad, size, _lib.stream_ptr())
-    return out
+    return _crop(images, boxes, size, pad)
 
 
 class DropoutFn(Function):

@@ -1,5 +1,6 @@
 """ResNet-50 v1.5 trunk (reference model/backbone/resnet.py:89-252) and the MPN-COV dimension-reduction block
-(MPNCOV.py:64-69) as explicit forward/backward pipelines over the C-ABI kernels.  NHWC fp32 inside.
+(MPNCOV.py:64-69) as explicit forward/backward pipelines over the C-ABI kernels, NHWC fp32 inside, and the same BatchNorm
+over [P, C] rows for the methods' heads (RowBatchNormFn).
 
 conv unit = convolution (wgmma GEMM / implicit GEMM) -> BatchNorm (+ residual) (+ ReLU).  BatchNorm runs on the batch
 statistics in train mode and on the running statistics in eval mode; both have a backward (eval mode: the statistics are
@@ -9,8 +10,8 @@ import torch
 from torch.autograd import Function
 
 from . import _lib, ops as _ops
-from .ops import (_check_cuda, _f32c, _ws, conv3x3_dgrad, conv3x3_fwd, conv3x3_pack, conv3x3_wgrad, gemm, nchw_to_nhwc,
-                  nhwc_to_nchw)
+from .ops import (_check_cuda, _f32c, _ws, add_, conv3x3_dgrad, conv3x3_fwd, conv3x3_pack, conv3x3_wgrad, gemm,
+                  nchw_to_nhwc, nhwc_to_nchw)
 
 BN_EPS = 1e-5
 
@@ -60,19 +61,7 @@ class Unit:
                 Ho, Wo = c.shape[1:3]
                 rec['xin'] = x
             P = N * Ho * Wo
-        y = torch.empty_like(c)
-        bn = self.bn
-        if training:
-            mean = torch.empty(cout, device=dev, dtype=torch.float32)
-            invstd = torch.empty(cout, device=dev, dtype=torch.float32)
-            ws = _ws(_lib.query('hk_bn_workspace_bytes', P, cout), dev)
-            _lib.call('hk_bn_fwd', c, gamma, beta, residual, y, mean, invstd, bn.running_mean, bn.running_var,
-                      float(bn.momentum), float(bn.eps), P, cout, int(self.relu), ws, ws.numel(), s)
-            bn.num_batches_tracked += 1
-        else:
-            mean = bn.running_mean
-            invstd = torch.rsqrt(bn.running_var + bn.eps)
-            _lib.call('hk_bn_apply', c, mean, invstd, gamma, beta, residual, y, P, cout, int(self.relu), s)
+        y, mean, invstd = bn_forward(c, P, cout, gamma, beta, residual, self.bn, training, self.relu, s)
         if _ops.CAPTURE is not None and self.relu:
             _ops.CAPTURE.append(('relu', y))
         if save:
@@ -88,15 +77,10 @@ class Unit:
         dev = dy.device
         P, cout = rec['P'], rec['cout']
         N, Ho, Wo = rec['shape']
-        dc = torch.empty(N, Ho, Wo, cout, device=dev, dtype=torch.float32)
-        dres = torch.empty_like(dc) if rec['has_res'] else None
-        dgamma = torch.empty(cout, device=dev, dtype=torch.float32)
-        dbeta = torch.empty(cout, device=dev, dtype=torch.float32)
-        ws = _ws(_lib.query('hk_bn_workspace_bytes', P, cout), dev)
         # BN + ReLU without a residual: the mask is recomputed from x (hk_bn_bwd_ex), y is not read
         mask_beta = rec['beta'] if (self.relu and not rec['has_res']) else None
-        _lib.call('hk_bn_bwd_frozen' if rec['frozen'] else 'hk_bn_bwd_ex', rec['c'], rec['y'], dy, rec['gamma'], mask_beta,
-                  rec['mean'], rec['invstd'], dc, dres, dgamma, dbeta, P, cout, int(self.relu), ws, ws.numel(), s)
+        dc, dres, dgamma, dbeta = bn_backward(rec['c'], rec['y'], dy, rec['gamma'], mask_beta, rec['mean'], rec['invstd'],
+                                              rec['has_res'], self.relu, rec['frozen'], P, cout, s)
         w, xin = rec['w'], rec['xin']
         dx = None
         if self.kind == 'stem':
@@ -134,13 +118,41 @@ class Unit:
             if need_dx:
                 dx = conv3x3_dgrad(g, rec['wd'])
         if addend is not None and dx is not None:
-            dx = _add(dx, addend)
+            dx = add_(dx, addend)
         return dx, dres, dw, dgamma, dbeta
 
 
-def _add(a, b):
-    _lib.call('hk_add_inplace', a, b, a.numel(), _lib.stream_ptr())
-    return a
+def bn_forward(x, P, C, gamma, beta, residual, bn, training, relu, s):
+    """BatchNorm of x as [P, C] rows (+ residual) (+ ReLU) with the parameters gamma, beta and the statistics of the
+    nn.BatchNorm ``bn`` -> (y, mean, invstd).  Train mode normalises with the batch statistics, updates the running ones and
+    counts ``num_batches_tracked``; eval mode normalises with the running statistics."""
+    y = torch.empty_like(x)
+    if training:
+        mean = torch.empty(C, device=x.device, dtype=torch.float32)
+        invstd = torch.empty(C, device=x.device, dtype=torch.float32)
+        ws = _ws(_lib.query('hk_bn_workspace_bytes', P, C), x.device)
+        _lib.call('hk_bn_fwd', x, gamma, beta, residual, y, mean, invstd, bn.running_mean, bn.running_var,
+                  float(bn.momentum), float(bn.eps), P, C, int(relu), ws, ws.numel(), s)
+        bn.num_batches_tracked += 1
+    else:
+        mean = bn.running_mean
+        invstd = torch.rsqrt(bn.running_var + bn.eps)
+        _lib.call('hk_bn_apply', x, mean, invstd, gamma, beta, residual, y, P, C, int(relu), s)
+    return y, mean, invstd
+
+
+def bn_backward(x, y, dy, gamma, mask_beta, mean, invstd, has_res, relu, frozen, P, C, s):
+    """The backward of bn_forward from its input x, output y (read for the ReLU mask unless ``mask_beta`` lets the kernel
+    recompute it from x) and (mean, invstd) -> (dx, dresidual or None, dgamma, dbeta).  ``frozen`` (eval mode) holds the
+    statistics constant."""
+    dx = torch.empty_like(x)
+    dres = torch.empty_like(dx) if has_res else None
+    dgamma = torch.empty(C, device=x.device, dtype=torch.float32)
+    dbeta = torch.empty(C, device=x.device, dtype=torch.float32)
+    ws = _ws(_lib.query('hk_bn_workspace_bytes', P, C), x.device)
+    _lib.call('hk_bn_bwd_frozen' if frozen else 'hk_bn_bwd_ex', x, y, dy, gamma, mask_beta, mean, invstd, dx, dres, dgamma,
+              dbeta, P, C, int(relu), ws, ws.numel(), s)
+    return dx, dres, dgamma, dbeta
 
 
 def block_units(blk):
@@ -322,3 +334,28 @@ class DRBlockFn(Function):
         dx, _, dw, dg, db = ctx.unit.backward(ctx.rec, nchw_to_nhwc(_f32c(dout)))
         ctx.rec = None
         return nhwc_to_nchw(dx), None, None, None, dw, dg, db
+
+
+class RowBatchNormFn(Function):
+    """nn.BatchNorm over [P, C] rows (Interp-Parts' groupingbn on the pooled features, Interp_Parts.py:365; AP-CNN's
+    BatchNorm1d heads) on bn_forward / bn_backward."""
+
+    @staticmethod
+    def forward(ctx, x, gamma, beta, bn, training):
+        _check_cuda(x, gamma, beta)
+        x = _f32c(x)
+        P, C = x.shape
+        if training and P < 2:
+            raise _lib.HawkeyeLibError(f'BatchNorm over rows: train mode needs more than one row (got {P})')
+        y, mean, invstd = bn_forward(x, P, C, gamma, beta, None, bn, training, False, _lib.stream_ptr())
+        ctx.save_for_backward(x, gamma, mean, invstd)
+        ctx.frozen = not training
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, gamma, mean, invstd = ctx.saved_tensors
+        P, C = x.shape
+        dx, _, dgamma, dbeta = bn_backward(x, None, _f32c(dy), gamma, None, mean, invstd, False, False, ctx.frozen, P, C,
+                                           _lib.stream_ptr())
+        return dx, dgamma, dbeta, None, None

@@ -225,7 +225,7 @@ def main():
         p_ = ops_resnet.block_stack(region, m._post_blocks, True)
         pooled, att = OP.AttentionPoolFn.apply(a_.view(N * K, -1), p_.view(N * K, -1), m.attconv[2].weight, m.attconv[2].bias,
                                                m.attconv[3].weight, m.attconv[3].bias, m.attconv[3], True, N, K)
-        out = OP.RowBatchNormFn.apply(pooled, m.groupingbn.weight, m.groupingbn.bias, m.groupingbn, True)
+        out = ops_resnet.RowBatchNormFn.apply(pooled, m.groupingbn.weight, m.groupingbn.bias, m.groupingbn, True)
         logits = ops.linear(out, m.mylinear.weight, m.mylinear.bias)
         crit((logits, att.view(N, 1, K, 1), assign), labels).backward()
 

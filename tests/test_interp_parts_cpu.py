@@ -56,21 +56,6 @@ def test_registration_and_yaml(monkeypatch):
     assert cfg.dataset.batch_size == 16 and cfg.dataset.transformer.image_size == 448
 
 
-def test_pretrained_trunk_loads(monkeypatch, tmp_path):
-    from hawkeye_b200.registry import MODEL
-    from hawkeye_b200.config import load_config
-    import hawkeye_b200.methods  # noqa: F401
-    src = _net((3, 4, 6, 3))
-    sd = {k: v for k, v in detgen.state_like(src).items() if k.split('.')[0] in ('conv1', 'bn1', 'layer1', 'layer2', 'layer3')}
-    sd['fc.weight'] = torch.zeros(1000, 2048)                               # torchvision's classifier: not loaded
-    path = tmp_path / 'resnet50.pth'
-    torch.save(sd, path)
-    monkeypatch.setenv('HAWKEYE_RESNET50_PTH', str(path))
-    cfg = load_config(os.path.join(REPO, 'configs', 'InterpPartsNet.yaml'))
-    net = MODEL.get('IP_ResNet50')(cfg.model)
-    assert torch.equal(net.layer3[0].conv2.weight, sd['layer3.0.conv2.weight'])
-
-
 def test_rejected_options():
     from hawkeye_b200 import _lib, ops_interp_parts as OP
     from hawkeye_b200.cfgnode import CfgNode
