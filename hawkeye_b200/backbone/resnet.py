@@ -5,7 +5,7 @@ The modules below are parameter containers (same attribute names => same state_d
 """
 import torch.nn as nn
 
-from .. import ops_resnet
+from .. import ops, ops_resnet
 from ..registry import BACKBONE
 from ..utils import load_pretrained
 
@@ -80,7 +80,7 @@ class ResNetTrunk(nn.Sequential):
         self.__dict__['_plan'] = ops_resnet.TrunkPlan(self)
 
     def forward(self, x):
-        return ops_resnet.resnet_trunk(x, self)
+        return ops.ToNCHWFn.apply(ops_resnet.resnet_trunk(x, self._plan, self.training))
 
 
 TRUNK_KEYS = {n: str(i) for i, n in enumerate(RESNET_NAMES)}      # torchvision's top-level name -> ResNetTrunk index

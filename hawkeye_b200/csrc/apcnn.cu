@@ -529,24 +529,8 @@ __global__ void ap_refine_bwd_kernel(const float* __restrict__ dy, const int* __
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// heads: ReLU / ELU on vectors, the bottom-up channel attention with the attended pool, and mask_cat
+// heads: the bottom-up channel attention with the attended pool, and mask_cat
 // ---------------------------------------------------------------------------------------------------------------
-__global__ void ap_act_fwd_kernel(const float* __restrict__ x, float* __restrict__ y, size_t n, int elu) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const float v = x[i];
-    y[i] = v > 0.f ? v : (elu ? expm1f(v) : 0.f);
-  }
-}
-
-// from the output: ReLU passes where y > 0; ELU (alpha 1) has slope y + 1 where y <= 0
-__global__ void ap_act_bwd_kernel(const float* __restrict__ y, const float* __restrict__ dy, float* __restrict__ dx, size_t n,
-                                  int elu) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const float v = y[i];
-    dx[i] = v > 0.f ? dy[i] : (elu ? dy[i] * (v + 1.f) : 0.f);
-  }
-}
-
 // z, pm, psf, v, ch: [3, N, C] (levels 3, 4, 5).  ch_3 = sig(z_3), ch_4 = (sig(z_4) + ch_3) / 2, ch_5 = (sig(z_5) + ch_4) / 2
 // (PyramidAttentions.forward, :251-268); v_l = psf_l + ch_l pm_l = mean_hw((s_l + ch_l) F_l).
 __global__ void ap_mix_fwd_kernel(const float* __restrict__ z, const float* __restrict__ pm, const float* __restrict__ psf,
@@ -749,20 +733,6 @@ int hk_apcnn_refine_bwd(const float* dy, const int* meta, float* dx, int N, int 
   HK_REQUIRE(aligned16(dy) && aligned16(dx), HK_ERR_ALIGN, "hk_apcnn_refine_bwd: 16-byte alignment");
   ap_refine_bwd_kernel<<<grid_1d((size_t)N * H * W * (C / 4), 256), 256, 0, (cudaStream_t)stream>>>(dy, meta, dx, N, H, W, C / 4);
   HK_LAUNCH_CHECK("ap_refine_bwd_kernel");
-  return 0;
-}
-
-int hk_apcnn_act_fwd(const float* x, float* y, size_t n, int elu, void* stream) {
-  HK_REQUIRE(x && y && n > 0, HK_ERR_ARG, "hk_apcnn_act_fwd: null pointer or n = 0");
-  ap_act_fwd_kernel<<<grid_1d(n, 256), 256, 0, (cudaStream_t)stream>>>(x, y, n, elu);
-  HK_LAUNCH_CHECK("ap_act_fwd_kernel");
-  return 0;
-}
-
-int hk_apcnn_act_bwd(const float* y, const float* dy, float* dx, size_t n, int elu, void* stream) {
-  HK_REQUIRE(y && dy && dx && n > 0, HK_ERR_ARG, "hk_apcnn_act_bwd: null pointer or n = 0");
-  ap_act_bwd_kernel<<<grid_1d(n, 256), 256, 0, (cudaStream_t)stream>>>(y, dy, dx, n, elu);
-  HK_LAUNCH_CHECK("ap_act_bwd_kernel");
   return 0;
 }
 

@@ -111,13 +111,6 @@ __global__ void se_gate_bwd_kernel(const float* __restrict__ x, const float* __r
   acc = warp_sum(acc);
   if (lane == 0) dm[r] = acc * g * (1.f - g);
 }
-__global__ void relu_fwd_kernel(const float* __restrict__ x, float* __restrict__ y, size_t n) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) y[i] = fmaxf(x[i], 0.f);
-}
-__global__ void relu_bwd_kernel(const float* __restrict__ y, const float* __restrict__ dy, float* __restrict__ dx, size_t n) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    dx[i] = y[i] > 0.f ? dy[i] : 0.f;
-}
 
 }  // namespace hk
 
@@ -164,18 +157,6 @@ int hk_se_gate_bwd(const float* x, const float* m, const float* ds, float* dx, f
   HK_REQUIRE(x && m && ds && dx && dm && rows > 0 && hw > 0, HK_ERR_ARG, "hk_se_gate_bwd: bad args");
   se_gate_bwd_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream>>>(x, m, ds, dx, dm, rows, hw);
   HK_LAUNCH_CHECK("se_gate_bwd_kernel");
-  return 0;
-}
-int hk_relu_fwd(const float* x, float* y, size_t n, void* stream) {
-  HK_REQUIRE(x && y, HK_ERR_ARG, "hk_relu_fwd: null pointer");
-  relu_fwd_kernel<<<grid_1d(n, 256), 256, 0, (cudaStream_t)stream>>>(x, y, n);
-  HK_LAUNCH_CHECK("relu_fwd_kernel");
-  return 0;
-}
-int hk_relu_bwd(const float* y, const float* dy, float* dx, size_t n, void* stream) {
-  HK_REQUIRE(y && dy && dx, HK_ERR_ARG, "hk_relu_bwd: null pointer");
-  relu_bwd_kernel<<<grid_1d(n, 256), 256, 0, (cudaStream_t)stream>>>(y, dy, dx, n);
-  HK_LAUNCH_CHECK("relu_bwd_kernel");
   return 0;
 }
 int hk_row_mean_fwd(const float* x, float* y, long long rows, int cols, int ld, void* stream) {

@@ -1197,16 +1197,6 @@ __global__ void bias_grad_kernel(const float* __restrict__ dy, float* __restrict
   }
 }
 
-// elementwise: dy *= (act > 0)
-__global__ void relu_mask_kernel(float* __restrict__ dy, const float* __restrict__ act, size_t n4) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
-    float4 g = reinterpret_cast<float4*>(dy)[i];
-    const float4 a = reinterpret_cast<const float4*>(act)[i];
-    g.x = a.x > 0.f ? g.x : 0.f; g.y = a.y > 0.f ? g.y : 0.f; g.z = a.z > 0.f ? g.z : 0.f; g.w = a.w > 0.f ? g.w : 0.f;
-    reinterpret_cast<float4*>(dy)[i] = g;
-  }
-}
-
 }  // namespace hk
 
 using namespace hk;
@@ -1368,13 +1358,6 @@ int hk_maxpool2x2_bwd_idx(const unsigned char* code, const float* dy, float* dx_
   const size_t total = (size_t)N * (H / 2) * (W / 2) * (C / 4);
   maxpool2x2_bwd_idx_kernel<<<grid_1d(total, 256), 256, 0, (cudaStream_t)stream>>>(code, dy, dx_nhwc, N, H, W, C, dy_nchw);
   HK_LAUNCH_CHECK("maxpool2x2_bwd_idx_kernel");
-  return 0;
-}
-
-int hk_relu_mask_inplace(float* dy, const float* act, size_t n, void* stream) {
-  HK_REQUIRE(dy && act && n % 4 == 0, HK_ERR_ARG, "hk_relu_mask_inplace: bad args");
-  relu_mask_kernel<<<grid_1d(n / 4, 256), 256, 0, (cudaStream_t)stream>>>(dy, act, n / 4);
-  HK_LAUNCH_CHECK("relu_mask_kernel");
   return 0;
 }
 

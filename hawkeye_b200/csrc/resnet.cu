@@ -1,7 +1,8 @@
 // Support kernels of the ResNet-50 v1.5 trunk (reference model/backbone/resnet.py:89-252) around the tensor-core
 // convolutions: 7x7/s2 stem patch extraction, train-mode BatchNorm2d (batch statistics, running-stat update,
 // fused residual add + ReLU) forward/backward, MaxPool2d(3,2,1), stride-2 sub/up-sampling, 1x1-conv weight
-// gradient (split-K GEMM).  All activations NHWC fp32; every kernel here is HBM-bound.
+// gradient (split-K GEMM), and the elementwise layers the methods share (in-place add, ReLU / ELU, NCHW <-> NHWC).
+// All activations NHWC fp32; every kernel here is HBM-bound.
 #include "common.cuh"
 #include "host.h"
 #include "gemm.h"
@@ -343,6 +344,22 @@ __global__ void nhwc_to_nchw_kernel(const float* __restrict__ x, float* __restri
     y[i] = x[((size_t)n * HW + p) * C + c];
   }
 }
+// ReLU (elu = 0) or ELU with alpha 1 (elu = 1)
+__global__ void act_fwd_kernel(const float* __restrict__ x, float* __restrict__ y, size_t n, int elu) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float v = x[i];
+    y[i] = v > 0.f ? v : (elu ? expm1f(v) : 0.f);
+  }
+}
+
+// from the output: ReLU passes where y > 0; ELU (alpha 1) has slope y + 1 where y <= 0
+__global__ void act_bwd_kernel(const float* __restrict__ y, const float* __restrict__ dy, float* __restrict__ dx, size_t n,
+                               int elu) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float v = y[i];
+    dx[i] = v > 0.f ? dy[i] : (elu ? dy[i] * (v + 1.f) : 0.f);
+  }
+}
 __global__ void nchw_to_nhwc_kernel(const float* __restrict__ x, float* __restrict__ y, int N, int HW, int C) {
   const size_t total = (size_t)N * HW * C;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
@@ -520,6 +537,18 @@ int hk_nchw_to_nhwc(const float* x, float* y, int N, int HW, int C, void* stream
   HK_REQUIRE(x && y, HK_ERR_ARG, "hk_nchw_to_nhwc: null pointer");
   nchw_to_nhwc_kernel<<<grid_1d((size_t)N * HW * C, 256), 256, 0, (cudaStream_t)stream>>>(x, y, N, HW, C);
   HK_LAUNCH_CHECK("nchw_to_nhwc_kernel");
+  return 0;
+}
+int hk_act_fwd(const float* x, float* y, size_t n, int elu, void* stream) {
+  HK_REQUIRE(x && y && n > 0, HK_ERR_ARG, "hk_act_fwd: null pointer or n = 0");
+  act_fwd_kernel<<<grid_1d(n, 256), 256, 0, (cudaStream_t)stream>>>(x, y, n, elu);
+  HK_LAUNCH_CHECK("act_fwd_kernel");
+  return 0;
+}
+int hk_act_bwd(const float* y, const float* dy, float* dx, size_t n, int elu, void* stream) {
+  HK_REQUIRE(y && dy && dx && n > 0, HK_ERR_ARG, "hk_act_bwd: null pointer or n = 0");
+  act_bwd_kernel<<<grid_1d(n, 256), 256, 0, (cudaStream_t)stream>>>(y, dy, dx, n, elu);
+  HK_LAUNCH_CHECK("act_bwd_kernel");
   return 0;
 }
 

@@ -46,7 +46,7 @@ class BasicConv(nn.Module):
         self.__dict__['_unit'] = ops_resnet.Unit('1x1', self.conv, self.bn, True)
 
     def forward(self, x_nhwc):
-        return ops_apcnn.unit(x_nhwc, self._unit, self.training)
+        return ops_resnet.unit(x_nhwc, self._unit, self.training)
 
 
 class SimpleFPA(nn.Module):
@@ -60,7 +60,7 @@ class SimpleFPA(nn.Module):
 
     def forward(self, x):
         N, _, _, C = x.shape
-        gpb = self.conv_gpb(ops_apcnn.PoolFn.apply(x).view(N, 1, 1, C))
+        gpb = self.conv_gpb(ops.NHWCMeanFn.apply(x).view(N, 1, 1, C))
         return ops_apcnn.BcastAddFn.apply(self.conv_master(x), gpb.view(N, -1))
 
 
@@ -78,7 +78,7 @@ class PyramidFeatures(nn.Module):
 
     def forward(self, inputs):
         B3, B4, B5 = inputs
-        c1, c3 = ops_apcnn.Conv1x1BiasFn.apply, ops_apcnn.Conv3x3BiasFn.apply
+        c1, c3 = ops.Conv1x1Fn.apply, ops.Conv3x3Fn.apply
         P5 = self.P5_1(B5)
         P4 = ops_apcnn.LateralFn.apply(P5, c1(B4, self.P4_1.weight, self.P4_1.bias))
         P3 = ops_apcnn.LateralFn.apply(P4, c1(B3, self.P3_1.weight, self.P3_1.bias))
@@ -101,7 +101,7 @@ class ChannelGate(nn.Module):
     def forward(self, pooled):
         """mean_hw F [N, C] -> conv2's output before the sigmoid (:291-294)."""
         w1, w2 = self.conv1.weight, self.conv2.weight
-        h = ops_apcnn.ActFn.apply(ops.linear(pooled, w1.view(w1.shape[0], -1), self.conv1.bias), False)
+        h = ops.ActFn.apply(ops.linear(pooled, w1.view(w1.shape[0], -1), self.conv1.bias), False)
         return ops.linear(h, w2.view(w2.shape[0], -1), self.conv2.bias)
 
 
@@ -144,7 +144,7 @@ def _run_head(seq, v, training):
     bn1, fc1, bn2, _, fc2 = list(seq)[-5:]
     v = RowBatchNormFn.apply(v, bn1.weight, bn1.bias, bn1, training)
     v = RowBatchNormFn.apply(ops.linear(v, fc1.weight, fc1.bias), bn2.weight, bn2.bias, bn2, training)
-    return ops.linear(ops_apcnn.ActFn.apply(v, True), fc2.weight, fc2.bias)
+    return ops.linear(ops.ActFn.apply(v, True), fc2.weight, fc2.bias)
 
 
 class ResNet(ResNetBody):
@@ -196,7 +196,7 @@ class ResNet(ResNetBody):
         win = self.check_input(img_h, img_w)
         if self.training and n < 2:
             raise ValueError('APCNN: the heads\' BatchNorm1d needs more than one image in train mode')
-        x2 = ops_resnet.resnet_trunk_nhwc(inputs, self._plan, self.training)
+        x2 = ops_resnet.resnet_trunk(inputs, self._plan, self.training)
         outs1, gates = self.stage(x2)
         boxes, counts = ops_apcnn.roi_select(gates, torch.from_numpy(win), self.nms_keep, img_h, img_w)
         if self.training and draws is None:

@@ -28,7 +28,8 @@ class ChannelInteractionModule(nn.Module):
 
     def _conv(self, yp, B, C, W, H, WH):
         y = yp[:, :, :WH] if yp.shape[-1] != WH else yp
-        return ops_cin.Conv3x3NCHWFn.apply(y.reshape(B, C, W, H), self.conv.weight, self.conv.bias).view(B, C, WH)
+        y = ops.Conv3x3Fn.apply(ops.ToNHWCFn.apply(y.reshape(B, C, W, H)), self.conv.weight, self.conv.bias)
+        return ops.ToNCHWFn.apply(y).view(B, C, WH)
 
     def _fc(self, v):
         # nn.Linear(., 1): the GEMM kernels want a 16-byte pitch on the [rows, out] side, so the single output row is padded

@@ -102,7 +102,7 @@ class ResNet(ResNetBody):
     def forward(self, x):
         N = x.shape[0]
         K = self.n_parts
-        feat = ops_resnet.resnet_trunk_nhwc(x, self._trunk_plan, self.training)          # NHWC [N, H, W, 1024]
+        feat = ops_resnet.resnet_trunk(x, self._trunk_plan, self.training)          # NHWC [N, H, W, 1024]
         region, assign = self.grouping(feat)                                              # [N, K, C]: NHWC [N, K, 1, C]
         region = region.view(N, K, 1, region.shape[-1])
         a = ops_resnet.block_stack(region, self._att_blocks, self.training)

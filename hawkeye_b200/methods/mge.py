@@ -89,7 +89,7 @@ class LocalCamNet(nn.Module):
     def trunk(self, x, branch):
         """conv4 and conv5 of ``branch`` on an NCHW image -> (NHWC layer3 map, NHWC layer4 map, pooled [N, 2048])."""
         plan, blocks = self._plans[branch]
-        c4 = ops_resnet.resnet_trunk_nhwc(x, plan, self.training)
+        c4 = ops_resnet.resnet_trunk(x, plan, self.training)
         c5 = ops_resnet.block_stack(c4, blocks, self.training)
         return c4, c5, ops.NHWCMeanFn.apply(c5)
 

@@ -26,10 +26,7 @@ class MPNCOV(nn.Module):
 
     def forward(self, x):
         if self.dr is not None:
-            u = self._dr_unit
-            ps = u.params()
-            save = ops.wants_grad(x, ps)
-            x = ops_resnet.DRBlockFn.apply(x, u, save, self.training, *ps)
+            x = ops.ToNCHWFn.apply(ops_resnet.unit(ops.ToNHWCFn.apply(x), self._dr_unit, self.training))
         x = ops.CovpoolLayer(x)
         if self.is_sqrt:
             x = ops.SqrtmLayer(x, self.iterNum)

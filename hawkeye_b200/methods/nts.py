@@ -86,8 +86,7 @@ class ResNet(ResNetBody):
         self.__dict__['_plan'] = ops_resnet.TrunkPlan(self.trunk_modules())
 
     def forward(self, x, seed, call):
-        params = self._plan.params()
-        fmap = ops_resnet.ResNetTrunkFn.apply(x, self._plan, ops.wants_grad(x, params), self.training, False, *params)
+        fmap = ops.ToNCHWFn.apply(ops_resnet.resnet_trunk(x, self._plan, self.training))
         n, C, H, W = fmap.shape
         feature = ops_nts.dropout(ops.RowMeanFn.apply(fmap.reshape(n, C, H * W)), float(self.drop.p), seed, call)
         return ops.linear(feature, self.fc.weight, self.fc.bias), fmap, feature

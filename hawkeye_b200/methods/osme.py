@@ -3,7 +3,7 @@
 ``OSME_block`` = squeeze (spatial mean) -> Linear -> ReLU -> Linear -> sigmoid -> channel-wise re-scaling of the feature map;
 ``OSME`` = P such blocks, each followed by a Linear over the flattened gated map; ``OSMENet`` = ResNet-101 trunk + OSME +
 classifier, returning ``(logits, per-attention features)`` for the MAMC loss (model/loss/MAMC_loss.py, not part of this package).
-All arithmetic runs on the library's kernels (hk_row_mean, hk_linear, hk_relu, hk_se_gate); the reference hard-codes a 7x7 feature
+All arithmetic runs on the library's kernels (hk_row_mean, hk_linear, hk_act, hk_se_gate); the reference hard-codes a 7x7 feature
 map (OSME.py:57) — here ``config.feature_shape`` may override it (14 for 448x448 inputs).
 """
 import torch
@@ -24,7 +24,7 @@ class OSME_block(nn.Module):
     def forward(self, x):
         N, C, H, W = x.size()
         z = ops.RowMeanFn.apply(x.reshape(N, C, H * W))                                  # OSME.py:21
-        h = ops.ReluFn.apply(ops.linear(z, self.block[0].weight, self.block[0].bias))
+        h = ops.ActFn.apply(ops.linear(z, self.block[0].weight, self.block[0].bias), False)
         m = ops.linear(h, self.block[2].weight, self.block[2].bias)                      # pre-sigmoid excitation
         return ops_cin.SEGateFn.apply(x, m)                                              # sigmoid(m) * x, OSME.py:22-23
 

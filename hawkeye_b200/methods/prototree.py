@@ -186,6 +186,12 @@ class ProtoTreeNet(nn.Module):
 
     def forward(self, x):
         feat = self.backbone(x)
-        c = ops_prototree.NeckFn.apply(feat, self.neck_conv[0].weight)
+        w = self.neck_conv[0].weight
+        if feat.dim() != 4 or w.dim() != 4 or w.shape[1] != feat.shape[1] or w.shape[2:] != (1, 1):
+            raise _lib.HawkeyeLibError(f'ProtoTree neck: map {tuple(feat.shape)} and weight {tuple(w.shape)} are not a '
+                                       '[N, C, H, W] map and a [D, C, 1, 1] convolution')
+        N, _, H, W = feat.shape
+        # the neck's pre-activation [N, H*W, D], position-major: the layout hk_prototree_dist_fwd reads
+        c = ops.Conv1x1Fn.apply(ops.ToNHWCFn.apply(feat), w, None).view(N, H * W, w.shape[0])
         mind, _ = ops_prototree.PrototypeDistanceFn.apply(c, self.tree.prototype_layer.prototype_vectors, True)
         return self.tree.route(mind)

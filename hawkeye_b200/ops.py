@@ -44,7 +44,7 @@ def wants_grad(x, params):
 
 
 # ----------------------------------------------------------------------------------------------------------
-# shared host bindings: GEMM, linear forward, NCHW <-> NHWC, 3x3 convolution on NHWC maps
+# shared host bindings: GEMM, linear forward, NCHW <-> NHWC, 1x1 and 3x3 convolutions on NHWC maps
 # ----------------------------------------------------------------------------------------------------------
 def gemm(A, a_mn, lda, sA, B, b_mn, ldb, sB, C, ldc, sC, M, N, K, batch=1, alpha=1.0, alpha_vec=None, diag=0.0, D=None,
          ldd=0, sD=0, beta=0.0, beta_vec=None, relu=False, trans_c=False, exact=False):
@@ -78,6 +78,41 @@ def nhwc_to_nchw(x):
     y = torch.empty(N, C, H, W, device=x.device, dtype=torch.float32)
     _lib.call('hk_nhwc_to_nchw', x, y, N, H * W, C, _lib.stream_ptr())
     return y
+
+
+def nhwc_channel_sum(x, N, HW, C, scale):
+    """scale * the sum over the HW positions of x [N, HW, C] (any shape of that size) -> [N, C]"""
+    y = torch.empty(N, C, device=x.device, dtype=torch.float32)
+    ws = _ws(_lib.query('hk_apcnn_pool_workspace_bytes', N, HW, C), x.device)
+    _lib.call('hk_apcnn_pool', x, y, N, HW, C, scale, ws, ws.numel(), _lib.stream_ptr())
+    return y
+
+
+# A matrix-form convolution (1x1, or the im2col'd stem) is a GEMM over the rows of its input: x [..., K] as [P, K] rows,
+# w [Cout, K] (or [Cout, K, 1, 1]), y [..., Cout] as [P, Cout] rows.
+def conv1x1_fwd(x, w, b=None):
+    """y = x w^T (+ b [Cout], the epilogue's row addend) -> [..., Cout]"""
+    K, cout = x.shape[-1], w.shape[0]
+    y = torch.empty(*x.shape[:-1], cout, device=x.device, dtype=torch.float32)
+    gemm(x, 0, K, 0, w, 0, K, 0, y, cout, 0, x.numel() // K, cout, K, D=b, ldd=0, beta=0.0 if b is None else 1.0)
+    return y
+
+
+def conv1x1_dgrad(dy, w, addend=None):
+    """dx = dy w (+ addend, same shape as dx, in the epilogue) -> [..., K]  (w as the MN-major B)"""
+    cout, K = w.shape[:2]
+    dx = torch.empty(*dy.shape[:-1], K, device=dy.device, dtype=torch.float32)
+    gemm(dy, 0, cout, 0, w, 1, K, 0, dx, K, 0, dy.numel() // cout, K, cout, D=addend, ldd=0 if addend is None else K,
+         beta=0.0 if addend is None else 1.0)
+    return dx
+
+
+def conv1x1_wgrad(x, dy, dw):
+    """dw [Cout, K] (any shape of that size) = dy^T x, written"""
+    K, cout = x.shape[-1], dy.shape[-1]
+    P = x.numel() // K
+    ws = _ws(_lib.query('hk_matconv_wgrad_workspace_bytes', P, K, cout), x.device)
+    _lib.call('hk_matconv_wgrad', x, dy, dw, P, K, cout, ws, ws.numel(), _lib.stream_ptr())
 
 
 def conv3x3_pack(w, dgrad):
@@ -118,7 +153,7 @@ def conv3x3_dgrad(g, wd, mask=None):
 
 
 # ----------------------------------------------------------------------------------------------------------
-# layers the methods share: in-place add, image crops, means, ReLU
+# layers the methods share: in-place add, image crops, means, activations, layout changes, 1x1 and 3x3 convolutions
 # ----------------------------------------------------------------------------------------------------------
 def add_(a, b):
     """a += b (contiguous fp32 tensors of one size) -> a"""
@@ -167,11 +202,8 @@ class NHWCMeanFn(Function):
         _check_cuda(x)
         x = _f32c(x)
         N, H, W, C = x.shape
-        y = torch.empty(N, C, device=x.device, dtype=torch.float32)
-        ws = _ws(_lib.query('hk_apcnn_pool_workspace_bytes', N, H * W, C), x.device)
-        _lib.call('hk_apcnn_pool', x, y, N, H * W, C, 1.0 / (H * W), ws, ws.numel(), _lib.stream_ptr())
         ctx.shape = x.shape
-        return y
+        return nhwc_channel_sum(x, N, H * W, C, 1.0 / (H * W))
 
     @staticmethod
     def backward(ctx, dy):
@@ -181,21 +213,104 @@ class NHWCMeanFn(Function):
         return dx
 
 
-class ReluFn(Function):
+class ActFn(Function):
+    """ReLU (elu False) or nn.ELU with alpha 1 (elu True), elementwise on any shape (OSME's bottleneck, AP-CNN's channel
+    gates and heads); the backward reads the output."""
+
     @staticmethod
-    def forward(ctx, x):
+    def forward(ctx, x, elu):
+        _check_cuda(x)
         x = _f32c(x)
         y = torch.empty_like(x)
-        _lib.call('hk_relu_fwd', x, y, x.numel(), _lib.stream_ptr())
+        _lib.call('hk_act_fwd', x, y, x.numel(), int(elu), _lib.stream_ptr())
         ctx.save_for_backward(y)
+        ctx.elu = int(elu)
         return y
 
     @staticmethod
     def backward(ctx, dy):
         (y,) = ctx.saved_tensors
         dx = torch.empty_like(y)
-        _lib.call('hk_relu_bwd', y, _f32c(dy), dx, y.numel(), _lib.stream_ptr())
-        return dx
+        _lib.call('hk_act_bwd', y, _f32c(dy), dx, y.numel(), ctx.elu, _lib.stream_ptr())
+        return dx, None
+
+
+class ToNHWCFn(Function):
+    """NCHW [N, C, H, W] -> NHWC [N, H, W, C]; the backward is the opposite transpose."""
+
+    @staticmethod
+    def forward(ctx, x):
+        _check_cuda(x)
+        return nchw_to_nhwc(_f32c(x))
+
+    @staticmethod
+    def backward(ctx, dy):
+        return nhwc_to_nchw(_f32c(dy))
+
+
+class ToNCHWFn(Function):
+    """NHWC [N, H, W, C] -> NCHW [N, C, H, W]; the backward is the opposite transpose."""
+
+    @staticmethod
+    def forward(ctx, x):
+        _check_cuda(x)
+        return nhwc_to_nchw(_f32c(x))
+
+    @staticmethod
+    def backward(ctx, dy):
+        return nchw_to_nhwc(_f32c(dy))
+
+
+class Conv1x1Fn(Function):
+    """nn.Conv2d(Cin, Cout, 1) (+ bias) on an NHWC map [N, H, W, Cin] -> [N, H, W, Cout]: one GEMM over the N H W rows with
+    the bias as the epilogue's row addend.  The backward computes dX, dW and db each only when it is needed."""
+
+    @staticmethod
+    def forward(ctx, x, w, b):
+        _check_cuda(x, w, b)
+        x, w = _f32c(x), _f32c(w)
+        ctx.save_for_backward(x, w)
+        ctx.has_bias = b is not None
+        return conv1x1_fwd(x, w, None if b is None else _f32c(b))
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, w = ctx.saved_tensors
+        dy = _f32c(dy)
+        cout = w.shape[0]
+        dx = dw = db = None
+        if ctx.needs_input_grad[0]:
+            dx = conv1x1_dgrad(dy, w)
+        if ctx.needs_input_grad[1]:
+            dw = torch.empty_like(w)
+            conv1x1_wgrad(x, dy, dw)
+        if ctx.has_bias and ctx.needs_input_grad[2]:
+            db = nhwc_channel_sum(dy, 1, dy.numel() // cout, cout, 1.0).view(cout)
+        return dx, dw, db
+
+
+class Conv3x3Fn(Function):
+    """nn.Conv2d(Cin, Cout, 3, 1, 1) (+ bias) on an NHWC map [N, H, W, Cin] -> [N, H, W, Cout] on the implicit-GEMM
+    hk_conv3x3_* kernels."""
+
+    @staticmethod
+    def forward(ctx, x, w, b):
+        _check_cuda(x, w, b)
+        x = _f32c(x)
+        wf, wd = conv3x3_pack(_f32c(w), True)
+        ctx.save_for_backward(x, wd)
+        ctx.has_bias = b is not None
+        return conv3x3_fwd(x, wf, b, relu=False)
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, wd = ctx.saved_tensors
+        dy = _f32c(dy)
+        cin, cout = x.shape[-1], dy.shape[-1]
+        dw = torch.empty(cout, cin, 3, 3, device=dy.device, dtype=torch.float32)
+        db = torch.empty(cout, device=dy.device, dtype=torch.float32) if ctx.has_bias else None
+        conv3x3_wgrad(x, dy, dw, db)
+        return (conv3x3_dgrad(dy, wd) if ctx.needs_input_grad[0] else None), dw, db
 
 
 # ----------------------------------------------------------------------------------------------------------

@@ -10,8 +10,7 @@ import torch
 from torch.autograd import Function
 
 from . import _lib
-from .ops import (NHWCMeanFn, _check_cuda, _f32c, _ws, conv3x3_dgrad, conv3x3_fwd, conv3x3_pack, conv3x3_wgrad, gemm,
-                  wants_grad)
+from .ops import _check_cuda, _f32c, _ws, nhwc_channel_sum
 
 STRIDES = (8, 16, 32)            # get_att_roi calls, :567-569
 ANCHOR_SIZES = (64, 128, 256)
@@ -60,33 +59,6 @@ def roi_to_reference(boxes, counts):
     return out
 
 
-class UnitFn(Function):
-    """One ops_resnet.Unit (conv + BatchNorm + ReLU) on an NHWC map as an autograd node (SimpleFPA's BasicConvs, :180-183)."""
-
-    @staticmethod
-    def forward(ctx, x, unit, save, training, w, gamma, beta):
-        _check_cuda(x)
-        y, rec = unit.forward(_f32c(x), _f32c(w), gamma, beta, None, save, training)
-        ctx.unit, ctx.rec = unit, rec
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        if ctx.rec is None:
-            return (None,) * 7
-        dx, _, dw, dg, db = ctx.unit.backward(ctx.rec, _f32c(dy), need_dx=ctx.needs_input_grad[0])
-        ctx.rec = None
-        return dx, None, None, None, dw, dg, db
-
-
-def unit(x, u, training):
-    params = u.params()
-    return UnitFn.apply(x, u, wants_grad(x, params), training, *params)
-
-
-PoolFn = NHWCMeanFn          # the AvgPool2d of SimpleFPA's global branch (:194): NHWC [N, H, W, C] -> [N, C]
-
-
 class BcastAddFn(Function):
     """a [N, H, W, C] + b [N, C] on every pixel (x_master + x_gpb, :197)."""
 
@@ -103,66 +75,7 @@ class BcastAddFn(Function):
     def backward(ctx, dy):
         dy = _f32c(dy)
         N, H, W, C = dy.shape
-        db = torch.empty(N, C, device=dy.device, dtype=torch.float32)
-        ws = _ws(_lib.query('hk_apcnn_pool_workspace_bytes', N, H * W, C), dy.device)
-        _lib.call('hk_apcnn_pool', dy, db, N, H * W, C, 1.0, ws, ws.numel(), _lib.stream_ptr())
-        return dy, db
-
-
-class Conv1x1BiasFn(Function):
-    """nn.Conv2d(Cin, Cout, 1) with bias and no BatchNorm on an NHWC map (P4_1 / P3_1, :211-214): one GEMM over the N H W
-    rows with the bias as the epilogue's row addend."""
-
-    @staticmethod
-    def forward(ctx, x, w, b):
-        _check_cuda(x, w, b)
-        x, w = _f32c(x), _f32c(w)
-        N, H, W, cin = x.shape
-        cout = w.shape[0]
-        y = torch.empty(N, H, W, cout, device=x.device, dtype=torch.float32)
-        gemm(x, 0, cin, 0, w, 0, cin, 0, y, cout, 0, N * H * W, cout, cin, D=_f32c(b), ldd=0, beta=1.0)
-        ctx.save_for_backward(x, w)
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        x, w = ctx.saved_tensors
-        dy = _f32c(dy)
-        N, H, W, cin = x.shape
-        cout, P, dev = w.shape[0], N * H * W, x.device
-        dx = None
-        if ctx.needs_input_grad[0]:
-            dx = torch.empty_like(x)
-            gemm(dy, 0, cout, 0, w, 1, cin, 0, dx, cin, 0, P, cin, cout)
-        dw = torch.empty(cout, cin, 1, 1, device=dev, dtype=torch.float32)
-        ws = _ws(_lib.query('hk_matconv_wgrad_workspace_bytes', P, cin, cout), dev)
-        _lib.call('hk_matconv_wgrad', x, dy, dw, P, cin, cout, ws, ws.numel(), _lib.stream_ptr())
-        db = torch.empty(1, cout, device=dev, dtype=torch.float32)
-        ws = _ws(_lib.query('hk_apcnn_pool_workspace_bytes', 1, P, cout), dev)
-        _lib.call('hk_apcnn_pool', dy, db, 1, P, cout, 1.0, ws, ws.numel(), _lib.stream_ptr())
-        return dx, dw, db.view(cout)
-
-
-class Conv3x3BiasFn(Function):
-    """nn.Conv2d(C, C, 3, 1, 1) with bias on an NHWC map (P5_2 / P4_2 / P3_2, :209-215) on hk_conv3x3_*."""
-
-    @staticmethod
-    def forward(ctx, x, w, b):
-        _check_cuda(x, w, b)
-        x = _f32c(x)
-        wf, wd = conv3x3_pack(_f32c(w), True)
-        ctx.save_for_backward(x, wd)
-        ctx.wshape = w.shape
-        return conv3x3_fwd(x, wf, b, relu=False)
-
-    @staticmethod
-    def backward(ctx, dy):
-        x, wd = ctx.saved_tensors
-        dy = _f32c(dy)
-        dw = torch.empty(ctx.wshape, device=dy.device, dtype=torch.float32)
-        db = torch.empty(ctx.wshape[0], device=dy.device, dtype=torch.float32)
-        conv3x3_wgrad(x, dy, dw, db)
-        return (conv3x3_dgrad(dy, wd) if ctx.needs_input_grad[0] else None), dw, db
+        return dy, nhwc_channel_sum(dy, N, H * W, C, 1.0)
 
 
 class LateralFn(Function):
@@ -223,27 +136,6 @@ class AttentionFn(Function):
         _lib.call('hk_apcnn_att_bwd', F, w, gate, None if dpf is None else _f32c(dpf), _f32c(dpsf), dF, dw, db, N, H, W, C, ws,
                   ws.numel(), _lib.stream_ptr())
         return dF, dw, db
-
-
-class ActFn(Function):
-    """ReLU (elu False) or nn.ELU (elu True) on a vector."""
-
-    @staticmethod
-    def forward(ctx, x, elu):
-        _check_cuda(x)
-        x = _f32c(x)
-        y = torch.empty_like(x)
-        _lib.call('hk_apcnn_act_fwd', x, y, x.numel(), int(elu), _lib.stream_ptr())
-        ctx.save_for_backward(y)
-        ctx.elu = int(elu)
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        (y,) = ctx.saved_tensors
-        dx = torch.empty_like(y)
-        _lib.call('hk_apcnn_act_bwd', y, _f32c(dy), dx, y.numel(), ctx.elu, _lib.stream_ptr())
-        return dx, None
 
 
 class MixFn(Function):

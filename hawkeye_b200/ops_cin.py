@@ -1,13 +1,11 @@
 """Autograd bindings for the channel-interaction module (reference model/methods/CIN.py:24-60): batched Gram and W.X
-products on the wgmma GEMM, softmax(-G), the contrastive weight |W_SCI - w W_SCI_BA|, the 3x3 convolution on the
-implicit-GEMM kernels (NCHW in / out), the residual add and OSME's excitation gate.  Host plumbing only; all arithmetic is in
-libhawkeye_b200.so."""
+products on the wgmma GEMM, softmax(-G), the contrastive weight |W_SCI - w W_SCI_BA|, the residual add and OSME's
+excitation gate (the 3x3 convolution is ops.Conv3x3Fn).  Host plumbing only; all arithmetic is in libhawkeye_b200.so."""
 import torch
 from torch.autograd import Function
 
 from . import _lib
-from .ops import (_check_cuda, _f32c, add_, conv3x3_dgrad, conv3x3_fwd, conv3x3_pack, conv3x3_wgrad, gemm, nchw_to_nhwc,
-                  nhwc_to_nchw)
+from .ops import _check_cuda, _f32c, add_, gemm
 
 
 class GramFn(Function):
@@ -106,31 +104,6 @@ class CCIWeightFn(Function):
         d_w = torch.empty_like(weight)
         _lib.call('hk_cci_weight_bwd', w_sci, weight, _f32c(d), d_sci, d_w, B, w_sci.numel() // B, _lib.stream_ptr())
         return d_sci, d_w
-
-
-class Conv3x3NCHWFn(Function):
-    """nn.Conv2d(C, C, 3, 1, 1) on an NCHW map (CIN.py:22,36,57): NHWC inside, wgmma implicit GEMM."""
-
-    @staticmethod
-    def forward(ctx, x, w, b):
-        _check_cuda(x, w, b)
-        xn = nchw_to_nhwc(_f32c(x))
-        wf, wd = conv3x3_pack(_f32c(w), True)
-        y = nhwc_to_nchw(conv3x3_fwd(xn, wf, b, relu=False))
-        ctx.save_for_backward(xn, wd)
-        ctx.has_bias = b is not None
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        xn, wd = ctx.saved_tensors
-        g = nchw_to_nhwc(_f32c(dy))
-        cin, cout = xn.shape[-1], g.shape[-1]
-        dw = torch.empty(cout, cin, 3, 3, device=g.device, dtype=torch.float32)
-        db = torch.empty(cout, device=g.device, dtype=torch.float32) if ctx.has_bias else None
-        conv3x3_wgrad(xn, g, dw, db)
-        dx = nhwc_to_nchw(conv3x3_dgrad(g, wd)) if ctx.needs_input_grad[0] else None
-        return dx, dw, db
 
 
 class AddFn(Function):

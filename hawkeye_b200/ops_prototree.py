@@ -1,7 +1,6 @@
-"""Autograd bindings for ProtoTree (reference model/methods/ProtoTree/ and Examples/ProtoTreeNet.py): the 1x1 neck as one
-GEMM node, the prototype distance with its global min-pool, the soft decision tree, the NLL of its output and the
-derivative-free leaf update.  Host plumbing only: shapes are checked here before any launch, all arithmetic is in
-libhawkeye_b200.so.
+"""Autograd bindings for ProtoTree (reference model/methods/ProtoTree/ and Examples/ProtoTreeNet.py): the prototype
+distance with its global min-pool, the soft decision tree, the NLL of its output and the derivative-free leaf update.
+Host plumbing only: shapes are checked here before any launch, all arithmetic is in libhawkeye_b200.so.
 
 Tree layout: height H, 2^H - 1 branches, 2^H leaves, nodes numbered in pre-order as the reference numbers them
 (prototree.py:275-287).  Prototype row k belongs to the k-th branch in pre-order and leaf row j to the j-th leaf from the left.
@@ -10,7 +9,7 @@ import torch
 from torch.autograd import Function
 
 from . import _lib
-from .ops import _check_cuda, _f32c, _ws, gemm, nchw_to_nhwc, nhwc_to_nchw
+from .ops import _check_cuda, _f32c
 
 MAX_HEIGHT = 12            # hk_prototree_*: one float per node of the tree in shared memory
 
@@ -18,48 +17,6 @@ MAX_HEIGHT = 12            # hk_prototree_*: one float per node of the tree in s
 def check_height(height):
     if not 1 <= int(height) <= MAX_HEIGHT:
         raise _lib.HawkeyeLibError(f'ProtoTree: height={height} is outside the supported 1..{MAX_HEIGHT}')
-
-
-class NeckFn(Function):
-    """Trunk map [N, C, H, W] (NCHW) and the neck's 1x1 weight [D, C, 1, 1] -> pre-activation [N, H*W, D]
-    (position-major, the layout hk_prototree_dist_fwd reads).  One hk_gemm_tf32; backward one dgrad GEMM and one
-    hk_matconv_wgrad."""
-
-    @staticmethod
-    def forward(ctx, feat, w):
-        _check_cuda(feat, w)
-        feat, w = _f32c(feat), _f32c(w)
-        if feat.dim() != 4 or w.dim() != 4 or w.shape[1] != feat.shape[1] or w.shape[2:] != (1, 1):
-            raise _lib.HawkeyeLibError(f'ProtoTree neck: map {tuple(feat.shape)} and weight {tuple(w.shape)} are not a '
-                                       '[N, C, H, W] map and a [D, C, 1, 1] convolution')
-        N, C, H, W = feat.shape
-        D = w.shape[0]
-        x = nchw_to_nhwc(feat)
-        w2 = w.view(D, C)
-        c = torch.empty(N, H * W, D, device=feat.device, dtype=torch.float32)
-        gemm(x, 0, C, 0, w2, 0, C, 0, c, D, 0, N * H * W, D, C)
-        ctx.save_for_backward(x, w2)
-        ctx.w_shape = w.shape
-        return c
-
-    @staticmethod
-    def backward(ctx, dc):
-        x, w2 = ctx.saved_tensors
-        N, H, W, C = x.shape
-        D = w2.shape[0]
-        M = N * H * W
-        dc = _f32c(dc)
-        s = _lib.stream_ptr()
-        dfeat = dw = None
-        if ctx.needs_input_grad[0]:
-            dx = torch.empty_like(x)
-            gemm(dc, 0, D, 0, w2, 1, C, 0, dx, C, 0, M, C, D)
-            dfeat = nhwc_to_nchw(dx)
-        if ctx.needs_input_grad[1]:
-            dw = torch.empty(ctx.w_shape, device=x.device, dtype=torch.float32)
-            ws = _ws(_lib.query('hk_matconv_wgrad_workspace_bytes', M, C, D), x.device)
-            _lib.call('hk_matconv_wgrad', x, dc, dw, M, C, D, ws, ws.numel(), s)
-        return dfeat, dw
 
 
 class PrototypeDistanceFn(Function):

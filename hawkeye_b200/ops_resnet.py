@@ -1,6 +1,6 @@
-"""ResNet-50 v1.5 trunk (reference model/backbone/resnet.py:89-252) and the MPN-COV dimension-reduction block
-(MPNCOV.py:64-69) as explicit forward/backward pipelines over the C-ABI kernels, NHWC fp32 inside, and the same BatchNorm
-over [P, C] rows for the methods' heads (RowBatchNormFn).
+"""ResNet-50 v1.5 trunk (reference model/backbone/resnet.py:89-252), stacks of its bottleneck blocks and single conv units
+(UnitFn) as explicit forward/backward pipelines over the C-ABI kernels, NHWC fp32 inside, and the same BatchNorm over
+[P, C] rows for the methods' heads (RowBatchNormFn).
 
 conv unit = convolution (wgmma GEMM / implicit GEMM) -> BatchNorm (+ residual) (+ ReLU).  BatchNorm runs on the batch
 statistics in train mode and on the running statistics in eval mode; both have a backward (eval mode: the statistics are
@@ -10,8 +10,8 @@ import torch
 from torch.autograd import Function
 
 from . import _lib, ops as _ops
-from .ops import (_check_cuda, _f32c, _ws, add_, conv3x3_dgrad, conv3x3_fwd, conv3x3_pack, conv3x3_wgrad, gemm,
-                  nchw_to_nhwc, nhwc_to_nchw)
+from .ops import (_check_cuda, _f32c, _ws, add_, conv1x1_dgrad, conv1x1_fwd, conv1x1_wgrad, conv3x3_dgrad, conv3x3_fwd,
+                  conv3x3_pack, conv3x3_wgrad)
 
 BN_EPS = 1e-5
 
@@ -39,8 +39,7 @@ class Unit:
             w147 = torch.empty(cout, 160, device=dev, dtype=torch.float32)
             _lib.call('hk_stem_im2col', x, x147, N, H, W, s)
             _lib.call('hk_pack_stem_weights', w, w147, cout, s)
-            c = torch.empty(N, Ho, Wo, cout, device=dev, dtype=torch.float32)
-            gemm(x147, 0, 160, 0, w147, 0, 160, 0, c, cout, 0, P, cout, 160)
+            c = conv1x1_fwd(x147, w147).view(N, Ho, Wo, cout)
             rec['xin'] = x147
         else:
             N, H, W, cin = x.shape
@@ -51,9 +50,7 @@ class Unit:
                     _lib.call('hk_subsample2', x, xin, N, H, W, cin, s)
                     rec['full_hw'] = (H, W)
                 Ho, Wo = xin.shape[1], xin.shape[2]
-                P = N * Ho * Wo
-                c = torch.empty(N, Ho, Wo, cout, device=dev, dtype=torch.float32)
-                gemm(xin, 0, cin, 0, w, 0, cin, 0, c, cout, 0, P, cout, cin)
+                c = conv1x1_fwd(xin, w)
                 rec['xin'] = xin
             else:
                 wf, rec['wd'] = conv3x3_pack(w, save)
@@ -85,20 +82,16 @@ class Unit:
         dx = None
         if self.kind == 'stem':
             dwm = torch.empty(cout, 160, device=dev, dtype=torch.float32)
-            wsb = _ws(_lib.query('hk_matconv_wgrad_workspace_bytes', P, 160, cout), dev)
-            _lib.call('hk_matconv_wgrad', xin, dc, dwm, P, 160, cout, wsb, wsb.numel(), s)
+            conv1x1_wgrad(xin, dc, dwm)
             dw = dwm[:, :147].reshape(w.shape).contiguous()
         elif self.kind in ('1x1', '1x1s2'):
             cin = xin.shape[-1]
             dw = torch.empty(cout, cin, 1, 1, device=dev, dtype=torch.float32)
-            wsb = _ws(_lib.query('hk_matconv_wgrad_workspace_bytes', P, cin, cout), dev)
-            _lib.call('hk_matconv_wgrad', xin, dc, dw, P, cin, cout, wsb, wsb.numel(), s)
+            conv1x1_wgrad(xin, dc, dw)
             if need_dx:
-                dxs = torch.empty_like(xin)
-                # dX = dC . W (+ addend, in the epilogue)  (W [Cout,Cin] as the MN-major B)
+                # the addend goes into the dgrad GEMM's epilogue unless the stride's zero insertion comes after it
                 fuse = addend is not None and self.kind == '1x1'
-                gemm(dc, 0, cout, 0, w, 1, cin, 0, dxs, cin, 0, P, cin, cout, D=addend if fuse else None,
-                     ldd=cin if fuse else 0, beta=1.0 if fuse else 0.0)
+                dxs = conv1x1_dgrad(dc, w, addend if fuse else None)
                 if fuse:
                     addend = None
                 if self.kind == '1x1s2':
@@ -236,11 +229,10 @@ def _param_iter(params):
 
 
 class ResNetTrunkFn(Function):
-    """NCHW image -> NCHW feature map [N, 2048, H/32, W/32]; with ``nhwc`` the NHWC map [N, H/32, W/32, 2048] as the last
-    block writes it (and its gradient arrives in NHWC)."""
+    """NCHW image -> NHWC feature map [N, H/32, W/32, 2048] as the last block writes it."""
 
     @staticmethod
-    def forward(ctx, x, plan, save, training, nhwc, *params):
+    def forward(ctx, x, plan, save, training, *params):
         _check_cuda(x)
         x = _f32c(x)
         s = _lib.stream_ptr()
@@ -255,18 +247,17 @@ class ResNetTrunkFn(Function):
         if _ops.CAPTURE is not None:
             _ops.CAPTURE.append(('pool3', am, (N, H, W, C)))
         cur, brecs = blocks_forward(p, plan.blocks, pget, save, training)
-        ctx.plan, ctx.nparams, ctx.nhwc = plan, len(params), nhwc
+        ctx.plan, ctx.nparams = plan, len(params)
         ctx.recs = ((r, tuple(y.shape), am), brecs) if save else None
-        return cur if nhwc else nhwc_to_nchw(cur)
+        return cur
 
     @staticmethod
     def backward(ctx, dfeat):
         if ctx.recs is None:
-            return (None,) * (5 + ctx.nparams)
+            return (None,) * (4 + ctx.nparams)
         plan, ((r0, yshape, am), brecs) = ctx.plan, ctx.recs
         s = _lib.stream_ptr()
-        g = _f32c(dfeat) if ctx.nhwc else nchw_to_nhwc(_f32c(dfeat))
-        g, grads = blocks_backward(g, plan.blocks, brecs)
+        g, grads = blocks_backward(_f32c(dfeat), plan.blocks, brecs)
         N, H, W, C = yshape
         dy0 = torch.empty(N, H, W, C, device=dfeat.device, dtype=torch.float32)
         _lib.call('hk_maxpool3x3s2_bwd', am, g, dy0, N, H, W, C, s)
@@ -274,7 +265,7 @@ class ResNetTrunkFn(Function):
         grads = [(dw0, dg0, db0)] + grads
         ctx.recs = None
         flat = [t for trip in grads for t in trip]
-        return (None, None, None, None, None) + tuple(flat)
+        return (None, None, None, None) + tuple(flat)
 
 
 class BlockStackFn(Function):
@@ -303,37 +294,36 @@ def block_stack(x, blocks, training):
     return BlockStackFn.apply(x, blocks, _ops.wants_grad(x, params), training, *params)
 
 
-def resnet_trunk(x, trunk_module):
-    plan = trunk_module._plan
+def resnet_trunk(x, plan, training):
+    """The trunk of ``plan`` on an NCHW image -> its NHWC output map."""
     params = plan.params()
-    training = trunk_module.training
-    save = _ops.wants_grad(x, params)
-    return ResNetTrunkFn.apply(x, plan, save, training, False, *params)
+    return ResNetTrunkFn.apply(x, plan, _ops.wants_grad(x, params), training, *params)
 
 
-def resnet_trunk_nhwc(x, plan, training):
-    """The trunk of ``plan`` on an NCHW image -> its NHWC output map, without the NCHW transpose."""
-    params = plan.params()
-    return ResNetTrunkFn.apply(x, plan, _ops.wants_grad(x, params), training, True, *params)
-
-
-class DRBlockFn(Function):
-    """MPNCOV.conv_dr_block (MPNCOV.py:64-69): 1x1 conv (no bias) + BN + ReLU, NCHW in / NCHW out."""
+class UnitFn(Function):
+    """One Unit (conv + BatchNorm (+ ReLU)) on an NHWC map as an autograd node: SimpleFPA's BasicConvs (APCNN.py:180-183),
+    MPN-COV's conv_dr_block (MPNCOV.py:64-69)."""
 
     @staticmethod
     def forward(ctx, x, unit, save, training, w, gamma, beta):
         _check_cuda(x)
-        y, rec = unit.forward(nchw_to_nhwc(_f32c(x)), _f32c(w), gamma, beta, None, save, training)
+        y, rec = unit.forward(_f32c(x), _f32c(w), gamma, beta, None, save, training)
         ctx.unit, ctx.rec = unit, rec
-        return nhwc_to_nchw(y)
+        return y
 
     @staticmethod
-    def backward(ctx, dout):
+    def backward(ctx, dy):
         if ctx.rec is None:
             return (None,) * 7
-        dx, _, dw, dg, db = ctx.unit.backward(ctx.rec, nchw_to_nhwc(_f32c(dout)))
+        dx, _, dw, dg, db = ctx.unit.backward(ctx.rec, _f32c(dy), need_dx=ctx.needs_input_grad[0])
         ctx.rec = None
-        return nhwc_to_nchw(dx), None, None, None, dw, dg, db
+        return dx, None, None, None, dw, dg, db
+
+
+def unit(x, u, training):
+    """x NHWC through the Unit ``u`` with its own parameters."""
+    params = u.params()
+    return UnitFn.apply(x, u, _ops.wants_grad(x, params), training, *params)
 
 
 class RowBatchNormFn(Function):

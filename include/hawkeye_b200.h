@@ -146,7 +146,6 @@ int hk_maxpool2x2_fwd_idx(const float* x_nhwc, float* y, unsigned char* code, in
                           void* stream);
 int hk_maxpool2x2_bwd_idx(const unsigned char* code, const float* dy, float* dx_nhwc, int N, int H, int W, int C,
                           int dy_nchw, void* stream);
-int hk_relu_mask_inplace(float* dy, const float* act, size_t n, void* stream);
 
 /* ---- ResNet-50 v1.5 trunk support (model/backbone/resnet.py:89-252); activations NHWC [P = N*H*W, C] -----------------
  * stem 7x7/s2/p3 (resnet.py:176): patches X147 [P][160] (+ packed weights [64][160]) feed one wgmma GEMM. */
@@ -186,9 +185,13 @@ int hk_maxpool3x3s2_bwd(const unsigned char* argmax, const float* dy, float* dx,
 /* stride-2 sampling of an NHWC map (1x1/s2 down-sample convs) and its adjoint (zero insertion); H, W = full-res dims */
 int hk_subsample2(const float* x, float* y, int N, int H, int W, int C, void* stream);
 int hk_upsample2_zero(const float* y, float* x, int N, int H, int W, int C, void* stream);
+/* layers the methods share: a += b; NCHW <-> NHWC; ReLU (elu = 0) or ELU with alpha 1 (elu = 1) of n > 0 elements, whose
+ * backward reads the output y */
 int hk_add_inplace(float* a, const float* b, size_t n, void* stream);
 int hk_nhwc_to_nchw(const float* x, float* y, int N, int HW, int C, void* stream);
 int hk_nchw_to_nhwc(const float* x, float* y, int N, int HW, int C, void* stream);
+int hk_act_fwd(const float* x, float* y, size_t n, int elu, void* stream);
+int hk_act_bwd(const float* y, const float* dy, float* dx, size_t n, int elu, void* stream);
 /* weight gradient of a matrix-form conv (1x1, or im2col'd stem): dw [Cout][K] = dY[P][Cout]^T . X[P][K] */
 size_t hk_matconv_wgrad_workspace_bytes(long long P, int K, int Cout);
 int hk_matconv_wgrad(const float* x, const float* dy, float* dw, long long P, int K, int Cout, void* workspace,
@@ -208,7 +211,7 @@ int hk_row_mean_fwd(const float* x, float* y, long long rows, int cols, int ld, 
 int hk_row_mean_bwd(const float* dy, float* dx, long long rows, int cols, int ld, void* stream);
 
 /* ---- OSME excitation: s = sigmoid(m)[n,c] * x[n,c,:] and its backward; the
- * squeeze (AdaptiveAvgPool2d) is hk_row_mean_*, the two Linear layers are hk_linear_*, ReLU on the bottleneck hk_relu_* */
+ * squeeze (AdaptiveAvgPool2d) is hk_row_mean_*, the two Linear layers are hk_linear_*, ReLU on the bottleneck hk_act_* */
 int hk_se_gate_fwd(const float* x, const float* m, float* s, long long rows, int hw, void* stream);
 int hk_se_gate_bwd(const float* x, const float* m, const float* ds, float* dx, float* dm, long long rows, int hw,
                    void* stream);
@@ -221,8 +224,6 @@ int hk_se_gate_bwd(const float* x, const float* m, const float* ds, float* dx, f
 int hk_l2norm_rows_fwd(const float* x, float* y, float* inv_norm, int rows, int D, void* stream);
 int hk_l2norm_rows_bwd(const float* y, const float* inv_norm, const float* dy, float* dx, int rows, int D, void* stream);
 int hk_npair_loss(const float* prod, const int* cls, const int* part, double* loss_acc, float* dprod, int n, void* stream);
-int hk_relu_fwd(const float* x, float* y, size_t n, void* stream);
-int hk_relu_bwd(const float* y, const float* dy, float* dx, size_t n, void* stream);
 
 /* ---- APINet: model/methods/APINet.py:28-119, model/loss/APINet_loss.py:33-39 -------------------------------------------
  * hk_apinet_pairs (get_pairs + pdist, :76-119): pool [n,D], labels [n] -> intra[i] = argmin over j != i of the same label,
@@ -439,7 +440,6 @@ int hk_nts_rank_loss(const float* part_logits, const long long* labels, const fl
  *   level-4 ROI; the crop is multiplied by the untruncated window area over its kept cells.  meta int32 [N,12] is written for
  *   the backward.  An image without any ROI keeps its whole map.  _bwd: dy -> dx (zero outside the window and in the dropped
  *   block), gather form.  C % 4 == 0.
- * hk_apcnn_act_fwd / _bwd: ReLU (elu = 0) or ELU with alpha 1 (elu = 1, the heads' nn.ELU, :383); the backward reads y.
  * hk_apcnn_mix_fwd / _bwd (PyramidAttentions.forward, :251-268, on vectors): z, pm, psf, v, ch [3,N,C] (levels 3, 4, 5);
  *   ch_3 = sig(z_3), ch_4 = (sig(z_4) + ch_3) / 2, ch_5 = (sig(z_5) + ch_4) / 2, v_l = psf_l + ch_l pm_l; the backward gives
  *   dz and dpm from dv (dpsf is dv).
@@ -460,8 +460,6 @@ int hk_apcnn_roi(const float* g3, const float* g4, const float* g5, const int* w
 int hk_apcnn_refine_fwd(const float* x, const float* boxes, const int* counts, const float* draws, float* y, int* meta, int N,
                         int H, int W, int C, void* stream);
 int hk_apcnn_refine_bwd(const float* dy, const int* meta, float* dx, int N, int H, int W, int C, void* stream);
-int hk_apcnn_act_fwd(const float* x, float* y, size_t n, int elu, void* stream);
-int hk_apcnn_act_bwd(const float* y, const float* dy, float* dx, size_t n, int elu, void* stream);
 int hk_apcnn_mix_fwd(const float* z, const float* pm, const float* psf, float* v, float* ch, int N, int C, void* stream);
 int hk_apcnn_mix_bwd(const float* z, const float* pm, const float* ch, const float* dv, float* dz, float* dpm, int N, int C,
                      void* stream);

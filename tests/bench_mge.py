@@ -161,7 +161,7 @@ def bench_heads(net, N, image, steps, warmup):
     layer3 / layer4 maps (the trunks are replaced; the eval-mode layer4 recompute is replaced too)"""
     from hawkeye_b200 import ops_resnet
     from hawkeye_b200.losses import MGECNNLoss
-    from hawkeye_b200.ops_apcnn import PoolFn
+    from hawkeye_b200.ops import NHWCMeanFn
     h = image // 32
     c4 = torch.randn(N, 2 * h, 2 * h, 1024, device='cuda').relu()
     c5 = torch.randn(N, h, h, 2048, device='cuda').relu().requires_grad_(True)
@@ -171,7 +171,7 @@ def bench_heads(net, N, image, steps, warmup):
     real_trunk, real_stack = net.trunk, ops_resnet.block_stack
 
     def step():
-        net.trunk = lambda img, b: (c4, c5, PoolFn.apply(c5))
+        net.trunk = lambda img, b: (c4, c5, NHWCMeanFn.apply(c5))
         ops_resnet.block_stack = lambda a, blocks, training: c5.detach()
         try:
             out = net(x)

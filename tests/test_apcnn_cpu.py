@@ -159,7 +159,7 @@ def test_trainer_groups_and_schedule():
         assert math.isclose(Opt.param_groups[0]['lr'], want / 10, rel_tol=1e-12, abs_tol=1e-18)
 
 
-def test_c_entries_reject_bad_arguments():
+def test_apcnn_and_act_entries_reject_bad_arguments():
     from hawkeye_b200 import _lib
     lib = _lib.lib()
     buf = (ctypes.c_float * 64)()
@@ -179,8 +179,8 @@ def test_c_entries_reject_bad_arguments():
     assert b'central window' in lib.hk_last_error()
     assert lib.hk_apcnn_refine_fwd(p, p, p, None, p, None, 1, 2, 2, 4, None) == -1
     assert lib.hk_apcnn_refine_bwd(p, p, p, 1, 2, 2, 6, None) == -1
-    assert lib.hk_apcnn_act_fwd(p, p, 0, 1, None) == -1
-    assert lib.hk_apcnn_act_bwd(p, None, p, 4, 1, None) == -1
+    assert lib.hk_act_fwd(p, p, 0, 1, None) == -1
+    assert lib.hk_act_bwd(p, None, p, 4, 1, None) == -1
     assert lib.hk_apcnn_mix_fwd(p, p, p, p, None, 1, 4, None) == -1
     assert lib.hk_apcnn_mix_bwd(p, p, p, p, p, p, 0, 4, None) == -1
     assert lib.hk_apcnn_mask_cat(p, p, p, p, 1, 6, 8, None) == -1

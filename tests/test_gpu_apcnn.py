@@ -56,8 +56,8 @@ def _select(gates, nc, image):
 
 
 @pytest.mark.parametrize('N,h,w,C', [(1, 1, 1, 4), (2, 3, 5, 256), (16, 7, 7, 256)])
-def test_lateral_pool_bcast(N, h, w, C):
-    from hawkeye_b200 import ops_apcnn
+def test_lateral_mean_bcast(N, h, w, C):
+    from hawkeye_b200 import ops, ops_apcnn
     torch.manual_seed(N + h)
     top = torch.randn(N, h, w, C, device='cuda', requires_grad=True)
     lat = torch.randn(N, 2 * h, 2 * w, C, device='cuda', requires_grad=True)
@@ -72,7 +72,7 @@ def test_lateral_pool_bcast(N, h, w, C):
         x = torch.randn(N, 2 * h, 2 * w, C, device='cuda', requires_grad=True)
         b = torch.randn(N, C, device='cuda', requires_grad=True)
         y = ops_apcnn.BcastAddFn.apply(x, b) * 1.0
-        p = ops_apcnn.PoolFn.apply(y)
+        p = ops.NHWCMeanFn.apply(y)
         assert (p.double() - (x.double() + b.double()[:, None, None]).mean((1, 2))).abs().max() < 1e-5
         p.backward(torch.ones_like(p))
         assert (x.grad - 1.0 / (4 * h * w)).abs().max() < 1e-6 and (b.grad - 1.0).abs().max() < 1e-5
@@ -183,13 +183,13 @@ def test_refine_fwd_bwd_against_interpolate(N, H, C):
     assert torch.equal(dx1, x.grad)
 
 
-def test_vector_ops_against_torch():
-    from hawkeye_b200 import ops_apcnn
+def test_act_and_mix_against_torch():
+    from hawkeye_b200 import ops, ops_apcnn
     torch.manual_seed(3)
     x = torch.randn(16, 512, device='cuda', requires_grad=True)
     for elu in (False, True):
         x.grad = None
-        y = ops_apcnn.ActFn.apply(x, elu)
+        y = ops.ActFn.apply(x, elu)
         g = torch.randn_like(y)
         y.backward(g)
         x64 = x.detach().double().requires_grad_(True)
