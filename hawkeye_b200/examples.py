@@ -9,13 +9,21 @@ which LR schedule — the step itself is ``Trainer.batch_training``.
 import os
 import sys
 
-from .train import PeerLearningTrainer, Trainer, _Cosine, _Plateau, _Step
+from .train import PeerLearningTrainer, Trainer, _Cosine, _Plateau, _Step, warmup_cosine_args
 
 
 def _warmup_cosine(opt, config, total_epoch):
-    return _Cosine(opt, config['T_max'] if 'T_max' in config else total_epoch, 0.0,
-                   config['warmup_epochs'] if 'warmup_epochs' in config else 0,
-                   config['lr_warmup_decay'] if 'lr_warmup_decay' in config else 0.01)
+    T_max, warmup_epochs, warmup_decay = warmup_cosine_args(config, total_epoch)
+    return _Cosine(opt, T_max, 0.0, warmup_epochs, warmup_decay)
+
+
+def _momentum_sgd(trainer, config):
+    """SGD with momentum 0.9 and the yaml's weight_decay over the trained groups (Examples/InterpPartsNet.py,
+    Examples/APCNN.py)."""
+    from . import engine
+    return engine.FusedSGD(trainer.flat, lr=config.lr, momentum=0.9,
+                           weight_decay=config.weight_decay if 'weight_decay' in config else 0.0,
+                           group_lrs=[config.lr * m for _, m in trainer.trained_groups()])
 
 
 def _balanced_loaders(trainer, config):
@@ -97,14 +105,6 @@ class OSMENetTrainer(Trainer):
     # batch_training is the base Trainer's: it hands the model's (pred, x_part) pair to the criterion as is, and MAMCLoss exposes
     # the top-1 count of its cross-entropy kernel (last_correct), so the step has no host synchronisation either.
 
-    def batch_validate(self, data):
-        import torch
-        from .train import accuracy
-        images, labels = self.to_device(data['img']), self.to_device(data['label'])
-        with torch.no_grad():
-            pred, _ = self.model(images)
-        self.average_meters['acc'].update(accuracy(pred, labels, 1), images.size(0))
-
 
 class _FrozenWarmupCosine(_Cosine):
     """_Cosine with the first ``frozen`` parameter groups at lr 0 until the warm-up ends.  That is what the reference's
@@ -142,9 +142,8 @@ class APINetTrainer(Trainer):
         return [(list(m.backbone.parameters()), 1.0), ([p for p in m.parameters() if id(p) not in backbone], 1.0)]
 
     def get_scheduler(self, config):
-        return _FrozenWarmupCosine(self.optimizer, config['T_max'] if 'T_max' in config else self.total_epoch, 0.0,
-                                   config['warmup_epochs'] if 'warmup_epochs' in config else 0,
-                                   config['lr_warmup_decay'] if 'lr_warmup_decay' in config else 0.01)
+        T_max, warmup_epochs, warmup_decay = warmup_cosine_args(config, self.total_epoch)
+        return _FrozenWarmupCosine(self.optimizer, T_max, 0.0, warmup_epochs, warmup_decay)
 
     def forward_model(self, images, labels):
         return self.model(images, labels, flag='train')
@@ -189,28 +188,15 @@ class DCLTrainer(Trainer):
         }
 
     def get_dataloader(self, config):
-        from torch.utils.data import DataLoader
         from .data import DCLDataset, collate_fn4train, collate_fn4val
         t = config.transformer
         tf = self.get_transformers(t)
         swap = t.swap_num if 'swap_num' in t else [7, 7]
         mc = self.config.model
-        self.datasets = {s: DCLDataset(config.root_dir, os.path.join(config.meta_dir, s + '.txt'), transforms=tf,
-                                       swap_size=swap, mode=s, cls_2=mc.cls_2, cls_2xmul=mc.cls_2xmul)
-                         for s in ('train', 'val')}
-        if config.batch_size % self.world != 0:
-            raise ValueError(f'dataset.batch_size={config.batch_size} must be a multiple of the {self.world} ranks')
-        loaders = {}
-        for s, collate in (('train', collate_fn4train), ('val', collate_fn4val)):
-            sampler = None
-            if self.world > 1:
-                from torch.utils.data.distributed import DistributedSampler
-                sampler = DistributedSampler(self.datasets[s], num_replicas=self.world, rank=self.rank, shuffle=s == 'train')
-            self.samplers[s] = sampler
-            loaders[s] = DataLoader(self.datasets[s], config.batch_size // self.world, num_workers=config.num_workers,
-                                    pin_memory=True, sampler=sampler, shuffle=(s == 'train' and sampler is None),
-                                    collate_fn=collate)
-        return loaders
+        return self.rank_loaders(config, {s: DCLDataset(config.root_dir, os.path.join(config.meta_dir, s + '.txt'),
+                                                        transforms=tf, swap_size=swap, mode=s, cls_2=mc.cls_2,
+                                                        cls_2xmul=mc.cls_2xmul) for s in ('train', 'val')},
+                                 {'train': collate_fn4train, 'val': collate_fn4val})
 
     def get_criterion(self, config):
         from .losses import DCLLoss
@@ -224,9 +210,8 @@ class DCLTrainer(Trainer):
 
     def get_optimizer(self, config):
         from . import engine
-        lrs = [config.lr * m for g, m in self.param_groups() if any(p.requires_grad for p in g)]
         return engine.FusedSGD(self.flat, lr=config.lr, momentum=config.momentum if 'momentum' in config else 0.0,
-                               weight_decay=0.0, group_lrs=lrs)
+                               weight_decay=0.0, group_lrs=[config.lr * m for _, m in self.trained_groups()])
 
     def get_scheduler(self, config):
         return _Step(self.optimizer, config.step_size, config.gamma)
@@ -234,18 +219,6 @@ class DCLTrainer(Trainer):
     def batch_tensors(self, data):
         images, labels, labels_swap, swap_law, _ = data
         return images, (labels, labels_swap, swap_law)
-
-    def batch_validate(self, data):
-        import torch
-        from .train import accuracy
-        images, labels = self.to_device(data[0]), self.to_device(data[1].long())
-        with torch.no_grad():
-            out = self.model(images)
-        logit = out[0]
-        if self.config.model.cls_2xmul:
-            K = logit.shape[1]
-            logit = logit + out[1][:, :K] + out[1][:, K:2 * K]
-        self.average_meters['acc'].update(accuracy(logit, labels, 1), labels.size(0))
 
 
 class ProtoTreeTrainer(Trainer):
@@ -299,8 +272,8 @@ class ProtoTreeTrainer(Trainer):
         if name == 'AdamW' and wd != 0:
             raise ValueError(f'ProtoTreeTrainer: AdamW with weight_decay={wd} needs decoupled weight decay, which FusedAdam '
                              'does not have; use weight_decay: 0.0')
-        lrs = [config.lr * m for g, m in self.param_groups() if any(p.requires_grad for p in g)]
-        return engine.FusedAdam(self.flat, lr=config.lr, eps=1e-7, weight_decay=0.0, group_lrs=lrs)
+        return engine.FusedAdam(self.flat, lr=config.lr, eps=1e-7, weight_decay=0.0,
+                                group_lrs=[config.lr * m for _, m in self.trained_groups()])
 
     def get_scheduler(self, config):
         return _warmup_cosine(self.optimizer, config, self.total_epoch)
@@ -310,13 +283,7 @@ class ProtoTreeTrainer(Trainer):
 
     def _graph_step_on_stream(self, images, labels, gs):
         if self.model.training:
-            from .train import _as_tuple
-            outputs = self.forward_model(images, labels)
-            loss = self.criterion(outputs, *_as_tuple(labels))
-            self.optimizer.zero_grad()
-            loss.backward()
-            self.allreduce.finish()
-            return outputs, loss
+            return self.eager_step(images, labels)
         outputs, loss = super()._graph_step_on_stream(images, labels, gs)
         # the step's own outputs (the graph's static tensors after a replay): on the capturing step the criterion last saw
         # the static tensors of a graph that has not run yet
@@ -342,14 +309,6 @@ class ProtoTreeTrainer(Trainer):
             leaf_update(self.get_model_module().tree.leaf_params, self._theta0, pa, pred, labels, self.num_batches, reduce)
         self.model.eval()
 
-    def batch_validate(self, data):
-        import torch
-        from .train import accuracy
-        images, labels = self.to_device(data['img']), self.to_device(data['label'])
-        with torch.no_grad():
-            pred, _ = self.model(images)
-        self.average_meters['acc'].update(accuracy(pred, labels, 1), images.size(0))
-
 
 class InterpPartsNetTrainer(Trainer):
     """Examples/InterpPartsNet.py: the reference's train / validation transforms; criterion = InterpPartsLoss (cross-entropy
@@ -372,30 +331,6 @@ class InterpPartsNetTrainer(Trainer):
                                        transforms.ToTensor(), norm]),
         }
 
-    def get_dataloader(self, config):
-        """The base Trainer's datasets, rank sharding and loaders, with the transforms above."""
-        try:
-            from dataset.dataset import FGDataset
-        except Exception:
-            from .data import FGDataset
-        from torch.utils.data import DataLoader
-        tf = self.get_transformers(config.transformer)
-        self.datasets = {s: FGDataset(config.root_dir, os.path.join(config.meta_dir, s + '.txt'), transform=tf[s])
-                         for s in ('train', 'val')}
-        if config.batch_size % self.world != 0:
-            raise ValueError(f'dataset.batch_size={config.batch_size} must be a multiple of the {self.world} ranks')
-        loaders = {}
-        for s in ('train', 'val'):
-            sampler = None
-            if self.world > 1:
-                from torch.utils.data.distributed import DistributedSampler
-                sampler = DistributedSampler(self.datasets[s], num_replicas=self.world, rank=self.rank, shuffle=s == 'train',
-                                             drop_last=False)
-            self.samplers[s] = sampler
-            loaders[s] = DataLoader(self.datasets[s], config.batch_size // self.world, num_workers=config.num_workers,
-                                    pin_memory=True, sampler=sampler, shuffle=(s == 'train' and sampler is None))
-        return loaders
-
     def get_criterion(self, config):
         from .losses import InterpPartsLoss
         return InterpPartsLoss(config)
@@ -405,11 +340,7 @@ class InterpPartsNetTrainer(Trainer):
         return [([p for n, p in named if n.split('.')[0] in self.FINETUNE], 1.0),
                 ([p for n, p in named if n.split('.')[0] not in self.FINETUNE], 20.0)]
 
-    def get_optimizer(self, config):
-        from . import engine
-        lrs = [config.lr * m for g, m in self.param_groups() if any(p.requires_grad for p in g)]
-        return engine.FusedSGD(self.flat, lr=config.lr, momentum=0.9,
-                               weight_decay=config.weight_decay if 'weight_decay' in config else 0.0, group_lrs=lrs)
+    get_optimizer = _momentum_sgd
 
     def get_scheduler(self, config):
         iters = len(self.dataloaders['train']) if 'train' in self.dataloaders else 1
@@ -420,14 +351,6 @@ class InterpPartsNetTrainer(Trainer):
 
     def do_scheduler_step(self):
         pass
-
-    def batch_validate(self, data):
-        import torch
-        from .train import accuracy
-        images, labels = self.to_device(data['img']), self.to_device(data['label'])
-        with torch.no_grad():
-            pred, _, _ = self.model(images)
-        self.average_meters['acc'].update(accuracy(pred, labels, 1), images.size(0))
 
 
 class NTSNetTrainer(Trainer):
@@ -442,14 +365,6 @@ class NTSNetTrainer(Trainer):
 
     def get_scheduler(self, config):
         return _warmup_cosine(self.optimizer, config, self.total_epoch)
-
-    def batch_validate(self, data):
-        import torch
-        from .train import accuracy
-        images, labels = self.to_device(data['img']), self.to_device(data['label'])
-        with torch.no_grad():
-            concat_logits = self.model(images)[1]
-        self.average_meters['acc'].update(accuracy(concat_logits, labels, 1), images.size(0))
 
 
 class _EpochCosine:
@@ -494,8 +409,6 @@ class APCNNTrainer(Trainer):
                                        transforms.CenterCrop(config.image_size), transforms.ToTensor(), norm]),
         }
 
-    get_dataloader = InterpPartsNetTrainer.get_dataloader        # the base datasets and rank sharding with the transforms above
-
     def get_criterion(self, config):
         from .losses import APCNNLoss
         return APCNNLoss(config)
@@ -505,11 +418,7 @@ class APCNNTrainer(Trainer):
         return [([p for n, p in named if n.split('.')[0] in self.EARLY], 0.1),
                 ([p for n, p in named if n.split('.')[0] not in self.EARLY], 1.0)]
 
-    def get_optimizer(self, config):
-        from . import engine
-        lrs = [config.lr * m for g, m in self.param_groups() if any(p.requires_grad for p in g)]
-        return engine.FusedSGD(self.flat, lr=config.lr, momentum=0.9,
-                               weight_decay=config.weight_decay if 'weight_decay' in config else 0.0, group_lrs=lrs)
+    get_optimizer = _momentum_sgd
 
     def get_scheduler(self, config):
         return _EpochCosine(self.optimizer, self.total_epoch)
@@ -522,14 +431,6 @@ class APCNNTrainer(Trainer):
 
     def forward_model(self, images, labels):
         return self.model(images, labels)
-
-    def batch_validate(self, data):
-        import torch
-        from .train import accuracy
-        images, labels = self.to_device(data['img']), self.to_device(data['label'])
-        with torch.no_grad():
-            out_mean = self.model(images, labels)[0]
-        self.average_meters['acc'].update(accuracy(out_mean, labels, 1), images.size(0))
 
 
 class MGE_CNNTrainer(Trainer):
@@ -555,14 +456,6 @@ class MGE_CNNTrainer(Trainer):
 
     def get_scheduler(self, config):
         return _warmup_cosine(self.optimizer, config, self.total_epoch)
-
-    def batch_validate(self, data):
-        import torch
-        from .train import accuracy
-        images, labels = self.to_device(data['img']), self.to_device(data['label'])
-        with torch.no_grad():
-            logits_gate = self.model(images)['logits'][-1]
-        self.average_meters['acc'].update(accuracy(logits_gate, labels, 1), images.size(0))
 
 
 TRAINERS = {'BCNN': BCNNTrainer, 'CBCNN': CBCNNTrainer, 'MPN': MPNTrainer, 'PeerLearning': PeerLearningTrainer,

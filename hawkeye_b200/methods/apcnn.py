@@ -208,6 +208,9 @@ class ResNet(ResNetBody):
         roi_list = [(boxes[:, o:o + k], counts[:, l]) for l, (o, k) in enumerate(zip(ops_apcnn.ROI_OFFSETS, ops_apcnn.TOPK))]
         return out_mean, out_list, ops_apcnn.mask_cat(gates), roi_list
 
+    def prediction(self, outputs):
+        return outputs[0]
+
 
 def resnet50(num_classes):
     return ResNet(num_classes, (3, 4, 6, 3))

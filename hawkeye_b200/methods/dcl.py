@@ -39,3 +39,11 @@ class DCL(nn.Module):
         logits = ops_dcl.StackedClassifierFn.apply(pooled, self.classifier.weight, self.classifier_swap.weight)
         K, K2 = self.classifier.weight.shape[0], self.classifier_swap.weight.shape[0]
         return [logits[:, :K], logits[:, K:K + K2], mask]
+
+    def prediction(self, outputs):
+        """The logits, plus both halves of the swap logits under cls_2xmul (Examples/DCL.py's validation)."""
+        logits = outputs[0]
+        if self.cls_2xmul:
+            K = logits.shape[1]
+            logits = logits + outputs[1][:, :K] + outputs[1][:, K:2 * K]
+        return logits

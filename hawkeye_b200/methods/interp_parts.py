@@ -115,6 +115,9 @@ class ResNet(ResNetBody):
         logits = ops.linear(out, self.mylinear.weight, self.mylinear.bias)
         return logits, att.view(N, 1, K, 1), assign
 
+    def prediction(self, outputs):
+        return outputs[0]
+
 
 @MODEL.register
 def IP_ResNet50(config):

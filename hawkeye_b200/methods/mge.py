@@ -144,6 +144,9 @@ class LocalCamNet(nn.Module):
                        logits_cat_2, logits_gate]
         return {'logits': logits_list, 'pr_gate': pr_gate, 'boxes': torch.stack([boxes, boxes_2])}
 
+    def prediction(self, outputs):
+        return outputs['logits'][-1]
+
     def get_params(self, prefix='extractor'):
         """MGE.py:225-240: the four trunks (conv5 before conv4 in each pair), or every other parameter."""
         extractor = [p for b in BRANCHES for m in ('conv5', 'conv4') for p in getattr(self, m + b).parameters()]

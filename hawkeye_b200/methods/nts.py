@@ -148,3 +148,6 @@ class NTSNet(nn.Module):
         concat_logits = ops.linear(torch.cat([part_feature, feature], dim=1), self.concat_net.weight, self.concat_net.bias)
         part_logits = ops.linear(part_features, self.partcls_net.weight, self.partcls_net.bias).view(B, T, -1)
         return [raw_logits, concat_logits, part_logits, idx, prob]
+
+    def prediction(self, outputs):
+        return outputs[1]

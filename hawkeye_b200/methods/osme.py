@@ -62,3 +62,6 @@ class OSMENet(nn.Module):
         x = self.backbone(x)
         x1, x_part = self.osme(x)
         return ops.linear(x1, self.classifier.weight, self.classifier.bias), x_part
+
+    def prediction(self, outputs):
+        return outputs[0]

@@ -42,3 +42,6 @@ class PeerLearningNet(nn.Module):
             feat = self.base_model.features(x)
             return self.base_model.head(feat), self.base_model2.head(feat)
         return self.base_model(x), self.base_model2(x)                              # :17-20
+
+    def prediction(self, outputs):
+        return tuple(outputs)

@@ -195,3 +195,6 @@ class ProtoTreeNet(nn.Module):
         c = ops.Conv1x1Fn.apply(ops.ToNHWCFn.apply(feat), w, None).view(N, H * W, w.shape[0])
         mind, _ = ops_prototree.PrototypeDistanceFn.apply(c, self.tree.prototype_layer.prototype_vectors, True)
         return self.tree.route(mind)
+
+    def prediction(self, outputs):
+        return outputs[0]

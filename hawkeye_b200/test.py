@@ -14,16 +14,10 @@ import torch
 from . import _lib
 from .config import setup_config
 from .registry import MODEL
+from .train import AverageMeter, accuracy, prediction
 from .utils import load_state_dict
 
 IMAGENET_MEAN, IMAGENET_STD = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)      # test.py:84, dataset/transforms.py:18-19
-
-
-def accuracy(output, target, topk=1):
-    """utils/utils.py accuracy(): top-k hit rate in percent."""
-    with torch.no_grad():
-        _, pred = output.topk(topk, 1, True, True)
-        return (pred.eq(target.view(-1, 1)).any(dim=1).float().sum() * (100.0 / target.size(0))).item()
 
 
 def normalize_u8(images_u8, mean=IMAGENET_MEAN, std=IMAGENET_STD):
@@ -36,19 +30,6 @@ def normalize_u8(images_u8, mean=IMAGENET_MEAN, std=IMAGENET_STD):
     _lib.call('hk_normalize_u8', x, out, N, H, W, float(mean[0]), float(mean[1]), float(mean[2]), float(std[0]), float(std[1]),
               float(std[2]), _lib.stream_ptr())
     return out
-
-
-class AverageMeter:
-    def __init__(self):
-        self.sum, self.count = 0.0, 0
-
-    def update(self, val, n=1):
-        self.sum += val * n
-        self.count += n
-
-    @property
-    def avg(self):
-        return self.sum / max(self.count, 1)
 
 
 class Tester:
@@ -105,21 +86,9 @@ class Tester:
         images, labels = self.to_device(data['img']), self.to_device(data['label'])
         if images.dtype == torch.uint8:                          # HWC uint8 batches: ToTensor + Normalize on the GPU
             images = normalize_u8(images)
-        logits = self.model(images)
-        if isinstance(logits, tuple) and isinstance(logits[1], dict):   # ProtoTreeNet returns (pred, info)
-            logits = logits[0]
-        if isinstance(logits, dict) and 'pr_gate' in logits:     # MGE_CNN: accuracy on logits_gate, the last of the ten
-            logits = logits['logits'][-1]
-        if isinstance(logits, tuple) and len(logits) == 3 and logits[1].dim() == 4:   # Interp-Parts: (logits, att, assign)
-            logits = logits[0]
-        if isinstance(logits, list) and len(logits) == 5:        # NTSNet's five outputs: accuracy on concat_logits
-            logits = logits[1]
-        if isinstance(logits, tuple) and len(logits) == 4 and isinstance(logits[1], list):   # APCNN: accuracy on out_mean
-            logits = logits[0]
-        if isinstance(logits, tuple):                            # PeerLearningNet returns both heads (PeerLearning.py:94-101)
-            self.average_meters['acc'].update(max(accuracy(l, labels, 1) for l in logits), images.size(0))
-        else:
-            self.average_meters['acc'].update(accuracy(logits, labels, 1), images.size(0))
+        logits = prediction(self.get_model_module(), self.model(images))
+        heads = logits if isinstance(logits, tuple) else (logits,)   # PeerLearningNet: its better head (PeerLearning.py:94-101)
+        self.average_meters['acc'].update(max(accuracy(h, labels, 1) for h in heads), images.size(0))
 
 
 if __name__ == '__main__':

@@ -68,6 +68,19 @@ def _as_tuple(labels):
     return labels if isinstance(labels, tuple) else (labels,)
 
 
+def prediction(model, outputs):
+    """The part of a model's ``outputs`` that validation scores: ``model.prediction(outputs)`` for a model whose forward
+    returns more than its logits, the outputs themselves otherwise (so models of the reference's registry still work)."""
+    return model.prediction(outputs) if hasattr(model, 'prediction') else outputs
+
+
+def warmup_cosine_args(config, total_epoch):
+    """-> (T_max, warmup_epochs, lr_warmup_decay) of a scheduler config, each with its default."""
+    return (config['T_max'] if 'T_max' in config else total_epoch,
+            config['warmup_epochs'] if 'warmup_epochs' in config else 0,
+            config['lr_warmup_decay'] if 'lr_warmup_decay' in config else 0.01)
+
+
 class Trainer:
     def __init__(self, config=None, dataloaders=None):
         self.config = config if config is not None else setup_config()
@@ -111,39 +124,47 @@ class Trainer:
             load_state_dict(model, torch.load(config.load, map_location='cpu'))
         return model
 
-    def get_dataloader(self, config):
+    def get_transformers(self, config):
+        """{'train', 'val'} transforms of the ``dataset.transformer`` config."""
         try:        # inside a Hawkeye checkout: the reference's own classes; otherwise the mirror in hawkeye_b200.data
-            from dataset.dataset import FGDataset
             from dataset.transforms import ClassificationPresetTrain, ClassificationPresetEval
         except Exception:
-            from .data import FGDataset, ClassificationPresetTrain, ClassificationPresetEval
+            from .data import ClassificationPresetTrain, ClassificationPresetEval
+        resize = config['resize_size'] if 'resize_size' in config else int(config['image_size'] / 0.875)
+        return {'train': ClassificationPresetTrain(crop_size=config['image_size'], auto_augment_policy='ta_wide',
+                                                   random_erase_prob=0.1),
+                'val': ClassificationPresetEval(crop_size=config['image_size'], resize_size=resize)}
+
+    def get_dataloader(self, config):
+        try:
+            from dataset.dataset import FGDataset
+        except Exception:
+            from .data import FGDataset
+        tf = self.get_transformers(config.transformer)
+        return self.rank_loaders(config, {s: FGDataset(config.root_dir, os.path.join(config.meta_dir, s + '.txt'),
+                                                       transform=tf[s]) for s in ('train', 'val')})
+
+    def rank_loaders(self, config, datasets, collate_fn=None):
+        """{'train', 'val'} loaders of this rank over ``datasets``; ``collate_fn`` maps a split to its collate function.
+
+        One process per GPU replaces nn.DataParallel (train.py:220-228), which SPLITS config.batch_size across the visible
+        GPUs: batch_size stays the GLOBAL batch, each rank draws batch_size / world images from its own shard of the
+        training set (DistributedSampler, reshuffled per epoch in train()); validation is sharded the same way and the
+        accuracy meters are reduced over ranks in validate()."""
         from torch.utils.data import DataLoader
-        t = config.transformer
-        resize = t['resize_size'] if 'resize_size' in t else int(t['image_size'] / 0.875)
-        tf = {'train': ClassificationPresetTrain(crop_size=t['image_size'], auto_augment_policy='ta_wide',
-                                                 random_erase_prob=0.1),
-              'val': ClassificationPresetEval(crop_size=t['image_size'], resize_size=resize)}
-        ds = {s: FGDataset(config.root_dir, os.path.join(config.meta_dir, s + '.txt'), transform=tf[s])
-              for s in ('train', 'val')}
-        self.datasets = ds
-        # One process per GPU replaces nn.DataParallel (train.py:220-228), which SPLITS config.batch_size across the visible
-        # GPUs: batch_size stays the GLOBAL batch, each rank draws batch_size / world images from its own shard of the
-        # training set (DistributedSampler, reshuffled per epoch in train()); validation is sharded the same way and the
-        # accuracy meters are reduced over ranks in validate().
         if config.batch_size % self.world != 0:
             raise ValueError(f'dataset.batch_size={config.batch_size} must be a multiple of the {self.world} ranks')
-        per_rank = config.batch_size // self.world
-        self.samplers = {}
-        loaders = {}
+        self.datasets, self.samplers, loaders = datasets, {}, {}
         for s in ('train', 'val'):
             sampler = None
             if self.world > 1:
                 from torch.utils.data.distributed import DistributedSampler
-                sampler = DistributedSampler(ds[s], num_replicas=self.world, rank=self.rank, shuffle=s == 'train',
+                sampler = DistributedSampler(datasets[s], num_replicas=self.world, rank=self.rank, shuffle=s == 'train',
                                              drop_last=False)
             self.samplers[s] = sampler
-            loaders[s] = DataLoader(ds[s], per_rank, num_workers=config.num_workers, pin_memory=True, sampler=sampler,
-                                    shuffle=(s == 'train' and sampler is None))
+            loaders[s] = DataLoader(datasets[s], config.batch_size // self.world, num_workers=config.num_workers,
+                                    pin_memory=True, sampler=sampler, shuffle=(s == 'train' and sampler is None),
+                                    collate_fn=(collate_fn or {}).get(s))
         return loaders
 
     def get_criterion(self, config):
@@ -158,18 +179,20 @@ class Trainer:
         rest = [p for p in m.parameters() if id(p) not in ids]
         return [(rest, 1.0), (head, 1.0)]
 
+    def trained_groups(self):
+        """The (params, lr_multiplier) pairs of ``param_groups`` that have a trainable parameter: the flat buffer's groups."""
+        return [(g, m) for g, m in self.param_groups() if any(p.requires_grad for p in g)]
+
     def early_group(self):
-        gs = [g for g, _ in self.param_groups() if any(p.requires_grad for p in g)]
-        return len(gs) - 1 if len(gs) > 1 else None
+        n = len(self.trained_groups())
+        return n - 1 if n > 1 else None
 
     def flatten_parameters(self):
-        groups = [g for g, _ in self.param_groups() if any(p.requires_grad for p in g)]
-        return engine.FlatParams(None, groups=groups)
+        return engine.FlatParams(None, groups=[g for g, _ in self.trained_groups()])
 
     def get_optimizer(self, config):
         name = config.name if 'name' in config else 'Adam'
-        mult = [m for g, m in self.param_groups() if any(p.requires_grad for p in g)]
-        lrs = [config.lr * m for m in mult]
+        lrs = [config.lr * m for _, m in self.trained_groups()]
         wd = config.weight_decay if 'weight_decay' in config else 0.0
         if name == 'SGD':
             return engine.FusedSGD(self.flat, lr=config.lr, momentum=config.momentum if 'momentum' in config else 0.0,
@@ -180,10 +203,8 @@ class Trainer:
         name = config.name if 'name' in config else ''
         if name == 'ReduceLROnPlateau':                              # Examples/BCNN.py:42-44 (without verbose=)
             return _Plateau(self.optimizer, mode='max', factor=0.1, patience=3, threshold=1e-4)
-        return _Cosine(self.optimizer, config.T_max if 'T_max' in config else self.total_epoch,
-                       config.eta_min if 'eta_min' in config else 0.0,
-                       config.warmup_epochs if 'warmup_epochs' in config else 0,
-                       config.lr_warmup_decay if 'lr_warmup_decay' in config else 0.01)
+        T_max, warmup_epochs, warmup_decay = warmup_cosine_args(config, self.total_epoch)
+        return _Cosine(self.optimizer, T_max, config.eta_min if 'eta_min' in config else 0.0, warmup_epochs, warmup_decay)
 
     def to_device(self, m, parallel=False):
         return m.to(self.device, non_blocking=True) if isinstance(m, torch.Tensor) else m.to(self.device)
@@ -264,11 +285,7 @@ class Trainer:
             self._graph = None                                         # another batch shape (last batch of an epoch): eager
             self._graph_steps = -1
         if self._graph is None:
-            outputs = self.forward_model(images, labels)
-            loss = self.criterion(outputs, *targets)
-            self.optimizer.zero_grad()
-            loss.backward()
-            self.allreduce.finish()
+            outputs, loss = self.eager_step(images, labels)
             if self._graph_steps >= 0:
                 self._graph_steps += 1
             if self._graph_steps == 3:
@@ -297,28 +314,36 @@ class Trainer:
             self.criterion.last_correct = g['correct']
         return g['out'], g['loss']
 
+    def eager_step(self, images, labels):
+        """-> (outputs, loss) of forward, criterion, zero_grad, backward and the gradient all-reduce, launched from Python."""
+        outputs = self.forward_model(images, labels)
+        loss = self.criterion(outputs, *_as_tuple(labels))
+        self.optimizer.zero_grad()
+        loss.backward()
+        self.allreduce.finish()
+        return outputs, loss
+
+    @staticmethod
+    def release_inputs(slot):
+        """Lets the next copy into ``slot`` (from ``stage_inputs``) start once the work enqueued so far has finished."""
+        if slot is not None:
+            slot['free'] = torch.cuda.Event()
+            slot['free'].record()
+
     def batch_training(self, data):
         """train.py:310-325: forward, CE(label_smoothing), zero_grad, backward, (grad all-reduce), step, meters.
         No host synchronisation: loss and top-1 count are copied back asynchronously every step (8 bytes into pinned
         memory) and folded into the meters when they have landed."""
         images, labels, slot = self.stage_inputs(data)
-        if self._graph_wanted():
-            outputs, loss = self._graph_step(images, labels)
-        else:
-            outputs = self.forward_model(images, labels)
-            loss = self.criterion(outputs, *_as_tuple(labels))
-            self.optimizer.zero_grad()
-            loss.backward()
-            self.allreduce.finish()
+        outputs, loss = self._graph_step(images, labels) if self._graph_wanted() else self.eager_step(images, labels)
         self.optimizer.step()
         self.after_optimizer_step()
-        if slot is not None:                                          # the input slot may be overwritten from here on
-            slot['free'] = torch.cuda.Event()
-            slot['free'].record()
+        self.release_inputs(slot)
         n = images.size(0)
         correct = getattr(self.criterion, 'last_correct', None)
         if correct is None:                                           # a user-supplied criterion: reference behaviour
-            self.average_meters['acc'].update(accuracy(outputs, labels, 1), n)
+            self.average_meters['acc'].update(accuracy(prediction(self.get_model_module(), outputs),
+                                                       _as_tuple(labels)[0], 1), n)
             self.average_meters['loss'].update(loss.item(), n)
             return loss
         n_acc, n_loss = self.meter_counts(n)
@@ -353,10 +378,12 @@ class Trainer:
         return n, n
 
     def batch_validate(self, data):
-        images, labels = self.to_device(data['img']), self.to_device(data['label'])
+        images, labels = self.batch_tensors(data)
+        images, labels = self.to_device(images), self.to_device(_as_tuple(labels)[0])
         with torch.no_grad():
-            logits = self.model(images)
-        self.average_meters['acc'].update(accuracy(logits, labels, 1), images.size(0))
+            outputs = self.model(images)
+        self.average_meters['acc'].update(accuracy(prediction(self.get_model_module(), outputs), labels, 1),
+                                          images.size(0))
 
     def validate(self):
         self.model.train(False)
@@ -475,9 +502,7 @@ class PeerLearningTrainer(Trainer):
         loss2.backward()
         self.allreduce.finish()
         self.optimizer.step()
-        if slot is not None:
-            slot['free'] = torch.cuda.Event()
-            slot['free'].record()
+        self.release_inputs(slot)
         n = images.size(0)
         acc1, acc2 = accuracy(logits1, labels, 1), accuracy(logits2, labels, 1)
         for k, v in (('acc', max(acc1, acc2)), ('acc1', acc1), ('acc2', acc2), ('loss1', loss1.item()), ('loss2', loss2.item())):
