@@ -7,7 +7,7 @@
 // exactly the K-major wgmma operand layout — and TMA's out-of-bounds zero fill *is* the conv padding.
 //   fwd   : Y[pix, co]  = sum_{tap,ci} X[pix+tap, ci] * Wf[tap][co][ci]        (+bias, ReLU)
 //   dgrad : dX[pix, ci] = sum_{tap,co} dY[pix+tap, co] * Wd[tap][ci][co]       (Wd = flipped/transposed W; * (act>0))
-//   wgrad : dW[tap][co][ci] = sum_pix dY[pix, co] * X[pix+tap, ci]             (both operands MN-major; split-K)
+//   wgrad : dW[tap][ci][co] = sum_pix X[pix+tap, ci] * dY[pix, co]             (X in registers, dY^T in smem; split-K)
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -32,14 +32,14 @@ __global__ void pack_weights_kernel(const float* __restrict__ W, float* __restri
     if (Wd) Wd[((size_t)(8 - t) * Cin + ci) * Cout + co] = v;
   }
 }
-// dWp [9][Cout][Cin] -> dW [Cout][Cin][3][3]
+// dWp [9][Cin][Cout] -> dW [Cout][Cin][3][3]
 __global__ void unpack_wgrad_kernel(const float* __restrict__ dWp, float* __restrict__ dW, int Cout, int Cin, int accumulate) {
   const size_t n = (size_t)Cout * Cin * 9;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     const int t = i % 9;
     const int ci = (i / 9) % Cin;
     const int co = i / ((size_t)9 * Cin);
-    const float v = dWp[((size_t)t * Cout + co) * Cin + ci];
+    const float v = dWp[((size_t)t * Cin + ci) * Cout + co];
     dW[i] = accumulate ? dW[i] + v : v;
   }
 }
@@ -676,68 +676,47 @@ static int conv3x3_igemm_1x(const float* x, const float* wp, const float* bias, 
 }
 
 // ------------------------------------------------------------------------------------------------
-// weight gradient: one CTA accumulates dWp[tap][co0 : co0 + CO][ci0 : ci0 + CI] for ALL 9 taps over its share of the
+// weight gradient: one CTA accumulates dWp[tap][ci0 : ci0 + CI][co0 : co0 + CO] for ALL 9 taps over its share of the
 // pixels (split-K across CTAs, fp32 atomics at the end).  A stage covers a 64-pixel tile (TW x TH x TN, a template
-// parameter: the producer's transposition map and the consumers' tap offsets are compile-time):
-//   A = dY^T (M = co, k = pixel).  TMA lands dY pixel-major ([64 px][32 co] boxes, 128B-swizzled); each consumer thread
-//       reads its m64k8 register fragment straight from there and feeds it to all of its taps, so dY is neither
-//       transposed nor re-read per tap.  The same registers give the bias gradient.
-//   B = X: ONE TMA box of (TH+2) x (TW+2) x TN pixels x 32 ci (the halo patch), transposed by the producer warpgroup
-//       into three kw-shifted K-major copies [32 ci][(TH+2) TW TN px].  Tap (kh, kw) reads copy kw kh*TW pixels further
-//       along k (TW a multiple of 8: whole wgmma k-steps).  A producer task is 4 pixels of one halo row: lane = ci reads
-//       the 6 halo pixels the three kw shifts need (one 128-byte row each) and writes one 16-byte chunk per copy.
-//   Tile: 64 co x 32 ci.  Three consumer warpgroups, one per kernel row kh, load the same dY fragment; warpgroup kh
-//       accumulates taps (kh, 0..2) over all 32 ci with m64n32k8 (48 fp32 registers per thread): 24 wgmmas per stage
-//       and warpgroup.  With A in registers the B bytes a wgmma reads per FLOP depend on M alone, so n32 costs the
-//       shared memory no more than n16, and it runs at the full tensor rate where register-A m64n16k8 reaches about
-//       60 % of it (290 vs 490 TFLOP/s in a throughput loop, H100 SXM at 700 W).
-//   Pipeline: three stage slots {dY boxes, kw copies} and three halo buffers.  The halo box of stage k + 3 is requested
-//   as soon as stage k's has been transposed; dY goes out as soon as its slot is released, up to three stages before
-//   the consumers need it.  The tile origin advances incrementally (no division inside the loop).
+// parameter: the fragment addresses and the k-step of every tap are compile-time).  The GEMM is dW^T: M = ci, N = co.
+//   A = X (M = 64 ci, k = pixel), in registers.  TMA lands the halo patch, (TH+2) x (TW+2) x TN pixels, as two
+//       [pixels][32 ci] boxes (128B-swizzled, zero fill = the conv padding).  Each consumer thread loads its m64k8
+//       fragment straight from there: the kw shift of a tap is a row offset, so X is never transposed or copied.
+//   B = dY^T (N = 64 co, k = pixel), K-major: the producer warp transposes the two [64 px][32 co] dY boxes once
+//       per stage into [co][pixel] (two k-chunks of [64 co][32 px]) and sums the bias gradient on the way.
+//   Consumers: three warpgroups, one per kernel column kw.  Warpgroup kw walks the halo rows; the fragment of halo row
+//       y (one 8-pixel segment) is the A operand of output row y - kh for each kh with 0 <= y - kh < TH, so it is loaded
+//       once and feeds up to three m64n64k8 wgmmas into acc[kh] (3 x 32 fp32 registers per thread): 24 wgmmas per stage
+//       and warpgroup.  The 13-warp CTA puts four warps on one SM sub-partition, so ptxas caps every thread at 128
+//       registers (a producer warpgroup would not raise it: setmaxnreg does not lift the compile-time cap).  Beside the
+//       96 accumulators that leaves room for one fragment: a fragment's wgmmas complete before the next one is loaded,
+//       while the other two warpgroups keep the tensor cores busy.  The swizzle phase of a fragment row depends on y,
+//       the segment, kw and the lane's column; the loads reach at most two threads per bank (8 ci in two 16-byte
+//       chunks x 4 consecutive halo rows).
+//   Pipeline: three stage slots {halo boxes, dY^T, raw dY}.  Raw dY of stage k + 3 is requested as soon as stage k's
+//   has been transposed; the halo boxes as soon as the three consumer warpgroups release the slot.  The tile origin
+//   advances incrementally (no division inside the loop).
 // ------------------------------------------------------------------------------------------------
 struct WgradArgs {
-  float* dWp;  // [9][Cout][Cin], pre-zeroed
+  float* dWp;  // [9][Cin][Cout], pre-zeroed
   float* db;   // [Cout], pre-zeroed, or null
   int N, H, W, Cin, Cout;
   int TW, TH, TN, tiles_w, tiles_h, tiles_n;
   int total_tiles, per;   // pixel tiles, and tiles per split-K CTA (blockIdx.y)
 };
 
-constexpr int WG_THREADS = 512;                    // producer warpgroup + one consumer warpgroup per kernel row
-constexpr int WG_STAGES = 3;                       // stage slots = halo buffers
+constexpr int WG_THREADS = 3 * 128 + 32;           // one consumer warpgroup per kernel column, then one producer warp
+constexpr int WG_STAGES = 3;                       // stage slots
 constexpr int WG_KP = 64;                          // pixels per stage
-constexpr int WG_PATCH_PX = 96;                    // (TH+2) * TW * TN: transposed patch pixels, at most 3 k-chunks of 32
-constexpr int WG_RAW_ROWS = 120;                   // (TH+2) * (TW+2) * TN: halo box rows (TW >= 8)
-constexpr int WG_RAW_BYTES = WG_RAW_ROWS * 128;    // one ci chunk of the halo box (15 KB, whole swizzle atoms)
-constexpr int WG_XT_KW = 3 * 32 * 128;             // one kw copy: 3 k-chunks of [32 ci x 32 px]
-constexpr int WG_XT_CHUNK = 3 * WG_XT_KW;          // the three kw copies of one ci chunk
+constexpr int WG_RAW_ROWS = 120;                   // (TH + 2) * (TW + 2) * TN: halo box rows (TW >= 8)
+constexpr int WG_RAW_BYTES = WG_RAW_ROWS * 128;    // one 32-ci halo box (15 KB, whole swizzle atoms)
 
-constexpr int WG_CO = 64, WG_CI = 32;             // CTA tile
-constexpr int WG_DY_BYTES = (WG_CO / 32) * WG_KP * 128;
-constexpr int WG_STAGE_BYTES = WG_DY_BYTES + WG_XT_CHUNK;
-constexpr int WG_SMEM = WG_STAGES * (WG_STAGE_BYTES + WG_RAW_BYTES) + 1024 + 256;   // 202 KB + alignment + barriers
+constexpr int WG_CI = 64, WG_CO = 64;             // CTA tile
+constexpr int WG_X_BYTES = (WG_CI / 32) * WG_RAW_BYTES;
+constexpr int WG_DY_BYTES = (WG_CO / 32) * WG_KP * 128;                   // raw dY boxes, and dY^T
+constexpr int WG_STAGE_BYTES = WG_X_BYTES + 2 * WG_DY_BYTES;              // {halo boxes, dY^T, raw dY}
+constexpr int WG_SMEM = WG_STAGES * WG_STAGE_BYTES + 1024 + 256;          // 186 KB + alignment + barriers
 static_assert(WG_SMEM <= 227 * 1024, "wgrad shared memory");
-
-// producer warp WARP's share of one halo-box transposition (tasks WARP, WARP + 4, ...).  rw / xt: shared addresses of
-// the halo box and of the stage's kw copies.  xr[m]: this lane's (ci's) swizzled byte offset in a halo row r with
-// r & 7 == m; xw[c]: this lane's offset of 16-byte chunk c in its row of a kw copy.  Everything else is an immediate.
-template <int TW, int TH, int TN, int WARP>
-__device__ __forceinline__ void wgrad_transpose(uint32_t rw, uint32_t xt, const uint32_t (&xr)[8],
-                                                const uint32_t (&xw)[8]) {
-  constexpr int NTASK = (TH + 2) * TW * TN / 4;
-  static_assert(NTASK % 4 == 0, "tasks split evenly over the producer warps");
-#pragma unroll
-  for (int task = WARP; task < NTASK; task += 4) {
-    const int p0 = 4 * task, q = p0 / TW, j0 = p0 % TW;   // patch pixels p0..p0+3: halo row q, columns j0..j0+3
-    const int r0 = q * (TW + 2) + j0;                   // halo rows r0..r0+5 cover the three kw shifts
-    uint32_t v[6];
-#pragma unroll
-    for (int c = 0; c < 6; ++c) v[c] = ld_shared_u32(rw + xr[(r0 + c) & 7] + (r0 + c) * 128);
-#pragma unroll
-    for (int kw = 0; kw < 3; ++kw)
-      st_shared_v4(xt + xw[(p0 & 31) >> 2] + kw * WG_XT_KW + (p0 >> 5) * 4096, v[kw], v[kw + 1], v[kw + 2], v[kw + 3]);
-  }
-}
 
 // tile origin (w0, h0, n0) of pixel tile t, advanced one tile at a time
 template <int TW, int TH, int TN>
@@ -761,14 +740,13 @@ template <int TW, int TH, int TN>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX, WgradArgs a) {
   static_assert(TW * TH * TN == WG_KP && TW % 8 == 0, "64-pixel tile of whole 8-pixel rows");
-  static_assert((TH + 2) * TW * TN <= WG_PATCH_PX && (TH + 2) * (TW + 2) * TN <= WG_RAW_ROWS, "halo patch too large");
+  static_assert((TH + 2) * (TW + 2) * TN <= WG_RAW_ROWS, "halo patch too large");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* stages = smem;                                   // [WG_STAGES] x {dY boxes, three kw copies of X^T}
-  uint8_t* raw = smem + WG_STAGES * WG_STAGE_BYTES;         // [WG_STAGES] halo boxes
-  uint64_t* full = reinterpret_cast<uint64_t*>(raw + WG_STAGES * WG_RAW_BYTES);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + WG_STAGES * WG_STAGE_BYTES);
   uint64_t* empty = full + WG_STAGES;
-  uint64_t* raw_full = empty + WG_STAGES;
+  uint64_t* dy_full = empty + WG_STAGES;
+  const uint32_t stage0 = smem_u32(smem);
 
   const int warp = threadIdx.x >> 5;
   const int n_ci_tiles = (a.Cin + WG_CI - 1) / WG_CI;
@@ -781,141 +759,139 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_cons
     tma_prefetch_desc(&tmDY);
     tma_prefetch_desc(&tmX);
     for (int s = 0; s < WG_STAGES; ++s) {
-      mbar_init(&full[s], 2);       // the dY TMA's expect_tx arrival + the producer's once the X copies are written
+      mbar_init(&full[s], 2);       // the halo TMA's expect_tx arrival + the producer's once dY^T is written
       mbar_init(&empty[s], 3);      // one arrival per consumer warpgroup
-      mbar_init(&raw_full[s], 1);
+      mbar_init(&dy_full[s], 1);
     }
     fence_barrier_init();
   }
   __syncthreads();
   if (nk <= 0) return;
 
-  if (warp < 4) {
-    regs_dealloc<56>();
-    const int t = threadIdx.x, lane = t & 31;
-    constexpr uint32_t raw_tx = (TH + 2) * (TW + 2) * TN * 128;
-    uint32_t xr[8], xw[8];
-#pragma unroll
-    for (int m = 0; m < 8; ++m) {
-      xr[m] = (uint32_t)((((lane >> 2) ^ m) << 4) | ((lane & 3) << 2));
-      xw[m] = sw128_off(lane, 4 * m);
-    }
-    const uint32_t stage0 = smem_u32(stages), raw0 = smem_u32(raw);
-    WgradTile<TW, TH, TN> dy_tile((int)t_begin, a), raw_tile = dy_tile;   // only thread 0 issues TMAs
-    if (t == 0)
+  if (warp == 3 * 4) {
+    // lane transposes rows co = lane and lane + 32 of dY^T (column co & 31 of raw dY box co / 32) and sums their bias
+    const int lane = threadIdx.x & 31;
+    constexpr uint32_t x_tx = (WG_CI / 32) * (TH + 2) * (TW + 2) * TN * 128;
+    WgradTile<TW, TH, TN> x_tile((int)t_begin, a), dy_tile = x_tile;   // only lane 0 issues TMAs
+    if (lane == 0)
       for (int u = 0; u < WG_STAGES && u < nk; ++u) {
-        mbar_expect_tx(&raw_full[u], raw_tx);
-        tma_load_4d(raw + u * WG_RAW_BYTES, &tmX, &raw_full[u], ci0, raw_tile.w0 - 1, raw_tile.h0 - 1, raw_tile.n0);
-        raw_tile.next(a);
+        uint8_t* dy = smem + u * WG_STAGE_BYTES + WG_X_BYTES + WG_DY_BYTES;
+        mbar_expect_tx(&dy_full[u], WG_DY_BYTES);
+#pragma unroll
+        for (int j = 0; j < WG_CO / 32; ++j)
+          tma_load_4d(dy + j * (WG_KP * 128), &tmDY, &dy_full[u], co0 + j * 32, dy_tile.w0, dy_tile.h0, dy_tile.n0);
+        dy_tile.next(a);
       }
+    float bsum[WG_CO / 32] = {};
     int s = 0;
     uint32_t ph = 0;
     for (int k = 0; k < nk; ++k) {
-      uint8_t* st = stages + s * WG_STAGE_BYTES;
+      uint8_t* st = smem + s * WG_STAGE_BYTES;
       mbar_wait(&empty[s], ph ^ 1);
-      if (t == 0) {
-        mbar_expect_tx(&full[s], WG_DY_BYTES);
+      if (lane == 0) {
+        mbar_expect_tx(&full[s], x_tx);
 #pragma unroll
-        for (int j = 0; j < WG_CO / 32; ++j)
-          tma_load_4d(st + j * (WG_KP * 128), &tmDY, &full[s], co0 + j * 32, dy_tile.w0, dy_tile.h0, dy_tile.n0);
-        dy_tile.next(a);
+        for (int j = 0; j < WG_CI / 32; ++j)
+          tma_load_4d(st + j * WG_RAW_BYTES, &tmX, &full[s], ci0 + j * 32, x_tile.w0 - 1, x_tile.h0 - 1, x_tile.n0);
+        x_tile.next(a);
       }
-      mbar_wait(&raw_full[s], ph);
-      const uint32_t rw = raw0 + s * WG_RAW_BYTES, xt = stage0 + s * WG_STAGE_BYTES + WG_DY_BYTES;
-      switch (warp) {
-        case 0: wgrad_transpose<TW, TH, TN, 0>(rw, xt, xr, xw); break;
-        case 1: wgrad_transpose<TW, TH, TN, 1>(rw, xt, xr, xw); break;
-        case 2: wgrad_transpose<TW, TH, TN, 2>(rw, xt, xr, xw); break;
-        default: wgrad_transpose<TW, TH, TN, 3>(rw, xt, xr, xw); break;
-      }
+      mbar_wait(&dy_full[s], ph);
+      const uint32_t dyt = smem_u32(st + WG_X_BYTES), dy = dyt + WG_DY_BYTES;
+#pragma unroll
+      for (int j = 0; j < WG_CO / 32; ++j)
+#pragma unroll
+        for (int k4 = 0; k4 < WG_KP / 4; ++k4) {   // pixels 4 k4 .. 4 k4 + 3: k-chunk k4 / 8
+          uint32_t v[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            v[i] = ld_shared_u32(dy + j * (WG_KP * 128) + sw128_off(4 * k4 + i, lane));
+            bsum[j] += __uint_as_float(v[i]);
+          }
+          st_shared_v4(dyt + (k4 >> 3) * (WG_CO * 128) + sw128_off(32 * j + lane, 4 * (k4 & 7)), v[0], v[1], v[2], v[3]);
+        }
       fence_proxy_async();
-      named_bar(1, 128);                            // every thread is done with halo buffer s
-      if (t == 0) {
+      __syncwarp();                                 // dY^T is complete and raw dY slot s is free
+      if (lane == 0) {
         if (k + WG_STAGES < nk) {
-          mbar_expect_tx(&raw_full[s], raw_tx);
-          tma_load_4d(raw + s * WG_RAW_BYTES, &tmX, &raw_full[s], ci0, raw_tile.w0 - 1, raw_tile.h0 - 1, raw_tile.n0);
-          raw_tile.next(a);
+          mbar_expect_tx(&dy_full[s], WG_DY_BYTES);
+#pragma unroll
+          for (int j = 0; j < WG_CO / 32; ++j)
+            tma_load_4d(st + WG_X_BYTES + WG_DY_BYTES + j * (WG_KP * 128), &tmDY, &dy_full[s], co0 + j * 32, dy_tile.w0,
+                        dy_tile.h0, dy_tile.n0);
+          dy_tile.next(a);
         }
         mbar_arrive(&full[s]);
       }
       if (++s == WG_STAGES) { s = 0; ph ^= 1; }
     }
-  } else {
-    regs_alloc<152>();
-    const int ct = threadIdx.x - 128;
-    const int kh = ct >> 7, t = ct & 127, wl = t >> 5, lane = t & 31, g = lane >> 2, q = lane & 3;
-    // this thread's A rows: co 16 wl + g (+8), in dY box wl / 2 at column 16 (wl & 1) + g (+8)
-    const int box = wl >> 1, col = 16 * (wl & 1) + g;
-    const uint32_t off0 = sw128_off(q, col), off1 = sw128_off(q, col + 8), off2 = sw128_off(q + 4, col),
-                   off3 = sw128_off(q + 4, col + 8);
-    // B start of k-step ks in copy 0, in 16-byte descriptor units: patch pixel 8 ks + 2 TW per earlier image + kh TW
-    uint32_t boff[8];
+    // bias: added once per co, by the ci-tile-0 CTAs
 #pragma unroll
-    for (int ks = 0; ks < 8; ++ks) {
-      const int kk = 8 * ks + (8 * ks) / (TH * TW) * 2 * TW + kh * TW;
-      boff[ks] = (uint32_t)((kk >> 5) * 4096 + (kk & 31) / 8 * 32) >> 4;
-    }
-    float acc[3][16];
+    for (int j = 0; j < WG_CO / 32; ++j)
+      if (a.db && ci_t == 0 && co0 + 32 * j + lane < a.Cout) atomicAdd(a.db + co0 + 32 * j + lane, bsum[j]);
+  } else {
+    const int kw = warp >> 2, t = threadIdx.x & 127, wl = t >> 5, lane = t & 31, g = lane >> 2, q = lane & 3;
+    // this thread's A rows: ci 16 wl + g (+8) = column cib (+8) of halo box wl / 2.  Its k columns q (+4) of a fragment
+    // whose 8 pixels start at halo row R read halo rows R + kw + q (+4).  In a SWIZZLE_128B box the 16-byte chunk of a
+    // row is XOR-ed with bits 7..9 of the row's address, which is computed per fragment: a table of phases would cost
+    // the registers the wgmma pipeline needs.  cq: chunk and word of ci cib in an unswizzled row.  cib / 4 is 0, 1, 4
+    // or 5, so ci cib + 8 is chunk ^ 2 (address ^ 32).
+    const int cib = 16 * (wl & 1) + g;
+    const uint32_t cq = (uint32_t)(((cib >> 2) << 4) | ((cib & 3) << 2));
+    const uint32_t xrow = (uint32_t)((wl >> 1) * WG_RAW_BYTES + (kw + q) * 128);
+    float acc[3][32];
 #pragma unroll
     for (int j = 0; j < 3; ++j)
 #pragma unroll
-      for (int e = 0; e < 16; ++e) acc[j][e] = 0.f;
-    float bsum0 = 0.f, bsum1 = 0.f;                 // bias gradient of rows g and g + 8
-    uint32_t fr[2][4];                              // two fragment sets: one may still be read by the wgmmas in flight
+      for (int e = 0; e < 32; ++e) acc[j][e] = 0.f;
+    uint32_t f[4];
+    constexpr int SEG = TW / 8, NF = TN * (TH + 2) * SEG;   // 8-pixel halo row segments per stage
     int s = 0;
     uint32_t ph = 0;
     for (int k = 0; k < nk; ++k) {
       mbar_wait(&full[s], ph);
-      const uint32_t dyb = smem_u32(stages + s * WG_STAGE_BYTES + box * (WG_KP * 128));
-      const uint64_t xdesc = make_sdesc(smem_u32(stages + s * WG_STAGE_BYTES + WG_DY_BYTES));
+      const uint32_t xb = stage0 + s * WG_STAGE_BYTES, xa = xb + xrow;
+      const uint64_t bdesc = make_sdesc(xb + WG_X_BYTES);
 #pragma unroll
-      for (int ks = 0; ks < 8; ++ks) {
-        uint32_t (&f)[4] = fr[ks & 1];
-        // pixel rows 8 ks + q (+4): the swizzle phase (row & 7) is the same every k-step, so one offset per element
-        const uint32_t fa = dyb + ks * 1024;
-        f[0] = ld_shared_u32(fa + off0);
-        f[1] = ld_shared_u32(fa + off1);
-        f[2] = ld_shared_u32(fa + off2);
-        f[3] = ld_shared_u32(fa + off3);
-        bsum0 += __uint_as_float(f[0]) + __uint_as_float(f[2]);
-        bsum1 += __uint_as_float(f[1]) + __uint_as_float(f[3]);
+      for (int i = 0; i < NF; ++i) {
+        const int n = i / ((TH + 2) * SEG), y = i / SEG % (TH + 2), js = i % SEG;
+        const int R = (n * (TH + 2) + y) * (TW + 2) + 8 * js;
+        const uint32_t r0 = xa + R * 128, r4 = xa + (R + 4) * 128;
+        const uint32_t p0 = r0 + (((r0 >> 3) & 0x70) ^ cq), p4 = r4 + (((r4 >> 3) & 0x70) ^ cq);
+        f[0] = ld_shared_u32(p0);
+        f[1] = ld_shared_u32(p0 ^ 32);
+        f[2] = ld_shared_u32(p4);
+        f[3] = ld_shared_u32(p4 ^ 32);
         wgmma_fence();
 #pragma unroll
-        for (int kw = 0; kw < 3; ++kw) wgmma_tf32(acc[kw], f, xdesc + boff[ks] + kw * (WG_XT_KW >> 4));
+        for (int kh = 0; kh < 3; ++kh) {
+          const int h = y - kh;
+          if (h < 0 || h >= TH) continue;
+          const int ks = ((n * TH + h) * TW + 8 * js) / 8;   // k-step of output pixels (n, h, 8 js .. 8 js + 7)
+          wgmma_tf32(acc[kh], f, bdesc + (uint32_t)(((ks >> 2) * (WG_CO * 128) + (ks & 3) * 32) >> 4));
+        }
         wgmma_commit();
-        wgmma_wait<1>();      // k-step ks stays in flight; ks - 1 (and its fragment set) is done
+        wgmma_wait<0>();      // f is free again; the other two warpgroups keep the tensor cores busy meanwhile
 #pragma unroll
         for (int j = 0; j < 3; ++j) wgmma_keep(acc[j]);
-        if (ks == 0 && k > 0 && t == 0) mbar_arrive(&empty[s == 0 ? WG_STAGES - 1 : s - 1]);   // stage k - 1 is done
       }
+      if (t == 0) mbar_arrive(&empty[s]);
       if (++s == WG_STAGES) { s = 0; ph ^= 1; }
     }
-    wgmma_wait<0>();
+    // accumulator element 4 i + e: ci row 16 wl + g + 8 (e >> 1), co columns 8 i + 2 q (+1), adjacent in dWp
 #pragma unroll
-    for (int j = 0; j < 3; ++j) wgmma_keep(acc[j]);
+    for (int kh = 0; kh < 3; ++kh)
 #pragma unroll
-    for (int kw = 0; kw < 3; ++kw)
-#pragma unroll
-      for (int e = 0; e < 16; ++e) {
-        const int co = co0 + 16 * wl + g + 8 * ((e >> 1) & 1);
-        const int ci = ci0 + 8 * (e >> 2) + 2 * q + (e & 1);
-        if (co < a.Cout) atomicAdd(a.dWp + ((size_t)(3 * kh + kw) * a.Cout + co) * a.Cin + ci, acc[kw][e]);
+      for (int e = 0; e < 32; e += 2) {
+        const int ci = ci0 + 16 * wl + g + 8 * ((e >> 1) & 1);
+        const int co = co0 + 8 * (e >> 2) + 2 * q;
+        if (ci < a.Cin && co < a.Cout)
+          atomicAdd(reinterpret_cast<float2*>(a.dWp + ((size_t)(3 * kh + kw) * a.Cin + ci) * a.Cout + co),
+                    make_float2(acc[kh][e], acc[kh][e + 1]));
       }
-    // bias: the quad's four threads hold the same rows at different pixels; one atomic per co on the ci-tile-0 CTAs
-    // (all three warpgroups read the same rows: warpgroup 0 adds them)
-    bsum0 += __shfl_xor_sync(0xffffffffu, bsum0, 1);
-    bsum0 += __shfl_xor_sync(0xffffffffu, bsum0, 2);
-    bsum1 += __shfl_xor_sync(0xffffffffu, bsum1, 1);
-    bsum1 += __shfl_xor_sync(0xffffffffu, bsum1, 2);
-    if (a.db && ci_t == 0 && kh == 0 && q == 0) {
-      const int co = co0 + 16 * wl + g;
-      if (co < a.Cout) atomicAdd(a.db + co, bsum0);
-      if (co + 8 < a.Cout) atomicAdd(a.db + co + 8, bsum1);
-    }
   }
 }
 
-// pixel tile for wgrad: TW in {8,16} (kh shifts must be whole wgmma k-steps of 8 pixels), TW*TH*TN = 64, TH*TW % 8 == 0.
+// pixel tile for wgrad: TW in {8,16} (a fragment is 8 pixels of one tile row), TW*TH*TN = 64, TH*TW % 8 == 0.
 // Returns one of the three tiles launch_wgrad instantiates: (16, 4, 1), (8, 8, 1), (8, 4, 2).
 static bool pick_wgrad_tile(int W, int H, int* TW, int* TH, int* TN) {
   int tw = 0;
@@ -924,7 +900,7 @@ static bool pick_wgrad_tile(int W, int H, int* TW, int* TH, int* TN) {
   int th = 1;
   while (th * 2 * tw <= 64 && H % (th * 2) == 0) th *= 2;
   int tn = 64 / (tw * th);
-  if ((th * tw) % 8 != 0 || (th + 2) * tw * tn > WG_PATCH_PX) {   // fall back to one image per tile, partial tiles in H allowed
+  if ((th * tw) % 8 != 0 || (th + 2) * (tw + 2) * tn > WG_RAW_ROWS) {   // fall back to one image per tile, partial tiles in H allowed
     th = 64 / tw;
     tn = 1;
   }
@@ -946,7 +922,7 @@ static int launch_wgrad(const float* x, const float* dy, WgradArgs a, cudaStream
   const long long out_tiles = (long long)((a.Cout + WG_CO - 1) / WG_CO) * ((a.Cin + WG_CI - 1) / WG_CI);
   const long long total_tiles = (long long)a.tiles_w * a.tiles_h * a.tiles_n;
   HK_REQUIRE(total_tiles < (1ll << 31), HK_ERR_UNSUPPORTED, "conv3x3_wgrad: too many pixel tiles");
-  // split-K factor.  The kernel runs one CTA per SM (its 202 KB of shared memory allow no second, and its 512 threads
+  // split-K factor.  The kernel runs one CTA per SM (its 186 KB of shared memory allow no second, and its 512 threads
   // hold the whole register file), so the grid executes in whole waves of `sms` CTAs: pick the split that fills
   // 1..3 waves best (ties -> fewer waves: fewer partial sums to add).
   const int sms = num_sms();
@@ -1006,7 +982,7 @@ static int conv3x3_wgrad_1x(const float* x, const float* dy, float* dwp, float* 
   WgradArgs a = {};
   a.dWp = dwp; a.db = db; a.N = N; a.H = H; a.W = W; a.Cin = Cin; a.Cout = Cout;
   pick_wgrad_tile(W, H, &a.TW, &a.TH, &a.TN);
-  HK_REQUIRE((a.TH + 2) * a.TW * a.TN <= WG_PATCH_PX && (a.TH + 2) * (a.TW + 2) * a.TN <= WG_RAW_ROWS, HK_ERR_UNSUPPORTED,
+  HK_REQUIRE((a.TH + 2) * (a.TW + 2) * a.TN <= WG_RAW_ROWS, HK_ERR_UNSUPPORTED,
              "conv3x3_wgrad: halo patch too large");
   a.tiles_w = (W + a.TW - 1) / a.TW; a.tiles_h = (H + a.TH - 1) / a.TH; a.tiles_n = (N + a.TN - 1) / a.TN;
   cudaError_t e = cudaSuccess;
