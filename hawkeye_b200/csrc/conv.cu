@@ -334,14 +334,23 @@ static int launch_conv(const CUtensorMap& tmX, const CUtensorMap& tmW, const Con
 //   * RESIDENT (Cin = 64, Cout = 64: VGG conv1_2 and its dgrad): all 9x2 weight tiles (144 KB) stay in shared memory for
 //     the life of the CTA; only activations stream.
 //   * the shared-memory ring runs across tiles, so the producer loads tile i+1 while the MMA warpgroups finish tile i.
+//   * BN = 128 has room for two 68 KB stages beside the staging tile, which is too shallow to hide a stage's load: with
+//     the epilogue removed the forward main loop ran at 295-310 TFLOP/s, at 340-360 when the weights were loaded only for
+//     a CTA's first tile, and at 380-420 with a third stage in place of the staging tile (H100 SXM, 700 W).  So the bound
+//     is the latency of a stage's load, not the bytes it moves (two-CTA clusters that multicast each weight tile, 35 %
+//     fewer L2 bytes per stage, ran at ~200 TFLOP/s: a slot is freed only when both CTAs have released it), and each
+//     stage there
+//     has three full barriers, {halo patch + kh 0 weights, kh 1 weights, kh 2 weights}, and one wgmma group per piece:
+//     the MMAs of a piece start as soon as it has landed, and the previous stage is handed back after the first group
+//     is issued, while the later pieces may still be in flight.  The accumulation order does not change.  The BN = 64
+//     ring is three stages deep and keeps one barrier per stage.
 //   * the MMA warpgroups hand each finished tile to a fourth, epilogue warpgroup through a shared-memory staging tile and
 //     go straight on to the next tile: the output stores and the mask loads of tile i overlap the MMAs of tile i+1.
 //   * the epilogue of the stored map has 8 lanes per pixel (one float4 of the 32-channel chunk each), so a warp's load
 //     or store instruction covers 4 whole 128-byte lines (with thread = pixel it touched 32 lines, 16 bytes of each).
 //     Mask loads and output stores are streaming (ld.global.cs / st.global.cs): each byte is touched once, and as
 //     ordinary accesses the mask pushed the halo rows and weight tiles that neighbouring CTAs re-read out of L2, which
-//     cost the data gradient of the 128-channel-and-deeper layers 8-20 %.  With no epilogue at all the main loop runs at
-//     295-305 TFLOP/s on every layer from conv2_1 on (H100 SXM, 700 W), so that is what is left to hide behind.  Asking
+//     cost the data gradient of the 128-channel-and-deeper layers 8-20 %.  Asking
 //     for the mask a chunk ahead of its use measured no different and is not done.  The fused pooling keeps thread =
 //     pixel, which its shuffles need.
 // ------------------------------------------------------------------------------------------------
@@ -354,6 +363,9 @@ struct ConvV2Cfg {
   static constexpr int STAGE_BYTES = A_BYTES + (RESIDENT ? 0 : 3 * B_TILE);
   static constexpr int STAGES = RESIDENT ? 2 : (BN == 64 ? 3 : 2);
   static constexpr int WRES_BYTES = RESIDENT ? 18 * B_TILE : 0;      // 9 taps x 2 chunks
+  // full barriers per stage: {halo patch + kh 0 weights, kh 1 weights, kh 2 weights} where the ring is two stages deep,
+  // else one for the whole stage
+  static constexpr int PIECES = STAGES == 2 && !RESIDENT ? 3 : 1;
   // staging tile [128 pixels][BN + 8] fp32: the padding makes the MMA threads' 8-byte fragment stores conflict-free
   // (rows 8 words apart in bank space, 4 lanes x 8 B per row); the epilogue of the stored map reads a pixel's 128-byte
   // chunk with 8 consecutive lanes, one float4 each: all 32 banks once per quarter-warp, whatever the pitch.
@@ -376,8 +388,8 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* stages = smem;
   uint8_t* wres = smem + Cfg::STAGES * Cfg::STAGE_BYTES;
-  uint64_t* full = reinterpret_cast<uint64_t*>(wres + Cfg::WRES_BYTES);
-  uint64_t* empty = full + Cfg::STAGES;
+  uint64_t* full = reinterpret_cast<uint64_t*>(wres + Cfg::WRES_BYTES);   // [STAGES][PIECES]
+  uint64_t* empty = full + Cfg::STAGES * Cfg::PIECES;
   uint64_t* wbar = empty + Cfg::STAGES;
   uint64_t* stg_full = wbar + 1;                    // the MMA threads wrote the staging tile (256 arrivals)
   uint64_t* stg_empty = wbar + 2;                   // the epilogue threads read it (128 arrivals)
@@ -390,7 +402,8 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmW);
-    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
+    for (int s = 0; s < Cfg::STAGES; ++s) mbar_init(&empty[s], 2);
+    for (int i = 0; i < Cfg::STAGES * Cfg::PIECES; ++i) mbar_init(&full[i], 1);
     mbar_init(wbar, 1);
     mbar_init(stg_full, 256);
     mbar_init(stg_empty, 128);
@@ -508,13 +521,17 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
           const uint32_t ph = (kbg / Cfg::STAGES) & 1;
           const int ck = kb / 3, kw = kb - ck * 3;
           mbar_wait(&empty[s], ph ^ 1);
-          mbar_expect_tx(&full[s], Cfg::STAGE_BYTES);
+          uint64_t* f = full + s * Cfg::PIECES;
           uint8_t* st = stages + s * Cfg::STAGE_BYTES;
-          tma_load_4d(st, &tmX, &full[s], ck * 32, w0 + kw - 1, h0 - 1, n0);
+          mbar_expect_tx(&f[0], Cfg::PIECES == 3 ? Cfg::A_BYTES + Cfg::B_TILE : Cfg::STAGE_BYTES);
+          tma_load_4d(st, &tmX, &f[0], ck * 32, w0 + kw - 1, h0 - 1, n0);
           if (!RESIDENT) {
 #pragma unroll
-            for (int kh = 0; kh < 3; ++kh)
-              tma_load_3d(st + Cfg::A_BYTES + kh * Cfg::B_TILE, &tmW, &full[s], ck * 32, co0, kh * 3 + kw);
+            for (int kh = 0; kh < 3; ++kh) {
+              uint64_t* fk = &f[Cfg::PIECES == 3 ? kh : 0];
+              if (Cfg::PIECES == 3 && kh > 0) mbar_expect_tx(fk, Cfg::B_TILE);
+              tma_load_3d(st + Cfg::A_BYTES + kh * Cfg::B_TILE, &tmW, fk, ck * 32, co0, kh * 3 + kw);
+            }
           }
         }
       }
@@ -534,22 +551,30 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
       for (int kb = 0; kb < nkb; ++kb, ++kbg) {
         const int s = kbg % Cfg::STAGES;
         const int ck = kb / 3, kw = kb - ck * 3;
-        mbar_wait(&full[s], (kbg / Cfg::STAGES) & 1);
+        const uint32_t ph = (kbg / Cfg::STAGES) & 1;
         // rows 64 wg.. of the tile in the patch of tap kh: + (WG_ROWS wg + TW kh) rows of 128 B
         const uint32_t a_addr = smem_u32(stages + s * Cfg::STAGE_BYTES) + wg * WG_ROWS * 128;
-        wgmma_fence();
 #pragma unroll
         for (int kh = 0; kh < 3; ++kh) {
+          // each piece of the stage is consumed as soon as it has landed, one wgmma group per piece
+          if (kh < Cfg::PIECES) {
+            mbar_wait(&full[s * Cfg::PIECES + kh], ph);
+            wgmma_fence();
+          }
           const uint32_t b_addr = RESIDENT ? smem_u32(wres + ((kh * 3 + kw) * 2 + ck) * Cfg::B_TILE)
                                            : smem_u32(stages + s * Cfg::STAGE_BYTES + Cfg::A_BYTES + kh * Cfg::B_TILE);
           const uint64_t ad = make_sdesc(a_addr + kh * TW * 128), bd = make_sdesc(b_addr);
 #pragma unroll
           for (int ks = 0; ks < 4; ++ks) wgmma_tf32(acc, ad + ks * 2, bd + ks * 2, (kb | kh | ks) != 0);
+          if (kh >= 3 - Cfg::PIECES) wgmma_commit();
+          if (kh == 3 - Cfg::PIECES) {
+            // the first group of step kb stays in flight; the stage of the previous step is free, and is handed back
+            // while this step's later pieces may still be landing
+            wgmma_wait<1>();
+            wgmma_keep(acc);
+            if (kb > 0 && (ct & 127) == 0) mbar_arrive(&empty[(kbg - 1) % Cfg::STAGES]);
+          }
         }
-        wgmma_commit();
-        wgmma_wait<1>();          // (chunk, kw) step kb stays in flight; the stage of the previous step is free
-        wgmma_keep(acc);
-        if (kb > 0 && (ct & 127) == 0) mbar_arrive(&empty[(kbg - 1) % Cfg::STAGES]);
       }
       wgmma_wait<0>();
       wgmma_keep(acc);
