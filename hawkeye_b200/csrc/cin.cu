@@ -112,6 +112,50 @@ __global__ void se_gate_bwd_kernel(const float* __restrict__ x, const float* __r
   if (lane == 0) dm[r] = acc * g * (1.f - g);
 }
 
+// CIN's contrastive loss (reference model/loss/CIN_loss.py:26-46).  d[i] = z[i] - z[half + i] over the flattened
+// [B, F] map: the pairs' difference before the projection h, whose bias cancels in h(a) - h(b).  Rounded to tf32 when
+// `round` (the default mode), as every operand handed to a single-pass TF32 product is.
+__global__ void cin_pair_diff_fwd_kernel(const float* __restrict__ z, float* __restrict__ d, size_t n, int round) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float v = z[i] - z[n + i];
+    d[i] = round ? tf32_round(v) : v;
+  }
+}
+// dz = [dd; -dd]
+__global__ void cin_pair_diff_bwd_kernel(const float* __restrict__ dd, float* __restrict__ dz, size_t n) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float g = dd[i];
+    dz[i] = g;
+    dz[n + i] = -g;
+  }
+}
+
+// nn.PairwiseDistance's eps: ||a - b + eps|| (CIN_loss.py:19)
+constexpr float kPairwiseEps = 1e-6f;
+
+// One block.  Pair i (< B/2) is matched when labels[i] == labels[B/2] (CIN_loss.py:39: every label of the first half
+// against the single label labels[B/2]).  L1 = sum over matched i of ||p_i + eps||^2; the hinge term of :40-42 is
+// overwritten by L1^2 at :43, so loss = alpha (L1 + L1^2) and dp_i = alpha (1 + 2 L1) 2 (p_i + eps) on matched rows, 0 on
+// the others.  The sum runs in fp32 in a fixed order, so the result has the same bits on every run.
+__global__ void cin_contrastive_loss_kernel(const float* __restrict__ p, const long long* __restrict__ labels,
+                                            float* __restrict__ loss, float* __restrict__ dp, int B, int R, float alpha) {
+  __shared__ float red[32];
+  const int half = B / 2;
+  const long long anchor = labels[half];
+  const size_t n = (size_t)half * R;
+  float s = 0.f;
+  for (size_t i = threadIdx.x; i < n; i += blockDim.x) {
+    if (labels[i / R] != anchor) continue;
+    const float v = p[i] + kPairwiseEps;
+    s = fmaf(v, v, s);
+  }
+  const float l1 = block_sum(s, red);
+  const float scale = 2.f * alpha * fmaf(2.f, l1, 1.f);
+  for (size_t i = threadIdx.x; i < n; i += blockDim.x)
+    dp[i] = labels[i / R] == anchor ? scale * (p[i] + kPairwiseEps) : 0.f;
+  if (threadIdx.x == 0) loss[0] = alpha * fmaf(l1, l1, l1);
+}
+
 }  // namespace hk
 
 using namespace hk;
@@ -144,6 +188,29 @@ int hk_cci_weight_bwd(const float* w_sci, const float* weight, const float* d_cc
   if (e != cudaSuccess) return set_error((int)e, "cudaMemsetAsync(d_weight): %s", cudaGetErrorString(e));
   cci_weight_bwd_kernel<<<dim3(64, B), 256, 0, (cudaStream_t)stream>>>(w_sci, weight, d_cci, d_sci, d_weight, B, (size_t)per);
   HK_LAUNCH_CHECK("cci_weight_bwd_kernel");
+  return 0;
+}
+int hk_cin_pair_diff_fwd(const float* z, float* d, int B, long long per, void* stream) {
+  HK_REQUIRE(z && d && B > 0 && B % 2 == 0 && per > 0, HK_ERR_ARG, "hk_cin_pair_diff_fwd: bad args (B must be even)");
+  const size_t n = (size_t)(B / 2) * per;
+  cin_pair_diff_fwd_kernel<<<grid_1d(n, 256), 256, 0, (cudaStream_t)stream>>>(z, d, n, precise() ? 0 : 1);
+  HK_LAUNCH_CHECK("cin_pair_diff_fwd_kernel");
+  return 0;
+}
+int hk_cin_pair_diff_bwd(const float* dd, float* dz, int B, long long per, void* stream) {
+  HK_REQUIRE(dd && dz && B > 0 && B % 2 == 0 && per > 0, HK_ERR_ARG, "hk_cin_pair_diff_bwd: bad args (B must be even)");
+  const size_t n = (size_t)(B / 2) * per;
+  cin_pair_diff_bwd_kernel<<<grid_1d(n, 256), 256, 0, (cudaStream_t)stream>>>(dd, dz, n);
+  HK_LAUNCH_CHECK("cin_pair_diff_bwd_kernel");
+  return 0;
+}
+int hk_cin_contrastive_loss(const float* p, const long long* labels, float* loss, float* dp, int B, int R, float alpha,
+                            void* stream) {
+  HK_REQUIRE(p && labels && loss && dp, HK_ERR_ARG, "hk_cin_contrastive_loss: null pointer");
+  HK_REQUIRE(B > 0 && B % 2 == 0 && R > 0, HK_ERR_ARG, "hk_cin_contrastive_loss: B=%d must be even and positive, R=%d > 0",
+             B, R);
+  cin_contrastive_loss_kernel<<<1, 512, 0, (cudaStream_t)stream>>>(p, labels, loss, dp, B, R, alpha);
+  HK_LAUNCH_CHECK("cin_contrastive_loss_kernel");
   return 0;
 }
 int hk_se_gate_fwd(const float* x, const float* m, float* s, long long rows, int hw, void* stream) {

@@ -1,5 +1,6 @@
 """Trainer subclasses of the hot-path methods with the reference's Examples/ surface:
-``python -m hawkeye_b200.examples {BCNN,CBCNN,MPN,PeerLearning,OSMENet,APINet,DCL,ProtoTreeNet,InterpPartsNet,NTSNet,APCNN,MGE_CNN}
+``python -m hawkeye_b200.examples {BCNN,CBCNN,MPN,PeerLearning,OSMENet,APINet,DCL,ProtoTreeNet,InterpPartsNet,NTSNet,APCNN,MGE_CNN,
+CIN}
 --config <yaml>`` replaces
 ``python Examples/<Method>.py --config <yaml>`` (same yaml files; one process per GPU under torchrun instead of nn.DataParallel).
 
@@ -458,12 +459,51 @@ class MGE_CNNTrainer(Trainer):
         return _warmup_cosine(self.optimizer, config, self.total_epoch)
 
 
+class CINTrainer(Trainer):
+    """Examples/CIN.py: class-balanced batches (n_classes x n_samples images); criterion = CINLoss (cross-entropy +
+    alpha x the contrastive term through the criterion's own projection ``h``), moved to the device; SGD over two groups,
+    the model's parameters and the criterion's, both at lr, with the yaml's weight_decay and momentum (the reference passes
+    none: 0 unless the yaml sets one); LinearLR warm-up into cosine annealing over T_max - warmup_epochs.  The step has no
+    host synchronisation, so ``cuda_graph: true`` captures and replays it.
+
+    save_model writes the model alone, the reference's format; save_checkpoint adds ``criterion``, the state of ``h``
+    (51 M weights with the shipped config), which load_checkpoint restores, so that ``h`` and its slice of the optimizer
+    resume together.  A checkpoint without it keeps the freshly initialised ``h``, with a warning."""
+
+    def get_dataloader(self, config):
+        return _balanced_loaders(self, config)
+
+    def get_criterion(self, config):
+        from .losses import CINLoss
+        return self.to_device(CINLoss(config))
+
+    def param_groups(self):
+        return [(list(self.get_model_module().parameters()), 1.0), (list(self.criterion.parameters()), 1.0)]
+
+    def get_scheduler(self, config):
+        return _warmup_cosine(self.optimizer, config, self.total_epoch)
+
+    def checkpoint_state(self):
+        ck = super().checkpoint_state()
+        ck['criterion'] = {k: v.detach().cpu().clone() for k, v in self.criterion.state_dict().items()}
+        return ck
+
+    def restore_checkpoint(self, ck, path):
+        super().restore_checkpoint(ck, path)
+        if 'criterion' in ck:
+            self.criterion.load_state_dict(ck['criterion'])
+        else:
+            self.logger.warning('checkpoint %s has no criterion state: the projection h of CINLoss keeps its fresh '
+                                'initialisation', path)
+
+
 TRAINERS = {'BCNN': BCNNTrainer, 'CBCNN': CBCNNTrainer, 'MPN': MPNTrainer, 'PeerLearning': PeerLearningTrainer,
             'OSMENet': OSMENetTrainer}
 # TRAINERS keeps the key set it has always had, so code that enumerates it sees no change; the command line dispatches
-# over every method, APINet, DCL, ProtoTreeNet, InterpPartsNet, NTSNet, APCNN and MGE_CNN included.
+# over every method, APINet, DCL, ProtoTreeNet, InterpPartsNet, NTSNet, APCNN, MGE_CNN and CIN included.
 ALL_TRAINERS = dict(TRAINERS, APINet=APINetTrainer, DCL=DCLTrainer, ProtoTreeNet=ProtoTreeTrainer,
-                   InterpPartsNet=InterpPartsNetTrainer, NTSNet=NTSNetTrainer, APCNN=APCNNTrainer, MGE_CNN=MGE_CNNTrainer)
+                   InterpPartsNet=InterpPartsNetTrainer, NTSNet=NTSNetTrainer, APCNN=APCNNTrainer, MGE_CNN=MGE_CNNTrainer,
+                   CIN=CINTrainer)
 
 
 def main(argv=None):

@@ -255,6 +255,57 @@ class MGECNNLoss(nn.Module):
         return loss
 
 
+class CINLoss(nn.Module):
+    """model/loss/CIN_loss.py with the reference's config keys, defaults and ``h`` (nn.Linear(channel * feature_size,
+    r_channel), initialised by utils.initialize_weights; state_dict keys ``h.weight`` / ``h.bias``).  What the reference
+    computes, reproduced here:
+    - pair_label = target[:B/2] == target[B/2]: every label of the first half against the ONE label target[B/2], not the
+      second half element by element;
+    - L1 = sum over those pairs of ||h(Z_CCI_i) - h(Z_CCI_{B/2+i}) + 1e-6||^2 (nn.PairwiseDistance's eps);
+    - the margin hinge with ``beta`` is computed and then overwritten by L1^2, so ``beta`` changes nothing;
+    - loss = CE_ls0.1(Z, target) + alpha (L1 + L1^2); the cross-entropy alone when the output is not a tuple (eval mode).
+    With the class-by-class batches of BalancedBatchSampler (n_classes x n_samples, 4 x 5 in configs/CIN.yaml), target[B/2]
+    is a class of the second half only, no pair matches, the contrastive term is 0 and ``h`` gets a zero gradient (not
+    None): the optimizer's weight decay still shrinks it every step, as in the reference.
+
+    The projection runs on the pair differences (ops_cin.PairDiffProjFn) and the contrastive term with its gradient in one
+    launch that builds the pair mask on the device (ops_cin.ContrastiveLossFn): no host read-back, where the reference's
+    boolean indexing synchronises four times per step.  ``last_correct`` is the top-1 count of the cross-entropy kernel."""
+
+    def __init__(self, config):
+        super().__init__()
+        from . import ops
+        from .utils import initialize_weights
+        self.alpha = config.alpha if 'alpha' in config else 2.0
+        self.beta = config.beta if 'beta' in config else 0.5            # read by nothing: see the class docstring
+        self.channel = config.channel if 'channel' in config else 2048
+        self.feature_size = config.feature_size if 'feature_size' in config else 7 * 7
+        self.r_channel = config.r_channel if 'r_channel' in config else 512
+        if self.r_channel % 4:
+            raise ValueError(f'CINLoss: r_channel={self.r_channel} must be a multiple of 4 (16-byte row pitch of the '
+                             'projection gradients)')
+        self.ce_loss = ops.CrossEntropyLS(0.1)
+        self.h = nn.Linear(self.channel * self.feature_size, self.r_channel)
+        self.apply(initialize_weights)
+
+    def forward(self, output, target):
+        from .ops_cin import ContrastiveLossFn, PairDiffProjFn
+        if not isinstance(output, tuple):
+            loss = self.ce_loss(output, target)
+            self.last_correct = self.ce_loss.last_correct
+            return loss
+        Z, Z_CCI = output
+        B = Z_CCI.shape[0]
+        if Z_CCI[0].numel() != self.h.in_features:
+            raise ValueError(f'CINLoss: Z_CCI {tuple(Z_CCI.shape)} has {Z_CCI[0].numel()} features per sample, the criterion '
+                             f'channel x feature_size = {self.channel} x {self.feature_size} = {self.h.in_features} (a '
+                             '448x448 input gives a 14x14 map: feature_size 196)')
+        loss_ce = self.ce_loss(Z, target)
+        self.last_correct = self.ce_loss.last_correct
+        p = PairDiffProjFn.apply(Z_CCI.reshape(B, -1), self.h.weight, self.h.bias)
+        return loss_ce + ContrastiveLossFn.apply(p, target, self.alpha)
+
+
 class InterpPartsLoss(nn.Module):
     """model/loss/InterpParts_loss.py: CrossEntropy(logits) + coeff x ShapingLoss(assign) on the (logits, att, assign)
     triple Interp-Parts returns, with the reference's config keys and defaults (radius 2, std 0.4, num_parts 5, alpha 1,

@@ -1,11 +1,12 @@
 """Autograd bindings for the channel-interaction module (reference model/methods/CIN.py:24-60): batched Gram and W.X
 products on the wgmma GEMM, softmax(-G), the contrastive weight |W_SCI - w W_SCI_BA|, the residual add and OSME's
-excitation gate (the 3x3 convolution is ops.Conv3x3Fn).  Host plumbing only; all arithmetic is in libhawkeye_b200.so."""
+excitation gate (the 3x3 convolution is ops.Conv3x3Fn), and the pair-difference projection and contrastive term of CIN's
+loss (model/loss/CIN_loss.py).  Host plumbing only; all arithmetic is in libhawkeye_b200.so."""
 import torch
 from torch.autograd import Function
 
 from . import _lib
-from .ops import _check_cuda, _f32c, add_, gemm
+from .ops import _check_cuda, _f32c, add_, gemm, linear_fwd
 
 
 class GramFn(Function):
@@ -116,6 +117,70 @@ class AddFn(Function):
     @staticmethod
     def backward(ctx, g):
         return g, g
+
+
+class PairDiffProjFn(Function):
+    """P = h(z[:B/2]) - h(z[B/2:]) = (z[:B/2] - z[B/2:]) W^T,  z [B, F], W [R, F] -> [B/2, R]       (CIN_loss.py:36-41)
+
+    The bias cancels, so the projection runs once, on the difference: half the GEMM, and TF32 rounds the difference instead
+    of two nearly equal operands (a same-class pair), whose separate rounding would lose most of it.  ``bias`` is an input
+    so that it receives its gradient, which is zero: a parameter that never accumulates one would keep the early-group
+    all-reduce of engine.GradAllReduce from firing."""
+
+    @staticmethod
+    def forward(ctx, z, weight, bias):
+        _check_cuda(z, weight, bias)
+        z, weight = _f32c(z), _f32c(weight)
+        B, F = z.shape
+        d = torch.empty(B // 2, F, device=z.device, dtype=torch.float32)
+        _lib.call('hk_cin_pair_diff_fwd', z, d, B, F, _lib.stream_ptr())
+        ctx.save_for_backward(d, weight)
+        ctx.B = B
+        return linear_fwd(d, weight, None)
+
+    @staticmethod
+    def backward(ctx, dp):
+        d, weight = ctx.saved_tensors
+        dp = _f32c(dp)
+        half, F = d.shape
+        R = weight.shape[0]
+        s = _lib.stream_ptr()
+        dz = dw = db = None
+        if ctx.needs_input_grad[0]:
+            dd = torch.empty_like(d)
+            _lib.call('hk_linear_dgrad', dp, weight, dd, half, F, R, s)
+            dz = torch.empty(ctx.B, F, device=d.device, dtype=torch.float32)
+            _lib.call('hk_cin_pair_diff_bwd', dd, dz, ctx.B, F, s)
+        if ctx.needs_input_grad[1]:
+            dw = torch.empty_like(weight)
+            _lib.call('hk_linear_wgrad', dp, d, dw, None, half, F, R, s)
+        if ctx.needs_input_grad[2]:
+            db = torch.zeros(R, device=d.device, dtype=torch.float32)
+        return dz, dw, db
+
+
+class ContrastiveLossFn(Function):
+    """alpha (L1 + L1^2) over the pairs i with labels[i] == labels[B/2], L1 = sum ||p_i + 1e-6||^2; p [B/2, R], labels [B].
+    Forward and gradient in one hk_cin_contrastive_loss launch (CIN_loss.py:36-46)."""
+
+    @staticmethod
+    def forward(ctx, p, labels, alpha):
+        _check_cuda(p, labels)
+        p = _f32c(p)
+        labels = labels.contiguous().to(torch.int64)
+        B = labels.numel()
+        if B % 2 or p.shape[0] != B // 2:
+            raise _lib.HawkeyeLibError(f'CIN contrastive loss: {B} labels for {p.shape[0]} pairs (the batch must be even)')
+        loss = torch.empty(1, device=p.device, dtype=torch.float32)
+        dp = torch.empty_like(p)
+        _lib.call('hk_cin_contrastive_loss', p, labels, loss, dp, B, p.shape[1], float(alpha), _lib.stream_ptr())
+        ctx.save_for_backward(dp)
+        return loss[0]
+
+    @staticmethod
+    def backward(ctx, g):
+        (dp,) = ctx.saved_tensors
+        return dp * g, None, None
 
 
 class SEGateFn(Function):

@@ -446,13 +446,19 @@ class Trainer:
     def save_checkpoint(self):
         os.makedirs(self.log_root, exist_ok=True)
         path = os.path.join(self.log_root, f'checkpoint_epoch_{self.epoch}.pth')
-        torch.save({'epoch': self.epoch,
-                    'model': {k: v.detach().cpu().clone() for k, v in self.model.state_dict().items()},
-                    'optimizer': self.optimizer.state_dict(), 'scheduler': self.scheduler.state_dict()}, path)
+        torch.save(self.checkpoint_state(), path)
         return path
 
+    def checkpoint_state(self):
+        """-> the dict save_checkpoint writes; a trainer with trained state outside the model adds its own keys."""
+        return {'epoch': self.epoch, 'model': {k: v.detach().cpu().clone() for k, v in self.model.state_dict().items()},
+                'optimizer': self.optimizer.state_dict(), 'scheduler': self.scheduler.state_dict()}
+
     def load_checkpoint(self, path):
-        ck = torch.load(path, map_location='cpu')
+        self.restore_checkpoint(torch.load(path, map_location='cpu'), path)
+
+    def restore_checkpoint(self, ck, path):
+        """Restores the loaded checkpoint ``ck`` (read from ``path``)."""
         self.start_epoch = ck['epoch']
         load_state_dict(self.model, ck['model'])
         opt = ck.get('optimizer', {})

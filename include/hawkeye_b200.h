@@ -209,6 +209,16 @@ int hk_cci_weight_bwd(const float* w_sci, const float* weight, const float* d_cc
                       long long per, void* stream);
 int hk_row_mean_fwd(const float* x, float* y, long long rows, int cols, int ld, void* stream);
 int hk_row_mean_bwd(const float* dy, float* dx, long long rows, int cols, int ld, void* stream);
+/* ---- CIN's contrastive loss: model/loss/CIN_loss.py:26-46 ----------------------------------------------------------------
+ * hk_cin_pair_diff_fwd: d [B/2, per] = z[:B/2] - z[B/2:] of z [B, per] (the bias of h cancels in h(a) - h(b), so the projection
+ * runs once, on the difference, through hk_linear_*); hk_cin_pair_diff_bwd: dz = [dd; -dd].
+ * hk_cin_contrastive_loss: p [B/2, R] projected differences, labels [B] int64 -> loss[0] = alpha (L1 + L1^2) with
+ * L1 = sum_{i : labels[i] == labels[B/2]} ||p_i + 1e-6||^2, and dp [B/2, R] = alpha (1 + 2 L1) 2 (p_i + 1e-6) on those rows, 0 on
+ * the others.  One launch, no read-back.  B even. */
+int hk_cin_pair_diff_fwd(const float* z, float* d, int B, long long per, void* stream);
+int hk_cin_pair_diff_bwd(const float* dd, float* dz, int B, long long per, void* stream);
+int hk_cin_contrastive_loss(const float* p, const long long* labels, float* loss, float* dp, int B, int R, float alpha,
+                            void* stream);
 
 /* ---- OSME excitation: s = sigmoid(m)[n,c] * x[n,c,:] and its backward; the
  * squeeze (AdaptiveAvgPool2d) is hk_row_mean_*, the two Linear layers are hk_linear_*, ReLU on the bottleneck hk_act_* */
