@@ -1,8 +1,9 @@
 """Trainer subclasses of the hot-path methods with the reference's Examples/ surface:
 ``python -m hawkeye_b200.examples {BCNN,CBCNN,MPN,PeerLearning,OSMENet,APINet,DCL,ProtoTreeNet,InterpPartsNet,NTSNet,APCNN,MGE_CNN,
-CIN}
+CIN,Baseline,PairConfusion}
 --config <yaml>`` replaces
 ``python Examples/<Method>.py --config <yaml>`` (same yaml files; one process per GPU under torchrun instead of nn.DataParallel).
+Baseline and PairConfusion train the plain ResNet-50 classifier (configs/Baseline.yaml, configs/PC_resnet50.yaml).
 
 Only what the reference's Examples override is overridden here: which parameters train, with which learning rates, and
 which LR schedule — the step itself is ``Trainer.batch_training``.
@@ -497,13 +498,73 @@ class CINTrainer(Trainer):
                                 'initialisation', path)
 
 
+class BaselineTrainer(Trainer):
+    """Examples/Baseline.py: the plain classifier (ResNet50 in configs/Baseline.yaml) with RandomResizedCrop(224) and a flip
+    for training, Resize(256) and CenterCrop(224) for validation.  Everything else is the base Trainer's, which is what the
+    reference's Example restates: cross-entropy with label smoothing 0.1, Adam over all parameters with the yaml's lr and
+    weight_decay, and CosineAnnealingLR(T_max, eta_min) stepped once per epoch.  The step has no host synchronisation, so
+    ``cuda_graph: true`` captures and replays it."""
+
+    def get_transformers(self, config):
+        """Examples/Baseline.py:13-27 (fixed sizes: the reference does not read the transformer config)."""
+        from torchvision import transforms
+        norm = transforms.Normalize(mean=(0.485, 0.456, 0.406), std=(0.229, 0.224, 0.225))
+        return {
+            'train': transforms.Compose([transforms.RandomResizedCrop((224, 224)), transforms.RandomHorizontalFlip(),
+                                         transforms.ToTensor(), norm]),
+            'val': transforms.Compose([transforms.Resize(256), transforms.CenterCrop(224), transforms.ToTensor(), norm]),
+        }
+
+
+class PCResNetTrainer(Trainer):
+    """Examples/PairConfusion.py: criterion = PairwiseConfusionLoss (cross-entropy + lambda_a x the Euclidean confusion of
+    the pairs (i, B/2 + i)); Adam with weight_decay in two groups, ``fc`` at lr and every other parameter at 0.1 x lr;
+    LinearLR(lr_warmup_decay, warmup_epochs) into CosineAnnealingLR(T_max - warmup_epochs), stepped once per epoch.  The
+    base Trainer's transforms, as in the reference.  ``fc`` is listed last so that its gradient, the first one backward
+    produces, is all-reduced while the trunk's is still being computed.  The step has no host synchronisation, so
+    ``cuda_graph: true`` captures and replays it.
+
+    Under torchrun each rank pairs the two halves of its own batch of B / world images.  Its loss is lambda / (B / world)
+    times a sum over B / (2 world) pairs, and the gradient all-reduce averages the ranks, so the objective is the
+    reference's: lambda / B times a sum over B / 2 random pairs.  Only which random images get paired differs.  A rank's
+    batch must therefore be even: batch_size / world must be even (a ValueError otherwise, when the loaders are built), and
+    each rank's training loader drops its final partial batch, which could be odd.  On one GPU the loaders are the base
+    Trainer's and an odd final batch raises in the criterion, as in the reference."""
+
+    def get_dataloader(self, config):
+        loaders = super().get_dataloader(config)
+        if self.world > 1:
+            if (config.batch_size // self.world) % 2:
+                raise ValueError(f'PCResNetTrainer: dataset.batch_size={config.batch_size} over {self.world} ranks gives '
+                                 f'{config.batch_size // self.world} images per rank, which must be even (the criterion '
+                                 'pairs the two halves of each rank\'s batch)')
+            from torch.utils.data import DataLoader
+            t = loaders['train']
+            loaders['train'] = DataLoader(t.dataset, t.batch_size, num_workers=t.num_workers, pin_memory=t.pin_memory,
+                                          sampler=t.sampler, collate_fn=t.collate_fn, drop_last=True)
+        return loaders
+
+    def get_criterion(self, config):
+        from .losses import PairwiseConfusionLoss
+        return PairwiseConfusionLoss(config)
+
+    def param_groups(self):
+        m = self.get_model_module()
+        fc = {id(p) for p in m.fc.parameters()}
+        return [([p for p in m.parameters() if id(p) not in fc], 0.1), (list(m.fc.parameters()), 1.0)]
+
+    def get_scheduler(self, config):
+        return _warmup_cosine(self.optimizer, config, self.total_epoch)
+
+
 TRAINERS = {'BCNN': BCNNTrainer, 'CBCNN': CBCNNTrainer, 'MPN': MPNTrainer, 'PeerLearning': PeerLearningTrainer,
             'OSMENet': OSMENetTrainer}
 # TRAINERS keeps the key set it has always had, so code that enumerates it sees no change; the command line dispatches
-# over every method, APINet, DCL, ProtoTreeNet, InterpPartsNet, NTSNet, APCNN, MGE_CNN and CIN included.
+# over every method, APINet, DCL, ProtoTreeNet, InterpPartsNet, NTSNet, APCNN, MGE_CNN, CIN, Baseline and PairConfusion
+# included.
 ALL_TRAINERS = dict(TRAINERS, APINet=APINetTrainer, DCL=DCLTrainer, ProtoTreeNet=ProtoTreeTrainer,
                    InterpPartsNet=InterpPartsNetTrainer, NTSNet=NTSNetTrainer, APCNN=APCNNTrainer, MGE_CNN=MGE_CNNTrainer,
-                   CIN=CINTrainer)
+                   CIN=CINTrainer, Baseline=BaselineTrainer, PairConfusion=PCResNetTrainer)
 
 
 def main(argv=None):

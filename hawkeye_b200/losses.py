@@ -306,6 +306,53 @@ class CINLoss(nn.Module):
         return loss_ce + ContrastiveLossFn.apply(p, target, self.alpha)
 
 
+class PairConfusionFn(Function):
+    """CE_ls(logits, labels) + lambda_a * sum_{i < B/2} [y_i != y_{B/2+i}] ||z_i - z_{B/2+i}|| / B -> (loss, top-1 count),
+    forward and gradient in one hk_pc_loss launch (pair_confusion.py:15-28).  Backward scales the kept gradient."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, smoothing, lambda_a):
+        from . import _lib
+        from .ops import _check_cuda, _f32c
+        _check_cuda(logits, labels)
+        logits = _f32c(logits)
+        labels = labels.contiguous().to(torch.int64)
+        B, K = logits.shape
+        loss = torch.empty(1, device=logits.device, dtype=torch.float32)
+        dlogits = torch.empty_like(logits)
+        correct = torch.empty(1, device=logits.device, dtype=torch.int32)
+        _lib.call('hk_pc_loss', logits, labels, loss, dlogits, correct, B, K, float(smoothing), float(lambda_a), 1.0,
+                  _lib.stream_ptr())
+        ctx.save_for_backward(dlogits)
+        ctx.mark_non_differentiable(correct)
+        return loss[0], correct
+
+    @staticmethod
+    def backward(ctx, g, _g_correct=None):
+        (dlogits,) = ctx.saved_tensors
+        return dlogits * g, None, None, None
+
+
+class PairwiseConfusionLoss(nn.Module):
+    """model/loss/pair_confusion.py: CrossEntropy(label_smoothing=0.1) + lambda_a x the Euclidean confusion of the pairs
+    (i, B/2 + i) with different labels, ||z_i - z_{B/2+i}|| summed and divided by B; ``lambda_a`` from the criterion config,
+    10 by default.  An odd batch raises before any launch, as in the reference.  One hk_pc_loss launch; ``last_correct`` is
+    the top-1 count on the device, so the training step reads nothing back."""
+
+    def __init__(self, config):
+        super().__init__()
+        self.lambda_a = config.lambda_a if 'lambda_a' in config else 10
+        self.label_smoothing = 0.1
+
+    def forward(self, features, labels):
+        if features.shape[0] % 2 != 0:
+            raise ValueError(f'PairwiseConfusionLoss: incorrect batch size {features.shape[0]} (it must be even: the two '
+                             'halves of the batch are paired)')
+        loss, correct = PairConfusionFn.apply(features, labels, self.label_smoothing, self.lambda_a)
+        self.last_correct = correct
+        return loss
+
+
 class InterpPartsLoss(nn.Module):
     """model/loss/InterpParts_loss.py: CrossEntropy(logits) + coeff x ShapingLoss(assign) on the (logits, att, assign)
     triple Interp-Parts returns, with the reference's config keys and defaults (radius 2, std 0.4, num_parts 5, alpha 1,

@@ -11,3 +11,4 @@ from .interp_parts import IP_ResNet50, IP_ResNet101  # noqa: F401
 from .nts import NTSNet  # noqa: F401
 from .apcnn import APCNN  # noqa: F401
 from .mge import MGE_CNN  # noqa: F401
+from .resnet import ResNet50, ResNet101  # noqa: F401

@@ -528,6 +528,16 @@ int hk_linear_wgrad(const float* dy, const float* x, float* dw, float* db, int B
 int hk_softmax_ce_ls(const float* logits, const long long* labels, float* loss, float* dlogits, int* correct, int B,
                      int K, float label_smoothing, float grad_scale, void* stream);
 
+/* ---- Pairwise Confusion: model/loss/pair_confusion.py (PairwiseConfusionLoss) ------------------------------------------
+ * logits [B, K], labels int64 [B], B even.  loss[0] = CE_ls(z, y) + lambda_a * sum_{i < B/2} [y_i != y_{B/2+i}] ||d_i|| / B,
+ * d_i = z_i - z_{B/2+i}; dlogits = (softmax - target) * grad_scale / B plus, on a pair with differing labels and
+ * ||d_i|| > 0, +-(lambda_a / B) d_i / ||d_i|| * grad_scale on rows i and B/2+i (0 when ||d_i|| = 0, as torch's norm
+ * backward gives); correct[0] = top-1 hits over the B rows, as hk_softmax_ce_ls counts them.  dlogits is rounded to tf32
+ * once, in the default precision mode.  One launch, one block, fixed-order sums: the same bits on every run.
+ * HK_ERR_ARG on a null pointer, B odd or below 2, or K <= 0. */
+int hk_pc_loss(const float* logits, const long long* labels, float* loss, float* dlogits, int* correct, int B, int K,
+               float label_smoothing, float lambda_a, float grad_scale, void* stream);
+
 /* ---- input side: transforms.ToTensor + Normalize (dataset/transforms.py:14-19, test.py:80-85) fused on
  * the GPU: uint8 HWC batch [N,H,W,3] -> fp32 NCHW (x/255 - mean_c)/std_c; a quarter of the float pipeline's H2D bytes */
 int hk_normalize_u8(const unsigned char* x_nhwc, float* y_nchw, int N, int H, int W, float mean0, float mean1, float mean2,
