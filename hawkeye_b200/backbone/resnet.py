@@ -38,13 +38,17 @@ def _make_layer(inplanes, planes, blocks, stride):
     return nn.Sequential(*layers)
 
 
-def _resnet_modules(layers):
-    """conv1, bn1, relu, maxpool and one stage of ``layers[i]`` blocks per entry, created in torchvision's order."""
+def _resnet_modules(layers, on_layer=None):
+    """conv1, bn1, relu, maxpool and one stage of ``layers[i]`` blocks per entry, created in torchvision's order.
+    ``on_layer(i, layer)``, when given, runs as soon as stage i is built, before the next one is created (modules it adds
+    draw their initial values in that place of the RNG sequence)."""
     mods = [nn.Conv2d(3, 64, kernel_size=7, stride=2, padding=3, bias=False), nn.BatchNorm2d(64), nn.ReLU(inplace=True),
             nn.MaxPool2d(kernel_size=3, stride=2, padding=1)]
     inplanes = 64
-    for planes, n, stride in zip((64, 128, 256, 512), layers, (1, 2, 2, 2)):
+    for i, (planes, n, stride) in enumerate(zip((64, 128, 256, 512), layers, (1, 2, 2, 2))):
         mods.append(_make_layer(inplanes, planes, n, stride))
+        if on_layer is not None:
+            on_layer(i, mods[-1])
         inplanes = planes * 4
     return mods
 
@@ -53,9 +57,9 @@ class ResNetBody(nn.Module):
     """conv1, bn1, relu, maxpool, layer1..layer{len(layers)} under torchvision's attribute names: the base of the methods'
     ResNets, which register their own modules after these."""
 
-    def __init__(self, layers):
+    def __init__(self, layers, on_layer=None):
         super().__init__()
-        for name, m in zip(RESNET_NAMES, _resnet_modules(layers)):
+        for name, m in zip(RESNET_NAMES, _resnet_modules(layers, on_layer)):
             self.add_module(name, m)
         self.num_layers = len(layers)
 

@@ -1,6 +1,6 @@
 """Trainer subclasses of the hot-path methods with the reference's Examples/ surface:
 ``python -m hawkeye_b200.examples {BCNN,CBCNN,MPN,PeerLearning,OSMENet,APINet,DCL,ProtoTreeNet,InterpPartsNet,NTSNet,APCNN,MGE_CNN,
-CIN,Baseline,PairConfusion}
+CIN,Baseline,PairConfusion,CrossX}
 --config <yaml>`` replaces
 ``python Examples/<Method>.py --config <yaml>`` (same yaml files; one process per GPU under torchrun instead of nn.DataParallel).
 Baseline and PairConfusion train the plain ResNet-50 classifier (configs/Baseline.yaml, configs/PC_resnet50.yaml).
@@ -11,7 +11,7 @@ which LR schedule — the step itself is ``Trainer.batch_training``.
 import os
 import sys
 
-from .train import PeerLearningTrainer, Trainer, _Cosine, _Plateau, _Step, warmup_cosine_args
+from .train import PeerLearningTrainer, Trainer, _Cosine, _MultiStep, _Plateau, _Step, warmup_cosine_args
 
 
 def _warmup_cosine(opt, config, total_epoch):
@@ -557,14 +557,40 @@ class PCResNetTrainer(Trainer):
         return _warmup_cosine(self.optimizer, config, self.total_epoch)
 
 
+class CrossXTrainer(Trainer):
+    """Examples/CrossX.py: criterion = CrossXLoss; SGD over all parameters with the yaml's lr, momentum and weight_decay
+    (the base Trainer's SGD); MultiStepLR(milestones, gamma) stepped once per epoch; Resize((600, 600)), then
+    RandomCrop(448) and a horizontal flip for training or CenterCrop(448) for validation.  Accuracy and validation score
+    xf + xp + xc (``CrossXNet.prediction``).  The step has no host synchronisation, so ``cuda_graph: true`` captures and
+    replays it."""
+
+    def get_transformers(self, config):
+        """Examples/CrossX.py:16-31 (fixed sizes: the reference does not read the transformer config)."""
+        from torchvision import transforms
+        norm = transforms.Normalize([0.485, 0.456, 0.406], [0.229, 0.224, 0.225])
+        return {
+            'train': transforms.Compose([transforms.Resize((600, 600)), transforms.RandomCrop((448, 448)),
+                                         transforms.RandomHorizontalFlip(), transforms.ToTensor(), norm]),
+            'val': transforms.Compose([transforms.Resize((600, 600)), transforms.CenterCrop((448, 448)),
+                                       transforms.ToTensor(), norm]),
+        }
+
+    def get_criterion(self, config):
+        from .losses import CrossXLoss
+        return CrossXLoss(config)
+
+    def get_scheduler(self, config):
+        return _MultiStep(self.optimizer, config.milestones, config.gamma)
+
+
 TRAINERS = {'BCNN': BCNNTrainer, 'CBCNN': CBCNNTrainer, 'MPN': MPNTrainer, 'PeerLearning': PeerLearningTrainer,
             'OSMENet': OSMENetTrainer}
 # TRAINERS keeps the key set it has always had, so code that enumerates it sees no change; the command line dispatches
-# over every method, APINet, DCL, ProtoTreeNet, InterpPartsNet, NTSNet, APCNN, MGE_CNN, CIN, Baseline and PairConfusion
-# included.
+# over every method, APINet, DCL, ProtoTreeNet, InterpPartsNet, NTSNet, APCNN, MGE_CNN, CIN, Baseline, PairConfusion and
+# CrossX included.
 ALL_TRAINERS = dict(TRAINERS, APINet=APINetTrainer, DCL=DCLTrainer, ProtoTreeNet=ProtoTreeTrainer,
                    InterpPartsNet=InterpPartsNetTrainer, NTSNet=NTSNetTrainer, APCNN=APCNNTrainer, MGE_CNN=MGE_CNNTrainer,
-                   CIN=CINTrainer, Baseline=BaselineTrainer, PairConfusion=PCResNetTrainer)
+                   CIN=CINTrainer, Baseline=BaselineTrainer, PairConfusion=PCResNetTrainer, CrossX=CrossXTrainer)
 
 
 def main(argv=None):

@@ -353,6 +353,56 @@ class PairwiseConfusionLoss(nn.Module):
         return loss
 
 
+def _parts_npc(feats):
+    """A list of P part features [N, C, 1, 1] -> [N, P, C]: the tensor they are views of when CrossX's forward made them,
+    a stacked copy otherwise."""
+    base = feats[0]._base
+    N, C = feats[0].shape[:2]
+    if (base is not None and base.shape == (N, len(feats), C) and base.is_contiguous()
+            and all(f._base is base and f.data_ptr() == base.data_ptr() + i * C * base.element_size()
+                    for i, f in enumerate(feats))):
+        return base
+    return torch.stack([f.reshape(N, C) for f in feats], 1)
+
+
+class CrossXLoss(nn.Module):
+    """model/loss/CrossX_loss.py: with ``num_parts`` P > 1, CE(label_smoothing=0.1) of xf + xp + xc, plus
+    KL(softmax xf || softmax xp) / N and KL(softmax xf || softmax xc) / N (the target softmax xf is not detached), plus
+    gamma_g sum(triu(corr_g)) of each pooled part feature (ulti, plty, cmbn), corr_g[i, j] = the batch mean of the Gram of
+    the L2-normalised rows, 1 - corr on the diagonal; ``gamma`` from the config.  With P = 1 it is the cross-entropy of the
+    logits.  Two launches (hk_crossx_reg_sums, hk_crossx_loss) with no host read-back, where the reference copies every
+    correlation entry to the host; ``last_correct`` is the top-1 count of xf + xp + xc on the device.  The caller's feature
+    lists are not modified.  Two cases differ from the reference, where it gives NaN: an all-zero feature row contributes 0
+    with a zero gradient, and a class where softmax(xf) underflows to 0 adds 0 to the KL terms and to the gradient of xf
+    (the reference's gradient through its target is log 0 there).
+
+    Under torchrun each rank sums its normalised rows and the sums are all-reduced between the two launches, so the
+    regularisers are those of the global batch, as under nn.DataParallel; their gradient is scaled by the number of ranks,
+    which the optimizer's gradient average divides out."""
+
+    def __init__(self, config):
+        super().__init__()
+        self.num_parts = config.num_parts
+        self.gamma = [float(g) for g in config.gamma]
+        self.label_smoothing = 0.1
+        self.world, self.reduce_s = 1, None
+        import torch.distributed as dist
+        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+            self.world, self.reduce_s = dist.get_world_size(), dist.all_reduce
+
+    def forward(self, outputs, target):
+        from .ops import CrossEntropyLSFn
+        if self.num_parts == 1:
+            loss, correct = CrossEntropyLSFn.apply(outputs, target, self.label_smoothing)
+        else:
+            from .ops_crossx import CrossXLossFn
+            xf, xp, xc, fu, fp, fc = outputs
+            loss, correct = CrossXLossFn.apply(xf, xp, xc, _parts_npc(fu), _parts_npc(fp), _parts_npc(fc), target,
+                                               self.label_smoothing, self.gamma, self.world, self.reduce_s)
+        self.last_correct = correct
+        return loss
+
+
 class InterpPartsLoss(nn.Module):
     """model/loss/InterpParts_loss.py: CrossEntropy(logits) + coeff x ShapingLoss(assign) on the (logits, att, assign)
     triple Interp-Parts returns, with the reference's config keys and defaults (radius 2, std 0.4, num_parts 5, alpha 1,

@@ -572,6 +572,31 @@ class _Step:
         self._apply()
 
 
+class _MultiStep:
+    """MultiStepLR(milestones, gamma) over FusedSGD/FusedAdam param_groups, stepped once per epoch (Examples/CrossX.py:41-42):
+    lr = initial_lr * gamma ** (the number of milestones <= epoch)."""
+
+    def __init__(self, opt, milestones, gamma=0.1):
+        self.opt, self.milestones, self.gamma, self.e = opt, sorted(int(m) for m in milestones), gamma, 0
+        self._apply()
+
+    def _apply(self):
+        k = sum(1 for m in self.milestones if m <= self.e)
+        for g in self.opt.param_groups:
+            g['lr'] = g['initial_lr'] * self.gamma ** k
+
+    def step(self):
+        self.e += 1
+        self._apply()
+
+    def state_dict(self):
+        return dict(e=self.e)
+
+    def load_state_dict(self, sd):
+        self.e = sd['e']
+        self._apply()
+
+
 class _Cosine:
     """LinearLR warm-up -> CosineAnnealingLR (Examples/CBCNN.py:35-45, Examples/MPN.py:20-30; train.py:217-218)."""
 

@@ -42,10 +42,11 @@ def rename_state(state, names):
     return out
 
 
-def load_pretrained(module, env, arch, names):
+def load_pretrained(module, env, arch, names, own=()):
     """torchvision's ``arch`` checkpoint at $``env`` into ``module``, its top-level names mapped by ``names`` (see
     ``rename_state``).  Only the mapped tensors load, so torchvision's ``fc.*`` is ignored unless mapped; a file that lacks
-    any tensor of the mapped modules raises, and so does a shape mismatch.  Without the file the module keeps its own
+    any tensor of the mapped modules raises, and so does a shape mismatch; ``own`` lists substrings of the module's keys
+    that torchvision's checkpoint does not have by design (they keep their initial values).  Without the file the module keeps its own
     (random) initialisation, with a warning unless HAWKEYE_ALLOW_RANDOM_INIT=1 (benchmarks and parity tests).  -> module"""
     path = os.environ.get(env)
     if not (path and os.path.exists(path)):
@@ -56,6 +57,7 @@ def load_pretrained(module, env, arch, names):
                 arch, env, path, env, arch)
         return module
     missing, _ = module.load_state_dict(rename_state(torch.load(path, map_location='cpu'), names), strict=False)
+    missing = [k for k in missing if not any(o in k for o in own)]
     source = {v: k for k, v in names.items()}             # the module's top-level name -> the checkpoint's
     if '' in source:
         lacking = [source[''] + '.' + k for k in missing]

@@ -538,6 +538,47 @@ int hk_softmax_ce_ls(const float* logits, const long long* labels, float* loss, 
 int hk_pc_loss(const float* logits, const long long* labels, float* loss, float* dlogits, int* correct, int B, int K,
                float label_smoothing, float lambda_a, float grad_scale, void* stream);
 
+/* ---- CrossX: model/methods/CrossX.py (MELayer in Bottleneck, the conv2_i / conv3_i fusion), model/loss/CrossX_loss.py ---
+ * Maps NHWC fp32, 16-byte aligned.  Part maps are [N, HW, P, C]: the P parts of a pixel side by side.  P in 1..3.  Every sum
+ * runs in a fixed order, so results are bitwise repeatable.
+ * hk_crossx_me_fwd (Bottleneck.forward with meflag, CrossX.py:110-123): c = bn3 output [N,HW,C], r = residual, m = the
+ *   pre-sigmoid gate logits [N,P,C] -> out = relu(c + r) (optional: null skips it) and part p = relu(c sigmoid(m_p) + r).
+ *   c and r are read once.  C % 128.
+ * hk_crossx_me_bwd: dout (optional) and dparts [N,HW,P,C] -> dc, dr [N,HW,C] and dm [N,P,C] = g (1 - g) sum_hw dpart_p
+ *   [part_p > 0] c, the ReLU masks recomputed from c, r and m.  The squeeze's gradient (mean_hw c feeds the gates) is not
+ *   part of dc.  Workspace: hk_crossx_me_bwd_workspace_bytes.  C % 128.
+ * hk_crossx_fuse_fwd (CrossX.py:211-225, part p): parts = the layer3 parts [N,H,W,P,C], R = conv2_p(layer4 part p)
+ *   [N,H/2,W/2,C] -> S [N,H,W,C] = part_p + nearest-2x(R); pmax [N,P,C] (slice p) = the global max of part_p and pidx the
+ *   pixel h W + w where AdaptiveMaxPool2d(1)'s h-major scan finds it: the first of equal maxima, the last NaN.  H, W even,
+ *   C % 32.
+ * hk_crossx_fuse_bwd: dS, dpmax [N,P,C], pidx -> dparts (slice p) = dS + dpmax at pidx, dR = the 2x2 sums of dS.  C % 4.
+ * hk_crossx_reg_sums (RegularLoss, CrossX_loss.py:13-17): fu [N,P,Cu], fp and fc [N,P,Cp] -> s = (s_u [P,Cu], s_p [P,Cp],
+ *   s_c [P,Cp]) concatenated, s_g[p] = sum_n x[n,p] / ||x[n,p]||.  An all-zero row adds nothing (the reference: NaN).
+ * hk_crossx_loss (CrossXLoss.__call__, :44-64): logits xf, xp, xc [N,K], labels int64 [N], the features and s (summed over
+ *   every rank's batch, n_total images) -> loss[0] = CE_ls(xf + xp + xc) + (KL(xp) + KL(xc)) / N + sum_g gamma_g
+ *   sum(triu(corr_g)), KL(x) = sum q (log q - log_softmax x) with q = softmax xf (which receives gradient),
+ *   corr_g[i,j] = s_i . s_j / n_total^2 with 1 - corr on the diagonal; dxf, dxp, dxc (rounded to tf32 once in the default
+ *   mode) and dfu, dfp, dfc (the regularisers' gradient times reg_scale; zero for an all-zero row); correct[0] = top-1 hits
+ *   of xf + xp + xc.  A class where softmax xf underflows to 0 adds 0 to the KL terms and to dxf (the reference's gradient
+ *   through its target is log 0 there, so its dxf is NaN).  One launch, one block, no host read-back. */
+int hk_crossx_me_fwd(const float* c, const float* r, const float* m, float* out, float* parts, int N, int HW, int P, int C,
+                     void* stream);
+size_t hk_crossx_me_bwd_workspace_bytes(int N, int HW, int P, int C);
+int hk_crossx_me_bwd(const float* c, const float* r, const float* m, const float* dout, const float* dparts, float* dc,
+                     float* dr, float* dm, int N, int HW, int P, int C, void* workspace, size_t workspace_bytes,
+                     void* stream);
+int hk_crossx_fuse_fwd(const float* parts, const float* R, float* S, float* pmax, int* pidx, int N, int H, int W, int P,
+                       int C, int p, void* stream);
+int hk_crossx_fuse_bwd(const float* dS, const float* dpmax, const int* pidx, float* dparts, float* dR, int N, int H, int W,
+                       int P, int C, int p, void* stream);
+int hk_crossx_reg_sums(const float* fu, const float* fp, const float* fc, float* s, int N, int P, int Cu, int Cp,
+                       void* stream);
+int hk_crossx_loss(const float* xf, const float* xp, const float* xc, const long long* labels, const float* fu,
+                   const float* fp, const float* fc, const float* s, float* loss, float* dxf, float* dxp, float* dxc,
+                   float* dfu, float* dfp, float* dfc, int* correct, int N, int K, int P, int Cu, int Cp,
+                   float label_smoothing, float gamma_ulti, float gamma_plty, float gamma_cmbn, int n_total,
+                   float reg_scale, void* stream);
+
 /* ---- input side: transforms.ToTensor + Normalize (dataset/transforms.py:14-19, test.py:80-85) fused on
  * the GPU: uint8 HWC batch [N,H,W,3] -> fp32 NCHW (x/255 - mean_c)/std_c; a quarter of the float pipeline's H2D bytes */
 int hk_normalize_u8(const unsigned char* x_nhwc, float* y_nchw, int N, int H, int W, float mean0, float mean1, float mean2,
