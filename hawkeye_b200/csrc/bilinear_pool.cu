@@ -62,12 +62,31 @@ __global__ void colsum_partial_kernel(const float* __restrict__ X, float* __rest
   }
 }
 
+static inline int pad4(int v) { return (v + 3) & ~3; }
+
+constexpr int COLSUM_SPLITS = 16;
+constexpr int COLSUM_SMEM_MAX = 227 * 1024;   // largest dynamic shared memory a block may opt in to on sm_90
+// bytes of colsum_partial_kernel's row-lane buffer for a (padded) H*W: HW floats once H*W >= 1024, so H*W <= 58112
+static inline size_t colsum_smem(int HW) {
+  const int Q = HW / 4;
+  const int nrl = 256 / Q > 0 ? 256 / Q : 1;
+  return (size_t)nrl * HW * sizeof(float);
+}
+
 // bins[b][(h1[i]+h2[j]) mod d] += s1[i] s2[j] G[b][i][j]
 static int check_gram_shape(const char* op, const float* X, int B, int C, int HW) {
   HK_REQUIRE(X, HK_ERR_ARG, "%s: null input", op);
   HK_REQUIRE(B > 0 && B <= 65535 && C > 0 && HW > 0, HK_ERR_ARG, "%s: bad shape B=%d C=%d HW=%d", op, B, C, HW);
   HK_REQUIRE(C % 128 == 0, HK_ERR_UNSUPPORTED, "%s: C=%d must be a multiple of 128", op, C);
   HK_REQUIRE(aligned16(X), HK_ERR_ALIGN, "%s: input not 16-byte aligned", op);
+  return 0;
+}
+
+// the bilinear entry points also reduce each image's channel sums in shared memory
+static int check_bilinear_shape(const char* op, const float* X, int B, int C, int HW) {
+  if (int r = check_gram_shape(op, X, B, C, HW)) return r;
+  HK_REQUIRE(colsum_smem(pad4(HW)) <= (size_t)COLSUM_SMEM_MAX, HK_ERR_UNSUPPORTED,
+             "%s: H*W=%d above 58112: the channel sums do not fit in shared memory", op, HW);
   return 0;
 }
 
@@ -89,7 +108,6 @@ __global__ void unpad_cols_kernel(const float* __restrict__ xp, float* __restric
     x[i] = xp[r * HWp + c];
   }
 }
-static inline int pad4(int v) { return (v + 3) & ~3; }
 static int launch_pad(const float* x, float* xp, size_t rows, int HW, cudaStream_t st) {
   pad_cols_kernel<<<H100_SMS * 8, 256, 0, st>>>(x, xp, rows, HW, pad4(HW));
   HK_LAUNCH_CHECK("pad_cols_kernel");
@@ -99,13 +117,6 @@ static int launch_unpad(const float* xp, float* x, size_t rows, int HW, cudaStre
   unpad_cols_kernel<<<H100_SMS * 8, 256, 0, st>>>(xp, x, rows, HW, pad4(HW));
   HK_LAUNCH_CHECK("unpad_cols_kernel");
   return 0;
-}
-
-constexpr int COLSUM_SPLITS = 16;
-static inline size_t colsum_smem(int HW) {
-  const int Q = HW / 4;
-  const int nrl = 256 / Q > 0 ? 256 / Q : 1;
-  return (size_t)nrl * HW * sizeof(float);
 }
 
 // per-batch scalars for the bilinear backward epilogue:  alpha = 1/(n HW),  beta = -(c_raw/n^2) / (n HW)
@@ -166,11 +177,12 @@ size_t hk_bilinear_pool_fwd_workspace_bytes(int B, int C, int HW) {
 int hk_bilinear_pool_fwd(const float* x, float* y, float* inv_norm_out, int B, int C, int HW, void* workspace,
                          size_t workspace_bytes, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  int r = check_gram_shape("hk_bilinear_pool_fwd", x, B, C, HW);
+  int r = check_bilinear_shape("hk_bilinear_pool_fwd", x, B, C, HW);
   if (r) return r;
   HK_REQUIRE(y && aligned16(y), HK_ERR_ALIGN, "hk_bilinear_pool_fwd: output null/unaligned");
   HK_REQUIRE(workspace && workspace_bytes >= hk_bilinear_pool_fwd_workspace_bytes(B, C, HW), HK_ERR_WORKSPACE,
              "hk_bilinear_pool_fwd: workspace too small");
+  if ((r = allow_dynamic_smem<colsum_partial_kernel>(COLSUM_SMEM_MAX, "colsum_partial_kernel"))) return r;
   const float inv_hw = 1.f / (float)HW;              // normalisations use the true H*W ...
   const int HWp = pad4(HW);
   float* partial = static_cast<float*>(workspace);
@@ -210,11 +222,12 @@ size_t hk_bilinear_pool_bwd_workspace_bytes(int B, int C, int HW) {
 int hk_bilinear_pool_bwd(const float* x, const float* dy, float* dx, int B, int C, int HW, void* workspace,
                          size_t workspace_bytes, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  int r = check_gram_shape("hk_bilinear_pool_bwd", x, B, C, HW);
+  int r = check_bilinear_shape("hk_bilinear_pool_bwd", x, B, C, HW);
   if (r) return r;
   HK_REQUIRE(dy && dx && aligned16(dy) && aligned16(dx), HK_ERR_ALIGN, "hk_bilinear_pool_bwd: null/unaligned pointer");
   HK_REQUIRE(workspace && workspace_bytes >= hk_bilinear_pool_bwd_workspace_bytes(B, C, HW), HK_ERR_WORKSPACE,
              "hk_bilinear_pool_bwd: workspace too small");
+  if ((r = allow_dynamic_smem<colsum_partial_kernel>(COLSUM_SMEM_MAX, "colsum_partial_kernel"))) return r;
   const float inv_hw = 1.f / (float)HW;
   const int HW_true = HW, HWp = pad4(HW);
   float* S = static_cast<float*>(workspace);
@@ -387,7 +400,7 @@ int hk_cbp_bwd(const float* x, const float* pre, const float* dy, const int* h1,
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   int r = check_gram_shape("hk_cbp_bwd", x, B, C, HW);
   if (r) return r;
-  HK_REQUIRE(pre && dy && dx && h1 && h2 && s1 && s2, HK_ERR_ARG, "hk_cbp_bwd: null pointer");
+  HK_REQUIRE(pre && dy && dx && h1 && h2 && s1 && s2 && d > 0, HK_ERR_ARG, "hk_cbp_bwd: null pointer / bad d");
   HK_REQUIRE(workspace && workspace_bytes >= hk_cbp_bwd_workspace_bytes(B, C, d), HK_ERR_WORKSPACE,
              "hk_cbp_bwd: workspace too small");
   const int HWp = pad4(HW);

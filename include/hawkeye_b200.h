@@ -56,7 +56,8 @@ int hk_gemm_3xtf32(const float* A, int a_mn_major, long long lda, long long stri
 /* ---- BCNN bilinear pooling: model/methods/BCNN.py:13-27 (BilinearPooling.forward) ----------------
  * x [B,C,HW] (NCHW feature map viewed as in BCNN.py:17) -> y [B,C*C] = normalize(sqrt(x x^T/HW + 1e-5)).
  * inv_norm_out (optional, [B]) receives 1/||z||.  Requires C%128==0.  H*W need not be a multiple of 4 (7x7 maps of 224x224
- * inputs): the workspace then also holds a zero-padded copy of x (TMA needs a 16-byte row pitch). */
+ * inputs): the workspace then also holds a zero-padded copy of x (TMA needs a 16-byte row pitch).  H*W <= 58112 (the
+ * channel sums of one image are reduced in shared memory): forward and backward reject a larger map with -3. */
 size_t hk_bilinear_pool_fwd_workspace_bytes(int B, int C, int HW);
 int hk_bilinear_pool_fwd(const float* x, float* y, float* inv_norm_out, int B, int C, int HW, void* workspace,
                          size_t workspace_bytes, void* stream);

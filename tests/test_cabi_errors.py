@@ -44,6 +44,43 @@ def test_bilinear_pool_argument_errors(lib):
     assert b(FAKE, FAKE, FAKE, 2, 512, 196, FAKE, 16, None) == -4
 
 
+def test_pooling_head_errors_launch_nothing(lib):
+    """hk_bilinear_pool_fwd/bwd reject a map whose channel sums exceed shared memory (H*W > 58112, and not 58112 itself),
+    and hk_cbp_fwd/bwd reject C % 128, a null pointer, d <= 0 and a short workspace, before anything is launched, in both
+    precision modes."""
+    f, b = lib.hk_bilinear_pool_fwd, lib.hk_bilinear_pool_bwd
+    cf, cb = lib.hk_cbp_fwd, lib.hk_cbp_bwd
+    cbq = lib.hk_cbp_bwd_workspace_bytes
+
+    def cbp_bwd(x=FAKE, dx=FAKE, C=512, HW=196, d=8192, ws=1 << 30):
+        return cb(x, FAKE, FAKE, FAKE, FAKE, FAKE, FAKE, dx, 2, C, HW, d, FAKE, ws, None)
+
+    for precise in (0, 1):
+        lib.hk_set_precise(precise)
+        lib.hk_reset_launch_count()
+        try:
+            for hw in (58113, 241 * 242):
+                assert f(FAKE, FAKE, None, 2, 128, hw, FAKE, 1 << 40, None) == -3 and '58112' in err(lib)
+                assert b(FAKE, FAKE, FAKE, 2, 128, hw, FAKE, 1 << 40, None) == -3 and '58112' in err(lib)
+            for hw in (58112, 58110):        # the largest maps still pass the shape checks (a 16-byte workspace does not)
+                assert f(FAKE, FAKE, None, 2, 128, hw, FAKE, 16, None) == -4 and 'workspace' in err(lib)
+                assert b(FAKE, FAKE, FAKE, 2, 128, hw, FAKE, 16, None) == -4 and 'workspace' in err(lib)
+            assert cf(FAKE, FAKE, FAKE, FAKE, FAKE, FAKE, FAKE, 2, 100, 196, 8192, None) == -3 and 'multiple of 128' in err(lib)
+            assert cf(FAKE, FAKE, FAKE, FAKE, FAKE, None, FAKE, 2, 512, 196, 8192, None) == -1 and 'null' in err(lib)
+            assert cf(None, FAKE, FAKE, FAKE, FAKE, FAKE, FAKE, 2, 512, 196, 8192, None) == -1 and 'null' in err(lib)
+            assert cf(FAKE, FAKE, FAKE, FAKE, FAKE, FAKE, FAKE, 2, 512, 196, 0, None) == -1 and 'bad d' in err(lib)
+            assert cbp_bwd(C=100) == -3 and 'multiple of 128' in err(lib)
+            assert cbp_bwd(dx=None) == -1 and 'null' in err(lib)
+            assert cbp_bwd(x=None) == -1 and 'null' in err(lib)
+            for d in (0, -8192):
+                assert cbp_bwd(d=d) == -1 and 'bad d' in err(lib)
+            assert cbp_bwd(ws=cbq(2, 512, 8192) - 4) == -4 and 'workspace' in err(lib)
+            assert cbp_bwd(HW=49, ws=cbq(2, 512, 8192) - 4) == -4 and 'workspace' in err(lib)
+            assert lib.hk_launch_count() == 0
+        finally:
+            lib.hk_set_precise(0)
+
+
 def test_conv_argument_errors(lib):
     assert lib.hk_conv3x3_fwd(None, FAKE, None, FAKE, 2, 8, 8, 64, 64, 1, None) == -1
     assert lib.hk_conv3x3_fwd(FAKE, FAKE, None, FAKE, 2, 8, 8, 48, 64, 1, None) == -3 and 'multiples of 32' in err(lib)

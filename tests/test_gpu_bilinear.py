@@ -85,7 +85,7 @@ def test_baseline_batch_elementwise_vs_oracle():
         assert wf < 1e-3 and wb < 2e-3
 
 
-@pytest.mark.parametrize('shape', [(3, 14, 14), (37, 14, 14), (2, 2, 2), (150, 4, 4)])
+@pytest.mark.parametrize('shape', [(3, 14, 14), (37, 14, 14), (2, 2, 2), (150, 4, 4), (2, 7, 7), (3, 3, 3)])
 def test_bilinear_pool_shapes(shape):
     """hk_bilinear_pool_fwd (closed-form norm + Gram with the sqrt / L2-normalise epilogue) across batch sizes below and past
     one wave of GEMM tiles and tiny maps whose H*W is padded to a multiple of 4, per image against the fp64 oracle."""
