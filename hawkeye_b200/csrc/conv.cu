@@ -1060,6 +1060,160 @@ __global__ void pack_first_weights_kernel(const float* __restrict__ w, const flo
   w27[i] = round ? tf32_round(t) : t;
 }
 
+// tf32(x[n][ci][h + kh - 1][w + kw - 1]) for X27 column j = 9 ci + 3 kh + kw < 27 (zero padding), 1.0 for j = 27, 0 after:
+// the row of X27 that im2col_first_kernel writes, rebuilt where it is consumed.
+__device__ __forceinline__ float x27_value(const float* __restrict__ x, int n, int hq, int wq, int j, int H, int W) {
+  if (j >= 27) return j == 27 ? 1.f : 0.f;
+  const int ci = j / 9, hh = hq + (j % 9) / 3 - 1, ww = wq + j % 3 - 1;
+  return (hh >= 0 && hh < H && ww >= 0 && ww < W) ? tf32_round(__ldg(x + (((size_t)n * 3 + ci) * H + hh) * W + ww)) : 0.f;
+}
+
+// First-layer forward without X27 in memory: y = tf32(relu(X27 . W27^T)) for Cout = 64.  One warpgroup per 128 pixels:
+// each thread writes its pixel's X27 row and two W27 rows into 128B-swizzled K-major tiles, then the warpgroup issues
+// the same four m64n64k8 k-steps per 64 rows as the GEMM of hk_conv3x3_first_fwd, so y is bit-identical to it.
+constexpr int FIRST_FWD_PIX = 128;
+constexpr int FIRST_FWD_SMEM = 1024 + FIRST_FWD_PIX * 128 + 64 * 128;
+__global__ void __launch_bounds__(128) first_fwd_direct_kernel(const float* __restrict__ x, const float* __restrict__ w,
+                                                               const float* __restrict__ bias, float* __restrict__ y,
+                                                               int N, int H, int W) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* sA = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sB = sA + FIRST_FWD_PIX * 128;
+  const int t = threadIdx.x;
+  const long long P = (long long)N * H * W, p0 = (long long)blockIdx.x * FIRST_FWD_PIX;
+  {
+    const long long p = p0 + t;
+    float v[32];
+    if (p < P) {
+      const int wq = (int)(p % W), hq = (int)((p / W) % H), n = (int)(p / ((long long)W * H));
+#pragma unroll
+      for (int j = 0; j < 32; ++j) v[j] = x27_value(x, n, hq, wq, j, H, W);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 32; ++j) v[j] = 0.f;
+    }
+#pragma unroll
+    for (int j = 0; j < 32; j += 4)
+      *reinterpret_cast<float4*>(sA + sw128_off(t, j)) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+    // W27 (pack_first_weights_kernel's layout): thread t fills columns 16 (t & 1) .. + 15 of row t / 2
+    const int co = t >> 1, c0 = (t & 1) * 16;
+#pragma unroll
+    for (int j = 0; j < 16; j += 4) {
+      float4 q;
+      float* qq = reinterpret_cast<float*>(&q);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int r = c0 + j + e;
+        qq[e] = tf32_round(r < 27 ? __ldg(w + co * 27 + r) : (r == 27 && bias ? __ldg(bias + co) : 0.f));
+      }
+      *reinterpret_cast<float4*>(sB + sw128_off(co, c0 + j)) = q;
+    }
+  }
+  fence_proxy_async();
+  __syncthreads();
+  const uint64_t b_base = make_sdesc(smem_u32(sB));
+  float acc[2][32];
+#pragma unroll
+  for (int m = 0; m < 2; ++m)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[m][i] = 0.f;
+  wgmma_fence();
+#pragma unroll
+  for (int m = 0; m < 2; ++m) {
+    const uint64_t a_base = make_sdesc(smem_u32(sA + m * 64 * 128));
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) wgmma_tf32(acc[m], a_base + ks * 2, b_base + ks * 2, 1);
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_keep(acc[0]);
+  wgmma_keep(acc[1]);
+  // fragment (row 16 warp + lane / 4 (+8), columns 8 i + 2 (lane % 4) (+1)): four lanes fill one 32-byte sector
+  const int warp = t >> 5, lane = t & 31;
+#pragma unroll
+  for (int m = 0; m < 2; ++m)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const long long p = p0 + m * 64 + warp * 16 + (lane >> 2) + 8 * h;
+      if (p >= P) continue;
+      float* dst = y + p * 64 + 2 * (lane & 3);
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+        *reinterpret_cast<float2*>(dst + 8 * i) =
+            make_float2(tf32_round(fmaxf(acc[m][4 * i + 2 * h], 0.f)), tf32_round(fmaxf(acc[m][4 * i + 2 * h + 1], 0.f)));
+    }
+}
+
+// First-layer weight and bias gradient without X27 in memory, Cout = 64: part[cta] = dY^T . X27 over the pixels of the
+// CTA, on register-A m64n32k8 wgmma.  Each warpgroup takes 32-pixel blocks in turn: A = dY^T read straight from the NHWC
+// dY into the fragment layout (four lanes read one 32-byte sector), B = the block's X27 rebuilt from the image as a
+// [32 column][32 pixel] K-major tile.  The two warpgroups' sums meet in shared memory; sum_splits reduces the CTAs.
+constexpr int FIRST_WG_THREADS = 256;
+constexpr int FIRST_WG_SMEM = 1024 + 64 * 33 * 4;     // two 4 KB B tiles, then the [64][33] reduction tile
+__global__ void __launch_bounds__(FIRST_WG_THREADS, 2) first_wgrad_direct_kernel(const float* __restrict__ x,
+                                                                              const float* __restrict__ dy,
+                                                                              float* __restrict__ part, int N, int H, int W) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
+  uint8_t* sB = smem + wg * 32 * 128;
+  const int P = N * H * W, nblk = (P + 31) / 32;     // P < 2^31 (checked by the entry)
+  const uint64_t b_base = make_sdesc(smem_u32(sB));
+  float acc[16];
+#pragma unroll
+  for (int i = 0; i < 16; ++i) acc[i] = 0.f;
+  const int co = warp * 16 + (lane >> 2);
+  for (int blk = blockIdx.x * 2 + wg; blk < nblk; blk += gridDim.x * 2) {
+    const int pb = blk * 32;
+    uint32_t a[4][4];
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int p = pb + 8 * ks + (lane & 3) + 4 * (e >> 1);
+        a[ks][e] = p < P ? __float_as_uint(__ldg(dy + (size_t)p * 64 + co + 8 * (e & 1))) : 0u;
+      }
+    float v[8];
+    {
+      const int p = pb + lane;
+      if (p < P) {
+        const int wq = p % W, hq = (p / W) % H, n = p / (W * H);
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) v[jj] = x27_value(x, n, hq, wq, warp * 8 + jj, H, W);
+      } else {
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) v[jj] = 0.f;
+      }
+    }
+    named_bar(1 + wg, 128);     // the previous block's wgmma has completed in every warp: sB may be overwritten
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) *reinterpret_cast<float*>(sB + sw128_off(warp * 8 + jj, lane)) = v[jj];
+    fence_proxy_async();
+    named_bar(1 + wg, 128);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) wgmma_tf32(acc, a[ks], b_base + ks * 2);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_keep(acc);
+  }
+  __syncthreads();
+  float* red = reinterpret_cast<float*>(smem);     // [64][33], over the (now idle) B tiles
+  if (wg == 1) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) red[(co + 8 * ((i >> 1) & 1)) * 33 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1)] = acc[i];
+  }
+  __syncthreads();
+  if (wg == 0) {
+    float* dst = part + (size_t)blockIdx.x * 64 * 32;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const int r = co + 8 * ((i >> 1) & 1), c = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+      dst[r * 32 + c] = acc[i] + red[r * 33 + c];
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // MaxPool2d(2,2) (vgg.py:59) on NHWC; optional NCHW output for the last pool (feeds the pooling head)
 // ------------------------------------------------------------------------------------------------
@@ -1321,6 +1475,47 @@ int hk_conv3x3_first_wgrad_acc(const float* x27, const float* dy_nhwc, float* dw
   int r = gemm_splitk(dy_nhwc, 1, Cout, x27, 1, 32, Cout, 32, P, S, part, dw, 27, 27, nullptr, accumulate, stream);
   if (r || !db) return r;
   return sum_splits(part + 27, S, (long long)Cout * 32, Cout, 1, 32, db, 1, nullptr, accumulate, stream);
+}
+
+int hk_conv3x3_first_fwd_direct(const float* x_nchw, const float* w, const float* bias, float* y_nhwc, int N, int H, int W,
+                                int Cout, void* stream) {
+  HK_REQUIRE(!precise(), HK_ERR_UNSUPPORTED, "hk_conv3x3_first_fwd_direct: not available in 3xTF32 mode");
+  HK_REQUIRE(x_nchw && w && y_nhwc, HK_ERR_ARG, "hk_conv3x3_first_fwd_direct: null pointer");
+  HK_REQUIRE(Cout == 64, HK_ERR_UNSUPPORTED, "hk_conv3x3_first_fwd_direct: Cout=%d unsupported (64 only)", Cout);
+  HK_REQUIRE(N > 0 && H > 0 && W > 0, HK_ERR_ARG, "hk_conv3x3_first_fwd_direct: empty map");
+  HK_REQUIRE((reinterpret_cast<uintptr_t>(y_nhwc) & 7) == 0, HK_ERR_ALIGN, "hk_conv3x3_first_fwd_direct: y not 8-byte aligned");
+  const long long P = (long long)N * H * W;
+  HK_REQUIRE(P < (1ll << 31), HK_ERR_UNSUPPORTED, "hk_conv3x3_first_fwd_direct: too many pixels");
+  first_fwd_direct_kernel<<<(int)((P + FIRST_FWD_PIX - 1) / FIRST_FWD_PIX), 128, FIRST_FWD_SMEM, (cudaStream_t)stream>>>(
+      x_nchw, w, bias, y_nhwc, N, H, W);
+  HK_LAUNCH_CHECK("first_fwd_direct_kernel");
+  return 0;
+}
+
+static int first_wgrad_direct_ctas() { return 2 * num_sms(); }   // two CTAs per SM (launch bounds)
+
+size_t hk_conv3x3_first_wgrad_direct_workspace_bytes(void) {
+  return (size_t)first_wgrad_direct_ctas() * 64 * 32 * sizeof(float);
+}
+
+int hk_conv3x3_first_wgrad_direct_acc(const float* x_nchw, const float* dy_nhwc, float* dw, float* db, int N, int H, int W,
+                                      int Cout, void* workspace, size_t workspace_bytes, int accumulate, void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  HK_REQUIRE(!precise(), HK_ERR_UNSUPPORTED, "hk_conv3x3_first_wgrad_direct: not available in 3xTF32 mode");
+  HK_REQUIRE(x_nchw && dy_nhwc && dw, HK_ERR_ARG, "hk_conv3x3_first_wgrad_direct: null pointer");
+  HK_REQUIRE(Cout == 64, HK_ERR_UNSUPPORTED, "hk_conv3x3_first_wgrad_direct: Cout=%d unsupported (64 only)", Cout);
+  HK_REQUIRE(N > 0 && H > 0 && W > 0, HK_ERR_ARG, "hk_conv3x3_first_wgrad_direct: empty map");
+  HK_REQUIRE(workspace && workspace_bytes >= hk_conv3x3_first_wgrad_direct_workspace_bytes(), HK_ERR_WORKSPACE,
+             "hk_conv3x3_first_wgrad_direct: workspace too small");
+  HK_REQUIRE((long long)N * H * W < (1ll << 31), HK_ERR_UNSUPPORTED, "hk_conv3x3_first_wgrad_direct: too many pixels");
+  const int G = first_wgrad_direct_ctas();
+  float* part = static_cast<float*>(workspace);
+  first_wgrad_direct_kernel<<<G, FIRST_WG_THREADS, FIRST_WG_SMEM, stream>>>(x_nchw, dy_nhwc, part, N, H, W);
+  HK_LAUNCH_CHECK("first_wgrad_direct_kernel");
+  // partial columns 0..26 are dw[co][27]; column 27 (the ones column of X27) is db
+  int r = sum_splits(part, G, 64 * 32, 64, 27, 32, dw, 27, nullptr, accumulate, stream);
+  if (r || !db) return r;
+  return sum_splits(part + 27, G, 64 * 32, 64, 1, 32, db, 1, nullptr, accumulate, stream);
 }
 
 int hk_maxpool2x2_fwd(const float* x_nhwc, float* y, int N, int H, int W, int C, int out_nchw, void* stream) {

@@ -472,9 +472,15 @@ class VGGFeaturesFn(Function):
             fused = pool and li > 0 and fuse_ok and H % 2 == 0 and W % 2 == 0
             if li == 0:
                 y = torch.empty(N, H, W, cout, device=dev, dtype=torch.float32)
-                ws0 = _ws(_lib.query('hk_conv3x3_first_fwd_workspace_bytes', N, H, W, cout), dev)
-                _lib.call('hk_conv3x3_first_fwd', x, w, b, y, N, H, W, cout, ws0, ws0.numel(), s)
-                rec['x27'] = ws0 if save else None
+                # single-pass TF32 at 64 channels: the patches are rebuilt from the image by the forward and by the
+                # weight gradient, so no X27 (128 B per pixel) is written or kept; otherwise X27 is shared by both
+                rec['direct'] = fuse_ok and cout == 64
+                if rec['direct']:
+                    _lib.call('hk_conv3x3_first_fwd_direct', x, w, b, y, N, H, W, cout, s)
+                else:
+                    ws0 = _ws(_lib.query('hk_conv3x3_first_fwd_workspace_bytes', N, H, W, cout), dev)
+                    _lib.call('hk_conv3x3_first_fwd', x, w, b, y, N, H, W, cout, ws0, ws0.numel(), s)
+                    rec['x27'] = ws0 if save else None
             else:
                 wf, rec['wd'] = conv3x3_pack(w, save)
                 if not fused:
@@ -528,7 +534,11 @@ class VGGFeaturesFn(Function):
                 dw = torch.empty(pw.shape, device=g.device, dtype=torch.float32)
                 db = torch.empty(cout, device=g.device, dtype=torch.float32)
                 grads[2 * li], grads[2 * li + 1] = dw, db
-            if li == 0:
+            if li == 0 and rec['direct']:
+                ws = _ws(_lib.query('hk_conv3x3_first_wgrad_direct_workspace_bytes'), g.device)
+                _lib.call('hk_conv3x3_first_wgrad_direct_acc', rec['inp'], g, dw, db, N, H, W, cout, ws, ws.numel(),
+                          int(direct), s)
+            elif li == 0:
                 ws = _ws(_lib.query('hk_conv3x3_first_wgrad_workspace_bytes', N, H, W, cout), g.device)
                 _lib.call('hk_conv3x3_first_wgrad_acc', rec['x27'], g, dw, db, N, H, W, cout, ws, ws.numel(), int(direct), s)
             else:

@@ -136,6 +136,14 @@ int hk_conv3x3_first_wgrad(const float* x27, const float* dy_nhwc, float* dw, fl
                            int Cout, void* workspace, size_t workspace_bytes, void* stream);
 int hk_conv3x3_first_wgrad_acc(const float* x27, const float* dy_nhwc, float* dw, float* db, int N, int H, int W,
                                int Cout, void* workspace, size_t workspace_bytes, int accumulate, void* stream);
+/* first layer without X27 in memory (Cout = 64, single-pass TF32 only; HK_ERR_UNSUPPORTED in precise mode): each kernel
+ * rebuilds the patches of its pixels from the NCHW image.  fwd_direct: y bit-identical to hk_conv3x3_first_fwd.
+ * wgrad_direct_acc: dw [64,3,3,3], db [64] (optional) from the image and dy (ReLU-masked); accumulate != 0 adds. */
+int hk_conv3x3_first_fwd_direct(const float* x_nchw, const float* w, const float* bias, float* y_nhwc, int N, int H, int W,
+                                int Cout, void* stream);
+size_t hk_conv3x3_first_wgrad_direct_workspace_bytes(void);
+int hk_conv3x3_first_wgrad_direct_acc(const float* x_nchw, const float* dy_nhwc, float* dw, float* db, int N, int H, int W,
+                                      int Cout, void* workspace, size_t workspace_bytes, int accumulate, void* stream);
 /* MaxPool2d(2,2) on NHWC; out_nchw=1 writes the pooled map as NCHW (input of the pooling heads).
  * bwd routes dy to the first max (PyTorch semantics) and multiplies by (x>0), i.e. also applies the ReLU backward. */
 int hk_maxpool2x2_fwd(const float* x_nhwc, float* y, int N, int H, int W, int C, int out_nchw, void* stream);
