@@ -63,7 +63,7 @@ struct ConvArgs {
   // partners are lane^1, lane^TW, lane^(TW+1); the v2 kernel in its staging tile) and writes the pooled value plus, if
   // code != null, the byte maxpool2x2_bwd_idx reads (bits 0-1 = first maximum in scan order, bit 2 = max > 0).
   float* P;            // [N,H/2,W/2,Cout] (or [N,Cout,H/2,W/2] when pool_nchw)
-  unsigned char* code; // [N,H/2,W/2,Cout] or null
+  unsigned char* code; // [N,H/2,W/2,Cout] or null.  EPI_UNPOOL reads it instead: [N,H,W,Cout], and Y is [N,2H,2W,Cout]
   int pool_nchw;
 };
 
@@ -356,6 +356,33 @@ static int launch_conv(const CUtensorMap& tmX, const CUtensorMap& tmW, const Con
 // ------------------------------------------------------------------------------------------------
 constexpr int CONV_V2_THREADS = 512;
 
+// what the epilogue warpgroup of the stored map does with a finished tile (the fused pooling is selected by ConvArgs::P):
+//   EPI_MAP          store it (bias, ReLU, mask, tf32 rounding).
+//   EPI_UNPOOL       the data gradient of a layer whose input came from a 2x2 max-pool: round to tf32, keep it where the
+//                    pool's byte has bit 2, and store it at window position (code & 3) of the full-resolution map, zeros at
+//                    the other three — what maxpool2x2_bwd_idx_kernel does with the stored map, so the bits are the same
+//                    and the pooled gradient is never written.
+//   EPI_FIRST_WGRAD  the data gradient of VGG conv1_2 (resident 64 -> 64, 16 x 8 tile): mask and round as EPI_MAP, then,
+//                    instead of storing dX, accumulate conv1_1's D[co][j] += sum_px dX[px][co] X27[px][j] on mma.sync from
+//                    the staging tile and the tile's image halo.  Each CTA writes its D to fw.part at the end.
+enum { EPI_MAP = 0, EPI_UNPOOL = 1, EPI_FIRST_WGRAD = 2 };
+// EPI_FIRST_WGRAD image halo of one 16 x 8 tile: 3 channels x (8 + 2) rows x (16 + 2) columns, tf32-rounded, zero padded.
+// Two buffers (the tile being summed and the next one) beside the resident configuration's 226,560 bytes.
+constexpr int FW_HALO = 3 * 10 * 18;
+constexpr int FW_HALO_BYTES = 2 * FW_HALO * 4;
+struct FirstWgradArgs {
+  const float* img;   // the NCHW image conv1_1 read
+  float* part;        // [gridDim.x][64][32] partials of conv1_1's dW^T (column 27: db)
+};
+
+// D (16 x 8, fp32) += A (16 x 8, tf32, row-major) . B (8 x 8, tf32, column-major)
+__device__ __forceinline__ void mma_m16n8k8_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+               "{%0, %1, %2, %3};\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
 template <int BN, bool RESIDENT>
 struct ConvV2Cfg {
   static constexpr int A_BYTES = 160 * 128;                          // 20 KB halo patch
@@ -376,11 +403,12 @@ struct ConvV2Cfg {
 
 // warpgroup 0: TMA producer (one thread); warpgroups 1-2: wgmma on rows 0-63 / 64-127 of the 128-pixel tile; warpgroup 3:
 // the epilogue.  TW = 16: tile 16 x 8 x 1 image, TW = 8: tile 8 x 8 x 2 images.
-template <int BN, bool RESIDENT, int TW>
+template <int BN, bool RESIDENT, int TW, int EPI>
 __global__ void __launch_bounds__(CONV_V2_THREADS, 1)
 conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, ConvArgs a,
-                        int n_ntiles, int total_tiles) {
+                        int n_ntiles, int total_tiles, FirstWgradArgs fw) {
   using Cfg = ConvV2Cfg<BN, RESIDENT>;
+  static_assert(EPI != EPI_FIRST_WGRAD || (BN == 64 && RESIDENT && TW == 16), "conv1_1 weight gradient: 64 -> 64, 16 x 8");
   constexpr int NACC = BN / 2;
   constexpr int TN = 16 / TW;                       // images per tile
   constexpr int WG_ROWS = TW == 16 ? 64 : 80;       // patch rows between the two MMA warpgroups' A operands
@@ -411,7 +439,7 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
   }
   __syncthreads();
 
-  if (warp >= 12 && a.P) {
+  if (warp >= 12 && EPI == EPI_MAP && a.P) {
     // fused pooling: thread r owns pixel r of the tile, the mapping epi_chunk's pooling shuffles rely on.  The staging
     // tile is released as soon as its last chunk has been read.
     const int r = threadIdx.x - 384;
@@ -459,17 +487,53 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
       org = (((size_t)pt * TN * a.H + th * 8) * a.W + tw * TW) * a.Cout;
       return pt * TN + (TW == 16 ? 0 : ew >> 1) < a.N;
     };
+    // pixel-tile coordinates (column, row, first image) of tile t
+    auto tile_pos = [&](int t, int& tw, int& th, int& tn) {
+      int pt = t / n_ntiles;
+      tw = pt % a.tiles_w; pt /= a.tiles_w;
+      th = pt % a.tiles_h; tn = pt / a.tiles_h;
+    };
+    // EPI_UNPOOL: element offset of pixel k's window (top-left) from the full-resolution tile origin, as eoff
+    const int frow = 2 * a.W * a.Cout;
+    const int uoff0 = (TW == 16 ? 2 * (p0 >> 4) * frow + 2 * (p0 & 15) * a.Cout
+                                : ((p0 >> 6) * 2 * a.H + 2 * ((p0 >> 3) & 7)) * frow + 2 * (p0 & 7) * a.Cout) + u4;
+    auto uoff = [&](int k) { return uoff0 + (k / (TW / 4)) * 2 * frow + (k % (TW / 4)) * 8 * a.Cout; };
+    // EPI_FIRST_WGRAD.  mma.sync fragments of warp ew, which owns co 16 ew .. 16 ew + 15 and all 32 X27 columns
+    // (g = lane / 4, tq = lane % 4): A[co][px] = dX[px][co] is read from the staging tile, rows px = 8 ks + tq (+4),
+    // columns 16 ew + g (+8) (the 72-float pitch puts the 32 lanes in 32 banks); B[px][j] = X27[px][j] for column
+    // j = 8 nt + g is halo element hoff[nt] + (px / 16) * 18 + px % 16 (j < 27), 1 for j = 27, 0 after.
+    float* halo = stg + 128 * Cfg::STG_LD;
+    float dacc[4][4] = {};
+    const int lane = e & 31, g = lane >> 2, tq = lane & 3;
+    int hoff[4];
+#pragma unroll
+    for (int nt = 0; nt < 4; ++nt) {
+      const int jj = 8 * nt + g;
+      hoff[nt] = jj < 27 ? (jj / 9) * 180 + (jj % 9 / 3) * 18 + jj % 3 : 0;
+    }
     int co0 = 0, j = 0;
     size_t org = 0;
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++j) {
       const bool valid = tile_org(t, org, co0);
+      if constexpr (EPI == EPI_FIRST_WGRAD) {
+        // this tile's halo, loaded while the MMA warpgroups are still on it.  Buffer j & 1 was last read for tile j - 2,
+        // before every epilogue thread passed tile j - 1's barrier.
+        int tw, th, tn;
+        tile_pos(t, tw, th, tn);
+        float* hb = halo + (j & 1) * FW_HALO;
+        for (int i = e; i < FW_HALO; i += 128) {
+          const int ci = i / 180, hh = th * 8 - 1 + i / 18 % 10, ww = tw * 16 - 1 + i % 18;
+          hb[i] = hh >= 0 && hh < a.H && ww >= 0 && ww < a.W
+                      ? tf32_round(__ldg(fw.img + (((size_t)tn * 3 + ci) * a.H + hh) * a.W + ww)) : 0.f;
+        }
+      }
       mbar_wait(stg_full, j & 1);
 #pragma unroll
       for (int c = 0; c < BN / 32; ++c) {
         float4 v[8];
 #pragma unroll
         for (int k = 0; k < 8; ++k) v[k] = *reinterpret_cast<const float4*>(srow + 4 * k * Cfg::STG_LD + c * 32);
-        if (c == BN / 32 - 1) mbar_arrive(stg_empty);
+        if (EPI != EPI_FIRST_WGRAD && c == BN / 32 - 1) mbar_arrive(stg_empty);
         const int co = co0 + c * 32;
         const bool live = valid && co < a.Cout;
         if (live) {
@@ -495,12 +559,68 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
               v[k].z = mk[k].z > 0.f ? v[k].z : 0.f; v[k].w = mk[k].w > 0.f ? v[k].w : 0.f;
             }
           }
+          if constexpr (EPI == EPI_MAP) {
 #pragma unroll
-          for (int k = 0; k < 8; ++k)
-            __stcs(reinterpret_cast<float4*>(a.Y + org + co + eoff(k)),
-                   make_float4(tf32_round(v[k].x), tf32_round(v[k].y), tf32_round(v[k].z), tf32_round(v[k].w)));
+            for (int k = 0; k < 8; ++k)
+              __stcs(reinterpret_cast<float4*>(a.Y + org + co + eoff(k)),
+                     make_float4(tf32_round(v[k].x), tf32_round(v[k].y), tf32_round(v[k].z), tf32_round(v[k].w)));
+          } else if constexpr (EPI == EPI_UNPOOL) {
+            int tw, th, tn;
+            tile_pos(t, tw, th, tn);
+            float* dst = a.Y + (((size_t)tn * TN * 2 * a.H + th * 16) * 2 * a.W + tw * 2 * TW) * a.Cout + co;
+            // the four codes of a float4 as one word (byte i: channel i)
+            uint32_t cd[8];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) cd[k] = __ldcs(reinterpret_cast<const unsigned int*>(a.code + org + co + eoff(k)));
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+              const float4 q = make_float4((cd[k] & 4u) ? tf32_round(v[k].x) : 0.f, (cd[k] & (4u << 8)) ? tf32_round(v[k].y) : 0.f,
+                                           (cd[k] & (4u << 16)) ? tf32_round(v[k].z) : 0.f,
+                                           (cd[k] & (4u << 24)) ? tf32_round(v[k].w) : 0.f);
+              float* o = dst + uoff(k);
+#pragma unroll
+              for (int pos = 0; pos < 4; ++pos)
+                __stcs(reinterpret_cast<float4*>(o + (pos >> 1) * frow + (pos & 1) * a.Cout),
+                       make_float4((cd[k] & 3u) == (uint32_t)pos ? q.x : 0.f, (cd[k] >> 8 & 3u) == (uint32_t)pos ? q.y : 0.f,
+                                   (cd[k] >> 16 & 3u) == (uint32_t)pos ? q.z : 0.f,
+                                   (cd[k] >> 24 & 3u) == (uint32_t)pos ? q.w : 0.f));
+            }
+          } else {
+            // dX goes back into the staging tile, where the MMAs below read it
+#pragma unroll
+            for (int k = 0; k < 8; ++k)
+              *reinterpret_cast<float4*>(stg + (ew * 32 + sub + 4 * k) * Cfg::STG_LD + u4 + c * 32) =
+                  make_float4(tf32_round(v[k].x), tf32_round(v[k].y), tf32_round(v[k].z), tf32_round(v[k].w));
+          }
         }
       }
+      if constexpr (EPI == EPI_FIRST_WGRAD) {
+        named_bar(1, 128);    // the whole of dX and the halo are in shared memory
+        const float* hb = halo + (j & 1) * FW_HALO;
+        const float* arow = stg + tq * Cfg::STG_LD + 16 * ew + g;
+#pragma unroll 4
+        for (int ks = 0; ks < 16; ++ks) {
+          const float* ap = arow + 8 * ks * Cfg::STG_LD;
+          const uint32_t af[4] = {__float_as_uint(ap[0]), __float_as_uint(ap[8]), __float_as_uint(ap[4 * Cfg::STG_LD]),
+                                  __float_as_uint(ap[4 * Cfg::STG_LD + 8])};
+          const int hp = (ks >> 1) * 18 + 8 * (ks & 1) + tq;    // halo offset of pixel 8 ks + tq
+#pragma unroll
+          for (int nt = 0; nt < 4; ++nt) {
+            float b0 = hb[hoff[nt] + hp], b1 = hb[hoff[nt] + hp + 4];
+            if (nt == 3 && g >= 3) b0 = b1 = g == 3 ? 1.f : 0.f;
+            mma_m16n8k8_tf32(dacc[nt], af, __float_as_uint(b0), __float_as_uint(b1));
+          }
+        }
+        mbar_arrive(stg_empty);
+      }
+    }
+    if constexpr (EPI == EPI_FIRST_WGRAD) {
+      // accumulator i of n-tile nt: co 16 ew + g (+8 for i >= 2), column 8 nt + 2 tq + (i & 1)
+      float* dst = fw.part + (size_t)blockIdx.x * 64 * 32;
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) dst[(16 * ew + g + 8 * (i >> 1)) * 32 + 8 * nt + 2 * tq + (i & 1)] = dacc[nt][i];
     }
   } else if (warp < 4) {
     if (threadIdx.x == 0) {
@@ -590,10 +710,13 @@ conv3x3_igemm_v2_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
   }
 }
 
-template <int BN, bool RESIDENT, int TW>
-static int launch_conv_v2(const float* x, const float* wp, ConvArgs a, int N, int H, int W, cudaStream_t stream) {
+template <int BN, bool RESIDENT, int TW, int EPI = EPI_MAP>
+static int launch_conv_v2(const float* x, const float* wp, ConvArgs a, int N, int H, int W, cudaStream_t stream,
+                          FirstWgradArgs fw = {}) {
   using Cfg = ConvV2Cfg<BN, RESIDENT>;
-  if (int r = allow_dynamic_smem<conv3x3_igemm_v2_kernel<BN, RESIDENT, TW>>(Cfg::SMEM, BN == 64 ? "conv_v2<64>" : "conv_v2<128>"))
+  constexpr int SMEM = Cfg::SMEM + (EPI == EPI_FIRST_WGRAD ? FW_HALO_BYTES : 0);
+  static_assert(SMEM <= 232448, "conv_v2: dynamic shared memory above the sm_90 opt-in limit");
+  if (int r = allow_dynamic_smem<conv3x3_igemm_v2_kernel<BN, RESIDENT, TW, EPI>>(SMEM, BN == 64 ? "conv_v2<64>" : "conv_v2<128>"))
     return r;
   a.TW = TW; a.TH = 8; a.TN = 16 / TW;
   a.tiles_w = W / TW; a.tiles_h = H / 8; a.tiles_n = (N + a.TN - 1) / a.TN;
@@ -618,16 +741,16 @@ static int launch_conv_v2(const float* x, const float* wp, ConvArgs a, int N, in
   }
   const int sms = num_sms();
   const int grid = total < sms ? (int)total : sms;
-  conv3x3_igemm_v2_kernel<BN, RESIDENT, TW><<<grid, CONV_V2_THREADS, Cfg::SMEM, stream>>>(tmX, tmW, a, n_ntiles, (int)total);
+  conv3x3_igemm_v2_kernel<BN, RESIDENT, TW, EPI><<<grid, CONV_V2_THREADS, SMEM, stream>>>(tmX, tmW, a, n_ntiles, (int)total, fw);
   HK_LAUNCH_CHECK("conv3x3_igemm_v2_kernel");
   return 0;
 }
 
-template <int TW>
+template <int TW, int EPI = EPI_MAP>
 static int launch_conv_v2(const float* x, const float* wp, const ConvArgs& a, int N, int H, int W, cudaStream_t stream) {
-  if (a.Cin == 64 && a.Cout == 64) return launch_conv_v2<64, true, TW>(x, wp, a, N, H, W, stream);
-  if (a.Cout <= 64) return launch_conv_v2<64, false, TW>(x, wp, a, N, H, W, stream);
-  return launch_conv_v2<128, false, TW>(x, wp, a, N, H, W, stream);
+  if (a.Cin == 64 && a.Cout == 64) return launch_conv_v2<64, true, TW, EPI>(x, wp, a, N, H, W, stream);
+  if (a.Cout <= 64) return launch_conv_v2<64, false, TW, EPI>(x, wp, a, N, H, W, stream);
+  return launch_conv_v2<128, false, TW, EPI>(x, wp, a, N, H, W, stream);
 }
 
 static int conv3x3_igemm_1x(const float* x, const float* wp, const float* bias, const float* mask, const float* addend,
@@ -1391,6 +1514,58 @@ int hk_conv3x3_dgrad(const float* dy, const float* w_dgrad_packed, const float* 
                      int W, int Cin, int Cout, void* stream) {
   // dgrad is the same implicit GEMM with the roles of Cin/Cout swapped and flipped taps
   return conv3x3_igemm(dy, w_dgrad_packed, nullptr, relu_mask_act, dx, N, H, W, Cout, Cin, 0, (cudaStream_t)stream);
+}
+
+int hk_conv3x3_dgrad_unpool(const float* dy, const float* w_dgrad_packed, const unsigned char* code, float* dx_full, int N,
+                            int H, int W, int Cin, int Cout, void* stream) {
+  HK_REQUIRE(!precise(), HK_ERR_UNSUPPORTED, "hk_conv3x3_dgrad_unpool: not available in 3xTF32 mode");
+  HK_REQUIRE(dy && w_dgrad_packed && code && dx_full, HK_ERR_ARG, "hk_conv3x3_dgrad_unpool: null pointer");
+  HK_REQUIRE(N > 0 && H > 0 && W > 0, HK_ERR_ARG, "hk_conv3x3_dgrad_unpool: empty map");
+  HK_REQUIRE(Cin % 32 == 0 && Cout % 32 == 0, HK_ERR_UNSUPPORTED,
+             "hk_conv3x3_dgrad_unpool: Cin=%d Cout=%d must be multiples of 32", Cin, Cout);
+  HK_REQUIRE(H % 8 == 0 && W % 8 == 0, HK_ERR_UNSUPPORTED, "hk_conv3x3_dgrad_unpool: %dx%d map is not a multiple of 8x8",
+             H, W);
+  // the epilogue keeps full-resolution element offsets inside a tile (up to one image apart) as int
+  HK_REQUIRE(4ll * H * W * Cin < (1ll << 31), HK_ERR_UNSUPPORTED, "hk_conv3x3_dgrad_unpool: map too large");
+  HK_REQUIRE(aligned16(dy) && aligned16(w_dgrad_packed) && aligned16(code) && aligned16(dx_full), HK_ERR_ALIGN,
+             "hk_conv3x3_dgrad_unpool: pointer not 16-byte aligned");
+  ConvArgs a = {};
+  a.Y = dx_full; a.code = const_cast<unsigned char*>(code);
+  a.N = N; a.H = H; a.W = W; a.Cin = Cout; a.Cout = Cin; a.stride = 1;
+  if (W % 16 == 0) return launch_conv_v2<16, EPI_UNPOOL>(dy, w_dgrad_packed, a, N, H, W, (cudaStream_t)stream);
+  return launch_conv_v2<8, EPI_UNPOOL>(dy, w_dgrad_packed, a, N, H, W, (cudaStream_t)stream);
+}
+
+size_t hk_conv3x3_dgrad_first_wgrad_workspace_bytes(void) { return (size_t)num_sms() * 64 * 32 * sizeof(float); }
+
+int hk_conv3x3_dgrad_first_wgrad_acc(const float* dy, const float* w_dgrad_packed, const float* relu_mask_act,
+                                     const float* x_nchw, float* dw1, float* db1, int N, int H, int W, int Cin, int Cout,
+                                     void* workspace, size_t workspace_bytes, int accumulate, void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  HK_REQUIRE(!precise(), HK_ERR_UNSUPPORTED, "hk_conv3x3_dgrad_first_wgrad: not available in 3xTF32 mode");
+  HK_REQUIRE(dy && w_dgrad_packed && x_nchw && dw1, HK_ERR_ARG, "hk_conv3x3_dgrad_first_wgrad: null pointer");
+  HK_REQUIRE(N > 0 && H > 0 && W > 0, HK_ERR_ARG, "hk_conv3x3_dgrad_first_wgrad: empty map");
+  HK_REQUIRE(Cin == 64 && Cout == 64, HK_ERR_UNSUPPORTED, "hk_conv3x3_dgrad_first_wgrad: Cin=%d Cout=%d (64 -> 64 only)",
+             Cin, Cout);
+  HK_REQUIRE(W % 16 == 0 && H % 8 == 0, HK_ERR_UNSUPPORTED,
+             "hk_conv3x3_dgrad_first_wgrad: %dx%d map is not tiled by 16x8", H, W);
+  HK_REQUIRE(aligned16(dy) && aligned16(w_dgrad_packed) && (!relu_mask_act || aligned16(relu_mask_act)), HK_ERR_ALIGN,
+             "hk_conv3x3_dgrad_first_wgrad: pointer not 16-byte aligned");
+  HK_REQUIRE(workspace && workspace_bytes >= hk_conv3x3_dgrad_first_wgrad_workspace_bytes(), HK_ERR_WORKSPACE,
+             "hk_conv3x3_dgrad_first_wgrad: workspace too small");
+  const long long tiles = (long long)(W / 16) * (H / 8) * N;
+  HK_REQUIRE(tiles < (1ll << 31), HK_ERR_UNSUPPORTED, "hk_conv3x3_dgrad_first_wgrad: too many tiles");
+  float* part = static_cast<float*>(workspace);
+  ConvArgs a = {};
+  a.mask = relu_mask_act;
+  a.N = N; a.H = H; a.W = W; a.Cin = Cout; a.Cout = Cin; a.stride = 1;
+  int r = launch_conv_v2<64, true, 16, EPI_FIRST_WGRAD>(dy, w_dgrad_packed, a, N, H, W, stream, FirstWgradArgs{x_nchw, part});
+  if (r) return r;
+  const int G = tiles < num_sms() ? (int)tiles : num_sms();   // launch_conv_v2's grid: one partial per CTA
+  // partial columns 0..26 are dw[co][27]; column 27 (the ones column of X27) is db
+  if ((r = sum_splits(part, G, 64 * 32, 64, 27, 32, dw1, 27, nullptr, accumulate, stream))) return r;
+  if (!db1) return 0;
+  return sum_splits(part + 27, G, 64 * 32, 64, 1, 32, db1, 1, nullptr, accumulate, stream);
 }
 
 size_t hk_conv3x3_wgrad_workspace_bytes(int Cin, int Cout) { return (size_t)9 * Cin * Cout * sizeof(float); }

@@ -516,24 +516,31 @@ class VGGFeaturesFn(Function):
         s = _lib.stream_ptr()
         g = _f32c(dfeat)
         grads = [None] * ctx.nparams
-        for li in reversed(range(len(ctx.layers))):
-            rec, (cout, pool) = ctx.records[li], ctx.layers[li]
-            N, H, W = g.shape[0], rec['H'], rec['W']
-            if pool:
-                dx = torch.empty(N, H, W, cout, device=g.device, dtype=torch.float32)
-                _lib.call('hk_maxpool2x2_bwd_idx', rec['code'], g, dx, N, H, W, cout, int(rec['last']), s)
-                g = dx
+        single_pass = not _lib.get_precise()
+
+        def grad_bufs(li):
             # Accumulate straight into the parameters' .grad buffers when they exist (the Trainer keeps them as views of
             # one flat buffer): same semantics as autograd's own accumulation, without the temporaries and the 26 `add`
             # launches.  Otherwise (first backward, .grad is None) return fresh tensors and let autograd install them.
             pw, pb = ctx.params[2 * li], ctx.params[2 * li + 1]
             direct = _grad_ready(pw) and _grad_ready(pb)
             if direct:
-                dw, db = pw.grad, pb.grad
-            else:
-                dw = torch.empty(pw.shape, device=g.device, dtype=torch.float32)
-                db = torch.empty(cout, device=g.device, dtype=torch.float32)
-                grads[2 * li], grads[2 * li + 1] = dw, db
+                return pw.grad, pb.grad, direct
+            dw = torch.empty(pw.shape, device=g.device, dtype=torch.float32)
+            db = torch.empty(pb.shape, device=g.device, dtype=torch.float32)
+            grads[2 * li], grads[2 * li + 1] = dw, db
+            return dw, db, direct
+
+        unpooled = False     # g is already the gradient of the pool's input (the layer above did the pool's backward)
+        for li in reversed(range(len(ctx.layers))):
+            rec, (cout, pool) = ctx.records[li], ctx.layers[li]
+            N, H, W = g.shape[0], rec['H'], rec['W']
+            if pool and not unpooled:
+                dx = torch.empty(N, H, W, cout, device=g.device, dtype=torch.float32)
+                _lib.call('hk_maxpool2x2_bwd_idx', rec['code'], g, dx, N, H, W, cout, int(rec['last']), s)
+                g = dx
+            unpooled = False
+            dw, db, direct = grad_bufs(li)
             if li == 0 and rec['direct']:
                 ws = _ws(_lib.query('hk_conv3x3_first_wgrad_direct_workspace_bytes'), g.device)
                 _lib.call('hk_conv3x3_first_wgrad_direct_acc', rec['inp'], g, dw, db, N, H, W, cout, ws, ws.numel(),
@@ -543,6 +550,23 @@ class VGGFeaturesFn(Function):
                 _lib.call('hk_conv3x3_first_wgrad_acc', rec['x27'], g, dw, db, N, H, W, cout, ws, ws.numel(), int(direct), s)
             else:
                 conv3x3_wgrad(rec['inp'], g, dw, db, accumulate=direct)
+                cin = rec['inp'].shape[-1]
+                below = ctx.records[li - 1]
+                if li == 1 and below['direct'] and cin == 64 and cout == 64 and W % 16 == 0 and H % 8 == 0:
+                    # conv1_2's data gradient feeds only conv1_1's weight gradient: one kernel computes both, dx1 is
+                    # never written, and layer 0 is done
+                    dw0, db0, direct0 = grad_bufs(0)
+                    ws = _ws(_lib.query('hk_conv3x3_dgrad_first_wgrad_workspace_bytes'), g.device)
+                    _lib.call('hk_conv3x3_dgrad_first_wgrad_acc', g, rec['wd'], rec['inp'], below['inp'], dw0, db0, N, H,
+                              W, cin, cout, ws, ws.numel(), int(direct0), s)
+                    break
+                if (ctx.layers[li - 1][1] and single_pass and H % 8 == 0 and W % 8 == 0 and below['H'] == 2 * H
+                        and below['W'] == 2 * W):
+                    # the input came from a pool: the data gradient goes straight to the pool's input
+                    dx = torch.empty(N, 2 * H, 2 * W, cin, device=g.device, dtype=torch.float32)
+                    _lib.call('hk_conv3x3_dgrad_unpool', g, rec['wd'], below['code'], dx, N, H, W, cin, cout, s)
+                    g, unpooled = dx, True
+                    continue
                 # the input is a ReLU output unless a pool came in between (the pool's code carries that mask)
                 g = conv3x3_dgrad(g, rec['wd'], mask=None if ctx.layers[li - 1][1] else rec['inp'])
         ctx.records = ctx.params = None

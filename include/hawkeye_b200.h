@@ -119,6 +119,23 @@ int hk_conv3x3_s2_fwd(const float* x_nhwc, const float* w_fwd_packed, const floa
 /* dx = conv3x3^T(dy, w) * (relu_mask_act > 0)  (mask optional: the ReLU output that produced x) */
 int hk_conv3x3_dgrad(const float* dy_nhwc, const float* w_dgrad_packed, const float* relu_mask_act, float* dx_nhwc,
                      int N, int H, int W, int Cin, int Cout, void* stream);
+/* hk_conv3x3_dgrad (no mask) followed by hk_maxpool2x2_bwd_idx in ONE kernel: the data gradient of a conv whose input x
+ * [N,H,W,Cin] is the output of a 2x2 max-pool goes straight to the pool's input.  code: the pool's bytes [N,H,W,Cin];
+ * dx_full: [N,2H,2W,Cin], each window holding the gradient at its arg-max (zero where bit 2 is clear) and zeros elsewhere.
+ * The pooled gradient is never written; dx_full is bit-identical to the two-launch sequence.  H % 8 == 0, W % 8 == 0,
+ * Cin % 32 == 0, Cout % 32 == 0, 4*H*W*Cin < 2^31; single-pass TF32 only (HK_ERR_UNSUPPORTED otherwise). */
+int hk_conv3x3_dgrad_unpool(const float* dy_nhwc, const float* w_dgrad_packed, const unsigned char* code, float* dx_full,
+                            int N, int H, int W, int Cin, int Cout, void* stream);
+/* VGG conv1_2's data gradient with conv1_1's weight gradient in its epilogue: dx1 = conv3x3^T(dy, w) * (relu_mask_act > 0)
+ * (relu_mask_act optional: conv1_1's output) is never written; dw1 [64,3,3,3] and db1 [64] (optional) of the 3-channel
+ * layer are computed from it and the NCHW image x_nchw [N,3,H,W], as hk_conv3x3_first_wgrad_direct_acc would from the
+ * stored dx1 (the sums run in another order).  accumulate != 0 adds.  Cin = Cout = 64, W % 16 == 0, H % 8 == 0,
+ * single-pass TF32 only (HK_ERR_UNSUPPORTED otherwise).  Deterministic: per-CTA partials in the workspace, reduced in a
+ * fixed order. */
+size_t hk_conv3x3_dgrad_first_wgrad_workspace_bytes(void);
+int hk_conv3x3_dgrad_first_wgrad_acc(const float* dy_nhwc, const float* w_dgrad_packed, const float* relu_mask_act,
+                                     const float* x_nchw, float* dw1, float* db1, int N, int H, int W, int Cin, int Cout,
+                                     void* workspace, size_t workspace_bytes, int accumulate, void* stream);
 /* dw [Cout,Cin,3,3] (reference layout), db [Cout] (optional) from x, dy (dy already ReLU-masked).  Cin%32==0, W%4==0. */
 size_t hk_conv3x3_wgrad_workspace_bytes(int Cin, int Cout);
 int hk_conv3x3_wgrad(const float* x_nhwc, const float* dy_nhwc, float* dw, float* db, int N, int H, int W, int Cin,
