@@ -52,6 +52,12 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if (++spins > HK_SPIN_LIMIT) __trap();
   }
 }
+// mbar_wait without the watchdog, for loops where a live spin counter would cost registers the caller cannot spare.
+// Another thread of the CTA must mbar_wait on the same phase, so that a phase that never completes still traps.
+__device__ __forceinline__ void mbar_wait_unguarded(uint64_t* bar, uint32_t parity) {
+  while (!mbar_try_wait(bar, parity)) {
+  }
+}
 
 // warp-specialised register budget: the producer warpgroup gives registers back, the MMA warpgroups take them
 template <int N>

@@ -830,20 +830,28 @@ static int conv3x3_igemm_1x(const float* x, const float* wp, const float* bias, 
 //   A = X (M = 64 ci, k = pixel), in registers.  TMA lands the halo patch, (TH+2) x (TW+2) x TN pixels, as two
 //       [pixels][32 ci] boxes (128B-swizzled, zero fill = the conv padding).  Each consumer thread loads its m64k8
 //       fragment straight from there: the kw shift of a tap is a row offset, so X is never transposed or copied.
-//   B = dY^T (N = 64 co, k = pixel), K-major: the producer warp transposes the two [64 px][32 co] dY boxes once
-//       per stage into [co][pixel] (two k-chunks of [64 co][32 px]) and sums the bias gradient on the way.
-//   Consumers: three warpgroups, one per kernel column kw.  Warpgroup kw walks the halo rows; the fragment of halo row
+//   B = dY^T (N = 64 co, k = pixel), K-major: the producer warpgroup transposes the two [64 px][32 co] dY boxes once
+//       per stage into [co][pixel] (two k-chunks of [64 co][32 px]), one box and k-chunk per warp, and sums the bias
+//       gradient on the way.
+//   Consumers: warpgroups 1..3, one per kernel column kw.  Warpgroup kw walks the halo rows; the fragment of halo row
 //       y (one 8-pixel segment) is the A operand of output row y - kh for each kh with 0 <= y - kh < TH, so it is loaded
 //       once and feeds up to three m64n64k8 wgmmas into acc[kh] (3 x 32 fp32 registers per thread): 24 wgmmas per stage
-//       and warpgroup.  The 13-warp CTA puts four warps on one SM sub-partition, so ptxas caps every thread at 128
-//       registers (a producer warpgroup would not raise it: setmaxnreg does not lift the compile-time cap).  Beside the
-//       96 accumulators that leaves room for one fragment: a fragment's wgmmas complete before the next one is loaded,
-//       while the other two warpgroups keep the tensor cores busy.  The swizzle phase of a fragment row depends on y,
-//       the segment, kw and the lane's column; the loads reach at most two threads per bank (8 ci in two 16-byte
-//       chunks x 4 consecutive halo rows).
+//       and warpgroup, one commit group per fragment.  Two fragment buffers keep two groups in flight: fragment i + 1 is
+//       loaded and issued while group i runs, and wgmma_wait<1> then retires group i, whose buffer takes fragment i + 2.
+//       The swizzle phase of a fragment row depends on y, the segment, kw and the lane's column; the loads reach at most
+//       two threads per bank (8 ci in two 16-byte chunks x 4 consecutive halo rows).
+//   Registers: setmaxnreg moves registers from the producer (56) to the consumers (152; 128 x 56 + 3 x 128 x 152 =
+//       65536, the whole register file).  ptxas allocates code after setmaxnreg against the new limit, but decides
+//       whether wgmmas may stay in flight against the 128 of the 512-thread launch bound: 96 accumulators, two
+//       fragments and the addressing just fit (R0..R127), and one more live register (a spin counter in the consumers'
+//       full-barrier wait) makes it serialise every wgmma (advisory C7512).  So the consumers wait unguarded, and the
+//       producer carries the watchdog: it cannot refill a slot the consumers never released, and at the end it waits
+//       guarded on the full phases of the last stages itself.
 //   Pipeline: three stage slots {halo boxes, dY^T, raw dY}.  Raw dY of stage k + 3 is requested as soon as stage k's
-//   has been transposed; the halo boxes as soon as the three consumer warpgroups release the slot.  The tile origin
-//   advances incrementally (no division inside the loop).
+//       has been transposed; the halo boxes as soon as the three consumer warpgroups release the slot, which each does
+//       once the group of the slot's last fragment has retired, one fragment into the next stage (the fragment buffers
+//       alternate across stages: a stage has an even number of fragments).  The tile origin advances incrementally (no
+//       division inside the loop).
 // ------------------------------------------------------------------------------------------------
 struct WgradArgs {
   float* dWp;  // [9][Cin][Cout], pre-zeroed
@@ -853,7 +861,9 @@ struct WgradArgs {
   int total_tiles, per;   // pixel tiles, and tiles per split-K CTA (blockIdx.y)
 };
 
-constexpr int WG_THREADS = 3 * 128 + 32;           // one consumer warpgroup per kernel column, then one producer warp
+constexpr int WG_THREADS = 4 * 128;                // the producer warpgroup, then one consumer warpgroup per kernel column
+constexpr int WG_PRODUCER_REGS = 56, WG_CONSUMER_REGS = 152;   // setmaxnreg budgets
+static_assert(128 * WG_PRODUCER_REGS + 3 * 128 * WG_CONSUMER_REGS <= 65536, "wgrad register budget");
 constexpr int WG_STAGES = 3;                       // stage slots
 constexpr int WG_KP = 64;                          // pixels per stage
 constexpr int WG_RAW_ROWS = 120;                   // (TH + 2) * (TW + 2) * TN: halo box rows (TW >= 8)
@@ -916,55 +926,55 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_cons
   __syncthreads();
   if (nk <= 0) return;
 
-  if (warp == 3 * 4) {
-    // lane transposes rows co = lane and lane + 32 of dY^T (column co & 31 of raw dY box co / 32) and sums their bias
-    const int lane = threadIdx.x & 31;
+  if (warp < 4) {
+    regs_dealloc<WG_PRODUCER_REGS>();
+    // warp w transposes k-chunk c = w / 2 (pixels 32 c .. 32 c + 31) of raw dY box j = w % 2: its lane writes row
+    // co = 32 j + lane of dY^T (column lane of the box) and sums that part of co's bias
+    const int lane = threadIdx.x & 31, j = warp & 1, c = warp >> 1;
     constexpr uint32_t x_tx = (WG_CI / 32) * (TH + 2) * (TW + 2) * TN * 128;
-    WgradTile<TW, TH, TN> x_tile((int)t_begin, a), dy_tile = x_tile;   // only lane 0 issues TMAs
-    if (lane == 0)
+    WgradTile<TW, TH, TN> x_tile((int)t_begin, a), dy_tile = x_tile;   // only thread 0 issues TMAs
+    if (threadIdx.x == 0)
       for (int u = 0; u < WG_STAGES && u < nk; ++u) {
         uint8_t* dy = smem + u * WG_STAGE_BYTES + WG_X_BYTES + WG_DY_BYTES;
         mbar_expect_tx(&dy_full[u], WG_DY_BYTES);
 #pragma unroll
-        for (int j = 0; j < WG_CO / 32; ++j)
-          tma_load_4d(dy + j * (WG_KP * 128), &tmDY, &dy_full[u], co0 + j * 32, dy_tile.w0, dy_tile.h0, dy_tile.n0);
+        for (int b = 0; b < WG_CO / 32; ++b)
+          tma_load_4d(dy + b * (WG_KP * 128), &tmDY, &dy_full[u], co0 + b * 32, dy_tile.w0, dy_tile.h0, dy_tile.n0);
         dy_tile.next(a);
       }
-    float bsum[WG_CO / 32] = {};
+    float bsum = 0.f;
     int s = 0;
     uint32_t ph = 0;
     for (int k = 0; k < nk; ++k) {
       uint8_t* st = smem + s * WG_STAGE_BYTES;
       mbar_wait(&empty[s], ph ^ 1);
-      if (lane == 0) {
+      if (threadIdx.x == 0) {
         mbar_expect_tx(&full[s], x_tx);
 #pragma unroll
-        for (int j = 0; j < WG_CI / 32; ++j)
-          tma_load_4d(st + j * WG_RAW_BYTES, &tmX, &full[s], ci0 + j * 32, x_tile.w0 - 1, x_tile.h0 - 1, x_tile.n0);
+        for (int b = 0; b < WG_CI / 32; ++b)
+          tma_load_4d(st + b * WG_RAW_BYTES, &tmX, &full[s], ci0 + b * 32, x_tile.w0 - 1, x_tile.h0 - 1, x_tile.n0);
         x_tile.next(a);
       }
       mbar_wait(&dy_full[s], ph);
       const uint32_t dyt = smem_u32(st + WG_X_BYTES), dy = dyt + WG_DY_BYTES;
 #pragma unroll
-      for (int j = 0; j < WG_CO / 32; ++j)
+      for (int k4 = 0; k4 < 8; ++k4) {             // pixels 32 c + 4 k4 .. 32 c + 4 k4 + 3
+        uint32_t v[4];
 #pragma unroll
-        for (int k4 = 0; k4 < WG_KP / 4; ++k4) {   // pixels 4 k4 .. 4 k4 + 3: k-chunk k4 / 8
-          uint32_t v[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            v[i] = ld_shared_u32(dy + j * (WG_KP * 128) + sw128_off(4 * k4 + i, lane));
-            bsum[j] += __uint_as_float(v[i]);
-          }
-          st_shared_v4(dyt + (k4 >> 3) * (WG_CO * 128) + sw128_off(32 * j + lane, 4 * (k4 & 7)), v[0], v[1], v[2], v[3]);
+        for (int i = 0; i < 4; ++i) {
+          v[i] = ld_shared_u32(dy + j * (WG_KP * 128) + sw128_off(32 * c + 4 * k4 + i, lane));
+          bsum += __uint_as_float(v[i]);
         }
+        st_shared_v4(dyt + c * (WG_CO * 128) + sw128_off(32 * j + lane, 4 * k4), v[0], v[1], v[2], v[3]);
+      }
       fence_proxy_async();
-      __syncwarp();                                 // dY^T is complete and raw dY slot s is free
-      if (lane == 0) {
+      named_bar(1, 128);                            // dY^T is complete and raw dY slot s is free
+      if (threadIdx.x == 0) {
         if (k + WG_STAGES < nk) {
           mbar_expect_tx(&dy_full[s], WG_DY_BYTES);
 #pragma unroll
-          for (int j = 0; j < WG_CO / 32; ++j)
-            tma_load_4d(st + WG_X_BYTES + WG_DY_BYTES + j * (WG_KP * 128), &tmDY, &dy_full[s], co0 + j * 32, dy_tile.w0,
+          for (int b = 0; b < WG_CO / 32; ++b)
+            tma_load_4d(st + WG_X_BYTES + WG_DY_BYTES + b * (WG_KP * 128), &tmDY, &dy_full[s], co0 + b * 32, dy_tile.w0,
                         dy_tile.h0, dy_tile.n0);
           dy_tile.next(a);
         }
@@ -972,12 +982,14 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_cons
       }
       if (++s == WG_STAGES) { s = 0; ph ^= 1; }
     }
-    // bias: added once per co, by the ci-tile-0 CTAs
-#pragma unroll
-    for (int j = 0; j < WG_CO / 32; ++j)
-      if (a.db && ci_t == 0 && co0 + 32 * j + lane < a.Cout) atomicAdd(a.db + co0 + 32 * j + lane, bsum[j]);
+    // the watchdog for the consumers' unguarded full waits: a stage before the last WG_STAGES was released by them, so
+    // its full phase completed; the last ones are checked here
+    for (int kk = max(nk - WG_STAGES, 0); kk < nk; ++kk) mbar_wait(&full[kk % WG_STAGES], (kk / WG_STAGES) & 1);
+    // bias: added once per co and k-chunk, by the ci-tile-0 CTAs
+    if (a.db && ci_t == 0 && co0 + 32 * j + lane < a.Cout) atomicAdd(a.db + co0 + 32 * j + lane, bsum);
   } else {
-    const int kw = warp >> 2, t = threadIdx.x & 127, wl = t >> 5, lane = t & 31, g = lane >> 2, q = lane & 3;
+    regs_alloc<WG_CONSUMER_REGS>();
+    const int kw = (warp >> 2) - 1, t = threadIdx.x & 127, wl = t >> 5, lane = t & 31, g = lane >> 2, q = lane & 3;
     // this thread's A rows: ci 16 wl + g (+8) = column cib (+8) of halo box wl / 2.  Its k columns q (+4) of a fragment
     // whose 8 pixels start at halo row R read halo rows R + kw + q (+4).  In a SWIZZLE_128B box the 16-byte chunk of a
     // row is XOR-ed with bits 7..9 of the row's address, which is computed per fragment: a table of phases would cost
@@ -991,12 +1003,13 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_cons
     for (int j = 0; j < 3; ++j)
 #pragma unroll
       for (int e = 0; e < 32; ++e) acc[j][e] = 0.f;
-    uint32_t f[4];
+    uint32_t f[2][4];   // fragment i of a stage goes to f[i % 2]
     constexpr int SEG = TW / 8, NF = TN * (TH + 2) * SEG;   // 8-pixel halo row segments per stage
-    int s = 0;
+    static_assert(NF % 2 == 0, "the fragment buffers alternate across stages");
+    int s = 0, s_prev = 0;
     uint32_t ph = 0;
     for (int k = 0; k < nk; ++k) {
-      mbar_wait(&full[s], ph);
+      mbar_wait_unguarded(&full[s], ph);   // the producer's guarded waits trap if this phase never completes
       const uint32_t xb = stage0 + s * WG_STAGE_BYTES, xa = xb + xrow;
       const uint64_t bdesc = make_sdesc(xb + WG_X_BYTES);
 #pragma unroll
@@ -1005,26 +1018,31 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_cons
         const int R = (n * (TH + 2) + y) * (TW + 2) + 8 * js;
         const uint32_t r0 = xa + R * 128, r4 = xa + (R + 4) * 128;
         const uint32_t p0 = r0 + (((r0 >> 3) & 0x70) ^ cq), p4 = r4 + (((r4 >> 3) & 0x70) ^ cq);
-        f[0] = ld_shared_u32(p0);
-        f[1] = ld_shared_u32(p0 ^ 32);
-        f[2] = ld_shared_u32(p4);
-        f[3] = ld_shared_u32(p4 ^ 32);
+        uint32_t (&fi)[4] = f[i & 1];   // its previous fragment's group retired at the last wgmma_wait<1>
+        fi[0] = ld_shared_u32(p0);
+        fi[1] = ld_shared_u32(p0 ^ 32);
+        fi[2] = ld_shared_u32(p4);
+        fi[3] = ld_shared_u32(p4 ^ 32);
         wgmma_fence();
 #pragma unroll
         for (int kh = 0; kh < 3; ++kh) {
           const int h = y - kh;
           if (h < 0 || h >= TH) continue;
           const int ks = ((n * TH + h) * TW + 8 * js) / 8;   // k-step of output pixels (n, h, 8 js .. 8 js + 7)
-          wgmma_tf32(acc[kh], f, bdesc + (uint32_t)(((ks >> 2) * (WG_CO * 128) + (ks & 3) * 32) >> 4));
+          wgmma_tf32(acc[kh], fi, bdesc + (uint32_t)(((ks >> 2) * (WG_CO * 128) + (ks & 3) * 32) >> 4));
         }
         wgmma_commit();
-        wgmma_wait<0>();      // f is free again; the other two warpgroups keep the tensor cores busy meanwhile
+        wgmma_wait<1>();      // retires the previous fragment's group: its buffer takes the next fragment
 #pragma unroll
         for (int j = 0; j < 3; ++j) wgmma_keep(acc[j]);
+        if (i == 0 && k > 0 && t == 0) mbar_arrive(&empty[s_prev]);   // the previous stage's last group has retired
       }
-      if (t == 0) mbar_arrive(&empty[s]);
+      s_prev = s;
       if (++s == WG_STAGES) { s = 0; ph ^= 1; }
     }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int j = 0; j < 3; ++j) wgmma_keep(acc[j]);
     // accumulator element 4 i + e: ci row 16 wl + g + 8 (e >> 1), co columns 8 i + 2 q (+1), adjacent in dWp
 #pragma unroll
     for (int kh = 0; kh < 3; ++kh)
