@@ -229,6 +229,7 @@ int hk_sqrtm_bwd(const float* x, const float* y, const float* g, float* saved, f
   cudaStream_t st = (cudaStream_t)stream_;
   HK_REQUIRE(x && y && g && saved && grad_x, HK_ERR_ARG, "hk_sqrtm_bwd: null pointer");
   HK_REQUIRE(iterN >= 2, HK_ERR_UNSUPPORTED, "hk_sqrtm_bwd: iterN=%d (< 2) is not supported", iterN);
+  HK_REQUIRE(n % 4 == 0, HK_ERR_UNSUPPORTED, "hk_sqrtm_bwd: dim=%d must be a multiple of 4", n);
   HK_REQUIRE(workspace && workspace_bytes >= hk_sqrtm_bwd_workspace_bytes(B, n), HK_ERR_WORKSPACE,
              "hk_sqrtm_bwd: workspace too small");
   SqrtmSaved sv = saved_view(saved, B, n, iterN);

@@ -101,6 +101,22 @@ def test_head_and_mpncov_argument_errors(lib):
 
 
 @pytest.mark.parametrize('precise', [0, 1], ids=['tf32', 'precise'])
+def test_sqrtm_dim_not_multiple_of_4_launches_nothing(lib, precise):
+    """hk_sqrtm_fwd and hk_sqrtm_bwd reject n % 4 != 0 (the (hi, lo) rows are TMA operands at a 16-byte pitch) at the
+    entry point, before the backward's first element-wise kernel, in both precision modes."""
+    lib.hk_set_precise(precise)
+    lib.hk_reset_launch_count()
+    try:
+        for n in (6, 255, 258):
+            assert lib.hk_sqrtm_fwd(FAKE, FAKE, FAKE, 2, n, 5, FAKE, 1 << 40, None) == -3 and 'multiple of 4' in err(lib)
+            assert lib.hk_sqrtm_bwd(FAKE, FAKE, FAKE, FAKE, FAKE, 2, n, 5, FAKE, 1 << 40, None) == -3
+            assert f'dim={n}' in err(lib) and 'multiple of 4' in err(lib)
+        assert lib.hk_launch_count() == 0
+    finally:
+        lib.hk_set_precise(0)
+
+
+@pytest.mark.parametrize('precise', [0, 1], ids=['tf32', 'precise'])
 @pytest.mark.parametrize('entry', ['hk_gemm_tf32', 'hk_gemm_3xtf32'])
 def test_gemm_operand_errors_before_any_allocation_or_launch(lib, entry, precise):
     """The GEMM's TMA preconditions (16-byte aligned operand base, row pitch and batch stride in 16-byte units,
