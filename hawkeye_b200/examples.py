@@ -1,6 +1,6 @@
 """Trainer subclasses of the hot-path methods with the reference's Examples/ surface:
 ``python -m hawkeye_b200.examples {BCNN,CBCNN,MPN,PeerLearning,OSMENet,APINet,DCL,ProtoTreeNet,InterpPartsNet,NTSNet,APCNN,MGE_CNN,
-CIN,Baseline,PairConfusion,CrossX}
+CIN,Baseline,PairConfusion,CrossX,S3N}
 --config <yaml>`` replaces
 ``python Examples/<Method>.py --config <yaml>`` (same yaml files; one process per GPU under torchrun instead of nn.DataParallel).
 Baseline and PairConfusion train the plain ResNet-50 classifier (configs/Baseline.yaml, configs/PC_resnet50.yaml).
@@ -583,14 +583,94 @@ class CrossXTrainer(Trainer):
         return _MultiStep(self.optimizer, config.milestones, config.gamma)
 
 
+class S3NTrainer(Trainer):
+    """Examples/S3N.py: criterion = MultiSmoothLoss(smooth_ratio); SGD without momentum (the reference passes none, whatever
+    the yaml says) and with the yaml's weight_decay in four groups: the parameters whose name holds 'classifier' at lr,
+    ``radius`` at 1e-5 lr, ``filter`` at 1e-5 lr and everything else at 0.1 lr — ``radius_inv`` included, as the reference
+    separates ``model.radius`` only; CosineAnnealingLR(T_max, eta_min) once per epoch.  RandomResizedCrop(448, scale
+    (0.5, 1)) and a horizontal flip for training, Resize(448) and CenterCrop(448) for validation.  Accuracy on aggregation.
+
+    ``p`` is 0 in training before epoch 20 and 1 from then on; validation uses 1 before epoch 20 and 2 from then on.  The
+    training value lives in an int32 device tensor written before each step, outside any captured graph, so the step has no
+    host synchronisation and ``cuda_graph: true`` replays one capture across the change of ``p``.  ``backbone.fc`` and
+    ``map_origin`` never get a gradient, so the reference's torch SGD never touches them; here they stay out of the
+    optimizer's flat buffer for the same result (no weight decay on them)."""
+
+    def __init__(self, config=None, dataloaders=None):
+        super().__init__(config, dataloaders)
+        import torch
+        self.p_train = torch.zeros(1, dtype=torch.int32, device=self.device)
+
+    def get_transformers(self, config):
+        """Examples/S3N.py:18-32 (fixed sizes: the reference does not read the transformer config)."""
+        from torchvision import transforms
+        norm = transforms.Normalize(mean=(0.485, 0.456, 0.406), std=(0.229, 0.224, 0.225))
+        return {
+            'train': transforms.Compose([transforms.RandomResizedCrop(448, scale=(0.5, 1)), transforms.RandomHorizontalFlip(),
+                                         transforms.ToTensor(), norm]),
+            'val': transforms.Compose([transforms.Resize(448), transforms.CenterCrop(448), transforms.ToTensor(), norm]),
+        }
+
+    def get_criterion(self, config):
+        from .losses import MultiSmoothLoss
+        return MultiSmoothLoss(config)
+
+    def param_groups(self):
+        m = self.get_model_module()
+        named = list(m.named_parameters())
+        classifier = [p for n, p in named if 'classifier' in n]
+        special = {id(p) for p in classifier + list(m.radius.parameters()) + list(m.filter.parameters())
+                   + list(m.no_grad_parameters())}
+        return [(classifier, 1.0), (list(m.radius.parameters()), 1e-5), (list(m.filter.parameters()), 1e-5),
+                ([p for _, p in named if id(p) not in special], 0.1)]
+
+    def early_group(self):
+        """The classifiers: their gradients are complete first in the backward, so their all-reduce overlaps the rest."""
+        return 0
+
+    def get_optimizer(self, config):
+        from . import engine
+        return engine.FusedSGD(self.flat, lr=config.lr, momentum=0.0,
+                               weight_decay=config.weight_decay if 'weight_decay' in config else 0.0,
+                               group_lrs=[config.lr * m for _, m in self.trained_groups()])
+
+    def get_scheduler(self, config):
+        return _Cosine(self.optimizer, config.T_max, config.eta_min, 0)
+
+    @staticmethod
+    def train_p(epoch):
+        return 0 if epoch < 20 else 1
+
+    @staticmethod
+    def val_p(epoch):
+        return 1 if epoch < 20 else 2
+
+    def batch_training(self, data):
+        self.p_train.fill_(self.train_p(self.epoch))
+        return super().batch_training(data)
+
+    def forward_model(self, images, labels):
+        return self.model(images, self.p_train)
+
+    def batch_validate(self, data):
+        import torch
+        from .train import accuracy
+        images, labels = self.batch_tensors(data)
+        images, labels = self.to_device(images), self.to_device(labels)
+        with torch.no_grad():
+            aggregation = self.model(images, self.val_p(self.epoch))[0]
+        self.average_meters['acc'].update(accuracy(aggregation, labels, 1), images.size(0))
+
+
 TRAINERS = {'BCNN': BCNNTrainer, 'CBCNN': CBCNNTrainer, 'MPN': MPNTrainer, 'PeerLearning': PeerLearningTrainer,
             'OSMENet': OSMENetTrainer}
 # TRAINERS keeps the key set it has always had, so code that enumerates it sees no change; the command line dispatches
-# over every method, APINet, DCL, ProtoTreeNet, InterpPartsNet, NTSNet, APCNN, MGE_CNN, CIN, Baseline, PairConfusion and
-# CrossX included.
+# over every method, APINet, DCL, ProtoTreeNet, InterpPartsNet, NTSNet, APCNN, MGE_CNN, CIN, Baseline, PairConfusion,
+# CrossX and S3N included.
 ALL_TRAINERS = dict(TRAINERS, APINet=APINetTrainer, DCL=DCLTrainer, ProtoTreeNet=ProtoTreeTrainer,
                    InterpPartsNet=InterpPartsNetTrainer, NTSNet=NTSNetTrainer, APCNN=APCNNTrainer, MGE_CNN=MGE_CNNTrainer,
-                   CIN=CINTrainer, Baseline=BaselineTrainer, PairConfusion=PCResNetTrainer, CrossX=CrossXTrainer)
+                   CIN=CINTrainer, Baseline=BaselineTrainer, PairConfusion=PCResNetTrainer, CrossX=CrossXTrainer,
+                   S3N=S3NTrainer)
 
 
 def main(argv=None):

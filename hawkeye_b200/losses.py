@@ -465,3 +465,35 @@ class InterpPartsLoss(nn.Module):
         loss_ce = self.ce_loss(logits, target)
         self.last_correct = self.ce_loss.last_correct
         return loss_ce + self.coeff * self.shaping_loss(assign)
+
+
+def smooth_ratio_eps(smooth_ratio, K):
+    """The label smoothing eps of hk_softmax_ce_ls whose target (1 - eps) onehot + eps / K is MultiSmoothLoss's
+    r onehot + (1 - r)(1 - onehot) / (K - 1): eps = (1 - r) K / (K - 1)."""
+    return (1.0 - smooth_ratio) * K / (K - 1)
+
+
+class MultiSmoothLoss(nn.Module):
+    """model/loss/S3N_loss.py: over the outputs (aggregation, agg_origin, agg_sampler, agg_sampler1) of S3N, the sum of
+    cross-entropy on terms 0 and 2 and of the smoothed cross-entropy (target smooth_ratio on the label, (1 - smooth_ratio) /
+    (K - 1) elsewhere) on term 1 and the last term, each a mean over the rows, on hk_softmax_ce_ls.  ``loss_weight`` (a
+    {index: weight} dict) scales the terms as in the reference.  ``last_correct`` is the top-1 count on ``aggregation``."""
+
+    def __init__(self, config):
+        super().__init__()
+        self.smooth_ratio = config.smooth_ratio
+
+    def forward(self, output, target, loss_weight=None):
+        from .ops import CrossEntropyLSFn
+        assert isinstance(output, tuple), 'input is less than 2'
+        weights = [1.0] * len(output)
+        for k, v in (loss_weight or {}).items():
+            weights[int(k)] = float(v)
+        loss = 0
+        for i, logits in enumerate(output):
+            eps = smooth_ratio_eps(self.smooth_ratio, logits.shape[1]) if i in (1, len(output) - 1) else 0.0
+            term, correct = CrossEntropyLSFn.apply(logits, target, eps)
+            if i == 0:
+                self.last_correct = correct
+            loss = loss + weights[i] * term
+        return loss

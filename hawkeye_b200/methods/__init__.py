@@ -13,3 +13,4 @@ from .apcnn import APCNN  # noqa: F401
 from .mge import MGE_CNN  # noqa: F401
 from .resnet import ResNet50, ResNet101  # noqa: F401
 from .crossx import CrossX  # noqa: F401
+from .s3n import S3N  # noqa: F401

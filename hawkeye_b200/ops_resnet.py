@@ -40,7 +40,7 @@ class Unit:
             _lib.call('hk_stem_im2col', x, x147, N, H, W, s)
             _lib.call('hk_pack_stem_weights', w, w147, cout, s)
             c = conv1x1_fwd(x147, w147).view(N, Ho, Wo, cout)
-            rec['xin'] = x147
+            rec['xin'], rec['in_hw'] = x147, (H, W)
         else:
             N, H, W, cin = x.shape
             if self.kind in ('1x1', '1x1s2'):
@@ -84,6 +84,10 @@ class Unit:
             dwm = torch.empty(cout, 160, device=dev, dtype=torch.float32)
             conv1x1_wgrad(xin, dc, dwm)
             dw = dwm[:, :147].reshape(w.shape).contiguous()
+            if need_dx:                                 # the image gradient (S3N's sampled images): a gather per pixel
+                H, W = rec['in_hw']
+                dx = torch.empty(N, w.shape[1], H, W, device=dev, dtype=torch.float32)
+                _lib.call('hk_stem_dgrad', dc, w, dx, N, H, W, s)
         elif self.kind in ('1x1', '1x1s2'):
             cin = xin.shape[-1]
             dw = torch.empty(cout, cin, 1, 1, device=dev, dtype=torch.float32)
@@ -229,7 +233,8 @@ def _param_iter(params):
 
 
 class ResNetTrunkFn(Function):
-    """NCHW image -> NHWC feature map [N, H/32, W/32, 2048] as the last block writes it."""
+    """NCHW image -> NHWC feature map [N, H/32, W/32, 2048] as the last block writes it.  The image gets a gradient
+    (hk_stem_dgrad) only when it requires one."""
 
     @staticmethod
     def forward(ctx, x, plan, save, training, *params):
@@ -261,11 +266,11 @@ class ResNetTrunkFn(Function):
         N, H, W, C = yshape
         dy0 = torch.empty(N, H, W, C, device=dfeat.device, dtype=torch.float32)
         _lib.call('hk_maxpool3x3s2_bwd', am, g, dy0, N, H, W, C, s)
-        _, _, dw0, dg0, db0 = plan.stem.backward(r0, dy0, need_dx=False)
+        dx, _, dw0, dg0, db0 = plan.stem.backward(r0, dy0, need_dx=ctx.needs_input_grad[0])
         grads = [(dw0, dg0, db0)] + grads
         ctx.recs = None
         flat = [t for trip in grads for t in trip]
-        return (None, None, None, None) + tuple(flat)
+        return (dx, None, None, None) + tuple(flat)
 
 
 class BlockStackFn(Function):

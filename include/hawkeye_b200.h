@@ -605,6 +605,49 @@ int hk_crossx_loss(const float* xf, const float* xp, const float* xc, const long
                    float label_smoothing, float gamma_ulti, float gamma_plty, float gamma_cmbn, int n_total,
                    float reg_scale, void* stream);
 
+/* ---- S3N: model/methods/S3N.py (grid_size 31, padding_size 30, a 61x61 filter) ---------------------------------------
+ * hk_s3n_sample_maps (S3N.py:193-270, generate_map up to the two torch.cat): one block per image.  crm [N,h,w,K] are the
+ *   class response maps as the 1x1 conv's NHWC rows (S3N.py:290-291 before the interpolation), rnd [N,961] uniform draws
+ *   (a peak at grid position q uses rnd[n,q]), p int32 [1] on the device (0, 1 or 2, S3N.py:226-258), radius / radius_inv
+ *   [1] (the ScaleLayer scales).  Interpolates to 31x31 (align_corners=True), takes softmax, top-5 and the gate of the maps'
+ *   spatial means, the decision map, its min-max normalisation and its peaks (first maximum of the 3x3 window and >= the
+ *   mean), assigns them by p and writes xs [2N,961]: rows [0,N) the zoom maps base + sum s G(radius sqrt s), rows [N,2N)
+ *   the complementary maps base + sum (1/s) G(radius_inv sqrt s), G(t) = exp(-d^2 / 2(31 t)^2) (kernel_generate over its
+ *   maximum).  The peak record for the backward: counts [N], peaks [N,961] int32 = position | flags << 16 (1: zoom map,
+ *   2: complementary map) and scores [N,961], in row-major order.  An image without peaks keeps base in both maps.
+ *   h, w <= 64, 5 <= K <= 4096; no host synchronisation.
+ * hk_s3n_sample_maps_bwd: dxs [2N,961] and the peak record -> dradius [1], dradius_inv [1], one block, fixed order.
+ * hk_s3n_grid_fwd (create_grid, S3N.py:156-183, after ReplicationPad2d(30) at :272/:277): maps [B,961] (B = 2N: zoom then
+ *   complementary), filter [61,61] -> grid [B,31,31,2] = clamp(2 Sx / S0 - 1, -1, 1), clamp(2 Sy / S0 - 1, -1, 1), with S0,
+ *   Sx, Sy the correlations of the padded map alone, times the x basis and times the y basis; sums [B,31,31,3] = (S0,Sx,Sy)
+ *   for the backward.
+ * hk_s3n_grid_bwd: dgrid [B,31,31,2] -> dmaps [B,961] (through the clamp, inclusive at the bounds, the quotient, the
+ *   correlations and the replication pad) and dfilter [61,61] summed over the B maps in index order.  Workspace:
+ *   hk_s3n_grid_bwd_workspace_bytes(B).
+ * hk_s3n_warp_fwd (S3N.py:186 + :274/:279): x [N,C,H,W], grid [B,31,31,2] -> out [B,C,Ho,Wo] = grid_sample(x[b % N],
+ *   interpolate(grid, (Ho,Wo), bilinear, align_corners=True), bilinear, zeros, align_corners=True); the Ho x Wo grid is
+ *   never written.
+ * hk_s3n_warp_bwd: dout [B,C,Ho,Wo] -> dgrid [B,31,31,2] (x gets no gradient); workspace
+ *   hk_s3n_warp_bwd_workspace_bytes(B,Ho,Wo) holds the Ho x Wo grid gradient, which is gathered per coarse node.
+ * hk_stem_dgrad (backbone/resnet.py:176, conv1 7x7 / 2, padding 3, 64 outputs): dc NHWC [N,Ho,Wo,64] (16-byte aligned),
+ *   w [64,3,7,7] -> dx NCHW [N,3,H,W], a gather per input pixel: no atomics, no column workspace. */
+int hk_s3n_sample_maps(const float* crm, const float* rnd, const int* p, const float* radius, const float* radius_inv,
+                       float base_ratio, float* xs, int* peaks, float* scores, int* counts, int N, int h, int w, int K,
+                       void* stream);
+int hk_s3n_sample_maps_bwd(const float* dxs, const int* peaks, const float* scores, const int* counts,
+                           const float* radius, const float* radius_inv, float* dradius, float* dradius_inv, int N,
+                           void* stream);
+int hk_s3n_grid_fwd(const float* maps, const float* filter, float* grid, float* sums, int B, void* stream);
+size_t hk_s3n_grid_bwd_workspace_bytes(int B);
+int hk_s3n_grid_bwd(const float* maps, const float* filter, const float* sums, const float* dgrid, float* dmaps,
+                    float* dfilter, int B, void* workspace, size_t workspace_bytes, void* stream);
+int hk_s3n_warp_fwd(const float* x, const float* grid, float* out, int N, int B, int C, int H, int W, int Ho, int Wo,
+                    void* stream);
+size_t hk_s3n_warp_bwd_workspace_bytes(int B, int Ho, int Wo);
+int hk_s3n_warp_bwd(const float* x, const float* grid, const float* dout, float* dgrid, int N, int B, int C, int H, int W,
+                    int Ho, int Wo, void* workspace, size_t workspace_bytes, void* stream);
+int hk_stem_dgrad(const float* dc, const float* w, float* dx, int N, int H, int W, void* stream);
+
 /* ---- input side: transforms.ToTensor + Normalize (dataset/transforms.py:14-19, test.py:80-85) fused on
  * the GPU: uint8 HWC batch [N,H,W,3] -> fp32 NCHW (x/255 - mean_c)/std_c; a quarter of the float pipeline's H2D bytes */
 int hk_normalize_u8(const unsigned char* x_nhwc, float* y_nchw, int N, int H, int W, float mean0, float mean1, float mean2,
