@@ -237,6 +237,12 @@ __device__ __forceinline__ float tf32_round(float x) {
   return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u);
 }
 
+// ToTensor + Normalize of one uint8 channel value (dataset/transforms.py:14-19): (v/255 - mean) * (1/std).  Every kernel
+// that turns decoded pixels into model inputs (hk_normalize_u8, hk_augment_apply) goes through this one expression.
+__device__ __forceinline__ float normalize_u8_value(unsigned char v, float mean, float inv_std) {
+  return ((float)v * (1.f / 255.f) - mean) * inv_std;
+}
+
 }  // namespace hk
 
 #include "reduce.cuh"

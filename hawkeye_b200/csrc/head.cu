@@ -95,9 +95,9 @@ __global__ void normalize_u8_kernel(const unsigned char* __restrict__ x, float* 
     const size_t n = p / hw, q = p - n * hw;
     const unsigned char* s = x + p * 3;
     float* d = y + n * 3 * hw + q;
-    d[0] = ((float)s[0] * (1.f / 255.f) - m0) * i0;
-    d[hw] = ((float)s[1] * (1.f / 255.f) - m1) * i1;
-    d[2 * hw] = ((float)s[2] * (1.f / 255.f) - m2) * i2;
+    d[0] = normalize_u8_value(s[0], m0, i0);
+    d[hw] = normalize_u8_value(s[1], m1, i1);
+    d[2 * hw] = normalize_u8_value(s[2], m2, i2);
   }
 }
 

@@ -4,6 +4,9 @@ the train / eval transform presets (dataset/transforms.py:14-73) and the class-b
 Python plumbing, not a kernel path; the tensor part of the eval preset (``ToTensor + Normalize``) can run on the GPU instead
 (``hawkeye_b200.test.normalize_u8``).  Used by ``Trainer.get_dataloader`` when the reference's ``dataset`` package is not
 importable, so the package also trains outside a Hawkeye checkout.
+
+``DevicePresetTrain`` / ``DevicePresetEval`` are the two default presets with everything after the decode on the GPU
+(``hawkeye_b200.ops_augment``), selected by ``dataset.transformer.device: cuda``.
 """
 import os
 
@@ -94,6 +97,111 @@ class ClassificationPresetEval:
 
     def __call__(self, img):
         return self.transforms(img)
+
+
+def _bilinear_only(interpolation):
+    from torchvision.transforms.functional import InterpolationMode
+    if interpolation not in (None, InterpolationMode.BILINEAR):
+        raise ValueError(f'the device presets resize with BILINEAR only, not {interpolation}')
+    return InterpolationMode.BILINEAR
+
+
+def _square(crop_size):
+    size = (crop_size, crop_size) if isinstance(crop_size, int) else tuple(crop_size)
+    if len(size) == 1:
+        size = (size[0], size[0])
+    if size[0] != size[1]:
+        raise ValueError(f'the device presets produce square images, not {size}')
+    return int(size[0])
+
+
+class DevicePresetTrain:
+    """``ClassificationPresetTrain`` with everything after the decode on the GPU (``hawkeye_b200.ops_augment``).  Called on a
+    decoded PIL image in a loader worker, it makes the host preset's random draws — the same torchvision calls, in the same
+    order, on the same torch RNG — and returns ``(uint8 HWC array, parameter row)``; ``collate`` packs a batch of them.
+    A seeded worker therefore draws the same parameters for an image under either preset and leaves the RNG in the same
+    state.  Only ``auto_augment_policy`` None or 'ta_wide' and BILINEAR interpolation are supported."""
+
+    def __init__(self, crop_size, mean=(0.485, 0.456, 0.406), std=(0.229, 0.224, 0.225), interpolation=None, hflip_prob=0.5,
+                 auto_augment_policy=None, random_erase_prob=0.0):
+        from torchvision.transforms import autoaugment, transforms
+        if auto_augment_policy not in (None, 'ta_wide'):
+            raise ValueError(f"the device train preset supports auto_augment_policy None or 'ta_wide', not "
+                             f"{auto_augment_policy!r}")
+        interpolation = _bilinear_only(interpolation)
+        self.size, self.mean, self.std, self.hflip_prob = _square(crop_size), tuple(mean), tuple(std), hflip_prob
+        self.crop = transforms.RandomResizedCrop(crop_size, interpolation=interpolation)
+        self.ta = autoaugment.TrivialAugmentWide(interpolation=interpolation) if auto_augment_policy else None
+        self.erase = transforms.RandomErasing(p=random_erase_prob) if random_erase_prob > 0 else None
+
+    def draw(self, img):
+        """-> the parameter row of one PIL image, drawn as the host preset draws it."""
+        from .ops_augment import param_row
+        S = self.size
+        i, j, h, w = self.crop.get_params(img, self.crop.scale, self.crop.ratio)
+        flip = self.hflip_prob > 0 and bool(torch.rand(1) < self.hflip_prob)
+        op, magnitude = 'Identity', 0.0
+        if self.ta is not None:                          # TrivialAugmentWide.forward's draws
+            op_meta = self.ta._augmentation_space(self.ta.num_magnitude_bins)
+            op = list(op_meta.keys())[int(torch.randint(len(op_meta), (1,)).item())]
+            magnitudes, signed = op_meta[op]
+            magnitude = (float(magnitudes[torch.randint(len(magnitudes), (1,), dtype=torch.long)].item())
+                         if magnitudes.ndim > 0 else 0.0)
+            if signed and torch.randint(2, (1,)):
+                magnitude *= -1.0
+        erase = None
+        if self.erase is not None and torch.rand(1) < self.erase.p:   # RandomErasing.forward on a [3, S, S] image
+            ei, ej, eh, ew, _ = self.erase.get_params(torch.empty(3, S, S, device='meta'), scale=self.erase.scale,
+                                                      ratio=self.erase.ratio, value=[float(self.erase.value)])
+            if eh < S:                                   # otherwise get_params gave up: the image is left as it is
+                erase = (ei, ej, eh, ew)
+        return param_row((j, i, w, h), (S, S), (0, 0), flip, op, magnitude, S, erase)
+
+    def __call__(self, img):
+        return np.asarray(img, dtype=np.uint8), self.draw(img)
+
+    def collate(self, batch):
+        return collate_packed(batch, self.size, self.mean, self.std)
+
+
+class DevicePresetEval:
+    """``ClassificationPresetEval`` (Resize, CenterCrop, ToTensor, Normalize) with everything after the decode on the GPU:
+    the image is resized with PIL's arithmetic and the centred window kept, in one pass.  No random draw."""
+
+    def __init__(self, crop_size, resize_size=256, mean=(0.485, 0.456, 0.406), std=(0.229, 0.224, 0.225), interpolation=None):
+        _bilinear_only(interpolation)
+        self.size, self.mean, self.std = _square(crop_size), tuple(mean), tuple(std)
+        self.resize_size = [resize_size] if isinstance(resize_size, int) else list(resize_size)
+
+    def draw(self, img):
+        from torchvision.transforms.functional import _compute_resized_output_size
+        from .ops_augment import param_row
+        W, H = img.size
+        vh, vw = _compute_resized_output_size((H, W), self.resize_size, None)      # F.resize's output size
+        S = self.size
+        # F.center_crop: pad to the crop if the image is smaller, then the offset int(round((size - S) / 2))
+        pad_l, pad_t = ((S - vw) // 2 if S > vw else 0), ((S - vh) // 2 if S > vh else 0)
+        left = int(round((max(vw, S) - S) / 2.0)) - pad_l
+        top = int(round((max(vh, S) - S) / 2.0)) - pad_t
+        return param_row((0, 0, W, H), (vw, vh), (left, top))
+
+    def __call__(self, img):
+        return np.asarray(img, dtype=np.uint8), self.draw(img)
+
+    def collate(self, batch):
+        return collate_packed(batch, self.size, self.mean, self.std)
+
+
+def collate_packed(batch, size, mean, std):
+    """FGDataset items whose 'img' is a device preset's (uint8 array, parameter row) -> {'img': PackedImages, 'label'
+    [, 'id']}: the images back to back in one uint8 buffer (pinned by the DataLoader) with their offset, size and
+    parameter tables."""
+    from .ops_augment import pack
+    out = {'img': pack([b['img'][0] for b in batch], [b['img'][1] for b in batch], size, mean, std),
+           'label': torch.as_tensor(np.array([b['label'] for b in batch])).long()}
+    if 'id' in batch[0]:
+        out['id'] = torch.as_tensor([b['id'] for b in batch])
+    return out
 
 
 def _grid_cells(image, cols, rows):

@@ -11,7 +11,7 @@ which LR schedule — the step itself is ``Trainer.batch_training``.
 import os
 import sys
 
-from .train import PeerLearningTrainer, Trainer, _Cosine, _MultiStep, _Plateau, _Step, warmup_cosine_args
+from .train import PeerLearningTrainer, Trainer, _Cosine, _MultiStep, _Plateau, _Step, device_collate, warmup_cosine_args
 
 
 def _warmup_cosine(opt, config, total_epoch):
@@ -42,7 +42,7 @@ def _balanced_loaders(trainer, config):
         np.random.seed((trainer.config.experiment.seed if 'seed' in trainer.config.experiment else 0) + trainer.rank)
     sampler = BalancedBatchSampler(trainer.datasets['train'], config.n_classes, config.n_samples)
     loaders['train'] = DataLoader(trainer.datasets['train'], num_workers=config.num_workers, pin_memory=True,
-                                  batch_sampler=sampler)
+                                  batch_sampler=sampler, collate_fn=loaders['train'].collate_fn)
     return loaders
 
 
@@ -193,6 +193,7 @@ class DCLTrainer(Trainer):
         from .data import DCLDataset, collate_fn4train, collate_fn4val
         t = config.transformer
         tf = self.get_transformers(t)
+        device_collate(t, tf, type(self).__name__)              # the jigsaw presets stay on the host: rejects device: cuda
         swap = t.swap_num if 'swap_num' in t else [7, 7]
         mc = self.config.model
         return self.rank_loaders(config, {s: DCLDataset(config.root_dir, os.path.join(config.meta_dir, s + '.txt'),

@@ -14,7 +14,8 @@ import torch
 from . import _lib
 from .config import setup_config
 from .registry import MODEL
-from .train import AverageMeter, accuracy, prediction
+from .ops_augment import PackedImages
+from .train import AverageMeter, accuracy, prediction, transformer_device
 from .utils import load_state_dict
 
 IMAGENET_MEAN, IMAGENET_STD = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)      # test.py:84, dataset/transforms.py:18-19
@@ -59,12 +60,20 @@ class Tester:
         from torch.utils.data import DataLoader
         from torchvision import transforms
         t = config.transformer
+        if transformer_device(t) == 'cuda':             # decode on the host, the rest of the preset on the GPU
+            from .data import DevicePresetEval
+            tf = DevicePresetEval(crop_size=t.image_size, resize_size=t.resize_size, mean=IMAGENET_MEAN, std=IMAGENET_STD)
+            ds = FGDataset(config.root_dir, os.path.join(config.meta_dir, 'val.txt'), transform=tf)
+            return DataLoader(ds, config.batch_size, num_workers=config.num_workers, pin_memory=True, shuffle=False,
+                              collate_fn=tf.collate)
         tf = transforms.Compose([transforms.Resize(size=t.resize_size), transforms.CenterCrop(size=t.image_size),
                                  transforms.ToTensor(), transforms.Normalize(mean=IMAGENET_MEAN, std=IMAGENET_STD)])
         ds = FGDataset(config.root_dir, os.path.join(config.meta_dir, 'val.txt'), transform=tf)   # test.py:91-93
         return DataLoader(ds, config.batch_size, num_workers=config.num_workers, pin_memory=True, shuffle=False)
 
     def to_device(self, m, parallel=False):
+        if isinstance(m, PackedImages):                 # a batch of the device eval preset: its model input
+            return m.to(self.device, non_blocking=True).images()
         return m.to(self.device, non_blocking=True) if isinstance(m, torch.Tensor) else m.to(self.device)
 
     def get_model_module(self, model=None):

@@ -16,6 +16,7 @@ import torch
 
 from . import engine, ops
 from .config import setup_config
+from .ops_augment import PackedImages, augment
 from .registry import MODEL
 from .utils import load_state_dict
 
@@ -74,6 +75,26 @@ def prediction(model, outputs):
     return model.prediction(outputs) if hasattr(model, 'prediction') else outputs
 
 
+def transformer_device(config):
+    """'cuda' when a ``dataset.transformer`` config asks for the device presets (``device: cuda``), None when it has no
+    ``device`` key (the host presets)."""
+    device = config['device'] if 'device' in config else None
+    if device not in (None, 'cuda'):
+        raise ValueError(f"dataset.transformer.device must be 'cuda' or absent, not {device!r}")
+    return device
+
+
+def device_collate(config, transforms, who):
+    """{split: collate function} of the device presets in ``transforms`` when the transformer config asks for them, None
+    otherwise.  A trainer that builds its own presets keeps them on the host, so the key is an error there."""
+    if transformer_device(config) is None:
+        return None
+    if not all(hasattr(t, 'collate') for t in transforms.values()):
+        raise ValueError(f'dataset.transformer.device: cuda covers the default presets only; {who} builds its own, which '
+                         'run on the host')
+    return {s: t.collate for s, t in transforms.items()}
+
+
 def warmup_cosine_args(config, total_epoch):
     """-> (T_max, warmup_epochs, lr_warmup_decay) of a scheduler config, each with its default."""
     return (config['T_max'] if 'T_max' in config else total_epoch,
@@ -125,12 +146,18 @@ class Trainer:
         return model
 
     def get_transformers(self, config):
-        """{'train', 'val'} transforms of the ``dataset.transformer`` config."""
+        """{'train', 'val'} transforms of the ``dataset.transformer`` config.  With ``device: cuda`` these are the device
+        presets of ``hawkeye_b200.data``: the workers decode and draw, and ``stage_inputs`` runs the rest on the GPU."""
+        resize = config['resize_size'] if 'resize_size' in config else int(config['image_size'] / 0.875)
+        if transformer_device(config) == 'cuda':
+            from .data import DevicePresetTrain, DevicePresetEval
+            return {'train': DevicePresetTrain(crop_size=config['image_size'], auto_augment_policy='ta_wide',
+                                               random_erase_prob=0.1),
+                    'val': DevicePresetEval(crop_size=config['image_size'], resize_size=resize)}
         try:        # inside a Hawkeye checkout: the reference's own classes; otherwise the mirror in hawkeye_b200.data
             from dataset.transforms import ClassificationPresetTrain, ClassificationPresetEval
         except Exception:
             from .data import ClassificationPresetTrain, ClassificationPresetEval
-        resize = config['resize_size'] if 'resize_size' in config else int(config['image_size'] / 0.875)
         return {'train': ClassificationPresetTrain(crop_size=config['image_size'], auto_augment_policy='ta_wide',
                                                    random_erase_prob=0.1),
                 'val': ClassificationPresetEval(crop_size=config['image_size'], resize_size=resize)}
@@ -142,7 +169,8 @@ class Trainer:
             from .data import FGDataset
         tf = self.get_transformers(config.transformer)
         return self.rank_loaders(config, {s: FGDataset(config.root_dir, os.path.join(config.meta_dir, s + '.txt'),
-                                                       transform=tf[s]) for s in ('train', 'val')})
+                                                       transform=tf[s]) for s in ('train', 'val')},
+                                 collate_fn=device_collate(config.transformer, tf, type(self).__name__))
 
     def rank_loaders(self, config, datasets, collate_fn=None):
         """{'train', 'val'} loaders of this rank over ``datasets``; ``collate_fn`` maps a split to its collate function.
@@ -207,6 +235,9 @@ class Trainer:
         return _Cosine(self.optimizer, T_max, config.eta_min if 'eta_min' in config else 0.0, warmup_epochs, warmup_decay)
 
     def to_device(self, m, parallel=False):
+        """A tensor or module on the trainer's device; a packed batch of the device presets becomes its model input."""
+        if isinstance(m, PackedImages):
+            return m.to(self.device, non_blocking=True).images()
         return m.to(self.device, non_blocking=True) if isinstance(m, torch.Tensor) else m.to(self.device)
 
     def get_model_module(self, model=None):
@@ -227,6 +258,8 @@ class Trainer:
         labels is a tuple when ``batch_tensors`` gives one, each target with its own buffer in the slot."""
         img, lab = self.batch_tensors(data)
         labs = lab if isinstance(lab, tuple) else (lab,)
+        if isinstance(img, PackedImages):
+            return self.stage_packed(img, lab, labs)
         if img.is_cuda and all(t.is_cuda for t in labs):
             return img, lab, None
         key = (tuple(img.shape), img.dtype) + tuple((tuple(t.shape), t.dtype) for t in labs)
@@ -248,6 +281,47 @@ class Trainer:
             ev = torch.cuda.Event()
             ev.record()
         cur.wait_event(ev)
+        return slot['img'], (tuple(slot['lab']) if isinstance(lab, tuple) else slot['lab'][0]), slot
+
+    def stage_packed(self, packed, lab, labs):
+        """``stage_inputs`` of a packed batch of the device presets: the packed images and their tables are copied on the
+        copy stream into a ring slot whose byte buffer grows to the largest batch seen, then the augment kernels write
+        the slot's fp32 image buffer on the compute stream.  A graph-replayed step copies from that buffer into its static
+        input afterwards, as it does for any staged batch."""
+        N, S = len(packed), packed.size
+        key = ('packed', N, S) + tuple((tuple(t.shape), t.dtype) for t in labs)
+        ring = self._in_ring.get(key)
+        dev = self.device
+        if ring is None:
+            ring = self._in_ring[key] = dict(i=0, slots=[dict(
+                src=torch.empty(0, dtype=torch.uint8, device=dev),
+                offsets=torch.empty(N, dtype=torch.int64, device=dev), sizes=torch.empty(N, 2, dtype=torch.int32, device=dev),
+                params=torch.empty(packed.params.shape, dtype=torch.float64, device=dev),
+                work=torch.empty(N, S, S, 3, dtype=torch.uint8, device=dev),
+                lut=torch.empty(N, 3, 256, dtype=torch.uint8, device=dev),
+                img=torch.empty(N, 3, S, S, dtype=torch.float32, device=dev),
+                lab=[torch.empty(t.shape, dtype=t.dtype, device=dev) for t in labs], free=None) for _ in range(3)])
+        slot = ring['slots'][ring['i'] % 3]
+        ring['i'] += 1
+        cur = torch.cuda.current_stream()
+        nbytes = packed.data.numel()
+        grown = slot['src'].numel() < nbytes
+        if grown:       # allocated on the compute stream: the copy stream must not write it before that stream's earlier work
+            slot['src'] = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            self.copy_stream.wait_stream(cur)
+        with torch.cuda.stream(self.copy_stream):
+            if slot['free'] is not None:
+                self.copy_stream.wait_event(slot['free'])
+            slot['src'][:nbytes].copy_(packed.data, non_blocking=True)
+            for k in ('offsets', 'sizes', 'params'):
+                slot[k].copy_(getattr(packed, k), non_blocking=True)
+            for d, t in zip(slot['lab'], labs):
+                d.copy_(t, non_blocking=True)
+            ev = torch.cuda.Event()
+            ev.record()
+        cur.wait_event(ev)
+        augment(slot['src'], slot['offsets'], slot['sizes'], slot['params'], S, packed.mean, packed.std, out=slot['img'],
+                work=slot['work'], lut=slot['lut'])
         return slot['img'], (tuple(slot['lab']) if isinstance(lab, tuple) else slot['lab'][0]), slot
 
     # ---- CUDA-graph replay of forward + loss + backward (+ gradient all-reduce) ----------------------------------------

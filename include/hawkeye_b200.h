@@ -653,6 +653,25 @@ int hk_stem_dgrad(const float* dc, const float* w, float* dx, int N, int H, int 
 int hk_normalize_u8(const unsigned char* x_nhwc, float* y_nchw, int N, int H, int W, float mean0, float mean1, float mean2,
                     float std0, float std1, float std2, void* stream);
 
+/* ---- input side: the default train / eval presets (dataset/transforms.py ClassificationPresetTrain: RandomResizedCrop,
+ * flip, TrivialAugmentWide, ToTensor, Normalize, RandomErasing; ClassificationPresetEval: Resize, CenterCrop, ToTensor,
+ * Normalize) on the GPU.  The input is a ragged batch of N decoded RGB images: uint8 HWC, image n at byte offsets[n] of
+ * src with sizes[n] = (H, W).  params [N, hk_augment_params_cols()] (double) holds each image's draws, made on the host
+ * (hawkeye_b200/ops_augment.py documents the columns).  Three launches, in order:
+ * hk_augment_crop_resize: -> img [N,S,S,3] uint8, the source box resized to the virtual size with PIL's BILINEAR
+ *   arithmetic (bit-identical to Image.resize), the S x S window kept, mirrored on request.  A box outside its image gives
+ *   a zero image.
+ * hk_augment_stats: img -> lut [N,3,256] uint8, the tables of the images whose op is Contrast, AutoContrast or Equalize
+ *   (one block per image; the others' rows are not written).
+ * hk_augment_apply: img, lut -> y [N,3,S,S] fp32 = the image's TrivialAugmentWide op, then (x/255 - mean_c)/std_c as
+ *   hk_normalize_u8 computes it, 0 inside the erasing rectangle. */
+int hk_augment_params_cols(void);
+int hk_augment_crop_resize(const unsigned char* src, const long long* offsets, const int* sizes, const double* params,
+                           unsigned char* img, int N, int S, void* stream);
+int hk_augment_stats(const unsigned char* img, const double* params, unsigned char* lut, int N, int S, void* stream);
+int hk_augment_apply(const unsigned char* img, const double* params, const unsigned char* lut, float* y, int N, int S,
+                     float mean0, float mean1, float mean2, float std0, float std1, float std2, void* stream);
+
 /* ---- optimizers over flat fp32 buffers: torch.optim.SGD (Examples/BCNN.py:40), Adam (Examples/MPN.py:14-18) */
 int hk_sgd_momentum(float* p, const float* g, float* buf, size_t n, float lr, float momentum, float weight_decay,
                     float grad_scale, int first_step, void* stream);
