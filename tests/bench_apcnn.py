@@ -12,38 +12,16 @@ and power limit are read in the same run.  A stock-PyTorch restatement of the re
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import torch
+
+from benchutil import card, timed
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 sys.path.insert(0, os.path.join(REPO, 'tests'))
 HBM_BYTES_PER_S = 3.35e12        # H100 SXM data sheet
-
-
-def card():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power, clock = [s.strip() for s in q.split(',')]
-        return dict(gpu=name, power_limit=power, max_sm_clock=clock)
-    except Exception as e:
-        return dict(gpu=torch.cuda.get_device_name(), power_limit=f'not read ({e})')
-
-
-def timed(fn, steps, warmup):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(steps):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / steps
 
 
 def kernel_bytes(N, H3, C2=512):

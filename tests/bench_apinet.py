@@ -15,6 +15,8 @@ import numpy as np
 import torch
 import torch.nn as nn
 
+from benchutil import timed
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, 'tests'))
@@ -107,19 +109,6 @@ class StockLoss(nn.Module):
         idx = torch.arange(s.shape[0], device=s.device)
         ss, so = torch.softmax(s, 1)[idx, t], torch.softmax(o, 1)[idx, t]
         return self.ce(torch.cat([s, o]), torch.cat([t, t])) + self.rank(ss, so, torch.ones_like(ss))
-
-
-def timed(step, steps, warmup):
-    for _ in range(warmup):
-        step()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(steps):
-        step()
-    b.record()
-    b.synchronize()
-    return a.elapsed_time(b) / steps
 
 
 def gpu_info():

@@ -13,9 +13,7 @@ power limit are read in the same run.
 import argparse
 import json
 import os
-import subprocess
 import sys
-import warnings
 
 import torch
 import torch.nn as nn
@@ -25,29 +23,7 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 sys.path.insert(0, os.path.join(REPO, 'tests'))
 import cin_inputs as I  # noqa: E402
-
-
-def card():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power, clock = [s.strip() for s in q.split(',')]
-        return dict(gpu=name, power_limit=power, max_sm_clock=clock)
-    except Exception as e:
-        return dict(gpu=torch.cuda.get_device_name(), power_limit=f'not read ({e})')
-
-
-def timed(fn, steps, warmup):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(steps):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / steps
+from benchutil import card, count_syncs, timed  # noqa: E402
 
 
 # ---- the stock-PyTorch restatement of the reference (model/methods/CIN.py, model/loss/CIN_loss.py, Examples/CIN.py) -------
@@ -111,18 +87,6 @@ def stock_step(x, y, steps, warmup):
     torch.cuda.empty_cache()
     torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
     return round(ms, 3), syncs, round(head_ms, 3)
-
-
-def count_syncs(fn):
-    torch.cuda.synchronize()
-    with warnings.catch_warnings(record=True) as w:
-        warnings.simplefilter('always')
-        torch.cuda.set_sync_debug_mode('warn')
-        try:
-            fn()
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
-    return sum('synchroniz' in str(m.message) for m in w)
 
 
 def trunk_map():

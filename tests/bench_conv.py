@@ -15,7 +15,6 @@ NVIDIA's H100 SXM data-sheet dense TF32 figure, not a measured peak.
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -24,42 +23,10 @@ sys.path.insert(0, os.path.join(ROOT, 'tests'))
 
 import torch  # noqa: E402
 
+from benchutil import device_line, time_call  # noqa: E402
+from fp64_refs import BATCH, VGG16_LAYERS  # noqa: E402
+
 DATASHEET_TF32 = 495.0
-BATCH = 32
-# (name, H = W, Cin, Cout, max-pool follows)
-VGG16_LAYERS = [('conv1_2', 448, 64, 64, True),
-                ('conv2_1', 224, 64, 128, False), ('conv2_2', 224, 128, 128, True),
-                ('conv3_1', 112, 128, 256, False), ('conv3_2', 112, 256, 256, False), ('conv3_3', 112, 256, 256, True),
-                ('conv4_1', 56, 256, 512, False), ('conv4_2', 56, 512, 512, False), ('conv4_3', 56, 512, 512, True),
-                ('conv5_1', 28, 512, 512, False), ('conv5_2', 28, 512, 512, False), ('conv5_3', 28, 512, 512, True)]
-
-
-def device_line():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
-                           capture_output=True, text=True, timeout=60).stdout.strip().splitlines()[0]
-    except (OSError, IndexError, subprocess.SubprocessError) as e:
-        q = f'nvidia-smi unavailable ({e!r})'
-    return f'device: {q}'
-
-
-def time_call(fn, min_ms):
-    """ms per call: CUDA events over a window of at least min_ms, after warm-up"""
-    for _ in range(3):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    fn()
-    e1.record()
-    e1.synchronize()
-    n = max(3, int(min_ms / max(e0.elapsed_time(e1), 1e-3)) + 1)
-    e0.record()
-    for _ in range(n):
-        fn()
-    e1.record()
-    e1.synchronize()
-    return e0.elapsed_time(e1) / n
 
 
 def per_layer(args, out):

@@ -18,7 +18,8 @@ sys.path.insert(0, os.path.join(ROOT, 'tests'))
 
 import torch  # noqa: E402
 
-from bench_conv import BATCH, VGG16_LAYERS, device_line, time_call  # noqa: E402
+from benchutil import device_line, time_call  # noqa: E402
+from fp64_refs import BATCH, VGG16_LAYERS  # noqa: E402
 
 
 def fused(args):

@@ -20,10 +20,11 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from benchutil import card, count_syncs, timed
+
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 sys.path.insert(0, os.path.join(REPO, 'tests'))
-from bench_cin import card, count_syncs, timed  # noqa: E402
 
 N, P, K, GAMMA = 8, 2, 200, (0.5, 0.25, 0.5)
 HBM = 3.35e12

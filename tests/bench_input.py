@@ -25,10 +25,11 @@ import time
 import numpy as np
 import torch
 
+from benchutil import card, timed
+
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 sys.path.insert(0, os.path.join(REPO, 'tests'))
-from bench_dcl import card, timed  # noqa: E402
 
 S, RESIZE, BATCH = 448, 512, 32
 HBM_BYTES_PER_S = 3.35e12

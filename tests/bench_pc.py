@@ -18,10 +18,11 @@ import sys
 import torch
 import torch.nn as nn
 
+from benchutil import card, count_syncs, timed
+
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 sys.path.insert(0, os.path.join(REPO, 'tests'))
-from bench_cin import card, count_syncs, timed  # noqa: E402
 
 B, K, LAMBDA = 24, 200, 0.1
 

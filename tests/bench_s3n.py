@@ -18,10 +18,11 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from benchutil import card, timed
+
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 sys.path.insert(0, os.path.join(REPO, 'tests'))
-from bench_dcl import card, timed  # noqa: E402
 
 N, SIZE, K = 8, 448, 200
 

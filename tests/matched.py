@@ -10,15 +10,11 @@ plumbing bug (wrong tap, wrong stride adjoint, missing term) shows up as O(1) wh
 import torch
 import torch.nn.functional as F
 
+from conftest import rel_l2
+from kernel_check import nchw
 
-def rel_l2(a, b):
-    a = torch.as_tensor(a).double().flatten()
-    b = torch.as_tensor(b).double().flatten()
-    return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
-
-
-def _nchw(t):
-    return t.permute(0, 3, 1, 2)
+# rel-L2 tolerance of the gradients by precision mode: single-pass TF32 and 3xTF32 (test_gpu_matched.py)
+TOL = {0: 3e-3, 1: 2e-4}
 
 
 def tape_items(capture):
@@ -27,13 +23,13 @@ def tape_items(capture):
     for rec in capture:
         kind = rec[0]
         if kind == 'relu':
-            items.append(('relu', (_nchw(rec[1]) > 0).cpu()))
+            items.append(('relu', (nchw(rec[1]) > 0).cpu()))
         elif kind == 'pool2':
             # same routing rule as hk_maxpool2x2_bwd and torch: first maximum in scan order
-            _, idx = F.max_pool2d(_nchw(rec[1]).cpu().contiguous(), 2, 2, return_indices=True)
+            _, idx = F.max_pool2d(nchw(rec[1]).cpu().contiguous(), 2, 2, return_indices=True)
             items.append(('pool', idx))
         elif kind == 'pool3':
-            am, (N, H, W, C) = _nchw(rec[1]).cpu().long(), rec[2]
+            am, (N, H, W, C) = nchw(rec[1]).cpu().long(), rec[2]
             Ho, Wo = am.shape[2:]
             hh = 2 * torch.arange(Ho).view(1, 1, Ho, 1) + am // 3 - 1
             ww = 2 * torch.arange(Wo).view(1, 1, 1, Wo) + am % 3 - 1

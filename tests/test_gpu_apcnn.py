@@ -15,23 +15,12 @@ import apcnn_inputs as I
 import detgen
 from conftest import load_golden, rel_l2
 from oracle import apcnn_oracle as O
+from kernel_check import nhwc, precise_on  # noqa: F401  (a fixture)
 
 pytestmark = pytest.mark.gpu
 G = load_golden('reference_apcnn')
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 os.environ['HAWKEYE_ALLOW_RANDOM_INIT'] = '1'
-
-
-@pytest.fixture
-def precise():
-    from hawkeye_b200 import _lib
-    _lib.set_precise(1)
-    yield
-    _lib.set_precise(0)
-
-
-def _nhwc(t):
-    return t.permute(0, 2, 3, 1).contiguous()
 
 
 def _draws(rec, counts):
@@ -107,7 +96,7 @@ def test_attention_against_reference_fixture():
     apn = PyramidAttentions(256)
     apn.load_state_dict(detgen.state_like(apn, seed=11))
     apn.cuda()
-    Fs = [_nhwc(detgen.det((3, 256, s, s), 4200 + s).cuda()).requires_grad_(True) for s in (12, 6, 3)]
+    Fs = [nhwc(detgen.det((3, 256, s, s), 4200 + s).cuda()).requires_grad_(True) for s in (12, 6, 3)]
     gates, pm, v = apn(Fs)
     Gv = torch.stack([detgen.det((3, 256), 4300 + i) for i in range(3)]).cuda()
     (v * Gv).sum().backward()
@@ -147,9 +136,9 @@ def test_refine_matches_reference_fixture():
     from hawkeye_b200 import ops_apcnn
     boxes, counts = _fixture_rois('roi_200')
     b, c = torch.from_numpy(boxes).cuda(), torch.from_numpy(counts).cuda()
-    Gw = _nhwc(detgen.det((I.ROI_BATCH, 8, 28, 28), 4101).cuda())
+    Gw = nhwc(detgen.det((I.ROI_BATCH, 8, 28, 28), 4101).cuda())
     for mode, draws in (('train', _draws(G['refine_draws'], counts)), ('eval', None)):
-        x = _nhwc(detgen.det((I.ROI_BATCH, 8, 28, 28), 4100).cuda()).requires_grad_(True)
+        x = nhwc(detgen.det((I.ROI_BATCH, 8, 28, 28), 4100).cuda()).requires_grad_(True)
         y = ops_apcnn.RefineFn.apply(x, b, c, draws)
         (y * Gw).sum().backward()
         assert (y.detach().permute(0, 3, 1, 2).cpu() - torch.from_numpy(G[f'refine_{mode}_y'])).abs().max() < 5e-5      # fp32 on both sides; values of a few units times a rescale of up to ~2
@@ -231,7 +220,7 @@ def _e2e_step(net, zero_stage2=False):
     return out, loss
 
 
-def test_model_against_fixture(precise):
+def test_model_against_fixture(precise_on):
     """Tolerances as for DCL and NTS-Net: fp32 here (3xTF32 products) against the reference's fp32 CPU run; the trunk's
     gradients pass through two stages of batch-statistics BatchNorm over 4 images and drift the most."""
     net = _shallow()
@@ -254,7 +243,7 @@ def test_model_against_fixture(precise):
         assert rel_l2(sd[k + '.running_var'].cpu(), G[f'e2e_rv_{k}']) < 1e-3, k
 
 
-def test_layer2_receives_gradient_from_stage_two(precise):
+def test_layer2_receives_gradient_from_stage_two(precise_on):
     a = _shallow()
     _e2e_step(a)
     b = _shallow()

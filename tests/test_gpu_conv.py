@@ -6,17 +6,10 @@ import torch.nn.functional as F
 
 import detgen
 from conftest import rel_l2
+from kernel_check import nchw, nhwc
 
 pytestmark = pytest.mark.gpu
 TOL = 2e-3
-
-
-def _nhwc(t):
-    return t.permute(0, 2, 3, 1).contiguous()
-
-
-def _nchw(t):
-    return t.permute(0, 3, 1, 2).contiguous()
 
 
 @pytest.mark.parametrize('N,H,W,Cin,Cout', [(2, 16, 16, 64, 64), (2, 16, 32, 64, 128), (2, 24, 16, 128, 64), (1, 16, 16, 128, 256),
@@ -36,26 +29,26 @@ def test_conv3x3_fwd_dgrad_wgrad(N, H, W, Cin, Cout):
     dpre = dy.double() * (y_ref > 0)
     gx, gw, gb = torch.autograd.grad(y_ref, (xd, wd_, bd), dy.double())
 
-    xg, wg, bg = _nhwc(x).cuda(), w.cuda(), b.cuda()
+    xg, wg, bg = nhwc(x).cuda(), w.cuda(), b.cuda()
     wf = torch.empty(9 * Cout * Cin, device='cuda')
     wdg = torch.empty(9 * Cout * Cin, device='cuda')
     _lib.call('hk_conv3x3_pack_weights', wg, wf, wdg, Cout, Cin, s)
     y = torch.empty(N, H, W, Cout, device='cuda')
     _lib.call('hk_conv3x3_fwd', xg, wf, bg, y, N, H, W, Cin, Cout, 1, s)
     torch.cuda.synchronize()
-    e = rel_l2(_nchw(y).cpu(), y_ref.detach())
+    e = rel_l2(nchw(y).cpu(), y_ref.detach())
     print(f'conv fwd {N}x{H}x{W} {Cin}->{Cout}: {e:.2e}')
     assert e < TOL
-    dpre_g = _nhwc(dpre.float()).cuda()
+    dpre_g = nhwc(dpre.float()).cuda()
     dx = torch.empty(N, H, W, Cin, device='cuda')
     _lib.call('hk_conv3x3_dgrad', dpre_g, wdg, None, dx, N, H, W, Cin, Cout, s)
-    e = rel_l2(_nchw(dx).cpu(), gx)
+    e = rel_l2(nchw(dx).cpu(), gx)
     print(f'conv dgrad: {e:.2e}')
     assert e < TOL
     # fused ReLU mask of the *previous* layer
-    mask = _nhwc(detgen.det((N, Cin, H, W), 9)).cuda()
+    mask = nhwc(detgen.det((N, Cin, H, W), 9)).cuda()
     _lib.call('hk_conv3x3_dgrad', dpre_g, wdg, mask, dx, N, H, W, Cin, Cout, s)
-    assert rel_l2(_nchw(dx).cpu(), gx * (_nchw(mask).cpu() > 0)) < TOL
+    assert rel_l2(nchw(dx).cpu(), gx * (nchw(mask).cpu() > 0)) < TOL
     dw = torch.empty(Cout, Cin, 3, 3, device='cuda')
     db = torch.empty(Cout, device='cuda')
     nb = _lib.query('hk_conv3x3_wgrad_workspace_bytes', Cin, Cout)
@@ -79,11 +72,11 @@ def test_first_layer_and_pool():
     nb0 = _lib.query('hk_conv3x3_first_fwd_workspace_bytes', N, H, W, Cout)
     ws0 = torch.empty(nb0, dtype=torch.uint8, device='cuda')
     _lib.call('hk_conv3x3_first_fwd', x.cuda(), w.cuda(), b.cuda(), y, N, H, W, Cout, ws0, nb0, s)
-    print('first fwd', rel_l2(_nchw(y).cpu(), y_ref.detach()))
-    assert rel_l2(_nchw(y).cpu(), y_ref.detach()) < 1e-3   # fp32 math, tf32-rounded on store
+    print('first fwd', rel_l2(nchw(y).cpu(), y_ref.detach()))
+    assert rel_l2(nchw(y).cpu(), y_ref.detach()) < 1e-3   # fp32 math, tf32-rounded on store
     dy = detgen.det((N, Cout, H, W), 4).double()
     gw, gb = torch.autograd.grad(y_ref, (wd_, bd), dy)
-    dpre = _nhwc((dy * (y_ref > 0)).float()).cuda()
+    dpre = nhwc((dy * (y_ref > 0)).float()).cuda()
     dw = torch.empty(Cout, 3, 3, 3, device='cuda')
     db = torch.empty(Cout, device='cuda')
     nb = _lib.query('hk_conv3x3_first_wgrad_workspace_bytes', N, H, W, Cout)
@@ -100,19 +93,19 @@ def test_first_layer_and_pool():
     p_ref = F.max_pool2d(a, 2, 2)
     g = detgen.det(p_ref.shape, 8).double()
     (ga,) = torch.autograd.grad(p_ref, a, g)
-    ag = _nhwc(a.detach().float()).cuda()
+    ag = nhwc(a.detach().float()).cuda()
     out = torch.empty(N, H // 2, W // 2, 64, device='cuda')
     _lib.call('hk_maxpool2x2_fwd', ag, out, N, H, W, 64, 0, s)
-    assert torch.equal(_nchw(out).cpu().double(), p_ref.detach())
+    assert torch.equal(nchw(out).cpu().double(), p_ref.detach())
     out2 = torch.empty(N, 64, H // 2, W // 2, device='cuda')
     _lib.call('hk_maxpool2x2_fwd', ag, out2, N, H, W, 64, 1, s)
     assert torch.equal(out2.cpu().double(), p_ref.detach())
     dx = torch.empty_like(ag)
-    _lib.call('hk_maxpool2x2_bwd', ag, _nhwc(g.float()).cuda(), dx, N, H, W, 64, 0, s)
+    _lib.call('hk_maxpool2x2_bwd', ag, nhwc(g.float()).cuda(), dx, N, H, W, 64, 0, s)
     ref = ga * (a.detach() > 0)
-    assert rel_l2(_nchw(dx).cpu(), ref) < 1e-6
+    assert rel_l2(nchw(dx).cpu(), ref) < 1e-6
     _lib.call('hk_maxpool2x2_bwd', ag, g.float().cuda(), dx, N, H, W, 64, 1, s)
-    assert rel_l2(_nchw(dx).cpu(), ref) < 1e-6
+    assert rel_l2(nchw(dx).cpu(), ref) < 1e-6
 
 
 @pytest.mark.parametrize('N,H,W,Cin,Cout', [(2, 16, 32, 64, 64),     # v2 kernel, resident weights (VGG conv1_2)

@@ -13,21 +13,17 @@ import time
 import pytest
 import torch
 
-from bench_conv import BATCH
-from test_gpu_conv_vgg16 import (C_TF32_WGRAD, HK_ERR_UNSUPPORTED, _assert_guard, _gen, _guarded, _nhwc, _pack, _randn,
-                                 _tf32, _wgrad_ref, check_bound)
+import detgen
+from fp64_refs import BATCH, C_TF32_WGRAD, gen, pack, randn, wgrad_ref
+from kernel_check import HK_ERR_UNSUPPORTED, abi, assert_guards, c_bound, check, guarded, nhwc, workspace
 
 pytestmark = pytest.mark.gpu
 
 
 def _first_wgrad_fused(dy, wd, mask, x, dw, db, accumulate):
-    from hawkeye_b200 import _lib
     N, H, W, C = dy.shape
-    nb = _lib.query('hk_conv3x3_dgrad_first_wgrad_workspace_bytes')
-    ws = torch.empty(nb, dtype=torch.uint8, device='cuda')
-    _lib.call('hk_conv3x3_dgrad_first_wgrad_acc', dy, wd, mask, x, dw, db, N, H, W, C, C, ws, nb, int(accumulate),
-              _lib.stream_ptr())
-    torch.cuda.synchronize()
+    ws, nb = workspace('hk_conv3x3_dgrad_first_wgrad_workspace_bytes')
+    abi('hk_conv3x3_dgrad_first_wgrad_acc', dy, wd, mask, x, dw, db, N, H, W, C, C, ws, nb, int(accumulate))
 
 
 @pytest.mark.parametrize('N,H,W', [(BATCH, 448, 448),   # the train step
@@ -40,24 +36,24 @@ def test_dgrad_first_wgrad(N, H, W):
     t0 = time.time()
     s = _lib.stream_ptr()
     C = 64
-    g = _gen(5000 + W)
-    x = _tf32(_randn((N, 3, H, W), g))
-    mask = torch.relu(_randn((N, H, W, C), g))            # conv1_1's output: about half the ReLU mask is zero
-    dy = _tf32(_randn((N, H, W, C), g))
-    _, wd = _pack(_randn((C, C, 3, 3), g, (2.0 / (9 * C)) ** 0.5))
+    g = gen(5000 + W)
+    x = detgen.tf32_rna(randn((N, 3, H, W), g))
+    mask = torch.relu(randn((N, H, W, C), g))            # conv1_1's output: about half the ReLU mask is zero
+    dy = detgen.tf32_rna(randn((N, H, W, C), g))
+    _, wd = pack(randn((C, C, 3, 3), g, (2.0 / (9 * C)) ** 0.5))
     # dx1 as the unfused backward stores it
     dx1 = torch.empty(N, H, W, C, device='cuda')
     _lib.call('hk_conv3x3_dgrad', dy, wd, mask, dx1, N, H, W, C, C, s)
-    gw, aw, gb, ab = _wgrad_ref(_nhwc(x), dx1, 3, C)
+    gw, aw, gb, ab = wgrad_ref(nhwc(x), dx1, 3, C)
     names = ('co', 'ci', 'kh', 'kw')
 
-    dw, gd = _guarded((C, 3, 3, 3))
-    db, gdb = _guarded((C,))
+    dw = guarded((C, 3, 3, 3))
+    db = guarded((C,))
     _first_wgrad_fused(dy, wd, mask, x, dw, db, 0)
-    _assert_guard(gd, tag='fused dw1')
-    _assert_guard(gdb, tag='fused db1')
-    rw = check_bound(dw, gw, aw, C_TF32_WGRAD, f'fused dw1 {N}x{H}x{W}', rnd=False, names=names)
-    rb = check_bound(db, gb, ab, C_TF32_WGRAD, f'fused db1 {N}x{H}x{W}', rnd=False, names=('co',))
+    assert_guards(dw, tag='fused dw1')
+    assert_guards(db, tag='fused db1')
+    rw = check(dw, gw, c_bound(aw, C_TF32_WGRAD), f'fused dw1 {N}x{H}x{W}', names=names)
+    rb = check(db, gb, c_bound(ab, C_TF32_WGRAD), f'fused db1 {N}x{H}x{W}', names=('co',))
 
     # the unfused weight gradient of the same dx1: both are within the bound of fp64, so within twice it of each other
     nbd = _lib.query('hk_conv3x3_first_wgrad_direct_workspace_bytes')
@@ -66,30 +62,29 @@ def test_dgrad_first_wgrad(N, H, W):
     dbu = torch.empty(C, device='cuda')
     _lib.call('hk_conv3x3_first_wgrad_direct_acc', x, dx1, dwu, dbu, N, H, W, C, wsd, nbd, 0, s)
     torch.cuda.synchronize()
-    check_bound(dw, dwu, aw, 2 * C_TF32_WGRAD, f'fused dw1 against the unfused pair {N}x{H}x{W}', rnd=False, names=names)
-    check_bound(db, dbu, ab, 2 * C_TF32_WGRAD, f'fused db1 against the unfused pair {N}x{H}x{W}', rnd=False,
-                names=('co',))
+    check(dw, dwu, c_bound(aw, 2 * C_TF32_WGRAD), f'fused dw1 against the unfused pair {N}x{H}x{W}', names=names)
+    check(db, dbu, c_bound(ab, 2 * C_TF32_WGRAD), f'fused db1 against the unfused pair {N}x{H}x{W}', names=('co',))
 
     # deterministic: per-CTA partials reduced in a fixed order
-    dw2, _ = _guarded((C, 3, 3, 3))
-    db2, _ = _guarded((C,))
+    dw2 = guarded((C, 3, 3, 3))
+    db2 = guarded((C,))
     _first_wgrad_fused(dy, wd, mask, x, dw2, db2, 0)
     assert torch.equal(dw2.view(torch.int32), dw.view(torch.int32)) and torch.equal(db2.view(torch.int32),
                                                                                      db.view(torch.int32))
 
-    dw0 = _randn((C, 3, 3, 3), g, float(gw.abs().mean()))
-    db0 = _randn((C,), g, float(gb.abs().mean()))
-    dw, gd = _guarded((C, 3, 3, 3))
-    db, gdb = _guarded((C,))
+    dw0 = randn((C, 3, 3, 3), g, float(gw.abs().mean()))
+    db0 = randn((C,), g, float(gb.abs().mean()))
+    dw = guarded((C, 3, 3, 3))
+    db = guarded((C,))
     dw.copy_(dw0)
     db.copy_(db0)
     _first_wgrad_fused(dy, wd, mask, x, dw, db, 1)
-    _assert_guard(gd, tag='fused dw1 accumulate')
-    _assert_guard(gdb, tag='fused db1 accumulate')
-    rwa = check_bound(dw, dw0.double() + gw, dw0.double().abs() + aw, C_TF32_WGRAD, 'fused dw1 accumulate', rnd=False,
-                      names=names)
-    rba = check_bound(db, db0.double() + gb, db0.double().abs() + ab, C_TF32_WGRAD, 'fused db1 accumulate', rnd=False,
-                      names=('co',))
+    assert_guards(dw, tag='fused dw1 accumulate')
+    assert_guards(db, tag='fused db1 accumulate')
+    rwa = check(dw, dw0.double() + gw, c_bound(dw0.double().abs() + aw, C_TF32_WGRAD),
+                'fused dw1 accumulate', names=names)
+    rba = check(db, db0.double() + gb, c_bound(db0.double().abs() + ab, C_TF32_WGRAD),
+                'fused db1 accumulate', names=('co',))
     print(f'dgrad + first wgrad N={N} {H}x{W}: worst c-term share dw {rw:.3g} db {rb:.3g} accumulate dw {rwa:.3g} '
           f'db {rba:.3g}; {time.time() - t0:.1f} s', flush=True)
 
@@ -137,24 +132,24 @@ def test_dgrad_unpool_bit_exact(N, H, W, Cin, Cout):
     from hawkeye_b200 import _lib
     _lib.set_precise(0)
     s = _lib.stream_ptr()
-    g = _gen(6000 + H + Cin)
+    g = gen(6000 + H + Cin)
     # pre-pool activations with whole windows at or below zero, so that bit 2 of the code is clear in places
-    pre = torch.relu(_randn((N, 2 * H, 2 * W, Cin), g) - 0.8)
+    pre = torch.relu(randn((N, 2 * H, 2 * W, Cin), g) - 0.8)
     pooled = torch.empty(N, H, W, Cin, device='cuda')
     code = torch.empty(N, H, W, Cin, device='cuda', dtype=torch.uint8)
     _lib.call('hk_maxpool2x2_fwd_idx', pre, pooled, code, N, 2 * H, 2 * W, Cin, 0, s)
     del pre, pooled
-    dy = _randn((N, H, W, Cout), g)
-    _, wd = _pack(_randn((Cout, Cin, 3, 3), g, (2.0 / (9 * Cin)) ** 0.5))
+    dy = randn((N, H, W, Cout), g)
+    _, wd = pack(randn((Cout, Cin, 3, 3), g, (2.0 / (9 * Cin)) ** 0.5))
     dx = torch.empty(N, H, W, Cin, device='cuda')
     _lib.call('hk_conv3x3_dgrad', dy, wd, None, dx, N, H, W, Cin, Cout, s)
     ref = torch.empty(N, 2 * H, 2 * W, Cin, device='cuda')
     _lib.call('hk_maxpool2x2_bwd_idx', code, dx, ref, N, 2 * H, 2 * W, Cin, 0, s)
     del dx
-    out, guard = _guarded((N, 2 * H, 2 * W, Cin))
+    out = guarded((N, 2 * H, 2 * W, Cin))
     _lib.call('hk_conv3x3_dgrad_unpool', dy, wd, code, out, N, H, W, Cin, Cout, s)
     torch.cuda.synchronize()
-    _assert_guard(guard, tag='dgrad unpool')
+    assert_guards(out, tag='dgrad unpool')
     ndiff = int((out.view(torch.int32) != ref.view(torch.int32)).sum())
     assert ndiff == 0, f'dgrad unpool differs from dgrad + max-pool backward in {ndiff} of {out.numel()} elements'
     assert int((code & 4 == 0).sum()) > 0 and int((ref != 0).sum()) > 0
@@ -188,7 +183,6 @@ def test_vgg_features_fused_backward_matches_capture_path():
     data gradient at conv2_1 (32x32, 16 x 8 tile), conv3_1 (16x16) and conv4_1 (8x8, 8 x 8 x 2-image tile); conv5_1 (4x4)
     keeps the separate max-pool backward.  The capture path runs the X27 input layer and the unfused conv1_2 data
     gradient, so conv1_1's gradients sum in another order there."""
-    import detgen
     from oracle import hop_oracle as O
     from hawkeye_b200 import _lib, ops
     _lib.set_precise(0)

@@ -7,9 +7,9 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from bench_conv import BATCH
-from test_gpu_conv_vgg16 import (C_TF32, C_TF32_WGRAD, CHUNK, HK_ERR_UNSUPPORTED, _assert_guard, _fp32_exact, _gen,
-                                 _guarded, _nhwc, _randn, _tf32, _wgrad_ref, check_bound)
+import detgen
+from fp64_refs import BATCH, C_TF32, C_TF32_WGRAD, CHUNK, fp32_exact, gen, randn, wgrad_ref
+from kernel_check import HK_ERR_UNSUPPORTED, assert_guards, c_bound, check, guarded, nhwc, rnd_bound
 
 pytestmark = pytest.mark.gpu
 
@@ -23,22 +23,22 @@ def test_first_direct(N, H, W):
     t0 = time.time()
     s = _lib.stream_ptr()
     cout = 64
-    g = _gen(4000 + W)
-    x = _tf32(_randn((N, 3, H, W), g))
-    w = _tf32(_randn((cout, 3, 3, 3), g, 0.2))
-    b = _tf32(_randn((cout,), g, 0.5))
-    y, gy = _guarded((N, H, W, cout))
+    g = gen(4000 + W)
+    x = detgen.tf32_rna(randn((N, 3, H, W), g))
+    w = detgen.tf32_rna(randn((cout, 3, 3, 3), g, 0.2))
+    b = detgen.tf32_rna(randn((cout,), g, 0.5))
+    y = guarded((N, H, W, cout))
     _lib.call('hk_conv3x3_first_fwd_direct', x, w, b, y, N, H, W, cout, s)
     torch.cuda.synchronize()
-    _assert_guard(gy, tag='first fwd direct')
+    assert_guards(y, tag='first fwd direct')
     worst = 0.0
     for n0 in range(0, N, CHUNK):
         xc = x[n0:n0 + CHUNK]
-        ref = _nhwc(F.relu(F.conv2d(xc.double(), w.double(), b.double(), padding=1)))
-        with _fp32_exact():
-            absref = _nhwc(F.conv2d(xc.abs(), w.abs(), b.abs(), padding=1))
-        worst = max(worst, check_bound(y[n0:n0 + CHUNK], ref, absref, C_TF32,
-                                       f'first fwd direct {N}x{H}x{W} [{n0}:{n0 + CHUNK}]', n0=n0))
+        ref = nhwc(F.relu(F.conv2d(xc.double(), w.double(), b.double(), padding=1)))
+        with fp32_exact():
+            absref = nhwc(F.conv2d(xc.abs(), w.abs(), b.abs(), padding=1))
+        worst = max(worst, check(y[n0:n0 + CHUNK], ref, rnd_bound(absref, C_TF32),
+                                 f'first fwd direct {N}x{H}x{W} [{n0}:{n0 + CHUNK}]', n0=n0))
         del ref, absref
     # same operands, same k order, same wgmma shape as the X27 GEMM: the same bits
     nb0 = _lib.query('hk_conv3x3_first_fwd_workspace_bytes', N, H, W, cout)
@@ -50,33 +50,33 @@ def test_first_direct(N, H, W):
     assert ndiff == 0, f'direct forward differs from the X27 forward in {ndiff} elements'
     del y, y27, ws0
 
-    dy = _tf32(_randn((N, H, W, cout), g))
-    gw, aw, gb, ab = _wgrad_ref(_nhwc(x), dy, 3, cout)
+    dy = detgen.tf32_rna(randn((N, H, W, cout), g))
+    gw, aw, gb, ab = wgrad_ref(nhwc(x), dy, 3, cout)
     nb = _lib.query('hk_conv3x3_first_wgrad_direct_workspace_bytes')
     ws = torch.empty(nb, dtype=torch.uint8, device='cuda')
-    dw, gd = _guarded((cout, 3, 3, 3))
-    db, gdb = _guarded((cout,))
+    dw = guarded((cout, 3, 3, 3))
+    db = guarded((cout,))
     _lib.call('hk_conv3x3_first_wgrad_direct_acc', x, dy, dw, db, N, H, W, cout, ws, nb, 0, s)
     torch.cuda.synchronize()
-    _assert_guard(gd, tag='first dw direct')
-    _assert_guard(gdb, tag='first db direct')
+    assert_guards(dw, tag='first dw direct')
+    assert_guards(db, tag='first db direct')
     names = ('co', 'ci', 'kh', 'kw')
-    rw = check_bound(dw, gw, aw, C_TF32_WGRAD, f'first wgrad direct dw {N}x{H}x{W}', rnd=False, names=names)
-    rb = check_bound(db, gb, ab, C_TF32_WGRAD, f'first wgrad direct db {N}x{H}x{W}', rnd=False, names=('co',))
-    dw0 = _randn((cout, 3, 3, 3), g, float(gw.abs().mean()))
-    db0 = _randn((cout,), g, float(gb.abs().mean()))
-    dw, gd = _guarded((cout, 3, 3, 3))
-    db, gdb = _guarded((cout,))
+    rw = check(dw, gw, c_bound(aw, C_TF32_WGRAD), f'first wgrad direct dw {N}x{H}x{W}', names=names)
+    rb = check(db, gb, c_bound(ab, C_TF32_WGRAD), f'first wgrad direct db {N}x{H}x{W}', names=('co',))
+    dw0 = randn((cout, 3, 3, 3), g, float(gw.abs().mean()))
+    db0 = randn((cout,), g, float(gb.abs().mean()))
+    dw = guarded((cout, 3, 3, 3))
+    db = guarded((cout,))
     dw.copy_(dw0)
     db.copy_(db0)
     _lib.call('hk_conv3x3_first_wgrad_direct_acc', x, dy, dw, db, N, H, W, cout, ws, nb, 1, s)
     torch.cuda.synchronize()
-    _assert_guard(gd, tag='first dw direct accumulate')
-    _assert_guard(gdb, tag='first db direct accumulate')
-    rwa = check_bound(dw, dw0.double() + gw, dw0.double().abs() + aw, C_TF32_WGRAD, 'first wgrad direct dw accumulate',
-                      rnd=False, names=names)
-    rba = check_bound(db, db0.double() + gb, db0.double().abs() + ab, C_TF32_WGRAD, 'first wgrad direct db accumulate',
-                      rnd=False, names=('co',))
+    assert_guards(dw, tag='first dw direct accumulate')
+    assert_guards(db, tag='first db direct accumulate')
+    rwa = check(dw, dw0.double() + gw, c_bound(dw0.double().abs() + aw, C_TF32_WGRAD),
+                'first wgrad direct dw accumulate', names=names)
+    rba = check(db, db0.double() + gb, c_bound(db0.double().abs() + ab, C_TF32_WGRAD),
+                'first wgrad direct db accumulate', names=('co',))
     print(f'first layer direct N={N} {H}x{W}: worst c-term share fwd {worst:.3g} dw {rw:.3g} db {rb:.3g} accumulate dw '
           f'{rwa:.3g} db {rba:.3g}; {time.time() - t0:.1f} s', flush=True)
 
@@ -103,7 +103,6 @@ def test_vgg_features_direct_first_layer_matches_x27_path():
     """All 26 parameter gradients of VGGFeaturesFn with the direct input layer (the training path) against the X27 path
     (taken under activation capture).  The forward is bit-identical; the backward differs only where the weight
     gradients sum in another order."""
-    import detgen
     from oracle import hop_oracle as O
     from hawkeye_b200 import _lib, ops
     _lib.set_precise(0)

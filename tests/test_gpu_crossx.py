@@ -13,6 +13,7 @@ import crossx_inputs as I
 import detgen
 from conftest import load_golden, rel_l2
 from oracle import crossx_oracle as O
+from kernel_check import precise  # noqa: F401  (a fixture)
 
 pytestmark = pytest.mark.gpu
 G = load_golden('reference_crossx')
@@ -23,14 +24,6 @@ os.environ['HAWKEYE_ALLOW_RANDOM_INIT'] = '1'
 TOL = 1e-5
 DX_TOL = {0: 5e-4, 1: 1e-5}
 TRUNK_TOL_PRECISE = 2e-4
-
-
-@pytest.fixture
-def precise(request):
-    from hawkeye_b200 import _lib
-    _lib.set_precise(request.param)
-    yield request.param
-    _lib.set_precise(0)
 
 
 def _call(name, *args):

@@ -11,18 +11,11 @@ import torch
 import detgen
 from conftest import load_golden, rel_l2
 from oracle import dcl_oracle as D
+from kernel_check import precise  # noqa: F401  (a fixture)
 
 pytestmark = pytest.mark.gpu
 G = load_golden('reference_dcl')
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture(params=[0, 1], ids=['tf32', 'precise'])
-def precise(request):
-    from hawkeye_b200 import _lib
-    _lib.set_precise(request.param)
-    yield request.param
-    _lib.set_precise(0)
 
 
 @pytest.mark.parametrize('N', [2, 16])

@@ -6,25 +6,10 @@ import torch.nn.functional as F
 
 import detgen
 from conftest import rel_l2
+from kernel_check import nchw, nhwc, precise  # noqa: F401  (a fixture)
 
 pytestmark = pytest.mark.gpu
 TOL = {0: 2e-3, 1: 1e-4}     # single-pass TF32 operands / 3xTF32, fp32 accumulate
-
-
-@pytest.fixture(params=[0, 1], ids=['tf32', 'precise'])
-def precise(request):
-    from hawkeye_b200 import _lib
-    _lib.set_precise(request.param)
-    yield request.param
-    _lib.set_precise(0)
-
-
-def _nhwc(t):
-    return t.permute(0, 2, 3, 1).contiguous()
-
-
-def _nchw(t):
-    return t.permute(0, 3, 1, 2).contiguous()
 
 
 def _check_conv(fn, k, N, H, W, cin, cout, bias, grad_x, grad_w, tol):
@@ -37,16 +22,16 @@ def _check_conv(fn, k, N, H, W, cin, cout, bias, grad_x, grad_w, tol):
     ref = F.conv2d(xd, wd, bd, padding=k // 2)
     ref.backward(g.double())
 
-    xg = _nhwc(x).cuda().requires_grad_(grad_x)
+    xg = nhwc(x).cuda().requires_grad_(grad_x)
     wg = w.cuda().requires_grad_(grad_w)
     bg = b.cuda().requires_grad_(True) if bias else None
     y = fn(xg, wg, bg)
-    y.backward(_nhwc(g).cuda())
+    y.backward(nhwc(g).cuda())
     assert y.shape == (N, H, W, cout)
-    assert rel_l2(_nchw(y.detach()).cpu(), ref.detach()) < tol
+    assert rel_l2(nchw(y.detach()).cpu(), ref.detach()) < tol
     assert (xg.grad is not None) == grad_x and (wg.grad is not None) == grad_w
     if grad_x:
-        assert rel_l2(_nchw(xg.grad).cpu(), xd.grad) < tol
+        assert rel_l2(nchw(xg.grad).cpu(), xd.grad) < tol
     if grad_w:
         assert rel_l2(wg.grad.cpu(), wd.grad) < tol
     if bias:

@@ -19,23 +19,15 @@ import torch
 
 import detgen
 import matched
+from matched import TOL
 from conftest import rel_l2
+from kernel_check import precise  # noqa: F401  (a fixture)
 
 pytestmark = pytest.mark.gpu
-
-TOL = {0: 3e-3, 1: 2e-4}
 
 
 class Cfg(dict):
     __getattr__ = dict.__getitem__
-
-
-@pytest.fixture
-def precision(request):
-    from hawkeye_b200 import _lib
-    _lib.set_precise(request.param)
-    yield request.param
-    _lib.set_precise(0)
 
 
 @pytest.fixture(scope='module')
@@ -75,8 +67,8 @@ def _mpn():
     return net.cuda().train(), state
 
 
-@pytest.mark.parametrize('size,precision', [(64, 1), (448, 0), (448, 1)], indirect=['precision'])
-def test_bcnn_s2_all_gradients(size, precision):
+@pytest.mark.parametrize('size,precise', [(64, 1), (448, 0), (448, 1)], indirect=['precise'])
+def test_bcnn_s2_all_gradients(size, precise):
     from oracle import hop_oracle as O
     torch.set_num_threads(16)
     net, state = _bcnn()
@@ -85,14 +77,14 @@ def test_bcnn_s2_all_gradients(size, precision):
     ref_logits, ref_loss, ref = matched.oracle_step(lambda xx, st, nl: O.bcnn_forward(xx, st, 2, nl=nl), x, labels, state,
                                                     items, grads.keys())
     e = rel_l2(logits, ref_logits)
-    print(f'bcnn {size} precise={precision}: logits rel {e:.2e} loss {loss:.6f} vs {ref_loss:.6f}')
+    print(f'bcnn {size} precise={precise}: logits rel {e:.2e} loss {loss:.6f} vs {ref_loss:.6f}')
     assert len(grads) == 28 and e < 1e-3 and abs(loss - ref_loss) < 1e-4
-    matched.compare_grads(grads, ref, TOL[precision], f'bcnn_s2 {size}x{size} precise={precision}')
+    matched.compare_grads(grads, ref, TOL[precise], f'bcnn_s2 {size}x{size} precise={precise}')
 
 
-@pytest.mark.parametrize('precision', [0, 1], indirect=True)
+@pytest.mark.parametrize('precise', [0, 1], indirect=True)
 @pytest.mark.parametrize('size,d', [(128, 8192), (448, 8192), (448, 6000)])
-def test_cbcnn_all_gradients(size, d, precision):
+def test_cbcnn_all_gradients(size, d, precise):
     from oracle import hop_oracle as O
     torch.set_num_threads(16)
     net, state = _cbcnn(d)
@@ -101,14 +93,14 @@ def test_cbcnn_all_gradients(size, d, precision):
     ref_logits, ref_loss, ref = matched.oracle_step(lambda xx, st, nl: O.cbcnn_forward(xx, st, d, 2, nl=nl), x, labels,
                                                     state, items, grads.keys())
     e = rel_l2(logits, ref_logits)
-    print(f'cbcnn {size} d={d} precise={precision}: logits rel {e:.2e} loss {loss:.6f} vs {ref_loss:.6f}')
+    print(f'cbcnn {size} d={d} precise={precise}: logits rel {e:.2e} loss {loss:.6f} vs {ref_loss:.6f}')
     assert len(grads) == 28 and e < 1e-3 and abs(loss - ref_loss) < 1e-4
-    matched.compare_grads(grads, ref, TOL[precision], f'cbcnn {size}x{size} d={d} precise={precision}')
+    matched.compare_grads(grads, ref, TOL[precise], f'cbcnn {size}x{size} d={d} precise={precise}')
 
 
-@pytest.mark.parametrize('precision', [1], indirect=True)
+@pytest.mark.parametrize('precise', [1], indirect=True)
 @pytest.mark.parametrize('size,B', [(128, 4), (448, 2)])
-def test_mpn_all_gradients(size, B, precision):
+def test_mpn_all_gradients(size, B, precise):
     """A random-weight train-mode ResNet-50 amplifies a perturbation of its input ~170x by the last block (measured in fp64),
     so single-pass TF32 (5e-4 per layer) cannot track ANY reference run of it; the 3xTF32 mode can.
     fp32 itself is only reproducible to ~2e-4 here (fp32 vs fp64 oracle on the same branch), hence the looser bound."""
@@ -120,9 +112,9 @@ def test_mpn_all_gradients(size, B, precision):
     ref_logits, ref_loss, ref = matched.oracle_step(lambda xx, st, nl: O.mpn_forward(xx, st, 5, nl=nl), x, labels, state,
                                                     items, grads.keys())
     e = rel_l2(logits, ref_logits)
-    print(f'mpn {size} B={B} precise={precision}: logits rel {e:.2e} loss {loss:.6f} vs {ref_loss:.6f}')
+    print(f'mpn {size} B={B} precise={precise}: logits rel {e:.2e} loss {loss:.6f} vs {ref_loss:.6f}')
     assert len(grads) == len(list(net.parameters()))
-    errs = matched.compare_grads(grads, ref, 1e-3, f'mpn {size}x{size} precise={precision}')
+    errs = matched.compare_grads(grads, ref, 1e-3, f'mpn {size}x{size} precise={precise}')
     assert e < 1e-3 and abs(loss - ref_loss) < 1e-4, (e, errs)
 
 
@@ -164,9 +156,9 @@ def _check_fixture(tag, ref448, logits, loss, grads, tol=1e-3):
     assert errs and not bad, bad
 
 
-@pytest.mark.parametrize('precision', [1], indirect=True)
+@pytest.mark.parametrize('precise', [1], indirect=True)
 @pytest.mark.parametrize('stage', [1, 2])
-def test_bcnn_448_vs_reference(stage, precision, ref448):
+def test_bcnn_448_vs_reference(stage, precise, ref448):
     net, _ = _bcnn(stage)
     x, labels = detgen.det((2, 3, 448, 448), 41), detgen.det_labels(2, 200, 42)
     logits, loss, grads, _ = matched.gpu_step(net, x, labels)
@@ -175,9 +167,9 @@ def test_bcnn_448_vs_reference(stage, precision, ref448):
         assert set(grads) == {'classifier.weight', 'classifier.bias'}
 
 
-@pytest.mark.parametrize('precision', [1], indirect=True)
+@pytest.mark.parametrize('precise', [1], indirect=True)
 @pytest.mark.parametrize('d', [8192, 6000])
-def test_cbcnn_448_vs_reference(d, precision, ref448):
+def test_cbcnn_448_vs_reference(d, precise, ref448):
     """Logits, loss and the classifier gradients at 1e-3.  The backbone gradients pass through the signed square root
     d/dv = 1/(2 sqrt(|v|+1e-10)) of 2*d sketch bins: a relative perturbation eps of the Gram changes them by ~1000 eps
     (tests/diag/cbp_sensitivity.py: 3e-7 -> 3e-4), and the tensor core's truncating fp32 accumulation leaves ~2e-5 in
@@ -197,8 +189,8 @@ def test_cbcnn_448_vs_reference(d, precision, ref448):
     assert max(errs.values()) < 5e-2
 
 
-@pytest.mark.parametrize('precision', [1], indirect=True)
-def test_mpn_448_vs_reference(precision, ref448):
+@pytest.mark.parametrize('precise', [1], indirect=True)
+def test_mpn_448_vs_reference(precise, ref448):
     net, _ = _mpn()
     x, labels = detgen.det((2, 3, 448, 448), 51), detgen.det_labels(2, 200, 52)
     logits, loss, grads, _ = matched.gpu_step(net, x, labels)
@@ -209,9 +201,9 @@ def test_mpn_448_vs_reference(precision, ref448):
 # 224x224 inputs: 7x7 feature maps, H*W = 49 is not a multiple of 4 (the reference's stock MPN / CBCNN / PeerLearning
 # configs).  The pooling heads zero-pad the map to a 16-byte row pitch; results must be those of the reference.
 # ------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize('precision', [0, 1], indirect=True)
+@pytest.mark.parametrize('precise', [0, 1], indirect=True)
 @pytest.mark.parametrize('model', ['bcnn_s2', 'cbcnn_6000', 'mpn'])
-def test_224_vs_reference(model, precision, ref224):
+def test_224_vs_reference(model, precise, ref224):
     if model == 'bcnn_s2':
         net, _ = _bcnn(2)
         x, labels = detgen.det((2, 3, 224, 224), 41), detgen.det_labels(2, 200, 42)
@@ -224,10 +216,10 @@ def test_224_vs_reference(model, precision, ref224):
     logits, loss, grads, _ = matched.gpu_step(net, x, labels)
     e = rel_l2(logits, ref224[f'{model}_logits'])
     eb = rel_l2(grads['classifier.bias'], ref224[f'{model}_g_classifier.bias'])
-    print(f'{model} 224 precise={precision}: logits rel {e:.2e} loss {loss:.6f} vs {float(ref224[f"{model}_loss"]):.6f} '
+    print(f'{model} 224 precise={precise}: logits rel {e:.2e} loss {loss:.6f} vs {float(ref224[f"{model}_loss"]):.6f} '
           f'classifier.bias grad {eb:.2e}')
-    if model == 'mpn' and not precision:
+    if model == 'mpn' and not precise:
         return        # single-pass TF32 cannot track a random-weight train-mode ResNet-50 (see test_mpn_all_gradients)
-    assert e < 1e-3 and abs(loss - float(ref224[f'{model}_loss'])) < 1e-4 and eb < (2e-3 if not precision else 1e-3)
-    if precision:
+    assert e < 1e-3 and abs(loss - float(ref224[f'{model}_loss'])) < 1e-4 and eb < (2e-3 if not precise else 1e-3)
+    if precise:
         _check_fixture(model, ref224, logits, loss, grads) if model != 'cbcnn_6000' else None

@@ -14,19 +14,12 @@ import detgen
 import mge_inputs as I
 from conftest import load_golden, rel_l2
 from oracle import mge_oracle as O
+from kernel_check import precise_on  # noqa: F401  (a fixture)
 
 pytestmark = pytest.mark.gpu
 G = load_golden('reference_mge')
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 os.environ['HAWKEYE_ALLOW_RANDOM_INIT'] = '1'
-
-
-@pytest.fixture
-def precise():
-    from hawkeye_b200 import _lib
-    _lib.set_precise(1)
-    yield
-    _lib.set_precise(0)
 
 
 def _cfg(**kw):
@@ -35,7 +28,7 @@ def _cfg(**kw):
 
 
 @pytest.mark.parametrize('N,H', [(1, 14), (3, 14), (1, 28), (5, 28)])
-def test_part_head_against_fp64(N, H, precise):
+def test_part_head_against_fp64(N, H, precise_on):
     from hawkeye_b200 import ops_mge
     torch.manual_seed(N * H)
     O_ = 40
@@ -154,7 +147,7 @@ def _e2e_inputs():
     return x, labels
 
 
-def test_model_against_fixture(precise):
+def test_model_against_fixture(precise_on):
     """Tolerances as for AP-CNN: fp32 here (3xTF32 products) against the reference's fp32 CPU run; the trunks' gradients
     pass through batch-statistics BatchNorm over 4 images and drift the most."""
     from hawkeye_b200.losses import MGECNNLoss

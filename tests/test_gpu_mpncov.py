@@ -7,19 +7,12 @@ import torch
 
 import detgen
 from conftest import rel_l2
+from kernel_check import precise  # noqa: F401  (a fixture)
 
 pytestmark = pytest.mark.gpu
 
 PATTERN = 0x7FA5A5A5   # guard words around the outputs (a NaN payload)
 GUARD = 64
-
-
-@pytest.fixture(params=[0, 1], ids=['tf32', 'precise'])
-def precise(request):
-    from hawkeye_b200 import _lib
-    _lib.set_precise(request.param)
-    yield request.param
-    _lib.set_precise(0)
 
 
 def _guarded(n):

@@ -1,6 +1,7 @@
 """The Fast MPN-COV head of the mpn train step, element by element against fp64: hk_covpool_fwd / _bwd, hk_sqrtm_fwd /
 _bwd and hk_triuvec_fwd / _bwd at the batch-32, 448x448 shapes (and the 224x224 batch-8 shape of the reference config),
-the dimension-reduction unit in front of them, the classifier behind them, and the composed head through autograd.
+the classifier behind them, and the composed head through autograd.  The dimension-reduction unit in front of them is
+checked with the other ResNet-50 units (test_gpu_resnet50_units.py).
 
 Every kernel is called through the C ABI into NaN-filled outputs followed by guard words, with NaN-filled workspaces of
 exactly the queried size and a NaN-filled `saved` buffer of exactly hk_sqrtm_saved_floats floats, also followed by
@@ -51,8 +52,7 @@ of each c over it:
 Of the whole bound (fixed + c * scale), the worst element took 0.80 in covpool dx, 0.48 in cov, 0.37 in sqrtm y and 0.31
 in sqrtm dx; xc's bound is its rounding on store, which any element just below a rounding midpoint nearly fills (0.997).
 
-The dimension-reduction unit (1x1, 2048 -> 256, train-mode BN, ReLU at 14x14) runs through test_gpu_resnet50_units's
-_check_unit with that file's constants.  The composed head's rel-L2 to the fp64 composition is printed and loosely bounded:
+The composed head's rel-L2 to the fp64 composition is printed and loosely bounded:
 it measures how the chain amplifies the trunk's TF32 rounding, not a kernel's error.
 
 The self-tests (no GPU) compute defects in fp64 at a small shape, round them to fp32, and check that the loosest bounds
@@ -68,18 +68,13 @@ import pytest
 import torch
 
 import detgen
-from test_gpu_conv_vgg16 import _assert_guard, _guarded, bound_of, check_bound
-from test_gpu_resnet50_units import _check_unit
+from fp64_refs import C_LIN, classifier_inputs, linear_refs, linear_splits
+from kernel_check import (PAIR, RND, TRUNC, U, Bound, Out, Worst, abi, c_bound, check, guarded, poisoned, rnd_bound,
+                          workspace)
 
-U = 2.0 ** -24
-RND = 2.0 ** -11
-TRUNC = 2.0 ** -10
-PAIR = 2.0 ** -22
 EPI = 4 * U
 C_COV = 2.0 ** -20
 C_NS = 2.0 ** -19
-C_LIN = 2.0 ** -19
-CONSTS = {'C_COV': C_COV, 'C_NS': C_NS, 'C_LIN': C_LIN}
 CHUNK = 8
 F64 = torch.float64
 
@@ -92,7 +87,6 @@ CASES = {
     'b37_7x7': (37, 256, 7, 7, 2, 0),           # 296 tiles; B % 4 != 0 pads normA; iterN = 2: empty Newton-Schulz loops
     'precise_b4_14x14': (4, 256, 14, 14, 5, 1),
 }
-DR_UNIT = ('pool.conv_dr_block', '1x1', 14, 2048, 256, True, False)
 F_CLS, N_CLS = 256 * 257 // 2, 200
 
 
@@ -279,44 +273,6 @@ def triuvec_bwd64(g, n):
     return dx
 
 
-def linear_splits(F):
-    """hk_linear_fwd's K slices (head.cu)"""
-    S = min(max(F // 1024, 1), 512)
-    while F % S or (F // S) % 4:
-        S -= 1
-        if S <= 1:
-            return 1
-    return S
-
-
-def classifier_inputs(B, F, N, seed, device):
-    """tf32 x, w, dy and an fp32 bias; the last 4 columns of every K slice of x and w (a partial k-block: 1028 = 32 x 32
-    + 4) are 16x larger, so that leaving them out cannot hide"""
-    g = torch.Generator(device=device).manual_seed(seed)
-    S = linear_splits(F)
-    x = torch.relu(torch.randn(B, F, generator=g, device=device))
-    w = torch.randn(N, F, generator=g, device=device) * F ** -0.5
-    tail = torch.zeros(F, dtype=torch.bool, device=device)
-    for s in range(S):
-        tail[(s + 1) * (F // S) - 4:(s + 1) * (F // S)] = True
-    x[:, tail] *= 16
-    w[:, tail] *= 16
-    b = torch.randn(N, generator=g, device=device) * 0.1
-    dy = torch.randn(B, N, generator=g, device=device) * 0.01
-    return detgen.tf32_rna(x), detgen.tf32_rna(w), b, detgen.tf32_rna(dy), S
-
-
-def linear_refs(x, w, b, dy, S):
-    """fp64 y, dx, dw, db and their (fixed, scale) bounds"""
-    xd, wd, bd, dd = (t.to(F64) for t in (x, w, b, dy))
-    sy = xd.abs() @ wd.abs().T + bd.abs()
-    out = {'y': (xd @ wd.T + bd, (S + 1) * U * sy, sy),
-           'dx': (dd @ wd, 0 * xd, dd.abs() @ wd.abs()),
-           'dw': (dd.T @ xd, 0 * wd, dd.abs().T @ xd.abs())}
-    out['db'] = (dd.sum(0), 2.0 ** -19 * dd.abs().sum(0), dd.abs().sum(0))
-    return out
-
-
 # ------------------------------------------------------------------------------------------------------------------
 # 2. inputs and checks
 # ------------------------------------------------------------------------------------------------------------------
@@ -337,43 +293,8 @@ def upstream(B, n, seed):
     return detgen.det((B, n * (n + 1) // 2, 1), seed)
 
 
-WORST = {}
-
-
-def check_c(const, tag, out, ref, fixed, scale, names):
-    """|out - ref| <= fixed + c * scale for every element; prints and records the worst share of c * scale that the error
-    beyond `fixed` takes"""
-    c = CONSTS[const]
-    o = out.to(F64)
-    excess = ((o - ref).abs() - fixed).clamp_min(0)
-    share = torch.where(excess == 0, torch.zeros_like(excess), excess / (c * scale))
-    share = float(torch.nan_to_num(share, nan=math.inf).max())
-    print(f'{tag}: share of {const} = 2^{math.log2(c):.0f} taken {share:.3g}', flush=True)
-    if share > WORST.get(const, (-1.0, ''))[0]:
-        WORST[const] = (share, tag)
-    check_bound(o, ref, None, None, tag, bound=fixed + c * scale, names=names)
-    return share
-
-
-def _input(t):
-    """a device copy of t followed by 16 KB of NaN"""
-    buf, _ = _guarded(t.shape, guard=float('nan'))
-    buf.copy_(t)
-    return buf
-
-
-def _ws(query, *args):
-    from hawkeye_b200 import _lib
-    nb = int(_lib.query(query, *args))
-    assert nb % 4 == 0
-    w, g = _guarded((nb // 4,))
-    return w, g, nb
-
-
-def _call(name, *args):
-    from hawkeye_b200 import _lib
-    _lib.call(name, *args, _lib.stream_ptr())
-    torch.cuda.synchronize()
+WORST = Worst(C_COV=C_COV, C_NS=C_NS, C_LIN=C_LIN)
+check_c = WORST.check_c
 
 
 def pair_tiles_per_cta(B, n, sms):
@@ -390,38 +311,17 @@ def run_head(case, seed=300):
     from hawkeye_b200 import _lib
     B, C, H, W, iterN, precise = CASES[case]
     M, Mp, L = H * W, pad4(H * W), C * (C + 1) // 2
-    _lib.set_precise(precise)
-    try:
-        x = _input(feature_map(B, C, H, W, seed).cuda())
-        gv = _input(upstream(B, C, seed + 2).cuda())
-        cov, gc = _guarded((B, C, C))
-        xc, gxc = _guarded((B, C, Mp))
-        _call('hk_covpool_fwd', x, cov, xc, B, C, M)
-        _assert_guard(gc, tag='covpool cov')
-        _assert_guard(gxc, tag='covpool xc')
-        y, gy = _guarded((B, C, C))
-        saved, gs = _guarded((int(_lib.query('hk_sqrtm_saved_floats', B, C, iterN)),))
-        ws, gw, nb = _ws('hk_sqrtm_fwd_workspace_bytes', B, C)
-        _call('hk_sqrtm_fwd', cov, y, saved, B, C, iterN, ws, nb)
-        for gg, t in ((gy, 'sqrtm y'), (gs, 'sqrtm saved'), (gw, 'sqrtm fwd workspace')):
-            _assert_guard(gg, tag=t)
-        v, gvv = _guarded((B, L, 1))
-        _call('hk_triuvec_fwd', y, v, B, C)
-        _assert_guard(gvv, tag='triuvec y')
-        g, gg_ = _guarded((B, C, C))
-        _call('hk_triuvec_bwd', gv, g, B, C)
-        _assert_guard(gg_, tag='triuvec dx')
-        gx, ggx = _guarded((B, C, C))
-        ws, gw, nb = _ws('hk_sqrtm_bwd_workspace_bytes', B, C)
-        _call('hk_sqrtm_bwd', cov, y, g, saved, gx, B, C, iterN, ws, nb)
-        _assert_guard(ggx, tag='sqrtm dx')
-        _assert_guard(gw, tag='sqrtm bwd workspace')
-        _assert_guard(gs, tag='sqrtm saved (backward)')
-        dx, gdx = _guarded((B, C, M))
-        _call('hk_covpool_bwd', xc, gx, dx, B, C, M)
-        _assert_guard(gdx, tag='covpool dx')
-    finally:
-        _lib.set_precise(0)
+    x = poisoned(feature_map(B, C, H, W, seed).cuda())
+    gv = poisoned(upstream(B, C, seed + 2).cuda())
+    cov, xc = abi('hk_covpool_fwd', x, Out((B, C, C)), Out((B, C, Mp)), B, C, M, precise=precise)
+    saved = guarded((int(_lib.query('hk_sqrtm_saved_floats', B, C, iterN)),))
+    ws, nb = workspace('hk_sqrtm_fwd_workspace_bytes', B, C)
+    (y,) = abi('hk_sqrtm_fwd', cov, Out((B, C, C)), saved, B, C, iterN, ws, nb, precise=precise)
+    (v,) = abi('hk_triuvec_fwd', y, Out((B, L, 1)), B, C, precise=precise)
+    (g,) = abi('hk_triuvec_bwd', gv, Out((B, C, C)), B, C, precise=precise)
+    ws, nb = workspace('hk_sqrtm_bwd_workspace_bytes', B, C)
+    (gx,) = abi('hk_sqrtm_bwd', cov, y, g, saved, Out((B, C, C)), B, C, iterN, ws, nb, precise=precise)
+    (dx,) = abi('hk_covpool_bwd', xc, gx, Out((B, C, M)), B, C, M, precise=precise)
     return dict(x=x, gv=gv, cov=cov, xc=xc, y=y, v=v, g=g, gx=gx, dx=dx)
 
 
@@ -463,8 +363,9 @@ def test_head_stages(case):
         tag = f'{case} [{n0}:{min(n0 + CHUNK, B)}]'
         ref, xc64, e_s, fixed, S = covpool_fwd_bounds(x[sl], precise)
         xo = xc[sl, :, :M]
-        rb = bound_of(xo, xc64, e_s.expand_as(xc64), 1.0, rnd=not precise) + 2 * U * torch.fmax(xo.abs(), xc64.abs())
-        check_bound(xo, xc64, None, None, f'{tag} covpool xc', bound=rb, n0=n0, names=('image', 'channel', 'pos'))
+        rb = (c_bound if precise else rnd_bound)(e_s.expand_as(xc64), 1.0).total(xo, xc64) + \
+            2 * U * torch.fmax(xo.abs(), xc64.abs())
+        check(xo, xc64, rb, f'{tag} covpool xc', names=('image', 'channel', 'pos'), n0=n0)
         check_c('C_COV', f'{tag} covpool cov', cov[sl], ref, fixed, S, nm)
         del ref, xc64, fixed, S
         chain = Chain(C, 'cuda')
@@ -475,16 +376,7 @@ def test_head_stages(case):
         del sv, yr, ey, gr, eg
         ref, fixed, scale = covpool_bwd_bounds(xc[sl, :, :M], gx[sl], M, precise)
         check_c('C_COV', f'{tag} covpool dx', dx[sl], ref, fixed, scale, ('image', 'channel', 'pos'))
-    print(f'{case}: {time.time() - t0:.1f} s; worst shares so far: ' +
-          ', '.join(f'{k} {v:.3g} ({t})' for k, (v, t) in sorted(WORST.items())), flush=True)
-
-
-@pytest.mark.gpu
-def test_dr_unit_b32():
-    """the dimension-reduction unit of the mpn step at 448x448 batch 32, TF32 train mode, with the units file's bounds"""
-    from hawkeye_b200 import _lib
-    _lib.set_precise(0)
-    _check_unit('tf32-448-b32', DR_UNIT, 6000)
+    print(f'{case}: {time.time() - t0:.1f} s; worst shares so far: ' + WORST.summary(), flush=True)
 
 
 @pytest.mark.gpu
@@ -496,23 +388,17 @@ def test_classifier_b32():
     B, F, N = 32, F_CLS, N_CLS
     x, w, b, dy, S = classifier_inputs(B, F, N, 400, 'cuda')
     assert S == 32 and F // S == 1028
-    xi, wi, bi, dyi = (_input(t) for t in (x, w, b, dy))
-    ws, gw, nb = _ws('hk_linear_fwd_workspace_bytes', B, F, N)
-    y, gy = _guarded((B, N))
-    _call('hk_linear_fwd', xi, wi, bi, y, B, F, N, ws, nb)
-    dx, gdx = _guarded((B, F))
-    _call('hk_linear_dgrad', dyi, wi, dx, B, F, N)
-    dw, gdw = _guarded((N, F))
-    db, gdb = _guarded((N,))
-    _call('hk_linear_wgrad', dyi, xi, dw, db, B, F, N)
-    for gg, t in ((gw, 'linear workspace'), (gy, 'y'), (gdx, 'dx'), (gdw, 'dw'), (gdb, 'db')):
-        _assert_guard(gg, tag=t)
+    xi, wi, bi, dyi = (poisoned(t) for t in (x, w, b, dy))
+    ws, nb = workspace('hk_linear_fwd_workspace_bytes', B, F, N)
+    (y,) = abi('hk_linear_fwd', xi, wi, bi, Out((B, N)), B, F, N, ws, nb)
+    (dx,) = abi('hk_linear_dgrad', dyi, wi, Out((B, F)), B, F, N)
+    dw, db = abi('hk_linear_wgrad', dyi, xi, Out((N, F)), Out((N,)), B, F, N)
     refs = linear_refs(x, w, b, dy, S)
     for key, out, names in (('y', y, ('image', 'class')), ('dx', dx, ('image', 'feature')),
                             ('dw', dw, ('class', 'feature')), ('db', db, ('class',))):
         ref, fixed, scale = refs[key]
         if key == 'db':
-            check_bound(out, ref, None, None, 'classifier db', bound=fixed, names=names)
+            check(out, ref, fixed, 'classifier db', names=names)
         else:
             check_c('C_LIN', f'classifier {key}', out, ref, fixed, scale, names)
 
@@ -572,34 +458,34 @@ def test_composed_head_b32():
     logits.backward(dlogits)
     assert torch.equal(logits, logits_m) and torch.equal(xs.grad, dx_m), 'the staged path differs from the module'
     with torch.no_grad():
-        cov, _ = _guarded((B, C, C))
-        xc, _ = _guarded((B, C, pad4(M)))
-        _call('hk_covpool_fwd', h.contiguous(), cov, xc, B, C, M)
+        cov = guarded((B, C, C))
+        xc = guarded((B, C, pad4(M)))
+        abi('hk_covpool_fwd', h.contiguous(), cov, xc, B, C, M)
         assert torch.equal(cov, c), 'CovpoolFn forward differs from hk_covpool_fwd'
-        dh, _ = _guarded((B, C, H, H))
-        _call('hk_covpool_bwd', xc, c.grad.contiguous(), dh, B, C, M)
+        dh = guarded((B, C, H, H))
+        abi('hk_covpool_bwd', xc, c.grad.contiguous(), dh, B, C, M)
         assert torch.equal(dh, h.grad), 'CovpoolFn backward differs from hk_covpool_bwd'
-        y, _ = _guarded((B, C, C))
-        saved, _ = _guarded((int(_lib.query('hk_sqrtm_saved_floats', B, C, 5)),))
-        ws, _, nb = _ws('hk_sqrtm_fwd_workspace_bytes', B, C)
-        _call('hk_sqrtm_fwd', c, y, saved, B, C, 5, ws, nb)
+        y = guarded((B, C, C))
+        saved = guarded((int(_lib.query('hk_sqrtm_saved_floats', B, C, 5)),))
+        ws, nb = workspace('hk_sqrtm_fwd_workspace_bytes', B, C)
+        abi('hk_sqrtm_fwd', c, y, saved, B, C, 5, ws, nb)
         assert torch.equal(y, s), 'SqrtmFn forward differs from hk_sqrtm_fwd'
-        gc, _ = _guarded((B, C, C))
-        ws, _, nb = _ws('hk_sqrtm_bwd_workspace_bytes', B, C)
-        _call('hk_sqrtm_bwd', c, y, s.grad.contiguous(), saved, gc, B, C, 5, ws, nb)
+        gc = guarded((B, C, C))
+        ws, nb = workspace('hk_sqrtm_bwd_workspace_bytes', B, C)
+        abi('hk_sqrtm_bwd', c, y, s.grad.contiguous(), saved, gc, B, C, 5, ws, nb)
         assert torch.equal(gc, c.grad), 'SqrtmFn backward differs from hk_sqrtm_bwd'
-        v, _ = _guarded((B, L, 1))
-        _call('hk_triuvec_fwd', s, v, B, C)
+        v = guarded((B, L, 1))
+        abi('hk_triuvec_fwd', s, v, B, C)
         assert torch.equal(v, t), 'TriuvecFn forward differs from hk_triuvec_fwd'
-        gs, _ = _guarded((B, C, C))
-        _call('hk_triuvec_bwd', t.grad.contiguous(), gs, B, C)
+        gs = guarded((B, C, C))
+        abi('hk_triuvec_bwd', t.grad.contiguous(), gs, B, C)
         assert torch.equal(gs, s.grad), 'TriuvecFn backward differs from hk_triuvec_bwd'
-        ws, _, nb = _ws('hk_linear_fwd_workspace_bytes', B, L, N_CLS)
-        lo, _ = _guarded((B, N_CLS))
-        _call('hk_linear_fwd', t, w, b, lo, B, L, N_CLS, ws, nb)
+        ws, nb = workspace('hk_linear_fwd_workspace_bytes', B, L, N_CLS)
+        lo = guarded((B, N_CLS))
+        abi('hk_linear_fwd', t, w, b, lo, B, L, N_CLS, ws, nb)
         assert torch.equal(lo, logits), 'LinearFn forward differs from hk_linear_fwd'
-        gt, _ = _guarded((B, L))
-        _call('hk_linear_dgrad', dlogits, w, gt, B, L, N_CLS)
+        gt = guarded((B, L))
+        abi('hk_linear_dgrad', dlogits, w, gt, B, L, N_CLS)
         assert torch.equal(gt.view(B, L, 1), t.grad), 'LinearFn backward differs from hk_linear_dgrad'
     assert bool(torch.isfinite(logits).all()) and bool(torch.isfinite(xs.grad).all())
     # the fp64 composition
@@ -648,7 +534,7 @@ def test_restatement_matches_oracle(iterN):
 def _rejected(tag, bad, ref, fixed, scale, c, rnd=False):
     """the fp32-rounded defect violates fixed + c * scale (+ the tf32 rounding where the kernel rounds) -> worst ratio"""
     out = bad.float().to(F64)
-    bound = fixed + bound_of(out, ref, scale, c, rnd)
+    bound = fixed + Bound(c * scale.double(), rounded=rnd).total(out, ref)
     err = (out - ref).abs()
     r = float(torch.where(err == 0, torch.zeros_like(err), err / bound).max())
     print(f'defect {tag}: worst |err| / bound {r:.3g}', flush=True)

@@ -15,18 +15,11 @@ import detgen
 import nts_inputs
 from conftest import load_golden, rel_l2
 from oracle import nts_oracle as O
+from kernel_check import precise_on  # noqa: F401  (a fixture)
 
 pytestmark = pytest.mark.gpu
 G = load_golden('reference_nts')
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture
-def precise():
-    from hawkeye_b200 import _lib
-    _lib.set_precise(1)
-    yield
-    _lib.set_precise(0)
 
 
 def _net(seed_state=True, **kw):
@@ -83,7 +76,7 @@ def test_crop_matches_interpolate(B, T):
 
 
 @pytest.mark.parametrize('B,H', [(1, 7), (4, 7), (3, 14)])
-def test_proposal_head_fwd_bwd(precise, B, H):
+def test_proposal_head_fwd_bwd(precise_on, B, H):
     from hawkeye_b200.methods.nts import ProposalNet, edge_anchors
     torch.manual_seed(B + H)
     pn = ProposalNet().cuda()
@@ -120,7 +113,7 @@ def test_rank_loss_fwd_bwd(B, T):
     assert (prob.grad.cpu().double() - p64.grad).abs().max() < 1e-6
 
 
-def test_model_against_fixture(precise):
+def test_model_against_fixture(precise_on):
     from hawkeye_b200.losses import NTSLoss
     from hawkeye_b200.cfgnode import CfgNode
     net = _net()

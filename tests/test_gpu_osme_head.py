@@ -74,16 +74,16 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 import detgen
-from test_gpu_conv_vgg16 import _assert_guard, _guarded, check_bound
-from test_gpu_mpncov_head import (CONSTS, PAIR, U, WORST, _call, _input, _ws, check_c, classifier_inputs, linear_refs,
-                                  linear_splits)
+from conftest import rel_l2
+from fp64_refs import C_LIN, classifier_inputs, linear_refs, linear_splits
+from kernel_check import PAIR, U, Worst, abi, check, guarded, poisoned, workspace
 
 EPI = 4 * U
-C_LIN = CONSTS['C_LIN']
 C_LONGK = 2.0 ** -18
 C_GRAM = 2.0 ** -15
 C_NP = 2.0 ** -19
-CONSTS.update(C_LONGK=C_LONGK, C_GRAM=C_GRAM, C_NP=C_NP)
+WORST = Worst(C_LIN=C_LIN, C_LONGK=C_LONGK, C_GRAM=C_GRAM, C_NP=C_NP)
+check_c = WORST.check_c
 F64 = torch.float64
 ROWS = 128            # output features per fp64 reference chunk of the attention FCs
 SGD_CHUNK = 1 << 25   # parameters per fp64 reference chunk of the optimizer step
@@ -275,19 +275,17 @@ def run_linear(x, w, b, dy, precise):
     N = w.shape[0]
     _lib.set_precise(precise)
     try:
-        ws, gw, nb = _ws('hk_linear_fwd_workspace_bytes', B, Fi, N)
+        ws, nb = workspace('hk_linear_fwd_workspace_bytes', B, Fi, N)
         assert nb == linear_splits(Fi) * B * N * 4
-        y, gy = _guarded((B, N))
-        _call('hk_linear_fwd', x, w, b, y, B, Fi, N, ws, nb)
-        dx, gdx = _guarded((B, Fi))
-        _call('hk_linear_dgrad', dy, w, dx, B, Fi, N)
-        dw, gdw = _guarded((N, Fi))
-        db, gdb = _guarded((N,))
-        _call('hk_linear_wgrad', dy, x, dw, db, B, Fi, N)
+        y = guarded((B, N))
+        abi('hk_linear_fwd', x, w, b, y, B, Fi, N, ws, nb)
+        dx = guarded((B, Fi))
+        abi('hk_linear_dgrad', dy, w, dx, B, Fi, N)
+        dw = guarded((N, Fi))
+        db = guarded((N,))
+        abi('hk_linear_wgrad', dy, x, dw, db, B, Fi, N)
     finally:
         _lib.set_precise(0)
-    for gg, t in ((gw, 'linear workspace'), (gy, 'y'), (gdx, 'dx'), (gdw, 'dw'), (gdb, 'db')):
-        _assert_guard(gg, tag=t)
     return y, dx, dw, db
 
 
@@ -307,7 +305,7 @@ def check_linear(tag, x, w, b, dy, out, precise):
             ref, fixed, scale = refs[key]
             check_c(c, f'{tag} {key} [features {r0}:{rs.stop}]', o, ref, fixed + extra * scale, scale, names)
         ref, fixed, _ = refs['db']
-        check_bound(db[rs], ref, None, None, f'{tag} db [{r0}:{rs.stop}]', bound=fixed, names=('feature',))
+        check(db[rs], ref, fixed, f'{tag} db [{r0}:{rs.stop}]', names=('feature',))
         ref, _, scale = refs['dx']
         dx_ref = ref if dx_ref is None else dx_ref + ref
         dx_scale = scale if dx_scale is None else dx_scale + scale
@@ -319,7 +317,7 @@ def check_linear(tag, x, w, b, dy, out, precise):
 def _report(tag, t0):
     peak = torch.cuda.max_memory_allocated() / 2 ** 30
     print(f'{tag}: {time.time() - t0:.1f} s, peak device memory {peak:.2f} GiB; worst shares so far: ' +
-          ', '.join(f'{k} {v:.3g} ({t})' for k, (v, t) in sorted(WORST.items())), flush=True)
+          WORST.summary(), flush=True)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -333,51 +331,45 @@ def test_row_mean_and_gate(case):
     t0 = time.time()
     B, C, H = CASES[case][:3]
     HW, R = H * H, B * C
-    x = _input(trunk_map(B, C, HW, 800).reshape(R, HW))
-    y, gy = _guarded((R,))
-    _call('hk_row_mean_fwd', x, y, R, HW, HW)
-    _assert_guard(gy, tag='row mean y')
+    x = poisoned(trunk_map(B, C, HW, 800).reshape(R, HW))
+    y = guarded((R,))
+    abi('hk_row_mean_fwd', x, y, R, HW, HW)
     ref, bound = row_mean_bound(x, HW)
-    check_bound(y, ref, None, None, f'{case} row mean (cols {HW})', bound=bound, names=('row',))
-    dy = _input(detgen.det((R,), 801).cuda())
-    dx, gdx = _guarded((R, HW))
-    _call('hk_row_mean_bwd', dy, dx, R, HW, HW)
-    _assert_guard(gdx, tag='row mean dx')
+    check(y, ref, bound, f'{case} row mean (cols {HW})', names=('row',))
+    dy = poisoned(detgen.det((R,), 801).cuda())
+    dx = guarded((R, HW))
+    abi('hk_row_mean_bwd', dy, dx, R, HW, HW)
     assert torch.equal(dx, (dy.to(F64) / HW).float()[:, None].expand(R, HW)), 'row mean dx is not the fp32 dy / cols'
     # the gate: typical m, then channels where g saturates at both ends, and rows whose ds is zero
     m = detgen.det((R,), 802, 2.0)
     for k, v in enumerate((60.0, -60.0, 30.0, -30.0, 15.0, -15.0)):
         m[k::97] = v
-    m = _input(m.cuda())
+    m = poisoned(m.cuda())
     ds = detgen.det((R, HW), 803, 1e-3)
     ds[7::61] = 0
-    ds = _input(ds.cuda())
-    s, gs = _guarded((R, HW))
-    _call('hk_se_gate_fwd', x, m, s, R, HW)
-    dxg, gdxg = _guarded((R, HW))
-    dm, gdm = _guarded((R,))
-    _call('hk_se_gate_bwd', x, m, ds, dxg, dm, R, HW)
-    for gg, t in ((gs, 'gate s'), (gdxg, 'gate dx'), (gdm, 'gate dm')):
-        _assert_guard(gg, tag=t)
+    ds = poisoned(ds.cuda())
+    s = guarded((R, HW))
+    abi('hk_se_gate_fwd', x, m, s, R, HW)
+    dxg = guarded((R, HW))
+    dm = guarded((R,))
+    abi('hk_se_gate_bwd', x, m, ds, dxg, dm, R, HW)
     (sr, sb), (dxr, dxb), (dmr, dmb) = se_gate_bounds(x, m, ds, HW)
-    check_bound(s, sr, None, None, f'{case} gate s', bound=sb, names=('row', 'pos'))
-    check_bound(dxg, dxr, None, None, f'{case} gate dx', bound=dxb, names=('row', 'pos'))
-    check_bound(dm, dmr, None, None, f'{case} gate dm', bound=dmb, names=('row',))
+    check(s, sr, sb, f'{case} gate s', names=('row', 'pos'))
+    check(dxg, dxr, dxb, f'{case} gate dx', names=('row', 'pos'))
+    check(dm, dmr, dmb, f'{case} gate dm', names=('row',))
     assert not bool(dm[7::61].view(torch.int32).any()) and not bool(dxg[7::61].view(torch.int32).any()), \
         'rows with ds = 0 did not get +0.0'
     # the bottleneck ReLU on [B, 128], with zeros, -0.0 and negatives
     a = detgen.det((B, C // RATIO), 804)
     a[:, ::5] = 0.0
     a[:, 1::7] = -0.0
-    a = _input(a.cuda())
-    h, gh = _guarded(a.shape)
-    _call('hk_act_fwd', a, h, a.numel(), 0)
+    a = poisoned(a.cuda())
+    h = guarded(a.shape)
+    abi('hk_act_fwd', a, h, a.numel(), 0)
     torch.cuda.synchronize()
-    da = _input(detgen.det(a.shape, 805).cuda())
-    dh, gdh = _guarded(a.shape)
-    _call('hk_act_bwd', h, da, dh, a.numel(), 0)
-    for gg, t in ((gh, 'relu y'), (gdh, 'relu dx')):
-        _assert_guard(gg, tag=t)
+    da = poisoned(detgen.det(a.shape, 805).cuda())
+    dh = guarded(a.shape)
+    abi('hk_act_bwd', h, da, dh, a.numel(), 0)
     zero = torch.zeros((), device='cuda')
     assert torch.equal(h.view(torch.int32), torch.where(a > 0, a, zero).view(torch.int32)), 'ReLU forward'
     assert torch.equal(dh.view(torch.int32), torch.where(h > 0, da, zero).view(torch.int32)), 'ReLU backward'
@@ -399,7 +391,7 @@ def test_excitation_linears(case):
         dy = torch.randn(B, N, generator=g, device='cuda') * 0.01
         assert linear_splits(Fi) == (2 if Fi == C else 1)
         x, w, dy = (operands(t, precise, seed + k) for k, t in enumerate((x, w, dy)))
-        x, w, b, dy = (_input(t) for t in (x, w, b, dy))
+        x, w, b, dy = (poisoned(t) for t in (x, w, b, dy))
         check_linear(f'{case} {name}', x, w, b, dy, run_linear(x, w, b, dy, precise), precise)
     _report(case, t0)
 
@@ -435,7 +427,7 @@ def test_attention_fcs(case):
     for i in range(P):
         x, w, b, dy, S = classifier_inputs(B, Fi, D, 700 + 10 * i, 'cuda')
         x, w, dy = (operands(t, precise, 710 + 10 * i + k) for k, t in enumerate((x, w, dy)))
-        x, w, b, dy = (_input(t) for t in (x, w, b, dy))
+        x, w, b, dy = (poisoned(t) for t in (x, w, b, dy))
         check_linear(f'{case} fcs[{i}]', x, w, b, dy, run_linear(x, w, b, dy, precise), precise)
         del x, w, b, dy
     _report(case, t0)
@@ -452,7 +444,7 @@ def test_classifier(case):
     x, w, b, dy, S = classifier_inputs(B, D, K, 720, 'cuda')
     assert S == 1
     x, w, dy = (operands(t, precise, 721 + k) for k, t in enumerate((x, w, dy)))
-    x, w, b, dy = (_input(t) for t in (x, w, b, dy))
+    x, w, b, dy = (poisoned(t) for t in (x, w, b, dy))
     check_linear(f'{case} classifier', x, w, b, dy, run_linear(x, w, b, dy, precise), precise)
     _report(case, t0)
 
@@ -462,33 +454,25 @@ def run_npairs(feats, labels):
     F + t, l2norm backward -> dict of every output"""
     b, p, D = feats.shape
     n = b * p
-    x = _input(feats.reshape(n, D))
-    cls = _input_i32(labels.to(torch.int32).repeat_interleave(p))
-    part = _input_i32(torch.arange(p, device='cuda', dtype=torch.int32).repeat(b))
-    xn, g1 = _guarded((n, D))
-    inv, g2 = _guarded((n,))
-    _call('hk_l2norm_rows_fwd', x, xn, inv, n, D)
-    prod, g3 = _guarded((n, n))
-    _call('hk_gemm_3xtf32', xn, 0, D, 0, xn, 0, D, 0, prod, n, 0, 0, n, n, D, 1, 1.0, None, 0.0, None, 0, 0, 0.0, None,
-          0)
-    acc, g4 = _guarded((1,), dtype=F64, fill=0.0)
-    dprod, g5 = _guarded((n, n))
-    _call('hk_npair_loss', prod, cls, part, acc, dprod, n)
-    t, g6 = _guarded((n, D))
-    _call('hk_gemm_3xtf32', dprod, 0, n, 0, xn, 1, D, 0, t, D, 0, 0, n, D, n, 1, 1.0, None, 0.0, None, 0, 0, 0.0, None, 0)
-    dxn, g7 = _guarded((n, D))
-    _call('hk_gemm_3xtf32', dprod, 1, n, 0, xn, 1, D, 0, dxn, D, 0, 0, n, D, n, 1, 1.0, None, 0.0, t, D, 0, 1.0, None, 0)
-    dx, g8 = _guarded((n, D))
-    _call('hk_l2norm_rows_bwd', xn, inv, dxn, dx, n, D)
-    for k, gg in enumerate((g1, g2, g3, g5, g6, g7, g8)):
-        _assert_guard(gg, tag=f'npairs output {k}')
+    x = poisoned(feats.reshape(n, D))
+    cls = poisoned(labels.to(torch.int32).repeat_interleave(p))
+    part = poisoned(torch.arange(p, device='cuda', dtype=torch.int32).repeat(b))
+    xn = guarded((n, D))
+    inv = guarded((n,))
+    abi('hk_l2norm_rows_fwd', x, xn, inv, n, D)
+    prod = guarded((n, n))
+    abi('hk_gemm_3xtf32', xn, 0, D, 0, xn, 0, D, 0, prod, n, 0, 0, n, n, D, 1, 1.0, None, 0.0, None, 0, 0, 0.0, None,
+        0)
+    acc = guarded((1,), dtype=F64, fill=0.0)
+    dprod = guarded((n, n))
+    abi('hk_npair_loss', prod, cls, part, acc, dprod, n)
+    t = guarded((n, D))
+    abi('hk_gemm_3xtf32', dprod, 0, n, 0, xn, 1, D, 0, t, D, 0, 0, n, D, n, 1, 1.0, None, 0.0, None, 0, 0, 0.0, None, 0)
+    dxn = guarded((n, D))
+    abi('hk_gemm_3xtf32', dprod, 1, n, 0, xn, 1, D, 0, dxn, D, 0, 0, n, D, n, 1, 1.0, None, 0.0, t, D, 0, 1.0, None, 0)
+    dx = guarded((n, D))
+    abi('hk_l2norm_rows_bwd', xn, inv, dxn, dx, n, D)
     return dict(x=x, xn=xn, inv=inv, prod=prod, loss=acc, dprod=dprod, t=t, dxn=dxn, dx=dx)
-
-
-def _input_i32(t):
-    buf, _ = _guarded(t.shape, dtype=torch.int32, fill=-7, guard=-7)
-    buf.copy_(t)
-    return buf
 
 
 def npair_features(B, P, D, labels, seed, device='cuda'):
@@ -519,8 +503,8 @@ def test_npairs(case, layout):
         _lib.set_precise(0)
     n = B * P
     y, inv, yb, ib = l2norm_bounds(r['x'])
-    check_bound(r['xn'], y, None, None, f'{tag} l2norm y', bound=yb, names=('anchor', 'feature'))
-    check_bound(r['inv'], inv, None, None, f'{tag} l2norm inv', bound=ib, names=('anchor',))
+    check(r['xn'], y, yb, f'{tag} l2norm y', names=('anchor', 'feature'))
+    check(r['inv'], inv, ib, f'{tag} l2norm inv', names=('anchor',))
     xd = r['xn'].to(F64)
     sc = xd.abs() @ xd.abs().T
     check_c('C_GRAM', f'{tag} prod (K = {D})', r['prod'], xd @ xd.T, (3 * PAIR + EPI) * sc, sc, ('anchor', 'anchor'))
@@ -534,7 +518,7 @@ def test_npairs(case, layout):
     check_c('C_LIN', f'{tag} t = dprod F (K = {n})', r['t'], tr, tf, ts, ('anchor', 'feature'))
     check_c('C_LIN', f'{tag} dF = dprod^T F + t', r['dxn'], dr, df, ds, ('anchor', 'feature'))
     dx, bound = l2norm_bwd64(r['xn'], r['inv'], r['dxn'])
-    check_bound(r['dx'], dx, None, None, f'{tag} l2norm dx', bound=bound, names=('anchor', 'feature'))
+    check(r['dx'], dx, bound, f'{tag} l2norm dx', names=('anchor', 'feature'))
     _report(tag, t0)
 
 
@@ -564,12 +548,7 @@ class _FC64(torch.autograd.Function):
         return ds, None, None, None
 
 
-def rel_l2(a, b):
-    a, b = a.detach().to(F64), b.detach().to(F64)
-    return float((a - b).norm() / b.norm())
-
-
-def _gpu_osme_call(x, blk, fc, up):
+def _gpu_osmeabi(x, blk, fc, up):
     """one attention of OSME forward and backward through direct C-ABI calls; up = the upstream gradients the autograd
     run gave (f, s, m, h, a, z) -> every forward output, input gradient and parameter gradient"""
     from hawkeye_b200 import _lib
@@ -583,9 +562,9 @@ def _gpu_osme_call(x, blk, fc, up):
     def lin(key, xin, w, b):
         Bn, K = xin.shape
         N = w.shape[0]
-        ws, _, nb = _ws('hk_linear_fwd_workspace_bytes', Bn, K, N)
+        ws, nb = workspace('hk_linear_fwd_workspace_bytes', Bn, K, N)
         y = torch.empty(Bn, N, device='cuda')
-        _call('hk_linear_fwd', xin, w, b, y, Bn, K, N, ws, nb)
+        abi('hk_linear_fwd', xin, w, b, y, Bn, K, N, ws, nb)
         out[key] = y
         return y
 
@@ -593,34 +572,34 @@ def _gpu_osme_call(x, blk, fc, up):
         Bn, K = xin.shape
         N = w.shape[0]
         dx = torch.empty(Bn, K, device='cuda')
-        _call('hk_linear_dgrad', dy, w, dx, Bn, K, N)
+        abi('hk_linear_dgrad', dy, w, dx, Bn, K, N)
         dw, db = torch.empty_like(w), torch.empty(N, device='cuda')
-        _call('hk_linear_wgrad', dy, xin, dw, db, Bn, K, N)
+        abi('hk_linear_wgrad', dy, xin, dw, db, Bn, K, N)
         out[key] = (dx, dw, db)
 
     z = torch.empty(B, C, device='cuda')
-    _call('hk_row_mean_fwd', x, z, R, HW, HW)
+    abi('hk_row_mean_fwd', x, z, R, HW, HW)
     out['z'] = z
     a = lin('a', z, w0, b0)
     h = torch.empty_like(a)
-    _call('hk_act_fwd', a, h, a.numel(), 0)
+    abi('hk_act_fwd', a, h, a.numel(), 0)
     out['h'] = h
     m = lin('m', h, w2, b2)
     s = torch.empty_like(x)
-    _call('hk_se_gate_fwd', x, m, s, R, HW)
+    abi('hk_se_gate_fwd', x, m, s, R, HW)
     out['s'] = s
     lin('f', s.reshape(B, Fi), wf, bf)
     lin_bwd('df', up['f'], s.reshape(B, Fi), wf)
     dxg, dm = torch.empty_like(x), torch.empty_like(m)
-    _call('hk_se_gate_bwd', x, m, up['s'].contiguous(), dxg, dm, R, HW)
+    abi('hk_se_gate_bwd', x, m, up['s'].contiguous(), dxg, dm, R, HW)
     out['ds'] = (dxg, dm)
     lin_bwd('dm', up['m'], h, w2)
     da = torch.empty_like(a)
-    _call('hk_act_bwd', h, up['h'], da, a.numel(), 0)
+    abi('hk_act_bwd', h, up['h'], da, a.numel(), 0)
     out['da'] = da
     lin_bwd('da_', up['a'], z, w0)
     dxz = torch.empty(R, HW, device='cuda')
-    _call('hk_row_mean_bwd', up['z'].contiguous(), dxz, R, HW, HW)
+    abi('hk_row_mean_bwd', up['z'].contiguous(), dxz, R, HW, HW)
     out['dz'] = dxz.reshape(x.shape)
     return out
 
@@ -682,22 +661,22 @@ def test_composed_head_b32():
     assert torch.equal(x_part.detach(), part_m) and torch.equal(xs.grad, dx_m), 'staged path differs from the module'
     with torch.no_grad():
         # the loss: cross-entropy and the N-pairs chain
-        ce, _ = _guarded((1,))
-        dlog, _ = _guarded((B, K))
-        corr, _ = _guarded((1,), dtype=torch.int32, fill=-1, guard=-7)
-        _call('hk_softmax_ce_ls', logits, labels, ce, dlog, corr, B, K, 0.1, 1.0)
+        ce = guarded((1,))
+        dlog = guarded((B, K))
+        corr = guarded((1,), dtype=torch.int32, fill=-1, word=-7)
+        abi('hk_softmax_ce_ls', logits, labels, ce, dlog, corr, B, K, 0.1, 1.0)
         np_ = run_npairs(x_part.detach(), labels)
         assert torch.equal(loss, ce[0] + LAMBDA_A * np_['loss'][0].float()), 'MAMCLoss differs from its C-ABI calls'
         assert torch.equal(logits.grad, dlog), 'the cross-entropy gradient differs from hk_softmax_ce_ls'
         assert torch.equal(x_part.grad, (np_['dx'] * LAMBDA_A).reshape(B, P, D)), 'the N-pairs gradient differs'
         assert torch.equal(crit.last_correct, corr), 'last_correct differs from hk_softmax_ce_ls'
-        ws, _, nb = _ws('hk_linear_fwd_workspace_bytes', B, D, K)
+        ws, nb = workspace('hk_linear_fwd_workspace_bytes', B, D, K)
         lo = torch.empty(B, K, device='cuda')
-        _call('hk_linear_fwd', x1, cls.weight, cls.bias, lo, B, D, K, ws, nb)
+        abi('hk_linear_fwd', x1, cls.weight, cls.bias, lo, B, D, K, ws, nb)
         assert torch.equal(lo, logits), 'classifier forward differs from hk_linear_fwd'
         dx1, dwc, dbc = torch.empty(B, D, device='cuda'), torch.empty(K, D, device='cuda'), torch.empty(K, device='cuda')
-        _call('hk_linear_dgrad', logits.grad, cls.weight, dx1, B, D, K)
-        _call('hk_linear_wgrad', logits.grad, x1, dwc, dbc, B, D, K)
+        abi('hk_linear_dgrad', logits.grad, cls.weight, dx1, B, D, K)
+        abi('hk_linear_wgrad', logits.grad, x1, dwc, dbc, B, D, K)
         assert torch.equal(dx1, x1.grad) and torch.equal(dwc, cls.weight.grad) and torch.equal(dbc, cls.bias.grad), \
             'classifier backward differs from hk_linear_dgrad / _wgrad'
         contrib = []
@@ -705,7 +684,7 @@ def test_composed_head_b32():
             d = st[i]
             assert torch.equal(d['f'].grad, x1.grad + x_part.grad[:, i]), f'attention {i}: f.grad is not the sum'
             up = {k: d[k].grad for k in ('f', 's', 'm', 'h', 'a', 'z')}
-            o = _gpu_osme_call(x, blk, fc, up)
+            o = _gpu_osmeabi(x, blk, fc, up)
             for k in ('z', 'a', 'h', 'm', 's', 'f'):
                 assert torch.equal(o[k], d[k].detach()), f'attention {i}: forward {k} differs from its C-ABI call'
             checks = (('s', o['df'][0].reshape(B, C, H, H)), ('m', o['ds'][1]), ('h', o['dm'][0]), ('a', o['da']),
@@ -722,8 +701,7 @@ def test_composed_head_b32():
         cs = [c.to(F64) for c in contrib]
         ref = sum(cs)
         bound = 3 * U * sum(c.abs() for c in cs)
-        check_bound(xs.grad, ref, None, None, 'composed x.grad (four contributions)', bound=bound,
-                    names=('image', 'channel', 'h', 'w'))
+        check(xs.grad, ref, bound, 'composed x.grad (four contributions)', names=('image', 'channel', 'h', 'w'))
         del cs, ref, bound, contrib
     # the fp64 composition
     x64 = x.to(F64).reshape(B, C, HW)
@@ -833,11 +811,11 @@ def test_head_sgd_steps():
     n, lo = 4099, b - 4100
     keep = (flat.flat[lo:lo + 4100].clone(), opt.buf[lo:lo + 4100].clone())
     lr32, wd32 = f32(lr), f32(wd)
-    _call('hk_sgd_momentum', flat.flat[lo:lo + n], flat.grad[lo:lo + n], opt.buf[lo:lo + n], n, lr32, 0.9, wd32, 1.0, 0)
+    abi('hk_sgd_momentum', flat.flat[lo:lo + n], flat.grad[lo:lo + n], opt.buf[lo:lo + n], n, lr32, 0.9, wd32, 1.0, 0)
     p_ref, b_ref, pb, bb = sgd_bounds(keep[0][:n].to(F64), flat.grad[lo:lo + n].to(F64), keep[1][:n].to(F64), lr32,
                                       f32(0.9), wd32, False)
-    check_bound(flat.flat[lo:lo + n], p_ref, None, None, 'SGD 4099 floats p', bound=pb, names=('element',))
-    check_bound(opt.buf[lo:lo + n], b_ref, None, None, 'SGD 4099 floats buf', bound=bb, names=('element',))
+    check(flat.flat[lo:lo + n], p_ref, pb, 'SGD 4099 floats p', names=('element',))
+    check(opt.buf[lo:lo + n], b_ref, bb, 'SGD 4099 floats buf', names=('element',))
     assert torch.equal(flat.flat[lo + n], keep[0][n]) and torch.equal(opt.buf[lo + n], keep[1][n]), \
         'hk_sgd_momentum wrote past n'
     _report('SGD', t0)

@@ -12,6 +12,7 @@ import detgen
 import pc_inputs as I
 from conftest import load_golden, rel_l2
 from oracle import pc_oracle as O
+from kernel_check import precise  # noqa: F401  (a fixture)
 
 pytestmark = pytest.mark.gpu
 G = load_golden('reference_pc')
@@ -22,14 +23,6 @@ os.environ['HAWKEYE_ALLOW_RANDOM_INIT'] = '1'
 # (half an ulp of 2^-10, ~3e-4 rms), unrounded fp32 in the precise mode.  The loss is fp32 sums over at most 256 rows.
 DZ_TOL = {0: 5e-4, 1: 1e-5}
 LOSS_TOL = 1e-5
-
-
-@pytest.fixture
-def precise(request):
-    from hawkeye_b200 import _lib
-    _lib.set_precise(request.param)
-    yield request.param
-    _lib.set_precise(0)
 
 
 def _run(z, y, lam):

@@ -55,18 +55,12 @@ import pytest
 import torch
 
 import detgen
+from kernel_check import RND, TRUNC, U, abi, check, guarded, poisoned, store_bound, workspace, worst_ratio
 from oracle import hop_oracle as O
 
-U = 2.0 ** -24          # fp32 unit roundoff
-TRUNC = 2.0 ** -10      # tf32 truncation of an MMA operand (TF32 mode)
-RND = 2.0 ** -11        # tf32 round-to-nearest on store (TF32 mode)
 EPS_BP = 1e-5           # BCNN.py:21
 EPS_CBP = 1e-10         # CBCNN.py:132
 MODES = ('tf32', 'precise')
-
-GUARD = 64              # guard words after every output and workspace
-GUARD_WORD = 0x5A5A5A5A
-NAN_WORD = -1           # 0xffffffff: a NaN
 
 
 def pad4(v):
@@ -283,79 +277,6 @@ def cbp_case(name):
     return x, hashes, pre, gabs, npairs, g, pre32, dx, dx_scale
 
 
-# ------------------------------------------------------------------------------------------------ the comparison
-def worst_ratio(out, ref, bound):
-    """max |out - ref| / bound over the elements, and the index of the worst one (NaN / Inf output -> inf there)."""
-    out = out.double()
-    err = (out - ref).abs()
-    ratio = torch.where(err == 0, torch.zeros_like(err), err / bound)
-    ratio = torch.where(torch.isfinite(out), ratio, torch.full_like(ratio, math.inf))
-    k = int(torch.argmax(ratio.flatten()))
-    return ratio.flatten()[k].item(), tuple(int(i) for i in np.unravel_index(k, ratio.shape))
-
-
-def check(label, out, ref, bound, rounded, dims):
-    """Assert |out - ref| <= bound (+ 2^-11 |out| where the kernel rounds to tf32 on store) element by element."""
-    out = out.cpu()
-    b = bound + (RND * out.double().abs() if rounded else 0.0)
-    r, idx = worst_ratio(out, ref, b)
-    where = ', '.join(f'{n} {i}' for n, i in zip(dims, idx))
-    print(f'{label}: worst err/bound {r:.3g} at ({where})')
-    assert r <= 1.0, (f'{label}: ({where}): out {out.reshape(-1)[np.ravel_multi_index(idx, out.shape)].item():.9g} '
-                      f'ref {ref[idx].item():.9g} bound {b[idx].item():.3g}, ratio {r:.3g}')
-    return r
-
-
-# ------------------------------------------------------------------------------------------------ guarded device buffers
-def _filled(n, word):
-    return torch.full((n,), word, dtype=torch.int32, device='cuda')
-
-
-class Guarded:
-    """n floats filled with NaN, followed by GUARD guard words."""
-
-    def __init__(self, n):
-        self.n = n
-        self.buf = torch.cat([_filled(n, NAN_WORD), _filled(GUARD, GUARD_WORD)])
-
-    @property
-    def body(self):
-        return self.buf[:self.n].view(torch.float32)
-
-    def intact(self):
-        return bool((self.buf[self.n:] == GUARD_WORD).all())
-
-
-def guarded_input(t):
-    """A device copy of t followed by NaN: a read past its end poisons the result."""
-    buf = torch.cat([t.reshape(-1).cuda(), torch.full((GUARD,), math.nan, device='cuda')])
-    return buf, buf[:t.numel()].view(t.shape)
-
-
-def workspace(query, *args):
-    from hawkeye_b200 import _lib
-    nbytes = _lib.query(query, *args)
-    assert nbytes % 4 == 0
-    return Guarded(nbytes // 4), nbytes
-
-
-def run(mode, name, *args, outputs=(), inputs=()):
-    """One entry-point call in the given precision mode; checks the guards and that the inputs are unchanged."""
-    from hawkeye_b200 import _lib
-    before = [t.clone() for t in inputs]
-    prev = _lib.get_precise()
-    _lib.set_precise(mode == 'precise')
-    try:
-        _lib.call(name, *args, _lib.stream_ptr())
-        torch.cuda.synchronize()
-    finally:
-        _lib.set_precise(prev)
-    for i, g in enumerate(outputs):
-        assert g.intact(), f'{name}: guard words after buffer {i} overwritten'
-    for t, b in zip(inputs, before):
-        assert torch.equal(t.view(torch.int32), b.view(torch.int32)), f'{name}: an input was modified'
-
-
 # ------------------------------------------------------------------------------------------------ GPU tests
 @pytest.mark.gpu
 @pytest.mark.parametrize('mode', MODES)
@@ -364,22 +285,22 @@ def test_bilinear_pool_fwd_bwd(case, mode):
     B, C, H, W, tf32in = BILINEAR[case]
     HW = H * W
     x, dy, p = bilinear_case(case)
-    xbuf, xd = guarded_input(x)
-    dybuf, dyd = guarded_input(dy)
-    y, invn = Guarded(B * C * C), Guarded(B)
+    xd, dyd = poisoned(x), poisoned(dy)
+    y, invn = guarded((B, C, C)), guarded((B,))
     ws, nb = workspace('hk_bilinear_pool_fwd_workspace_bytes', B, C, HW)
-    run(mode, 'hk_bilinear_pool_fwd', xd, y.body, invn.body, B, C, HW, ws.body, nb, outputs=(y, invn, ws), inputs=(xbuf,))
-    dx = Guarded(B * C * HW)
+    precise = mode == 'precise'
+    abi('hk_bilinear_pool_fwd', xd, y, invn, B, C, HW, ws, nb, inputs=(xd,), precise=precise)
+    dx = guarded((B, C, HW))
     wsb, nbb = workspace('hk_bilinear_pool_bwd_workspace_bytes', B, C, HW)
-    run(mode, 'hk_bilinear_pool_bwd', xd, dyd, dx.body, B, C, HW, wsb.body, nbb, outputs=(dx, wsb),
-        inputs=(xbuf, dybuf))
+    abi('hk_bilinear_pool_bwd', xd, dyd, dx, B, C, HW, wsb, nbb, inputs=(xd, dyd), precise=precise)
     bd = bilinear_bounds(x.double(), p, mode, tf32in)
     tag = f'bilinear {case} {mode}'
-    yk = y.body.view(B, C, C)
-    check(f'{tag} y', yk, p['y'].view(B, C, C), bd['y'].view(B, C, C), mode == 'tf32', ('image', 'row', 'col'))
-    check(f'{tag} inv_norm', invn.body, 1.0 / p['n'], bd['inv_norm'], False, ('image',))
-    dxk = dx.body.view(B, C, HW)
-    check(f'{tag} dx', dxk, p['dx'].view(B, C, HW), bd['dx'].view(B, C, HW), mode == 'tf32', ('image', 'channel', 'pos'))
+    yk, dxk = y.cpu(), dx.cpu()
+    check(yk, p['y'].view(B, C, C), store_bound(yk, bd['y'].view(B, C, C), not precise), f'{tag} y',
+          names=('image', 'row', 'col'))
+    check(invn, 1.0 / p['n'], bd['inv_norm'], f'{tag} inv_norm', names=('image',))
+    check(dxk, p['dx'].view(B, C, HW), store_bound(dxk, bd['dx'].view(B, C, HW), not precise), f'{tag} dx',
+          names=('image', 'channel', 'pos'))
     if B >= 5:                               # the all-zero image: y is 1/C (an ulp of the product in precise mode), dx 0
         z = B - 4
         yz = yk[z].double().cpu() * C
@@ -395,16 +316,16 @@ def test_cbp_fwd(case, mode):
     x, hashes, pre_ref, gabs, npairs, *_ = cbp_case(case)
     h1, s1, h2, s2 = [torch.from_numpy(a).cuda() for a in hashes]
     h1, h2, s1, s2 = h1.int(), h2.int(), s1.float(), s2.float()
-    xbuf, xd = guarded_input(x)
-    y, pre = Guarded(B * d), Guarded(B * d)
-    run(mode, 'hk_cbp_fwd', xd, h1, h2, s1, s2, y.body, pre.body, B, C, H * W, d, outputs=(y, pre), inputs=(xbuf,))
+    xd = poisoned(x)
+    y, pre = guarded((B, d)), guarded((B, d))
+    abi('hk_cbp_fwd', xd, h1, h2, s1, s2, y, pre, B, C, H * W, d, inputs=(xd,), precise=mode == 'precise')
     tag = f'cbp {case} {mode}'
-    check(f'{tag} pre', pre.body.view(B, d), pre_ref, cbp_pre_bound(H, W, mode, tf32in, gabs, npairs), False,
-          ('image', 'bin'))
-    y_ref, dn2 = cbp_finalize(pre.body.view(B, d).double().cpu())
-    check(f'{tag} y', y.body.view(B, d), y_ref, cbp_y_bound(y_ref, dn2), mode == 'tf32', ('image', 'bin'))
+    check(pre, pre_ref, cbp_pre_bound(H, W, mode, tf32in, gabs, npairs), f'{tag} pre', names=('image', 'bin'))
+    y_ref, dn2 = cbp_finalize(pre.double().cpu())
+    yk = y.cpu()
+    check(yk, y_ref, store_bound(yk, cbp_y_bound(y_ref, dn2), mode == 'tf32'), f'{tag} y', names=('image', 'bin'))
     if B >= 5:                               # the all-zero image
-        assert (pre.body.view(B, d)[B - 4] == 0).all() and (y.body.view(B, d)[B - 4] == 0).all()
+        assert (pre[B - 4] == 0).all() and (y[B - 4] == 0).all()
 
 
 @pytest.mark.gpu
@@ -415,16 +336,15 @@ def test_cbp_bwd(case, mode):
     x, hashes, _, _, _, g, pre32, dx_ref, dx_scale = cbp_case(case)
     h1, s1, h2, s2 = [torch.from_numpy(a).cuda() for a in hashes]
     h1, h2, s1, s2 = h1.int(), h2.int(), s1.float(), s2.float()
-    xbuf, xd = guarded_input(x)
-    prebuf, pred = guarded_input(pre32)
-    gbuf, gd = guarded_input(g)
-    dx = Guarded(B * C * H * W)
+    xd, pred, gd = poisoned(x), poisoned(pre32), poisoned(g)
+    dx = guarded((B, C, H * W))
     ws, nb = workspace('hk_cbp_bwd_workspace_bytes', B, C, d)
-    run(mode, 'hk_cbp_bwd', xd, pred, gd, h1, h2, s1, s2, dx.body, B, C, H * W, d, ws.body, nb, outputs=(dx, ws),
-        inputs=(xbuf, prebuf, gbuf))
-    dxk = dx.body.view(B, C, H * W)
-    check(f'cbp {case} {mode} dx', dxk, dx_ref.view(B, C, H * W), cbp_dx_c(C, d, mode, tf32in) * dx_scale.view(B, C, H * W),
-          mode == 'tf32', ('image', 'channel', 'pos'))
+    abi('hk_cbp_bwd', xd, pred, gd, h1, h2, s1, s2, dx, B, C, H * W, d, ws, nb, inputs=(xd, pred, gd),
+        precise=mode == 'precise')
+    dxk = dx.cpu()
+    check(dxk, dx_ref.view(B, C, H * W),
+          store_bound(dxk, cbp_dx_c(C, d, mode, tf32in) * dx_scale.view(B, C, H * W), mode == 'tf32'),
+          f'cbp {case} {mode} dx', names=('image', 'channel', 'pos'))
     if B >= 5:
         assert (dxk[B - 4] == 0).all()
 
@@ -435,7 +355,8 @@ def test_cbp_bwd(case, mode):
 def rejected(bad, ref, bound, rounded):
     """Worst err/bound ratio of the fp32-rounded defect, and where; > 1 means the GPU check would fail it."""
     out = bad.float().double()
-    return worst_ratio(out, ref, bound + (RND * out.abs() if rounded else 0.0))
+    r, idx = worst_ratio(out, ref, store_bound(out, bound, rounded))
+    return r, tuple(idx)
 
 
 def loosest_bilinear(x, p):

@@ -13,18 +13,11 @@ import detgen
 from conftest import load_golden, rel_l2
 from oracle import prototree_oracle as O
 from prototree_inputs import theta0, tree_inputs
+from kernel_check import precise  # noqa: F401  (a fixture)
 
 pytestmark = pytest.mark.gpu
 G = load_golden('reference_prototree')
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture(params=[0, 1], ids=['tf32', 'precise'])
-def precise(request):
-    from hawkeye_b200 import _lib
-    _lib.set_precise(request.param)
-    yield request.param
-    _lib.set_precise(0)
 
 
 def _head(z, protos, theta, labels, height):

@@ -8,16 +8,9 @@ import torch.nn.functional as F
 
 import detgen
 from conftest import rel_l2
+from kernel_check import nchw, nhwc
 
 pytestmark = pytest.mark.gpu
-
-
-def _nhwc(t):
-    return t.permute(0, 2, 3, 1).contiguous()
-
-
-def _nchw(t):
-    return t.permute(0, 3, 1, 2).contiguous()
 
 
 # (N, H, W, C, relu, residual, k): the channels' means sit at k x their spread.  P = N*H*W pixels are summed in
@@ -47,12 +40,12 @@ def test_batchnorm_train(N, H, W, C, relu, res, k):
     if res:
         y_ref = y_ref + rd
     P = N * H * W
-    xg, y = _nhwc(x).cuda(), torch.empty(N, H, W, C, device='cuda')
+    xg, y = nhwc(x).cuda(), torch.empty(N, H, W, C, device='cuda')
     mean, invstd = torch.empty(C, device='cuda'), torch.empty(C, device='cuda')
     rmg, rvg = torch.zeros(C, device='cuda'), torch.ones(C, device='cuda')
     nb = _lib.query('hk_bn_workspace_bytes', P, C)
     ws = torch.empty(nb, dtype=torch.uint8, device='cuda')
-    rg = _nhwc(r).cuda() if res else None
+    rg = nhwc(r).cuda() if res else None
     _lib.call('hk_bn_fwd', xg, gamma.cuda(), beta.cuda(), rg, y, mean, invstd, rmg, rvg, 0.1, 1e-5, P, C, relu, ws, nb, s)
     # the statistics at fp32 accuracy whatever the offset; a mean near 0 has no relative scale of its own, so its error is
     # taken in units of the channel's spread (which is what it shifts xhat = (x - mean) * invstd by)
@@ -65,23 +58,23 @@ def test_batchnorm_train(N, H, W, C, relu, res, k):
             'running_var': ((rvg.cpu().double() - rv).abs() / rv).max().item()}
     print(f'bn P={P} C={C} mean={k} sigma:', {n: f'{e:.1e}' for n, e in errs.items()})
     assert max(errs.values()) < 1e-5, errs
-    assert rel_l2(_nchw(y).cpu(), (F.relu(y_ref) if relu else y_ref).detach()) < 5e-4          # tf32-rounded on store
+    assert rel_l2(nchw(y).cpu(), (F.relu(y_ref) if relu else y_ref).detach()) < 5e-4          # tf32-rounded on store
     # the gradients on the ReLU branch this forward took: at a mean of 100 sigma, the fp32 mean itself is off by up to
     # 6e-6 sigma, which flips the few outputs that close to zero, each an O(1) change of one dx element
     if relu:
-        y_ref = y_ref * (_nchw(y) > 0).cpu().double()
+        y_ref = y_ref * (nchw(y) > 0).cpu().double()
     grads = torch.autograd.grad(y_ref, [xd, gd, bd] + ([rd] if res else []), dy.double())
     dx, dres = torch.empty_like(xg), (torch.empty_like(xg) if res else None)
     dg, db = torch.empty(C, device='cuda'), torch.empty(C, device='cuda')
-    _lib.call('hk_bn_bwd', xg, y, _nhwc(dy).cuda(), gamma.cuda(), mean, invstd, dx, dres, dg, db, P, C, relu, ws, nb, s)
-    assert rel_l2(_nchw(dx).cpu(), grads[0]) < 2e-3
+    _lib.call('hk_bn_bwd', xg, y, nhwc(dy).cuda(), gamma.cuda(), mean, invstd, dx, dres, dg, db, P, C, relu, ws, nb, s)
+    assert rel_l2(nchw(dx).cpu(), grads[0]) < 2e-3
     assert rel_l2(dg.cpu(), grads[1]) < 2e-3 and rel_l2(db.cpu(), grads[2]) < 2e-3
     if res:
-        assert rel_l2(_nchw(dres).cpu(), grads[3]) < 1e-6
+        assert rel_l2(nchw(dres).cpu(), grads[3]) < 1e-6
     if relu and not res:
         # hk_bn_bwd_ex: the ReLU mask re-evaluated from x (y not read, passed as null) must give the same bits
         dx2, dg2, db2 = torch.empty_like(xg), torch.empty(C, device='cuda'), torch.empty(C, device='cuda')
-        _lib.call('hk_bn_bwd_ex', xg, None, _nhwc(dy).cuda(), gamma.cuda(), beta.cuda(), mean, invstd, dx2, None, dg2, db2, P, C,
+        _lib.call('hk_bn_bwd_ex', xg, None, nhwc(dy).cuda(), gamma.cuda(), beta.cuda(), mean, invstd, dx2, None, dg2, db2, P, C,
                   relu, ws, nb, s)
         assert torch.equal(dx2, dx) and torch.equal(dg2, dg) and torch.equal(db2, db)
 
@@ -106,11 +99,11 @@ def test_bn_apply_eval(relu, res, precision):
     y = torch.empty(N, H, W, C, device='cuda')
     _lib.set_precise(precision)
     try:
-        _lib.call('hk_bn_apply', _nhwc(x).cuda(), rmean.cuda(), invstd, gamma.cuda(), beta.cuda(),
-                  _nhwc(r).cuda() if res else None, y, N * H * W, C, relu, _lib.stream_ptr())
+        _lib.call('hk_bn_apply', nhwc(x).cuda(), rmean.cuda(), invstd, gamma.cuda(), beta.cuda(),
+                  nhwc(r).cuda() if res else None, y, N * H * W, C, relu, _lib.stream_ptr())
     finally:
         _lib.set_precise(0)
-    e = rel_l2(_nchw(y).cpu(), y_ref)
+    e = rel_l2(nchw(y).cpu(), y_ref)
     print('bn apply', relu, res, precision, e)
     assert e < (5e-4 if not precision else 1e-6)
     if relu:
@@ -130,11 +123,11 @@ def test_maxpool3x3_s2_edges(N, H, W, C):
     Ho, Wo = p_ref.shape[2], p_ref.shape[3]
     out = torch.empty(N, Ho, Wo, C, device='cuda')
     am = torch.empty(N, Ho, Wo, C, device='cuda', dtype=torch.uint8)
-    _lib.call('hk_maxpool3x3s2_fwd', _nhwc(a.detach().float()).cuda(), out, am, N, H, W, C, s)
-    assert torch.equal(_nchw(out).cpu().double(), p_ref.detach())
+    _lib.call('hk_maxpool3x3s2_fwd', nhwc(a.detach().float()).cuda(), out, am, N, H, W, C, s)
+    assert torch.equal(nchw(out).cpu().double(), p_ref.detach())
     dx = torch.empty(N, H, W, C, device='cuda')
-    _lib.call('hk_maxpool3x3s2_bwd', am, _nhwc(g.float()).cuda(), dx, N, H, W, C, s)
-    assert rel_l2(_nchw(dx).cpu(), ga) < 1e-6
+    _lib.call('hk_maxpool3x3s2_bwd', am, nhwc(g.float()).cuda(), dx, N, H, W, C, s)
+    assert rel_l2(nchw(dx).cpu(), ga) < 1e-6
 
 
 def test_maxpool3x3_s2_and_stride_helpers():
@@ -145,15 +138,15 @@ def test_maxpool3x3_s2_and_stride_helpers():
     p_ref = F.max_pool2d(a, 3, 2, 1)
     g = detgen.det(p_ref.shape, 8).double()
     (ga,) = torch.autograd.grad(p_ref, a, g)
-    ag = _nhwc(a.detach().float()).cuda()
+    ag = nhwc(a.detach().float()).cuda()
     Ho, Wo = p_ref.shape[2], p_ref.shape[3]
     out = torch.empty(N, Ho, Wo, C, device='cuda')
     am = torch.empty(N, Ho, Wo, C, device='cuda', dtype=torch.uint8)
     _lib.call('hk_maxpool3x3s2_fwd', ag, out, am, N, H, W, C, s)
-    assert torch.equal(_nchw(out).cpu().double(), p_ref.detach())
+    assert torch.equal(nchw(out).cpu().double(), p_ref.detach())
     dx = torch.empty_like(ag)
-    _lib.call('hk_maxpool3x3s2_bwd', am, _nhwc(g.float()).cuda(), dx, N, H, W, C, s)
-    assert rel_l2(_nchw(dx).cpu(), ga) < 1e-6
+    _lib.call('hk_maxpool3x3s2_bwd', am, nhwc(g.float()).cuda(), dx, N, H, W, C, s)
+    assert rel_l2(nchw(dx).cpu(), ga) < 1e-6
     sub = torch.empty(N, H // 2, W // 2, C, device='cuda')
     _lib.call('hk_subsample2', ag, sub, N, H, W, C, s)
     assert torch.equal(sub.cpu(), ag.cpu()[:, ::2, ::2])
@@ -174,8 +167,8 @@ def test_conv3x3_stride2_fwd(N, H, W, Cin, Cout):
     wf = torch.empty(9 * Cout * Cin, device='cuda')
     _lib.call('hk_conv3x3_pack_weights', w.cuda(), wf, None, Cout, Cin, s)
     y = torch.empty(N, H // 2, W // 2, Cout, device='cuda')
-    _lib.call('hk_conv3x3_s2_fwd', _nhwc(x).cuda(), wf, None, y, N, H, W, Cin, Cout, 0, s)
-    e = rel_l2(_nchw(y).cpu(), y_ref)
+    _lib.call('hk_conv3x3_s2_fwd', nhwc(x).cuda(), wf, None, y, N, H, W, Cin, Cout, 0, s)
+    e = rel_l2(nchw(y).cpu(), y_ref)
     print('conv s2', e)
     assert e < 2e-3
 
@@ -192,7 +185,7 @@ def test_conv3x3_wgrad_14x14_and_7x7():
         dw = torch.empty(Cout, Cin, 3, 3, device='cuda')
         nb = _lib.query('hk_conv3x3_wgrad_workspace_bytes', Cin, Cout)
         ws = torch.empty(nb, dtype=torch.uint8, device='cuda')
-        _lib.call('hk_conv3x3_wgrad', _nhwc(x.float()).cuda(), _nhwc(dy.float()).cuda(), dw, None, N, H, W, Cin, Cout, ws, nb, s)
+        _lib.call('hk_conv3x3_wgrad', nhwc(x.float()).cuda(), nhwc(dy.float()).cuda(), dw, None, N, H, W, Cin, Cout, ws, nb, s)
         e = rel_l2(dw.cpu(), gw)
         print('wgrad', H, W, e)
         assert e < 2e-3

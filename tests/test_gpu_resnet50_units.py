@@ -8,7 +8,7 @@ then Unit.backward (with an addend on the 1x1 units, so that the dgrad GEMM's fu
 stage is compared with fp64 of the same operation on the fp32 values it was given.  In TF32 mode those values are
 TF32-representable (the inputs here are rounded, and the im2col, the BN outputs and dC are rounded on store), so every
 tensor-core product is exact and what is left is fp32 accumulation plus, where the kernel rounds its output, one TF32
-rounding (test_gpu_conv_vgg16.ROUND = 2^-11).  The bound of every check is |out - ref| <= ROUND * max(|out|, |ref|)
+rounding (kernel_check.RND = 2^-11).  The bound of every check is |out - ref| <= RND * max(|out|, |ref|)
 (where the output is rounded) + c * scale, with `scale` the same expression over absolute values:
 
   conv output c        scale = the same conv of |x|, |w|                                     C_CONV (C_PRECISE)
@@ -34,7 +34,7 @@ import torch.nn.functional as F
 
 import detgen
 from oracle.hop_oracle import RESNET50_LAYERS
-from test_gpu_conv_vgg16 import _assert_guard, _guarded, bound_of, check_bound
+from kernel_check import Bound, Out, Worst, abi, c_bound, check, rnd_bound, workspace
 
 # Each constant is at least 4x the worst (|err| - rounding term) / scale measured over every check of this file (the
 # four sweeps of test_unit) on an H100 80GB HBM3 at 700 W:
@@ -55,7 +55,6 @@ C_PRECISE = 2.0 ** -16
 # (the worst measured is 0.70 of it).
 CHUNK = 4
 BN_EPS = 1e-5
-CODE_GUARD = 0xA5
 
 # sweep: (image side, batch, precise, train mode)
 SWEEPS = {'tf32-448-b32': (448, 32, 0, True), 'tf32-224-b24': (224, 24, 0, True),
@@ -255,13 +254,14 @@ def drop_rows(dw, x, g, n, r0, r1):
     return dw - wgrad_nhwc(x[n:n + 1], gi, 3, 1, 1).to(dw.dtype)
 
 
-def rejected(bad, ref, absref, c, tag, rnd=False, bound=None, names=('image', 'h', 'w', 'channel')):
-    """assert that check_bound rejects `bad` and that its worst violation is at least 2x the bound -> that ratio"""
-    b = bound if bound is not None else bound_of(bad, ref, absref, c, rnd)
+def rejected(bad, ref, absref, c, tag, rnd=False, names=('image', 'h', 'w', 'channel')):
+    """assert that check rejects `bad` and that its worst violation is at least 2x the bound -> that ratio"""
+    bound = Bound(c * absref.double(), rounded=rnd)
+    b = bound.total(bad, ref)
     err = (bad.double() - ref.double()).abs()
     ratio = float(torch.where(err == 0, torch.zeros_like(err), err / b).max())
     with pytest.raises(AssertionError):
-        check_bound(bad, ref, absref, c, tag, rnd=rnd, bound=bound, names=names)
+        check(bad, ref, bound, tag, names=names)
     print(f'{tag}: rejected, violation ratio {ratio:.3g}', flush=True)
     assert ratio >= 2, f'{tag}: violation ratio {ratio:.3g} < 2'
     return ratio
@@ -400,51 +400,18 @@ def test_cpu_bounds_reject_defects():
 # ------------------------------------------------------------------------------------------------------------------
 # 4. the production path on the GPU
 # ------------------------------------------------------------------------------------------------------------------
-WORST = {}      # constant -> (worst c-term share over the checks run so far, its tag)
+WORST = Worst()
 
 
-def _chk(const, out, ref, absref, c, tag, **kw):
-    share = check_bound(out, ref, absref, c, tag, **kw)
-    if share > WORST.get(const, (-1.0, ''))[0]:
-        WORST[const] = (share, tag)
-    return share
-
-
-class _Out:
-    """an output argument of _abi: NaN-filled (uint8: 255) and followed by guard words"""
-    def __init__(self, shape, dtype=torch.float32):
-        self.shape, self.dtype = tuple(shape), dtype
-
-
-def _abi(name, *args):
-    """call the C-ABI entry point `name` (stream appended) with each _Out replaced by a fresh guarded buffer -> those"""
-    from hawkeye_b200 import _lib
-    outs, real = [], []
-    for a in args:
-        if isinstance(a, _Out):
-            u8 = a.dtype == torch.uint8
-            t, g = _guarded(a.shape, a.dtype, 255, CODE_GUARD) if u8 else _guarded(a.shape)
-            outs.append((t, g, u8))
-            a = t
-        real.append(a)
-    _lib.call(name, *real, _lib.stream_ptr())
-    torch.cuda.synchronize()
-    for t, g, u8 in outs:
-        _assert_guard(g, CODE_GUARD if u8 else 12345.0, tag=name)
-    return [t for t, _, _ in outs]
+def _chk(const, out, ref, absref, c, tag, rnd=True, **kw):
+    return WORST.add(const, check(out, ref, (rnd_bound if rnd else c_bound)(absref, c), tag, **kw), tag)
 
 
 def _gemm(A, B, b_mn, M, N, K, D=None):
     """the GEMM of conv1x1_fwd (B = w [N, K]) or conv1x1_dgrad (b_mn: B = w [K, N], D: the epilogue addend)"""
-    (C,) = _abi('hk_gemm_tf32', A, 0, K, 0, B, int(b_mn), N if b_mn else K, 0, _Out((M, N)), N, 0, 0, M, N, K, 1, 1.0, None,
-                0.0, D, 0 if D is None else N, 0, 0.0 if D is None else 1.0, None, 0)
+    (C,) = abi('hk_gemm_tf32', A, 0, K, 0, B, int(b_mn), N if b_mn else K, 0, Out((M, N)), N, 0, 0, M, N, K, 1, 1.0,
+               None, 0.0, D, 0 if D is None else N, 0, 0.0 if D is None else 1.0, None, 0)
     return C
-
-
-def _ws(name, *args):
-    from hawkeye_b200 import _lib
-    nb = int(_lib.query(name, *args))
-    return torch.empty(max(nb, 16), dtype=torch.uint8, device='cuda'), nb
 
 
 def _inputs(spec, N, seed, tf32):
@@ -505,7 +472,7 @@ def _nhwc_in(d, kind):
 
 
 
-def _check_abi(spec, d, tag):
+def _checkabi(spec, d, tag):
     """every kernel of the unit once more through the C ABI into NaN-filled buffers followed by guard words: the Unit's
     bits -> the directly called 3x3 weight gradient (its splits add with atomics: held to its bound by the caller), or None"""
     from hawkeye_b200.ops import conv3x3_pack
@@ -514,43 +481,43 @@ def _check_abi(spec, d, tag):
     N, P = x.shape[0], rec['P']
     # forward convolution
     if kind == 'stem':
-        (x147,) = _abi('hk_stem_im2col', x, _Out(rec['xin'].shape), N, H, H)
-        (w147,) = _abi('hk_pack_stem_weights', w, _Out((cout, 160)), cout)
+        (x147,) = abi('hk_stem_im2col', x, Out(rec['xin'].shape), N, H, H)
+        (w147,) = abi('hk_pack_stem_weights', w, Out((cout, 160)), cout)
         assert torch.equal(x147, rec['xin']), f'{tag}: im2col differs'
         assert torch.equal(_gemm(x147, w147, 0, P, cout, 160), c.view(P, cout)), f'{tag}: stem GEMM differs'
     elif kind in ('1x1', '1x1s2'):
         if kind == '1x1s2':
-            (xs,) = _abi('hk_subsample2', x, _Out(rec['xin'].shape), N, H, H, cin)
+            (xs,) = abi('hk_subsample2', x, Out(rec['xin'].shape), N, H, H, cin)
             assert torch.equal(xs, rec['xin']) and torch.equal(xs, x[:, ::2, ::2]), f'{tag}: subsample differs'
         assert torch.equal(_gemm(rec['xin'], w, 0, P, cout, cin), c.view(P, cout)), f'{tag}: GEMM differs'
     else:
         wf, wd = conv3x3_pack(w, True)
-        (cd,) = _abi('hk_conv3x3_s2_fwd' if kind == '3x3s2' else 'hk_conv3x3_fwd', x, wf, None, _Out(c.shape), N, H, H,
-                     cin, cout, 0)
+        (cd,) = abi('hk_conv3x3_s2_fwd' if kind == '3x3s2' else 'hk_conv3x3_fwd', x, wf, None, Out(c.shape), N, H, H,
+                    cin, cout, 0)
         assert torch.equal(cd, c), f'{tag}: conv differs'
     # BatchNorm forward and backward
     bn = d['u'].bn
-    ws, nb = _ws('hk_bn_workspace_bytes', P, cout)
+    ws, nb = workspace('hk_bn_workspace_bytes', P, cout)
     if rec['frozen']:
-        (y,) = _abi('hk_bn_apply', c, d['mean'], d['invstd'], d['gamma'], d['beta'], d['res'], _Out(c.shape), P, cout,
-                    int(relu))
+        (y,) = abi('hk_bn_apply', c, d['mean'], d['invstd'], d['gamma'], d['beta'], d['res'], Out(c.shape), P, cout,
+                   int(relu))
     else:
         rm, rv = d['rm0'].clone(), d['rv0'].clone()
-        y, mean, invstd = _abi('hk_bn_fwd', c, d['gamma'], d['beta'], d['res'], _Out(c.shape), _Out((cout,)),
-                               _Out((cout,)), rm, rv, float(bn.momentum), float(bn.eps), P, cout, int(relu), ws, nb)
+        y, mean, invstd = abi('hk_bn_fwd', c, d['gamma'], d['beta'], d['res'], Out(c.shape), Out((cout,)),
+                              Out((cout,)), rm, rv, float(bn.momentum), float(bn.eps), P, cout, int(relu), ws, nb)
         assert torch.equal(mean, d['mean']) and torch.equal(invstd, d['invstd']), f'{tag}: BN statistics differ'
         assert torch.equal(rm, bn.running_mean) and torch.equal(rv, bn.running_var), f'{tag}: running statistics differ'
     assert torch.equal(y, d['y']), f'{tag}: BN output differs'
-    outs = _abi('hk_bn_bwd_frozen' if rec['frozen'] else 'hk_bn_bwd_ex', c, rec['y'], d['dy'], d['gamma'], d['mask_beta'],
-                d['mean'], d['invstd'], _Out(c.shape), _Out(c.shape) if has_res else None, _Out((cout,)), _Out((cout,)),
-                P, cout, int(relu), ws, nb)
+    outs = abi('hk_bn_bwd_frozen' if rec['frozen'] else 'hk_bn_bwd_ex', c, rec['y'], d['dy'], d['gamma'],
+               d['mask_beta'], d['mean'], d['invstd'], Out(c.shape), Out(c.shape) if has_res else None, Out((cout,)),
+               Out((cout,)), P, cout, int(relu), ws, nb)
     want = [dc] + ([d['dres']] if has_res else []) + [d['dg'], d['db']]
     assert all(torch.equal(a, b) for a, b in zip(outs, want)), f'{tag}: BN backward differs'
     # weight and data gradients
     if kind in ('stem', '1x1', '1x1s2'):
         K = 160 if kind == 'stem' else cin
-        ws, nb = _ws('hk_matconv_wgrad_workspace_bytes', P, K, cout)
-        (dwm,) = _abi('hk_matconv_wgrad', rec['xin'], dc, _Out((cout, K)), P, K, cout, ws, nb)
+        ws, nb = workspace('hk_matconv_wgrad_workspace_bytes', P, K, cout)
+        (dwm,) = abi('hk_matconv_wgrad', rec['xin'], dc, Out((cout, K)), P, K, cout, ws, nb)
         assert torch.equal(dwm[:, :d['dw'][0].numel()], d['dw'].view(cout, -1)), f'{tag}: matconv wgrad differs'
         if kind == 'stem':
             assert not bool(dwm[:, 147:].any()), f'{tag}: the zero im2col columns have a non-zero weight gradient'
@@ -559,20 +526,20 @@ def _check_abi(spec, d, tag):
             assert torch.equal(_gemm(dc, w, 1, P, cin, cout, D=d['addend']), dx.view(P, cin)), f'{tag}: dgrad differs'
             return None
         dxs = _gemm(dc, w, 1, P, cin, cout)
-        (up,) = _abi('hk_upsample2_zero', dxs, _Out(dx.shape), N, H, H, cin)
+        (up,) = abi('hk_upsample2_zero', dxs, Out(dx.shape), N, H, H, cin)
         assert torch.equal(up[:, ::2, ::2], dxs.view(N, (H + 1) // 2, (H + 1) // 2, cin)), f'{tag}: upsample differs'
         assert not bool(up[:, 1::2].any()) and not bool(up[:, :, 1::2].any()), f'{tag}: upsample odd rows not zero'
         assert torch.equal(up + d['addend'], dx), f'{tag}: stride-2 dgrad differs'
         return None
     g = dc
     if kind == '3x3s2':
-        (g,) = _abi('hk_upsample2_zero', dc, _Out((N, H, H, cout)), N, H, H, cout)
+        (g,) = abi('hk_upsample2_zero', dc, Out((N, H, H, cout)), N, H, H, cout)
         assert torch.equal(g[:, ::2, ::2], dc) and not bool(g[:, 1::2].any()) and not bool(g[:, :, 1::2].any()), \
             f'{tag}: zero insertion of dC differs'
-    (dxd,) = _abi('hk_conv3x3_dgrad', g, wd, None, _Out(dx.shape), N, H, H, cin, cout)
+    (dxd,) = abi('hk_conv3x3_dgrad', g, wd, None, Out(dx.shape), N, H, H, cin, cout)
     assert torch.equal(dxd, dx), f'{tag}: dgrad differs'
-    ws, nb = _ws('hk_conv3x3_wgrad_workspace_bytes', cin, cout)
-    (dwd,) = _abi('hk_conv3x3_wgrad_acc', x, g, _Out(w.shape), None, N, H, H, cin, cout, ws, nb, 0)
+    ws, nb = workspace('hk_conv3x3_wgrad_workspace_bytes', cin, cout)
+    (dwd,) = abi('hk_conv3x3_wgrad_acc', x, g, Out(w.shape), None, N, H, H, cin, cout, ws, nb, 0)
     return dwd
 
 
@@ -591,9 +558,8 @@ def _check_stats(d, tag):
     # the statistics' own bound, scaled by the momentum, plus the update's three fp32 roundings
     bm = mom * C_SUMS * sig + 2.0 ** -22 * ((1 - mom) * rm0.abs() + mom * m.abs())
     bv = mom * 2 * C_SUMS * unb + 2.0 ** -22 * ((1 - mom) * rv0.abs() + mom * unb)
-    check_bound(bn.running_mean, (1 - mom) * rm0 + mom * m, None, None, f'{tag} running mean', bound=bm, names=('channel',))
-    check_bound(bn.running_var, (1 - mom) * rv0 + mom * unb, None, None, f'{tag} running var', bound=bv,
-                names=('channel',))
+    check(bn.running_mean, (1 - mom) * rm0 + mom * m, bm, f'{tag} running mean', names=('channel',))
+    check(bn.running_var, (1 - mom) * rv0 + mom * unb, bv, f'{tag} running var', names=('channel',))
 
 
 def _check_maxpool(y, tag, seed):
@@ -601,9 +567,9 @@ def _check_maxpool(y, tag, seed):
     2^-22 of its |terms|"""
     N, H, W, C = y.shape
     Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
-    p, am = _abi('hk_maxpool3x3s2_fwd', y, _Out((N, Ho, Wo, C)), _Out((N, Ho, Wo, C), torch.uint8), N, H, W, C)
+    p, am = abi('hk_maxpool3x3s2_fwd', y, Out((N, Ho, Wo, C)), Out((N, Ho, Wo, C), torch.uint8), N, H, W, C)
     dp = torch.randn(p.shape, device='cuda', generator=torch.Generator(device='cuda').manual_seed(seed))
-    (dx,) = _abi('hk_maxpool3x3s2_bwd', am, dp, _Out(y.shape), N, H, W, C)
+    (dx,) = abi('hk_maxpool3x3s2_bwd', am, dp, Out(y.shape), N, H, W, C)
     ties = 0
     for n0 in range(0, N, CHUNK):
         sl = slice(n0, n0 + CHUNK)
@@ -612,7 +578,7 @@ def _check_maxpool(y, tag, seed):
         assert torch.equal(am[sl].long(), arg), f'{tag} maxpool [{n0}:]: arg-max bytes differ from the first maximum'
         ties += int((val == 0).sum())
         ref, ax = maxpool_bwd_ref(arg, dp[sl], H, W)
-        check_bound(dx[sl], ref, ax, 2.0 ** -22, f'{tag} maxpool dx [{n0}:]', rnd=False, n0=n0)
+        check(dx[sl], ref, c_bound(ax, 2.0 ** -22), f'{tag} maxpool dx [{n0}:]', n0=n0)
     print(f'{tag} maxpool: {ties / p.numel():.1%} of the windows are all zero (tied)', flush=True)
 
 
@@ -624,7 +590,7 @@ def _check_unit(sweep, spec, seed):
     crnd = rnd and kind.startswith('3x3')     # the 3x3 convolutions store TF32, the GEMMs fp32
     tag = f'{sweep} {name}'
     d = run_unit(spec, N, seed, precise, training)
-    dw3 = _check_abi(spec, d, tag)
+    dw3 = _checkabi(spec, d, tag)
     if training:
         _check_stats(d, tag)
     k, stride, pad = GEOM[kind]
@@ -689,8 +655,20 @@ def test_unit(sweep, unit):
     finally:
         _lib.set_precise(0)
     print(f'{sweep} {unit} ({spec[1]}, N={N}, {spec[2]}x{spec[2]}, {spec[3]}->{spec[4]}): {time.time() - t0:.1f} s, peak '
-          f'{torch.cuda.max_memory_allocated() / 2**30:.1f} GiB; worst c-term share so far: ' +
-          ', '.join(f'{k} {v:.3g} ({t})' for k, (v, t) in sorted(WORST.items())), flush=True)
+          f'{torch.cuda.max_memory_allocated() / 2**30:.1f} GiB; worst c-term share so far: ' + WORST.summary(),
+          flush=True)
+
+
+# the dimension-reduction unit in front of the mpn step's covariance head (1x1, 2048 -> 256 at 14x14, BN, ReLU)
+DR_UNIT = ('pool.conv_dr_block', '1x1', 14, 2048, 256, True, False)
+
+
+@pytest.mark.gpu
+def test_dr_unit_b32():
+    """the dimension-reduction unit of the mpn step at 448x448 batch 32, TF32 train mode"""
+    from hawkeye_b200 import _lib
+    _lib.set_precise(0)
+    _check_unit('tf32-448-b32', DR_UNIT, 6000)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -705,13 +683,13 @@ def test_gpu_bounds_reject_conv_defects():
         d = run_unit(spec, 2, 900)
         x, w, c = d['x'], d['w'], d['c']
         ref, a = conv_nhwc(x, w, 1, 0), conv_nhwc(x.abs(), w.abs(), 1, 0)
-        check_bound(c, ref, a, C_CONV, f'sensitivity {name} unedited', rnd=False)
+        check(c, ref, c_bound(a, C_CONV), f'sensitivity {name} unedited')
         rejected(drop_k_slice(c, x, w, 128, spec[3] // 2), ref, a, C_CONV,
                  f'sensitivity {name} K={spec[3]}: one 32-wide K slice of one 128-row tile left out')
     d = run_unit(UNITS['layer2.0.conv2'], 2, 901)                # 112 -> 56, 8 x 8 output tiles
     x, w, c = d['x'], d['w'], d['c']
     ref, a = conv_nhwc(x, w, 2, 1), conv_nhwc(x.abs(), w.abs(), 2, 1)
-    check_bound(c, ref, a, C_CONV, 'sensitivity layer2.0.conv2 unedited')
+    check(c, ref, rnd_bound(a, C_CONV), 'sensitivity layer2.0.conv2 unedited')
     rejected(drop_tap(c, x, w, 2, 8, 16, 8, 8, (0, 2), 32), ref, a, C_CONV,
              'sensitivity layer2.0.conv2: tap (0, 2) of channels 32..63 left out over one 8x8 tile', rnd=True)
     rejected(wrong_phase_row(c, x, w, 9), ref, a, C_CONV, 'sensitivity layer2.0.conv2: row 9 at the wrong stride phase',
@@ -719,7 +697,7 @@ def test_gpu_bounds_reject_conv_defects():
     d = run_unit(UNITS['stem'], 2, 902)
     x, w, c = _nhwc_in(d, 'stem'), d['w'], d['c']
     ref, a = conv_nhwc(x, w, 2, 3), conv_nhwc(x.abs(), w.abs(), 2, 3)
-    check_bound(c, ref, a, C_CONV, 'sensitivity stem unedited', rnd=False)
+    check(c, ref, c_bound(a, C_CONV), 'sensitivity stem unedited')
     rejected(drop_stem_column(c, d['rec']['xin'], w.reshape(64, 147), 4096, 73), ref, a, C_CONV,
              'sensitivity stem: im2col column 73 left out over 128 pixels')
 
@@ -735,7 +713,7 @@ def test_gpu_bounds_reject_bn_defects():
     m, v = bn_stats_ref(c)
     sig, inv = v.sqrt(), (v + BN_EPS).rsqrt()
     ch, nm = 7, ('channel',)
-    check_bound(mean, m, sig, C_SUMS, 'sensitivity BN mean unedited', rnd=False, names=nm)
+    check(mean, m, c_bound(sig, C_SUMS), 'sensitivity BN mean unedited', names=nm)
     bad = mean.clone()
     bad[ch] += float(1e-4 * sig[ch])
     rejected(bad, m, sig, C_SUMS, 'sensitivity BN: one mean moved by 1e-4 sigma', names=nm)
@@ -744,7 +722,7 @@ def test_gpu_bounds_reject_bn_defects():
     rejected(bad, inv, inv, C_SUMS, 'sensitivity BN: one invstd x (1 + 1e-4)', names=nm)
     gp = torch.where(d['mask'], d['dy'], torch.zeros((), device='cuda'))
     db, dg, ab, ag = bn_bwd_sums(c, gp, mean, invstd)
-    _, nb = _ws('hk_bn_workspace_bytes', P, cout)
+    _, nb = workspace('hk_bn_workspace_bytes', P, cout)
     nblk = nb // (2 * cout * 4)
     assert P == 6272 and nblk == 25
     xh = (c.double() - mean.double()) * invstd.double()
@@ -770,18 +748,18 @@ def test_gpu_bounds_reject_wgrad_defects():
     # the stem at 448x448 batch 32: hk_matconv_wgrad over P = 1,605,632 pixels in S splits
     d = run_unit(UNITS['stem'], 32, 904)
     P, dc = d['rec']['P'], d['dc']
-    _, nb = _ws('hk_matconv_wgrad_workspace_bytes', P, 160, 64)
+    _, nb = workspace('hk_matconv_wgrad_workspace_bytes', P, 160, 64)
     S = nb // (64 * 160 * 4)
     assert S == 256, S
     gw, aw = _wgrad_refs(_nhwc_in(d, 'stem'), dc, 7, 2, 3)
     dw = d['dw'].view(64, 147)
     gw, aw = gw.view(64, 147), aw.view(64, 147)
-    check_bound(dw, gw, aw, C_WGRAD, 'sensitivity stem dW unedited', rnd=False, names=('co', 'k'))
+    check(dw, gw, c_bound(aw, C_WGRAD), 'sensitivity stem dW unedited', names=('co', 'k'))
     rejected(drop_split(dw, d['rec']['xin'][:, :147], dc, S, 100), gw, aw, C_WGRAD,
              f'sensitivity stem dW: one split of {S} left out', names=('co', 'k'))
     # layer4's 3x3 at 14x14, batch 32: the last, partial tile row (rows 12-13) of one image
     d = run_unit(UNITS['layer4.1.conv2'], 32, 905)
     gw, aw = _wgrad_refs(d['x'], d['dc'], 3, 1, 1)
-    check_bound(d['dw'], gw, aw, C_WGRAD, 'sensitivity layer4.1.conv2 dW unedited', rnd=False, names=names)
+    check(d['dw'], gw, c_bound(aw, C_WGRAD), 'sensitivity layer4.1.conv2 dW unedited', names=names)
     rejected(drop_rows(d['dw'], d['x'], d['dc'], 3, 12, 14), gw, aw, C_WGRAD,
              'sensitivity layer4.1.conv2 dW: rows 12-13 of image 3 left out', names=names)

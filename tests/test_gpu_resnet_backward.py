@@ -18,6 +18,7 @@ import torch.nn.functional as F
 import detgen
 import matched
 from conftest import rel_l2
+from kernel_check import nchw, nhwc, precise  # noqa: F401  (a fixture)
 
 pytestmark = pytest.mark.gpu
 
@@ -30,22 +31,6 @@ SHALLOW = (2, 1, 1, 1)      # stem, 1x1 downsample at stride 1, an identity bloc
 # above that and stays 5x below the ~3e-4 that a single un-split TF32 operand anywhere in the unit would leave, so a precise
 # path that drops to single-pass TF32 fails.
 UNIT_TOL = {0: 2e-3, 1: 5e-5}
-
-
-def _nhwc(t):
-    return t.permute(0, 2, 3, 1).contiguous()
-
-
-def _nchw(t):
-    return t.permute(0, 3, 1, 2).contiguous()
-
-
-@pytest.fixture
-def precision(request):
-    from hawkeye_b200 import _lib
-    _lib.set_precise(request.param)
-    yield request.param
-    _lib.set_precise(0)
 
 
 @pytest.fixture
@@ -97,8 +82,8 @@ def _unit_errors(unit, x64, r64, seed):
     r32 = r64.float() if r64 is not None else None
     need_dx = unit.kind != 'stem'
     with torch.no_grad():
-        xin = x32.cuda() if unit.kind == 'stem' else _nhwc(x32).cuda()
-        y, rec = unit.forward(xin, w, g, b, _nhwc(r32).cuda() if r32 is not None else None, True)
+        xin = x32.cuda() if unit.kind == 'stem' else nhwc(x32).cuda()
+        y, rec = unit.forward(xin, w, g, b, nhwc(r32).cuda() if r32 is not None else None, True)
     dy = detgen.det(y.shape, seed)                                  # NHWC, like y
     # fp64 reference on the same fp32 values, on the ReLU branch this forward took
     xd = x32.double().requires_grad_(need_dx)
@@ -109,10 +94,10 @@ def _unit_errors(unit, x64, r64, seed):
     if rd is not None:
         z = z + rd
     if unit.relu:
-        z = z * _nchw(y > 0).cpu().double()
+        z = z * nchw(y > 0).cpu().double()
     inputs = [wd, gd, bd] + ([xd] if need_dx else []) + ([rd] if rd is not None else [])
     ref = dict(zip(['dw', 'dgamma', 'dbeta'] + (['dx'] if need_dx else []) + (['dres'] if rd is not None else []),
-                   torch.autograd.grad(z, inputs, _nchw(dy).double())))
+                   torch.autograd.grad(z, inputs, nchw(dy).double())))
     # an addend of dx's own size on the 1x1 units: a dropped or doubled addend is an O(1) error, a wrong dx still shows
     addend = None
     if need_dx and unit.kind.startswith('1x1'):
@@ -120,13 +105,13 @@ def _unit_errors(unit, x64, r64, seed):
         ref['dx'] = ref['dx'] + addend.double()
     with torch.no_grad():
         dx, dres, dw, dg, db = unit.backward(rec, dy.cuda(), need_dx=need_dx,
-                                             addend=_nhwc(addend).cuda() if addend is not None else None)
+                                             addend=nhwc(addend).cuda() if addend is not None else None)
     torch.cuda.synchronize()
     got = {'dw': dw, 'dgamma': dg, 'dbeta': db}
     if need_dx:
-        got['dx'] = _nchw(dx)
+        got['dx'] = nchw(dx)
     if rd is not None:
-        got['dres'] = _nchw(dres)
+        got['dres'] = nchw(dres)
     assert set(got) == set(ref)
     return {k: rel_l2(got[k].cpu(), ref[k]) for k in ref}
 
@@ -153,8 +138,8 @@ def _by_kind(errs):
     return worst
 
 
-@pytest.mark.parametrize('size,precision', [(224, 0), (224, 1), (448, 0)], indirect=['precision'])
-def test_unit_backward(size, precision):
+@pytest.mark.parametrize('size,precise', [(224, 0), (224, 1), (448, 0)], indirect=['precise'])
+def test_unit_backward(size, precise):
     """224x224 / batch 2: every unit of the shallow trunk.  448x448: the layer1 3x3 at 112x112, the only ResNet map the v2
     forward kernel takes (W % 16 == 0, default mode only)."""
     torch.set_num_threads(16)
@@ -162,9 +147,9 @@ def test_unit_backward(size, precision):
     x = detgen.det((2, 3, size, size), 61)
     errs = _units(trunk, st, x, SHALLOW, only=None if size == 224 else ['4.0.bn2'])
     worst = _by_kind(errs)
-    print(f'unit backward {size}x{size} precise={precision}, worst per kind: ' +
+    print(f'unit backward {size}x{size} precise={precise}, worst per kind: ' +
           ', '.join(f'{k} {v[0]:.2e} ({v[1]} {v[2]})' for k, v in sorted(worst.items())))
-    bad = {k: e for k, e in errs.items() if not max(e.values()) < UNIT_TOL[precision]}
+    bad = {k: e for k, e in errs.items() if not max(e.values()) < UNIT_TOL[precise]}
     assert len(errs) == (20 if size == 224 else 1) and not bad, bad
 
 
@@ -198,12 +183,12 @@ def _bn_modules(trunk):
     return {name: m for name, m in trunk.named_modules() if isinstance(m, torch.nn.BatchNorm2d)}
 
 
-@pytest.mark.parametrize('precision', [0, 1], indirect=True)
-def test_shallow_trunk_train_and_eval(precision):
+@pytest.mark.parametrize('precise', [0, 1], indirect=True)
+def test_shallow_trunk_train_and_eval(precise):
     from hawkeye_b200 import ops
     from oracle import hop_oracle as O
     torch.set_num_threads(16)
-    tol = TRUNK_TOL[precision]
+    tol = TRUNK_TOL[precise]
     trunk, st = _trunk(SHALLOW)
     x = detgen.det((2, 3, 224, 224), 61)
 
@@ -223,9 +208,9 @@ def test_shallow_trunk_train_and_eval(precision):
     ref_feat, ref, stats = _oracle_trunk(st, x, G, SHALLOW, tape)
     assert tape.done(), 'oracle consumed fewer decisions than the GPU forward recorded'
     ef = rel_l2(feat.detach().cpu(), ref_feat)
-    print(f'shallow trunk precise={precision}: features rel {ef:.2e}')
+    print(f'shallow trunk precise={precise}: features rel {ef:.2e}')
     assert len(grads) == len(ref) == len(list(trunk.parameters()))
-    errs = matched.compare_grads(grads, ref, tol, f'shallow trunk precise={precision}')
+    errs = matched.compare_grads(grads, ref, tol, f'shallow trunk precise={precise}')
     assert ef < tol
 
     # ---- running statistics after that step: momentum 0.1 from (0, 1); the mean's error in units of the batch spread
@@ -237,12 +222,12 @@ def test_shallow_trunk_train_and_eval(precision):
         assert int(m.num_batches_tracked) == 1, name
         worst_m = max(worst_m, ((m.running_mean.cpu().double() - 0.1 * mean).abs() / (0.1 * var.sqrt())).max().item())
         worst_v = max(worst_v, rel_l2(m.running_var.cpu(), 0.9 + 0.1 * unb))
-    print(f'shallow trunk precise={precision}: running mean {worst_m:.2e} (batch sigmas), running var {worst_v:.2e}')
+    print(f'shallow trunk precise={precise}: running mean {worst_m:.2e} (batch sigmas), running var {worst_v:.2e}')
     assert worst_m < tol and worst_v < tol
 
     # ---- per-unit errors on the same batch, for the amplification through the trunk
     unit_worst = max(max(e.values()) for e in _units(trunk, st, x, SHALLOW).values())
-    print(f'shallow trunk precise={precision}: worst gradient {max(errs.values()):.2e}, worst unit {unit_worst:.2e}, '
+    print(f'shallow trunk precise={precise}: worst gradient {max(errs.values()):.2e}, worst unit {unit_worst:.2e}, '
           f'amplification {max(errs.values()) / unit_worst:.1f}x')
 
     # ---- eval mode: running statistics = the fp64 batch statistics of a second batch (activations stay at training scale)
@@ -263,7 +248,7 @@ def test_shallow_trunk_train_and_eval(precision):
         feat_e = trunk(x2.cuda()).cpu()
     ref_e = O.resnet50_trunk_fwd(x2.double(), st64, prefix='', layers=O.resnet_layers(SHALLOW), bn=O._bn_eval)
     ee = rel_l2(feat_e, ref_e)
-    print(f'shallow trunk precise={precision}: eval-mode features rel {ee:.2e}')
+    print(f'shallow trunk precise={precise}: eval-mode features rel {ee:.2e}')
     assert ee < tol
 
 

@@ -14,8 +14,9 @@ import torch.nn.functional as F
 import detgen
 from conftest import load_golden, rel_l2
 from oracle import s3n_oracle as O
+from kernel_check import precise_on  # noqa: F401  (a fixture)
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures('precise_on')]
 GG = 31 * 31
 CFG = dict(num_classes=200, image_size=128, radius=0.12, radius_inv=0.3, base_ratio=0.09)
 SAMPLER_PARAMS = ('radius.scale', 'radius_inv.scale', 'filter.weight')
@@ -23,14 +24,6 @@ SAMPLER_PARAMS = ('radius.scale', 'radius_inv.scale', 'filter.weight')
 
 class Cfg(dict):
     __getattr__ = dict.__getitem__
-
-
-@pytest.fixture(autouse=True)
-def precise():
-    from hawkeye_b200 import _lib
-    _lib.set_precise(1)
-    yield
-    _lib.set_precise(0)
 
 
 def gaussian_filter():

@@ -31,9 +31,8 @@ import torch
 
 import detgen
 import matched
-from matched import rel_l2, tape_items
-from test_gpu_conv_vgg16 import check_bound
-from test_gpu_matched import TOL
+from kernel_check import c_bound, check
+from matched import TOL, rel_l2, tape_items
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BATCH, SIZE, CLASSES = 32, 448, 200
@@ -171,10 +170,10 @@ class Checks:
         if not share <= 1.0:
             self.failed.append(f'{name}: {share:.3g} of its bound {what}')
 
-    def bound(self, name, *args, **kw):
-        """check_bound (test_gpu_conv_vgg16.py) of one tensor; its share is of the whole bound here (rnd=False)"""
+    def bound(self, name, out, ref, absref, c, tag, names):
+        """kernel_check.check of one tensor against c * absref"""
         try:
-            self.add(name, check_bound(*args, **kw))
+            self.add(name, check(out, ref, c_bound(absref, c), tag, names=names))
         except AssertionError as e:
             self.failed.append(f'{name}: {e}')
             self.worst[name] = max(self.worst.get(name, 0.0), _ratio_of(e))
@@ -211,9 +210,9 @@ def rejects(name, share):
 
 
 def _bound_share(out, ref, absref, c):
-    """the worst |out - ref| / (c * absref) that check_bound would report (a check expected to fail)"""
+    """the worst |out - ref| / (c * absref) that kernel_check.check would report (a check expected to fail)"""
     try:
-        check_bound(out, ref, absref, c, 'planted', rnd=False, names=('i',))
+        check(out, ref, c_bound(absref, c), 'planted', names=('i',))
     except AssertionError as e:
         return _ratio_of(e)
     return 0.0
@@ -465,9 +464,9 @@ def test_vgg_train_step_vs_fp64(workload, monkeypatch):
         c = SGD_ULPS * U
         for gi, (a, b, p_ref, buf_ref, pabs, babs) in enumerate(_sgd_refs(tr, layout, p0, g0, b0, first)):
             checks.bound('sgd p', tr.flat.flat[a:b], p_ref, pabs, c, f'{workload} step {step} sgd p group {gi}',
-                         rnd=False, names=('i',))
+                         names=('i',))
             checks.bound('sgd buf', tr.optimizer.buf[a:b], buf_ref, babs, c, f'{workload} step {step} sgd buf group {gi}',
-                         rnd=False, names=('i',))
+                         names=('i',))
         check_padding(checks, pad, params=tr.flat.flat, grad=g0, momentum=tr.optimizer.buf)
         gi = len(tr.optimizer.param_groups) - 1
         a, b, p_ref, _, pabs, _ = _sgd_refs(tr, layout, p0, g0, b0, first, lr_scale={gi: 0.1})[gi]
@@ -575,7 +574,7 @@ def test_mpn_graph_replay_and_adam(monkeypatch):
     dev_state = (tr.flat.flat, tr.optimizer.m, tr.optimizer.v)
     for gi, (a, b, refs, scales) in enumerate(_adam_refs(tr, snap['p'], snap['m'], snap['v'], g_replay, t)):
         for nm, got, ref, sc in zip(('p', 'm', 'v'), dev_state, refs, scales):
-            checks.bound(f'adam {nm}', got[a:b], ref, sc, c, f'mpn adam {nm} group {gi}', rnd=False, names=('i',))
+            checks.bound(f'adam {nm}', got[a:b], ref, sc, c, f'mpn adam {nm} group {gi}', names=('i',))
     check_padding(checks, pad, params=tr.flat.flat, grad=g_replay, m=tr.optimizer.m, v=tr.optimizer.v)
     a, b, refs, scales = _adam_refs(tr, snap['p'], snap['m'], snap['v'], g_replay, t - 1)[0]
     rejects('Adam step count off by one', _bound_share(tr.flat.flat[a:b], refs[0], scales[0], c))
