@@ -4,7 +4,6 @@ refinement against the fixture with the reference's draws replayed, the attentio
 A3..A5, bitwise repeatability, the full model in precise mode against the end-to-end fixture, and the behaviour of a step:
 two BatchNorm updates, gradient into layer2 from stage II, no host synchronisation, CUDA-graph replay, the trainer."""
 import json
-import os
 
 import numpy as np
 import pytest
@@ -16,11 +15,11 @@ import detgen
 from conftest import load_golden, rel_l2
 from oracle import apcnn_oracle as O
 from kernel_check import nhwc, precise_on  # noqa: F401  (a fixture)
+from step_check import (assert_trainer_replays, capture, make_trainer, no_host_sync, random_init,  # noqa: F401
+                        replay_against_eager, side_stream)
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures('random_init')]
 G = load_golden('reference_apcnn')
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-os.environ['HAWKEYE_ALLOW_RANDOM_INIT'] = '1'
 
 
 def _draws(rec, counts):
@@ -269,13 +268,10 @@ def test_train_step_448_batch_16_no_sync():
     crit(net(x, labels), labels).backward()                          # warm-up: workspaces, first-call attributes
     torch.cuda.synchronize()
     before = net.cls3[2].num_batches_tracked.item()
-    torch.cuda.set_sync_debug_mode('error')
-    try:
+    with no_host_sync():
         out = net(x, labels)
         loss = crit(out, labels)
         loss.backward()
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     assert net.cls3[2].num_batches_tracked.item() == before + 2 and net.layer4[2].bn3.num_batches_tracked.item() == before + 2
     assert net.fpn.P5_1.conv_gpb.bn.num_batches_tracked.item() == before + 2 and net.bn1.num_batches_tracked.item() == 2
     assert torch.isfinite(loss).item() and crit.last_correct.dtype == torch.int32
@@ -293,66 +289,27 @@ def test_graph_replay_equals_eager_and_draws_afresh():
     labels = detgen.det_labels(I.E2E_BATCH, I.E2E_CLASSES, 4401).cuda()
     _, counts = _fixture_rois('e2e')
     fixed = _draws(G['e2e_draws'], counts)
-    params = list(net.parameters())
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            for p in params:
-                p.grad = None
-            crit(net(x, labels, draws=fixed), labels).backward()
-        state = {k: v.clone() for k, v in net.state_dict().items()}
-        for p in params:
-            p.grad.zero_()
+
+    def step():
+        net.zero_grad()
         out = net(x, labels, draws=fixed)
         loss = crit(out, labels)
         loss.backward()
-        eager = [o.detach().clone() for o in out[1]] + [loss.detach().clone(), out[3][0][0].clone()]
-        eager_g = [p.grad.clone() for p in params]
-        net.load_state_dict(state)
-        g = torch.cuda.CUDAGraph()
-        for p in params:
-            p.grad.zero_()
-        with torch.cuda.graph(g, stream=s):
-            gout = net(x, labels, draws=fixed)
-            gloss = crit(gout, labels)
-            gloss.backward()
-        net.load_state_dict(state)
-        for p in params:
-            p.grad.zero_()
-        g.replay()
-        s.synchronize()
-        got = [o.detach() for o in gout[1]] + [gloss.detach(), gout[3][0][0]]
-        for a, b in zip(got, eager):
-            assert torch.equal(a, b)
-        for p, e in zip(params, eager_g):                  # the 3x3 weight gradients add their tiles with atomics
-            assert rel_l2(p.grad, e) < 1e-5
-        # without explicit draws the captured torch.rand draws afresh on every replay: the stage-II logits change
-        g2 = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g2, stream=s):
-            with torch.no_grad():
-                free = net(x, labels)
-        seen = set()
+        return out[1] + [loss, out[3][0][0]]
+    # the 3x3 weight gradients add their tiles with atomics
+    replay_against_eager(step, net, net.parameters(), grad_bound=1e-5)
+    # without explicit draws the captured torch.rand draws afresh on every replay: the stage-II logits change
+    seen = set()
+    with side_stream(), torch.no_grad():
+        graph, free = capture(lambda: net(x, labels))
         for _ in range(6):
-            g2.replay()
-            s.synchronize()
+            graph.replay()
             seen.add(tuple(free[1][4].flatten()[:4].tolist()))
-        assert len(seen) > 1
-    torch.cuda.current_stream().wait_stream(s)
+    assert len(seen) > 1
 
 
-def test_trainer_captures_and_replays():
-    from hawkeye_b200 import examples
-    from hawkeye_b200.config import load_config
+def test_trainer_captures_and_replays(monkeypatch):
     data = dict(img=detgen.det((4, 3, 224, 224), 4600).cuda(), label=detgen.det_labels(4, 200, 4601).cuda())
-    os.environ['HK_CUDA_GRAPH'] = '1'
-    try:
-        tr = examples.APCNNTrainer(load_config(os.path.join(REPO, 'configs', 'APCNN.yaml')), dataloaders={})
-        tr.on_start_epoch(None)
-        for _ in range(6):
-            tr.batch_training(data)
-    finally:
-        del os.environ['HK_CUDA_GRAPH']
-    assert tr._graph is not None and tr._graph['kernels'] > 0
+    tr = make_trainer(monkeypatch, 'APCNN', 'APCNN.yaml', graph=True)
+    assert_trainer_replays(tr, [data] * 6)
     assert [g['lr'] for g in tr.optimizer.param_groups] == pytest.approx([0.0005 / 10, 0.0005])
-    assert np.isfinite(tr.average_meters['loss'].avg) and 0 <= tr.average_meters['acc'].avg <= 100

@@ -2,9 +2,6 @@
 gather / scatter, the gate and dropout kernels against the oracle fed the numpy-regenerated masks, the head and the loss
 against fixtures of the unmodified reference (tests/golden/make_golden_apinet.py), the 224x224 train step (no host
 synchronisation, frozen backbone in the warm-up), CUDA-graph replay and evaluation through Tester."""
-import copy
-import os
-
 import numpy as np
 import pytest
 import torch
@@ -13,10 +10,10 @@ import torch.nn as nn
 import detgen
 from conftest import load_golden, rel_l2
 from oracle import apinet_oracle as A
+from step_check import eager_and_graph_losses, make_trainer, no_host_sync
 
 pytestmark = pytest.mark.gpu
 G = load_golden('reference_apinet')
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _s():
@@ -205,14 +202,8 @@ def test_loss_matches_reference(precise):
 
 
 def _trainer(monkeypatch, graph=False, p=0.5):
-    from hawkeye_b200 import examples
-    from hawkeye_b200.config import load_config
-    monkeypatch.setenv('HAWKEYE_ALLOW_RANDOM_INIT', '1')
-    monkeypatch.setenv('HK_CUDA_GRAPH', '1' if graph else '0')
-    cfg = load_config(os.path.join(REPO, 'configs', 'APINet.yaml'))
-    tr = examples.APINetTrainer(cfg, dataloaders={})
+    tr = make_trainer(monkeypatch, 'APINet', 'APINet.yaml', graph=graph)
     tr.model.drop.p = p
-    tr.model.train()
     return tr
 
 
@@ -235,12 +226,9 @@ def test_train_step_224(monkeypatch):
     for g in tr.optimizer.param_groups:                         # after the warm-up: everything trains
         g['lr'] = 1e-4
     tr.model.drop.p = 0.5
-    torch.cuda.set_sync_debug_mode('error')                     # no host synchronisation inside the step
-    try:
+    with no_host_sync():
         for _ in range(3):
             losses.append(tr.batch_training({'img': x, 'label': y}))
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     losses[1:] = [float(v.item()) for v in losses[1:]]
     print('apinet 224 losses', losses, 'oracle', ref)
     assert all(not torch.equal(a, b.detach()) for a, b in zip(backbone, tr.model.backbone.parameters()))
@@ -251,22 +239,15 @@ def test_train_step_224(monkeypatch):
 def test_graph_replay_matches_eager(monkeypatch):
     x = detgen.det((8, 3, 224, 224), 421).cuda()
     y = torch.arange(4).repeat_interleave(2).cuda()
-    losses, state0 = {}, None
-    for graph in (False, True):
-        torch.manual_seed(0)
+
+    def build(graph):
         tr = _trainer(monkeypatch, graph=graph, p=0.0)
-        if state0 is None:
-            state0 = copy.deepcopy(tr.model.state_dict())
-        else:
-            tr.model.load_state_dict(state0)
         tr.optimizer.param_groups[1]['lr'] = 1e-4     # a warm-up epoch: backbone frozen (lr 0), the head trains
-        losses[graph] = [float(tr.batch_training({'img': x, 'label': y}).item()) for _ in range(6)]
-        if graph:
-            assert tr._graph is not None
-        del tr
-    print('apinet graph', losses)
-    for a, b in zip(losses[False], losses[True]):
-        assert abs(a - b) <= 1e-5 * abs(a), losses
+        return tr
+    (eager, _), (replayed, _) = eager_and_graph_losses(build, [{'img': x, 'label': y}] * 6)
+    print('apinet graph', eager, replayed)
+    for a, b in zip(eager, replayed):
+        assert abs(a - b) <= 1e-5 * abs(a), (eager, replayed)
     # p = 0.5 inside the graph: the seed is drawn on the device, so two replays draw different masks
     tr = _trainer(monkeypatch, graph=True, p=0.5)
     for g in tr.optimizer.param_groups:

@@ -2,6 +2,7 @@
 the same draws: the crop-resize bit for bit against PIL, every TrivialAugmentWide op at every magnitude bin and sign, the
 erasing rectangle, the whole train and eval presets, a BCNN train step fed by the device presets (eager and graph
 replay, no host synchronisation) and the Tester with both presets.  The images are synthetic JPEGs drawn from a seed."""
+import contextlib
 import os
 
 import numpy as np
@@ -12,6 +13,7 @@ from PIL import Image
 import detgen
 from conftest import rel_l2
 from hawkeye_b200 import data, ops_augment as A
+from step_check import no_host_sync
 
 pytestmark = pytest.mark.gpu
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -244,13 +246,8 @@ def test_bcnn_train_step_with_the_device_presets(folder, tmp_path, monkeypatch):
         w0 = tr.model.classifier.weight.detach().clone()
         for i, batch in enumerate(tr.dataloaders['train']):
             assert isinstance(batch['img'], A.PackedImages) and batch['img'].data.is_pinned()
-            check = i not in (0, 2)
-            if check:
-                torch.cuda.set_sync_debug_mode('error')
-            try:
+            with no_host_sync() if i not in (0, 2) else contextlib.nullcontext():
                 tr.batch_training(batch)
-            finally:
-                torch.cuda.set_sync_debug_mode(0)
         torch.cuda.synchronize()
         assert len(images) == 6 and all(x.shape == (4, 3, 448, 448) for x in images)
         assert (tr._graph is not None) == graph and np.isfinite(tr.average_meters['loss'].avg)

@@ -2,8 +2,6 @@
 trains (tests/golden/make_golden_cin_loss.py) in both precision modes, a near-cancelling pair against the fp64 oracle, the
 channel-interaction module's train-mode backward at batch 20, C = 2048, 7x7, and the trainer: a step without host
 synchronisation, CUDA-graph replay, the zero-pair weight decay of h, checkpoints and the Tester."""
-import os
-
 import numpy as np
 import pytest
 import torch
@@ -12,11 +10,10 @@ import cin_inputs as I
 import detgen
 from conftest import load_golden, rel_l2
 from oracle import cin_oracle as O
+from step_check import assert_trainer_replays, make_trainer, no_host_sync, random_init, replay_against_eager  # noqa: F401
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures('random_init')]
 G = load_golden('reference_cin_loss')
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-os.environ['HAWKEYE_ALLOW_RANDOM_INIT'] = '1'
 
 
 def _criterion():
@@ -122,21 +119,16 @@ def test_module_train_backward_full_size(precise):
     assert max(errs[k] for k in ('dx', 'dx_sums', 'conv.weight', 'conv.bias', 'fc.weight', 'fc.bias')) < tol_b
 
 
-def _trainer(**over):
-    from hawkeye_b200 import examples
-    from hawkeye_b200.config import load_config
-    cfg = load_config(os.path.join(REPO, 'configs', 'CIN.yaml'))
-    for k, v in over.items():
-        cfg.experiment[k] = v
-    return examples.CINTrainer(cfg, dataloaders={})
+def _trainer(monkeypatch, graph=False, **experiment):
+    return make_trainer(monkeypatch, 'CIN', 'CIN.yaml', graph=graph, experiment=experiment)
 
 
 def _batch(name, seed=6100):
     return dict(img=detgen.det((I.B, 3, 224, 224), seed).cuda(), label=I.labels(name).cuda())
 
 
-def test_trainer_step_no_sync_and_h_updates(tmp_path):
-    tr = _trainer(log_dir=str(tmp_path))
+def test_trainer_step_no_sync_and_h_updates(tmp_path, monkeypatch):
+    tr = _trainer(monkeypatch, log_dir=str(tmp_path))
     assert tr.optimizer.param_groups[1]['params'] == [tr.criterion.h.weight, tr.criterion.h.bias]
     lr, wd = tr.optimizer.param_groups[1]['lr'], tr.optimizer.param_groups[1]['weight_decay']
     assert tr.optimizer.defaults['momentum'] == 0.0 and wd == 0.0002
@@ -144,11 +136,8 @@ def test_trainer_step_no_sync_and_h_updates(tmp_path):
     batch = _batch('balanced', 6101)
     torch.cuda.synchronize()
     h0 = tr.criterion.h.weight.detach().clone()
-    torch.cuda.set_sync_debug_mode('error')
-    try:
+    with no_host_sync():
         tr.batch_training(batch)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     for p in list(tr.model.parameters()) + list(tr.criterion.parameters()):
         assert p.grad is not None
     assert not tr.criterion.h.weight.grad.any() and not tr.criterion.h.bias.grad.any()
@@ -165,14 +154,14 @@ def test_trainer_step_no_sync_and_h_updates(tmp_path):
     # checkpoint: h restored with the model; without 'criterion' the fresh h stays, with a warning
     path = tr.save_checkpoint()
     saved = tr.criterion.h.weight.detach().clone()
-    tr2 = _trainer(log_dir=str(tmp_path), resume=path)
+    tr2 = _trainer(monkeypatch, log_dir=str(tmp_path), resume=path)
     assert torch.equal(tr2.criterion.h.weight, saved) and tr2.start_epoch == tr.epoch
     assert tr2.criterion.h.weight.data_ptr() >= tr2.flat.flat.data_ptr()       # still a view of the flat buffer
     ck = torch.load(path, map_location='cpu')
     del ck['criterion']
     path2 = str(tmp_path / 'no_criterion.pth')
     torch.save(ck, path2)
-    tr3 = _trainer(log_dir=str(tmp_path), resume=path2)
+    tr3 = _trainer(monkeypatch, log_dir=str(tmp_path), resume=path2)
     assert not torch.equal(tr3.criterion.h.weight.cpu(), saved.cpu())
 
     # the Tester scores the model save_model writes (the reference's format: the model alone)
@@ -196,50 +185,20 @@ def test_graph_replay_equals_eager():
     net = hb.MODEL.get('CIN')(CfgNode(dict(name='CIN', num_classes=200))).cuda().train()
     crit = _criterion()
     x, labels = detgen.det((I.B, 3, 224, 224), 6200).cuda(), I.labels('some').cuda()
-    params = list(net.parameters()) + list(crit.parameters())
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            for p in params:
-                p.grad = None
-            crit(net(x), labels).backward()
-        assert all(p.grad is not None for p in crit.parameters())        # h.bias too, though its gradient is zero
-        state = {k: v.clone() for k, v in net.state_dict().items()}
-        for p in params:
-            p.grad.zero_()
+
+    def step():
+        net.zero_grad()
+        crit.zero_grad()
         out = net(x)
         loss = crit(out, labels)
         loss.backward()
-        eager = [out[0].detach().clone(), loss.detach().clone()]
-        eager_g = [p.grad.clone() for p in params]
-        net.load_state_dict(state)
-        g = torch.cuda.CUDAGraph()
-        for p in params:
-            p.grad.zero_()
-        with torch.cuda.graph(g, stream=s):
-            gout = net(x)
-            gloss = crit(gout, labels)
-            gloss.backward()
-        net.load_state_dict(state)
-        for p in params:
-            p.grad.zero_()
-        g.replay()
-        s.synchronize()
-        assert torch.equal(gout[0], eager[0]) and torch.equal(gloss, eager[1])
-        assert crit.h.weight.grad.abs().sum() > 0
-        for p, e in zip(params, eager_g):                  # the 3x3 weight gradients add their tiles with atomics
-            assert rel_l2(p.grad, e) < 1e-5
-    torch.cuda.current_stream().wait_stream(s)
+        return [out[0], loss]
+    # the 3x3 weight gradients add their tiles with atomics
+    replay_against_eager(step, net, list(net.parameters()) + list(crit.parameters()), grad_bound=1e-5)
+    assert all(p.grad is not None for p in crit.parameters())           # h.bias too, though its gradient is zero
+    assert crit.h.weight.grad.abs().sum() > 0
 
 
-def test_trainer_captures_and_replays(tmp_path):
-    os.environ['HK_CUDA_GRAPH'] = '1'
-    try:
-        tr = _trainer(log_dir=str(tmp_path))
-        for i in range(5):
-            tr.batch_training(_batch('balanced', 6300 + i))
-    finally:
-        del os.environ['HK_CUDA_GRAPH']
-    assert tr._graph is not None and tr._graph['kernels'] > 0
-    assert np.isfinite(tr.average_meters['loss'].avg)
+def test_trainer_captures_and_replays(tmp_path, monkeypatch):
+    tr = _trainer(monkeypatch, graph=True, log_dir=str(tmp_path))
+    assert_trainer_replays(tr, [_batch('balanced', 6300 + i) for i in range(5)])

@@ -3,8 +3,6 @@ modes, the loss against fixtures of the unmodified reference (tests/golden/make_
 regularisers, the 1024 -> 1024 3x3 convolution of the fusion head against fp64, the model's train- and eval-mode step
 against the reference's fp64 run, and the CrossX trainer: no host synchronisation, CUDA-graph replay, and save_model read
 back by the Tester."""
-import os
-
 import numpy as np
 import pytest
 import torch
@@ -14,11 +12,10 @@ import detgen
 from conftest import load_golden, rel_l2
 from oracle import crossx_oracle as O
 from kernel_check import precise  # noqa: F401  (a fixture)
+from step_check import make_trainer, no_host_sync, random_init, replay_against_eager  # noqa: F401
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures('random_init')]
 G = load_golden('reference_crossx')
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-os.environ['HAWKEYE_ALLOW_RANDOM_INIT'] = '1'
 
 # fp32 elementwise kernels: a few ulps; the logit gradients are rounded to tf32 in the default mode
 TOL = 1e-5
@@ -292,34 +289,23 @@ def test_p1_p3_logits_and_input_check(precise):
             _net(2)(torch.zeros(1, 3, 480, 480, device='cuda'))
 
 
-def _trainer(log_dir, dataloaders=None):
-    from hawkeye_b200 import examples
-    from hawkeye_b200.config import load_config
-    cfg = load_config(os.path.join(REPO, 'configs', 'CrossX.yaml'))
-    cfg.experiment['log_dir'] = log_dir
-    cfg.model['pretrained'] = False
-    return examples.CrossXTrainer(cfg, dataloaders=dataloaders if dataloaders is not None else {})
-
-
 def _batch(seed, n=8):
     return dict(img=detgen.det((n, 3, 448, 448), seed).cuda(), label=detgen.det_labels(n, 200, seed + 1).cuda())
 
 
-def test_trainer_step_no_sync_and_tester(tmp_path):
+def test_trainer_step_no_sync_and_tester(tmp_path, monkeypatch):
     from hawkeye_b200.cfgnode import CfgNode
     from hawkeye_b200.test import Tester
     x = detgen.det((4, 3, 448, 448), 8600)
     val = [{'img': x, 'label': torch.zeros(4, dtype=torch.int64)}]
-    tr = _trainer(str(tmp_path), {'val': val})
+    tr = make_trainer(monkeypatch, 'CrossX', 'CrossX.yaml', graph=False, experiment=dict(log_dir=str(tmp_path)),
+                      dataloaders={'val': val}, pretrained=False)
     tr.batch_training(_batch(8610))
     batch = _batch(8612)
     torch.cuda.synchronize()
     w0 = tr.model.fc_cmbn.weight.detach().clone()
-    torch.cuda.set_sync_debug_mode('error')
-    try:
+    with no_host_sync():
         tr.batch_training(batch)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     assert not torch.equal(tr.model.fc_cmbn.weight, w0)
     assert np.isfinite(tr.average_meters['loss'].avg) and 0 <= tr.average_meters['acc'].avg <= 100
     with torch.no_grad():
@@ -343,34 +329,12 @@ def test_graph_replay_equals_eager():
     crit = CrossXLoss(CfgNode(dict(num_parts=2, gamma=list(I.GAMMA))))
     b = _batch(8700, 4)
     x, labels = b['img'], b['label']
-    params = list(net.parameters())
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            for p in params:
-                p.grad = None
-            crit(net(x), labels).backward()
-        for p in params:
-            p.grad.zero_()
+
+    def step():
+        net.zero_grad()
         out = net(x)
         loss = crit(out, labels)
         loss.backward()
-        eager = [out[0].detach().clone(), loss.detach().clone(), crit.last_correct.clone()]
-        eager_g = [p.grad.clone() for p in params]
-        g = torch.cuda.CUDAGraph()
-        for p in params:
-            p.grad.zero_()
-        with torch.cuda.graph(g, stream=s):
-            gout = net(x)
-            gloss = crit(gout, labels)
-            gcorrect = crit.last_correct
-            gloss.backward()
-        for p in params:
-            p.grad.zero_()
-        g.replay()
-    torch.cuda.current_stream().wait_stream(s)
-    torch.cuda.synchronize()
-    assert torch.equal(gout[0], eager[0]) and torch.equal(gloss, eager[1]) and torch.equal(gcorrect, eager[2])
-    for p, e in zip(params, eager_g):                     # the 3x3 weight gradients add their tiles with atomics
-        assert rel_l2(p.grad, e) < 1e-5
+        return [out[0], loss, crit.last_correct]
+    # the 3x3 weight gradients add their tiles with atomics
+    replay_against_eager(step, net, net.parameters(), grad_bound=1e-5)

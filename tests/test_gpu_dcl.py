@@ -2,9 +2,6 @@
 fixtures of the unmodified reference (tests/golden/make_golden_dcl.py) and fp64 autograd, the loss on row slices of the
 stacked classifier output, the full model against the reference's end-to-end fixture, the 448x448 train step from DCLTrainer (no host synchronisation), CUDA-graph replay,
 and the host-side errors."""
-import copy
-import os
-
 import pytest
 import torch
 
@@ -12,10 +9,10 @@ import detgen
 from conftest import load_golden, rel_l2
 from oracle import dcl_oracle as D
 from kernel_check import precise  # noqa: F401  (a fixture)
+from step_check import eager_and_graph_losses, make_trainer, no_host_sync
 
 pytestmark = pytest.mark.gpu
 G = load_golden('reference_dcl')
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.mark.parametrize('N', [2, 16])
@@ -93,16 +90,7 @@ def test_loss_many_rows():
 
 
 def _trainer(monkeypatch, graph=False, **model):
-    from hawkeye_b200 import examples
-    from hawkeye_b200.config import load_config
-    monkeypatch.setenv('HAWKEYE_ALLOW_RANDOM_INIT', '1')
-    monkeypatch.setenv('HK_CUDA_GRAPH', '1' if graph else '0')
-    cfg = load_config(os.path.join(REPO, 'configs', 'DCL.yaml'))
-    for k, v in model.items():
-        cfg.model[k] = v
-    tr = examples.DCLTrainer(cfg, dataloaders={})
-    tr.model.train()
-    return tr
+    return make_trainer(monkeypatch, 'DCL', 'DCL.yaml', graph=graph, **model)
 
 
 def _batch(n, seed, K=200, cls_2xmul=False):
@@ -220,12 +208,9 @@ def test_train_step_448(monkeypatch):
     losses = [float(tr.batch_training(data).item())]
     torch.cuda.synchronize()
     assert abs(losses[0] - ref) < 1e-4 * max(1.0, abs(ref)), (losses[0], ref)
-    torch.cuda.set_sync_debug_mode('error')                     # no host synchronisation inside the step
-    try:
+    with no_host_sync():
         for _ in range(5):
             losses.append(tr.batch_training(data))
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     losses[1:] = [float(v.item()) for v in losses[1:]]
     print('dcl 448 losses', losses, 'oracle', ref)
     assert all(torch.isfinite(p).all() for p in tr.model.parameters())
@@ -241,22 +226,12 @@ def test_graph_replay_matches_eager(monkeypatch, cls_2xmul):
     bit-reproducible, so replay and eager agree to 1e-5."""
     x, y, ys, law = _batch(2, 640, cls_2xmul=cls_2xmul)
     data = (x, y, ys, law, ['n'] * 2)
-    losses, state0 = {}, None
-    for graph in (False, True):
-        torch.manual_seed(0)
-        tr = _trainer(monkeypatch, graph=graph, cls_2=not cls_2xmul, cls_2xmul=cls_2xmul)
-        if state0 is None:
-            state0 = copy.deepcopy(tr.model.state_dict())
-        else:
-            tr.model.load_state_dict(state0)
-        tr.optimizer.param_groups[0]['lr'] = 0.0
-        losses[graph] = [float(tr.batch_training(data).item()) for _ in range(6)]
-        if graph:
-            assert tr._graph is not None
-        del tr
-    print('dcl graph', cls_2xmul, losses)
-    for a, b in zip(losses[False], losses[True]):
-        assert abs(a - b) <= 1e-5 * abs(a), losses
+    (eager, _), (replayed, _) = eager_and_graph_losses(
+        lambda graph: _trainer(monkeypatch, graph=graph, cls_2=not cls_2xmul, cls_2xmul=cls_2xmul), [data] * 6,
+        frozen_groups=(0,))
+    print('dcl graph', cls_2xmul, eager, replayed)
+    for a, b in zip(eager, replayed):
+        assert abs(a - b) <= 1e-5 * abs(a), (eager, replayed)
 
 
 def test_errors(monkeypatch):

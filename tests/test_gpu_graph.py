@@ -1,43 +1,19 @@
 """CUDA-graph replay of the train step (Trainer cuda_graph mode) must train exactly like the eager step."""
-import copy
-import os
-
 import pytest
-import torch
 
 import detgen
+from step_check import eager_and_graph_losses, make_trainer
 
 pytestmark = pytest.mark.gpu
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.mark.parametrize('cfg_name,trainer', [('BCNN_S2.yaml', 'BCNN'), ('MPN.yaml', 'MPN')])
 def test_graph_replay_matches_eager(cfg_name, trainer, monkeypatch):
-    from hawkeye_b200 import examples
-    from hawkeye_b200.config import load_config
-    monkeypatch.setenv('HAWKEYE_ALLOW_RANDOM_INIT', '1')
-    cfg = load_config(os.path.join(REPO, 'configs', cfg_name))
     size = 128
     batches = [{'img': detgen.det((4, 3, size, size), 200 + i).cuda(), 'label': detgen.det_labels(4, 200, 300 + i).cuda()}
                for i in range(7)]
-    losses = {}
-    state0 = None
-    for mode in ('0', '1'):
-        monkeypatch.setenv('HK_CUDA_GRAPH', mode)
-        torch.manual_seed(0)
-        tr = examples.TRAINERS[trainer](cfg, dataloaders={})
-        if state0 is None:
-            state0 = copy.deepcopy(tr.model.state_dict())
-        else:
-            tr.model.load_state_dict(state0)
-        tr.model.train()
-        out = []
-        for b in batches:
-            out.append(float(tr.batch_training(b).item()))     # the replayed loss lives in ONE static tensor: read it per step
-        torch.cuda.synchronize()
-        losses[mode] = out
-        if mode == '1':
-            assert tr._graph is not None            # steps 4.. were replays
-    print(trainer, losses)
-    for a, b in zip(losses['0'], losses['1']):
-        assert abs(a - b) < 2e-3 * max(1.0, abs(a)), (losses['0'], losses['1'])
+    (eager, _), (replayed, _) = eager_and_graph_losses(
+        lambda graph: make_trainer(monkeypatch, trainer, cfg_name, graph=graph), batches)    # steps 4.. are replays
+    print(trainer, eager, replayed)
+    for a, b in zip(eager, replayed):
+        assert abs(a - b) < 2e-3 * max(1.0, abs(a)), (eager, replayed)

@@ -3,9 +3,7 @@ C = 1024, odd maps and N from 1 to 16 (dsmooth and the blur / argmax path of the
 argmax on a planted tie, bitwise repeatability, the full model against fixtures of the unmodified reference
 (tests/golden/make_golden_interp_parts.py), the 448x448 batch-16 train step (no host synchronisation, CUDA-graph replay
 bit-identical to eager), the shaping term split over two emulated ranks, Tester on the model's triple, and error paths."""
-import copy
 import json
-import os
 
 import numpy as np
 import pytest
@@ -15,10 +13,10 @@ import detgen
 from conftest import load_golden, rel_l2
 from oracle import interp_parts_oracle as O
 from kernel_check import precise  # noqa: F401  (a fixture)
+from step_check import eager_and_graph_losses, make_trainer, no_host_sync
 
 pytestmark = pytest.mark.gpu
 G = load_golden('reference_interp_parts')
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _unit_inputs(N, C, H, W, K, seed):
@@ -205,14 +203,7 @@ def test_two_rank_shaping_equals_one_rank():
 
 
 def _trainer(monkeypatch, graph=False):
-    from hawkeye_b200 import examples
-    from hawkeye_b200.config import load_config
-    monkeypatch.setenv('HAWKEYE_ALLOW_RANDOM_INIT', '1')
-    monkeypatch.setenv('HK_CUDA_GRAPH', '1' if graph else '0')
-    cfg = load_config(os.path.join(REPO, 'configs', 'InterpPartsNet.yaml'))
-    tr = examples.InterpPartsNetTrainer(cfg, dataloaders={})
-    tr.model.train()
-    return tr
+    return make_trainer(monkeypatch, 'InterpPartsNet', 'InterpPartsNet.yaml', graph=graph)
 
 
 def _batch(n, seed):
@@ -226,12 +217,9 @@ def test_train_step_448_no_sync(monkeypatch):
     losses = [float(tr.batch_training(data).item())]
     assert tr.optimizer.param_groups[1]['lr'] < lr0             # the cosine schedule stepped after the batch
     torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode('error')                      # no host synchronisation inside the step
-    try:
+    with no_host_sync():
         for _ in range(4):
             losses.append(tr.batch_training(data))
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     losses[1:] = [float(v.item()) for v in losses[1:]]
     print('interp-parts 448 losses', losses)
     assert all(np.isfinite(losses))
@@ -244,25 +232,12 @@ def test_graph_replay_matches_eager(monkeypatch):
     """Six steps with and without the graph.  The trunk (conv1, bn1, layer1-3) is held at lr 0, as the other methods' graph
     tests hold theirs: it still runs forward and backward, and the head, trained by the SGD step under the per-iteration
     schedule, and the losses must then be the same bits."""
-    data = _batch(16, 2010)
-    out, state0 = {}, None
-    for graph in (False, True):
-        torch.manual_seed(0)
-        tr = _trainer(monkeypatch, graph=graph)
-        if state0 is None:
-            state0 = copy.deepcopy(tr.model.state_dict())
-        else:
-            tr.model.load_state_dict(state0)
-        tr.optimizer.param_groups[0]['initial_lr'] = tr.optimizer.param_groups[0]['lr'] = 0.0
-        losses = [float(tr.batch_training(data).item()) for _ in range(6)]
-        out[graph] = (losses, {k: v.detach().clone() for k, v in tr.model.state_dict().items()})
-        if graph:
-            assert tr._graph is not None
-        del tr
-    print('interp-parts graph', out[False][0], out[True][0])
-    assert out[False][0] == out[True][0]
-    for k in out[False][1]:
-        assert torch.equal(out[False][1][k], out[True][1][k]), k
+    (eager, eager_state), (replayed, replayed_state) = eager_and_graph_losses(
+        lambda graph: _trainer(monkeypatch, graph=graph), [_batch(16, 2010)] * 6, frozen_groups=(0,))
+    print('interp-parts graph', eager, replayed)
+    assert eager == replayed
+    for k in eager_state:
+        assert torch.equal(eager_state[k], replayed_state[k]), k
 
 
 def test_tester_reads_logits(monkeypatch):

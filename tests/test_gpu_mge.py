@@ -4,7 +4,6 @@ oracle at the 224 and 448 map sizes, the boxes index-exact on fixtures of the un
 and the behaviour of a step: one BatchNorm update per trunk, no host synchronisation, an eval mode without the layer4
 recompute, CUDA-graph replay and the trainer."""
 import json
-import os
 
 import numpy as np
 import pytest
@@ -15,11 +14,10 @@ import mge_inputs as I
 from conftest import load_golden, rel_l2
 from oracle import mge_oracle as O
 from kernel_check import precise_on  # noqa: F401  (a fixture)
+from step_check import assert_trainer_replays, make_trainer, no_host_sync, random_init, replay_against_eager  # noqa: F401
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures('random_init')]
 G = load_golden('reference_mge')
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-os.environ['HAWKEYE_ALLOW_RANDOM_INIT'] = '1'
 
 
 def _cfg(**kw):
@@ -192,13 +190,10 @@ def test_train_step_no_sync(size, batch):
     crit(net(x), labels).backward()                                  # warm-up: workspaces, first-call attributes
     torch.cuda.synchronize()
     before = _nbt(net)
-    torch.cuda.set_sync_debug_mode('error')
-    try:
+    with no_host_sync():
         out = net(x)
         loss = crit(out, labels)
         loss.backward()
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     assert _nbt(net) == [b + 1 for b in before] and before == [1] * 8
     assert torch.isfinite(loss).item() and crit.last_correct.dtype == torch.int32
     assert len(out['logits']) == 10 and tuple(out['boxes'].shape) == (2, batch, 4) and tuple(out['pr_gate'].shape) == (batch, 3)
@@ -234,55 +229,21 @@ def test_graph_replay_equals_eager():
     net, crit = _shallow(), MGECNNLoss()
     x, labels = _e2e_inputs()
     params = [p for p in net.parameters() if p is not net.cls_cat_a.fc.weight and p is not net.cls_cat_a.fc.bias]
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            for p in params:
-                p.grad = None
-            crit(net(x), labels).backward()
-        state = {k: v.clone() for k, v in net.state_dict().items()}
-        for p in params:
-            p.grad.zero_()
+
+    def step():
+        net.zero_grad()
         out = net(x)
         loss = crit(out, labels)
         loss.backward()
-        eager = [o.detach().clone() for o in out['logits']] + [loss.detach().clone(), out['boxes'].clone()]
-        eager_g = [p.grad.clone() for p in params]
-        net.load_state_dict(state)
-        g = torch.cuda.CUDAGraph()
-        for p in params:
-            p.grad.zero_()
-        with torch.cuda.graph(g, stream=s):
-            gout = net(x)
-            gloss = crit(gout, labels)
-            gloss.backward()
-        net.load_state_dict(state)
-        for p in params:
-            p.grad.zero_()
-        g.replay()
-        s.synchronize()
-        got = [o.detach() for o in gout['logits']] + [gloss.detach(), gout['boxes']]
-        for a, b in zip(got, eager):
-            assert torch.equal(a, b)
-        for p, e in zip(params, eager_g):                  # the 3x3 weight gradients add their tiles with atomics
-            assert rel_l2(p.grad, e) < 1e-5
-    torch.cuda.current_stream().wait_stream(s)
+        return out['logits'] + [loss, out['boxes']]
+    # the 3x3 weight gradients add their tiles with atomics
+    replay_against_eager(step, net, params, grad_bound=1e-5)
 
 
-def test_trainer_captures_and_replays():
-    from hawkeye_b200 import examples
-    from hawkeye_b200.config import load_config
+def test_trainer_captures_and_replays(monkeypatch):
     data = dict(img=detgen.det((4, 3, 224, 224), 5500).cuda(), label=detgen.det_labels(4, 200, 5501).cuda())
-    os.environ['HK_CUDA_GRAPH'] = '1'
-    try:
-        tr = examples.MGE_CNNTrainer(load_config(os.path.join(REPO, 'configs', 'MGE_CNN.yaml')), dataloaders={})
-        w0 = tr.model.cls_cat_a.fc.weight.detach().clone()
-        for _ in range(6):
-            tr.batch_training(data)
-    finally:
-        del os.environ['HK_CUDA_GRAPH']
-    assert tr._graph is not None and tr._graph['kernels'] > 0
+    tr = make_trainer(monkeypatch, 'MGE_CNN', 'MGE_CNN.yaml', graph=True)
+    w0 = tr.model.cls_cat_a.fc.weight.detach().clone()
+    assert_trainer_replays(tr, [data] * 6)
     assert [g['lr'] for g in tr.optimizer.param_groups] == pytest.approx([0.0004 * 0.01, 0.0004 * 0.1 * 0.01])
     assert torch.equal(tr.model.cls_cat_a.fc.weight, w0)                 # never trained, never decayed
-    assert np.isfinite(tr.average_meters['loss'].avg) and 0 <= tr.average_meters['acc'].avg <= 100

@@ -4,7 +4,6 @@ ranking loss forward and backward against fp64, the full model in precise mode a
 (tests/golden/make_golden_nts.py), and the behaviour of a step: dropout in eval mode, two BatchNorm updates per step, no host
 synchronisation, CUDA-graph replay equal to the eager step, and the trainer's captured steps."""
 import json
-import os
 
 import numpy as np
 import pytest
@@ -16,14 +15,13 @@ import nts_inputs
 from conftest import load_golden, rel_l2
 from oracle import nts_oracle as O
 from kernel_check import precise_on  # noqa: F401  (a fixture)
+from step_check import assert_trainer_replays, make_trainer, no_host_sync, random_init, replay_against_eager  # noqa: F401
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures('random_init')]
 G = load_golden('reference_nts')
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _net(seed_state=True, **kw):
-    os.environ['HAWKEYE_ALLOW_RANDOM_INIT'] = '1'
     from hawkeye_b200.cfgnode import CfgNode
     from hawkeye_b200.methods.nts import NTSNet
     net = NTSNet(CfgNode(dict(dict(proposal_num=6, cat_num=4, image_size=224), **kw)))
@@ -171,12 +169,9 @@ def test_train_step_no_sync_two_bn_updates():
     crit(net(x), labels).backward()                                  # warm-up: workspaces, first-call attributes
     torch.cuda.synchronize()
     before = net.pretrained_model.bn1.num_batches_tracked.item()
-    torch.cuda.set_sync_debug_mode('error')
-    try:
+    with no_host_sync():
         loss = crit(net(x), labels)
         loss.backward()
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     assert net.pretrained_model.bn1.num_batches_tracked.item() == before + 2
     assert net.pretrained_model.layer4[2].bn3.num_batches_tracked.item() == before + 2
     assert torch.isfinite(loss).item() and crit.last_correct.dtype == torch.int32
@@ -190,53 +185,17 @@ def test_graph_replay_equals_eager():
     crit = NTSLoss(CfgNode(dict(proposal_num=6)))
     x = detgen.det((4, 3, 224, 224), 3400).cuda()
     labels = detgen.det_labels(4, 200, 3401).cuda()
-    params = list(net.parameters())
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            for p in params:
-                p.grad = None
-            crit(net(x), labels).backward()
-        torch.cuda.manual_seed(77)
-        for p in params:
-            p.grad = None
+
+    def step():
+        net.zero_grad()
         out = net(x)
         loss = crit(out, labels)
         loss.backward()
-        eager = [t.detach().clone() for t in (out[0], out[1], out[2], out[4], loss)] + [out[3].clone()]
-        eager_g = [p.grad.clone() for p in params]
-        g = torch.cuda.CUDAGraph()
-        for p in params:
-            p.grad.zero_()
-        with torch.cuda.graph(g, stream=s):
-            gout = net(x)
-            gloss = crit(gout, labels)
-            gloss.backward()
-        torch.cuda.manual_seed(77)
-        for p in params:
-            p.grad.zero_()
-        g.replay()
-    torch.cuda.current_stream().wait_stream(s)
-    torch.cuda.synchronize()
-    got = [t.detach() for t in (gout[0], gout[1], gout[2], gout[4], gloss)] + [gout[3]]
-    for a, b in zip(got, eager):
-        assert torch.equal(a, b)
-    for p, e in zip(params, eager_g):                   # the 3x3 weight gradients add their tiles with atomics
-        assert rel_l2(p.grad, e) < 1e-5
+        return [out[0], out[1], out[2], out[4], loss, out[3]]
+    # dropout draws: the same seed for both; the 3x3 weight gradients add their tiles with atomics
+    replay_against_eager(step, net, net.parameters(), grad_bound=1e-5, seed=77)
 
 
-def test_trainer_captures_and_replays():
-    from hawkeye_b200 import examples
-    from hawkeye_b200.config import load_config
-    os.environ['HAWKEYE_ALLOW_RANDOM_INIT'] = '1'
+def test_trainer_captures_and_replays(monkeypatch):
     data = dict(img=detgen.det((4, 3, 224, 224), 3500).cuda(), label=detgen.det_labels(4, 200, 3501).cuda())
-    os.environ['HK_CUDA_GRAPH'] = '1'
-    try:
-        tr = examples.NTSNetTrainer(load_config(os.path.join(REPO, 'configs', 'NTSNet.yaml')), dataloaders={})
-        for _ in range(6):
-            tr.batch_training(data)
-    finally:
-        del os.environ['HK_CUDA_GRAPH']
-    assert tr._graph is not None and tr._graph['kernels'] > 0
-    assert np.isfinite(tr.average_meters['loss'].avg) and 0 <= tr.average_meters['acc'].avg <= 100
+    assert_trainer_replays(make_trainer(monkeypatch, 'NTSNet', 'NTSNet.yaml', graph=True), [data] * 6)

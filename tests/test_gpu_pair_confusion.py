@@ -2,8 +2,6 @@
 reference (tests/golden/make_golden_pc.py) and the fp64 oracle in both precision modes, ResNet50 against the reference's
 train- and eval-mode step, and the PairConfusion and Baseline trainers: no host synchronisation, CUDA-graph replay, the
 top-1 count, and save_model read back by the Tester."""
-import os
-
 import numpy as np
 import pytest
 import torch
@@ -13,11 +11,10 @@ import pc_inputs as I
 from conftest import load_golden, rel_l2
 from oracle import pc_oracle as O
 from kernel_check import precise  # noqa: F401  (a fixture)
+from step_check import assert_trainer_replays, make_trainer, no_host_sync, random_init, replay_against_eager  # noqa: F401
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures('random_init')]
 G = load_golden('reference_pc')
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-os.environ['HAWKEYE_ALLOW_RANDOM_INIT'] = '1'
 
 # dlogits: the bound of the cross-entropy tests (tests/test_gpu_cin_train.py): rounded to TF32 on store in the default mode
 # (half an ulp of 2^-10, ~3e-4 rms), unrounded fp32 in the precise mode.  The loss is fp32 sums over at most 256 rows.
@@ -144,13 +141,9 @@ def test_resnet50_against_reference(precise):
         assert rel_l2(getattr(net.bn1, k).cpu(), G[f'net64_bn1_{k}']) < TRUNK_TOL_PRECISE
 
 
-def _trainer(yaml, log_dir, dataloaders=None):
-    from hawkeye_b200 import examples
-    from hawkeye_b200.config import load_config
-    cfg = load_config(os.path.join(REPO, 'configs', yaml))
-    cfg.experiment['log_dir'] = log_dir
-    cls = examples.PCResNetTrainer if yaml == 'PC_resnet50.yaml' else examples.BaselineTrainer
-    return cls(cfg, dataloaders=dataloaders if dataloaders is not None else {})
+def _trainer(monkeypatch, yaml, log_dir, graph=False, dataloaders=None):
+    name = 'PairConfusion' if yaml == 'PC_resnet50.yaml' else 'Baseline'
+    return make_trainer(monkeypatch, name, yaml, graph=graph, experiment=dict(log_dir=log_dir), dataloaders=dataloaders)
 
 
 def _batch(seed, n=24):
@@ -158,12 +151,12 @@ def _batch(seed, n=24):
 
 
 @pytest.mark.parametrize('yaml', ['PC_resnet50.yaml', 'Baseline.yaml'])
-def test_trainer_step_no_sync_and_tester(yaml, tmp_path):
+def test_trainer_step_no_sync_and_tester(yaml, tmp_path, monkeypatch):
     from hawkeye_b200.cfgnode import CfgNode
     from hawkeye_b200.test import Tester
     x = detgen.det((8, 3, 224, 224), 7500)
     val = [{'img': x, 'label': torch.zeros(8, dtype=torch.int64)}]
-    tr = _trainer(yaml, str(tmp_path), {'val': val})
+    tr = _trainer(monkeypatch, yaml, str(tmp_path), dataloaders={'val': val})
     if yaml == 'PC_resnet50.yaml':
         groups = tr.optimizer.param_groups
         assert [len(g['params']) for g in groups] == [159, 2] and groups[1]['params'][0] is tr.model.fc.weight
@@ -172,11 +165,8 @@ def test_trainer_step_no_sync_and_tester(yaml, tmp_path):
     batch = _batch(7402)
     torch.cuda.synchronize()
     w0 = tr.model.fc.weight.detach().clone()
-    torch.cuda.set_sync_debug_mode('error')
-    try:
+    with no_host_sync():
         tr.batch_training(batch)
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     assert not torch.equal(tr.model.fc.weight, w0)
     assert np.isfinite(tr.average_meters['loss'].avg) and 0 <= tr.average_meters['acc'].avg <= 100
 
@@ -208,49 +198,19 @@ def test_graph_replay_equals_eager(lam):
     crit = ops.CrossEntropyLS(0.1) if lam is None else PairwiseConfusionLoss(CfgNode(dict(lambda_a=lam)))
     b = _batch(7600)
     x, labels = b['img'], b['label']
-    params = list(net.parameters())
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            for p in params:
-                p.grad = None
-            crit(net(x), labels).backward()
-        for p in params:
-            p.grad.zero_()
+
+    def step():
+        net.zero_grad()
         out = net(x)
         loss = crit(out, labels)
         loss.backward()
-        eager = [out.detach().clone(), loss.detach().clone(), crit.last_correct.clone()]
-        eager_g = [p.grad.clone() for p in params]
-        g = torch.cuda.CUDAGraph()
-        for p in params:
-            p.grad.zero_()
-        with torch.cuda.graph(g, stream=s):
-            gout = net(x)
-            gloss = crit(gout, labels)
-            gcorrect = crit.last_correct
-            gloss.backward()
-        for p in params:
-            p.grad.zero_()
-        g.replay()
-    torch.cuda.current_stream().wait_stream(s)
-    torch.cuda.synchronize()
-    assert torch.equal(gout, eager[0]) and torch.equal(gloss, eager[1]) and torch.equal(gcorrect, eager[2])
-    assert gcorrect.item() == int((eager[0].argmax(1) == labels).sum())          # a host top-1
-    assert torch.equal(net.fc.bias.grad, eager_g[-1])
-    for p, e in zip(params, eager_g):                     # the 3x3 weight gradients add their tiles with atomics
-        assert rel_l2(p.grad, e) < 1e-5
+        return [out, loss, crit.last_correct, net.fc.bias.grad]
+    # the 3x3 weight gradients add their tiles with atomics; the logit gradient's consumers are bit-exact
+    eager, replayed = replay_against_eager(step, net, net.parameters(), grad_bound=1e-5)
+    assert replayed[2].item() == int((eager[0].argmax(1) == labels).sum())       # a host top-1
 
 
 @pytest.mark.parametrize('yaml', ['PC_resnet50.yaml', 'Baseline.yaml'])
-def test_trainer_captures_and_replays(yaml, tmp_path):
-    os.environ['HK_CUDA_GRAPH'] = '1'
-    try:
-        tr = _trainer(yaml, str(tmp_path))
-        for i in range(5):
-            tr.batch_training(_batch(7700 + 2 * i))
-    finally:
-        del os.environ['HK_CUDA_GRAPH']
-    assert tr._graph is not None and tr._graph['kernels'] > 0
-    assert np.isfinite(tr.average_meters['loss'].avg) and 0 <= tr.average_meters['acc'].avg <= 100
+def test_trainer_captures_and_replays(yaml, tmp_path, monkeypatch):
+    tr = _trainer(monkeypatch, yaml, str(tmp_path), graph=True)
+    assert_trainer_replays(tr, [_batch(7700 + 2 * i) for i in range(5)])

@@ -14,6 +14,7 @@ from conftest import load_golden, rel_l2
 from oracle import prototree_oracle as O
 from prototree_inputs import theta0, tree_inputs
 from kernel_check import precise  # noqa: F401  (a fixture)
+from step_check import eager_and_graph_losses, make_trainer, no_host_sync
 
 pytestmark = pytest.mark.gpu
 G = load_golden('reference_prototree')
@@ -329,18 +330,12 @@ def test_full_model_matches_reference(monkeypatch):
     assert all(torch.isfinite(p.grad).all() for p in net.parameters() if p.grad is not None)
 
 
-def _trainer(monkeypatch, graph=False, **model):
-    from hawkeye_b200 import examples
-    from hawkeye_b200.config import load_config
-    monkeypatch.setenv('HAWKEYE_ALLOW_RANDOM_INIT', '1')
-    monkeypatch.setenv('HK_CUDA_GRAPH', '1' if graph else '0')
-    cfg = load_config(os.path.join(REPO, 'configs', 'ProtoTreeNet.yaml'))
-    cfg.model.backbone['pretrain'] = ''                      # no iNat checkpoint here: the trunk keeps its random init
-    for k, v in model.items():
-        cfg.model[k] = v
-    tr = examples.ProtoTreeTrainer(cfg, dataloaders={})
+def _trainer(monkeypatch, graph=False):
+    from hawkeye_b200.cfgnode import CfgNode
+    # no iNat checkpoint here: the trunk keeps its random init
+    tr = make_trainer(monkeypatch, 'ProtoTreeNet', 'ProtoTreeNet.yaml', graph=graph,
+                      backbone=CfgNode(dict(name='resnet50', pretrain='')))
     tr.num_batches = 10
-    tr.model.train()
     return tr
 
 
@@ -357,12 +352,9 @@ def test_train_step_224_no_sync(monkeypatch):
     assert not tr.model.training                             # eval() after the first leaf update, as the reference
     assert not torch.equal(tr.model.tree.leaf_params, theta0)
     torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode('error')                  # no host synchronisation inside the step
-    try:
+    with no_host_sync():
         for _ in range(4):
             losses.append(tr.batch_training(data))
-    finally:
-        torch.cuda.set_sync_debug_mode(0)
     losses[1:] = [float(v.item()) for v in losses[1:]]
     print('prototree 224 losses', losses)
     assert all(torch.isfinite(torch.tensor(losses)))          # a random-init trunk: the loss need not fall in 5 steps
@@ -375,26 +367,15 @@ def test_graph_replay_matches_eager_on_eval_steps(monkeypatch):
     """224x224, batch 64.  First batch eager in train mode, then eval-mode steps; with the graph they replay.  The trunk, neck and prototypes
     are held at lr 0 (they still run forward and backward): the leaves, updated by the deterministic leaf-update kernel, and
     the losses must then be the same bits with and without the graph."""
-    data = _batch(64, 850)
-    out, state0 = {}, None
-    for graph in (False, True):
-        torch.manual_seed(0)
-        tr = _trainer(monkeypatch, graph=graph)
-        if state0 is None:
-            state0 = copy.deepcopy(tr.model.state_dict())
-        else:
-            tr.model.load_state_dict(state0)
-        for g in tr.optimizer.param_groups:
-            g['lr'] = 0.0
-        tr.on_start_epoch(None)
-        losses = [float(tr.batch_training(data).item()) for _ in range(7)]    # a replay overwrites the graph's loss tensor
-        out[graph] = (losses, tr.model.tree.leaf_params.detach().clone())
-        if graph:
-            assert tr._graph is not None
-        del tr
-    print('prototree graph', out[False][0], out[True][0])
-    assert out[False][0] == out[True][0]
-    assert torch.equal(out[False][1], out[True][1])
+    (eager, eager_state), (replayed, replayed_state) = eager_and_graph_losses(
+        lambda graph: _trainer(monkeypatch, graph=graph), [_batch(64, 850)] * 7,
+        frozen_groups=range(4))                                  # all four: trunk, layer4[2], neck and prototypes
+    print('prototree graph', eager, replayed)
+    assert eager == replayed
+    leaves = [k for k in eager_state if k.endswith('._dist_params')]        # tree.leaf_params, one entry per leaf
+    assert len(leaves) == 512
+    for k in leaves:
+        assert torch.equal(eager_state[k], replayed_state[k]), k
 
 
 def test_errors():

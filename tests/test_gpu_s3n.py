@@ -4,6 +4,7 @@ reference's own class response maps against its fixtures for p = 0, 1, 2, the sa
 gradient against torchvision's ResNet-50 in fp64, the full model against the reference's fixtures (radius, radius_inv and
 filter from the model's own image gradient), the reference checkpoint in eval mode, CUDA-graph replay across p = 0, 1, 2,
 and one S3NTrainer epoch with no host synchronisation in the step.  Precise mode unless stated."""
+import contextlib
 import json
 
 import numpy as np
@@ -15,6 +16,7 @@ import detgen
 from conftest import load_golden, rel_l2
 from oracle import s3n_oracle as O
 from kernel_check import precise_on  # noqa: F401  (a fixture)
+from step_check import capture, make_trainer, no_host_sync, side_stream
 
 pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures('precise_on')]
 GG = 31 * 31
@@ -352,15 +354,11 @@ def test_graph_replay_matches_eager_across_p(monkeypatch):
         loss.backward()
         return out, loss, [q.grad for q in watched]
 
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
+    with side_stream() as s:
         for _ in range(2):
             step()
         state = {k: v.clone() for k, v in net.state_dict().items()}
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph, stream=s):
-            g_out, g_loss, g_grads = step()
+        graph, (g_out, g_loss, g_grads) = capture(step)
         for p in (0, 1, 2):
             net.load_state_dict(state)
             pt.fill_(p)
@@ -375,41 +373,28 @@ def test_graph_replay_matches_eager_across_p(monkeypatch):
             assert torch.equal(e_loss, g_loss)
             for a, b in zip(e_grads, g_grads):
                 assert torch.equal(a, b)
-    torch.cuda.current_stream().wait_stream(s)
 
 
-def test_trainer_epoch_no_sync(tmp_path):
+def test_trainer_epoch_no_sync(tmp_path, monkeypatch):
     """One S3NTrainer epoch of six synthetic 448x448 batches with ``cuda_graph: true``: two eager steps, the capture, then
     replays, with the epoch moved to 20 before the last step so that p changes from 0 to 1 under replay.  The steps other
     than the capture run with no host synchronisation; every parameter the optimizer owns gets a gradient, the classifiers
     move, and validation (p = 2 from epoch 20) scores aggregation."""
-    import os
-    from hawkeye_b200 import examples
-    from hawkeye_b200.config import load_config
-    cfg = load_config(os.path.join(os.path.dirname(os.path.abspath(__file__)), '..', 'configs', 'S3N.yaml'))
-    cfg.experiment['log_dir'] = str(tmp_path)
-    cfg.experiment['cuda_graph'] = True
     batches = [dict(img=detgen.det((4, 3, 448, 448), 7700 + i).pin_memory(),
                     label=detgen.det_labels(4, 200, 7710 + i).pin_memory()) for i in range(6)]
     val = [dict(img=detgen.det((4, 3, 448, 448), 7720), label=torch.zeros(4, dtype=torch.int64))]
     from hawkeye_b200 import _lib
     _lib.set_precise(0)
-    tr = examples.S3NTrainer(cfg, dataloaders={'train': batches, 'val': val})
+    tr = make_trainer(monkeypatch, 'S3N', 'S3N.yaml', graph=True, experiment=dict(log_dir=str(tmp_path)),
+                      dataloaders={'train': batches, 'val': val})
     assert [g['lr'] for g in tr.optimizer.param_groups] == pytest.approx([0.005, 5e-8, 5e-8, 5e-4])
     w0 = tr.model.con_classifier.weight.detach().clone()
     tr.epoch = 0
     for i, data in enumerate(batches):
         if i == 5:
             tr.epoch = 20
-        if i == 2:                                   # the third step captures the graph after its eager run
+        with no_host_sync() if i not in (0, 2) else contextlib.nullcontext():   # step 3 captures after its eager run
             tr.batch_training(data)
-            continue
-        if i > 0:
-            torch.cuda.set_sync_debug_mode('error')
-        try:
-            tr.batch_training(data)
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
         if i == 1:                                   # p = 0: every peak feeds both maps, so every gradient is non-zero
             for g in tr.flat.groups:
                 for q in g:

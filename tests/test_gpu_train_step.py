@@ -33,8 +33,8 @@ import detgen
 import matched
 from kernel_check import c_bound, check
 from matched import TOL, rel_l2, tape_items
+from step_check import make_trainer
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BATCH, SIZE, CLASSES = 32, 448, 200
 CHUNK = 4                   # images per fp64 oracle evaluation (VGG-16 at 448x448 in fp64: ~2 GB of activations each)
 U = 2.0 ** -24              # fp32 unit roundoff
@@ -283,16 +283,11 @@ def logit_errs(dev, ref):
 
 
 def _trainer(cfg_name, trainer, monkeypatch, graph):
-    from hawkeye_b200 import _lib, examples
-    from hawkeye_b200.config import load_config
-    monkeypatch.setenv('HAWKEYE_ALLOW_RANDOM_INIT', '1')
-    monkeypatch.setenv('HK_CUDA_GRAPH', '1' if graph else '0')
+    from hawkeye_b200 import _lib
     _lib.set_precise(0)
-    cfg = load_config(os.path.join(REPO, 'configs', cfg_name))
     torch.manual_seed(0)
-    tr = examples.TRAINERS[trainer](cfg, dataloaders={})
-    tr.model.train()
-    return tr, cfg
+    tr = make_trainer(monkeypatch, trainer, cfg_name, graph=graph)
+    return tr, tr.config
 
 
 def _batches(n, dev):
