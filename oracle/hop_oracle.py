@@ -447,15 +447,25 @@ def _bottleneck(x, st, pre, stride, has_ds, nl=Plain, bn=_bn_train):
     return nl.relu(out + identity)
 
 
+def resnet_stem(x, st, prefix='backbone.', nl=Plain, bn=_bn_train):
+    """conv1 (7x7/s2), bn1, relu, maxpool (3x3/s2) of ResNet._forward_impl (resnet.py:235-238)."""
+    x = F.conv2d(x, st[prefix + '0.weight'], stride=2, padding=3)
+    return nl.maxpool(nl.relu(bn(x, st, prefix + '1')), 3, 2, 1)
+
+
+def resnet_block_plan(layers, prefix='backbone.'):
+    """[(state prefix, stride, has downsample)] of every Bottleneck of layer1..4 in forward order (_make_layer,
+    resnet.py:208-231): the first block of a layer strides and carries the downsample."""
+    return [(f'{prefix}{4 + li}.{b}', stride if b == 0 else 1, b == 0)
+            for li, (_, blocks, stride) in enumerate(layers) for b in range(blocks)]
+
+
 def resnet50_trunk_fwd(x, st, prefix='backbone.', nl=Plain, layers=RESNET50_LAYERS, bn=_bn_train):
     """children()[:-2] of ResNet-50 (MPNCOV.py:28-29): conv1, bn1, relu, maxpool, layer1..4 -> [B,2048,H/32,W/32].
     ``layers`` gives other depths (``resnet_layers((3, 4, 23, 3))`` is ResNet-101); ``bn=_bn_eval`` is the eval-mode trunk."""
-    x = F.conv2d(x, st[prefix + '0.weight'], stride=2, padding=3)
-    x = nl.relu(bn(x, st, prefix + '1'))
-    x = nl.maxpool(x, 3, 2, 1)
-    for li, (planes, blocks, stride) in enumerate(layers):
-        for b in range(blocks):
-            x = _bottleneck(x, st, f'{prefix}{4 + li}.{b}', stride if b == 0 else 1, b == 0, nl=nl, bn=bn)
+    x = resnet_stem(x, st, prefix, nl, bn)
+    for pre, stride, has_ds in resnet_block_plan(layers, prefix):
+        x = _bottleneck(x, st, pre, stride, has_ds, nl=nl, bn=bn)
     return x
 
 
@@ -475,7 +485,7 @@ def npairs_loss(feats, labels):
     n = b * p
     x = F.normalize(feats.reshape(n, -1), p=2, dim=1)                                  # :41-43
     t = torch.repeat_interleave(labels, p)                                             # :44
-    parts = torch.arange(p).repeat(b)                                                  # :45
+    parts = torch.arange(p, device=labels.device).repeat(b)                            # :45
     prod = x @ x.t()                                                                   # :46
     sc = t.expand(n, n).eq(t.expand(n, n).t())                                         # :50
     sa = parts.expand(n, n).eq(parts.expand(n, n).t())                                 # :51
@@ -494,3 +504,38 @@ def npairs_loss(feats, labels):
 def mamc_loss(pred, x_part, labels, lambda_a=0.5):
     """MAMCLoss.forward (MAMC_loss.py:15-21): CE(label_smoothing=0.1) + lambda_a * N-pairs."""
     return F.cross_entropy(pred, labels, label_smoothing=0.1) + lambda_a * npairs_loss(x_part, labels)
+
+
+# --------------------------------------------------------------------------------------
+# OSMENet: ResNet-101 trunk + OSME (model/methods/OSME.py:8-64)
+# --------------------------------------------------------------------------------------
+RESNET101_LAYERS = resnet_layers((3, 4, 23, 3))
+
+
+def osme_forward(x, st, prefix='osme.', nl=Plain, linear=F.linear):
+    """OSME.forward (OSME.py:36-44) on the trunk map x [N, C, H, W] -> (sum of the attention features [N, D], the features
+    stacked [N, P, D]).  Each OSME_block.forward (:19-24): z = the spatial mean (:21), m = sigmoid(Linear(ReLU(Linear(z))))
+    (:22, the Sequential of :12-17), s = m * x per channel (:23); then every attention's Linear over s flattened in NCHW
+    order (:43).  The bottleneck ReLU goes through ``nl`` so that a MaskTape replays it; ``linear`` computes the
+    attention Linears (a caller may evaluate them in row blocks)."""
+    N, C = x.shape[:2]
+    P = sum(1 for k in st if k.startswith(prefix + 'blocks.') and k.endswith('.block.0.weight'))
+    s = []
+    for i in range(P):                                                                 # :42
+        pre = f'{prefix}blocks.{i}.block.'
+        z = x.mean(dim=(2, 3))                                                         # :21
+        h = nl.relu(F.linear(z, st[pre + '0.weight'], st[pre + '0.bias']))             # :22 (:13-14)
+        m = torch.sigmoid(F.linear(h, st[pre + '2.weight'], st[pre + '2.bias']))       # :22 (:15-16)
+        s.append(m.view(N, C, 1, 1) * x)                                               # :23
+    feats = [linear(s[i].reshape(N, -1), st[f'{prefix}fcs.{i}.weight'], st[f'{prefix}fcs.{i}.bias'])
+             for i in range(P)]                                                        # :43
+    return sum(feats), torch.stack(feats, dim=1)                                       # :44
+
+
+def osmenet_forward(x, st, nl=Plain, layers=RESNET101_LAYERS, linear=F.linear, bn=_bn_train):
+    """OSMENet.forward (OSME.py:60-64): the ResNet trunk (children()[:-2], :55-56), OSME, the classifier on the sum of the
+    attention features -> (logits, x_part).  Device- and dtype-agnostic: it runs wherever, and in whatever precision,
+    x and st are."""
+    f = resnet50_trunk_fwd(x, st, nl=nl, layers=layers, bn=bn)                         # :61
+    x1, x_part = osme_forward(f, st, 'osme.', nl, linear)                              # :62
+    return F.linear(x1, st['classifier.weight'], st['classifier.bias']), x_part       # :63-64
