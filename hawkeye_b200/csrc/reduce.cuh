@@ -53,23 +53,31 @@ __device__ __forceinline__ float block_max(float v, float* red) {
   return t;
 }
 
+// The softmax statistics of one row segment z[0, K), by one warp: lse = log sum_k exp z[k] and sl = sum_k z[k], in every
+// lane.  The one softmax of the cross-entropies below.
+__device__ __forceinline__ void warp_lse(const float* __restrict__ z, int K, float& lse, float& sl) {
+  const int lane = threadIdx.x & 31;
+  float m = -INFINITY;
+  for (int k = lane; k < K; k += 32) m = fmaxf(m, z[k]);
+  m = warp_max(m);
+  float se = 0.f, s = 0.f;
+  for (int k = lane; k < K; k += 32) {
+    se += expf(z[k] - m);
+    s += z[k];
+  }
+  se = warp_sum(se);
+  sl = warp_sum(s);
+  lse = m + logf(se);
+}
+
 // Label-smoothed cross-entropy of one row segment z[0, K) with target y (eps = smoothing), by one warp: returns the row's
 // loss term and, unless g is null, writes (softmax - target distribution) * scale to g (rounded to tf32 when `round`).  A
 // target outside [0, K) gets no one-hot term and z is not read at it.
 __device__ __forceinline__ float warp_ce_ls(const float* __restrict__ z, int K, long long y, float eps, float scale,
                                             float* __restrict__ g, int round) {
   const int lane = threadIdx.x & 31;
-  float m = -INFINITY;
-  for (int k = lane; k < K; k += 32) m = fmaxf(m, z[k]);
-  m = warp_max(m);
-  float se = 0.f, sl = 0.f;
-  for (int k = lane; k < K; k += 32) {
-    se += expf(z[k] - m);
-    sl += z[k];
-  }
-  se = warp_sum(se);
-  sl = warp_sum(sl);
-  const float lse = m + logf(se);
+  float lse, sl;
+  warp_lse(z, K, lse, sl);
   const bool valid = y >= 0 && y < K;
   const float zy = valid ? z[y] : lse;
   if (g) {
@@ -82,6 +90,25 @@ __device__ __forceinline__ float warp_ce_ls(const float* __restrict__ z, int K, 
   // (1 - eps) (lse - z[y]) + eps (lse - mean(z)), with the fused multiply-add spelled out: left to the compiler, which
   // product it fuses depends on the kernel this is inlined into
   return fmaf(1.f - eps, lse - zy, eps * (lse - sl / (float)K));
+}
+
+// warp_ce_ls against the soft target wa onehot(ya) + wb onehot(yb) (Mixup / CutMix; ya == yb sums the two weights): the
+// loss term (1 - eps) [wa (lse - z[ya]) + wb (lse - z[yb])] + eps (lse - mean(z)), and unless g is null
+// (softmax - ((1 - eps) target + eps / K)) * scale written to g.  A label outside [0, K) gets no one-hot term.
+__device__ __forceinline__ float warp_ce_ls_mix(const float* __restrict__ z, int K, long long ya, float wa, long long yb,
+                                                float wb, float eps, float scale, float* __restrict__ g, int round) {
+  const int lane = threadIdx.x & 31;
+  float lse, sl;
+  warp_lse(z, K, lse, sl);
+  const float za = (ya >= 0 && ya < K) ? z[ya] : lse, zb = (yb >= 0 && yb < K) ? z[yb] : lse;
+  if (g) {
+    for (int k = lane; k < K; k += 32) {
+      const float t = ((k == ya ? wa : 0.f) + (k == yb ? wb : 0.f)) * (1.f - eps) + eps / (float)K;
+      const float v = (expf(z[k] - lse) - t) * scale;
+      g[k] = round ? tf32_round(v) : v;
+    }
+  }
+  return fmaf(1.f - eps, fmaf(wa, lse - za, wb * (lse - zb)), eps * (lse - sl / (float)K));
 }
 
 }  // namespace hk

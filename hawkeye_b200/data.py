@@ -204,6 +204,62 @@ def collate_packed(batch, size, mean, std):
     return out
 
 
+class MixupCutmixCollateFn:
+    """dataset/collate_fn.py: one of RandomMixup(p=1.0, alpha=0.2) and RandomCutmix(p=1.0, alpha=1.0) per batch
+    (dataset/transforms.py:76-231), picked with torchvision's RandomChoice.  The draws are the reference's own calls in
+    its order, on the worker's RNGs: ``random.choices``, ``torch.rand(1)`` (drawn although p = 1 never skips),
+    ``torch._sample_dirichlet`` and, for CutMix, ``torch.randint(W)`` then ``torch.randint(H)``.
+
+    The images are not mixed here.  The batch of ``collate`` (``default_collate``, or a device preset's ``collate`` for
+    ``PackedImages``) gains ``'mix'``: the float64 row of ``hawkeye_b200.ops_mixup`` with the kind, lambda, the CutMix box
+    and the target weight, which ``Trainer.stage_inputs`` applies on the device.  ``'label'`` stays int64 [B]: the target
+    of row i is w onehot(label i) + (1 - w) onehot(label i - 1 mod B), the reference's rolled dense target."""
+
+    def __init__(self, num_classes, collate=None):
+        if num_classes <= 0:
+            raise ValueError('MixupCutmixCollateFn: num_classes must be positive')
+        self.num_classes, self.collate = int(num_classes), collate
+        self.alphas = (0.2, 1.0)           # RandomMixup, RandomCutmix
+
+    def draw(self, height, width):
+        """-> the mix row of one batch of H x W images, drawn as the reference's collate draws it."""
+        import math
+        import random
+        from .ops_mixup import CUTMIX, MIXUP, check_row, mix_row
+        kind = random.choices((MIXUP, CUTMIX))[0]                     # transforms.RandomChoice.__call__
+        torch.rand(1)                                                 # the p = 1.0 test: never skips, still a draw
+        alpha = self.alphas[kind]
+        lam = float(torch._sample_dirichlet(torch.tensor([alpha, alpha]))[0])
+        if kind == MIXUP:
+            row = mix_row(MIXUP, lam)
+        else:                                                         # transforms.py:211-226
+            r_x, r_y = int(torch.randint(width, (1,))), int(torch.randint(height, (1,)))
+            r = 0.5 * math.sqrt(1.0 - lam)
+            r_w_half, r_h_half = int(r * width), int(r * height)
+            x1, y1 = max(r_x - r_w_half, 0), max(r_y - r_h_half, 0)
+            x2, y2 = min(r_x + r_w_half, width), min(r_y + r_h_half, height)
+            row = mix_row(CUTMIX, lam, (x1, y1, x2, y2), float(1.0 - (x2 - x1) * (y2 - y1) / (width * height)))
+        check_row(row, height, width)
+        return row
+
+    def __call__(self, batch):
+        from torch.utils.data import default_collate
+        from .ops_augment import PackedImages
+        data = (self.collate or default_collate)(batch)
+        img, label = data['img'], data['label']
+        if label.ndim != 1 or label.dtype != torch.int64:
+            raise TypeError(f'MixupCutmixCollateFn: labels must be int64 [B], not {label.dtype} {tuple(label.shape)}')
+        if isinstance(img, PackedImages):
+            height = width = img.size
+        else:
+            if img.ndim != 4 or not img.is_floating_point():
+                raise TypeError(f'MixupCutmixCollateFn: images must be a float [B, C, H, W] batch, not {img.dtype} '
+                                f'{tuple(img.shape)}')
+            height, width = img.shape[-2:]
+        data['mix'] = self.draw(int(height), int(width))
+        return data
+
+
 def _grid_cells(image, cols, rows):
     """The ``cols x rows`` grid of crops of a PIL image, row by row; cell edges at int(size / count * i)."""
     width, height = image.size

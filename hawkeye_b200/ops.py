@@ -426,6 +426,46 @@ class CrossEntropyLS(torch.nn.Module):
         return loss
 
 
+class CrossEntropyLSMixFn(Function):
+    @staticmethod
+    def forward(ctx, logits, labels, mix, smoothing):
+        _check_cuda(logits, labels, mix)
+        logits = _f32c(logits)
+        labels = labels.contiguous().to(torch.int64)
+        if mix.dtype != torch.float64 or not mix.is_contiguous():
+            raise _lib.HawkeyeLibError('CrossEntropyLSMix: mix must be a contiguous float64 row (hawkeye_b200.ops_mixup)')
+        B, K = logits.shape
+        loss = torch.empty(1, device=logits.device, dtype=torch.float32)
+        dlogits = torch.empty_like(logits)
+        correct = torch.empty(1, device=logits.device, dtype=torch.int32)
+        _lib.call('hk_softmax_ce_ls_mix', logits, labels, mix, loss, dlogits, correct, B, K, float(smoothing), 1.0,
+                  _lib.stream_ptr())
+        ctx.save_for_backward(dlogits)
+        ctx.mark_non_differentiable(correct)
+        return loss[0], correct
+
+    @staticmethod
+    def backward(ctx, g, _g_correct=None):
+        (dlogits,) = ctx.saved_tensors
+        return dlogits * g, None, None, None
+
+
+class CrossEntropyLSMix(torch.nn.Module):
+    """``CrossEntropyLS`` on the soft target of a Mixup / CutMix batch (``hawkeye_b200.data.MixupCutmixCollateFn``): row
+    i's target is w onehot(labels[i]) + (1 - w) onehot(labels[i - 1 mod B]), w = mix[ops_mixup.WEIGHT], which is
+    ``torch.nn.CrossEntropyLoss(label_smoothing=...)`` on the reference's dense [B, K] target.  ``last_correct`` counts the
+    rows whose top-1 is the target's argmax (the larger weight's label, the lower class on a tie)."""
+
+    def __init__(self, label_smoothing=0.1):
+        super().__init__()
+        self.label_smoothing = label_smoothing
+
+    def forward(self, logits, labels, mix):
+        loss, correct = CrossEntropyLSMixFn.apply(logits, labels, mix, self.label_smoothing)
+        self.last_correct = correct
+        return loss
+
+
 # ----------------------------------------------------------------------------------------------------------
 # VGG-style backbone (reference model/backbone/vgg.py:56-70), whole feature stack as ONE autograd node
 # ----------------------------------------------------------------------------------------------------------

@@ -17,6 +17,7 @@ import torch
 from . import engine, ops
 from .config import setup_config
 from .ops_augment import PackedImages, augment
+from .ops_mixup import mix_batch
 from .registry import MODEL
 from .utils import load_state_dict
 
@@ -95,6 +96,18 @@ def device_collate(config, transforms, who):
     return {s: t.collate for s, t in transforms.items()}
 
 
+def mixup_cutmix(config, trainer_cls):
+    """True when the ``dataset`` config sets ``mixup_cutmix: true``: the training batches are mixed by the reference's
+    ``MixupCutmixCollateFn(model.num_classes)`` and the criterion is ``ops.CrossEntropyLSMix``.  Only trainers whose
+    criterion is the base Trainer's cross-entropy on one logits tensor learn from the soft target; any other trainer
+    (one that overrides ``get_criterion``) is an error, not a quiet fall-back to hard labels."""
+    on = bool(config['mixup_cutmix']) if 'mixup_cutmix' in config else False
+    if on and trainer_cls.get_criterion is not Trainer.get_criterion:
+        raise ValueError(f'dataset.mixup_cutmix covers the trainers whose criterion is the base cross-entropy on one '
+                         f'logits tensor; {trainer_cls.__name__} has its own loss')
+    return on
+
+
 def warmup_cosine_args(config, total_epoch):
     """-> (T_max, warmup_epochs, lr_warmup_decay) of a scheduler config, each with its default."""
     return (config['T_max'] if 'T_max' in config else total_epoch,
@@ -105,6 +118,7 @@ def warmup_cosine_args(config, total_epoch):
 class Trainer:
     def __init__(self, config=None, dataloaders=None):
         self.config = config if config is not None else setup_config()
+        self.mixing = mixup_cutmix(self.config.dataset, type(self))
         self.epoch = 0
         self.start_epoch = 0
         self.total_epoch = self.config.train.epoch
@@ -168,9 +182,13 @@ class Trainer:
         except Exception:
             from .data import FGDataset
         tf = self.get_transformers(config.transformer)
+        collate = device_collate(config.transformer, tf, type(self).__name__)
+        if mixup_cutmix(config, type(self)):           # the training batches only: validation is never mixed
+            from .data import MixupCutmixCollateFn
+            collate = dict(collate or {}, train=MixupCutmixCollateFn(self.config.model.num_classes,
+                                                                     (collate or {}).get('train')))
         return self.rank_loaders(config, {s: FGDataset(config.root_dir, os.path.join(config.meta_dir, s + '.txt'),
-                                                       transform=tf[s]) for s in ('train', 'val')},
-                                 collate_fn=device_collate(config.transformer, tf, type(self).__name__))
+                                                       transform=tf[s]) for s in ('train', 'val')}, collate_fn=collate)
 
     def rank_loaders(self, config, datasets, collate_fn=None):
         """{'train', 'val'} loaders of this rank over ``datasets``; ``collate_fn`` maps a split to its collate function.
@@ -196,6 +214,8 @@ class Trainer:
         return loaders
 
     def get_criterion(self, config):
+        if mixup_cutmix(self.config.dataset, type(self)):          # the soft target of dataset/collate_fn.py's batches
+            return ops.CrossEntropyLSMix(label_smoothing=0.1)
         return ops.CrossEntropyLS(label_smoothing=0.1)              # train.py:211-212
 
     def param_groups(self):
@@ -247,7 +267,10 @@ class Trainer:
     def batch_tensors(self, data):
         """-> (images, labels): the tensors of one loader batch the step uses.  ``labels`` is one tensor for the dict
         batches of FGDataset; a method whose criterion takes several targets returns their tuple, which reaches the
-        criterion as ``criterion(outputs, *labels)``."""
+        criterion as ``criterion(outputs, *labels)``.  A batch mixed by ``MixupCutmixCollateFn`` gives (labels, mix), which
+        ``ops.CrossEntropyLSMix`` takes."""
+        if 'mix' in data:
+            return data['img'], (data['label'], data['mix'])
         return data['img'], data['label']
 
     def stage_inputs(self, data):
@@ -255,13 +278,14 @@ class Trainer:
         preallocated device buffers per batch shape — no allocator traffic in the step.  The compute stream waits for the
         copy in-stream, and the copy stream waits (device-side) until the step that last used the slot has finished, so the
         copy of step n+1 overlaps the kernels of step n whenever the host runs ahead.  Returns (images, labels, slot);
-        labels is a tuple when ``batch_tensors`` gives one, each target with its own buffer in the slot."""
+        labels is a tuple when ``batch_tensors`` gives one, each target with its own buffer in the slot.  A mixed batch
+        (``dataset.mixup_cutmix``) is mixed on the compute stream after the copy (``mix_staged``)."""
         img, lab = self.batch_tensors(data)
         labs = lab if isinstance(lab, tuple) else (lab,)
         if isinstance(img, PackedImages):
             return self.stage_packed(img, lab, labs)
         if img.is_cuda and all(t.is_cuda for t in labs):
-            return img, lab, None
+            return self.mix_staged(img, lab, None), lab, None
         key = (tuple(img.shape), img.dtype) + tuple((tuple(t.shape), t.dtype) for t in labs)
         ring = self._in_ring.get(key)
         if ring is None:
@@ -281,7 +305,8 @@ class Trainer:
             ev = torch.cuda.Event()
             ev.record()
         cur.wait_event(ev)
-        return slot['img'], (tuple(slot['lab']) if isinstance(lab, tuple) else slot['lab'][0]), slot
+        lab = tuple(slot['lab']) if isinstance(lab, tuple) else slot['lab'][0]
+        return self.mix_staged(slot['img'], lab, slot), lab, slot
 
     def stage_packed(self, packed, lab, labs):
         """``stage_inputs`` of a packed batch of the device presets: the packed images and their tables are copied on the
@@ -322,7 +347,20 @@ class Trainer:
         cur.wait_event(ev)
         augment(slot['src'], slot['offsets'], slot['sizes'], slot['params'], S, packed.mean, packed.std, out=slot['img'],
                 work=slot['work'], lut=slot['lut'])
-        return slot['img'], (tuple(slot['lab']) if isinstance(lab, tuple) else slot['lab'][0]), slot
+        lab = tuple(slot['lab']) if isinstance(lab, tuple) else slot['lab'][0]
+        return self.mix_staged(slot['img'], lab, slot), lab, slot
+
+    def mix_staged(self, images, labels, slot):
+        """The staged images of a batch ``MixupCutmixCollateFn`` mixed (labels = (labels, mix row)): ``hk_mix_batch`` on
+        the compute stream, after the copy (and the augment kernels), into the slot's own buffer — out of place, with no
+        allocation once the slot has one and no host read of the draws.  Any other batch is returned as it is."""
+        if not (self.mixing and isinstance(labels, tuple)):
+            return images
+        if slot is None:
+            return mix_batch(images, labels[1])
+        if slot.get('mixed') is None:
+            slot['mixed'] = torch.empty_like(images)
+        return mix_batch(images, labels[1], out=slot['mixed'])
 
     # ---- CUDA-graph replay of forward + loss + backward (+ gradient all-reduce) ----------------------------------------
     # A ResNet-50 step is ~1500 short launches issued from Python: the host, not the GPU, sets the step time.  With

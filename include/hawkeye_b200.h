@@ -672,6 +672,28 @@ int hk_augment_stats(const unsigned char* img, const double* params, unsigned ch
 int hk_augment_apply(const unsigned char* img, const double* params, const unsigned char* lut, float* y, int N, int S,
                      float mean0, float mean1, float mean2, float std0, float std1, float std2, void* stream);
 
+/* ---- Mixup / CutMix: dataset/transforms.py RandomMixup, RandomCutmix; dataset/collate_fn.py MixupCutmixCollateFn -------
+ * One batch's draws are a row of hk_mix_cols() doubles in device memory: kind (0 Mixup, 1 CutMix), lambda, the CutMix
+ * box x1, y1, x2, y2 (columns [x1, x2), rows [y1, y2)) and the target weight w (hawkeye_b200/ops_mixup.py).  Image n is
+ * paired with image n - 1 mod N, the reference's roll(1, 0).
+ * hk_mix_check: validates a row in HOST memory for H x W images before it is staged: HK_ERR_ARG on a null pointer, H or
+ *   W <= 0, an unknown kind, lambda or w outside [0, 1], or a box that is not integral or lies outside the image.
+ * hk_mix_batch: x [N,C,H,W] fp32 -> y, out of place (y must not alias x).  Replaces transforms.py:129-135 (Mixup):
+ *   y_n = fl(fl(x_n (float)lambda) + fl(x_{n-1} (float)(1 - lambda))), bit-identical to the reference; and
+ *   transforms.py:206,225 (CutMix): y_n = x_n with the box copied from x_{n-1}.  Reads x once (image N-1 twice) and
+ *   writes y once.  HK_ERR_ARG on a null pointer, a size <= 0 or y == x.
+ * hk_softmax_ce_ls_mix: replaces transforms.py:123,130,137-138 / :228-229 (the rolled dense target) and train.py:211-212
+ *   (nn.CrossEntropyLoss(label_smoothing) on it): the target of row b is w onehot(y_b) + (1 - w) onehot(y_{b-1 mod B}),
+ *   loss[0] = mean over rows, dlogits (optional) = (softmax - ((1 - eps) target + eps / K)) * grad_scale / B (rounded to
+ *   tf32 in the default mode, as hk_softmax_ce_ls), correct (optional) = rows whose first argmax is the target's argmax
+ *   (the larger weight's label; the lower class index on a tie, as target.max(1)[1]).  One launch, fixed-order sums.
+ *   HK_ERR_ARG on a null pointer, B <= 0 or K <= 0. */
+int hk_mix_cols(void);
+int hk_mix_check(const double* mix, int H, int W);
+int hk_mix_batch(const float* x, const double* mix, float* y, int N, int C, int H, int W, void* stream);
+int hk_softmax_ce_ls_mix(const float* logits, const long long* labels, const double* mix, float* loss, float* dlogits,
+                         int* correct, int B, int K, float label_smoothing, float grad_scale, void* stream);
+
 /* ---- optimizers over flat fp32 buffers: torch.optim.SGD (Examples/BCNN.py:40), Adam (Examples/MPN.py:14-18) */
 int hk_sgd_momentum(float* p, const float* g, float* buf, size_t n, float lr, float momentum, float weight_decay,
                     float grad_scale, int first_step, void* stream);
