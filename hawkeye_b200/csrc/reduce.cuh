@@ -53,6 +53,29 @@ __device__ __forceinline__ float block_max(float v, float* red) {
   return t;
 }
 
+// Block exclusive prefix sum in thread order: returns the sum of v over the threads below this one and sets total to
+// the sum over all threads.  Same conditions on blockDim.x and red[] as block_sum.
+template <typename T>
+__device__ __forceinline__ T block_exclusive_scan(T v, T* red, T& total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  T inc = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const T u = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += u;
+  }
+  __syncthreads();
+  if (lane == 31) red[warp] = inc;
+  __syncthreads();
+  T below = T(0);
+  total = T(0);
+  for (int i = 0; i < (int)(blockDim.x >> 5); ++i) {
+    if (i < warp) below += red[i];
+    total += red[i];
+  }
+  return below + inc - v;
+}
+
 // The softmax statistics of one row segment z[0, K), by one warp: lse = log sum_k exp z[k] and sl = sum_k z[k], in every
 // lane.  The one softmax of the cross-entropies below.
 __device__ __forceinline__ void warp_lse(const float* __restrict__ z, int K, float& lse, float& sl) {

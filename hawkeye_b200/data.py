@@ -6,7 +6,8 @@ Python plumbing, not a kernel path; the tensor part of the eval preset (``ToTens
 importable, so the package also trains outside a Hawkeye checkout.
 
 ``DevicePresetTrain`` / ``DevicePresetEval`` are the two default presets with everything after the decode on the GPU
-(``hawkeye_b200.ops_augment``), selected by ``dataset.transformer.device: cuda``.
+(``hawkeye_b200.ops_augment``), selected by ``dataset.transformer.device: cuda``.  With ``decode: cuda`` as well, the
+loader is ``encoded_loader`` and the JPEGs the device decodes travel encoded (``hawkeye_b200.ops_jpeg``).
 """
 import os
 
@@ -20,6 +21,28 @@ def default_loader(path):
     from PIL import Image
     img = Image.open(path)
     return img.convert('RGB')
+
+
+def encoded_loader(path):
+    """The loader of ``dataset.transformer.decode: cuda`` (``hawkeye_b200.ops_jpeg.encoded_loader``): an
+    ``EncodedJPEG`` for a JPEG the device decodes, the PIL image of ``default_loader`` for any other file."""
+    from .ops_jpeg import encoded_loader as load
+    return load(path)
+
+
+def _image_like(img):
+    """What torchvision's get_params reads the size of: the PIL image itself, or a [3, H, W] meta tensor standing in
+    for an encoded JPEG (no pixels are needed to draw)."""
+    from .ops_jpeg import EncodedJPEG
+    if isinstance(img, EncodedJPEG):
+        return torch.empty(3, img.size[1], img.size[0], device='meta')
+    return img
+
+
+def _pixels(img):
+    """A device preset's image: an encoded JPEG as it is, a PIL image as its uint8 HWC array."""
+    from .ops_jpeg import EncodedJPEG
+    return img if isinstance(img, EncodedJPEG) else np.asarray(img, dtype=np.uint8)
 
 
 def webfg_loader(path):
@@ -135,10 +158,10 @@ class DevicePresetTrain:
         self.erase = transforms.RandomErasing(p=random_erase_prob) if random_erase_prob > 0 else None
 
     def draw(self, img):
-        """-> the parameter row of one PIL image, drawn as the host preset draws it."""
+        """-> the parameter row of one PIL image (or ``EncodedJPEG``), drawn as the host preset draws it."""
         from .ops_augment import param_row
         S = self.size
-        i, j, h, w = self.crop.get_params(img, self.crop.scale, self.crop.ratio)
+        i, j, h, w = self.crop.get_params(_image_like(img), self.crop.scale, self.crop.ratio)
         flip = self.hflip_prob > 0 and bool(torch.rand(1) < self.hflip_prob)
         op, magnitude = 'Identity', 0.0
         if self.ta is not None:                          # TrivialAugmentWide.forward's draws
@@ -158,7 +181,7 @@ class DevicePresetTrain:
         return param_row((j, i, w, h), (S, S), (0, 0), flip, op, magnitude, S, erase)
 
     def __call__(self, img):
-        return np.asarray(img, dtype=np.uint8), self.draw(img)
+        return _pixels(img), self.draw(img)
 
     def collate(self, batch):
         return collate_packed(batch, self.size, self.mean, self.std)
@@ -186,7 +209,7 @@ class DevicePresetEval:
         return param_row((0, 0, W, H), (vw, vh), (left, top))
 
     def __call__(self, img):
-        return np.asarray(img, dtype=np.uint8), self.draw(img)
+        return _pixels(img), self.draw(img)
 
     def collate(self, batch):
         return collate_packed(batch, self.size, self.mean, self.std)

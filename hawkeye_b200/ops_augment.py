@@ -78,18 +78,24 @@ def param_row(box, virtual, window=(0, 0), flip=False, op='Identity', magnitude=
 
 class PackedImages:
     """One batch of decoded images and their draws (see the module docstring), on the host or on the device.  ``size``
-    is S, ``mean`` and ``std`` the Normalize constants.  The DataLoader pins it through ``pin_memory``."""
+    is S, ``mean`` and ``std`` the Normalize constants.  The DataLoader pins it through ``pin_memory``.
 
-    def __init__(self, data, offsets, sizes, params, size, mean, std):
+    With ``dataset.transformer.decode: cuda`` some images may still be encoded: ``jpeg`` is then their
+    ``ops_jpeg.JpegBatch``, ``data`` holds the pixel images only, as the first bytes of a device pixel buffer of
+    ``pixel_bytes`` bytes, and the encoded images' offsets point past them, where the decode writes."""
+
+    def __init__(self, data, offsets, sizes, params, size, mean, std, jpeg=None, pixel_bytes=None):
         self.data, self.offsets, self.sizes, self.params = data, offsets, sizes, params
         self.size, self.mean, self.std = int(size), tuple(mean), tuple(std)
+        self.jpeg = jpeg
+        self.pixel_bytes = int(data.numel() if pixel_bytes is None else pixel_bytes)
 
     def __len__(self):
         return self.offsets.shape[0]
 
     def _map(self, fn):
         return PackedImages(fn(self.data), fn(self.offsets), fn(self.sizes), fn(self.params), self.size, self.mean,
-                            self.std)
+                            self.std, None if self.jpeg is None else self.jpeg._map(fn), self.pixel_bytes)
 
     def pin_memory(self):
         return self._map(lambda t: t.pin_memory())
@@ -97,24 +103,48 @@ class PackedImages:
     def to(self, device, non_blocking=False):
         return self._map(lambda t: t.to(device, non_blocking=non_blocking))
 
+    def pixels(self, out=None, work=None):
+        """The uint8 pixel buffer of a batch on the device with every image decoded (``ops_jpeg.decode`` into ``out``,
+        with the grow-only buffers of ``work``), and the decode's status words (None without encoded images)."""
+        if self.jpeg is None:
+            return self.data, None
+        from .ops_jpeg import decode
+        out = torch.empty(self.pixel_bytes, dtype=torch.uint8, device=self.data.device) if out is None else out
+        out[:self.data.numel()].copy_(self.data)
+        return out, decode(self.jpeg, out, self.offsets, work=work)
+
     def images(self, out=None, work=None, lut=None):
-        """The model's fp32 NCHW input [N, 3, S, S] of a batch on the device (``augment``)."""
-        return augment(self.data, self.offsets, self.sizes, self.params, self.size, self.mean, self.std, out, work, lut)
+        """The model's fp32 NCHW input [N, 3, S, S] of a batch on the device (``augment``).  Encoded images are decoded
+        first, and a decode error raises here, naming the file."""
+        data, status = self.pixels()
+        if status is not None:
+            from .ops_jpeg import raise_on_status
+            raise_on_status(status.cpu().numpy(), self.jpeg.paths)
+        return augment(data, self.offsets, self.sizes, self.params, self.size, self.mean, self.std, out, work, lut)
 
 
 def pack(images, params, size, mean, std):
-    """Decoded uint8 HWC arrays and their parameter rows -> ``PackedImages`` on the host."""
+    """Decoded uint8 HWC arrays, or ``ops_jpeg.EncodedJPEG`` images, and their parameter rows -> ``PackedImages`` on the
+    host.  The pixel images come first in the pixel buffer, the encoded ones after them."""
+    from .ops_jpeg import EncodedJPEG, pack_encoded
     if not images:
         raise ValueError('pack: empty batch')
-    sizes = np.array([a.shape[:2] for a in images], np.int32)
-    nbytes = np.array([a.size for a in images], np.int64)
-    offsets = np.concatenate(([0], np.cumsum(nbytes)[:-1])).astype(np.int64)
-    data = torch.empty(int(nbytes.sum()), dtype=torch.uint8)
+    encoded = [i for i, a in enumerate(images) if isinstance(a, EncodedJPEG)]
+    plain = [i for i, a in enumerate(images) if not isinstance(a, EncodedJPEG)]
+    for i in plain:
+        a = images[i]
+        if not isinstance(a, np.ndarray) or a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3:
+            raise ValueError(f'pack: expected uint8 HWC RGB images, got {getattr(a, "dtype", type(a))} '
+                             f'{getattr(a, "shape", "")}')
+    sizes = np.array([(a.size[1], a.size[0]) if isinstance(a, EncodedJPEG) else a.shape[:2] for a in images], np.int32)
+    nbytes = sizes[:, 0].astype(np.int64) * sizes[:, 1] * 3
+    order = plain + encoded
+    offsets = np.zeros(len(images), np.int64)
+    offsets[order] = np.concatenate(([0], np.cumsum(nbytes[order])[:-1]))
+    data = torch.empty(int(nbytes[plain].sum()), dtype=torch.uint8)
     buf = data.numpy()
-    for a, o, n in zip(images, offsets, nbytes):
-        if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3:
-            raise ValueError(f'pack: expected uint8 HWC RGB images, got {a.dtype} {a.shape}')
-        buf[o:o + n] = np.ascontiguousarray(a).reshape(-1)
+    for i in plain:
+        buf[offsets[i]:offsets[i] + nbytes[i]] = np.ascontiguousarray(images[i]).reshape(-1)
     table = np.stack(params).astype(np.float64)
     if table.shape[1] != PARAM_COLS:
         raise ValueError(f'pack: parameter rows have {table.shape[1]} columns, expected {PARAM_COLS}')
@@ -122,7 +152,9 @@ def pack(images, params, size, mean, std):
     if (box[:, 2:] < 1).any() or (box[:, :2] < 0).any() or (box[:, 0] + box[:, 2] > sizes[:, 1]).any() or \
             (box[:, 1] + box[:, 3] > sizes[:, 0]).any():
         raise ValueError('pack: a source box lies outside its image')
-    return PackedImages(data, torch.from_numpy(offsets), torch.from_numpy(sizes), torch.from_numpy(table), size, mean, std)
+    jpeg = pack_encoded([images[i] for i in encoded], encoded) if encoded else None
+    return PackedImages(data, torch.from_numpy(offsets), torch.from_numpy(sizes), torch.from_numpy(table), size, mean, std,
+                        jpeg, int(nbytes.sum()))
 
 
 def augment(data, offsets, sizes, params, size, mean, std, out=None, work=None, lut=None):

@@ -15,7 +15,7 @@ from . import _lib
 from .config import setup_config
 from .registry import MODEL
 from .ops_augment import PackedImages
-from .train import AverageMeter, accuracy, prediction, transformer_device
+from .train import AverageMeter, accuracy, dataset_loader, prediction, transformer_decode, transformer_device
 from .utils import load_state_dict
 
 IMAGENET_MEAN, IMAGENET_STD = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)      # test.py:84, dataset/transforms.py:18-19
@@ -60,10 +60,11 @@ class Tester:
         from torch.utils.data import DataLoader
         from torchvision import transforms
         t = config.transformer
-        if transformer_device(t) == 'cuda':             # decode on the host, the rest of the preset on the GPU
+        if transformer_device(t) == 'cuda':             # decode on the host (or the device), the preset on the GPU
             from .data import DevicePresetEval
             tf = DevicePresetEval(crop_size=t.image_size, resize_size=t.resize_size, mean=IMAGENET_MEAN, std=IMAGENET_STD)
-            ds = FGDataset(config.root_dir, os.path.join(config.meta_dir, 'val.txt'), transform=tf)
+            kw = {'loader': dataset_loader(t)} if transformer_decode(t) else {}
+            ds = FGDataset(config.root_dir, os.path.join(config.meta_dir, 'val.txt'), transform=tf, **kw)
             return DataLoader(ds, config.batch_size, num_workers=config.num_workers, pin_memory=True, shuffle=False,
                               collate_fn=tf.collate)
         tf = transforms.Compose([transforms.Resize(size=t.resize_size), transforms.CenterCrop(size=t.image_size),

@@ -78,11 +78,25 @@ def prediction(model, outputs):
 
 def transformer_device(config):
     """'cuda' when a ``dataset.transformer`` config asks for the device presets (``device: cuda``), None when it has no
-    ``device`` key (the host presets)."""
+    ``device`` key (the host presets).  Also checks ``decode`` (``transformer_decode``)."""
     device = config['device'] if 'device' in config else None
     if device not in (None, 'cuda'):
         raise ValueError(f"dataset.transformer.device must be 'cuda' or absent, not {device!r}")
+    transformer_decode(config)
     return device
+
+
+def transformer_decode(config):
+    """'cuda' when a ``dataset.transformer`` config sets ``decode: cuda`` (the JPEGs the device decodes travel encoded,
+    ``hawkeye_b200.ops_jpeg``), None when it has no ``decode`` key.  Valid only with ``device: cuda``."""
+    from .ops_jpeg import decode_setting
+    return decode_setting(config)
+
+
+def dataset_loader(config):
+    """The image loader ``FGDataset`` is given: ``encoded_loader`` under ``decode: cuda``, else the default."""
+    from .data import default_loader, encoded_loader
+    return encoded_loader if transformer_decode(config) == 'cuda' else default_loader
 
 
 def device_collate(config, transforms, who):
@@ -91,8 +105,9 @@ def device_collate(config, transforms, who):
     if transformer_device(config) is None:
         return None
     if not all(hasattr(t, 'collate') for t in transforms.values()):
-        raise ValueError(f'dataset.transformer.device: cuda covers the default presets only; {who} builds its own, which '
-                         'run on the host')
+        key = 'device: cuda and decode: cuda cover' if transformer_decode(config) else 'device: cuda covers'
+        raise ValueError(f'dataset.transformer.{key} the default presets only; {who} builds its own, which run on the '
+                         'host')
     return {s: t.collate for s, t in transforms.items()}
 
 
@@ -187,8 +202,10 @@ class Trainer:
             from .data import MixupCutmixCollateFn
             collate = dict(collate or {}, train=MixupCutmixCollateFn(self.config.model.num_classes,
                                                                      (collate or {}).get('train')))
+        kw = {'loader': dataset_loader(config.transformer)} if transformer_decode(config.transformer) else {}
         return self.rank_loaders(config, {s: FGDataset(config.root_dir, os.path.join(config.meta_dir, s + '.txt'),
-                                                       transform=tf[s]) for s in ('train', 'val')}, collate_fn=collate)
+                                                       transform=tf[s], **kw) for s in ('train', 'val')},
+                                 collate_fn=collate)
 
     def rank_loaders(self, config, datasets, collate_fn=None):
         """{'train', 'val'} loaders of this rank over ``datasets``; ``collate_fn`` maps a split to its collate function.
@@ -312,7 +329,12 @@ class Trainer:
         """``stage_inputs`` of a packed batch of the device presets: the packed images and their tables are copied on the
         copy stream into a ring slot whose byte buffer grows to the largest batch seen, then the augment kernels write
         the slot's fp32 image buffer on the compute stream.  A graph-replayed step copies from that buffer into its static
-        input afterwards, as it does for any staged batch."""
+        input afterwards, as it does for any staged batch.
+
+        A batch with encoded JPEGs (``dataset.transformer.decode: cuda``) also has its scans and tables copied, into
+        grow-only buffers of the slot, and is decoded on the compute stream into the slot's pixel buffer before the
+        augment kernels.  The decode's status words come back asynchronously and are checked when the slot is next
+        used (or by ``check_decode``): a failed decode raises, naming the file."""
         N, S = len(packed), packed.size
         key = ('packed', N, S) + tuple((tuple(t.shape), t.dtype) for t in labs)
         ring = self._in_ring.get(key)
@@ -328,27 +350,76 @@ class Trainer:
                 lab=[torch.empty(t.shape, dtype=t.dtype, device=dev) for t in labs], free=None) for _ in range(3)])
         slot = ring['slots'][ring['i'] % 3]
         ring['i'] += 1
+        self.check_decode(slot)
         cur = torch.cuda.current_stream()
-        nbytes = packed.data.numel()
+        nbytes = packed.pixel_bytes
         grown = slot['src'].numel() < nbytes
         if grown:       # allocated on the compute stream: the copy stream must not write it before that stream's earlier work
             slot['src'] = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        jpeg = packed.jpeg
+        if jpeg is not None:
+            jbufs = slot.setdefault('jpeg', {})
+            for k in jpeg.tensors():
+                t = getattr(jpeg, k)
+                if k not in jbufs or jbufs[k].numel() < t.numel():
+                    jbufs[k] = torch.empty(t.numel(), dtype=t.dtype, device=dev)
+                    grown = True
+        if grown:
             self.copy_stream.wait_stream(cur)
         with torch.cuda.stream(self.copy_stream):
             if slot['free'] is not None:
                 self.copy_stream.wait_event(slot['free'])
-            slot['src'][:nbytes].copy_(packed.data, non_blocking=True)
+            slot['src'][:packed.data.numel()].copy_(packed.data, non_blocking=True)
             for k in ('offsets', 'sizes', 'params'):
                 slot[k].copy_(getattr(packed, k), non_blocking=True)
+            if jpeg is not None:
+                dev_jpeg = jpeg._map(lambda t: t)
+                for k in jpeg.tensors():
+                    t = getattr(jpeg, k)
+                    d = jbufs[k][:t.numel()].view(t.shape)
+                    d.copy_(t, non_blocking=True)
+                    setattr(dev_jpeg, k, d)
             for d, t in zip(slot['lab'], labs):
                 d.copy_(t, non_blocking=True)
             ev = torch.cuda.Event()
             ev.record()
         cur.wait_event(ev)
+        if jpeg is not None:
+            self.decode_staged(slot, dev_jpeg)
         augment(slot['src'], slot['offsets'], slot['sizes'], slot['params'], S, packed.mean, packed.std, out=slot['img'],
                 work=slot['work'], lut=slot['lut'])
         lab = tuple(slot['lab']) if isinstance(lab, tuple) else slot['lab'][0]
         return self.mix_staged(slot['img'], lab, slot), lab, slot
+
+    def decode_staged(self, slot, jpeg):
+        """Decodes the slot's encoded JPEGs into its pixel buffer on the compute stream and starts the copy of their
+        status words to the host; ``check_decode`` reads them."""
+        from .ops_jpeg import decode
+        work = slot.setdefault('jpeg_work', {})
+        status = decode(jpeg, slot['src'], slot['offsets'], work=work)
+        J = len(jpeg)
+        host = slot.get('status_host')
+        if host is None or host.numel() < J:
+            host = slot['status_host'] = torch.empty(J, dtype=torch.int32).pin_memory()
+        host[:J].copy_(status, non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record()
+        slot['decode'] = (ev, J, jpeg.paths)
+
+    def check_decode(self, slot=None):
+        """Raises, naming the file, when a decode whose status is pending in ``slot`` (every slot when None) failed.  By
+        the time a slot comes round again its decode has long finished, so the wait is a formality."""
+        slots = [slot] if slot is not None else [s for r in self._in_ring.values() for s in r['slots']]
+        for s in slots:
+            pending = s.get('decode')
+            if pending is None:
+                continue
+            s['decode'] = None
+            ev, J, paths = pending
+            if not ev.query():
+                ev.synchronize()
+            from .ops_jpeg import raise_on_status
+            raise_on_status(s['status_host'][:J].numpy(), paths)
 
     def mix_staged(self, images, labels, slot):
         """The staged images of a batch ``MixupCutmixCollateFn`` mixed (labels = (labels, mix row)): ``hk_mix_batch`` on
@@ -526,6 +597,7 @@ class Trainer:
                 self.on_start_forward(None)
                 self.batch_training(data)
                 self.on_end_forward(None)
+            self.check_decode()
             self.validate()
             val_acc = self.average_meters['acc'].avg
             is_best = epoch >= 5 and (best is None or val_acc > best)      # train.py:284-288

@@ -672,6 +672,33 @@ int hk_augment_stats(const unsigned char* img, const double* params, unsigned ch
 int hk_augment_apply(const unsigned char* img, const double* params, const unsigned char* lut, float* y, int N, int S,
                      float mean0, float mean1, float mean2, float std0, float std1, float std2, void* stream);
 
+/* ---- input side: baseline JPEG decode, bit-identical to PIL's Image.open(path).convert('RGB') through libjpeg-turbo,
+ * for the images the device presets leave encoded (dataset.transformer.decode: cuda).  hawkeye_b200/ops_jpeg.py parses
+ * the markers on the host and documents the batch layout: J encoded images; scan = their unstuffed scans back to back
+ * (4-byte aligned, scan_bytes including at least 8 bytes of padding); segs [G + 1] int32 = the byte offset of each
+ * restart segment in scan, the last entry the end; header [J, hk_jpeg_header_cols()] int32 = each image's batch index,
+ * size, components, luma sampling, MCUs, restart interval, first segment and count, first block, plane offset and its
+ * quant / DC / AC table indices per component; qtabs [Q, 64] int32 in natural order; htabs = the Huffman tables, 1424
+ * bytes each (canonical maxcode / valoffset / huffval and a 9-bit look-ahead).  Three launches, in order:
+ * hk_jpeg_huffman: scan -> coef [blocks, 64] int16 in natural order, DC absolute, each image's blocks in decode order
+ *   from its first block; status [J] int32 = 0 when the image decoded, else 1 invalid Huffman code, 2 the data ends
+ *   early, 3 data past a segment's last block, 4 a restart segment count that does not match the frame, 5 a
+ *   coefficient index beyond 63.  One CTA per image decodes chunks of chunk_bytes in parallel by self-synchronisation;
+ *   the result does not depend on chunk_bytes.  workspace of hk_jpeg_workspace_bytes(J, G, scan_bytes, chunk_bytes)
+ *   bytes (0 for bad arguments).  HK_ERR_ARG on a null pointer or a bad size, HK_ERR_ALIGN, HK_ERR_WORKSPACE.
+ * hk_jpeg_idct: coef -> planes uint8: dequantisation and jpeg_idct_islow with its range limit, each component's plane at
+ *   whole-MCU size from the image's plane offset (luma, then the chroma planes).
+ * hk_jpeg_color: planes -> pixels uint8 HWC at offsets[batch index]: libjpeg-turbo's fancy upsampling (h2v1, h2v2; plain
+ *   replication for chroma at most 2 samples wide) and its YCbCr -> RGB tables, or grey replicated, cropped to W x H. */
+int hk_jpeg_header_cols(void);
+size_t hk_jpeg_workspace_bytes(int J, int G, long long scan_bytes, int chunk_bytes);
+int hk_jpeg_huffman(const unsigned char* scan, const int* segs, const int* header, const unsigned char* htabs,
+                    short* coef, int* status, int J, int G, long long scan_bytes, int chunk_bytes, void* workspace,
+                    size_t workspace_bytes, void* stream);
+int hk_jpeg_idct(const short* coef, const int* header, const int* qtabs, unsigned char* planes, int J, void* stream);
+int hk_jpeg_color(const unsigned char* planes, const int* header, const long long* offsets, unsigned char* pixels,
+                  int J, void* stream);
+
 /* ---- Mixup / CutMix: dataset/transforms.py RandomMixup, RandomCutmix; dataset/collate_fn.py MixupCutmixCollateFn -------
  * One batch's draws are a row of hk_mix_cols() doubles in device memory: kind (0 Mixup, 1 CutMix), lambda, the CutMix
  * box x1, y1, x2, y2 (columns [x1, x2), rows [y1, y2)) and the target weight w (hawkeye_b200/ops_mixup.py).  Image n is
