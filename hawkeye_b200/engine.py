@@ -2,6 +2,7 @@
 one-process-per-GPU data-parallel gradient all-reduce that replaces ``nn.DataParallel`` (reference
 train.py:220-228).  torch.distributed/NCCL is plumbing here; all arithmetic runs in libhawkeye_b200.so.
 """
+import contextlib
 import os
 
 import torch
@@ -140,6 +141,101 @@ class FusedAdam:
         self.t = sd['t']
         for g, s in zip(self.param_groups, sd.get('param_groups', [])):     # lr reduced by a plateau scheduler survives
             g.update(s)
+
+
+EMA_COLS = 5                    # hk_ema_cols(): model pointer, average pointer, elements, kind, first chunk
+_EMA_KINDS = {torch.float32: 0, torch.int64: 1}
+
+
+class ModelEMA:
+    """Exponential moving average of ``model``: what ``torch.optim.swa_utils.AveragedModel(model, avg_fn=lambda a, p, n:
+    decay * a + (1 - decay) * p, use_buffers=True)`` computes, torchvision's ``ExponentialMovingAverage``, in one launch
+    (``hk_ema_update``) with no host synchronisation.
+
+    The average covers the flat parameter buffer ``flat`` (one float4 segment), every parameter outside it and every buffer
+    in ``model.buffers()``.  Only float32 and int64 tensors are supported; another dtype raises ValueError naming the
+    tensor.  If the flat buffer holds tensors other than the model's (CIN's criterion), those are averaged and swapped
+    along with the rest, but no state dict contains them.  The counter ``n_averaged`` is an int64 on the device: the
+    next update copies the model when it is 0.
+
+    ``swapped()`` evaluates the averaged weights by exchanging contents in place (``hk_ema_swap``), so every pointer, and
+    therefore every captured CUDA graph and every view into the flat buffer, stays valid."""
+
+    def __init__(self, model, flat: FlatParams, decay):
+        decay = float(decay)
+        if not 0.0 <= decay <= 1.0:
+            raise ValueError(f'ModelEMA: decay {decay} outside [0, 1]')
+        self.model, self.decay = model, decay
+        lo, hi = flat.flat.data_ptr(), flat.flat.data_ptr() + flat.numel * 4
+        self.model_tensors, self.averages = [flat.flat], [flat.flat.detach().clone()]
+        for name, t in list(model.named_parameters()) + list(model.named_buffers()):
+            if t.dtype not in _EMA_KINDS:
+                raise ValueError(f'ModelEMA: {name} is {t.dtype}; only float32 and int64 tensors can be averaged')
+            if lo <= t.data_ptr() < hi or t.numel() == 0:
+                continue
+            if t.device != flat.flat.device or not t.is_contiguous():
+                raise ValueError(f'ModelEMA: {name} must be a contiguous tensor on {flat.flat.device}')
+            self.model_tensors.append(t.detach())
+            self.averages.append(t.detach().clone())
+        table = torch.zeros(len(self.model_tensors), EMA_COLS, dtype=torch.int64)
+        for row, t, a in zip(table, self.model_tensors, self.averages):
+            row[:4] = torch.tensor([t.data_ptr(), a.data_ptr(), t.numel(), _EMA_KINDS[t.dtype]])
+        self.nseg = table.shape[0]
+        self.chunks = _lib.query('hk_ema_plan', table, self.nseg)
+        if self.chunks <= 0:
+            raise _lib.HawkeyeLibError(f'hk_ema_plan failed (rc={self.chunks}): {_lib.lib().hk_last_error().decode()}')
+        self.table = table.to(flat.flat.device)
+        self.n_averaged = torch.zeros((), dtype=torch.int64, device=flat.flat.device)
+
+    def update(self, reset_after=False):
+        """One averaging step of the model's current weights; with ``reset_after`` the counter is then set to 0, so the
+        next update copies the weights again (torchvision's warm-up reset)."""
+        _lib.call('hk_ema_update', self.table, self.nseg, self.chunks, self.n_averaged, self.decay, 1.0 - self.decay,
+                  int(bool(reset_after)), _lib.stream_ptr())
+
+    def reset(self):
+        """Sets the counter to 0: the next update copies the model."""
+        self.n_averaged.zero_()
+
+    def swap(self):
+        """Exchanges the contents of the model and the average; a second swap restores both bit for bit."""
+        _lib.call('hk_ema_swap', self.table, self.nseg, self.chunks, _lib.stream_ptr())
+
+    @contextlib.contextmanager
+    def swapped(self):
+        """The averaged weights in the model for the duration of the block, the model's own afterwards."""
+        self.swap()
+        try:
+            yield self.model
+        finally:
+            self.swap()
+
+    def model_state_dict(self):
+        """The average as a plain state_dict of the model, on the host: ``model.state_dict()`` with the average swapped
+        in, so the model's state-dict hooks apply (ProtoTree's nested leaf keys)."""
+        with self.swapped():
+            return {k: v.detach().cpu().clone() for k, v in self.model.state_dict().items()}
+
+    def state_dict(self):
+        return averaged_state(self.n_averaged.detach().cpu().clone(), self.model_state_dict())
+
+    def load_state_dict(self, sd):
+        """Loads a ``state_dict()`` (``AveragedModel``'s layout) through the model's ``load_state_dict``, strictly."""
+        with self.swapped():
+            self.model.load_state_dict(averaged_model_state(sd))
+        self.n_averaged.copy_(torch.as_tensor(sd['n_averaged']))
+
+
+def averaged_state(n_averaged, model_state):
+    """``AveragedModel.state_dict()``'s layout: ``n_averaged``, then the model's state_dict entries under ``module.``."""
+    sd = {'n_averaged': n_averaged}
+    sd.update(('module.' + k, v) for k, v in model_state.items())
+    return sd
+
+
+def averaged_model_state(sd):
+    """The model's state_dict entries of an ``averaged_state`` dict."""
+    return {k[len('module.'):]: v for k, v in sd.items() if k.startswith('module.')}
 
 
 # ----------------------------------------------------------------------------------------------------------

@@ -130,6 +130,39 @@ def warmup_cosine_args(config, total_epoch):
             config['lr_warmup_decay'] if 'lr_warmup_decay' in config else 0.01)
 
 
+EMA_DEFAULTS = dict(decay=0.99998, steps=32)       # torchvision's --model-ema-decay and --model-ema-steps
+
+
+def model_ema_setting(config):
+    """-> (decay, steps) of a ``train`` config's ``model_ema`` key, each with torchvision's default, or None without the
+    key: the weights' exponential moving average is on exactly when ``train.model_ema`` is present.  A ``decay`` outside
+    (0, 1) or a ``steps`` that is not an integer >= 1 raises ValueError naming the key."""
+    if 'model_ema' not in config:
+        return None
+    c = config['model_ema'] if config['model_ema'] is not None else {}
+    if not isinstance(c, dict):
+        raise ValueError(f'train.model_ema must be a mapping with decay and steps, or empty, not {c!r}')
+    unknown = sorted(set(c) - set(EMA_DEFAULTS))
+    if unknown:
+        raise ValueError(f'train.model_ema has unknown keys {unknown} (decay, steps)')
+    decay = c['decay'] if 'decay' in c else EMA_DEFAULTS['decay']
+    steps = c['steps'] if 'steps' in c else EMA_DEFAULTS['steps']
+    if isinstance(decay, bool) or not isinstance(decay, (int, float)) or not 0 < decay < 1:
+        raise ValueError(f'train.model_ema.decay must lie in (0, 1), not {decay!r}')
+    if isinstance(steps, bool) or not isinstance(steps, int) or steps < 1:
+        raise ValueError(f'train.model_ema.steps must be an integer >= 1, not {steps!r}')
+    return float(decay), steps
+
+
+def model_ema_decay(decay, steps, batch_size, epochs):
+    """The decay an update applies, torchvision's references/classification/train.py: the configured decay is per image
+    over the whole run, adjusted to one update every ``steps`` batches of ``batch_size`` (the global batch) images,
+    ``alpha = min(1, (1 - decay) * batch_size * steps / epochs)``, decay ``1 - alpha``."""
+    adjust = batch_size * steps / epochs
+    alpha = min(1.0, (1.0 - decay) * adjust)
+    return 1.0 - alpha
+
+
 class Trainer:
     def __init__(self, config=None, dataloaders=None):
         self.config = config if config is not None else setup_config()
@@ -158,6 +191,8 @@ class Trainer:
         self.optimizer = self.get_optimizer(self.config.train.optimizer)
         self.optimizer.grad_scale = 1.0 / self.world
         self.scheduler = self.get_scheduler(self.config.train.scheduler)
+        self.ema_steps, self.ema_warmup, self.acc_ema, self.epoch_batch = 0, 0, None, 0
+        self.ema = self.get_model_ema(self.config.train)
         self.average_meters = {'acc': AverageMeter(), 'loss': AverageMeter()}
         self.copy_stream = torch.cuda.Stream(device=self.device)    # input H2D overlaps the previous step's compute
         self._in_ring = {}
@@ -270,6 +305,18 @@ class Trainer:
             return _Plateau(self.optimizer, mode='max', factor=0.1, patience=3, threshold=1e-4)
         T_max, warmup_epochs, warmup_decay = warmup_cosine_args(config, self.total_epoch)
         return _Cosine(self.optimizer, T_max, config.eta_min if 'eta_min' in config else 0.0, warmup_epochs, warmup_decay)
+
+    def get_model_ema(self, config):
+        """The ``engine.ModelEMA`` of the model with ``train.model_ema`` (torchvision's ``--model-ema``), None without it.
+        Sets the update interval ``ema_steps`` and ``ema_warmup``, the epochs after whose updates the counter resets."""
+        setting = model_ema_setting(config)
+        if setting is None:
+            return None
+        decay, self.ema_steps = setting
+        sc = config.scheduler if 'scheduler' in config else {}
+        self.ema_warmup = sc['warmup_epochs'] if 'warmup_epochs' in sc else 0
+        return engine.ModelEMA(self.get_model_module(), self.flat,
+                               model_ema_decay(decay, self.ema_steps, self.config.dataset.batch_size, self.total_epoch))
 
     def to_device(self, m, parallel=False):
         """A tensor or module on the trainer's device; a packed batch of the device presets becomes its model input."""
@@ -521,6 +568,7 @@ class Trainer:
         outputs, loss = self._graph_step(images, labels) if self._graph_wanted() else self.eager_step(images, labels)
         self.optimizer.step()
         self.after_optimizer_step()
+        self.update_ema()
         self.release_inputs(slot)
         n = images.size(0)
         correct = getattr(self.criterion, 'last_correct', None)
@@ -550,6 +598,14 @@ class Trainer:
     def after_optimizer_step(self):
         """Work of the step that follows the optimizer, still before the step's input slot is released (it may read the
         step's labels).  ProtoTree's leaf update goes here."""
+
+    def update_ema(self):
+        """After the optimizer step (and ``after_optimizer_step``) of batch ``epoch_batch`` of the epoch: torchvision's
+        train_one_epoch updates the average when the index is a multiple of ``ema_steps``, and resets its counter after
+        an update in a warm-up epoch.  All of it on the device; nothing when the trainer has no EMA."""
+        if self.ema is not None and self.epoch_batch % self.ema_steps == 0:
+            self.ema.update(reset_after=self.epoch < self.ema_warmup)
+        self.epoch_batch += 1
 
     def forward_model(self, images, labels):
         """The model call of the training step (eager and graph-captured alike).  Methods whose forward takes the labels
@@ -582,12 +638,26 @@ class Trainer:
                 m.sum, m.count = t[0].item(), int(t[1].item())
         self.model.train(True)
 
+    def validate_ema(self):
+        """-> top-1 accuracy of the averaged weights: ``validate()`` with them swapped in, on meters of its own, so the
+        model's meters keep the model's results.  Also kept as ``acc_ema``."""
+        meters = self.average_meters
+        self.average_meters = {k: AverageMeter() for k in meters}
+        try:
+            with self.ema.swapped():
+                self.validate()
+                self.acc_ema = self.average_meters['acc'].avg
+        finally:
+            self.average_meters = meters
+        return self.acc_ema
+
     def train(self):
         cfg = self.config.train
         self.model.train()
-        best = None
+        best = best_ema = None
         for epoch in range(self.start_epoch, self.total_epoch):
             self.epoch = epoch
+            self.epoch_batch = 0
             for m in self.average_meters.values():
                 m.reset()
             self.on_start_epoch(None)
@@ -603,11 +673,19 @@ class Trainer:
             is_best = epoch >= 5 and (best is None or val_acc > best)      # train.py:284-288
             best = val_acc if best is None else max(best, val_acc)
             self.do_scheduler_step()
+            is_best_ema = False
+            if self.ema is not None:
+                acc_ema = self.validate_ema()
+                self.logger.info('epoch %d: acc %.4f acc_ema %.4f', epoch, val_acc, acc_ema)
+                is_best_ema = epoch >= 5 and (best_ema is None or acc_ema > best_ema)
+                best_ema = acc_ema if best_ema is None else max(best_ema, acc_ema)
             if self.rank == 0:
                 if epoch != 0 and (epoch + 1) % cfg.save_frequence == 0:
                     self.save_model()
                 if is_best:
                     self.save_model('best_model.pth')
+                if is_best_ema:
+                    self.save_model('best_model_ema.pth', self.ema.model_state_dict())
             self.on_end_epoch(None)
 
     def do_scheduler_step(self):
@@ -621,10 +699,12 @@ class Trainer:
     # top-level layout {'epoch','model','optimizer','scheduler'} with an identical 'model' part, but the optimizer /
     # scheduler parts are the fused optimizers' own state (flat momentum / Adam moments), not torch.optim's: a reference
     # checkpoint resumes here with its model weights only (load_checkpoint says so instead of failing). -----------------
-    def save_model(self, name=None):
+    def save_model(self, name=None, state=None):
+        """Writes ``state`` (the model's state_dict when None) as a plain state_dict .pth."""
         os.makedirs(self.log_root, exist_ok=True)
         path = os.path.join(self.log_root, name or f'{self.config.model.name}_epoch_{self.epoch + 1}.pth')
-        torch.save({k: v.detach().cpu().clone() for k, v in self.model.state_dict().items()}, path)
+        state = self.model.state_dict() if state is None else state
+        torch.save({k: v.detach().cpu().clone() for k, v in state.items()}, path)
         return path
 
     def save_checkpoint(self):
@@ -634,9 +714,13 @@ class Trainer:
         return path
 
     def checkpoint_state(self):
-        """-> the dict save_checkpoint writes; a trainer with trained state outside the model adds its own keys."""
-        return {'epoch': self.epoch, 'model': {k: v.detach().cpu().clone() for k, v in self.model.state_dict().items()},
-                'optimizer': self.optimizer.state_dict(), 'scheduler': self.scheduler.state_dict()}
+        """-> the dict save_checkpoint writes; a trainer with trained state outside the model adds its own keys.  With
+        ``train.model_ema`` it holds ``model_ema``, the average in ``AveragedModel.state_dict()``'s layout."""
+        ck = {'epoch': self.epoch, 'model': {k: v.detach().cpu().clone() for k, v in self.model.state_dict().items()},
+              'optimizer': self.optimizer.state_dict(), 'scheduler': self.scheduler.state_dict()}
+        if self.ema is not None:
+            ck['model_ema'] = self.ema.state_dict()
+        return ck
 
     def load_checkpoint(self, path):
         self.restore_checkpoint(torch.load(path, map_location='cpu'), path)
@@ -652,6 +736,14 @@ class Trainer:
         else:
             self.logger.warning('checkpoint %s carries torch.optim state (a reference checkpoint): model weights and epoch '
                                 'restored, optimizer / scheduler state re-initialised', path)
+        if self.ema is None:
+            return
+        if 'model_ema' in ck:
+            self.ema.load_state_dict(ck['model_ema'])
+        else:
+            self.logger.warning('checkpoint %s has no model_ema: the average starts from the restored weights', path)
+            model = {k: v.detach().clone() for k, v in self.get_model_module().state_dict().items()}
+            self.ema.load_state_dict(engine.averaged_state(torch.zeros((), dtype=torch.int64), model))
 
     def on_start_epoch(self, config):
         pass
@@ -692,6 +784,7 @@ class PeerLearningTrainer(Trainer):
         loss2.backward()
         self.allreduce.finish()
         self.optimizer.step()
+        self.update_ema()
         self.release_inputs(slot)
         n = images.size(0)
         acc1, acc2 = accuracy(logits1, labels, 1), accuracy(logits2, labels, 1)

@@ -721,6 +721,27 @@ int hk_mix_batch(const float* x, const double* mix, float* y, int N, int C, int 
 int hk_softmax_ce_ls_mix(const float* logits, const long long* labels, const double* mix, float* loss, float* dlogits,
                          int* correct, int B, int K, float label_smoothing, float grad_scale, void* stream);
 
+/* ---- model EMA: torch.optim.swa_utils.AveragedModel(model, avg_fn=d * avg + (1 - d) * p, use_buffers=True) with
+ * torchvision's ExponentialMovingAverage (references/classification/utils.py) and the update of train_one_epoch.
+ * table [nseg, hk_ema_cols()] int64 describes the tensors: model pointer, average pointer, elements, kind (0 float32,
+ * 1 int64) and the segment's first chunk (hawkeye_b200/engine.py ModelEMA builds it once and keeps it on the device).
+ * hk_ema_plan: validates a table in HOST memory and fills its chunk column; -> the chunk count (the grid of the two
+ *   launches below), or HK_ERR_ARG on a null pointer, nseg <= 0, a null or self-aliased segment, a length <= 0 or an
+ *   unknown kind, HK_ERR_ALIGN on a pointer not aligned to its elements.
+ * hk_ema_update: with the device counter *n_averaged == 0, avg = p; otherwise avg = fl(fl(decay avg) + fl(one_minus_decay
+ *   p)) with no fused multiply-add, torch's arithmetic for d * avg + (1 - d) * p (the caller computes 1 - d in double);
+ *   int64 tensors in fp32 on the converted values, truncated toward zero.  A 16-byte-aligned float32 segment (the flat
+ *   parameter buffer) is read as float4.  Then, in a second one-thread launch so that no block of the first reads it,
+ *   the counter is incremented, or set to 0 when reset_after (torchvision's warm-up reset).  No host synchronisation.
+ * hk_ema_swap: exchanges the contents of every model tensor and its average in place; two swaps restore every bit.
+ * Both: HK_ERR_ARG on a null pointer, nseg <= 0 or a chunk count <= 0 or above INT_MAX; update also on a factor outside
+ *   [0, 1]. */
+int hk_ema_cols(void);
+long long hk_ema_plan(long long* table, int nseg);
+int hk_ema_update(const long long* table, int nseg, long long nchunks, long long* n_averaged, float decay,
+                  float one_minus_decay, int reset_after, void* stream);
+int hk_ema_swap(const long long* table, int nseg, long long nchunks, void* stream);
+
 /* ---- optimizers over flat fp32 buffers: torch.optim.SGD (Examples/BCNN.py:40), Adam (Examples/MPN.py:14-18) */
 int hk_sgd_momentum(float* p, const float* g, float* buf, size_t n, float lr, float momentum, float weight_decay,
                     float grad_scale, int first_step, void* stream);
